@@ -1,5 +1,5 @@
 /*
- * loghisto_b200.h -- C ABI of the B200-native loghisto ingest/reduction engine.
+ * loghisto_b200.h -- C ABI of the H100-native loghisto ingest/reduction engine.
  *
  * This is the drop-in boundary for ONE path of spacejam/loghisto: the bodies of
  *   MetricSystem.Histogram      (metrics.go:273-295)  + compress (metrics.go:316-322)

@@ -145,7 +145,7 @@ func b200Status(st C.lh_status, ctx *C.lh_ctx, what string) error {
 }
 
 // engineFor returns the engine of a MetricSystem, creating it on first use.  There is no CPU fallback under the
-// b200 tag: without a usable B200 the process stops here (build without the tag for the pure-Go package).
+// b200 tag: without a usable H100 the process stops here (build without the tag for the pure-Go package).
 func engineFor(ms *MetricSystem) *b200Engine {
 	if e, ok := b200Engines.Load(ms); ok {
 		return e.(*b200Engine)

@@ -3,7 +3,7 @@
 
   python split_reference.py <loghisto checkout> [--dry-run]
 
-The five method bodies the B200 engine replaces -- MetricSystem.Counter, MetricSystem.Histogram, processHistograms,
+The five method bodies the GPU engine replaces -- MetricSystem.Counter, MetricSystem.Histogram, processHistograms,
 collectRawMetrics and processMetrics (metrics.go:251-295, 336-387, 420-506 at the surveyed commit) -- are MOVED, text
 unchanged, from metrics.go into a new metrics_cpu.go that carries `//go:build !b200`.  Import lists of both files are
 trimmed to what each still uses.  Afterwards:
@@ -90,7 +90,7 @@ def main():
         if ln.startswith("package "):
             break
         licence.append(ln)
-    new_cpu = (licence + ["// The pure-Go bodies of the five methods the B200 engine replaces (moved here unchanged from metrics.go by",
+    new_cpu = (licence + ["// The pure-Go bodies of the five methods the GPU engine replaces (moved here unchanged from metrics.go by",
                           "// integration/go/split_reference.py of loghisto_b200); compiled unless the b200 build tag is set.", "",
                           "//go:build !b200", "", pkg_line, "", "import ("] + used_imports(imports, body_moved) + [")", ""] + moved)
     out_metrics, out_cpu = "\n".join(new_metrics), "\n".join(new_cpu).rstrip("\n") + "\n"

@@ -1,4 +1,4 @@
-"""loghisto_b200: B200-native ingest + percentile-reduction engine behind loghisto's MetricSystem API.
+"""loghisto_b200: H100-native ingest + percentile-reduction engine behind loghisto's MetricSystem API.
 
 The CUDA library (libloghisto_b200.so, C ABI in include/loghisto_b200.h) is the
 product; this package only loads it and mirrors the reference's host-side

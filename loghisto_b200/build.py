@@ -1,4 +1,4 @@
-"""Builds libloghisto_b200.so in-tree with nvcc for sm_100a (no JIT cache, no torch extension)."""
+"""Builds libloghisto_b200.so in-tree with nvcc for sm_90a (H100; no JIT cache, no torch extension)."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libloghisto_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC,-fvisibility=hidden,-O2",
     "--fmad=true",           # FP32 fast path may contract; the exact path uses __d*_rn intrinsics only

@@ -1,4 +1,4 @@
-// lh_api.cu -- C ABI (include/loghisto_b200.h) over the sm_100a kernels.
+// lh_api.cu -- C ABI (include/loghisto_b200.h) over the sm_90a kernels.
 //
 // Host-side bookkeeping only: double-buffered bucket/counter arrays, stream
 // and event ordering between ingest and snapshot, the pinned staging ring,
@@ -72,13 +72,13 @@ void launch_probe(int grid, size_t, cudaStream_t s, const double *v32, size_t nv
 }
 
 #define LDG_VARIANT(T, U, M) \
-    { "ldg256_t" #T "_u" #U "_b" #M, launch_ldg<T, U, M>, (const void *)k_ingest_single_ldg<T, U, M>, T, 0, 0, 0 }
+    { "ldg_t" #T "_u" #U "_b" #M, launch_ldg<T, U, M>, (const void *)k_ingest_single_ldg<T, U, M>, T, 0, 0, 0 }
 #define BULK_VARIANT(W, S, B, M, F) \
     { "bulk2_w" #W "_s" #S "_" #B "_b" #M "_sign" #F, launch_bulk<W, S, B, M, F != 0>, (const void *)k_ingest_single_bulk<W, S, B, M, F != 0>, (W + 1) * 32, \
       (size_t)S * B + (size_t)S * 16, 0, 0 }
 
-// The shipped kernel plus what the parity tests and profiles/ compare it with (the round-1 sweep of 27 shapes is
-// archived in profiles/r01/k1_variants_sustained.txt; only the winners and the independent first version remain).
+// The shipped kernel plus what the parity tests compare it with (the winners of a sweep of 27 shapes and the
+// independent first version).
 K1Variant g_k1_variants[] = {
     BULK_VARIANT(16, 4, 32768, 1, 1),   // 0: default (sign folded into the slot)
     BULK_VARIANT(16, 3, 65536, 1, 1),   // 1
@@ -90,7 +90,7 @@ K1Variant g_k1_variants[] = {
     BULK_VARIANT(16, 3, 65536, 1, 0),   // 6
 };
 constexpr int kNumK1Variants = (int)(sizeof(g_k1_variants) / sizeof(g_k1_variants[0]));
-constexpr int kDefaultK1Variant = 6;   // 3 x 64 KB stages, negatives through the fix-up: best sustained time on streams U and N (profiles/r02/k1_sustained_r02c.txt)
+constexpr int kDefaultK1Variant = 6;   // 3 x 64 KB stages, negatives through the fix-up: best sustained time of the bulk variants (within 2 % of each other on H100)
 
 // Everything the kernels derive from `precision` (metrics.go:40-43), see lh_device.cuh.
 Prec make_prec(uint32_t precision) {
@@ -287,7 +287,7 @@ lh_status launch_single(lh_ctx *ctx, uint32_t hid, const double *d_values, size_
     while (done < n) {
         size_t m = std::min(n - done, kMaxPerLaunch);
         const double *p = d_values + done;
-        // peel up to 3 samples so the body is 32-byte aligned (256-bit loads, 16-byte bulk copies)
+        // peel up to 3 samples so the body is 32-byte aligned (4-sample load groups, 16-byte bulk copies)
         int nhead = (int)(((32u - ((uintptr_t)p & 31u)) & 31u) / 8u);
         if ((size_t)nhead > m) nhead = (int)m;
         const double *head = p;
@@ -344,7 +344,7 @@ lh_status launch_keyed_wc_spt(lh_ctx *ctx, int b, const IdT *ids, const ValT *va
     using S = WcShape<SPT>;
     const size_t hist_bytes = (((size_t)ids_per * ctx->pc.win + 3) & ~(size_t)3) * 4;
     // the owners' windows first, then the largest per-owner buffers that still fit (fewer SMs for ingest = more ids per
-    // owner = less room: 256 records at P = 147, 192 at P = 140 for H = 1024)
+    // owner = less room; on H100, 256 records at P = 131 for H = 1024)
     uint32_t row_cap = 0;
     size_t smem = 0;
     for (uint32_t cap_try : {256u, 192u, 128u}) {
@@ -357,8 +357,7 @@ lh_status launch_keyed_wc_spt(lh_ctx *ctx, int b, const IdT *ids, const ValT *va
     n2 = n2 / S::TILE * S::TILE;
     if (n4x4 + n2 == 0) return LH_OK;
     // chunks of about kp_chunk samples, EQUAL in size: with the nominal slice a short last chunk would be binned by a
-    // few CTAs at full slice length while the others idle (it cost a whole chunk time per launch: 50 M pairs ran at 211
-    // instead of 260 G samples/s, profiles/r02/keyed_batch_probe_r02l.txt)
+    // few CTAs at full slice length while the others idle, a whole chunk time per launch)
     const size_t slice_max = std::max<size_t>(1, ((size_t)ctx->kp_chunk + (size_t)P * S::TILE - 1) / ((size_t)P * S::TILE));
     const size_t tiles_all = n4x4 / S::TILE + n2 / S::TILE;
     const size_t nchunks = (tiles_all + slice_max * P - 1) / (slice_max * P);
@@ -735,9 +734,10 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
         std::lock_guard<std::mutex> lk(id_mu);
         ctx->ctx_id = next_id++;
     }
-    {   // replicas of the keyed hot window: as many as keep all copies within ~48 MB (L2-resident), at most 32
+    {   // replicas of the keyed hot window: as many as keep all copies within ~20 MB (L2-resident in H100's 50 MB
+        // L2 next to the streamed input), at most 32
         const size_t one = (size_t)ctx->H * 2u * ctx->pc.win * 4u;
-        ctx->hot_replicas = (uint32_t)std::max<size_t>(1, std::min<size_t>(32, ((size_t)48 << 20) / one));
+        ctx->hot_replicas = (uint32_t)std::max<size_t>(1, std::min<size_t>(32, ((size_t)20 << 20) / one));
     }
     ctx->staging_bytes = cfg->staging_bytes ? (size_t)cfg->staging_bytes : ((size_t)32 << 20);
     ctx->staging_bytes = (ctx->staging_bytes + 255) & ~(size_t)255;
@@ -756,8 +756,8 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
     LH_CREATE_CUDA(cudaSetDevice(ctx->device));
     cudaDeviceProp prop;
     LH_CREATE_CUDA(cudaGetDeviceProperties(&prop, ctx->device));
-    if (prop.major < 10) {
-        fprintf(stderr, "loghisto_b200: device %d is sm_%d%d; this library is built for sm_100a only\n", ctx->device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {   // sm_90a code runs on compute capability 9.0 only
+        fprintf(stderr, "loghisto_b200: device %d is sm_%d%d; this library is built for sm_90a only\n", ctx->device, prop.major, prop.minor);
         lh_destroy(ctx);
         return LH_ERR_NO_DEVICE;
     }

@@ -1,10 +1,10 @@
-// lh_kernels.cuh -- sm_100a kernels of the loghisto hot path.
+// lh_kernels.cuh -- sm_90a (H100) kernels of the loghisto hot path.
 //
 //   K1   k_ingest_single_*  one histogram, float64 stream -> bucket counts
 //                           (compress + Histogram increment, metrics.go:273-295, 316-322)
 //          _bulk  : cp.async.bulk (TMA 1-D, UBLKCP) into a shared-memory ring guarded by mbarriers, one producer
-//                   warp + N consumer warps, packed-FP32 bucket arithmetic: the shipped default
-//          _ldg   : 256-bit ld.global.nc loads, software-pipelined in registers, scalar fast_candidate() (first version;
+//                   warp + N consumer warps, pairwise FP32 bucket arithmetic: the shipped default
+//          _ldg   : 2 x 128-bit ld.global.nc loads per 4 samples, software-pipelined in registers, scalar fast_candidate() (first version;
 //                   kept as the second, independently written evaluator the parity tests run against the oracle)
 //        both privatise the histogram in shared memory (uint32 sub-histograms, ATOMS.POPC.INC) and flush once per
 //        CTA with one global 64-bit atomic per non-empty bucket.
@@ -33,16 +33,27 @@ namespace lh {
 
 // ---------------------------------------------------------------- helpers
 // Streaming loads: read-once data, keep it out of L1 and first in line for L2 eviction.
-// sm_100 has 256-bit global loads (ld.global.v4.b64 -> LDG.E.256); the L2
-// eviction-priority qualifier is only accepted on those.
+// sm_90 has no 256-bit global loads and accepts an L2 eviction priority on loads only through a cache-policy
+// operand, so one 32-byte group is two 128-bit loads (LDG.E.128) carrying an evict_first policy.
 struct f64x4 { double a, b, c, d; };
+__device__ __forceinline__ uint64_t policy_evict_first() {   // not volatile: the compiler hoists it out of loops
+    uint64_t p;
+    asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ void ldg_stream_u64x4(const void *p, unsigned long long (&r)[4]) {
+    const uint64_t pol = policy_evict_first();
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0, %1}, [%2], %3;"
+                 : "=l"(r[0]), "=l"(r[1]) : "l"(p), "l"(pol));
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.b64 {%0, %1}, [%2], %3;"
+                 : "=l"(r[2]), "=l"(r[3]) : "l"((const char *)p + 16), "l"(pol));
+}
 __device__ __forceinline__ f64x4 ldg_stream_f64x4(const void *p) {
-    unsigned long long a, b, c, d;
-    asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v4.b64 {%0, %1, %2, %3}, [%4];"
-                 : "=l"(a), "=l"(b), "=l"(c), "=l"(d) : "l"(p));
+    unsigned long long u[4];
+    ldg_stream_u64x4(p, u);
     f64x4 r;
-    r.a = __longlong_as_double((long long)a); r.b = __longlong_as_double((long long)b);
-    r.c = __longlong_as_double((long long)c); r.d = __longlong_as_double((long long)d);
+    r.a = __longlong_as_double((long long)u[0]); r.b = __longlong_as_double((long long)u[1]);
+    r.c = __longlong_as_double((long long)u[2]); r.d = __longlong_as_double((long long)u[3]);
     return r;
 }
 __device__ __forceinline__ f64x4 ldg_stream_f64x2x2(const void *p) {   // two 128-bit loads (comparison variant)
@@ -80,12 +91,6 @@ __device__ __forceinline__ void bulk_g2s(void *smem_dst, const void *gsrc, uint3
         "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
         ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(policy) : "memory");
 }
-__device__ __forceinline__ uint64_t policy_evict_first() {
-    uint64_t p;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-    return p;
-}
-
 __device__ __forceinline__ uint64_t policy_evict_last() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
@@ -141,7 +146,7 @@ __device__ __forceinline__ void bucket_stragglers(const double *p, int n, const 
 }
 
 // ------------------------------------------------------------------- K1/ldg
-// First version, kept as a second evaluator: scalar fast_candidate() per sample, 256-bit loads double-buffered in
+// First version, kept as a second evaluator: scalar fast_candidate() per sample, 32-byte groups double-buffered in
 // registers.  vals32: 32-byte aligned, nvec 32-byte vectors (4 samples each).
 template <int NS>
 __device__ __forceinline__ void bucket_samples(const double (&v)[NS], uint32_t *hist, const Prec &pc,
@@ -207,10 +212,11 @@ k_ingest_single_ldg(const double *__restrict__ vals32, size_t nvec, const double
     flush_subhist(s_hist, threadIdx.x, THREADS, counts, flag, pc.win);
 }
 
-// ------------------------------------------------------- packed-FP32 bucket arithmetic
-// Same algorithm as fast_candidate() with the per-sample instruction count cut from ~30 to ~20 so that the
-// kernel stays HBM-bound under sustained load (profiles/r01/sustained_probe.txt):
-//   * samples are processed in pairs with Blackwell's packed FP32 ops (fma.rn.f32x2 / add.f32x2);
+// ------------------------------------------------------- pairwise FP32 bucket arithmetic
+// Same algorithm as fast_candidate() with the per-sample instruction count cut so that the kernel stays HBM-bound
+// under sustained load:
+//   * samples are processed in pairs, each FP32 op written with an explicit rounding (__fmaf_rn / __fadd_rn) so the
+//     compiler neither contracts nor reorders them;
 //   * (float)e comes from one I2FP and the -1023 bias rides in the FMA addend (Prec::kb);
 //   * ONE flag per sample: estimate too close to a bucket boundary, OR x = 1+|v| outside the window
 //     (x's high word >= 0x43E00000: |v| >= 2^63, Inf, NaN);
@@ -242,11 +248,11 @@ __device__ __forceinline__ void bucket_offsets_v2(const double (&v)[NS], const P
         asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(lg.y) : "f"(__uint_as_float(m1)));
         const uint32_t e0 = h0 >> 20, e1 = h1 >> 20;                    // 1023 + e
         const float2 ef = make_float2(__uint2float_rn(e0), __uint2float_rn(e1));
-        const float2 a = __ffma2_rn(ef, make_float2(pc.c2, pc.c2), make_float2(pc.kb, pc.kb));
-        const float2 w = __ffma2_rn(lg, make_float2(pc.c1, pc.c1), a);
-        const float2 r = __fadd2_rn(w, make_float2(MAGIC, MAGIC));
-        const float2 s = __fadd2_rn(r, make_float2(-MAGIC, -MAGIC));
-        const float2 d = __ffma2_rn(s, make_float2(-1.0f, -1.0f), w);   // w - s, one rounding
+        const float2 a = make_float2(__fmaf_rn(ef.x, pc.c2, pc.kb), __fmaf_rn(ef.y, pc.c2, pc.kb));
+        const float2 w = make_float2(__fmaf_rn(lg.x, pc.c1, a.x), __fmaf_rn(lg.y, pc.c1, a.y));
+        const float2 r = make_float2(__fadd_rn(w.x, MAGIC), __fadd_rn(w.y, MAGIC));
+        const float2 s = make_float2(__fadd_rn(r.x, -MAGIC), __fadd_rn(r.y, -MAGIC));
+        const float2 d = make_float2(__fmaf_rn(s.x, -1.0f, w.x), __fmaf_rn(s.y, -1.0f, w.y));   // w - s, one rounding
         if (FOLD_SIGN) {
             flag[i] = (fabsf(d.x) > pc.thresh) | (h0 >= 0x43E00000u);
             flag[i + 1] = (fabsf(d.y) > pc.thresh) | (h1 >= 0x43E00000u);
@@ -285,7 +291,7 @@ __device__ __forceinline__ void bucket_samples_v2(const double (&v)[NS], uint32_
 }
 
 // --------------------------------------------------------------- read probe
-// Diagnostic only (a K1 "variant" that produces NO counts): the same 256-bit streaming loads as K1/ldg with the
+// Diagnostic only (a K1 "variant" that produces NO counts): the same streaming loads as K1/ldg with the
 // bucket arithmetic replaced by an XOR fold, to separate memory-side from SM-side limits.
 template <int THREADS, int UNROLL>
 __global__ void __launch_bounds__(THREADS, 2)
@@ -398,8 +404,8 @@ k_ingest_single_bulk(const double *__restrict__ vals32, size_t nvec32, const dou
 // in one CTA's shared memory.  The general fallback keeps the cells in L2: a compact uint32 "hot window"
 // [H][2*win] (36 MB at H = 1024, vs 512 MB for the dense uint64 arrays)
 // updated with no-return atomics that carry an L2 evict_last policy, while the
-// sample stream is read once with 256-bit evict_first loads so it does not push
-// the cells out of the 126 MB L2.  Keys outside the window go straight to the
+// sample stream is read once with evict_first loads so it does not push
+// the cells out of the 50 MB L2.  Keys outside the window go straight to the
 // uint64 array.  k_fold_hot drains the window into the uint64 buckets at every
 // snapshot (and before any cell could reach 2^32).
 template <typename T> __device__ __forceinline__ double sample_to_f64(T v);
@@ -459,8 +465,7 @@ __device__ __forceinline__ void load_ids4(const IdT *ids, size_t g, uint32_t (&i
     }
 }
 __device__ __forceinline__ void load_vals4(const void *vals, size_t g, unsigned long long (&raw)[4]) {
-    asm volatile("ld.global.nc.L1::no_allocate.L2::evict_first.v4.b64 {%0, %1, %2, %3}, [%4];"
-                 : "=l"(raw[0]), "=l"(raw[1]), "=l"(raw[2]), "=l"(raw[3]) : "l"(reinterpret_cast<const char *>(vals) + g * 32));
+    ldg_stream_u64x4(reinterpret_cast<const char *>(vals) + g * 32, raw);
 }
 
 // ids of one 4-sample group, kept PACKED while they wait in registers (unpacking right after the load would make the
@@ -482,7 +487,7 @@ template <> struct IdPack<unsigned int> {
     __device__ __forceinline__ uint32_t get(int j) const { return w[j]; }
 };
 
-// Vector body: every thread takes 4 consecutive pairs (one 256-bit value load, one 64/128-bit id load).
+// Vector body: every thread takes 4 consecutive pairs (two 128-bit value loads, one 64/128-bit id load).
 // vals must be 32-byte aligned and ids 4*sizeof(IdT)-aligned; n4 = number of 4-sample groups.
 // `hot` holds `replicas` copies of the window ([replicas][H][2*win]); CTA b updates copy b % replicas, which
 // divides the same-address pressure on hot cells (clustered, latency-like data) by the replica count while every
@@ -519,7 +524,7 @@ k_ingest_keyed(const IdT *__restrict__ ids, const ValT *__restrict__ vals, size_
 // ------------------------------------------------------------------ K1k/small
 // Keyed ingest when only a few histograms are configured: all their windows (uint32[ids][2*win]) are privatised
 // per CTA in shared memory, exactly like K1, so the kernel is HBM-bound (10 B/sample) instead of L2-atomic-bound.
-// Same packed-FP32 bucket arithmetic as K1 but with positive-only rows (uint32[ids][win]) so that twice as many
+// Same pairwise FP32 bucket arithmetic as K1 but with positive-only rows (uint32[ids][win]) so that twice as many
 // histograms fit; the ONE flag per sample also covers id >= H, and flagged samples (boundary-close estimates,
 // negatives, |v| >= 2^63, NaN/Inf, bad ids) take the L2 route of keyed_one().  Windows are added into the uint32
 // hot window at the end.
@@ -601,11 +606,10 @@ k_ingest_keyed_small(const IdT *__restrict__ ids, const ValT *__restrict__ vals,
 // rate (one RED sector per sample, ~0.25 x HBM roofline) by routing every sample to the SM that OWNS its histogram.
 // One persistent cooperative CTA per SM; CTA p owns the ids {p, p+P, p+2P, ...} and keeps their positive windows
 // (uint32[ids_per][win]) in shared memory for the whole launch.  The stream is processed in chunks; per chunk
-//   phase A  every CTA ("writer") bins its slice: bucket index via the packed-FP32 fast path, one 16-bit record
+//   phase A  every CTA ("writer") bins its slice: bucket index via the pairwise FP32 fast path, one 16-bit record
 //            (lid*win + slot) per sample appended to a per-owner WRITE-COMBINING buffer in shared memory -- the
-//            position comes from one returning shared atomic on the owner's fill counter (measured 3.6 cycles per
-//            warp on ~148 spread addresses, profiles/r02/ubench_smem_primitives.txt; MATCH.ANY or ballot ranking
-//            cost 8-16x that).  After each tile of WC_TILE samples the full 128-byte lines are copied to the
+//            position comes from one returning shared atomic on the owner's fill counter (tools/ubench.cu: a
+//            warp-wide shared atomic on spread addresses costs a fraction of MATCH.ANY or ballot ranking).  After each tile of WC_TILE samples the full 128-byte lines are copied to the
 //            (owner, writer) sub-queue in global memory (L2-resident) with 128-bit stores and the remainder (< 64
 //            records) moves to the front of the buffer.  Every (owner, writer) pair has its own region, so the
 //            append offsets live in shared memory and no global atomic is needed;
@@ -1004,7 +1008,7 @@ k_counter_add_smem(const IdT *__restrict__ ids, const unsigned long long *__rest
     }
 }
 
-// Vector body: 4 consecutive (id, amount) pairs per thread and iteration (one 256-bit amount load, one 64/128-bit id
+// Vector body: 4 consecutive (id, amount) pairs per thread and iteration (two 128-bit amount loads, one 64/128-bit id
 // load), the next group prefetched while the current one is added.  amounts 32-byte aligned, ids 4*sizeof(IdT)-aligned.
 template <typename IdT, int THREADS>
 __global__ void __launch_bounds__(THREADS)
@@ -1627,7 +1631,7 @@ __global__ void k_compress_probe(const double *__restrict__ v, size_t n, short *
 
 // max | estimate - precision*ln(x) | over samples inside the fast window, for both estimators that ship:
 //   [0] fast_candidate()      (k_ingest_keyed*, probes, ragged tails)
-//   [2] bucket_offsets_v2()   (packed-FP32 form with the -1023*c2 constant folded into the FMA; K1, keyed_small, keyed_wc)
+//   [2] bucket_offsets_v2()   (pairwise FP32 form with the -1023*c2 constant folded into the FMA; K1, keyed_small, keyed_wc)
 // plus [1] the tally of samples fast_candidate() sends to the exact path.
 __global__ void k_fastpath_margin(const double *__restrict__ v, size_t n, unsigned long long *__restrict__ out, Prec pc) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;

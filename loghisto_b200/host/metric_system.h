@@ -116,7 +116,7 @@ struct Options {
 
 class MetricSystem {
  public:
-    // NewMetricSystem(interval, sysStats), metrics.go:143.  Throws std::runtime_error if no B200 is usable.
+    // NewMetricSystem(interval, sysStats), metrics.go:143.  Throws std::runtime_error if no H100 is usable.
     MetricSystem(std::chrono::nanoseconds interval, bool sysStats, const Options &opt = Options());
     ~MetricSystem();
     MetricSystem(const MetricSystem &) = delete;

@@ -5,7 +5,7 @@
  * entry in __graft_entry__.py and bench.py's cpu_baseline / --impl reference
  * legs may load it.  The product (loghisto_b200/) never links or calls it.
  *
- * What it restates (all citations are /root/reference/<file>:<line>):
+ * What it restates (all citations are <file>:<line> in the reference repository):
  *   compress            metrics.go:316-322   (precision = 100, metrics.go:40-43)
  *   decompress          metrics.go:326-332
  *   Histogram ingest    metrics.go:273-295   (dense uint64[65536] indexed by (uint16)key)

@@ -120,7 +120,9 @@ def test_slow_subscriber_is_closed_not_blocked_on(MS):
     ms = MS()
     sub = ms.SubscribeToProcessedMetrics(1)
     ms.Start()
-    time.sleep(0.2)
+    # long enough for the reaper to send once and miss twice even where one collection takes a few hundred ms
+    # (a host whose CPU quota throttles the process); receiving earlier would drain the channel between its passes
+    time.sleep(2.0)
     got = sub.receive(0.5)           # the one buffered set
     assert got is not None
     with pytest.raises(EOFError):

@@ -1,7 +1,7 @@
 """Pin the CPU oracle against every known-answer vector the reference holds for
 the ingest + reduction path (SURVEY.md section 8c, KAT-1..KAT-6).
 
-All citations are /root/reference/<file>:<line>; nothing here reads that tree.
+All citations are <file>:<line> in the reference repository; nothing here reads it.
 """
 import math
 

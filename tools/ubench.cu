@@ -1,7 +1,7 @@
-// ubench.cu -- shared-memory primitive costs on sm_100a that decide the keyed-path design (round 2):
-// returning vs non-returning ATOMS on ~148 spread addresses, MATCH.ANY, ballot-built peer masks, plain LDS/STS.
+// ubench.cu -- shared-memory primitive costs that decide the keyed-path design:
+// returning vs non-returning ATOMS on ~132 spread addresses (one per SM-owner), MATCH.ANY, ballot-built peer masks, plain LDS/STS.
 // Prints cycles per warp-level operation per SM at a given number of resident warps.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/ubench tools/ubench.cu && tools/ubench
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/ubench tools/ubench.cu && tools/ubench
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
