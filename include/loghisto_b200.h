@@ -217,6 +217,25 @@ LH_API lh_status lh_snapshot_export(lh_ctx *ctx, lh_sparse *out);
 LH_API lh_status lh_snapshot_copy_histogram(lh_ctx *ctx, uint32_t histogram_id, uint64_t *h_out65536);
 LH_API lh_status lh_snapshot_end(lh_ctx *ctx);
 
+/* ---- reducing sparse histograms the caller holds ----------------------------
+ * processHistograms + percentile (metrics.go:336-418) over caller-supplied sparse histograms, independent of the
+ * context's bucket arrays and snapshot state.  Histogram i is entries [offsets[i], offsets[i+1]) of keys/counts
+ * (the lh_sparse layout, so an export can be passed back verbatim); keys may come in any order and may repeat
+ * (repeats are summed, wrapping uint64, as a merge would).  Outputs as lh_snapshot_reduce, n_histograms long.
+ *
+ * The answer for histogram i is processHistograms' for the Go map map[int16]*uint64 its entries form, including
+ * keys whose merged count is 0: with a total above 0, p <= 0 returns the smallest key present; a present key whose
+ * decompress is +-Inf (precision <= 46) with a merged count of 0 makes the sum and avg NaN (Inf * 0).
+ * n_histograms is not bounded by max_histograms.  Inputs are host memory (pageable or pinned); the call is
+ * synchronous.  LH_ERR_INVALID, before anything is launched, when offsets decrease, np > LH_MAX_PERCENTILES, or an
+ * input is NULL while there are entries; n_histograms == 0 is a no-op.  Thread-safe beside ingest, snapshots,
+ * the all-reduce and other calls of this function; the context's bucket arrays, snapshot results and stats
+ * counters of samples / snapshots are left as they were. */
+LH_API lh_status lh_reduce_sparse_host(lh_ctx *ctx, uint32_t n_histograms, const uint32_t *h_offsets,
+                                       const int16_t *h_keys, const uint64_t *h_counts,
+                                       const double *percentiles, uint32_t np,
+                                       uint64_t *counts, double *sums, double *avgs, int32_t *pkeys, double *pvals);
+
 /* ---- multi-GPU: sharded sample stream, bucket arrays summed at snapshot time (SURVEY.md section 8e) -------------
  * One context per GPU (one process per GPU, or one thread per GPU in one process).  Each rank ingests its shard
  * into its own arrays; between lh_snapshot_begin and the reduction, lh_snapshot_allreduce sums the live window of

@@ -496,9 +496,69 @@ func (ms *MetricSystem) processHistograms(name string, r *reducedHistogram, labe
 	return output
 }
 
-// processMetrics, metrics.go:483-506.  Accepts the sets collectRawMetrics produced (every caller in the reference:
-// the reaper at metrics.go:587 and metrics_test.go); a hand-built RawMetricSet has no device reduction to go with it,
-// so its histograms are reported as an error and skipped.
+// reduceSparse reduces the maps of `names` on the device (lh_reduce_sparse_host) with the percentiles configured
+// now, as processHistograms reads ms.percentiles: one CSR of every map, one call.  Keys with a count of 0 are passed
+// as entries like any other; the device keeps Go's answer for them.
+func (ms *MetricSystem) reduceSparse(e *b200Engine, hists map[string]map[int16]*uint64, names []string) *reducedSet {
+	red := &reducedSet{byName: map[string]*reducedHistogram{}}
+	for label, p := range ms.percentiles {
+		if len(red.labels) == C.LH_MAX_PERCENTILES {
+			glog.Errorf("loghisto (b200): more than %d percentiles configured; %q ignored", C.LH_MAX_PERCENTILES, label)
+			continue
+		}
+		red.labels = append(red.labels, label)
+		red.ps = append(red.ps, p)
+	}
+	np, n := len(red.ps), len(names)
+	// plain Go slices without Go pointers in them: cgo lets C read them for the duration of the call
+	total := 0
+	for _, name := range names {
+		total += len(hists[name])
+	}
+	offsets := make([]uint32, n+1)
+	keys := make([]int16, total+1)
+	cnts := make([]uint64, total+1)
+	pos := 0
+	for i, name := range names {
+		offsets[i] = uint32(pos)
+		for k, c := range hists[name] {
+			keys[pos], cnts[pos] = k, *c
+			pos++
+		}
+	}
+	offsets[n] = uint32(pos)
+	counts := make([]uint64, n)
+	sums := make([]float64, n)
+	avgs := make([]float64, n)
+	pkeys := make([]int32, n*np+1)
+	pvals := make([]float64, n*np+1)
+	var psPtr *C.double
+	if np > 0 {
+		psPtr = (*C.double)(unsafe.Pointer(&red.ps[0]))
+	}
+	st := C.lh_reduce_sparse_host(e.ctx, C.uint32_t(n), (*C.uint32_t)(unsafe.Pointer(&offsets[0])),
+		(*C.int16_t)(unsafe.Pointer(&keys[0])), (*C.uint64_t)(unsafe.Pointer(&cnts[0])), psPtr, C.uint32_t(np),
+		(*C.uint64_t)(unsafe.Pointer(&counts[0])), (*C.double)(unsafe.Pointer(&sums[0])),
+		(*C.double)(unsafe.Pointer(&avgs[0])), (*C.int32_t)(unsafe.Pointer(&pkeys[0])),
+		(*C.double)(unsafe.Pointer(&pvals[0])))
+	if err := b200Status(st, e.ctx, "lh_reduce_sparse_host"); err != nil {
+		glog.Errorf("loghisto (b200): %v; the histograms of this RawMetricSet are lost", err)
+		return red
+	}
+	for i, name := range names {
+		red.byName[name] = &reducedHistogram{
+			count: counts[i], sum: sums[i], avg: avgs[i],
+			pkeys: append([]int32(nil), pkeys[i*np:(i+1)*np]...),
+			pvals: append([]float64(nil), pvals[i*np:(i+1)*np]...),
+		}
+	}
+	return red
+}
+
+// processMetrics, metrics.go:483-506, for any RawMetricSet.  A set collectRawMetrics produced is processed with the
+// reduction the device made for its snapshot (parked beside it, consumed here); the histograms of every other set --
+// hand-built or deserialised sets, unions of several hosts' sets, a set processed a second time or after it aged out
+// of the ring -- are gathered into one CSR and reduced on the device by one lh_reduce_sparse_host call.
 func (ms *MetricSystem) processMetrics(rawMetrics *RawMetricSet) *ProcessedMetricSet {
 	e := engineFor(ms)
 	metrics := make(map[string]float64)
@@ -512,17 +572,24 @@ func (ms *MetricSystem) processMetrics(rawMetrics *RawMetricSet) *ProcessedMetri
 	}
 
 	red := e.takeReduced(rawMetrics)
+	var missing []string
 	for name := range rawMetrics.Histograms {
-		var r *reducedHistogram
-		if red != nil {
-			r = red.byName[name]
-		}
-		if r == nil {
-			glog.Errorf("loghisto (b200): no device reduction for histogram %q of this RawMetricSet; skipped", name)
+		if red == nil || red.byName[name] == nil {
+			missing = append(missing, name)
 			continue
 		}
-		for histoName, histoValue := range ms.processHistograms(name, r, red.labels) {
+		for histoName, histoValue := range ms.processHistograms(name, red.byName[name], red.labels) {
 			metrics[histoName] = histoValue
+		}
+	}
+	if len(missing) > 0 {
+		fresh := ms.reduceSparse(e, rawMetrics.Histograms, missing)
+		for _, name := range missing {
+			if r := fresh.byName[name]; r != nil {
+				for histoName, histoValue := range ms.processHistograms(name, r, fresh.labels) {
+					metrics[histoName] = histoValue
+				}
+			}
 		}
 	}
 

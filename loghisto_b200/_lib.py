@@ -104,6 +104,7 @@ SIGNATURES = {
     "lh_snapshot_export": (_i32, [_vp, C.POINTER(lh_sparse)]),
     "lh_snapshot_copy_histogram": (_i32, [_vp, _u32, _vp]),
     "lh_snapshot_end": (_i32, [_vp]),
+    "lh_reduce_sparse_host": (_i32, [_vp, _u32, _vp, _vp, _vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp]),
     "lh_comm_export": (_i32, [_vp, _vp]),
     "lh_comm_import": (_i32, [_vp, _u32, _u32, _vp]),
     "lh_snapshot_allreduce": (_i32, [_vp, _u32, C.POINTER(_u64)]),

@@ -204,6 +204,13 @@ struct lh_ctx {
     static constexpr int kCommRing = 8;
     cudaEvent_t comm_t0[kCommRing] = {}, comm_t1[kCommRing] = {};
     uint64_t ctx_id = 0;
+    // lh_reduce_sparse_host: its own stream and K6_BATCH scratch rows (allocated on first use), serialised by rs_mu;
+    // none of the arrays above is touched by it
+    std::mutex rs_mu;
+    cudaStream_t rs_stream = nullptr;
+    unsigned long long *d_rs_rows = nullptr;      // [K6_BATCH][65536], all zero between calls
+    uint32_t *d_rs_flags = nullptr, *d_rs_nnz = nullptr;
+    bool rs_dirty = false;                        // a call failed part-way: zero the rows before the next one
     K1Variant k1[kNumK1Variants];
     // timing of the most recent ingest kernel
     // CUDA events bracket every ingest launch; a ring keeps the last kTimingRing of them
@@ -879,6 +886,8 @@ extern "C" lh_status lh_destroy(lh_ctx *ctx) {
         if (ctx->res_done[i]) cudaEventDestroy(ctx->res_done[i]);
     }
     cudaFree(ctx->d_nnz); cudaFree(ctx->d_offsets);
+    cudaFree(ctx->d_rs_rows); cudaFree(ctx->d_rs_flags); cudaFree(ctx->d_rs_nnz);
+    if (ctx->rs_stream) cudaStreamDestroy(ctx->rs_stream);
     cudaFree(ctx->d_x_keys); cudaFree(ctx->d_x_counts);
     if (ctx->h_offsets) cudaFreeHost(ctx->h_offsets);
     if (ctx->h_x_keys) cudaFreeHost(ctx->h_x_keys);
@@ -1202,6 +1211,13 @@ View snapshot_view(lh_ctx *ctx) {
     return v;
 }
 
+// K3 takes the shared-memory window path when the 2*win-1 cells fit comfortably (two CTAs per SM); the dense path
+// otherwise (0 cells)
+uint32_t k3_smem_cells(uint32_t win) {
+    const size_t cells = (size_t)2 * win - 1;
+    return cells * 8 <= (size_t)100 * 1024 ? (uint32_t)cells : 0u;
+}
+
 // enqueue K3 + one packed D2H for the open snapshot into result slot `slot`
 lh_status enqueue_reduce(lh_ctx *ctx, const double *ps, uint32_t np, int slot) {
     cudaStream_t s = ctx->snap_stream;
@@ -1211,9 +1227,7 @@ lh_status enqueue_reduce(lh_ctx *ctx, const double *ps, uint32_t np, int slot) {
         LH_CUDA(ctx, cudaMemcpyAsync(ctx->d_ps[slot], ps, np * sizeof(double), cudaMemcpyHostToDevice, s));
     }
     char *d = ctx->d_res[slot];
-    // shared-memory window path when the 2*win-1 cells fit comfortably (two CTAs per SM); the dense path otherwise
-    const size_t cells = (size_t)2 * ctx->pc.win - 1;
-    const uint32_t smem_cells = cells * 8 <= (size_t)100 * 1024 ? (uint32_t)cells : 0u;
+    const uint32_t smem_cells = k3_smem_cells(ctx->pc.win);
     k_reduce<<<ctx->H, K3_THREADS, (size_t)smem_cells * 8, s>>>(v.buckets, v.flags, ctx->pc.win, ctx->d_decomp, ctx->d_ps[slot], (int)np,
                                            (unsigned long long *)(d + l.count), (double *)(d + l.sum), (double *)(d + l.avg),
                                            (int *)(d + l.pkeys), (double *)(d + l.pvals), ctx->d_nnz, smem_cells);
@@ -1365,6 +1379,127 @@ extern "C" lh_status lh_snapshot_end(lh_ctx *ctx) {
     ctx->frozen = false;
     ctx->view_reduced = false;
     ctx->view_counters_reduced = false;
+    return LH_OK;
+}
+
+// =========================================================== reduce caller-supplied sparse histograms
+namespace {
+struct AsyncBuf {   // stream-ordered device allocation, released on every return path
+    char *p = nullptr;
+    cudaStream_t s = nullptr;
+    ~AsyncBuf() { if (p) cudaFreeAsync(p, s); }
+};
+
+// The device part of lh_reduce_sparse_host, rs_mu held: one H2D of the input, per batch of K6_BATCH segments scatter
+// + K3 + epilogue + clear into the call's own result buffer, one D2H of the packed results into h_res.
+cudaError_t reduce_sparse_device(lh_ctx *ctx, uint32_t n, const uint32_t *h_offsets, const int16_t *h_keys,
+                                 const uint64_t *h_counts, const double *ps, uint32_t np, char *h_res, const char **what) {
+#define RS_CUDA(call)                                                    \
+    do {                                                                 \
+        cudaError_t _e = (call);                                         \
+        if (_e != cudaSuccess) { *what = #call; return _e; }             \
+    } while (0)
+    RS_CUDA(cudaSetDevice(ctx->device));
+    if (!ctx->rs_stream) RS_CUDA(cudaStreamCreateWithFlags(&ctx->rs_stream, cudaStreamNonBlocking));
+    cudaStream_t s = ctx->rs_stream;
+    const size_t row_bytes = (size_t)K6_BATCH * 65536u * 8u;
+    if (!ctx->d_rs_flags) RS_CUDA(cudaMalloc(&ctx->d_rs_flags, K6_BATCH * 4));
+    if (!ctx->d_rs_nnz) RS_CUDA(cudaMalloc(&ctx->d_rs_nnz, K6_BATCH * 4));
+    if (!ctx->d_rs_rows) {
+        RS_CUDA(cudaMalloc(&ctx->d_rs_rows, row_bytes));
+        ctx->rs_dirty = true;
+    }
+    if (ctx->rs_dirty) {
+        RS_CUDA(cudaMemsetAsync(ctx->d_rs_rows, 0, row_bytes, s));
+        RS_CUDA(cudaMemsetAsync(ctx->d_rs_flags, 0, K6_BATCH * 4, s));
+    }
+    ctx->rs_dirty = true;                        // until the last clear of this call has run
+
+    const uint32_t base = h_offsets[0];
+    const size_t ne = (size_t)h_offsets[n] - base;
+    const ResLayout l = res_layout(n, np);
+    const size_t off_keys = ((size_t)n + 1) * 4, off_counts = (off_keys + ne * 2 + 7) & ~(size_t)7;
+    const size_t off_ps = off_counts + ne * 8, off_res = off_ps + LH_MAX_PERCENTILES * 8;
+    AsyncBuf buf;
+    buf.s = s;
+    RS_CUDA(cudaMallocAsync((void **)&buf.p, off_res + l.total, s));
+    char *d = buf.p;
+    RS_CUDA(cudaMemcpyAsync(d, h_offsets, off_keys, cudaMemcpyHostToDevice, s));
+    if (ne) {
+        RS_CUDA(cudaMemcpyAsync(d + off_keys, h_keys + base, ne * 2, cudaMemcpyHostToDevice, s));
+        RS_CUDA(cudaMemcpyAsync(d + off_counts, h_counts + base, ne * 8, cudaMemcpyHostToDevice, s));
+    }
+    if (np) RS_CUDA(cudaMemcpyAsync(d + off_ps, ps, np * sizeof(double), cudaMemcpyHostToDevice, s));
+    const uint32_t *d_off = (const uint32_t *)d;
+    const short *d_keys = (const short *)(d + off_keys);
+    const unsigned long long *d_counts = (const unsigned long long *)(d + off_counts);
+    const double *d_ps = (const double *)(d + off_ps);
+    char *r = d + off_res;
+    unsigned long long *r_count = (unsigned long long *)(r + l.count);
+    double *r_sum = (double *)(r + l.sum), *r_avg = (double *)(r + l.avg), *r_pvals = (double *)(r + l.pvals);
+    int *r_pkeys = (int *)(r + l.pkeys);
+    const uint32_t win = ctx->pc.win, smem_cells = k3_smem_cells(win);
+    for (uint32_t b0 = 0; b0 < n; b0 += K6_BATCH) {
+        const uint32_t nb = std::min<uint32_t>(K6_BATCH, n - b0);
+        const size_t m = (size_t)h_offsets[b0 + nb] - h_offsets[b0];
+        const size_t po = (size_t)b0 * np;
+        if (m) {
+            const int grid = (int)std::min<size_t>((m + 255) / 256, (size_t)ctx->sm_count * 8);
+            k_scatter_segments<<<grid, 256, 0, s>>>(d_off + b0, nb, base, d_keys, d_counts, ctx->d_rs_rows, ctx->d_rs_flags, win);
+        }
+        k_reduce<<<nb, K3_THREADS, (size_t)smem_cells * 8, s>>>(ctx->d_rs_rows, ctx->d_rs_flags, win, ctx->d_decomp, d_ps, (int)np,
+                                                                 r_count + b0, r_sum + b0, r_avg + b0, r_pkeys + po, r_pvals + po,
+                                                                 ctx->d_rs_nnz, smem_cells);
+        k_sparse_epilogue<<<nb, 256, 0, s>>>(d_off + b0, base, d_keys, ctx->d_rs_rows, ctx->d_decomp, d_ps, (int)np,
+                                             r_count + b0, r_sum + b0, r_avg + b0, r_pkeys + po, r_pvals + po);
+        k_clear_touched<<<nb, 256, 0, s>>>(ctx->d_rs_rows, ctx->d_rs_flags, win);
+        RS_CUDA(cudaGetLastError());
+    }
+    RS_CUDA(cudaMemcpyAsync(h_res, r, l.total, cudaMemcpyDeviceToHost, s));
+    RS_CUDA(cudaStreamSynchronize(s));
+    ctx->rs_dirty = false;
+    return cudaSuccess;
+#undef RS_CUDA
+}
+}  // namespace
+
+// processHistograms + percentile over caller-supplied sparse histograms.  Never takes the context mutex while work is
+// in flight (only to record an error or the stats), and touches none of the snapshot / ingest state.
+extern "C" lh_status lh_reduce_sparse_host(lh_ctx *ctx, uint32_t n, const uint32_t *h_offsets, const int16_t *h_keys,
+                                           const uint64_t *h_counts, const double *percentiles, uint32_t np,
+                                           uint64_t *counts, double *sums, double *avgs, int32_t *pkeys, double *pvals) {
+    if (!ctx) return LH_ERR_INVALID;
+    auto bad = [ctx](lh_status st, const char *what, cudaError_t e = cudaSuccess) {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        return fail(ctx, st, what, e);
+    };
+    if (n == 0) return LH_OK;
+    if (!h_offsets) return bad(LH_ERR_INVALID, "offsets is NULL");
+    if (np > LH_MAX_PERCENTILES || (np && !percentiles)) return bad(LH_ERR_INVALID, "bad percentile array");
+    for (uint32_t i = 0; i < n; i++)
+        if (h_offsets[i + 1] < h_offsets[i]) return bad(LH_ERR_INVALID, "offsets decrease");
+    const size_t ne = (size_t)h_offsets[n] - h_offsets[0];
+    if (ne && (!h_keys || !h_counts)) return bad(LH_ERR_INVALID, "keys / counts NULL with entries");
+    const ResLayout l = res_layout(n, np);
+    std::vector<char> h_res(l.total);
+    {
+        std::lock_guard<std::mutex> rs(ctx->rs_mu);
+        const char *what = "";
+        const cudaError_t e = reduce_sparse_device(ctx, n, h_offsets, h_keys, h_counts, percentiles, np, h_res.data(), &what);
+        if (e != cudaSuccess) return bad(e == cudaErrorMemoryAllocation ? LH_ERR_NOMEM : LH_ERR_CUDA, what, e);
+    }
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        ctx->stats.kernel_launches += 4 * (((size_t)n + K6_BATCH - 1) / K6_BATCH);
+        ctx->stats.h2d_bytes += ((size_t)n + 1) * 4 + ne * 10 + np * 8;
+        ctx->stats.d2h_bytes += l.total;
+    }
+    const char *h = h_res.data();
+    if (counts) memcpy(counts, h + l.count, (size_t)n * 8);
+    if (sums) memcpy(sums, h + l.sum, (size_t)n * 8);
+    if (avgs) memcpy(avgs, h + l.avg, (size_t)n * 8);
+    if (pvals && np) memcpy(pvals, h + l.pvals, (size_t)n * np * 8);
+    if (pkeys && np) memcpy(pkeys, h + l.pkeys, (size_t)n * np * 4);
     return LH_OK;
 }
 

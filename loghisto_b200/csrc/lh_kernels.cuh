@@ -18,6 +18,8 @@
 //   K4   k_scan_nnz, k_export   sparse (key,count) lists (RawMetricSet.Histograms);  k_merge_sparse is the inverse
 //   K5   k_peer_allreduce       multi-GPU: sums the live window of every peer's frozen arrays over NVLink peer
 //                               mappings (SURVEY.md section 8e) -- no library collective
+//   K6   k_scatter_segments, k_sparse_epilogue   caller-supplied sparse histograms -> scratch rows -> K3
+//                               (lh_reduce_sparse_host)
 //   misc k_clear_touched, k_fill_decompress, k_compress_probe, k_fastpath_margin, k_stream_probe, k_gen_stream,
 //        k_gen_ids_u16
 //
@@ -1419,6 +1421,74 @@ k_clear_touched(unsigned long long *__restrict__ buckets, uint32_t *__restrict__
     }
     __syncthreads();
     if (threadIdx.x == 0) flags[h] = 0;
+}
+
+// ---------------------------------------------------------------------- K6
+// processHistograms over caller-supplied sparse histograms (lh_reduce_sparse_host), in batches of at most
+// K6_BATCH segments: k_scatter_segments adds a batch into scratch rows 0..nb-1 (flags raised as by every other
+// writer), K3 reduces the rows unchanged, k_sparse_epilogue restores what the dense rows cannot tell (a key that
+// is present with a merged count of 0), k_clear_touched zeroes the rows for the next batch.
+constexpr int K6_BATCH = 256;            // scratch rows: 256 x 512 KiB = 128 MiB
+
+// Entries [offsets[0], offsets[nb]) - base of the call's keys / counts; segment r of the batch goes to row r.
+// One thread per entry (a segment can hold the concatenated exports of many hosts); each entry finds its segment by
+// binary search over the batch's offsets in shared memory, then one 64-bit global RED per entry.
+__global__ void __launch_bounds__(256)
+k_scatter_segments(const uint32_t *__restrict__ offsets, uint32_t nb, uint32_t base, const short *__restrict__ keys,
+                   const unsigned long long *__restrict__ counts, unsigned long long *__restrict__ rows,
+                   uint32_t *__restrict__ flags, uint32_t win) {
+    __shared__ uint32_t s_off[K6_BATCH + 1];
+    for (uint32_t i = threadIdx.x; i <= nb; i += blockDim.x) s_off[i] = offsets[i] - base;
+    __syncthreads();
+    const size_t end = s_off[nb], stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t e = s_off[0] + (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < end; e += stride) {
+        uint32_t lo = 0, hi = nb - 1;              // last segment starting at or before e (empty ones share its offset)
+        while (lo < hi) { const uint32_t mid = (lo + hi + 1) >> 1; if (s_off[mid] <= e) lo = mid; else hi = mid - 1; }
+        add_bucket_global(rows + (size_t)lo * 65536u, flags + lo, (uint32_t)(int)keys[e] & 0xFFFFu, counts[e], win);
+    }
+}
+
+// One CTA per segment of the batch, after K3 and before the clear.  Go's map keeps a key whose counts summed to 0
+// (metrics.go:342-347), the dense row does not, and two answers depend on it:
+//   * p <= 0 with total > 0: percentile() returns the first entry in value order whatever its count
+//     (float64(0)/float64(total) >= p), i.e. the smallest key present; K3 gives the smallest non-empty one;
+//   * decompress(key) = +-Inf with count 0 (precision <= 46, the ends of the key range): Inf * 0 makes the sum and
+//     the average NaN; K3 skips empty cells.
+// out_* point at the batch's first result.
+__global__ void __launch_bounds__(256)
+k_sparse_epilogue(const uint32_t *__restrict__ offsets, uint32_t base, const short *__restrict__ keys,
+                  const unsigned long long *__restrict__ rows, const double *__restrict__ decomp,
+                  const double *__restrict__ ps, int np, const unsigned long long *__restrict__ out_count,
+                  double *__restrict__ out_sum, double *__restrict__ out_avg, int *__restrict__ out_pkeys,
+                  double *__restrict__ out_pvals) {
+    __shared__ int s_min[8];
+    __shared__ int s_infzero[8];
+    const uint32_t s = blockIdx.x, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    const unsigned long long *row = rows + (size_t)s * 65536u;
+    const uint32_t a = offsets[s] - base, b = offsets[s + 1] - base;
+    int kmin = 0x7FFFFFFF, infzero = 0;
+    for (uint32_t e = a + t; e < b; e += 256) {
+        const int k = keys[e];
+        const uint32_t slot = (uint32_t)k & 0xFFFFu;
+        kmin = min(kmin, k);
+        if (isinf(decomp[slot]) && row[slot] == 0ull) infzero = 1;
+    }
+    kmin = __reduce_min_sync(0xFFFFFFFFu, kmin);
+    infzero = __reduce_or_sync(0xFFFFFFFFu, (unsigned)infzero);
+    if (lane == 0) { s_min[warp] = kmin; s_infzero[warp] = infzero; }
+    __syncthreads();
+    if (t != 0) return;
+    for (int w = 1; w < 8; w++) { kmin = min(kmin, s_min[w]); infzero |= s_infzero[w]; }
+    if (infzero) {
+        out_sum[s] = __longlong_as_double(0x7FF8000000000000ll);
+        out_avg[s] = __longlong_as_double(0x7FF8000000000000ll);
+    }
+    if (out_count[s] == 0ull) return;                 // every percentile is an error (0/0 is never >= p)
+    for (int j = 0; j < np; j++)
+        if (ps[j] <= 0.0) {                           // false for NaN
+            out_pkeys[(size_t)s * np + j] = kmin;
+            out_pvals[(size_t)s * np + j] = decomp[(uint32_t)kmin & 0xFFFFu];
+        }
 }
 
 // ---------------------------------------------------------------------- K5

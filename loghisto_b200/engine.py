@@ -389,6 +389,31 @@ class Engine:
     def snapshot_end(self):
         self._check(self.lib.lh_snapshot_end(self.h))
 
+    def reduce_sparse(self, offsets, keys=None, counts=None, percentiles=()) -> Reduced:
+        """processHistograms + percentile over sparse histograms held by the caller (lh_reduce_sparse_host): histogram i
+        is entries [offsets[i], offsets[i+1]) of keys / counts, in any key order, repeats summed.  `offsets` may be a
+        `Sparse` (an export, from this engine or another), in which case keys / counts come from it and percentiles
+        may be passed as the second argument.  Touches none of the engine's snapshot or ingest state."""
+        if isinstance(offsets, Sparse):
+            if keys is not None and counts is None:
+                percentiles = keys
+            offsets, keys, counts = offsets.offsets, offsets.keys, offsets.counts
+        offsets = np.ascontiguousarray(offsets, dtype=np.uint32)
+        keys = np.ascontiguousarray(keys, dtype=np.int16)
+        counts = np.ascontiguousarray(counts, dtype=np.uint64)
+        assert offsets.size >= 1 and keys.size == counts.size and int(offsets[-1]) <= keys.size
+        ps =np.ascontiguousarray(percentiles, dtype=np.float64)
+        n, npct = offsets.size - 1, ps.size
+        out_counts = np.zeros(n, dtype=np.uint64)
+        sums = np.zeros(n, dtype=np.float64)
+        avgs = np.zeros(n, dtype=np.float64)
+        pkeys = np.zeros((n, npct), dtype=np.int32)
+        pvals = np.zeros((n, npct), dtype=np.float64)
+        self._check(self.lib.lh_reduce_sparse_host(self.h, n, offsets.ctypes.data, keys.ctypes.data, counts.ctypes.data,
+                                                   ps.ctypes.data if npct else 0, npct, out_counts.ctypes.data,
+                                                   sums.ctypes.data, avgs.ctypes.data, pkeys.ctypes.data, pvals.ctypes.data))
+        return Reduced(out_counts, sums, avgs, pkeys, pvals)
+
     def snapshot(self, percentiles, export: bool = True):
         """begin + reduce (+ export) + end; returns (Reduced, Sparse | None)."""
         self.snapshot_begin()

@@ -15,6 +15,11 @@
 
 #include "../../include/loghisto_b200.h"
 
+// Bound weakly, so that the mirror still loads over a build of the C ABI without this entry point (an older
+// libloghisto_b200.so, or a stand-in that implements only the snapshot path); processMetrics then refuses the
+// histograms of sets this system did not collect instead of failing to load.
+#pragma weak lh_reduce_sparse_host
+
 namespace loghisto {
 
 namespace {
@@ -640,20 +645,19 @@ std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
     return raw;
 }
 
-// processMetrics + processHistograms, metrics.go:483-506 and :336-387.
+// processMetrics + processHistograms, metrics.go:483-506 and :336-387.  A histogram of a set this system collected
+// uses the reduction the device made for that snapshot (parked in raw.reduced); every other histogram (hand-built or
+// deserialised sets, unions of several hosts' sets, another system's sets) is reduced from its map by one
+// lh_reduce_sparse_host call, with the percentile labels configured now, as processHistograms reads ms.percentiles.
 std::shared_ptr<ProcessedMetricSet> MetricSystem::processMetrics(const RawMetricSet &raw) {
-    if (raw.origin != this)
-        throw std::invalid_argument("processMetrics: RawMetricSet was not produced by this MetricSystem's collectRawMetrics");
     auto out = std::make_shared<ProcessedMetricSet>();
     out->Time = raw.Time;
     auto &m = out->Metrics;
     for (auto &c : raw.Counters) m[c.first] = (double)c.second;
     for (auto &r : raw.Rates) m[r.first + "_rate"] = (double)r.second;
-    for (auto &h : raw.Histograms) {
-        const std::string &name = h.first;
-        auto it = raw.reduced.find(name);
-        if (it == raw.reduced.end()) continue;
-        const ReducedHistogram &r = it->second;
+
+    auto emit = [&](const std::string &name, const ReducedHistogram &r,
+                    const std::vector<std::pair<std::string, double>> &labels) {
         const std::string sumName = name + "_sum", countName = name + "_count", avgName = name + "_avg";
         m[countName] = (double)r.count;
         m[sumName] = r.sum;
@@ -663,12 +667,56 @@ std::shared_ptr<ProcessedMetricSet> MetricSystem::processMetrics(const RawMetric
             histogram_count_store_[sumName] += go_f64_to_u64(r.sum);
             histogram_count_store_[countName] += r.count;
         }
-        for (size_t j = 0; j < raw.percentile_labels.size(); j++) {
+        for (size_t j = 0; j < labels.size(); j++) {
             if (r.pkeys[j] == std::numeric_limits<int32_t>::min()) {   // percentile() error: logged, key omitted (:380-382)
                 fprintf(stderr, "loghisto: unable to calculate percentile: Invalid percentile.  Should be between 0 and 1.\n");
                 continue;
             }
-            m[format_label(raw.percentile_labels[j].first, name)] = r.pvals[j];
+            m[format_label(labels[j].first, name)] = r.pvals[j];
+        }
+    };
+
+    // histograms without a parked reduction, as one CSR
+    std::vector<const std::string *> names;
+    std::vector<uint32_t> offsets{0};
+    std::vector<int16_t> keys;
+    std::vector<uint64_t> counts;
+    for (auto &h : raw.Histograms) {
+        if (raw.origin == this) {
+            auto it = raw.reduced.find(h.first);
+            if (it != raw.reduced.end()) {
+                emit(h.first, it->second, raw.percentile_labels);
+                continue;
+            }
+        }
+        names.push_back(&h.first);
+        for (auto &b : h.second) { keys.push_back(b.first); counts.push_back(b.second); }
+        offsets.push_back((uint32_t)keys.size());
+    }
+    if (!names.empty()) {
+        std::vector<std::pair<std::string, double>> labels;
+        {
+            std::lock_guard<std::mutex> lk(percentiles_mu_);
+            labels = percentiles_;
+        }
+        const uint32_t n = (uint32_t)names.size(), np = (uint32_t)labels.size();
+        std::vector<double> ps(np);
+        for (uint32_t j = 0; j < np; j++) ps[j] = labels[j].second;
+        std::vector<uint64_t> rc(n);
+        std::vector<double> sums(n), avgs(n), pvals((size_t)n * np);
+        std::vector<int32_t> pkeys((size_t)n * np);
+        if (!lh_reduce_sparse_host)
+            throw std::runtime_error("processMetrics: this libloghisto_b200 has no lh_reduce_sparse_host, so only sets this "
+                                     "MetricSystem collected can be processed");
+        check(ctx_, lh_reduce_sparse_host(ctx_, n, offsets.data(), keys.data(), counts.data(), ps.data(), np, rc.data(),
+                                          sums.data(), avgs.data(), pkeys.data(), pvals.data()),
+              "lh_reduce_sparse_host");
+        for (uint32_t i = 0; i < n; i++) {
+            ReducedHistogram r;
+            r.count = rc[i]; r.sum = sums[i]; r.avg = avgs[i];
+            r.pkeys.assign(pkeys.begin() + (size_t)i * np, pkeys.begin() + (size_t)(i + 1) * np);
+            r.pvals.assign(pvals.begin() + (size_t)i * np, pvals.begin() + (size_t)(i + 1) * np);
+            emit(*names[i], r, labels);
         }
     }
     for (auto &g : raw.Gauges) m[g.first] = g.second;
@@ -875,6 +923,36 @@ LHMS_API int lhms_collect_and_process(void *ms, lhms_emit_fn emit, void *ctx, ch
         auto raw = m->collectRawMetrics();
         auto p = m->processMetrics(*raw);
         emit_raw(*raw, emit, ctx);
+        emit_processed(*p, emit, ctx);
+        return 0;
+    } catch (const std::exception &e) {
+        if (err && errlen > 0) snprintf(err, (size_t)errlen, "%s", e.what());
+        return -1;
+    }
+}
+// processMetrics(raw) for a RawMetricSet built from flat arrays (a set this system did not collect): histogram i is
+// entries [offsets[i], offsets[i+1]) of keys / counts (repeated keys are summed).  Emits the processed metrics.
+// aggregates != 0 adds the reaper's _agg_* metrics as well (metrics.go:590-608).  Returns 0, or -1 with err filled.
+LHMS_API int lhms_process_metrics(void *ms, int64_t time_ns, int aggregates,
+                                  uint32_t n_counters, const char *const *counter_names, const uint64_t *counter_values,
+                                  uint32_t n_rates, const char *const *rate_names, const uint64_t *rate_values,
+                                  uint32_t n_hist, const char *const *hist_names, const uint32_t *offsets,
+                                  const int16_t *keys, const uint64_t *counts,
+                                  uint32_t n_gauges, const char *const *gauge_names, const double *gauge_values,
+                                  lhms_emit_fn emit, void *ctx, char *err, int errlen) {
+    try {
+        RawMetricSet raw;
+        raw.Time = TimePoint(std::chrono::duration_cast<TimePoint::duration>(std::chrono::nanoseconds(time_ns)));
+        for (uint32_t i = 0; i < n_counters; i++) raw.Counters[counter_names[i]] = counter_values[i];
+        for (uint32_t i = 0; i < n_rates; i++) raw.Rates[rate_names[i]] = rate_values[i];
+        for (uint32_t i = 0; i < n_hist; i++) {
+            auto &m = raw.Histograms[hist_names[i]];
+            for (uint32_t e = offsets[i]; e < offsets[i + 1]; e++) m[keys[e]] += counts[e];
+        }
+        for (uint32_t i = 0; i < n_gauges; i++) raw.Gauges[gauge_names[i]] = gauge_values[i];
+        auto *m = static_cast<MetricSystem *>(ms);
+        auto p = m->processMetrics(raw);
+        if (aggregates) m->add_aggregates(raw, *p);
         emit_processed(*p, emit, ctx);
         return 0;
     } catch (const std::exception &e) {

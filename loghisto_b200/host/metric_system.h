@@ -9,8 +9,9 @@
 //   * sysStats gauges (sys.Alloc, sys.NumGC, ... metrics.go:172-193) are Go-runtime facts and are not provided;
 //     RegisterGaugeFunc / DeregisterGaugeFunc work as in the reference.
 //   * channels are loghisto::Channel<T>: bounded, non-blocking send, closable (Go's `select { case ch <- x: default: }`).
-//   * processMetrics() accepts only RawMetricSets produced by this system's collectRawMetrics(): the
-//     per-histogram statistics were reduced on the GPU for exactly that snapshot and travel with it.
+//   * processMetrics() accepts any RawMetricSet, as the reference does.  For a set this system's collectRawMetrics()
+//     produced, the per-histogram statistics were reduced on the GPU for exactly that snapshot and travel with it;
+//     the histograms of any other set are reduced on the GPU from their maps (lh_reduce_sparse_host).
 #pragma once
 
 #include <atomic>
@@ -143,6 +144,7 @@ class MetricSystem {
     // unexported in Go, called directly by metrics_test.go; public here for the same purpose
     std::shared_ptr<RawMetricSet> collectRawMetrics();                                  // :420
     std::shared_ptr<ProcessedMetricSet> processMetrics(const RawMetricSet &raw);        // :483
+    void add_aggregates(const RawMetricSet &raw, ProcessedMetricSet &out);              // the reaper's step after it, :590-608
 
     lh_ctx *context() const { return ctx_; }
     uint64_t dropped_samples();   // ids beyond max_histograms / max_counters (never silent)
@@ -160,7 +162,6 @@ class MetricSystem {
     void commit_counters(Shard &s) noexcept;
     void flush_shard(Shard &s, std::vector<uint8_t> *touched);
     void reaper();
-    void add_aggregates(const RawMetricSet &raw, ProcessedMetricSet &out);
 
     lh_ctx *ctx_ = nullptr;
     std::chrono::nanoseconds interval_;

@@ -40,6 +40,11 @@ def _bind(L):
     L.lhms_register_constant_gauge.argtypes = [vp, C.c_char_p, C.c_double]
     L.lhms_collect_and_process.restype = C.c_int
     L.lhms_collect_and_process.argtypes = [vp, _EMIT, vp, C.c_char_p, C.c_int]
+    names, u64p = C.POINTER(C.c_char_p), C.POINTER(C.c_uint64)
+    L.lhms_process_metrics.restype = C.c_int
+    L.lhms_process_metrics.argtypes = [vp, C.c_int64, C.c_int, C.c_uint32, names, u64p, C.c_uint32, names, u64p,
+                                       C.c_uint32, names, C.POINTER(C.c_uint32), C.POINTER(C.c_int16), u64p,
+                                       C.c_uint32, names, C.POINTER(C.c_double), _EMIT, vp, C.c_char_p, C.c_int]
     L.lhms_start.argtypes = [vp]
     L.lhms_stop.argtypes = [vp]
     L.lhms_dropped.restype = C.c_uint64
@@ -206,6 +211,35 @@ class MetricSystem:
         if self._lib.lhms_collect_and_process(self._h, col.cb, None, err, 512) != 0:
             raise RuntimeError(err.value.decode())
         return col.raw, col.metrics
+
+    def processMetrics(self, raw: dict, aggregates: bool = False) -> dict:
+        """processMetrics(raw) (metrics.go:483-506) for a raw dict of the shape collect_and_process returns
+        ({"Counters", "Rates", "Histograms": {name: {key: count}}, "Gauges"}; missing parts are empty) -> metrics dict.
+        Any set is accepted: hand-built, deserialised, the union of several systems' sets, or one collected here.
+        aggregates=True also adds the _agg_avg / _agg_count / _agg_sum metrics the reaper adds (metrics.go:590-608)."""
+        def named(d, ctype):
+            keys = list(d)
+            return len(keys), (C.c_char_p * len(keys))(*[k.encode() for k in keys]), (ctype * len(keys))(*d.values())
+
+        nc, cn, cv = named(raw.get("Counters", {}), C.c_uint64)
+        nr, rn, rv = named(raw.get("Rates", {}), C.c_uint64)
+        ng, gn, gv = named(raw.get("Gauges", {}), C.c_double)
+        hists = raw.get("Histograms", {})
+        offsets, keys, counts = [0], [], []
+        for m in hists.values():
+            keys += [int(k) for k in m]
+            counts += [int(c) for c in m.values()]
+            offsets.append(len(keys))
+        hn = (C.c_char_p * len(hists))(*[k.encode() for k in hists])
+        col = _Collector()
+        err = C.create_string_buffer(512)
+        rc = self._lib.lhms_process_metrics(
+            self._h, int(raw.get("Time", 0)), 1 if aggregates else 0, nc, cn, cv, nr, rn, rv, len(hists), hn,
+            (C.c_uint32 * len(offsets))(*offsets), (C.c_int16 * len(keys))(*keys), (C.c_uint64 * len(counts))(*counts),
+            ng, gn, gv, col.cb, None, err, 512)
+        if rc != 0:
+            raise RuntimeError(err.value.decode())
+        return col.metrics
 
     def dropped(self) -> int:
         return int(self._lib.lhms_dropped(self._h))

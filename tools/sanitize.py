@@ -34,6 +34,10 @@ with lh.Engine(device=0, max_histograms=64, max_counters=64) as e:
     e.snapshot_end()
     red = e.snapshot_result(h)
     assert int(red.counts.sum()) == total, (int(red.counts.sum()), total)
+    # the export reduced again from the sparse form: more segments than one scratch batch, out-of-window keys
+    offsets = list(sp.offsets) + [int(sp.offsets[-1])] * 300
+    rs = e.reduce_sparse(offsets, sp.keys, sp.counts, PS + [-0.0])
+    assert int(rs.counts.sum()) == total
 with lh.Engine(device=0, max_histograms=4, max_counters=4) as e:    # few histograms: shared-memory privatised keyed kernel
     d = e.gen_stream(lh.STREAM_S, n, lh.DEFAULT_SEED)
     ids = e.gen_ids_u16(0, n, 4, lh.DEFAULT_SEED)
