@@ -36,7 +36,9 @@ import (
 	"github.com/golang/glog"
 )
 
-// Limits of one engine.  Names beyond them are dropped and counted (b200Dropped), never silently.
+// Limits of one engine.  Ids of idle names are recycled (nameTable), so a limit bounds the distinct names used in
+// any three consecutive intervals; a new name that finds no free id is dropped and counted (B200Dropped), never
+// silently.
 const (
 	b200MaxHistograms = 4096
 	b200MaxCounters   = 4096
@@ -80,16 +82,123 @@ type reducedSet struct {
 	byName map[string]*reducedHistogram
 }
 
+// Per-table id lifecycle (the same as the C++ mirror's NameTable, loghisto_b200/host/metric_system.h).  Each id is
+// free, live or retiring.  A name is live in an interval if a sample or counter op of it landed in that interval (a
+// histogram export segment, a counter delta or touched mark), or if intern created or revived it then.
+// collectRawMetrics, holding mu, labels the snapshot with names, then:
+//   - retiring and not live this interval -> free (name removed from ids, id pushed on freeIDs);
+//   - live and not live this interval     -> retiring, gen[id] += 1;
+//   - retiring and touched this interval  -> live (intern revives a retiring id at once, under the same name).
+// So a name last used in interval k holds its id through k+1 and k+2, and the id is free for k+3.
+//
+// Why this is enough: intern runs before the shard's mutex is taken, so a collection may run between the two.
+// Histogram and Counter therefore re-read gen[id] under s.mu and, on a mismatch, unlock, intern again and retry.
+// An append that passed that check before the bump of collection k sits in its shard until collection k+1 flushes
+// the shard at the latest (the flush takes s.mu), so it lands in interval k or k+1 and touches its id there, which
+// keeps the id under the appender's name.  An id is freed only after an interval with neither a touch nor a revival
+// following its bump, so no append validated against an older generation can land on an id handed to another name.
+const (
+	idFree uint8 = iota
+	idLive
+	idRetiring
+)
+
+type nameTable struct {
+	mu      sync.RWMutex // RLock fast path, Lock-and-recheck slow path: the idiom of metrics.go:275-294
+	ids     map[string]uint16
+	names   []string // id -> name; ids below len(names) were handed out before
+	state   []uint8
+	used    []bool   // created or revived by intern this interval
+	freeIDs []uint16 // recycled ids, taken before names grows
+	gen     []uint32 // [limit], read under a shard's mutex with atomic loads
+	limit   int
+}
+
+func newNameTable(limit int) *nameTable {
+	if limit > 65536 {
+		limit = 65536 // uint16 ids
+	}
+	return &nameTable{ids: map[string]uint16{}, gen: make([]uint32, limit), limit: limit}
+}
+
+// intern returns the id of name and its generation; ok is false when no id is free.
+func (t *nameTable) intern(name string) (id uint16, gen uint32, ok bool) {
+	t.mu.RLock()
+	id, ok = t.ids[name]
+	if ok && t.state[id] == idLive {
+		gen = atomic.LoadUint32(&t.gen[id])
+		t.mu.RUnlock()
+		return id, gen, true
+	}
+	t.mu.RUnlock()
+	t.mu.Lock()
+	defer t.mu.Unlock()
+	if id, ok = t.ids[name]; ok {
+		if t.state[id] == idRetiring {
+			t.state[id], t.used[id] = idLive, true
+		}
+		return id, atomic.LoadUint32(&t.gen[id]), true
+	}
+	switch {
+	case len(t.freeIDs) > 0:
+		id = t.freeIDs[len(t.freeIDs)-1]
+		t.freeIDs = t.freeIDs[:len(t.freeIDs)-1]
+		t.names[id] = name
+	case len(t.names) < t.limit:
+		id = uint16(len(t.names))
+		t.names = append(t.names, name)
+		t.state = append(t.state, idFree)
+		t.used = append(t.used, false)
+	default:
+		return 0, 0, false
+	}
+	t.ids[name] = id
+	t.state[id], t.used[id] = idLive, true
+	return id, atomic.LoadUint32(&t.gen[id]), true
+}
+
+// current reports whether gen is still the generation of id.  Called under the shard's mutex.
+func (t *nameTable) current(id uint16, gen uint32) bool {
+	return atomic.LoadUint32(&t.gen[id]) == gen
+}
+
+// collect returns the id -> name table the snapshot is labelled with (retiring ids included), then steps every id's
+// lifecycle; landed(id) reports whether a sample or counter op of id is in the snapshot.
+func (t *nameTable) collect(landed func(id int) bool) []string {
+	t.mu.Lock()
+	defer t.mu.Unlock()
+	labels := append([]string(nil), t.names...)
+	for id := range t.names {
+		liveNow := t.used[id] || landed(id)
+		t.used[id] = false
+		switch {
+		case t.state[id] == idRetiring && !liveNow:
+			delete(t.ids, t.names[id])
+			t.names[id] = ""
+			t.state[id] = idFree
+			t.freeIDs = append(t.freeIDs, uint16(id))
+		case t.state[id] == idLive && !liveNow:
+			t.state[id] = idRetiring
+			atomic.StoreUint32(&t.gen[id], t.gen[id]+1)
+		case t.state[id] == idRetiring:
+			t.state[id] = idLive
+		}
+	}
+	return labels
+}
+
+// snapshotNames is the id -> name table without a lifecycle step (a snapshot that failed on the device).
+func (t *nameTable) snapshotNames() []string {
+	t.mu.RLock()
+	defer t.mu.RUnlock()
+	return append([]string(nil), t.names...)
+}
+
 type b200Engine struct {
 	ctx *C.lh_ctx
 
-	histoMu    sync.RWMutex // RLock fast path, Lock-and-recheck slow path: the idiom of metrics.go:275-294
-	histoIDs   map[string]uint16
-	histoNames []string
-
-	counterMu    sync.RWMutex
-	counterIDs   map[string]uint16
-	counterNames []string
+	histos   *nameTable
+	counters *nameTable
 
 	shards  []*b200Shard
 	dropped uint64
@@ -164,7 +273,7 @@ func engineFor(ms *MetricSystem) *b200Engine {
 	cfg.staging_bytes = b200StagingBytes
 	cfg.staging_slots = C.uint32_t(2*nshards + 2) // memory of a slot is allocated on first use
 	cfg.precision = C.uint32_t(precision)          // the package constant of metrics.go:40-43
-	e := &b200Engine{histoIDs: map[string]uint16{}, counterIDs: map[string]uint16{}}
+	e := &b200Engine{histos: newNameTable(b200MaxHistograms), counters: newNameTable(b200MaxCounters)}
 	if err := b200Status(C.lh_create(&cfg, &e.ctx), nil, "lh_create"); err != nil {
 		glog.Fatalf("loghisto (b200 build): %v", err)
 	}
@@ -191,27 +300,6 @@ func (e *b200Engine) shard() *b200Shard {
 	h := uintptr(unsafe.Pointer(&marker)) // goroutine stacks are disjoint: a cheap, stable per-goroutine hash
 	h ^= h >> 17
 	return e.shards[(h>>10)%uintptr(len(e.shards))]
-}
-
-func intern(mu *sync.RWMutex, ids map[string]uint16, names *[]string, name string, limit int) (uint16, bool) {
-	mu.RLock()
-	id, ok := ids[name]
-	mu.RUnlock()
-	if ok {
-		return id, true
-	}
-	mu.Lock()
-	defer mu.Unlock()
-	if id, ok = ids[name]; ok {
-		return id, true
-	}
-	if len(*names) >= limit || len(*names) >= 65536 {
-		return 0, false
-	}
-	id = uint16(len(*names))
-	ids[name] = id
-	*names = append(*names, name)
-	return id, true
 }
 
 // openBuf acquires a pinned staging slot for b.  Called with the shard locked.
@@ -262,23 +350,35 @@ func (e *b200Engine) commitCounter(b *stagingBuf) {
 // has increased during an interval of this MetricSystem.  (metrics.go:251-269)
 func (ms *MetricSystem) Counter(name string, amount uint64) {
 	e := engineFor(ms)
-	id, ok := intern(&e.counterMu, e.counterIDs, &e.counterNames, name, b200MaxCounters)
-	if !ok {
-		atomic.AddUint64(&e.dropped, 1)
-		return
+	for {
+		id, gen, ok := e.counters.intern(name)
+		if !ok {
+			atomic.AddUint64(&e.dropped, 1)
+			return
+		}
+		if e.appendCounter(e.shard(), id, gen, amount) {
+			return
+		}
+		// the id was retired between intern and s.mu: look the name up again
 	}
-	s := e.shard()
+}
+
+// appendCounter reports false, appending nothing, when gen is no longer the generation of id (nameTable).
+func (e *b200Engine) appendCounter(s *b200Shard, id uint16, gen uint32, amount uint64) bool {
 	s.mu.Lock()
 	defer s.mu.Unlock()
+	if !e.counters.current(id, gen) {
+		return false
+	}
 	s.touched[id] = true // the name shows up in Rates even when amount == 0
 	s.anyC = true
 	if amount == 0 {
-		return
+		return true
 	}
 	b := &s.counter
 	if !b.open && !e.openBuf(b) {
 		atomic.AddUint64(&e.dropped, 1)
-		return
+		return true
 	}
 	b.items[b.n] = amount
 	b.ids[b.n] = id
@@ -286,24 +386,37 @@ func (ms *MetricSystem) Counter(name string, amount uint64) {
 	if b.n == b.cap {
 		e.commitCounter(b)
 	}
+	return true
 }
 
 // Histogram is used for generating rich metrics, such as percentiles, from
 // periodically occurring continuous values.  (metrics.go:273-295; compress() runs on the device, bit-exactly)
 func (ms *MetricSystem) Histogram(name string, value float64) {
 	e := engineFor(ms)
-	id, ok := intern(&e.histoMu, e.histoIDs, &e.histoNames, name, b200MaxHistograms)
-	if !ok {
-		atomic.AddUint64(&e.dropped, 1)
-		return
+	for {
+		id, gen, ok := e.histos.intern(name)
+		if !ok {
+			atomic.AddUint64(&e.dropped, 1)
+			return
+		}
+		if e.appendHist(e.shard(), id, gen, value) {
+			return
+		}
+		// the id was retired between intern and s.mu: look the name up again
 	}
-	s := e.shard()
+}
+
+// appendHist reports false, appending nothing, when gen is no longer the generation of id (nameTable).
+func (e *b200Engine) appendHist(s *b200Shard, id uint16, gen uint32, value float64) bool {
 	s.mu.Lock()
 	defer s.mu.Unlock()
+	if !e.histos.current(id, gen) {
+		return false
+	}
 	b := &s.hist
 	if !b.open && !e.openBuf(b) {
 		atomic.AddUint64(&e.dropped, 1)
-		return
+		return true
 	}
 	b.items[b.n] = math.Float64bits(value)
 	b.ids[b.n] = id
@@ -311,6 +424,7 @@ func (ms *MetricSystem) Histogram(name string, value float64) {
 	if b.n == b.cap {
 		e.commitHist(b)
 	}
+	return true
 }
 
 // collectRawMetrics, metrics.go:420-479: the cache swaps become lh_snapshot_begin (double-buffered device arrays),
@@ -355,16 +469,10 @@ func (ms *MetricSystem) collectRawMetrics() *RawMetricSet {
 	}
 	np := len(red.ps)
 
-	e.histoMu.RLock()
-	hnames := append([]string(nil), e.histoNames...)
-	e.histoMu.RUnlock()
-	e.counterMu.RLock()
-	cnames := append([]string(nil), e.counterNames...)
-	e.counterMu.RUnlock()
-
 	histograms := make(map[string]map[int16]*uint64)
 	rates := make(map[string]uint64)
-	deltas := make([]uint64, len(cnames))
+	deltas := make([]uint64, b200MaxCounters)
+	var cnames []string
 
 	if err := b200Status(C.lh_snapshot_begin(e.ctx), e.ctx, "lh_snapshot_begin"); err != nil {
 		glog.Errorf("loghisto (b200): %v; this interval's histograms and rates are lost", err)
@@ -398,6 +506,12 @@ func (ms *MetricSystem) collectRawMetrics() *RawMetricSet {
 				keys = unsafe.Slice((*int16)(unsafe.Pointer(sp.keys)), total)
 				cnts = unsafe.Slice((*uint64)(unsafe.Pointer(sp.counts)), total)
 			}
+			cd := unsafe.Slice((*uint64)(unsafe.Pointer(sp.counter_deltas)), b200MaxCounters)
+			copy(deltas, cd)
+			// label the export with the id -> name tables as they stand, then step every id's lifecycle (nameTable);
+			// a name interned since lh_snapshot_begin has no data in this export
+			hnames := e.histos.collect(func(id int) bool { return offsets[id] != offsets[id+1] })
+			cnames = e.counters.collect(func(id int) bool { return deltas[id] != 0 || touched[id] })
 			for h, name := range hnames {
 				a, b := int(offsets[h]), int(offsets[h+1])
 				if a == b {
@@ -416,12 +530,13 @@ func (ms *MetricSystem) collectRawMetrics() *RawMetricSet {
 					pvals: append([]float64(nil), pvals[h*np:(h+1)*np]...),
 				}
 			}
-			cd := unsafe.Slice((*uint64)(unsafe.Pointer(sp.counter_deltas)), b200MaxCounters)
-			copy(deltas, cd[:len(cnames)])
 		}
 		if err := b200Status(C.lh_snapshot_end(e.ctx), e.ctx, "lh_snapshot_end"); err != nil {
 			glog.Errorf("loghisto (b200): %v", err)
 		}
+	}
+	if cnames == nil { // no export: rates from the touched marks alone, and no lifecycle step this time
+		cnames = e.counters.snapshotNames()
 	}
 
 	// Rates = this interval's deltas of the counters touched (metrics.go:430-433); Counters = cumulative store,

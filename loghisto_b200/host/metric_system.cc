@@ -131,11 +131,13 @@ inline uint64_t hash_bytes(const char *p, size_t n) {
 
 struct NameCache {
     // open addressing, linear probing, load factor <= 1/2: a name that was interned once is found without ever going
-    // back to the shared table (a direct-mapped cache thrashes as soon as two hot names collide).  Entries are 24
-    // bytes; the names' bytes live in an append-only arena owned by the cache.
+    // back to the shared table (a direct-mapped cache thrashes as soon as two hot names collide).  Entries are 48
+    // bytes; the names' bytes live in an append-only arena owned by the cache.  An entry holds the id's generation
+    // too: the append re-checks it, and refreshes the entry through put() when the id was retired since.
     struct Entry {                               // id_plus1 == 0: empty
         uint64_t hash; const char *name; uint32_t len; uint32_t id_plus1;
         uint64_t w0, w1;                         // short_words() of a name of at most 16 bytes: it never touches the arena
+        uint32_t gen;
         bool matches(uint64_t h, const char *p, size_t n) const {
             if (hash != h || len != n) return false;
             if (n <= 16) {
@@ -152,24 +154,30 @@ struct NameCache {
     char *arena_next = nullptr;
     size_t count = 0;
     const Entry *last = nullptr;                 // most recently found entry: a thread that repeats one name skips the hash
-    bool find_last(const char *p, size_t n, uint32_t *id) const {
+    bool find_last(const char *p, size_t n, uint32_t *id, uint32_t *gen) const {
         const Entry *x = last;
         if (x && x->len == n) {
             bool same;
             if (n <= 16) { uint64_t a0, a1; short_words(p, n, &a0, &a1); same = a0 == x->w0 && a1 == x->w1; }
             else same = memcmp(x->name, p, n) == 0;
-            if (same) { *id = x->id_plus1 - 1; return true; }
+            if (same) { *id = x->id_plus1 - 1; *gen = x->gen; return true; }
         }
         return false;
     }
-    bool find(uint64_t h, const char *p, size_t n, uint32_t *id) {
-        if (e.empty()) return false;
+    Entry *probe(uint64_t h, const char *p, size_t n) {
+        if (e.empty()) return nullptr;
         const size_t mask = e.size() - 1;
         for (size_t i = h & mask;; i = (i + 1) & mask) {
-            const Entry &x = e[i];
-            if (!x.id_plus1) return false;
-            if (x.matches(h, p, n)) { *id = x.id_plus1 - 1; last = &x; return true; }
+            Entry &x = e[i];
+            if (!x.id_plus1) return nullptr;
+            if (x.matches(h, p, n)) return &x;
         }
+    }
+    bool find(uint64_t h, const char *p, size_t n, uint32_t *id, uint32_t *gen) {
+        const Entry *x = probe(h, p, n);
+        if (!x) return false;
+        *id = x->id_plus1 - 1; *gen = x->gen; last = x;
+        return true;
     }
     void insert_raw(const Entry &en) {
         const size_t mask = e.size() - 1;
@@ -177,7 +185,8 @@ struct NameCache {
         while (e[i].id_plus1) i = (i + 1) & mask;
         e[i] = en;
     }
-    void put(uint64_t h, const char *p, size_t n, uint32_t id) {
+    void put(uint64_t h, const char *p, size_t n, uint32_t id, uint32_t gen) {
+        if (Entry *x = probe(h, p, n)) { x->id_plus1 = id + 1; x->gen = gen; return; }   // refresh in place
         if (e.empty()) e.assign(256, Entry{});
         last = nullptr;
         if ((count + 1) * 2 > e.size()) {        // grow and rehash
@@ -193,7 +202,7 @@ struct NameCache {
         }
         memcpy(arena_next, p, n);
         Entry en{};
-        en.hash = h; en.name = arena_next; en.len = (uint32_t)n; en.id_plus1 = id + 1;
+        en.hash = h; en.name = arena_next; en.len = (uint32_t)n; en.id_plus1 = id + 1; en.gen = gen;
         if (n <= 16) short_words(p, n, &en.w0, &en.w1);
         insert_raw(en);
         arena_next += n; arena_left -= n;
@@ -311,7 +320,7 @@ std::atomic<bool> g_logged_staging{false};
 
 std::chrono::nanoseconds TimerToken::Stop() {
     auto d = std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - Start);
-    if (id_valid) System->histogram_id(id, (double)d.count());   // float64(duration.Nanoseconds()); name interned by StartTimer
+    if (id_valid) System->histogram_id(Name, id, gen, (double)d.count());   // float64(duration.Nanoseconds()); name interned by StartTimer
     else System->Histogram(Name, (double)d.count());
     return d;
 }
@@ -339,6 +348,11 @@ MetricSystem::MetricSystem(std::chrono::nanoseconds interval, bool /*sysStats*/,
     cfg.precision = opt.precision;
     lh_status st = lh_create(&cfg, &ctx_);
     if (st != LH_OK) throw std::runtime_error(std::string("lh_create: ") + lh_strerror(st));
+    for (auto *t : {&histos_, &counters_}) {
+        t->capacity = std::min<uint32_t>(t == &histos_ ? opt.max_histograms : opt.max_counters, 65536u);   // u16 ids
+        t->gen.reset(new std::atomic<uint32_t>[t->capacity]);
+        for (uint32_t i = 0; i < t->capacity; i++) t->gen[i].store(0, std::memory_order_relaxed);
+    }
     for (uint32_t i = 0; i < nshards + nshared; i++) {
         shards_.emplace_back(new Shard());
         shards_.back()->c_touched.assign(opt.max_counters, 0);
@@ -388,25 +402,65 @@ void MetricSystem::SpecifyPercentiles(const std::map<std::string, double> &perce
     if (percentiles_.size() > LH_MAX_PERCENTILES) percentiles_.resize(LH_MAX_PERCENTILES);
 }
 
-uint16_t MetricSystem::intern(std::shared_mutex &mu, std::unordered_map<std::string, uint32_t> &ids,
-                              std::vector<std::string> &names, const std::string &name, uint32_t limit, bool *ok) {
+// name -> (id, generation); false when no id is free (the caller drops and counts the sample).  A retiring name is
+// revived, a new one takes a free id; both count as a use of the name in this interval (NameTable).
+bool MetricSystem::intern(NameTable &t, const char *p, size_t n, uint32_t *id, uint32_t *gen) {
+    const std::string name(p, n);
     {   // read-lock fast path, then write-lock and re-check: the idiom of metrics.go:275-294
-        std::shared_lock<std::shared_mutex> rl(mu);
-        auto it = ids.find(name);
-        if (it != ids.end()) { *ok = true; return (uint16_t)it->second; }
+        std::shared_lock<std::shared_mutex> rl(t.mu);
+        auto it = t.ids.find(name);
+        if (it != t.ids.end() && t.state[it->second] == kLive) {
+            *id = it->second;
+            *gen = t.gen[*id].load(std::memory_order_relaxed);   // only changes under the write lock
+            return true;
+        }
     }
-    std::unique_lock<std::shared_mutex> wl(mu);
-    auto it = ids.find(name);
-    if (it != ids.end()) { *ok = true; return (uint16_t)it->second; }
-    if (names.size() >= limit || names.size() >= 65536) { *ok = false; return 0; }
-    uint32_t id = (uint32_t)names.size();
-    ids.emplace(name, id);
-    names.push_back(name);
-    *ok = true;
-    return (uint16_t)id;
+    std::unique_lock<std::shared_mutex> wl(t.mu);
+    auto it = t.ids.find(name);
+    if (it != t.ids.end()) {
+        *id = it->second;
+        if (t.state[*id] == kRetiring) { t.state[*id] = kLive; t.used[*id] = 1; }
+    } else {
+        if (!t.free_ids.empty()) {
+            *id = t.free_ids.back();
+            t.free_ids.pop_back();
+            t.names[*id] = name;
+        } else if (t.names.size() < t.capacity) {
+            *id = (uint32_t)t.names.size();
+            t.names.push_back(name);
+            t.state.push_back(kFree);
+            t.used.push_back(0);
+        } else {
+            return false;
+        }
+        t.ids.emplace(name, *id);
+        t.state[*id] = kLive;
+        t.used[*id] = 1;
+    }
+    *gen = t.gen[*id].load(std::memory_order_relaxed);
+    return true;
 }
 
-// name -> dense id through the calling thread's cache; false when the name table is full (sample dropped, counted)
+// The id lifecycle step of collectRawMetrics, with t.mu held for writing (NameTable).  touched[id]: a sample or
+// counter op of the id landed in the interval just collected.
+void MetricSystem::recycle(NameTable &t, const std::vector<uint8_t> &touched) {
+    for (uint32_t id = 0; id < (uint32_t)t.names.size(); id++) {
+        const bool live_now = touched[id] || t.used[id];
+        t.used[id] = 0;
+        if (t.state[id] == kRetiring && !live_now) {
+            t.ids.erase(t.names[id]);
+            t.names[id].clear();
+            t.state[id] = kFree;
+            t.free_ids.push_back(id);
+        } else if (t.state[id] == kLive && !live_now) {
+            t.state[id] = kRetiring;
+            t.gen[id].store(t.gen[id].load(std::memory_order_relaxed) + 1, std::memory_order_release);
+        } else if (t.state[id] == kRetiring) {
+            t.state[id] = kLive;
+        }
+    }
+}
+
 // The calling thread's state for THIS system (a thread that moves to another MetricSystem starts over).
 static inline ThreadState *thread_state(MetricSystem &ms, uint64_t system_id) {
     ThreadState *ts = tl_state;
@@ -421,48 +475,59 @@ static inline ThreadState *thread_state(MetricSystem &ms, uint64_t system_id) {
     return ts;
 }
 
-bool MetricSystem::lookup_histogram(const char *p, size_t n, uint32_t *id) {
+// name -> (id, generation) from the intern table, refreshing the calling thread's cache (after a miss, or after the
+// append found the cached generation stale); false when no id is free (sample dropped, counted).  Names come and go,
+// so a cache that has collected twice as many names as the table holds starts over instead of growing for ever.
+static inline void cache_put(NameCache &c, uint32_t capacity, const char *p, size_t n, uint32_t id, uint32_t gen) {
+    if (c.count >= 2 * (size_t)capacity + 64) c.reset();
+    c.put(hash_bytes(p, n), p, n, id, gen);
+}
+bool MetricSystem::lookup_histogram(const char *p, size_t n, uint32_t *id, uint32_t *gen) {
     ThreadState *ts = thread_state(*this, system_id_);
-    const uint64_t h = hash_bytes(p, n);
-    if (ts->h.find(h, p, n, id)) return true;
-    bool ok;
-    const uint16_t v = intern(histo_mu_, histo_ids_, histo_names_, std::string(p, n), opt_.max_histograms, &ok);
-    if (!ok) { dropped_over_limit_.fetch_add(1, std::memory_order_relaxed); return false; }
-    ts->h.put(h, p, n, v);
-    *id = v;
+    if (!intern(histos_, p, n, id, gen)) { dropped_over_limit_.fetch_add(1, std::memory_order_relaxed); return false; }
+    cache_put(ts->h, histos_.capacity, p, n, *id, *gen);
     return true;
 }
-bool MetricSystem::lookup_counter(const char *p, size_t n, uint32_t *id) {
+bool MetricSystem::lookup_counter(const char *p, size_t n, uint32_t *id, uint32_t *gen) {
     ThreadState *ts = thread_state(*this, system_id_);
-    const uint64_t h = hash_bytes(p, n);
-    if (ts->c.find(h, p, n, id)) return true;
-    bool ok;
-    const uint16_t v = intern(counter_mu_, counter_ids_, counter_names_, std::string(p, n), opt_.max_counters, &ok);
-    if (!ok) { dropped_over_limit_.fetch_add(1, std::memory_order_relaxed); return false; }
-    ts->c.put(h, p, n, v);
-    *id = v;
+    if (!intern(counters_, p, n, id, gen)) { dropped_over_limit_.fetch_add(1, std::memory_order_relaxed); return false; }
+    cache_put(ts->c, counters_.capacity, p, n, *id, *gen);
     return true;
 }
 
 // Ingest never fails the caller and never throws (metrics.go:570-573, 632-636: problems are logged and data is
 // dropped): a staging call that fails resets the shard, counts the samples it held as dropped and logs once.
-void MetricSystem::append_histogram(Shard &s, uint32_t id, double value) noexcept {
-    ShardGuard g(s);
-    if (!s.h_open) {
-        lh_status st = lh_staging_acquire(ctx_, &s.hs);
-        if (st != LH_OK) { s.dropped.fetch_add(1, std::memory_order_relaxed); log_once(g_logged_staging, ctx_, st, "lh_staging_acquire"); return; }
-        s.h_cap = ((size_t)s.hs.bytes / 10) & ~(size_t)15;
-        s.h_vals = reinterpret_cast<double *>(s.hs.host);
-        s.h_ids = reinterpret_cast<uint16_t *>(reinterpret_cast<char *>(s.hs.host) + s.h_cap * 8);
-        s.h_n = 0;
-        s.h_open = true;
+// The append re-checks `gen` inside the critical section, on purpose (NameTable).  If the id was retired since the
+// caller looked `name` up, it appends nothing, leaves the section and retries through the intern table (which
+// revives the name or gives it a free id); that retry cannot find a stale generation again unless another collection
+// retires the name in between, which its own revival prevents.
+void MetricSystem::append_histogram(Shard &s, uint32_t id, uint32_t gen, double value, const char *name, size_t len) noexcept {
+    {
+        ShardGuard g(s);
+        if (__builtin_expect(histos_.gen[id].load(std::memory_order_acquire) == gen, 1)) {
+            if (!s.h_open) {
+                lh_status st = lh_staging_acquire(ctx_, &s.hs);
+                if (st != LH_OK) { s.dropped.fetch_add(1, std::memory_order_relaxed); log_once(g_logged_staging, ctx_, st, "lh_staging_acquire"); return; }
+                s.h_cap = ((size_t)s.hs.bytes / 10) & ~(size_t)15;
+                s.h_vals = reinterpret_cast<double *>(s.hs.host);
+                s.h_ids = reinterpret_cast<uint16_t *>(reinterpret_cast<char *>(s.hs.host) + s.h_cap * 8);
+                s.h_n = 0;
+                s.h_open = true;
+            }
+            s.h_vals[s.h_n] = value;
+            s.h_ids[s.h_n] = (uint16_t)id;
+            if (++s.h_n == s.h_cap) commit_histograms(s);
+            return;
+        }
     }
-    s.h_vals[s.h_n] = value;
-    s.h_ids[s.h_n] = (uint16_t)id;
-    if (++s.h_n == s.h_cap) commit_histograms(s);
+    retry_histogram(s, value, name, len);
 }
-void MetricSystem::histogram_id(uint32_t id, double value) noexcept {
-    append_histogram(*static_cast<Shard *>(thread_state(*this, system_id_)->shard), id, value);
+void MetricSystem::retry_histogram(Shard &s, double value, const char *name, size_t len) noexcept {
+    uint32_t id, gen;
+    if (lookup_histogram(name, len, &id, &gen)) append_histogram(s, id, gen, value, name, len);   // else dropped, counted
+}
+void MetricSystem::histogram_id(const std::string &name, uint32_t id, uint32_t gen, double value) noexcept {
+    append_histogram(*static_cast<Shard *>(thread_state(*this, system_id_)->shard), id, gen, value, name.data(), name.size());
 }
 
 void MetricSystem::commit_histograms(Shard &s) noexcept {
@@ -494,44 +559,61 @@ void MetricSystem::Histogram(const char *name, size_t len, double value) noexcep
     // steady state: one thread-local pointer, one hash of the name's bytes, one probe of this thread's name cache, one
     // uncontended spinlock, two stores into pinned memory
     ThreadState *ts = thread_state(*this, system_id_);
-    uint32_t id;
-    if (!ts->h.find_last(name, len, &id) && __builtin_expect(!ts->h.find(hash_bytes(name, len), name, len, &id), 0)) {
-        if (!lookup_histogram(name, len, &id)) return;              // name table full: dropped and counted
+    uint32_t id, gen;
+    if (!ts->h.find_last(name, len, &id, &gen) && __builtin_expect(!ts->h.find(hash_bytes(name, len), name, len, &id, &gen), 0)) {
+        if (!lookup_histogram(name, len, &id, &gen)) return;        // no free id: dropped and counted
     }
-    append_histogram(*static_cast<Shard *>(ts->shard), id, value);
+    append_histogram(*static_cast<Shard *>(ts->shard), id, gen, value, name, len);
 }
 
 void MetricSystem::Counter(const std::string &name, uint64_t amount) noexcept {
     ThreadState *ts = thread_state(*this, system_id_);
-    uint32_t id;
-    if (!ts->c.find_last(name.data(), name.size(), &id) &&
-        __builtin_expect(!ts->c.find(hash_bytes(name.data(), name.size()), name.data(), name.size(), &id), 0)) {
-        if (!lookup_counter(name.data(), name.size(), &id)) return;  // name table full: dropped and counted
+    uint32_t id, gen;
+    if (!ts->c.find_last(name.data(), name.size(), &id, &gen) &&
+        __builtin_expect(!ts->c.find(hash_bytes(name.data(), name.size()), name.data(), name.size(), &id, &gen), 0)) {
+        if (!lookup_counter(name.data(), name.size(), &id, &gen)) return;   // no free id: dropped and counted
     }
-    Shard &s = *static_cast<Shard *>(ts->shard);
-    ShardGuard g(s);
-    s.c_touched[id] = 1;                    // Counter(name, 0) still makes the name appear in Rates (metrics.go:430-433)
-    s.c_any_touched = true;
-    if (amount == 0) return;                // nothing to add on the device
-    if (!s.c_open) {
-        lh_status st = lh_staging_acquire(ctx_, &s.cs);
-        if (st != LH_OK) { s.dropped.fetch_add(1, std::memory_order_relaxed); log_once(g_logged_staging, ctx_, st, "lh_staging_acquire"); return; }
-        s.c_cap = ((size_t)s.cs.bytes / 10) & ~(size_t)15;
-        s.c_amounts = reinterpret_cast<uint64_t *>(s.cs.host);
-        s.c_ids = reinterpret_cast<uint16_t *>(reinterpret_cast<char *>(s.cs.host) + s.c_cap * 8);
-        s.c_n = 0;
-        s.c_open = true;
+    append_counter(*static_cast<Shard *>(ts->shard), id, gen, amount, name.data(), name.size());
+}
+
+// as append_histogram: the generation is checked inside the critical section, a stale one retried by name
+void MetricSystem::append_counter(Shard &s, uint32_t id, uint32_t gen, uint64_t amount, const char *name, size_t len) noexcept {
+    {
+        ShardGuard g(s);
+        if (__builtin_expect(counters_.gen[id].load(std::memory_order_acquire) == gen, 1)) {
+            s.c_touched[id] = 1;            // Counter(name, 0) still makes the name appear in Rates (metrics.go:430-433)
+            s.c_any_touched = true;
+            if (amount == 0) return;        // nothing to add on the device
+            if (!s.c_open) {
+                lh_status st = lh_staging_acquire(ctx_, &s.cs);
+                if (st != LH_OK) { s.dropped.fetch_add(1, std::memory_order_relaxed); log_once(g_logged_staging, ctx_, st, "lh_staging_acquire"); return; }
+                s.c_cap = ((size_t)s.cs.bytes / 10) & ~(size_t)15;
+                s.c_amounts = reinterpret_cast<uint64_t *>(s.cs.host);
+                s.c_ids = reinterpret_cast<uint16_t *>(reinterpret_cast<char *>(s.cs.host) + s.c_cap * 8);
+                s.c_n = 0;
+                s.c_open = true;
+            }
+            s.c_amounts[s.c_n] = amount;
+            s.c_ids[s.c_n] = (uint16_t)id;
+            if (++s.c_n == s.c_cap) commit_counters(s);
+            return;
+        }
     }
-    s.c_amounts[s.c_n] = amount;
-    s.c_ids[s.c_n] = (uint16_t)id;
-    if (++s.c_n == s.c_cap) commit_counters(s);
+    retry_counter(s, amount, name, len);
+}
+void MetricSystem::retry_counter(Shard &s, uint64_t amount, const char *name, size_t len) noexcept {
+    uint32_t id, gen;
+    if (lookup_counter(name, len, &id, &gen)) append_counter(s, id, gen, amount, name, len);   // else dropped, counted
 }
 
 TimerToken MetricSystem::StartTimer(const std::string &name) {
     TimerToken t;
     t.Name = name;
     t.System = this;
-    t.id_valid = lookup_histogram(name.data(), name.size(), &t.id);   // interned once here; Stop() skips the lookup
+    // interned once here; Stop() skips the lookup unless the id was retired in between
+    ThreadState *ts = thread_state(*this, system_id_);
+    t.id_valid = ts->h.find(hash_bytes(name.data(), name.size()), name.data(), name.size(), &t.id, &t.gen) ||
+                 lookup_histogram(name.data(), name.size(), &t.id, &t.gen);
     t.Start = std::chrono::steady_clock::now();
     return t;
 }
@@ -588,15 +670,6 @@ std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
     for (auto &s : shards_) flush_shard(*s, &touched);
     check(ctx_, lh_snapshot_begin(ctx_), "lh_snapshot_begin");   // the cache swaps of :425-428 and :460-463
 
-    std::vector<std::string> hnames, cnames;
-    {
-        std::shared_lock<std::shared_mutex> rl(histo_mu_);
-        hnames = histo_names_;
-    }
-    {
-        std::shared_lock<std::shared_mutex> rl(counter_mu_);
-        cnames = counter_names_;
-    }
     const uint32_t H = opt_.max_histograms, np = (uint32_t)raw->percentile_labels.size();
     std::vector<double> ps(np);
     for (uint32_t j = 0; j < np; j++) ps[j] = raw->percentile_labels[j].second;
@@ -611,6 +684,24 @@ std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
     } catch (...) {
         lh_snapshot_end(ctx_);
         throw;
+    }
+    // Label the export with the id -> name tables as they stand (retiring ids included), then step every id's
+    // lifecycle (NameTable), each under its table's write lock.  A name interned since lh_snapshot_begin has no data
+    // in this export.
+    std::vector<std::string> hnames, cnames;
+    {
+        std::unique_lock<std::shared_mutex> wl(histos_.mu);
+        hnames = histos_.names;
+        std::vector<uint8_t> landed(hnames.size());
+        for (size_t h = 0; h < hnames.size(); h++) landed[h] = sp.offsets[h] != sp.offsets[h + 1];
+        recycle(histos_, landed);
+    }
+    {
+        std::unique_lock<std::shared_mutex> wl(counters_.mu);
+        cnames = counters_.names;
+        std::vector<uint8_t> landed(cnames.size());
+        for (size_t c = 0; c < cnames.size(); c++) landed[c] = sp.counter_deltas[c] != 0 || touched[c];
+        recycle(counters_, landed);
     }
     // histograms: present only when touched this interval (the swapped-out cache only holds touched names)
     for (size_t h = 0; h < hnames.size(); h++) {

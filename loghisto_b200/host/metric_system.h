@@ -9,6 +9,8 @@
 //   * sysStats gauges (sys.Alloc, sys.NumGC, ... metrics.go:172-193) are Go-runtime facts and are not provided;
 //     RegisterGaugeFunc / DeregisterGaugeFunc work as in the reference.
 //   * channels are loghisto::Channel<T>: bounded, non-blocking send, closable (Go's `select { case ch <- x: default: }`).
+//   * names map to dense ids on the device, and ids of idle names are recycled (NameTable below): max_histograms /
+//     max_counters bound the distinct names used in any three consecutive intervals.  The reference has no limit.
 //   * processMetrics() accepts any RawMetricSet, as the reference does.  For a set this system's collectRawMetrics()
 //     produced, the per-histogram statistics were reduced on the GPU for exactly that snapshot and travel with it;
 //     the histograms of any other set are reduced on the GPU from their maps (lh_reduce_sparse_host).
@@ -102,6 +104,7 @@ struct TimerToken {
     std::chrono::steady_clock::time_point Start;
     MetricSystem *System = nullptr;
     uint32_t id = 0;                   // dense histogram id interned by StartTimer (not in the Go type): Stop() skips the lookup
+    uint32_t gen = 0;                  // ... while the id still carries this generation (see MetricSystem::NameTable)
     bool id_valid = false;
     std::chrono::nanoseconds Stop();   // metrics.go:242-246
 };
@@ -135,7 +138,7 @@ class MetricSystem {
     void Histogram(const char *name, size_t len, double value) noexcept;  // same, without building a std::string
     void *assign_shard(size_t thread_slot, bool *exclusive);             // internal: a thread's staging shard (exclusive while any is free)
     void release_shard(void *shard);                                      // internal: a finished thread hands its exclusive shard back
-    void histogram_id(uint32_t id, double value) noexcept;                // body of Histogram once the name is interned
+    void histogram_id(const std::string &name, uint32_t id, uint32_t gen, double value) noexcept;   // body of Histogram once the name is interned
     void RegisterGaugeFunc(const std::string &name, std::function<double()> f);   // :299
     void DeregisterGaugeFunc(const std::string &name);                    // :306
     void Start();                                                         // :644
@@ -147,17 +150,51 @@ class MetricSystem {
     void add_aggregates(const RawMetricSet &raw, ProcessedMetricSet &out);              // the reaper's step after it, :590-608
 
     lh_ctx *context() const { return ctx_; }
-    uint64_t dropped_samples();   // ids beyond max_histograms / max_counters (never silent)
+    // Samples and counter ops that were not recorded: those of a new name that found no free id (the distinct names
+    // used in any three consecutive intervals exceed max_histograms / max_counters, see NameTable), and those lost
+    // to a failed staging call.  Never silent.
+    uint64_t dropped_samples();
 
  public:
     struct Shard;
 
  private:
-    uint16_t intern(std::shared_mutex &mu, std::unordered_map<std::string, uint32_t> &ids,
-                    std::vector<std::string> &names, const std::string &name, uint32_t limit, bool *ok);
-    bool lookup_histogram(const char *p, size_t n, uint32_t *id);
-    bool lookup_counter(const char *p, size_t n, uint32_t *id);
-    void append_histogram(Shard &s, uint32_t id, double value) noexcept;
+    // Name -> dense id, per table (histograms, counters).  Ids are recycled, so the limit bounds the names in use,
+    // not every name ever seen.  Each id is free, live or retiring.  A name is live in an interval if a sample or
+    // counter op of it landed in that interval (a histogram export segment, a counter delta or touched mark), or if
+    // a lookup created or revived it then.  collectRawMetrics, holding `mu`, labels the snapshot with `names`, then:
+    //   retiring and not live this interval -> free (name removed from `ids`, id pushed on `free_ids`);
+    //   live and not live this interval     -> retiring, gen[id] += 1;
+    //   retiring and touched this interval  -> live (a lookup revives a retiring id at once, under the same name).
+    // So a name last used in interval k holds its id through k+1 and k+2, and the id is free for k+3.
+    //
+    // Why this is enough: the name -> (id, gen) lookup runs outside the shard's critical section (thread caches,
+    // TimerToken), so a collection may run between the lookup and the append.  The append therefore re-reads
+    // gen[id] INSIDE the critical section and, on a mismatch, leaves it, looks the name up again and retries.
+    // An append that passed that check before the bump of collection k sits in its shard until collection k+1
+    // flushes the shard at the latest (the flush waits for the critical section), so it lands in interval k or
+    // k+1 and touches its id there, which keeps the id under the appender's name.  An id is freed only after an
+    // interval with neither a touch nor a revival following its bump, so no append validated against an older
+    // generation can land on an id that was handed to another name.
+    enum : uint8_t { kFree = 0, kLive = 1, kRetiring = 2 };
+    struct NameTable {
+        std::shared_mutex mu;
+        std::unordered_map<std::string, uint32_t> ids;   // live and retiring names
+        std::vector<std::string> names;                  // id -> name; ids below names.size() were handed out before
+        std::vector<uint8_t> state;                      // per id in names
+        std::vector<uint8_t> used;                       // created or revived by a lookup this interval
+        std::vector<uint32_t> free_ids;                  // recycled ids, taken before names grows
+        std::unique_ptr<std::atomic<uint32_t>[]> gen;    // [capacity], read inside shard critical sections without mu
+        uint32_t capacity = 0;
+    };
+    bool intern(NameTable &t, const char *p, size_t n, uint32_t *id, uint32_t *gen);
+    void recycle(NameTable &t, const std::vector<uint8_t> &touched);
+    bool lookup_histogram(const char *p, size_t n, uint32_t *id, uint32_t *gen);
+    bool lookup_counter(const char *p, size_t n, uint32_t *id, uint32_t *gen);
+    void append_histogram(Shard &s, uint32_t id, uint32_t gen, double value, const char *name, size_t len) noexcept;
+    void append_counter(Shard &s, uint32_t id, uint32_t gen, uint64_t amount, const char *name, size_t len) noexcept;
+    __attribute__((noinline, cold)) void retry_histogram(Shard &s, double value, const char *name, size_t len) noexcept;
+    __attribute__((noinline, cold)) void retry_counter(Shard &s, uint64_t amount, const char *name, size_t len) noexcept;
     void commit_histograms(Shard &s) noexcept;
     void commit_counters(Shard &s) noexcept;
     void flush_shard(Shard &s, std::vector<uint8_t> *touched);
@@ -170,9 +207,7 @@ class MetricSystem {
     std::mutex percentiles_mu_;
     std::vector<std::pair<std::string, double>> percentiles_;   // label (with %s) -> p
 
-    std::shared_mutex histo_mu_, counter_mu_;
-    std::unordered_map<std::string, uint32_t> histo_ids_, counter_ids_;
-    std::vector<std::string> histo_names_, counter_names_;
+    NameTable histos_, counters_;
 
     std::vector<std::unique_ptr<Shard>> shards_;
     std::mutex assign_mu_;

@@ -151,7 +151,11 @@ class MetricSystem:
 
     def __init__(self, interval_s: float, sysStats: bool = False, device: int = 0, max_histograms: int = 1024,
                  max_counters: int = 1024):
-        """A Channel(capacity=0) is treated as capacity 1 by the C++ mirror (Go's unbuffered rendezvous has no
+        """max_histograms / max_counters bound the distinct histogram / counter names used in any three consecutive
+        intervals: ids of idle names are recycled, a name last used in interval k keeping its id through k+2.  A new
+        name that finds no free id has its samples dropped and counted (dropped()).
+
+        A Channel(capacity=0) is treated as capacity 1 by the C++ mirror (Go's unbuffered rendezvous has no
         equivalent for a non-blocking sender; the reaper never blocks either way, metrics.go:570-573)."""
         self._lib = _load()
         err = C.create_string_buffer(512)
@@ -242,6 +246,8 @@ class MetricSystem:
         return col.metrics
 
     def dropped(self) -> int:
+        """Samples and counter ops not recorded so far: those of new names that found no free id (more distinct names
+        in three consecutive intervals than max_histograms / max_counters), and those lost to a failed staging call."""
         return int(self._lib.lhms_dropped(self._h))
 
     def histogram_stream(self, names, kind: int, seed: int, start: int, n: int, threads: int) -> float:
