@@ -156,6 +156,36 @@ LH_API lh_status lh_staging_commit_counter_u16(lh_ctx *ctx, const lh_staging *s,
 /* give a slot back unused */
 LH_API lh_status lh_staging_abandon(lh_ctx *ctx, const lh_staging *s);
 
+/* ---- recording from CUDA code (include/loghisto_b200_device.cuh) ----------
+ * A record scope lets the caller's own kernels add samples with lh::record / lh::record_ns / lh::count /
+ * lh::BlockHistogram, without materialising (id, value) pairs in memory first.
+ *
+ *   lh_record_begin  orders `stream` (NULL = the context's ingest stream) after the zeroing of the active interval's
+ *                    arrays, fills *out with them and opens a scope.  Never blocks.
+ *   lh_record_end    marks the end of the scope on its stream (the snapshot of the interval is ordered after it) and
+ *                    closes it.  LH_ERR_INVALID for an unknown ticket or one already closed.
+ *
+ * Contract: kernels that use a recorder are enqueued on the scope's stream between the two calls, and the recorder
+ * (passed to them by value) is not used after lh_record_end.  While scopes of the active interval are open,
+ * lh_snapshot_begin makes the spare arrays active (scopes opened from then on record into the next interval) and
+ * waits until every scope of the interval being frozen has been ended; it returns LH_ERR_STATE instead when the
+ * calling thread itself holds such a scope.  Ingest calls never wait for scopes.  lh_destroy returns LH_ERR_STATE
+ * while a scope is open.  Records do not count in lh_stats.samples / counter_ops; dropped ids count in
+ * lh_stats.dropped. */
+typedef struct lh_recorder {          /* passed by value to kernels; valid only inside its scope */
+    uint64_t *d_buckets;              /* [max_histograms][65536] of the interval */
+    uint32_t *d_flags;                /* [max_histograms] */
+    uint64_t *d_counters;             /* [max_counters] interval deltas */
+    uint64_t *d_dropped;              /* the context's dropped tally */
+    uint32_t max_histograms, max_counters;
+    uint32_t block_smem_bytes;        /* shared memory one lh::BlockHistogram needs at this precision */
+    uint32_t reserved;
+    uint64_t scope;                   /* ticket for lh_record_end */
+    uint8_t prec[48];                 /* lh::Prec, opaque to C */
+} lh_recorder;
+LH_API lh_status lh_record_begin(lh_ctx *ctx, void *stream, lh_recorder *out);
+LH_API lh_status lh_record_end(lh_ctx *ctx, const lh_recorder *rec);
+
 /* ---- snapshot = collectRawMetrics' cache swap (metrics.go:425-428, 460-463)
  *
  * lh_snapshot_begin   freezes the active bucket/counter arrays and makes the
@@ -294,9 +324,10 @@ LH_API lh_status lh_gen_ids_u16(lh_ctx *ctx, int kind, uint64_t seed, uint64_t s
 
 /* ---- misc ---------------------------------------------------------------- */
 typedef struct lh_stats {
-    uint64_t samples;        /* samples accepted by ingest calls (host-side tally) */
-    uint64_t counter_ops;
-    uint64_t dropped;        /* samples with id out of range (device-side tally) */
+    uint64_t samples;        /* samples accepted by host-issued ingest calls (host-side tally; device records
+                              * through lh_recorder are not counted) */
+    uint64_t counter_ops;    /* likewise */
+    uint64_t dropped;        /* samples with id out of range (device-side tally, device records included) */
     uint64_t kernel_launches;
     uint64_t h2d_bytes;
     uint64_t d2h_bytes;

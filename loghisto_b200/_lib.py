@@ -70,6 +70,15 @@ class lh_stats(C.Structure):
     ]
 
 
+class lh_recorder(C.Structure):
+    """What device code records through (include/loghisto_b200_device.cuh); passed by value to the caller's kernels."""
+    _fields_ = [
+        ("d_buckets", C.c_void_p), ("d_flags", C.c_void_p), ("d_counters", C.c_void_p), ("d_dropped", C.c_void_p),
+        ("max_histograms", C.c_uint32), ("max_counters", C.c_uint32), ("block_smem_bytes", C.c_uint32),
+        ("reserved", C.c_uint32), ("scope", C.c_uint64), ("prec", C.c_uint8 * 48),
+    ]
+
+
 _vp, _sz, _u32, _u64, _i32 = C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint64, C.c_int32
 
 # name -> (restype, argtypes); every symbol include/loghisto_b200.h declares
@@ -96,6 +105,8 @@ SIGNATURES = {
     "lh_staging_commit_keyed_f64_u16": (_i32, [_vp, C.POINTER(lh_staging), _sz, _u64]),
     "lh_staging_commit_counter_u16": (_i32, [_vp, C.POINTER(lh_staging), _sz, _u64]),
     "lh_staging_abandon": (_i32, [_vp, C.POINTER(lh_staging)]),
+    "lh_record_begin": (_i32, [_vp, _vp, C.POINTER(lh_recorder)]),
+    "lh_record_end": (_i32, [_vp, C.POINTER(lh_recorder)]),
     "lh_snapshot_begin": (_i32, [_vp]),
     "lh_snapshot_device": (_i32, [_vp, C.POINTER(lh_device_view)]),
     "lh_snapshot_reduce": (_i32, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp]),

@@ -60,7 +60,7 @@ def _newest(paths):
 def needs_build() -> bool:
     if not os.path.exists(LIB):
         return True
-    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(ROOT, "include", "loghisto_b200.h")]
+    deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(ROOT, "include", "loghisto_b200.h"), DEVICE_HEADER]
     return _newest(deps) > os.path.getmtime(LIB)
 
 
@@ -83,6 +83,31 @@ def build(force: bool = False, verbose: bool = False) -> str:
     return LIB
 
 
+CLIENT_SRC = os.path.join(ROOT, "tests", "device_record_client.cu")
+CLIENT_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_record_client.so")
+DEVICE_HEADER = os.path.join(ROOT, "include", "loghisto_b200_device.cuh")
+
+
+def build_device_client(force: bool = False) -> str:
+    """CUDA client of the device API (tests/device_record_client.cu): a separate shared library that records into a
+    context from its own kernels, knowing the library only through the public headers."""
+    deps = [CLIENT_SRC, DEVICE_HEADER, os.path.join(ROOT, "include", "loghisto_b200.h")]
+    if not force and os.path.exists(CLIENT_LIB) and _newest(deps) <= os.path.getmtime(CLIENT_LIB):
+        return CLIENT_LIB
+    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+    if not os.path.exists(nvcc):
+        raise RuntimeError("nvcc not found: cannot build the device-record client")
+    os.makedirs(os.path.dirname(CLIENT_LIB), exist_ok=True)
+    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
+           "-Xcompiler", "-fPIC", "-shared", "-I", os.path.join(ROOT, "include"), "-o", CLIENT_LIB, CLIENT_SRC]
+    res = subprocess.run(cmd, capture_output=True, text=True)
+    if res.returncode != 0:
+        sys.stderr.write(res.stdout + res.stderr)
+        raise RuntimeError("nvcc failed building " + CLIENT_LIB)
+    return CLIENT_LIB
+
+
 if __name__ == "__main__":
     print(build(force="--force" in sys.argv, verbose=True))
     print(build_host(force="--force" in sys.argv))
+    print(build_device_client(force="--force" in sys.argv))

@@ -14,6 +14,7 @@
 #include <mutex>
 #include <new>
 #include <string>
+#include <thread>
 #include <vector>
 #include <unistd.h>
 
@@ -22,6 +23,11 @@ using namespace lh;
 namespace {
 
 struct WriterEvent { cudaStream_t stream; cudaEvent_t ev; };
+
+// an open record scope (lh_record_begin .. lh_record_end): device code is writing buffer `buf` from `stream`
+struct Scope { uint64_t ticket; int buf; cudaStream_t stream; std::thread::id thread; };
+static_assert(sizeof(Prec) == sizeof(((lh_recorder *)0)->prec) && offsetof(lh_recorder, prec) % alignof(Prec) == 0,
+              "lh_recorder.prec must hold an lh::Prec");
 
 struct Buffer {
     unsigned long long *d_buckets = nullptr;   // [H][65536]
@@ -146,6 +152,7 @@ struct lh_ctx {
     Buffer buf[2];
     int active = 0;
     bool frozen = false;
+    bool freezing = false;               // lh_snapshot_begin flipped the buffers and waits for record scopes to end
     bool nnz_valid = false;
     cudaStream_t ingest_stream = nullptr, snap_stream = nullptr, copy_stream = nullptr;
     double *d_decomp = nullptr;
@@ -223,6 +230,9 @@ struct lh_ctx {
     lh_stats stats{};
     std::mutex mu;
     std::condition_variable slot_cv;     // a staging slot came back (see slot_wait_free)
+    std::vector<Scope> scopes;           // open record scopes
+    uint64_t next_scope = 1;
+    std::condition_variable scope_cv;    // a record scope ended (see lh_snapshot_begin)
     std::string last_error;
 };
 
@@ -864,6 +874,10 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
 
 extern "C" lh_status lh_destroy(lh_ctx *ctx) {
     if (!ctx) return LH_OK;
+    {
+        std::lock_guard<std::mutex> lk(ctx->mu);
+        if (!ctx->scopes.empty()) return fail(ctx, LH_ERR_STATE, "lh_destroy with record scopes open");
+    }
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
     comm_unmap(ctx);
@@ -1155,18 +1169,71 @@ extern "C" lh_status lh_staging_abandon(lh_ctx *ctx, const lh_staging *s) {
     return LH_OK;
 }
 
+// =========================================================== record scopes
+extern "C" lh_status lh_record_begin(lh_ctx *ctx, void *stream, lh_recorder *out) {
+    LH_ENTER(ctx);
+    if (!out) return fail(ctx, LH_ERR_INVALID, "out is NULL");
+    cudaStream_t s = pick_stream(ctx, stream);
+    const int b = ctx->active;
+    lh_status st = before_write(ctx, b, s);
+    if (st != LH_OK) return st;
+    memset(out, 0, sizeof *out);
+    out->d_buckets = reinterpret_cast<uint64_t *>(ctx->buf[b].d_buckets);
+    out->d_flags = ctx->buf[b].d_flags;
+    out->d_counters = reinterpret_cast<uint64_t *>(ctx->buf[b].d_counters);
+    out->d_dropped = reinterpret_cast<uint64_t *>(ctx->d_dropped);
+    out->max_histograms = ctx->H;
+    out->max_counters = ctx->C;
+    out->block_smem_bytes = subhist_words(ctx->pc.win) * 4u;
+    out->scope = ctx->next_scope++;
+    memcpy(out->prec, &ctx->pc, sizeof ctx->pc);
+    ctx->scopes.push_back(Scope{out->scope, b, s, std::this_thread::get_id()});
+    return LH_OK;
+}
+
+extern "C" lh_status lh_record_end(lh_ctx *ctx, const lh_recorder *rec) {
+    LH_ENTER(ctx);
+    if (!rec) return fail(ctx, LH_ERR_INVALID, "rec is NULL");
+    for (size_t i = 0; i < ctx->scopes.size(); i++) {
+        if (ctx->scopes[i].ticket != rec->scope) continue;
+        const Scope sc = ctx->scopes[i];
+        ctx->scopes.erase(ctx->scopes.begin() + (long)i);
+        ctx->scope_cv.notify_all();
+        return after_write(ctx, sc.buf, sc.stream);
+    }
+    return fail(ctx, LH_ERR_INVALID, "unknown or already ended record scope");
+}
+
 // =========================================================== snapshot
 extern "C" lh_status lh_snapshot_begin(lh_ctx *ctx) {
     LH_ENTER(ctx);
     if (ctx->frozen) return fail(ctx, LH_ERR_STATE, "previous snapshot not ended");
+    if (ctx->freezing) return fail(ctx, LH_ERR_STATE, "another snapshot is waiting for record scopes");
     const int f = ctx->active;
+    if (!ctx->scopes.empty()) {
+        // device code is still writing the interval: make the spare arrays active first, so that scopes and ingest
+        // calls from now on go to the next interval and cannot starve this one, then wait (mutex released) until
+        // every scope on the buffer being frozen has ended.  Every open scope is on `f`: a scope on the other buffer
+        // would have been waited for by the snapshot that froze it.
+        const std::thread::id me = std::this_thread::get_id();
+        for (const Scope &sc : ctx->scopes)
+            if (sc.thread == me) return fail(ctx, LH_ERR_STATE, "lh_snapshot_begin from a thread that holds an open record scope");
+        ctx->active ^= 1;
+        ctx->freezing = true;
+        ctx->scope_cv.wait(_lk, [&] {
+            for (const Scope &sc : ctx->scopes)
+                if (sc.buf == f) return false;
+            return true;
+        });
+        ctx->freezing = false;
+    }
     // order the snapshot stream after every ingest launch that wrote the buffer being frozen
     for (auto &w : ctx->buf[f].writers) LH_CUDA(ctx, cudaStreamWaitEvent(ctx->snap_stream, w.ev, 0));
     if (ctx->buf[f].hot_pending) {   // drain the keyed path's uint32 window into the uint64 buckets
         lh_status st = fold_hot(ctx, f, ctx->snap_stream);
         if (st != LH_OK) return st;
     }
-    ctx->active ^= 1;
+    ctx->active = f ^ 1;
     ctx->frozen = true;
     ctx->nnz_valid = false;
     ctx->view_reduced = false;

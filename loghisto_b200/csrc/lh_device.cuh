@@ -1,156 +1,16 @@
-// lh_device.cuh -- device-side bucket arithmetic for the loghisto hot path.
+// lh_device.cuh -- device-side helpers private to the library: decompress and the synthetic stream generator.
 //
-// Two evaluators of compress() (reference metrics.go:316-322; `precision` is metrics.go:40-43, 100 by default and
-// configurable here through lh_config.precision):
-//
-//   exact_key16()   evaluates Go's math.Log algorithm (src/math/log.go, the
-//                   FreeBSD e_log.c port; identical op tree to log_amd64.s) in
-//                   FP64 with one IEEE rounding per operation (__dadd_rn /
-//                   __dmul_rn / __ddiv_rn never contract to FMA), then Go's
-//                   precision*L+0.5 and the amd64 CVTTSD2SL + low-16-bit truncation.
-//                   IEEE-754 guarantees these are the same bits the Go code
-//                   produces on amd64 (GOAMD64=v1).
-//
-//   fast_candidate() a ~14-instruction FP32 estimate of precision*ln(1+|v|) whose
-//                   error is bounded by Prec::eps bucket units.  It returns
-//                   the bucket whenever the estimate is farther than
-//                   eps from a bucket boundary and flags the sample
-//                   for exact_key16() otherwise (~0.05 % of samples at precision 100).
-//
-// The result of the pair is therefore exactly exact_key16() for every input;
-// the fast path only decides how much work it takes to get there.
+// The bucket arithmetic (compress: exact_key16, fast_candidate, key16_of and Prec) and the writers' helpers live in
+// the public device header include/loghisto_b200_device.cuh, which CUDA callers include to record from their own
+// kernels; the library's kernels include it too, so there is one definition of the bucket function.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "../../include/loghisto_b200_device.cuh"
 
 namespace lh {
 
 constexpr int LH_MAX_PCT = 32;   // == LH_MAX_PERCENTILES in include/loghisto_b200.h
-
-// Everything that depends on `precision`, derived once on the host (make_prec in lh_api.cu) and passed to the
-// kernels by value (constant bank).
-//   precision * ln(x) = a_int * e + [ c2 * e + c1 * log2(m) ],   x = m * 2^e,  c1 = precision * ln 2,
-//   a_int = floor(c1), c2 = c1 - a_int: the integer part is exact integer arithmetic, the bracket (< 64 + c1)
-//   is evaluated in FP32.
-// Fast window: keys 0..win-1 cover every x = 1+|v| < 2^63 (win = floor(precision*ln(2^63) + 0.5) + 1; 4368 at 100).
-// Shared-memory sub-histograms hold [0,win) for v >= 0 and [win, 2*win) for v < 0.
-//
-// Error budget of the estimate, in bucket units, at precision P (derivation in DESIGN.md):
-//   lg2.approx on [1,2): 2^-22 abs          * c1     = 1.7e-5 * P/100
-//   mantissa truncated to 23 bits: 2^-23 rel * P      = 1.2e-5 * P/100
-//   three FP32 roundings at magnitude < 64 + c1       = 1.2e-5 (P <= 100) .. 2.3e-5 (P <= 250)
-//   constant representation                            = 0.6e-5 * P/100
-// eps = 2^-12 * max(1, P/100) leaves a >= 4x margin; lh_fastpath_margin() measures the realised error on the device.
-struct Prec {
-    double precision;   // as a float64, the factor Go multiplies by
-    float c1;           // precision * ln2
-    float c2;           // c1 - a_int
-    float kb;           // -1023 * c2 (folds the exponent bias into the FMA of the packed form)
-    float thresh;       // 0.5 - eps
-    uint32_t a_int;     // floor(c1)
-    uint32_t win;       // fast-window length
-    uint32_t coff;      // byte-offset constant of the packed form: 0 - 1023*a_int*4 - (0x4B400000 << 2)
-    uint32_t a4;        // a_int * 4
-    uint32_t coff0;     // slot-index constant of the packed form: 0 - 1023*a_int - 0x4B400000
-    uint32_t pad0;
-};
-
-__device__ __forceinline__ double u64_as_f64(uint64_t b) { return __longlong_as_double((long long)b); }
-__device__ __forceinline__ uint64_t f64_as_u64(double d) { return (uint64_t)__double_as_longlong(d); }
-
-// Go's math.Log for finite x >= 1 (compress only ever passes 1+|v|).
-__device__ __forceinline__ double go_log_ge1(double x) {
-    const double Ln2Hi = 6.93147180369123816490e-01;
-    const double Ln2Lo = 1.90821492927058770002e-10;
-    const double L1 = 6.666666666666735130e-01;
-    const double L2 = 3.999999999940941908e-01;
-    const double L3 = 2.857142874366239149e-01;
-    const double L4 = 2.222219843214978396e-01;
-    const double L5 = 1.818357216161805012e-01;
-    const double L6 = 1.531383769920937332e-01;
-    const double L7 = 1.479819860511658591e-01;
-    const double HalfSqrt2 = 7.07106781186547524401e-01;
-
-    uint64_t xb = f64_as_u64(x);
-    int ki = (int)(xb >> 52) - 1022;                                   // Frexp exponent
-    double f1 = u64_as_f64((xb & 0x000FFFFFFFFFFFFFull) | 0x3FE0000000000000ull);  // in [0.5,1)
-    if (f1 < HalfSqrt2) { f1 = __dmul_rn(f1, 2.0); ki--; }
-    double f = __dadd_rn(f1, -1.0);
-    double k = (double)ki;
-
-    double s = __ddiv_rn(f, __dadd_rn(2.0, f));
-    double s2 = __dmul_rn(s, s);
-    double s4 = __dmul_rn(s2, s2);
-    double t1 = __dmul_rn(s2, __dadd_rn(L1, __dmul_rn(s4, __dadd_rn(L3, __dmul_rn(s4, __dadd_rn(L5, __dmul_rn(s4, L7)))))));
-    double t2 = __dmul_rn(s4, __dadd_rn(L2, __dmul_rn(s4, __dadd_rn(L4, __dmul_rn(s4, L6)))));
-    double R = __dadd_rn(t1, t2);
-    double hfsq = __dmul_rn(__dmul_rn(0.5, f), f);
-    // k*Ln2Hi - ((hfsq - (s*(hfsq+R) + k*Ln2Lo)) - f)
-    double a = __dadd_rn(__dmul_rn(s, __dadd_rn(hfsq, R)), __dmul_rn(k, Ln2Lo));
-    double b = __dsub_rn(__dsub_rn(hfsq, a), f);
-    return __dsub_rn(__dmul_rn(k, Ln2Hi), b);
-}
-
-// compress(), bit-exact.  Returns (uint16)key zero-extended.
-__device__ __noinline__ uint32_t exact_key16(double v, double precision) {
-    double x = __dadd_rn(1.0, fabs(v));
-    uint32_t key;
-    if ((f64_as_u64(x) >> 52) >= 0x7FFull) {
-        key = 0;  // log(+Inf)=+Inf, log(NaN)=NaN -> CVTTSD2SL indefinite 0x80000000 -> low 16 bits 0
-    } else {
-        double t = __dadd_rn(__dmul_rn(precision, go_log_ge1(x)), 0.5);   // 0.5 <= t < 709.8*precision + 1 < 2^31
-        key = (uint32_t)__double2int_rz(t) & 0xFFFFu;                     // CVTTSD2SL, then int16 truncation
-    }
-    if (v < 0.0) key = (0u - key) & 0xFFFFu;                              // -1 * i, int16 wrap
-    return key;
-}
-
-// Fast estimate.  On return:
-//   idx  = sub-histogram slot (valid when !slow): key for v >= 0, win + key for v < 0
-//   slow = the sample needs exact_key16()
-__device__ __forceinline__ void fast_candidate(double v, const Prec &pc, uint32_t &idx, bool &slow) {
-    double x = __dadd_rn(1.0, fabs(v));          // exactly Go's 1.0+math.Abs(value)
-    uint32_t hi = (uint32_t)__double2hiint(x);
-    uint32_t lo = (uint32_t)__double2loint(x);
-    uint32_t t = __funnelshift_l(lo, hi, 3);     // top 23 mantissa bits of x in t[22:0]
-    float m = __uint_as_float((t & 0x007FFFFFu) | 0x3F800000u);
-    float lg;
-    asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(lg) : "f"(m));
-    uint32_t eb = hi >> 20;                      // 1023 + e (sign bit is 0: x >= 1)
-    float ef = __fadd_rn(__uint_as_float(0x4B000000u | eb), -(8388608.0f + 1023.0f));  // (float)e, exact
-    float w = __fmaf_rn(lg, pc.c1, __fmul_rn(ef, pc.c2));
-    float r = __fadd_rn(w, 12582912.0f);         // 1.5*2^23: low mantissa bits = rn(w)
-    float d = __fadd_rn(w, -__fadd_rn(r, -12582912.0f));
-    uint32_t k = (eb - 1023u) * pc.a_int + (__float_as_uint(r) - 0x4B400000u);
-    // x >= 2^63, Inf and NaN (hi >= 0x43E00000) leave the window: exact path.
-    slow = (fabsf(d) > pc.thresh) | (hi >= 0x43E00000u);
-    uint32_t neg = (uint32_t)__double2hiint(v) >> 31;
-    idx = k + neg * pc.win;
-}
-
-// Map an exact (uint16)key to a sub-histogram slot, or 0xFFFFFFFF if outside the window.
-__device__ __forceinline__ uint32_t key16_to_slot(uint32_t key16, uint32_t win) {
-    if (key16 < win) return key16;
-    uint32_t nk = 65536u - key16;                // |key| for negative keys
-    if (nk < win) return win + nk;
-    return 0xFFFFFFFFu;
-}
-// Inverse: slot -> (uint16)key.  Slot win (negative zero) folds onto key 0.
-__device__ __forceinline__ uint32_t slot_to_key16(uint32_t slot, uint32_t win) {
-    return slot < win ? slot : ((65536u - (slot - win)) & 0xFFFFu);
-}
-// Is (uint16)key inside the window the snapshot kernels scan when a histogram has no out-of-window counts?
-__device__ __forceinline__ bool key16_in_window(uint32_t key16, uint32_t win) {
-    return key16 < win || key16 > 65536u - win;
-}
-
-// (uint16)key for any input, via the fast path when possible.
-__device__ __forceinline__ uint32_t key16_of(double v, const Prec &pc) {
-    uint32_t idx; bool slow;
-    fast_candidate(v, pc, idx, slow);
-    if (slow) return exact_key16(v, pc.precision);
-    return slot_to_key16(idx, pc.win);
-}
 
 // math.Exp as amd64 Go evaluates it (src/math/exp_amd64.s, non-FMA path), one
 // IEEE rounding per op.  Used once at context creation to fill the decompress table.

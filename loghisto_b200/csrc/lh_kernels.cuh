@@ -102,45 +102,6 @@ __device__ __forceinline__ void red_add_u32_keep(unsigned int *addr, unsigned in
     asm volatile("red.relaxed.gpu.global.add.L2::cache_hint.u32 [%0], %1, %2;" ::"l"(addr), "r"(v), "l"(policy) : "memory");
 }
 
-// ---------------------------------------------------------------- flags
-// level 1 = the histogram has counts inside the fast window, 3 = also outside it.  Plain read first: the flag is
-// almost always already set, and same-address atomics from every thread would serialise in L2.
-__device__ __forceinline__ void mark(uint32_t *flag, uint32_t level) {
-    if ((*reinterpret_cast<volatile uint32_t *>(flag) & level) != level) atomicOr(flag, level);
-}
-// One count (or c of them) straight into the uint64 row of a histogram, raising its flag.
-__device__ __forceinline__ void add_bucket_global(unsigned long long *__restrict__ row, uint32_t *flag, uint32_t key16,
-                                                  unsigned long long c, uint32_t win) {
-    atomicAdd(&row[key16], c);
-    mark(flag, key16_in_window(key16, win) ? 1u : 3u);
-}
-
-// Shared sub-histogram of one histogram: [0, 2*win) slots + one trash slot that is never flushed (samples
-// outside the window are counted straight into the global array and redirected there so that the shared atomic
-// stays unconditional).
-__device__ __forceinline__ uint32_t subhist_words(uint32_t win) { return 2u * win + 8u; }
-
-// Flush: one 64-bit global atomic per non-empty slot, then one flag update per CTA.
-__device__ __forceinline__ void flush_subhist(const uint32_t *hist, int tid, int nthreads,
-                                              unsigned long long *__restrict__ counts, uint32_t *flag, uint32_t win) {
-    int any = 0;
-    for (uint32_t slot = tid; slot < 2u * win; slot += nthreads) {
-        const uint32_t c = hist[slot];
-        if (c) { atomicAdd(&counts[slot_to_key16(slot, win)], (unsigned long long)c); any = 1; }
-    }
-    any = __syncthreads_or(any);
-    if (any && tid == 0) mark(flag, 1u);
-}
-
-// Exact slot of one sample for the fix-up paths; out-of-window keys are counted globally and sent to the trash slot.
-__device__ __forceinline__ uint32_t fixup_slot(double v, const Prec &pc, unsigned long long *__restrict__ counts,
-                                               uint32_t *flag) {
-    const uint32_t key = key16_of(v, pc);
-    uint32_t slot = key16_to_slot(key, pc.win);
-    if (slot == 0xFFFFFFFFu) { add_bucket_global(counts, flag, key, 1ull, pc.win); slot = 2u * pc.win; }
-    return slot;
-}
-
 // Up to three scalar stragglers on either side of the vector body (misaligned head, ragged tail).
 __device__ __forceinline__ void bucket_stragglers(const double *p, int n, const Prec &pc,
                                                   unsigned long long *__restrict__ counts, uint32_t *flag) {

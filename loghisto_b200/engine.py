@@ -6,6 +6,7 @@ comes out of the CUDA kernels behind `lh_*`.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 from dataclasses import dataclass
 
@@ -328,6 +329,26 @@ class Engine:
 
     def staging_abandon(self, s):
         self._check(self.lib.lh_staging_abandon(self.h, C.byref(s)))
+
+    # ---- recording from CUDA code (include/loghisto_b200_device.cuh)
+    def record_begin(self, stream=None) -> L.lh_recorder:
+        """Open a record scope on `stream` (None = the engine's ingest stream).  Pass the returned recorder by value to
+        kernels enqueued on that stream, then close the scope with record_end(); a snapshot waits for it."""
+        rec = L.lh_recorder()
+        self._check(self.lib.lh_record_begin(self.h, _stream(stream), C.byref(rec)))
+        return rec
+
+    def record_end(self, rec: L.lh_recorder):
+        self._check(self.lib.lh_record_end(self.h, C.byref(rec)))
+
+    @contextlib.contextmanager
+    def recording(self, stream=None):
+        """`with eng.recording(stream) as rec:` -- record_begin / record_end around the block."""
+        rec = self.record_begin(stream)
+        try:
+            yield rec
+        finally:
+            self.record_end(rec)
 
     # ---- snapshot
     def snapshot_begin(self):
