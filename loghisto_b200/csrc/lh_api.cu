@@ -506,6 +506,8 @@ lh_status launch_keyed(lh_ctx *ctx, const IdT *d_ids, const ValT *d_vals, size_t
                 hot_used = n4 * 4;
                 ctx->keyed_kernel = "k_ingest_keyed_vec";
             }
+        } else {
+            ctx->keyed_kernel = "k_ingest_keyed";   // no vector body (short or misaligned batch): the scalar kernel only
         }
         if (tail_off < m) {
             size_t r = m - tail_off;

@@ -12,7 +12,7 @@ import time
 import numpy as np
 import pytest
 
-from test_gpu_precision import thresholds
+from _ingest_routes import thresholds
 
 pytestmark = pytest.mark.gpu
 

@@ -669,11 +669,15 @@ def test_merge_sparse_snapshots(lh, oracle):
         assert (red.pkeys[3] == ref["pkeys"]).all()
 
 
-@pytest.mark.parametrize("H", [1, 5, 11, 12, 23, 33, 34])
+@pytest.mark.parametrize("H", [1, 5, 11, 12, 23, 33, 34, 44, 45])
 def test_keyed_small_h_privatized_kernel(lh, oracle, H):
-    """H <= 11 histograms: windows privatised in shared memory (k_ingest_keyed_small); up to 33 in two or three
-    passes over id sub-ranges; H = 34 takes the L2 route.
-    Either way every bucket must match the oracle, for f64 and int64-ns samples, u16 and u32 ids, bad ids dropped."""
+    """At precision 100 one pass of k_ingest_keyed_small privatises the windows of 11 histograms in shared memory and
+    up to 4 passes over id sub-ranges are taken: H <= 11 in one pass, 12 ... 44 in two to four; H = 45 would need five
+    and takes the L2-atomic kernel (k_ingest_keyed_vec) at this batch size.  The misaligned call runs the scalar kernel.
+    Every bucket must match the oracle, for f64 and int64-ns samples, u16 and u32 ids, bad ids dropped."""
+    import torch
+    import _ingest_routes as routes
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
     n = 1_200_003
     vals = oracle.gen_stream(lh.STREAM_S, n, SEED ^ H)
     ids = oracle.gen_ids(0, n, H, SEED ^ H)
@@ -683,12 +687,15 @@ def test_keyed_small_h_privatized_kernel(lh, oracle, H):
     with lh.Engine(device=0, max_histograms=H, max_counters=1) as e:
         d_v, d_i16, d_i32 = e.upload(vals), e.upload(ids_bad.astype(np.uint16)), e.upload(ids_bad)
         e.ingest_keyed_f64_u16(d_i16, d_v, n)
+        route = routes.keyed_route(H, n, 100, sms)
+        assert route.kernel == (routes.SMALL if H <= 44 else routes.VEC) and e.keyed_kernel_name() == route.kernel
         red, sp = e.snapshot(PS)
         want = oracle.ingest_keyed(ids_bad[keep], vals[keep], H)
         for h in range(H):
             assert (dense_from_sparse(sp, h) == want[h]).all(), h
         assert e.stats()["dropped"] == int((~keep).sum())
         e.ingest_keyed_f64_u32(d_i32, d_v.offset(1), n - 1)          # misaligned values: scalar fallback path
+        assert e.keyed_kernel_name() == routes.keyed_route(H, n - 1, 100, sms, id_bytes=4, vals_addr=8).kernel == routes.SCALAR
         red, sp = e.snapshot(PS)
         keep1 = keep[:n - 1]
         want1 = oracle.ingest_keyed(ids_bad[:n - 1][keep1], vals[1:][keep1], H)
@@ -698,6 +705,7 @@ def test_keyed_small_h_privatized_kernel(lh, oracle, H):
         ns[::3] *= -1
         d_n = e.upload(ns)
         e.ingest_keyed_i64ns_u16(d_i16, d_n, n)
+        assert e.keyed_kernel_name() == route.kernel
         red, sp = e.snapshot(PS)
         want2 = oracle.ingest_keyed_i64(ids_bad[keep], ns[keep], H)
         for h in range(H):

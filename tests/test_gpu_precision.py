@@ -1,16 +1,21 @@
 """Configurable `precision` (reference metrics.go:40-43: `precision = 100`; compress/decompress :316-332 use it):
-every kernel family against the oracle at three precisions.  Bar: bit-exact keys, counts, percentile buckets and
+every kernel family against the oracle across the supported range 1 ... 250.  Bar: bit-exact keys, counts, percentile buckets and
 decompressed values."""
 import numpy as np
 import pytest
 
+import _ingest_routes as routes
 import _reduce_cases as rc
 
 pytestmark = pytest.mark.gpu
 
 SEED = 0x10C415C0
 PS = [0.0, 0.5, 0.75, 0.9, 0.95, 0.99, 0.999, 0.9999, 1.0]
-PRECISIONS = [50, 100, 200]
+# 1 and 2: a_int = floor(precision * ln 2) is 0 and 1; 146 / 147 and 249 / 250: the top of the range; and the last
+# precision before / the first at which lh_create runs another K1 variant's code under a variant's name (its ring and
+# the sub-histogram no longer fit shared memory; tests/_ingest_routes.py k1_variants has the table)
+_K1_SUBSTITUTED = set(routes.k1_substitution_precisions().values())
+PRECISIONS = sorted({1, 2, 50, 100, 146, 147, 200, 249, 250} | _K1_SUBSTITUTED | {p - 1 for p in _K1_SUBSTITUTED})
 
 
 @pytest.fixture(scope="module")
@@ -26,31 +31,11 @@ def dense_from_sparse(sp, hid):
     return out
 
 
-def thresholds(oracle, precision, kmax):
-    """T[k] = smallest positive double (as bits) whose un-wrapped bucket is >= k, for k = 1..kmax (bisection on the oracle)."""
-    ks = np.arange(1, kmax + 1, dtype=np.int64)
-    lo = np.zeros(ks.size, dtype=np.uint64)
-    hi = np.full(ks.size, 0x7FEFFFFFFFFFFFFF, dtype=np.uint64)
-
-    def pre_wrap(bits):
-        v = bits.view(np.float64)
-        k16 = oracle.compress_many(v, precision).astype(np.int64) & 0xFFFF
-        approx = np.floor(precision * np.log1p(v) + 0.5)
-        wraps = np.round((approx - k16) / 65536.0)
-        return k16 + wraps.astype(np.int64) * 65536
-    for _ in range(64):
-        mid = lo + (hi - lo) // np.uint64(2)
-        ge = pre_wrap(mid) >= ks
-        hi = np.where(ge, mid, hi)
-        lo = np.where(ge, lo, mid)
-    return hi
-
-
 @pytest.mark.parametrize("precision", PRECISIONS)
 def test_compress_at_every_threshold(lh, oracle, precision):
     """Every bucket boundary of the whole finite range, +-3 ulps, both signs, both evaluators, at this precision."""
     kmax = int(np.floor(precision * np.log1p(1.7976931348623157e308) + 0.5))
-    T = thresholds(oracle, precision, kmax)
+    T = routes.thresholds(oracle, precision, kmax)
     offs = np.arange(-3, 4, dtype=np.int64)
     bits = (T[:, None].astype(np.int64) + offs[None, :]).reshape(-1).astype(np.uint64)
     bits = np.concatenate([bits, bits | np.uint64(0x8000000000000000)])
@@ -93,6 +78,8 @@ def test_every_ingest_kernel(lh, oracle, precision):
                 assert (red.pvals[1].view(np.uint64) == ref["pvals"].view(np.uint64)).all()
                 assert rc.sum_ok(float(red.sums[1]), exact), (precision, stream, name)
         # keyed kernels: few ids (shared-memory windows), many ids (L2 atomics), many ids (owner-partitioned)
+        import torch
+        sms = torch.cuda.get_device_properties(0).multi_processor_count
         for H, mode in ((3, 0), (300, 1), (300, 2)):
             ids = oracle.gen_ids(0, n, H, SEED ^ precision)
             wantk = np.zeros((H, 65536), dtype=np.uint64)
@@ -102,6 +89,8 @@ def test_every_ingest_kernel(lh, oracle, precision):
                 eng.tune("keyed_mode", mode)
                 d, di = eng.upload(vals), eng.upload(ids.astype(np.uint16))
                 eng.ingest_keyed_f64_u16(di, d, n)
+                assert eng.keyed_kernel_name() == routes.keyed_route(H, n, precision, sms, keyed_mode=mode).kernel == \
+                    (routes.SMALL, routes.VEC, routes.WC)[mode], (precision, H, mode)
                 red, sp = eng.snapshot(PS)
                 assert (red.counts == wantk.sum(axis=1)).all(), (precision, stream, H, mode, eng.keyed_kernel_name())
                 for h in (0, 1, H - 1):
@@ -111,7 +100,7 @@ def test_every_ingest_kernel(lh, oracle, precision):
 def test_precision_range_is_checked(lh):
     with pytest.raises(lh.LhError):
         lh.Engine(device=0, precision=251)
-    with lh.Engine(device=0, precision=250) as e:     # the largest supported: K1 falls back to the register-pipelined kernel
+    with lh.Engine(device=0, precision=250) as e:     # the largest supported (test_every_ingest_kernel runs full streams there)
         vals = np.array([1.0, -1.0, 1e18, 0.0, 3.5], dtype=np.float64)
         d = e.upload(vals)
         e.ingest_f64(0, d, vals.size)
