@@ -5,11 +5,14 @@
 //   lh::record(rec, id, v)        Histogram(name, v)          metrics.go:273-295 (compress, metrics.go:316-322)
 //   lh::record_ns(rec, id, ns)    TimerToken.Stop()           metrics.go:242-246  value = float64(ns)
 //   lh::count(rec, id, amount)    Counter(name, amount)       metrics.go:251-269  wrapping uint64 add
+//   lh::start_timer(id) / lh::stop(rec, token)
+//                                 StartTimer(name) / Stop()   metrics.go:232-246  durations on the GPU's clock
 //   lh::BlockHistogram            one CTA feeding one histogram through a shared-memory sub-histogram
 //
 // `rec` is an lh_recorder (include/loghisto_b200.h) obtained from lh_record_begin on the host and passed to the kernel
 // by value.  Kernels that use it must be enqueued on the recorder's stream between lh_record_begin and lh_record_end;
-// the snapshot that takes the interval waits for lh_record_end.  Records go straight into the uint64 bucket rows of the
+// the snapshot that takes the interval waits for lh_record_end.  A MetricSystem (loghisto_b200/host/metric_system.h)
+// hands out recorders and ids by name through MetricSystem::BeginRecording.  Records go straight into the uint64 bucket rows of the
 // active interval, so they are visible to lh_snapshot_reduce / _export exactly like samples of the ingest calls.
 //
 // Every function here has internal or inline linkage: the header may be included by several translation units of one
@@ -245,6 +248,40 @@ __device__ __forceinline__ void record(const lh_recorder &rec, uint32_t id, doub
 // TimerToken.Stop(): the value is float64(duration.Nanoseconds()), round-to-nearest-even as Go's CVTSQ2SD.
 __device__ __forceinline__ void record_ns(const lh_recorder &rec, uint32_t id, long long ns) {
     record(rec, id, __ll2double_rn(ns));
+}
+
+// StartTimer(name) / TimerToken.Stop() (metrics.go:232-246) measured on the device.  The clock is %globaltimer, the
+// GPU's nanosecond timer: it is NOT the host's steady_clock, and the timers of two GPUs are not synchronised, so a token
+// is stopped on the GPU that started it.  A token is plain data: it may be written to memory and stopped by another
+// thread or by a later kernel on the same GPU (queueing time between a producer and a consumer kernel).
+// start_timer needs no recorder and may run before the scope opens; stop records, so it runs inside a scope.
+struct TimerToken {
+    uint64_t start_ns;
+    uint32_t id;
+    uint32_t pad;
+};
+static_assert(sizeof(TimerToken) == 16, "lh::TimerToken is 16 bytes of plain data");
+
+__device__ __forceinline__ uint64_t globaltimer_ns() {
+    uint64_t t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+
+__device__ __forceinline__ TimerToken start_timer(uint32_t id) {
+    TimerToken t;
+    t.start_ns = globaltimer_ns();
+    t.id = id;
+    t.pad = 0;
+    return t;
+}
+
+// Records float64(now - start) under the token's id, as record_ns does, and returns the duration in ns (Go's Stop
+// returns the time.Duration it recorded).
+__device__ __forceinline__ long long stop(const lh_recorder &rec, const TimerToken &t) {
+    const long long ns = (long long)(globaltimer_ns() - t.start_ns);
+    record_ns(rec, t.id, ns);
+    return ns;
 }
 
 // Counter(name, amount): one wrapping 64-bit add into the interval's counter delta.  An id >= max_counters is

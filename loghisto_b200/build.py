@@ -88,22 +88,28 @@ CLIENT_LIB = os.path.join(ROOT, "tests", "_build", "libdevice_record_client.so")
 DEVICE_HEADER = os.path.join(ROOT, "include", "loghisto_b200_device.cuh")
 
 
+NAMED_CLIENT_SRC = os.path.join(ROOT, "tests", "named_record_client.cu")
+NAMED_CLIENT_LIB = os.path.join(ROOT, "tests", "_build", "libnamed_record_client.so")
+
+
 def build_device_client(force: bool = False) -> str:
-    """CUDA client of the device API (tests/device_record_client.cu): a separate shared library that records into a
-    context from its own kernels, knowing the library only through the public headers."""
-    deps = [CLIENT_SRC, DEVICE_HEADER, os.path.join(ROOT, "include", "loghisto_b200.h")]
-    if not force and os.path.exists(CLIENT_LIB) and _newest(deps) <= os.path.getmtime(CLIENT_LIB):
-        return CLIENT_LIB
-    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    if not os.path.exists(nvcc):
-        raise RuntimeError("nvcc not found: cannot build the device-record client")
-    os.makedirs(os.path.dirname(CLIENT_LIB), exist_ok=True)
-    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
-           "-Xcompiler", "-fPIC", "-shared", "-I", os.path.join(ROOT, "include"), "-o", CLIENT_LIB, CLIENT_SRC]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    if res.returncode != 0:
-        sys.stderr.write(res.stdout + res.stderr)
-        raise RuntimeError("nvcc failed building " + CLIENT_LIB)
+    """CUDA clients of the device API (tests/device_record_client.cu, tests/named_record_client.cu): separate shared
+    libraries that record into a context from their own kernels, knowing the library only through the public headers.
+    Returns the path of the first."""
+    for src, lib in ((CLIENT_SRC, CLIENT_LIB), (NAMED_CLIENT_SRC, NAMED_CLIENT_LIB)):
+        deps = [src, DEVICE_HEADER, os.path.join(ROOT, "include", "loghisto_b200.h")]
+        if not force and os.path.exists(lib) and _newest(deps) <= os.path.getmtime(lib):
+            continue
+        nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+        if not os.path.exists(nvcc):
+            raise RuntimeError("nvcc not found: cannot build the device-record clients")
+        os.makedirs(os.path.dirname(lib), exist_ok=True)
+        cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo",
+               "-Xcompiler", "-fPIC", "-shared", "-I", os.path.join(ROOT, "include"), "-o", lib, src]
+        res = subprocess.run(cmd, capture_output=True, text=True)
+        if res.returncode != 0:
+            sys.stderr.write(res.stdout + res.stderr)
+            raise RuntimeError("nvcc failed building " + lib)
     return CLIENT_LIB
 
 

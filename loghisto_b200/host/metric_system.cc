@@ -19,6 +19,10 @@
 // libloghisto_b200.so, or a stand-in that implements only the snapshot path); processMetrics then refuses the
 // histograms of sets this system did not collect instead of failing to load.
 #pragma weak lh_reduce_sparse_host
+// Likewise for record scopes: over a build without them, BeginRecording throws.
+#pragma weak lh_record_begin
+#pragma weak lh_record_end
+#pragma weak lh_ingest_f64
 
 namespace loghisto {
 
@@ -618,6 +622,92 @@ TimerToken MetricSystem::StartTimer(const std::string &name) {
     return t;
 }
 
+// ---- record scopes bound to names ---------------------------------------------------------------------------
+// BeginRecording hands ids to device code, which cannot re-check a generation per record as the append does.  So the
+// ids are pinned for the scope instead:
+//   1. intern every name (a retiring name is revived, a new one takes a free id) and note each id's generation;
+//   2. lh_record_begin;
+//   3. under each table's write lock, re-read the generations; if any changed, end the empty scope and start over;
+//      otherwise mark every bound id used in the current interval.
+// Why this is enough: lh_snapshot_begin does not return while the scope is open, so the collection X that labels the
+// scope's records (the first to freeze after step 2) labels them after step 3.  An unchanged generation at step 3
+// means no collection retired the id since step 1, so it is still live under this name, and the used mark of step 3
+// keeps it live through the next recycle step; a later one can only retire it (the id and its name stay), and only
+// the one after that can free it.  The recycle steps that can run between step 3 and the labelling of the interval
+// after X are at most two: the one of a collection already past lh_snapshot_begin at step 2, and X's.  So device
+// records (interval of X) and ingest calls through the scope (interval of X, or the next one when X froze first) are
+// labelled with this name.  A collection between steps 1 and 3 that retired the id changed its generation, so the
+// retry catches every other case.
+void MetricSystem::bind_names(NameTable &t, const std::vector<std::string> &names, std::vector<uint32_t> &ids,
+                              std::vector<uint32_t> &gens) {
+    ids.assign(names.size(), RecordScope::kUnbound);
+    gens.assign(names.size(), 0);
+    for (size_t i = 0; i < names.size(); i++)
+        if (!intern(t, names[i].data(), names[i].size(), &ids[i], &gens[i])) ids[i] = RecordScope::kUnbound;
+}
+bool MetricSystem::pin_names(NameTable &t, const std::vector<uint32_t> &ids, const std::vector<uint32_t> &gens) {
+    std::unique_lock<std::shared_mutex> wl(t.mu);
+    for (size_t i = 0; i < ids.size(); i++)
+        if (ids[i] != RecordScope::kUnbound && t.gen[ids[i]].load(std::memory_order_acquire) != gens[i]) return false;
+    for (uint32_t id : ids)
+        if (id != RecordScope::kUnbound) t.used[id] = 1;
+    return true;
+}
+
+RecordScope MetricSystem::BeginRecording(void *stream, const std::vector<std::string> &histograms,
+                                         const std::vector<std::string> &counters) {
+    if (!lh_record_begin || !lh_record_end || !lh_ingest_f64)
+        throw std::runtime_error("BeginRecording: this libloghisto_b200 has no record scopes");
+    RecordScope s;
+    std::vector<uint32_t> hgen, cgen;
+    for (;;) {
+        bind_names(histos_, histograms, s.hids_, hgen);
+        bind_names(counters_, counters, s.cids_, cgen);
+        check(ctx_, lh_record_begin(ctx_, stream, &s.rec_), "lh_record_begin");
+        if (pin_names(histos_, s.hids_, hgen) && pin_names(counters_, s.cids_, cgen)) break;
+        lh_record_end(ctx_, &s.rec_);   // nothing was enqueued under the stale ids
+    }
+    s.ms_ = this;
+    s.stream_ = stream;
+    s.owner_ = std::this_thread::get_id();
+    std::lock_guard<std::mutex> lk(scope_mu_);
+    scope_threads_[s.owner_]++;
+    return s;
+}
+
+void MetricSystem::end_scope(RecordScope &s) {
+    const lh_status st = lh_record_end(ctx_, &s.rec_);
+    {
+        std::lock_guard<std::mutex> lk(scope_mu_);
+        auto it = scope_threads_.find(s.owner_);
+        if (it != scope_threads_.end() && --it->second == 0) scope_threads_.erase(it);
+    }
+    s.ms_ = nullptr;
+    check(ctx_, st, "lh_record_end");
+}
+
+RecordScope &RecordScope::operator=(RecordScope &&o) noexcept {
+    if (this != &o) {
+        try { End(); } catch (...) {}
+        ms_ = o.ms_; stream_ = o.stream_; owner_ = o.owner_;
+        hids_ = std::move(o.hids_); cids_ = std::move(o.cids_); rec_ = o.rec_;
+        o.ms_ = nullptr;
+    }
+    return *this;
+}
+RecordScope::~RecordScope() {
+    try { End(); } catch (...) {}
+}
+void RecordScope::End() {
+    if (ms_) ms_->end_scope(*this);
+}
+void RecordScope::Histogram(size_t i, const double *d_values, size_t n) {
+    const uint32_t id = hids_.at(i);
+    if (!ms_) throw std::runtime_error("RecordScope::Histogram after End()");
+    if (id == kUnbound) { ms_->dropped_over_limit_.fetch_add(n, std::memory_order_relaxed); return; }
+    check(ms_->ctx_, lh_ingest_f64(ms_->ctx_, id, d_values, n, stream_), "lh_ingest_f64");
+}
+
 void MetricSystem::RegisterGaugeFunc(const std::string &name, std::function<double()> f) {
     std::lock_guard<std::mutex> lk(gauge_mu_);
     gauge_funcs_[name] = std::move(f);
@@ -649,6 +739,11 @@ uint64_t MetricSystem::dropped_samples() {
 
 // collectRawMetrics, metrics.go:420-479.
 std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
+    {   // lh_snapshot_begin would refuse the call after the flush below; refuse it before anything moves
+        std::lock_guard<std::mutex> lk(scope_mu_);
+        if (scope_threads_.count(std::this_thread::get_id()))
+            throw std::runtime_error("collectRawMetrics from a thread that holds an open record scope");
+    }
     std::lock_guard<std::mutex> snap(snapshot_mu_);
     auto raw = std::make_shared<RawMetricSet>();
     const int64_t now = std::chrono::duration_cast<std::chrono::nanoseconds>(
@@ -668,7 +763,13 @@ std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
         asym_barrier();
     }
     for (auto &s : shards_) flush_shard(*s, &touched);
-    check(ctx_, lh_snapshot_begin(ctx_), "lh_snapshot_begin");   // the cache swaps of :425-428 and :460-463
+    for (size_t c = 0; c < carried_touched_.size(); c++) touched[c] |= carried_touched_[c];
+    carried_touched_.clear();
+    if (const lh_status st = lh_snapshot_begin(ctx_); st != LH_OK) {   // the marks stay for the next collection
+        carried_touched_ = std::move(touched);
+        check(ctx_, st, "lh_snapshot_begin");
+    }
+    // the cache swaps of :425-428 and :460-463 happened in lh_snapshot_begin
 
     const uint32_t H = opt_.max_histograms, np = (uint32_t)raw->percentile_labels.size();
     std::vector<double> ps(np);
@@ -957,7 +1058,26 @@ LHMS_API void *lhms_new(int64_t interval_ns, int device, uint32_t max_histograms
         return nullptr;
     }
 }
-LHMS_API void lhms_free(void *ms) { delete static_cast<MetricSystem *>(ms); }
+// as lhms_new, at a bucket precision other than the reference's 100 (Options.precision)
+LHMS_API void *lhms_new_precision(int64_t interval_ns, int device, uint32_t max_histograms, uint32_t max_counters,
+                                  uint32_t precision, char *err, int errlen) {
+    try {
+        Options o;
+        o.device = device;
+        o.max_histograms = max_histograms;
+        o.max_counters = max_counters;
+        o.precision = precision;
+        return new MetricSystem(std::chrono::nanoseconds(interval_ns), false, o);
+    } catch (const std::exception &e) {
+        if (err && errlen > 0) snprintf(err, (size_t)errlen, "%s", e.what());
+        return nullptr;
+    }
+}
+static void end_scopes_of(void *ms);
+LHMS_API void lhms_free(void *ms) {
+    end_scopes_of(ms);   // scopes the caller left open end before their system goes
+    delete static_cast<MetricSystem *>(ms);
+}
 // Nothing may unwind through these C entry points (ctypes / cgo callers): the ingest methods are noexcept, the
 // remaining allocations are guarded.
 LHMS_API void lhms_histogram(void *ms, const char *name, double v) {
@@ -1050,6 +1170,59 @@ LHMS_API int lhms_process_metrics(void *ms, int64_t time_ns, int aggregates,
         if (err && errlen > 0) snprintf(err, (size_t)errlen, "%s", e.what());
         return -1;
     }
+}
+// Record scopes bound to names (MetricSystem::BeginRecording), kept here by (system, lh_recorder.scope).  h_ids /
+// c_ids receive one id per name (0xFFFFFFFF: no free id, records dropped and counted).  Return an lh_status.
+static std::mutex g_scopes_mu;
+static std::map<std::pair<void *, uint64_t>, RecordScope> g_scopes;
+static lh_status scope_status(const std::exception &e) {
+    return dynamic_cast<const std::out_of_range *>(&e) ? LH_ERR_RANGE : LH_ERR_STATE;
+}
+LHMS_API int lhms_record_begin(void *ms, void *stream, uint32_t n_h, const char *const *h_names, uint32_t n_c,
+                               const char *const *c_names, lh_recorder *out, uint32_t *h_ids, uint32_t *c_ids) {
+    if (!ms || !out || (n_h && (!h_names || !h_ids)) || (n_c && (!c_names || !c_ids))) return LH_ERR_INVALID;
+    try {
+        std::vector<std::string> hs(h_names, h_names + n_h), cs(c_names, c_names + n_c);
+        RecordScope s = static_cast<MetricSystem *>(ms)->BeginRecording(stream, hs, cs);
+        *out = s.recorder();
+        for (uint32_t i = 0; i < n_h; i++) h_ids[i] = s.histogram_id(i);
+        for (uint32_t i = 0; i < n_c; i++) c_ids[i] = s.counter_id(i);
+        std::lock_guard<std::mutex> lk(g_scopes_mu);
+        g_scopes.emplace(std::make_pair(ms, out->scope), std::move(s));
+        return LH_OK;
+    } catch (const std::exception &e) {
+        return scope_status(e);
+    }
+}
+static void end_scopes_of(void *ms) {
+    std::vector<RecordScope> left;
+    {
+        std::lock_guard<std::mutex> lk(g_scopes_mu);
+        for (auto it = g_scopes.begin(); it != g_scopes.end();) {
+            if (it->first.first != ms) { ++it; continue; }
+            left.push_back(std::move(it->second));
+            it = g_scopes.erase(it);
+        }
+    }
+}   // `left` ends them
+LHMS_API int lhms_record_end(void *ms, const lh_recorder *rec) {
+    if (!ms || !rec) return LH_ERR_INVALID;
+    RecordScope s;
+    {
+        std::lock_guard<std::mutex> lk(g_scopes_mu);
+        auto it = g_scopes.find(std::make_pair(ms, rec->scope));
+        if (it == g_scopes.end()) return LH_ERR_INVALID;
+        s = std::move(it->second);
+        g_scopes.erase(it);
+    }
+    try { s.End(); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
+}
+LHMS_API int lhms_record_ingest_f64(void *ms, const lh_recorder *rec, uint32_t name_index, const double *d_values, size_t n) {
+    if (!ms || !rec) return LH_ERR_INVALID;
+    std::lock_guard<std::mutex> lk(g_scopes_mu);
+    auto it = g_scopes.find(std::make_pair(ms, rec->scope));
+    if (it == g_scopes.end()) return LH_ERR_INVALID;
+    try { it->second.Histogram(name_index, d_values, n); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
 }
 LHMS_API void lhms_start(void *ms) { static_cast<MetricSystem *>(ms)->Start(); }
 LHMS_API void lhms_stop(void *ms) { static_cast<MetricSystem *>(ms)->Stop(); }

@@ -31,7 +31,7 @@
 #include <unordered_map>
 #include <vector>
 
-struct lh_ctx;
+#include "loghisto_b200.h"
 
 namespace loghisto {
 
@@ -109,6 +109,49 @@ struct TimerToken {
     std::chrono::nanoseconds Stop();   // metrics.go:242-246
 };
 
+// A record scope bound to names (MetricSystem::BeginRecording): the caller's kernels record with lh::record /
+// lh::record_ns / lh::stop / lh::count (include/loghisto_b200_device.cuh) under the ids it hands out, and those ids
+// keep their names until the interval the scope records into has been collected.
+//
+//   loghisto::RecordScope s = ms.BeginRecording(stream, {"rpc_latency", "payload_bytes"}, {"requests"});
+//   kernel<<<g, b, 0, stream>>>(s.recorder(), s.histogram_id(0), s.histogram_id(1), s.counter_id(0));
+//   s.Histogram(0, d_values, n);   // optional: n float64 in device memory under histogram name 0, on the scope's stream
+//   s.End();                       // also on destruction; idempotent
+//
+// Kernels that use the recorder are enqueued on the scope's stream before End().  A name that found no free id is
+// bound to kUnbound: every record under it is dropped on the device and counted in dropped_samples().
+// A scope holds back the collection of its interval until it ends (the reaper's one included), so keep scopes short:
+// open, launch, end.  The thread that opened a scope must end it before it calls collectRawMetrics itself, and every
+// scope must end before the MetricSystem is destroyed.
+class RecordScope {
+ public:
+    static constexpr uint32_t kUnbound = 0xFFFFFFFFu;
+    RecordScope() = default;
+    RecordScope(RecordScope &&o) noexcept { *this = std::move(o); }
+    RecordScope &operator=(RecordScope &&o) noexcept;
+    RecordScope(const RecordScope &) = delete;
+    RecordScope &operator=(const RecordScope &) = delete;
+    ~RecordScope();
+
+    const lh_recorder &recorder() const { return rec_; }
+    uint32_t histogram_id(size_t i) const { return hids_.at(i); }
+    uint32_t counter_id(size_t i) const { return cids_.at(i); }
+    // lh_ingest_f64 of n float64 in device memory under histogram name i, on the scope's stream.  Under an unbound
+    // name the samples are dropped and counted.  Throws std::out_of_range for a bad index, std::runtime_error when the
+    // library refuses the call (e.g. a misaligned pointer) or the scope has ended.
+    void Histogram(size_t i, const double *d_values, size_t n);
+    void End();
+    bool open() const { return ms_ != nullptr; }
+
+ private:
+    friend class MetricSystem;
+    MetricSystem *ms_ = nullptr;
+    void *stream_ = nullptr;
+    std::thread::id owner_;
+    std::vector<uint32_t> hids_, cids_;
+    lh_recorder rec_{};
+};
+
 struct Options {
     int device = 0;
     uint32_t max_histograms = 1024;
@@ -139,6 +182,11 @@ class MetricSystem {
     void *assign_shard(size_t thread_slot, bool *exclusive);             // internal: a thread's staging shard (exclusive while any is free)
     void release_shard(void *shard);                                      // internal: a finished thread hands its exclusive shard back
     void histogram_id(const std::string &name, uint32_t id, uint32_t gen, double value) noexcept;   // body of Histogram once the name is interned
+    // Opens a record scope on `stream` (NULL = the context's ingest stream) with histogram names and counter names bound
+    // to ids for its lifetime (RecordScope).  Throws std::runtime_error only when the library refuses lh_record_begin;
+    // a full name table never makes it fail.
+    RecordScope BeginRecording(void *stream, const std::vector<std::string> &histograms,
+                               const std::vector<std::string> &counters);
     void RegisterGaugeFunc(const std::string &name, std::function<double()> f);   // :299
     void DeregisterGaugeFunc(const std::string &name);                    // :306
     void Start();                                                         // :644
@@ -199,6 +247,14 @@ class MetricSystem {
     void commit_counters(Shard &s) noexcept;
     void flush_shard(Shard &s, std::vector<uint8_t> *touched);
     void reaper();
+    // record scopes (BeginRecording)
+    friend class RecordScope;
+    void bind_names(NameTable &t, const std::vector<std::string> &names, std::vector<uint32_t> &ids, std::vector<uint32_t> &gens);
+    bool pin_names(NameTable &t, const std::vector<uint32_t> &ids, const std::vector<uint32_t> &gens);
+    void end_scope(RecordScope &s);
+    std::mutex scope_mu_;
+    std::unordered_map<std::thread::id, uint32_t> scope_threads_;   // open scopes per opening thread
+    std::vector<uint8_t> carried_touched_;   // touched-counter marks of a collection that lh_snapshot_begin refused
 
     lh_ctx *ctx_ = nullptr;
     std::chrono::nanoseconds interval_;

@@ -5,9 +5,12 @@ happens in the C++ layer and, below it, in the CUDA library; this module only ma
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 
+from . import _lib as _L
 from . import build as _build
+from .engine import _stream
 
 _EMIT = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_char_p, C.c_int, C.c_uint64, C.c_double)
 _lib = None
@@ -28,6 +31,8 @@ def _bind(L):
     vp = C.c_void_p
     L.lhms_new.restype = vp
     L.lhms_new.argtypes = [C.c_int64, C.c_int, C.c_uint32, C.c_uint32, C.c_char_p, C.c_int]
+    L.lhms_new_precision.restype = vp
+    L.lhms_new_precision.argtypes = [C.c_int64, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, C.c_char_p, C.c_int]
     L.lhms_free.argtypes = [vp]
     L.lhms_histogram.argtypes = [vp, C.c_char_p, C.c_double]
     L.lhms_counter.argtypes = [vp, C.c_char_p, C.c_uint64]
@@ -59,6 +64,13 @@ def _bind(L):
     L.lhms_timer_loop.argtypes = [C.c_char_p, C.c_uint, C.c_double, C.c_int64, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_double)]
     L.lhms_print_benchmark.restype = C.c_double
     L.lhms_print_benchmark.argtypes = [C.c_char_p, C.c_uint, C.c_double, C.c_int64, C.c_int, C.c_int]
+    rec, u32p = C.POINTER(_L.lh_recorder), C.POINTER(C.c_uint32)
+    L.lhms_record_begin.restype = C.c_int
+    L.lhms_record_begin.argtypes = [vp, vp, C.c_uint32, names, C.c_uint32, names, rec, u32p, u32p]
+    L.lhms_record_end.restype = C.c_int
+    L.lhms_record_end.argtypes = [vp, rec]
+    L.lhms_record_ingest_f64.restype = C.c_int
+    L.lhms_record_ingest_f64.argtypes = [vp, rec, C.c_uint32, vp, C.c_size_t]
     for kind in ("processed", "raw"):
         getattr(L, "lhms_subscribe_" + kind).restype = vp
         getattr(L, "lhms_subscribe_" + kind).argtypes = [vp, C.c_int]
@@ -113,6 +125,45 @@ class TimerToken:
             pass
 
 
+class RecordScope:
+    """An open record scope of a MetricSystem (MetricSystem.recording).  `recorder` is the lh_recorder to pass by value
+    to kernels enqueued on the scope's stream; `histogram_ids` / `counter_ids` map each bound name to the id those
+    kernels record under (0xFFFFFFFF when the name found no free id: its records are dropped and counted)."""
+    UNBOUND = 0xFFFFFFFF
+
+    def __init__(self, ms, stream, histograms, counters):
+        self._ms = ms
+        self._hnames, cnames = [str(x) for x in histograms], [str(x) for x in counters]
+        self.recorder = _L.lh_recorder()
+        hids = (C.c_uint32 * max(len(self._hnames), 1))()
+        cids = (C.c_uint32 * max(len(cnames), 1))()
+        hn = (C.c_char_p * max(len(self._hnames), 1))(*[x.encode() for x in self._hnames])
+        cn = (C.c_char_p * max(len(cnames), 1))(*[x.encode() for x in cnames])
+        st = ms._lib.lhms_record_begin(ms._h, _stream(stream), len(self._hnames), hn, len(cnames), cn,
+                                       C.byref(self.recorder), hids, cids)
+        if st != 0:
+            raise RuntimeError("lhms_record_begin failed (status %d)" % st)
+        self.histogram_ids = {nm: int(hids[i]) for i, nm in enumerate(self._hnames)}
+        self.counter_ids = {nm: int(cids[i]) for i, nm in enumerate(cnames)}
+        self._open = True
+
+    def histogram(self, name: str, values):
+        """Histogram(name, v) for every element of a contiguous float64 CUDA tensor, on the scope's stream."""
+        if not (values.is_cuda and str(values.dtype) == "torch.float64" and values.is_contiguous()):
+            raise TypeError("values must be a contiguous float64 CUDA tensor")
+        st = self._ms._lib.lhms_record_ingest_f64(self._ms._h, C.byref(self.recorder), self._hnames.index(name),
+                                                  values.data_ptr(), values.numel())
+        if st != 0:
+            raise RuntimeError("lhms_record_ingest_f64 failed (status %d)" % st)
+
+    def end(self):
+        if self._open:
+            self._open = False
+            st = self._ms._lib.lhms_record_end(self._ms._h, C.byref(self.recorder))
+            if st != 0:
+                raise RuntimeError("lhms_record_end failed (status %d)" % st)
+
+
 class Subscription:
     def __init__(self, ms, kind, capacity):
         self._ms, self._kind = ms, kind
@@ -150,8 +201,10 @@ class MetricSystem:
     """NewMetricSystem(interval, sysStats) -- sysStats (Go runtime gauges) is accepted and ignored."""
 
     def __init__(self, interval_s: float, sysStats: bool = False, device: int = 0, max_histograms: int = 1024,
-                 max_counters: int = 1024):
-        """max_histograms / max_counters bound the distinct histogram / counter names used in any three consecutive
+                 max_counters: int = 1024, precision: int = 0):
+        """precision: bucket precision of compress() (0 = the reference's 100).
+
+        max_histograms / max_counters bound the distinct histogram / counter names used in any three consecutive
         intervals: ids of idle names are recycled, a name last used in interval k keeping its id through k+2.  A new
         name that finds no free id has its samples dropped and counted (dropped()).
 
@@ -159,7 +212,11 @@ class MetricSystem:
         equivalent for a non-blocking sender; the reaper never blocks either way, metrics.go:570-573)."""
         self._lib = _load()
         err = C.create_string_buffer(512)
-        self._h = self._lib.lhms_new(max(int(interval_s * 1e9), 1), device, max_histograms, max_counters, err, 512)
+        if precision:
+            self._h = self._lib.lhms_new_precision(max(int(interval_s * 1e9), 1), device, max_histograms, max_counters,
+                                                   precision, err, 512)
+        else:
+            self._h = self._lib.lhms_new(max(int(interval_s * 1e9), 1), device, max_histograms, max_counters, err, 512)
         if not self._h:
             raise RuntimeError(err.value.decode())
 
@@ -192,6 +249,19 @@ class MetricSystem:
 
     def StartTimer(self, name: str) -> TimerToken:
         return TimerToken(self._lib, self._lib.lhms_start_timer(self._h, name.encode()))
+
+    @contextlib.contextmanager
+    def recording(self, stream=None, histograms=(), counters=()):
+        """`with ms.recording(stream, histograms=[...], counters=[...]) as s:` -- a record scope whose names keep their
+        ids until the interval it records into is collected.  Launch kernels that record with s.recorder under
+        s.histogram_ids[name] / s.counter_ids[name] on `stream` (None = the engine's ingest stream, an int handle, or a
+        torch.cuda.Stream) inside the block.  The collection of the interval waits for the block to end, so keep it
+        short; collecting from inside it raises."""
+        scope = RecordScope(self, stream, histograms, counters)
+        try:
+            yield scope
+        finally:
+            scope.end()
 
     def RegisterConstantGauge(self, name: str, value: float):
         self._lib.lhms_register_constant_gauge(self._h, name.encode(), float(value))
