@@ -358,11 +358,15 @@ LH_API int32_t lh_k1_variant_current(lh_ctx *ctx);
 LH_API const char *lh_k1_variant_name(lh_ctx *ctx, int32_t i);
 /* name of the kernel the most recent keyed ingest dispatched to */
 LH_API const char *lh_keyed_kernel_name(lh_ctx *ctx);
-/* time the last `lh_ingest_*` launch range on its stream: CUDA events bracket
- * every ingest kernel; returns the device time of the most recent one in ms */
+/* Ingest timing: two CUDA events on the launch stream bracket the kernels of one sequence number, which is
+ *   - one device-pointer ingest call, lh_ingest_keyed_pair_u16 included whichever kernels it takes;
+ *   - one staging chunk of a host-fed call (lh_*_host); its H2D copy is outside the bracket;
+ *   - one lh_staging_commit_* call.
+ * A call with no samples may take none.
+ * lh_last_kernel_ms = device time of the latest sequence number in ms;
+ * lh_ingest_seq = sequence numbers issued so far (the latest one, 1-based);
+ * lh_kernel_ms = device time of sequence number `seq` (its events stay available for the next 15) */
 LH_API lh_status lh_last_kernel_ms(lh_ctx *ctx, float *ms);
-/* lh_ingest_seq = number of ingest calls issued so far (1-based sequence number of the latest);
- * lh_kernel_ms = device time of ingest call `seq` (its events stay available for the next 15 calls) */
 LH_API uint64_t lh_ingest_seq(lh_ctx *ctx);
 LH_API lh_status lh_kernel_ms(lh_ctx *ctx, uint64_t seq, float *ms);
 

@@ -219,12 +219,12 @@ struct lh_ctx {
     uint32_t *d_rs_flags = nullptr, *d_rs_nnz = nullptr;
     bool rs_dirty = false;                        // a call failed part-way: zero the rows before the next one
     K1Variant k1[kNumK1Variants];
-    // timing of the most recent ingest kernel
-    // CUDA events bracket every ingest launch; a ring keeps the last kTimingRing of them
+    // timing of ingest: CUDA events bracket the kernels of every write_bracket (one sequence number); a ring keeps the
+    // last kTimingRing pairs
     static constexpr int kTimingRing = 16;
     cudaEvent_t ev_t0s[kTimingRing] = {}, ev_t1s[kTimingRing] = {};
-    cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;   // the pair of the launch being issued
-    uint64_t ingest_seq = 0;                         // launches issued so far
+    cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;   // the pair of the bracket being issued
+    uint64_t ingest_seq = 0;                         // brackets opened so far
     bool timing_valid = false;
     // stats
     lh_stats stats{};
@@ -284,13 +284,26 @@ int grid_1d(lh_ctx *ctx, size_t n, int threads, int per_thread, int blocks_per_s
     return (int)std::max<size_t>(1, std::min(need, cap));
 }
 
-// ---- K1 dispatch (locked) ----
-lh_status launch_single(lh_ctx *ctx, uint32_t hid, const double *d_values, size_t n, cudaStream_t s) {
-    if (hid >= ctx->H) return fail(ctx, LH_ERR_RANGE, "histogram_id >= max_histograms");
-    if (((uintptr_t)d_values & 7u) != 0) return fail(ctx, LH_ERR_INVALID, "d_values must be 8-byte aligned");
+// The write protocol of every timed ingest (locked): order `s` after the zeroing of the active buffer, bracket
+// body(b) with the CUDA events of one sequence number, then register `s` as a writer of b, which is what
+// lh_snapshot_begin orders the snapshot after.  The body only issues kernels into buffer b and counts them in stats;
+// when it fails, its status is returned without the end event or the writer registration.
+template <typename Body>
+lh_status write_bracket(lh_ctx *ctx, cudaStream_t s, Body body) {
     const int b = ctx->active;
     lh_status st = before_write(ctx, b, s);
     if (st != LH_OK) return st;
+    next_timing_slot(ctx);
+    LH_CUDA(ctx, cudaEventRecord(ctx->ev_t0, s));
+    st = body(b);
+    if (st != LH_OK) return st;
+    LH_CUDA(ctx, cudaEventRecord(ctx->ev_t1, s));
+    ctx->timing_valid = true;
+    return after_write(ctx, b, s);
+}
+
+// ---- ingest bodies (run inside write_bracket, on validated input) ----
+lh_status launch_single(lh_ctx *ctx, int b, uint32_t hid, const double *d_values, size_t n, cudaStream_t s) {
     unsigned long long *counts = ctx->buf[b].d_buckets + (size_t)hid * 65536u;
     uint32_t *flag = ctx->buf[b].d_flags + hid;
     const K1Variant &kv = ctx->k1[ctx->k1_variant];
@@ -299,8 +312,6 @@ lh_status launch_single(lh_ctx *ctx, uint32_t hid, const double *d_values, size_
     const int grid = std::max(1, ctx->sm_count - ctx->k1_reserve_sms) * kv.blocks_per_sm * ctx->k1_grid_mult;
     const size_t kMaxPerLaunch = std::min((size_t)1 << 36, (size_t)grid << 31);
     size_t done = 0;
-    next_timing_slot(ctx);
-    LH_CUDA(ctx, cudaEventRecord(ctx->ev_t0, s));
     while (done < n) {
         size_t m = std::min(n - done, kMaxPerLaunch);
         const double *p = d_values + done;
@@ -317,10 +328,8 @@ lh_status launch_single(lh_ctx *ctx, uint32_t hid, const double *d_values, size_
         ctx->stats.kernel_launches++;
         done += m;
     }
-    LH_CUDA(ctx, cudaEventRecord(ctx->ev_t1, s));
-    ctx->timing_valid = true;
     ctx->stats.samples += n;
-    return after_write(ctx, b, s);
+    return LH_OK;
 }
 
 lh_status fold_hot(lh_ctx *ctx, int b, cudaStream_t s) {
@@ -340,8 +349,26 @@ KeyedOut keyed_out(lh_ctx *ctx, int b) {
     return o;
 }
 
-// How many histograms' positive windows one pass of k_ingest_keyed_small can privatise.
-uint32_t ks_ids_per_pass(const lh_ctx *ctx) { return std::max<uint32_t>(1, (uint32_t)(KS_SMEM_BYTES / ((size_t)ctx->pc.win * 4))); }
+// The passes of k_ingest_keyed_small over id sub-ranges that cover all H histograms' positive windows.
+uint32_t ks_passes(const lh_ctx *ctx) {
+    const uint32_t per_max = std::max<uint32_t>(1, (uint32_t)(KS_SMEM_BYTES / ((size_t)ctx->pc.win * 4)));
+    return (ctx->H + per_max - 1) / per_max;
+}
+
+// Few histograms: their windows fit in shared memory (K1-style privatisation).  Up to KS_MAX_PASSES passes over id
+// sub-ranges match or beat the L2-atomic kernel (each pass is HBM-bound at 10 B/sample) and, unlike it, do not depend
+// on how clustered the values are.  launch_keyed also wants a vector body of at least 4096 groups of 4.
+constexpr uint32_t KS_MAX_PASSES = 4;
+bool small_route(const lh_ctx *ctx) { return ks_passes(ctx) <= KS_MAX_PASSES && ctx->keyed_mode == 0; }
+
+// The scalar keyed kernel over a ragged piece (a head before the aligned body, a tail after it); nothing when n == 0.
+template <typename IdT, typename ValT>
+void launch_keyed_scalar(lh_ctx *ctx, const KeyedOut &ko, const IdT *ids, const ValT *vals, size_t n, cudaStream_t s) {
+    if (!n) return;
+    constexpr int T = 256;
+    k_ingest_keyed<IdT, ValT, T><<<grid_1d(ctx, n, T, 1, ctx->keyed_blocks_per_sm), T, 0, s>>>(ids, vals, n, ko, ctx->pc);
+    ctx->stats.kernel_launches++;
+}
 
 // Owner-partitioned write-combining kernel: used when the histograms cannot be privatised per CTA in a few
 // passes but P owner CTAs (one per SM) can hold them all, and the batch is big enough to amortise the
@@ -436,21 +463,14 @@ lh_status launch_keyed_wc(lh_ctx *ctx, int b, const IdT *ids, const ValT *vals, 
 }
 
 template <typename IdT, typename ValT>
-lh_status launch_keyed(lh_ctx *ctx, const IdT *d_ids, const ValT *d_vals, size_t n, cudaStream_t s) {
-    if (((uintptr_t)d_vals & 7u) || ((uintptr_t)d_ids & (sizeof(IdT) - 1)))
-        return fail(ctx, LH_ERR_INVALID, "ids / values are not naturally aligned");
-    const int b = ctx->active;
-    lh_status st = before_write(ctx, b, s);
-    if (st != LH_OK) return st;
+lh_status launch_keyed(lh_ctx *ctx, int b, const IdT *d_ids, const ValT *d_vals, size_t n, cudaStream_t s) {
     constexpr int T = 256;
     const KeyedOut ko = keyed_out(ctx, b);
-    next_timing_slot(ctx);
-    LH_CUDA(ctx, cudaEventRecord(ctx->ev_t0, s));
     size_t done = 0;
     while (done < n) {
         // no uint32 cell of the hot window may wrap: drain it before 2^32 samples have gone in
         const unsigned long long kCap = 0xFFFFFFFFull;
-        if (ctx->buf[b].hot_pending >= kCap - (1ull << 30)) { st = fold_hot(ctx, b, s); if (st != LH_OK) return st; }
+        if (ctx->buf[b].hot_pending >= kCap - (1ull << 30)) { lh_status st = fold_hot(ctx, b, s); if (st != LH_OK) return st; }
         size_t m = (size_t)std::min<unsigned long long>(n - done, kCap - ctx->buf[b].hot_pending);
         const IdT *ids = d_ids + done;
         const ValT *vals = d_vals + done;
@@ -460,20 +480,12 @@ lh_status launch_keyed(lh_ctx *ctx, const IdT *d_ids, const ValT *d_vals, size_t
         size_t n4 = vec_ok ? (m - head) / 4 : 0;
         size_t tail_off = head + n4 * 4;
         if (!vec_ok) { head = 0; tail_off = 0; }
-        if (head) {
-            k_ingest_keyed<IdT, ValT, T><<<1, T, 0, s>>>(ids, vals, head, ko, ctx->pc);
-            ctx->stats.kernel_launches++;
-        }
+        launch_keyed_scalar(ctx, ko, ids, vals, head, s);
         size_t hot_used = 0;
         if (n4) {
             bool used = false;
-            // few histograms: their windows fit in shared memory (K1-style privatisation).  Up to KS_MAX_PASSES
-            // passes over id sub-ranges match or beat the L2-atomic kernel (each pass is HBM-bound at 10 B/sample) and,
-            // unlike it, do not depend on how clustered the values are.
-            constexpr uint32_t KS_MAX_PASSES = 4;
-            const uint32_t per_max = ks_ids_per_pass(ctx);
-            const uint32_t passes = (ctx->H + per_max - 1) / per_max;
-            if (passes <= KS_MAX_PASSES && ctx->keyed_mode == 0 && n4 >= 4096) {
+            if (small_route(ctx) && n4 >= 4096) {
+                const uint32_t passes = ks_passes(ctx);
                 const uint32_t per = (ctx->H + passes - 1) / passes;
                 const size_t smem = ((size_t)per * ctx->pc.win + 4) * 4;
                 const void *fn = (const void *)k_ingest_keyed_small<IdT, ValT>;
@@ -492,7 +504,7 @@ lh_status launch_keyed(lh_ctx *ctx, const IdT *d_ids, const ValT *d_vals, size_t
             }
             if (!used && ctx->keyed_mode != 1) {
                 size_t taken = 0;
-                st = launch_keyed_wc<IdT, ValT>(ctx, b, ids + head, vals + head, n4 * 4, s, &used, &taken);
+                lh_status st = launch_keyed_wc<IdT, ValT>(ctx, b, ids + head, vals + head, n4 * 4, s, &used, &taken);
                 if (st != LH_OK) return st;
                 if (used) {
                     ctx->keyed_kernel = "k_ingest_keyed_wc";
@@ -509,79 +521,48 @@ lh_status launch_keyed(lh_ctx *ctx, const IdT *d_ids, const ValT *d_vals, size_t
         } else {
             ctx->keyed_kernel = "k_ingest_keyed";   // no vector body (short or misaligned batch): the scalar kernel only
         }
-        if (tail_off < m) {
-            size_t r = m - tail_off;
-            int grid = grid_1d(ctx, r, T, 1, ctx->keyed_blocks_per_sm);
-            k_ingest_keyed<IdT, ValT, T><<<grid, T, 0, s>>>(ids + tail_off, vals + tail_off, r, ko, ctx->pc);
-            ctx->stats.kernel_launches++;
-        }
+        launch_keyed_scalar(ctx, ko, ids + tail_off, vals + tail_off, m - tail_off, s);
         LH_CUDA(ctx, cudaGetLastError());
         ctx->buf[b].hot_pending += hot_used;     // only k_ingest_keyed_small / _vec count into the uint32 hot window
         done += m;
     }
-    LH_CUDA(ctx, cudaEventRecord(ctx->ev_t1, s));
-    ctx->timing_valid = true;
     ctx->stats.samples += n;
-    return after_write(ctx, b, s);
+    return LH_OK;
 }
 
 // Histogram samples (float64) and Timer samples (int64 ns, metrics.go:242-246) of one batch in ONE launch of the
 // write-combining kernel: its fixed costs (zeroing and flushing the owners' windows, the last partly filled chunk) are
-// paid once.  Needs both arrays vector-aligned and the write-combining kernel eligible; otherwise two keyed ingests.
+// paid once.  Needs both arrays vector-aligned and the write-combining kernel eligible; otherwise launch_keyed for
+// each array in turn.  Either way one body, so one sequence number.
 template <typename IdT>
-lh_status launch_keyed_pair(lh_ctx *ctx, const IdT *ids_f, const double *vals_f, size_t n_f, const IdT *ids_ns, const long long *vals_ns,
-                            size_t n_ns, cudaStream_t s) {
+lh_status launch_keyed_pair(lh_ctx *ctx, int b, const IdT *ids_f, const double *vals_f, size_t n_f, const IdT *ids_ns,
+                            const long long *vals_ns, size_t n_ns, cudaStream_t s) {
     auto aligned = [](const void *v, const void *i) { return (((uintptr_t)v & 31u) == 0) && (((uintptr_t)i & (4 * sizeof(IdT) - 1)) == 0); };
     // few histograms: the shared-memory privatised kernel of launch_keyed() is the better one, per array
-    const uint32_t small_passes = (ctx->H + ks_ids_per_pass(ctx) - 1) / ks_ids_per_pass(ctx);
-    const bool small = small_passes <= 4 && ctx->keyed_mode == 0;
-    const bool fuse = n_f && n_ns && ctx->keyed_mode != 1 && !small && aligned(vals_f, ids_f) && aligned(vals_ns, ids_ns);
+    const bool fuse = n_f && n_ns && ctx->keyed_mode != 1 && !small_route(ctx) && aligned(vals_f, ids_f) && aligned(vals_ns, ids_ns);
     if (fuse) {
-        const int b = ctx->active;
-        lh_status st = before_write(ctx, b, s);
-        if (st != LH_OK) return st;
-        next_timing_slot(ctx);
-        LH_CUDA(ctx, cudaEventRecord(ctx->ev_t0, s));
         bool used = false;
         size_t took_f = 0, took_ns = 0;
-        st = launch_keyed_wc<IdT, double>(ctx, b, ids_f, vals_f, n_f, s, &used, &took_f, ids_ns, vals_ns, n_ns, &took_ns);
+        lh_status st = launch_keyed_wc<IdT, double>(ctx, b, ids_f, vals_f, n_f, s, &used, &took_f, ids_ns, vals_ns, n_ns, &took_ns);
         if (st != LH_OK) return st;
         if (used) {
-            constexpr int T = 256;
             const KeyedOut ko = keyed_out(ctx, b);
             ctx->keyed_kernel = "k_ingest_keyed_wc";
-            if (took_f < n_f) {          // the ragged ends go through the scalar kernel
-                k_ingest_keyed<IdT, double, T><<<grid_1d(ctx, n_f - took_f, T, 1, ctx->keyed_blocks_per_sm), T, 0, s>>>(
-                    ids_f + took_f, vals_f + took_f, n_f - took_f, ko, ctx->pc);
-                ctx->stats.kernel_launches++;
-            }
-            if (took_ns < n_ns) {
-                k_ingest_keyed<IdT, long long, T><<<grid_1d(ctx, n_ns - took_ns, T, 1, ctx->keyed_blocks_per_sm), T, 0, s>>>(
-                    ids_ns + took_ns, vals_ns + took_ns, n_ns - took_ns, ko, ctx->pc);
-                ctx->stats.kernel_launches++;
-            }
+            launch_keyed_scalar(ctx, ko, ids_f + took_f, vals_f + took_f, n_f - took_f, s);   // the ragged ends
+            launch_keyed_scalar(ctx, ko, ids_ns + took_ns, vals_ns + took_ns, n_ns - took_ns, s);
             LH_CUDA(ctx, cudaGetLastError());
-            LH_CUDA(ctx, cudaEventRecord(ctx->ev_t1, s));
-            ctx->timing_valid = true;
             ctx->stats.samples += n_f + n_ns;
-            return after_write(ctx, b, s);
+            return LH_OK;
         }
-        // not eligible after all (few histograms, small batch): the events recorded above are simply overwritten below
-        st = after_write(ctx, b, s);
-        if (st != LH_OK) return st;
+        // declined (too many histograms for the owners' windows, too few SMs, a small batch): one array at a time
     }
-    lh_status st = n_f ? launch_keyed<IdT, double>(ctx, ids_f, vals_f, n_f, s) : LH_OK;
+    lh_status st = launch_keyed<IdT, double>(ctx, b, ids_f, vals_f, n_f, s);
     if (st != LH_OK) return st;
-    return n_ns ? launch_keyed<IdT, long long>(ctx, ids_ns, vals_ns, n_ns, s) : LH_OK;
+    return launch_keyed<IdT, long long>(ctx, b, ids_ns, vals_ns, n_ns, s);
 }
 
 template <typename IdT>
-lh_status launch_counter(lh_ctx *ctx, const IdT *d_ids, const uint64_t *d_amounts, size_t n, cudaStream_t s) {
-    const int b = ctx->active;
-    lh_status st = before_write(ctx, b, s);
-    if (st != LH_OK) return st;
-    next_timing_slot(ctx);
-    LH_CUDA(ctx, cudaEventRecord(ctx->ev_t0, s));
+lh_status launch_counter(lh_ctx *ctx, int b, const IdT *d_ids, const uint64_t *d_amounts, size_t n, cudaStream_t s) {
     if (n) {
         constexpr int T = 512;
         const unsigned long long *amts = reinterpret_cast<const unsigned long long *>(d_amounts);
@@ -615,10 +596,8 @@ lh_status launch_counter(lh_ctx *ctx, const IdT *d_ids, const uint64_t *d_amount
         }
         LH_CUDA(ctx, cudaGetLastError());
     }
-    LH_CUDA(ctx, cudaEventRecord(ctx->ev_t1, s));
-    ctx->timing_valid = true;
     ctx->stats.counter_ops += n;
-    return after_write(ctx, b, s);
+    return LH_OK;
 }
 
 // ---- staging ring (locked) ----
@@ -933,26 +912,37 @@ extern "C" lh_status lh_destroy(lh_ctx *ctx) {
     std::unique_lock<std::mutex> _lk((ctx)->mu);        \
     LH_CUDA((ctx), cudaSetDevice((ctx)->device))
 
+namespace {
+template <typename IdT, typename ValT>
+lh_status ingest_keyed(lh_ctx *ctx, const IdT *d_ids, const ValT *d_vals, size_t n, void *stream) {
+    if (n && (!d_ids || !d_vals)) return fail(ctx, LH_ERR_INVALID, "NULL input");
+    if (((uintptr_t)d_vals & 7u) || ((uintptr_t)d_ids & (sizeof(IdT) - 1)))
+        return fail(ctx, LH_ERR_INVALID, "ids / values are not naturally aligned");
+    cudaStream_t s = pick_stream(ctx, stream);
+    return write_bracket(ctx, s, [&](int b) { return launch_keyed<IdT, ValT>(ctx, b, d_ids, d_vals, n, s); });
+}
+}  // namespace
+
 extern "C" lh_status lh_ingest_f64(lh_ctx *ctx, uint32_t hid, const double *d_values, size_t n, void *stream) {
     LH_ENTER(ctx);
     if (n && !d_values) return fail(ctx, LH_ERR_INVALID, "d_values is NULL");
     if (n == 0) return LH_OK;
-    return launch_single(ctx, hid, d_values, n, pick_stream(ctx, stream));
+    if (hid >= ctx->H) return fail(ctx, LH_ERR_RANGE, "histogram_id >= max_histograms");
+    if (((uintptr_t)d_values & 7u) != 0) return fail(ctx, LH_ERR_INVALID, "d_values must be 8-byte aligned");
+    cudaStream_t s = pick_stream(ctx, stream);
+    return write_bracket(ctx, s, [&](int b) { return launch_single(ctx, b, hid, d_values, n, s); });
 }
 extern "C" lh_status lh_ingest_keyed_f64_u16(lh_ctx *ctx, const uint16_t *d_ids, const double *d_values, size_t n, void *stream) {
     LH_ENTER(ctx);
-    if (n && (!d_ids || !d_values)) return fail(ctx, LH_ERR_INVALID, "NULL input");
-    return launch_keyed<unsigned short, double>(ctx, d_ids, d_values, n, pick_stream(ctx, stream));
+    return ingest_keyed<unsigned short, double>(ctx, d_ids, d_values, n, stream);
 }
 extern "C" lh_status lh_ingest_keyed_f64_u32(lh_ctx *ctx, const uint32_t *d_ids, const double *d_values, size_t n, void *stream) {
     LH_ENTER(ctx);
-    if (n && (!d_ids || !d_values)) return fail(ctx, LH_ERR_INVALID, "NULL input");
-    return launch_keyed<unsigned int, double>(ctx, d_ids, d_values, n, pick_stream(ctx, stream));
+    return ingest_keyed<unsigned int, double>(ctx, d_ids, d_values, n, stream);
 }
 extern "C" lh_status lh_ingest_keyed_i64ns_u16(lh_ctx *ctx, const uint16_t *d_ids, const int64_t *d_nanos, size_t n, void *stream) {
     LH_ENTER(ctx);
-    if (n && (!d_ids || !d_nanos)) return fail(ctx, LH_ERR_INVALID, "NULL input");
-    return launch_keyed<unsigned short, long long>(ctx, d_ids, reinterpret_cast<const long long *>(d_nanos), n, pick_stream(ctx, stream));
+    return ingest_keyed<unsigned short, long long>(ctx, d_ids, reinterpret_cast<const long long *>(d_nanos), n, stream);
 }
 extern "C" lh_status lh_ingest_keyed_pair_u16(lh_ctx *ctx, const uint16_t *d_ids_f64, const double *d_values, size_t n_f64,
                                               const uint16_t *d_ids_ns, const int64_t *d_nanos, size_t n_ns, void *stream) {
@@ -960,18 +950,24 @@ extern "C" lh_status lh_ingest_keyed_pair_u16(lh_ctx *ctx, const uint16_t *d_ids
     if ((n_f64 && (!d_ids_f64 || !d_values)) || (n_ns && (!d_ids_ns || !d_nanos))) return fail(ctx, LH_ERR_INVALID, "NULL input");
     if (((uintptr_t)d_values & 7u) || ((uintptr_t)d_nanos & 7u) || ((uintptr_t)d_ids_f64 & 1u) || ((uintptr_t)d_ids_ns & 1u))
         return fail(ctx, LH_ERR_INVALID, "ids / values are not naturally aligned");
-    return launch_keyed_pair<unsigned short>(ctx, d_ids_f64, d_values, n_f64, d_ids_ns, reinterpret_cast<const long long *>(d_nanos), n_ns,
-                                             pick_stream(ctx, stream));
+    if (n_f64 == 0 && n_ns == 0) return LH_OK;
+    cudaStream_t s = pick_stream(ctx, stream);
+    const long long *nanos = reinterpret_cast<const long long *>(d_nanos);
+    return write_bracket(ctx, s, [&](int b) {
+        return launch_keyed_pair<unsigned short>(ctx, b, d_ids_f64, d_values, n_f64, d_ids_ns, nanos, n_ns, s);
+    });
 }
 extern "C" lh_status lh_counter_add_u16(lh_ctx *ctx, const uint16_t *d_ids, const uint64_t *d_amounts, size_t n, void *stream) {
     LH_ENTER(ctx);
     if (n && (!d_ids || !d_amounts)) return fail(ctx, LH_ERR_INVALID, "NULL input");
-    return launch_counter<unsigned short>(ctx, d_ids, d_amounts, n, pick_stream(ctx, stream));
+    cudaStream_t s = pick_stream(ctx, stream);
+    return write_bracket(ctx, s, [&](int b) { return launch_counter<unsigned short>(ctx, b, d_ids, d_amounts, n, s); });
 }
 extern "C" lh_status lh_counter_add_u32(lh_ctx *ctx, const uint32_t *d_ids, const uint64_t *d_amounts, size_t n, void *stream) {
     LH_ENTER(ctx);
     if (n && (!d_ids || !d_amounts)) return fail(ctx, LH_ERR_INVALID, "NULL input");
-    return launch_counter<unsigned int>(ctx, d_ids, d_amounts, n, pick_stream(ctx, stream));
+    cudaStream_t s = pick_stream(ctx, stream);
+    return write_bracket(ctx, s, [&](int b) { return launch_counter<unsigned int>(ctx, b, d_ids, d_amounts, n, s); });
 }
 
 // =========================================================== ingest (host)
@@ -980,6 +976,41 @@ extern "C" lh_status lh_counter_add_u32(lh_ctx *ctx, const uint32_t *d_ids, cons
 namespace {
 enum HostKind { HK_SINGLE, HK_KEYED_U16, HK_COUNTER_U16, HK_KEYED_I64_U16 };
 
+// One staging step: copy n 8-byte items from h_a and, unless kind is HK_SINGLE, n uint16 ids from h_ids (to byte
+// ids_off) into the device buffer of slot `sl`, then ingest them in one write bracket.  The copies run on their own
+// stream so that chunk k+1's DMA overlaps chunk k's kernel; the bracket opens after the ingest stream has waited for
+// them, so the kernel time excludes the copy.  Unless a copy fails, the slot is in flight afterwards.
+lh_status staging_step(lh_ctx *ctx, Slot &sl, HostKind kind, uint32_t hid, const void *h_a, const void *h_ids, size_t n,
+                       size_t ids_off) {
+    cudaStream_t cs = ctx->copy_stream, s = ctx->ingest_stream;
+    lh_status st = LH_OK;
+    if (n) {
+        char *d_a = (char *)sl.d;
+        const unsigned short *d_i = (const unsigned short *)(d_a + ids_off);
+        // the device buffer is free again once the kernel that read it last is done (slot_wait_free already waited
+        // on the host for a recycled slot, the event wait covers the rest)
+        if (sl.seq) LH_CUDA(ctx, cudaStreamWaitEvent(cs, sl.done, 0));
+        LH_CUDA(ctx, cudaMemcpyAsync(d_a, h_a, n * 8, cudaMemcpyHostToDevice, cs));
+        if (kind != HK_SINGLE) LH_CUDA(ctx, cudaMemcpyAsync(d_a + ids_off, h_ids, n * 2, cudaMemcpyHostToDevice, cs));
+        LH_CUDA(ctx, cudaEventRecord(sl.copied, cs));
+        LH_CUDA(ctx, cudaStreamWaitEvent(s, sl.copied, 0));
+        ctx->stats.h2d_bytes += n * (kind == HK_SINGLE ? 8 : 10);
+        st = write_bracket(ctx, s, [&](int b) {
+            switch (kind) {
+            case HK_SINGLE: return launch_single(ctx, b, hid, (const double *)d_a, n, s);
+            case HK_KEYED_U16: return launch_keyed<unsigned short, double>(ctx, b, d_i, (const double *)d_a, n, s);
+            case HK_KEYED_I64_U16: return launch_keyed<unsigned short, long long>(ctx, b, d_i, (const long long *)d_a, n, s);
+            default: return launch_counter<unsigned short>(ctx, b, d_i, (const uint64_t *)d_a, n, s);   // HK_COUNTER_U16
+            }
+        });
+    }
+    LH_CUDA(ctx, cudaEventRecord(sl.done, s));
+    sl.state = SLOT_INFLIGHT;
+    sl.seq = ++ctx->slot_seq;
+    ctx->slot_cv.notify_all();
+    return st;
+}
+
 lh_status ingest_host(lh_ctx *ctx, std::unique_lock<std::mutex> &lk, HostKind kind, uint32_t hid,
                       const void *h_a /* 8-byte items */, const uint16_t *h_ids, size_t n) {
     const bool pinned = is_pinned_or_managed(h_a) && (!h_ids || is_pinned_or_managed(h_ids));
@@ -987,7 +1018,6 @@ lh_status ingest_host(lh_ctx *ctx, std::unique_lock<std::mutex> &lk, HostKind ki
     size_t per = ctx->staging_bytes / item;
     per &= ~(size_t)15;   // keeps the ids region 16-byte aligned
     if (per == 0) return fail(ctx, LH_ERR_INVALID, "staging_bytes too small");
-    cudaStream_t s = ctx->ingest_stream;
     size_t done = 0;
     cudaEvent_t last_copied = nullptr;
     while (done < n) {
@@ -996,42 +1026,22 @@ lh_status ingest_host(lh_ctx *ctx, std::unique_lock<std::mutex> &lk, HostKind ki
         lh_status st = slot_wait_free(ctx, lk, &si);
         if (st != LH_OK) return st;
         Slot &sl = ctx->slots[si];
-        const char *src_a = (const char *)h_a + done * 8;
-        char *d_a = (char *)sl.d;
-        char *d_i = (char *)sl.d + per * 8;
-        const void *cp_a = src_a;
-        const void *cp_i = h_ids ? (const void *)(h_ids + done) : nullptr;
+        const void *src_a = (const char *)h_a + done * 8;
+        const void *src_i = h_ids ? (const void *)(h_ids + done) : nullptr;
         if (!pinned) {
             // pageable source: stage through the slot's pinned buffer.  The memcpy (milliseconds per 32 MiB) runs with
-            // the context mutex RELEASED -- the slot is parked as ACQUIRED so no other thread can take it.
+            // the context mutex RELEASED -- the slot is parked as SLOT_FILLING so no other thread can take it.
             sl.state = SLOT_FILLING;
             lk.unlock();
             memcpy(sl.h, src_a, m * 8);
-            if (h_ids) memcpy((char *)sl.h + per * 8, h_ids + done, m * 2);
+            if (h_ids) memcpy((char *)sl.h + per * 8, src_i, m * 2);
             lk.lock();
-            cp_a = sl.h;
-            cp_i = (char *)sl.h + per * 8;
+            src_a = sl.h;
+            src_i = (char *)sl.h + per * 8;
         }
-        // copies run on their own stream so that chunk k+1's DMA overlaps chunk k's kernel; the slot's device
-        // buffer is free again once the kernel that read it last is done (slot_wait_free already waited on the host
-        // for a recycled slot, the event wait covers the rest)
-        cudaStream_t cs = ctx->copy_stream;
-        if (sl.seq) LH_CUDA(ctx, cudaStreamWaitEvent(cs, sl.done, 0));
-        LH_CUDA(ctx, cudaMemcpyAsync(d_a, cp_a, m * 8, cudaMemcpyHostToDevice, cs));
-        if (h_ids) LH_CUDA(ctx, cudaMemcpyAsync(d_i, cp_i, m * 2, cudaMemcpyHostToDevice, cs));
-        LH_CUDA(ctx, cudaEventRecord(sl.copied, cs));
-        LH_CUDA(ctx, cudaStreamWaitEvent(s, sl.copied, 0));
+        st = staging_step(ctx, sl, kind, hid, src_a, src_i, m, per * 8);
+        if (st != LH_OK) return st;
         last_copied = sl.copied;
-        ctx->stats.h2d_bytes += m * item;
-        if (kind == HK_SINGLE) st = launch_single(ctx, hid, (const double *)d_a, m, s);
-        else if (kind == HK_KEYED_U16) st = launch_keyed<unsigned short, double>(ctx, (const unsigned short *)d_i, (const double *)d_a, m, s);
-        else if (kind == HK_KEYED_I64_U16) st = launch_keyed<unsigned short, long long>(ctx, (const unsigned short *)d_i, (const long long *)d_a, m, s);
-        else st = launch_counter<unsigned short>(ctx, (const unsigned short *)d_i, (const uint64_t *)d_a, m, s);
-        if (st != LH_OK) { sl.state = SLOT_FREE; return st; }
-        LH_CUDA(ctx, cudaEventRecord(sl.done, s));
-        sl.state = SLOT_INFLIGHT;
-        sl.seq = ++ctx->slot_seq;
-        ctx->slot_cv.notify_all();
         done += m;
     }
     if (pinned && last_copied) {
@@ -1124,28 +1134,7 @@ lh_status staging_commit(lh_ctx *ctx, const lh_staging *sg, HostKind kind, uint3
         if ((ids_offset & 15u) || ids_offset < item_bytes || ids_offset + n * 2 > ctx->staging_bytes)
             return fail(ctx, LH_ERR_RANGE, "ids_offset / n do not fit the staging slot");
     }
-    cudaStream_t s = ctx->ingest_stream;
-    lh_status st = LH_OK;
-    if (n) {
-        cudaStream_t cs = ctx->copy_stream;
-        if (sl.seq) LH_CUDA(ctx, cudaStreamWaitEvent(cs, sl.done, 0));
-        LH_CUDA(ctx, cudaMemcpyAsync(sl.d, sl.h, item_bytes, cudaMemcpyHostToDevice, cs));
-        ctx->stats.h2d_bytes += item_bytes;
-        if (kind != HK_SINGLE) {
-            LH_CUDA(ctx, cudaMemcpyAsync((char *)sl.d + ids_offset, (char *)sl.h + ids_offset, n * 2, cudaMemcpyHostToDevice, cs));
-            ctx->stats.h2d_bytes += n * 2;
-        }
-        LH_CUDA(ctx, cudaEventRecord(sl.copied, cs));
-        LH_CUDA(ctx, cudaStreamWaitEvent(s, sl.copied, 0));
-        if (kind == HK_SINGLE) st = launch_single(ctx, hid, (const double *)sl.d, n, s);
-        else if (kind == HK_KEYED_U16) st = launch_keyed<unsigned short, double>(ctx, (const unsigned short *)((char *)sl.d + ids_offset), (const double *)sl.d, n, s);
-        else st = launch_counter<unsigned short>(ctx, (const unsigned short *)((char *)sl.d + ids_offset), (const uint64_t *)sl.d, n, s);
-    }
-    LH_CUDA(ctx, cudaEventRecord(sl.done, s));
-    sl.state = SLOT_INFLIGHT;
-    sl.seq = ++ctx->slot_seq;
-    ctx->slot_cv.notify_all();
-    return st;
+    return staging_step(ctx, sl, kind, hid, sl.h, (char *)sl.h + ids_offset, n, ids_offset);
 }
 }  // namespace
 
