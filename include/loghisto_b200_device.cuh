@@ -8,6 +8,7 @@
 //   lh::start_timer(id) / lh::stop(rec, token)
 //                                 StartTimer(name) / Stop()   metrics.go:232-246  durations on the GPU's clock
 //   lh::BlockHistogram            one CTA feeding one histogram through a shared-memory sub-histogram
+//   lh::BlockRecorder             one CTA feeding any number of histograms through a shared-memory combining table
 //
 // `rec` is an lh_recorder (include/loghisto_b200.h) obtained from lh_record_begin on the host and passed to the kernel
 // by value.  Kernels that use it must be enqueued on the recorder's stream between lh_record_begin and lh_record_end;
@@ -230,11 +231,10 @@ __device__ __forceinline__ uint32_t lane_id() {
     return l;
 }
 
-// Histogram(name, v): one sample of histogram `id`.  Callable from any thread under any divergence.  The lanes of a
-// warp that arrive together are combined: lanes with the same (id, bucket) elect one leader, which adds their number
-// with one 64-bit atomic.  An id >= max_histograms is dropped and counted in lh_stats.dropped.
-__device__ __forceinline__ void record(const lh_recorder &rec, uint32_t id, double v) {
-    const uint32_t key = key16_of(v, recorder_prec(rec));
+// One sample of histogram `id` whose (uint16)key is already known: the body of record() after the bucket function.
+// The lanes of a warp that arrive together are combined: lanes with the same (id, key) elect one leader, which adds
+// their number with one 64-bit atomic.  An id >= max_histograms is dropped and counted in lh_stats.dropped.
+__device__ __forceinline__ void record_key16(const lh_recorder &rec, uint32_t id, uint32_t key) {
     const bool ok = id < rec.max_histograms;
     const unsigned long long tag = ok ? ((unsigned long long)id << 16) | key : ~0ull;   // every dropped lane combines
     const uint32_t active = __activemask();
@@ -243,6 +243,12 @@ __device__ __forceinline__ void record(const lh_recorder &rec, uint32_t id, doub
     const unsigned long long c = (unsigned long long)__popc(peers);
     if (!ok) { atomicAdd(recorder_dropped(rec), c); return; }
     add_bucket_global(recorder_row(rec, id), rec.d_flags + id, key, c, recorder_prec(rec).win);
+}
+
+// Histogram(name, v): one sample of histogram `id`.  Callable from any thread under any divergence; lanes of a warp
+// with the same (id, bucket) are combined as record_key16 describes.
+__device__ __forceinline__ void record(const lh_recorder &rec, uint32_t id, double v) {
+    record_key16(rec, id, key16_of(v, recorder_prec(rec)));
 }
 
 // TimerToken.Stop(): the value is float64(duration.Nanoseconds()), round-to-nearest-even as Go's CVTSQ2SD.
@@ -291,6 +297,11 @@ __device__ __forceinline__ void count(const lh_recorder &rec, uint32_t id, uint6
     atomicAdd(reinterpret_cast<unsigned long long *>(rec.d_counters) + id, (unsigned long long)amount);
 }
 
+__device__ __forceinline__ uint32_t block_thread_rank() {
+    return threadIdx.x + blockDim.x * (threadIdx.y + blockDim.y * threadIdx.z);
+}
+__device__ __forceinline__ uint32_t block_thread_count() { return blockDim.x * blockDim.y * blockDim.z; }
+
 // One CTA feeding one histogram: samples are counted in a uint32 sub-histogram in shared memory (the arithmetic of
 // the library's single-histogram kernel) and flushed into the histogram's row with one 64-bit atomic per non-empty
 // bucket.  The caller provides rec.block_smem_bytes of shared memory (usually the kernel's dynamic shared memory).
@@ -315,7 +326,7 @@ class BlockHistogram {
         row_ = ok_ ? recorder_row(rec_, id) : nullptr;
         flag_ = ok_ ? rec_.d_flags + id : nullptr;
         const uint32_t words = subhist_words(recorder_prec(rec_).win);
-        for (uint32_t i = thread_rank(); i < words; i += block_threads()) hist_[i] = 0;
+        for (uint32_t i = block_thread_rank(); i < words; i += block_thread_count()) hist_[i] = 0;
         __syncthreads();
     }
 
@@ -336,23 +347,121 @@ class BlockHistogram {
     __device__ __forceinline__ void flush() {
         const uint32_t win = recorder_prec(rec_).win;
         __syncthreads();
-        if (ok_) flush_subhist(hist_, (int)thread_rank(), (int)block_threads(), row_, flag_, win);
+        if (ok_) flush_subhist(hist_, (int)block_thread_rank(), (int)block_thread_count(), row_, flag_, win);
         else __syncthreads();
-        for (uint32_t i = thread_rank(); i < 2u * win; i += block_threads()) hist_[i] = 0;
+        for (uint32_t i = block_thread_rank(); i < 2u * win; i += block_thread_count()) hist_[i] = 0;
         __syncthreads();
     }
 
   private:
-    __device__ __forceinline__ static uint32_t thread_rank() {
-        return threadIdx.x + blockDim.x * (threadIdx.y + blockDim.y * threadIdx.z);
-    }
-    __device__ __forceinline__ static uint32_t block_threads() { return blockDim.x * blockDim.y * blockDim.z; }
-
     const lh_recorder &rec_;
     uint32_t *hist_;
     unsigned long long *row_ = nullptr;
     uint32_t *flag_ = nullptr;
     bool ok_ = false;
+};
+
+// Any number of histograms from one CTA: a write-combining table in shared memory, keyed by the exact (id, bucket) of
+// each sample and flushed into the interval's rows with one 64-bit atomic per occupied slot.  Where the CTA's distinct
+// (id, bucket) pairs fit the table, a sample costs shared-memory atomics only (lh::record costs one global atomic per
+// distinct (id, bucket) per warp call).  The caller provides BlockRecorder::smem_bytes(entries) bytes of shared memory,
+// 8-byte aligned (usually the kernel's dynamic shared memory).
+//
+//   extern __shared__ __align__(16) unsigned char smem[];
+//   lh::BlockRecorder br(rec, smem, entries);
+//   br.init();                        // every thread of the CTA
+//   ... br.record(id, v) ...          // Histogram(name, v): any thread, any id, any divergence
+//   ... br.record_ns(id, ns) ...      // TimerToken.Stop(): float64(ns), as lh::record_ns
+//   ... ns = br.stop(token) ...       // lh::stop through the table; returns the duration
+//   br.flush();                       // every thread of the CTA; the table is empty afterwards and takes more records
+//
+// Table: `entries` rounded down to a power of two slots (no table below kMinEntries: every sample takes the direct
+// path), each a 64-bit tag ((id << 16 | key) + 1; 0 = empty) and a uint32 count, 12 B per slot, tags first.  A sample
+// probes at most kProbes consecutive slots from a multiplicative hash of its tag: a slot holding its tag is a hit, an
+// empty one is claimed with one 64-bit shared CAS (which may find the same tag, claimed by another lane: a hit too),
+// and a hit adds 1 to the slot's count.  A sample that finds neither goes straight into the row (record_key16, the
+// path of lh::record).  So every sample lands on key16_of(v) of its id however full the table is; only the speed
+// depends on it.  An id >= max_histograms is dropped and counted in lh_stats.dropped as by lh::record, and never
+// enters the table.
+//
+// Contract: at most 2^32 - 1 records per CTA between two flushes (the counts are uint32).  The table lives only as long
+// as the CTA: records after its last flush are lost, so every CTA ends with flush().  Above 48 KB of dynamic shared
+// memory the kernel needs cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes), as for
+// BlockHistogram.
+class BlockRecorder {
+  public:
+    static constexpr uint32_t kMinEntries = 32;
+    static constexpr uint32_t kProbes = 8;      // slots a sample probes before it takes the direct path
+
+    // Slots of a table asked for `entries`: the largest power of two <= entries, or 0 below kMinEntries.
+    __host__ __device__ static constexpr uint32_t table_entries(uint32_t entries) {
+        if (entries < kMinEntries) return 0;
+        uint32_t p = kMinEntries;
+        while (p <= entries / 2) p *= 2;
+        return p;
+    }
+    // Shared memory for a table asked for `entries` (a table that fits a CTA has at most 2^14 slots).
+    __host__ __device__ static constexpr uint32_t smem_bytes(uint32_t entries) { return 12u * table_entries(entries); }
+
+    __device__ __forceinline__ BlockRecorder(const lh_recorder &rec, void *smem, uint32_t entries)
+        : rec_(rec), n_(table_entries(entries)), tags_(reinterpret_cast<unsigned long long *>(smem)),
+          counts_(reinterpret_cast<uint32_t *>(tags_ + n_)) {}
+
+    // Empties the table.
+    __device__ __forceinline__ void init() {
+        for (uint32_t i = block_thread_rank(); i < n_; i += block_thread_count()) { tags_[i] = 0ull; counts_[i] = 0u; }
+        __syncthreads();
+    }
+
+    __device__ __forceinline__ void record(uint32_t id, double v) {
+        const uint32_t key = key16_of(v, recorder_prec(rec_));
+        if (id < rec_.max_histograms && insert((((unsigned long long)id << 16) | key) + 1ull)) return;
+        record_key16(rec_, id, key);
+    }
+
+    __device__ __forceinline__ void record_ns(uint32_t id, long long ns) { record(id, __ll2double_rn(ns)); }
+
+    __device__ __forceinline__ long long stop(const TimerToken &t) {
+        const long long ns = (long long)(globaltimer_ns() - t.start_ns);
+        record_ns(t.id, ns);
+        return ns;
+    }
+
+    // Adds every occupied slot's count into its row (raising the histogram's flag as every writer does) and empties
+    // the table for the next records.
+    __device__ __forceinline__ void flush() {
+        const uint32_t win = recorder_prec(rec_).win;
+        __syncthreads();
+        for (uint32_t i = block_thread_rank(); i < n_; i += block_thread_count()) {
+            const unsigned long long t = tags_[i];
+            if (t) {
+                const uint32_t id = (uint32_t)((t - 1ull) >> 16);
+                add_bucket_global(recorder_row(rec_, id), rec_.d_flags + id, (uint32_t)(t - 1ull) & 0xFFFFu, counts_[i], win);
+                tags_[i] = 0ull;
+                counts_[i] = 0u;
+            }
+        }
+        __syncthreads();
+    }
+
+  private:
+    // true when the sample was counted in the table
+    __device__ __forceinline__ bool insert(unsigned long long tag) {
+        if (n_ == 0) return false;
+        uint32_t s = (uint32_t)((tag * 0x9E3779B97F4A7C15ull) >> 32);
+        for (uint32_t p = 0; p < kProbes; ++p, ++s) {
+            const uint32_t i = s & (n_ - 1u);
+            unsigned long long t = *reinterpret_cast<volatile unsigned long long *>(&tags_[i]);
+            if (t == 0ull) t = atomicCAS(&tags_[i], 0ull, tag);
+            if (t == 0ull || t == tag) { atomicAdd(&counts_[i], 1u); return true; }
+        }
+        return false;
+    }
+
+    const lh_recorder &rec_;
+    uint32_t n_;
+    unsigned long long *tags_;
+    uint32_t *counts_;
 };
 
 }  // namespace lh

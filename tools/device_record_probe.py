@@ -1,11 +1,13 @@
 """Records per second of the device record API (include/loghisto_b200_device.cuh) next to the materialised path.
 
-For streams U and L and H = 1 and 1024 histograms, on the same n samples:
+For streams U and L and H = 1, 16 and 1024 histograms, on the same n samples:
   materialised  lh_gen_stream_f64 (+ lh_gen_ids_u16 at H > 1) writes the samples to HBM, then lh_ingest_f64 (H = 1) or
                 lh_ingest_keyed_f64_u16 reads them back; reported for the ingest alone and with the materialising write
   record        lh::record from the client kernel of tests/device_record_client.cu, one call per sample
   block         lh::BlockHistogram from the same client, one histogram per CTA (65536 samples per CTA)
-The client kernels read their values (8 B) and ids (4 B, record at H > 1; per-CTA for block) from HBM, so their rates
+  block_rec     lh::BlockRecorder from tests/block_recorder_client.cu: a 4096-entry table, 65536 samples per CTA, one
+                flush at the end
+The client kernels read their values (8 B) and ids (4 B, record and block_rec at H > 1; per-CTA for block) from HBM, so their rates
 are those of a producer that has its samples in memory already; one that computes them in registers skips that read.
 Every time is CUDA events on the recording / ingest stream, median of --reps after one warm-up.  Prints the card and
 its power limit, then one JSON line per configuration.
@@ -27,6 +29,7 @@ import loghisto_b200 as lh  # noqa: E402
 from loghisto_b200 import _lib, build  # noqa: E402
 
 CHUNK = 65536
+TABLE_ENTRIES = 4096
 
 
 def card():
@@ -42,7 +45,10 @@ def client():
     lib.lhc_record.argtypes = [rp, vp, vp, sz, vp]
     lib.lhc_block.argtypes = [rp, vp, vp, sz, sz, vp]
     lib.lhc_record.restype = lib.lhc_block.restype = C.c_int
-    return lib
+    br = C.CDLL(build.BLOCK_CLIENT_LIB)
+    br.brc_record.argtypes = [rp, vp, vp, sz, sz, C.c_uint32, C.c_int, vp]
+    br.brc_record.restype = C.c_int
+    return lib, br
 
 
 def timed(stream, fn, reps):
@@ -67,9 +73,9 @@ def main():
     n = a.n
     name, power = card()
     print(json.dumps({"card": name, "power_limit": power, "n": n}), flush=True)
-    cl = client()
+    cl, br = client()
     torch.cuda.init()
-    for H in (1, 1024):
+    for H in (1, 16, 1024):
         with lh.Engine(device=0, max_histograms=H, max_counters=1) as eng:
             stream = torch.cuda.ExternalStream(eng.ingest_stream)
             s = eng.ingest_stream
@@ -102,8 +108,14 @@ def main():
                     with eng.recording(s) as rec:
                         assert cl.lhc_block(C.byref(rec), d_blk.ptr, d_v.ptr, n, CHUNK, s) == 0
 
+                def block_rec():
+                    with eng.recording(s) as rec:
+                        assert br.brc_record(C.byref(rec), d_i32.ptr if d_i32 else None, d_v.ptr, n, CHUNK, TABLE_ENTRIES,
+                                             0, s) == 0
+
                 res = {}
-                for label, fn in (("gen", gen), ("ingest", ingest), ("record", record), ("block", block)):
+                for label, fn in (("gen", gen), ("ingest", ingest), ("record", record), ("block", block),
+                                  ("block_rec", block_rec)):
                     res[label] = timed(stream, fn, a.reps)
                     eng.snapshot([], export=False)      # keep every interval small; not timed
                 out = {"stream": sname, "H": H, "n": n, "card": name, "power_limit": power,
@@ -112,7 +124,8 @@ def main():
                            "ingest_only": n / res["ingest"] * 1e3,
                            "gen_plus_ingest": n / (res["gen"] + res["ingest"]) * 1e3,
                            "record": n / res["record"] * 1e3,
-                           "block_histogram": n / res["block"] * 1e3}}
+                           "block_histogram": n / res["block"] * 1e3,
+                           "block_recorder": n / res["block_rec"] * 1e3}}
                 print(json.dumps(out), flush=True)
 
 
