@@ -186,6 +186,37 @@ typedef struct lh_recorder {          /* passed by value to kernels; valid only 
 LH_API lh_status lh_record_begin(lh_ctx *ctx, void *stream, lh_recorder *out);
 LH_API lh_status lh_record_end(lh_ctx *ctx, const lh_recorder *rec);
 
+/* ---- GPU timers: StartTimer / Stop (metrics.go:232-246) from host code, timed on the device ------------------
+ * Host StartTimer / Stop around CUDA work time the enqueue.  These calls put the two ends of the span on the GPU
+ * instead: each end is a one-thread kernel on `stream` that reads %globaltimer (the clock of lh::start_timer), and
+ * the duration is recorded on the device; it never crosses to the host.  A span includes the launch latency of its
+ * two marks.  `stream` NULL = the context's ingest stream, as everywhere.
+ *
+ *   lh_gpu_timer_start    takes a free slot of the context's pool of 64-bit start marks (allocated on first use;
+ *                         65536 slots, or lh_tune(ctx, "gpu_timer_slots", n) before the first start), enqueues the
+ *                         mark on `stream` and records the slot's start event.  Never blocks.  LH_ERR_RANGE when
+ *                         every slot is held or still in use by kernels that have not completed.
+ *   lh_gpu_timer_stop     an ingest call of one sample: float64(now - start) into histogram `histogram_id` of the
+ *                         active interval, inside one write bracket (one sequence number, one lh_stats.samples), so a
+ *                         stop issued after lh_snapshot_begin lands in the next interval.  If d_duration_ns is not
+ *                         NULL (device memory) the kernel also writes the duration there.  When `stream` is not the
+ *                         start's stream, `stream` first waits for the start's mark, so the stop never reads an
+ *                         unwritten slot; ordering after the WORK on the start's stream stays the caller's job.  A
+ *                         token may be stopped any number of times (one sample each, from the same start).
+ *                         LH_ERR_RANGE for histogram_id >= max_histograms.
+ *   lh_gpu_timer_release  gives the slot back.  It is handed out again only after every kernel that read or wrote it
+ *                         has completed (events on each stream that touched it), so releasing before the GPU has run
+ *                         a stop never changes that stop's duration.
+ *
+ * A handle carries its slot, a generation and its context: a released, stale or foreign handle gets LH_ERR_INVALID
+ * and touches no slot.  Start and stop on a stream in CUDA-graph capture return LH_ERR_STATE and enqueue nothing
+ * (graph replay is not supported).  lh_destroy frees the pool whatever tokens are outstanding. */
+typedef struct lh_gpu_timer { uint64_t handle; } lh_gpu_timer;   /* opaque */
+LH_API lh_status lh_gpu_timer_start(lh_ctx *ctx, void *stream, lh_gpu_timer *out);
+LH_API lh_status lh_gpu_timer_stop(lh_ctx *ctx, const lh_gpu_timer *t, uint32_t histogram_id, void *stream,
+                                   int64_t *d_duration_ns);
+LH_API lh_status lh_gpu_timer_release(lh_ctx *ctx, const lh_gpu_timer *t);
+
 /* ---- snapshot = collectRawMetrics' cache swap (metrics.go:425-428, 460-463)
  *
  * lh_snapshot_begin   freezes the active bucket/counter arrays and makes the
@@ -351,7 +382,8 @@ LH_API lh_status lh_memcpy_d2h(lh_ctx *ctx, void *h_dst, const void *d_src, size
  * kernel, 2 owner-partitioned write-combining kernel whatever the batch size), and that kernel's knobs: "kp_chunk"
  * (samples per chunk, default 256 M), "wc_spt" (tile shape code: 6 = 896 threads x 4 samples (default), 4 = 1024 x 4,
  * 3 = 768 x 4, 8 = 512 x 8), "wc_flush" (samples a CTA bins between two flushes of its owner buffers, default 24576),
- * "wc_pf" (L2 prefetch distance of its input in tiles, default 1, 0 = off) */
+ * "wc_pf" (L2 prefetch distance of its input in tiles, default 1, 0 = off), "gpu_timer_slots" (size of the GPU
+ * timer pool, 1 ... 2^20, default 65536; LH_ERR_STATE once the pool exists) */
 LH_API lh_status lh_tune(lh_ctx *ctx, const char *key, int64_t value);
 LH_API int32_t lh_k1_variant_count(void);
 LH_API int32_t lh_k1_variant_current(lh_ctx *ctx);
@@ -361,7 +393,8 @@ LH_API const char *lh_keyed_kernel_name(lh_ctx *ctx);
 /* Ingest timing: two CUDA events on the launch stream bracket the kernels of one sequence number, which is
  *   - one device-pointer ingest call, lh_ingest_keyed_pair_u16 included whichever kernels it takes;
  *   - one staging chunk of a host-fed call (lh_*_host); its H2D copy is outside the bracket;
- *   - one lh_staging_commit_* call.
+ *   - one lh_staging_commit_* call;
+ *   - one lh_gpu_timer_stop.
  * A call with no samples may take none.
  * lh_last_kernel_ms = device time of the latest sequence number in ms;
  * lh_ingest_seq = sequence numbers issued so far (the latest one, 1-based);

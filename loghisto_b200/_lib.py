@@ -79,6 +79,11 @@ class lh_recorder(C.Structure):
     ]
 
 
+class lh_gpu_timer(C.Structure):
+    """Opaque handle of a GPU timer (lh_gpu_timer_start)."""
+    _fields_ = [("handle", C.c_uint64)]
+
+
 _vp, _sz, _u32, _u64, _i32 = C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint64, C.c_int32
 
 # name -> (restype, argtypes); every symbol include/loghisto_b200.h declares
@@ -107,6 +112,9 @@ SIGNATURES = {
     "lh_staging_abandon": (_i32, [_vp, C.POINTER(lh_staging)]),
     "lh_record_begin": (_i32, [_vp, _vp, C.POINTER(lh_recorder)]),
     "lh_record_end": (_i32, [_vp, C.POINTER(lh_recorder)]),
+    "lh_gpu_timer_start": (_i32, [_vp, _vp, C.POINTER(lh_gpu_timer)]),
+    "lh_gpu_timer_stop": (_i32, [_vp, C.POINTER(lh_gpu_timer), _u32, _vp, _vp]),
+    "lh_gpu_timer_release": (_i32, [_vp, C.POINTER(lh_gpu_timer)]),
     "lh_snapshot_begin": (_i32, [_vp]),
     "lh_snapshot_device": (_i32, [_vp, C.POINTER(lh_device_view)]),
     "lh_snapshot_reduce": (_i32, [_vp, _vp, _u32, _vp, _vp, _vp, _vp, _vp]),

@@ -29,6 +29,16 @@ struct Scope { uint64_t ticket; int buf; cudaStream_t stream; std::thread::id th
 static_assert(sizeof(Prec) == sizeof(((lh_recorder *)0)->prec) && offsetof(lh_recorder, prec) % alignof(Prec) == 0,
               "lh_recorder.prec must hold an lh::Prec");
 
+// one slot of the GPU timer pool (lh_gpu_timer_*)
+enum TimerState : uint8_t { TIMER_FRESH = 0 /* never handed out */, TIMER_HELD = 1, TIMER_RELEASED = 2 };
+struct TimerSlot {
+    uint32_t gen = 0;                  // bumped at every release: handles of earlier tokens stop matching
+    uint8_t state = TIMER_FRESH;
+    cudaStream_t start_stream = nullptr;
+    cudaEvent_t started = nullptr;     // after the mark (created on the slot's first use, kept)
+    std::vector<WriterEvent> stops;    // after the latest stop on each stream that stopped the token
+};
+
 struct Buffer {
     unsigned long long *d_buckets = nullptr;   // [H][65536]
     unsigned long long *d_counters = nullptr;  // [C]
@@ -226,6 +236,13 @@ struct lh_ctx {
     cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;   // the pair of the bracket being issued
     uint64_t ingest_seq = 0;                         // brackets opened so far
     bool timing_valid = false;
+    // GPU timers: a pool of 64-bit start marks on the device (allocated by the first lh_gpu_timer_start)
+    uint32_t timer_slots_n = 65536;
+    unsigned long long *d_timer_marks = nullptr;
+    std::vector<TimerSlot> timer_slots;
+    std::vector<uint32_t> timer_released;            // released slots, oldest first, reused once their kernels are done
+    uint32_t timer_fresh = 0;                         // slots [timer_fresh, n) have never been handed out
+    std::vector<cudaEvent_t> timer_spare_events;      // stop events of recycled slots
     // stats
     lh_stats stats{};
     std::mutex mu;
@@ -898,6 +915,12 @@ extern "C" lh_status lh_destroy(lh_ctx *ctx) {
         if (ctx->ev_t0s[i]) cudaEventDestroy(ctx->ev_t0s[i]);
         if (ctx->ev_t1s[i]) cudaEventDestroy(ctx->ev_t1s[i]);
     }
+    cudaFree(ctx->d_timer_marks);   // whatever tokens are still held
+    for (auto &ts : ctx->timer_slots) {
+        if (ts.started) cudaEventDestroy(ts.started);
+        for (auto &w : ts.stops) cudaEventDestroy(w.ev);
+    }
+    for (cudaEvent_t ev : ctx->timer_spare_events) cudaEventDestroy(ev);
     if (ctx->ingest_stream) cudaStreamDestroy(ctx->ingest_stream);
     if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
     if (ctx->snap_stream) cudaStreamDestroy(ctx->snap_stream);
@@ -1193,6 +1216,139 @@ extern "C" lh_status lh_record_end(lh_ctx *ctx, const lh_recorder *rec) {
         return after_write(ctx, sc.buf, sc.stream);
     }
     return fail(ctx, LH_ERR_INVALID, "unknown or already ended record scope");
+}
+
+// =========================================================== GPU timers
+namespace {
+// handle = context tag (16 bits) | generation (28 bits) | slot (20 bits)
+constexpr int kTimerSlotBits = 20, kTimerGenBits = 28;
+
+uint64_t timer_handle(const lh_ctx *ctx, uint32_t slot, uint32_t gen) {
+    const uint64_t tag = ctx->ctx_id % 0xFFFFu + 1u;   // 1 ... 65535, so no handle is 0
+    return tag << (kTimerSlotBits + kTimerGenBits) | (uint64_t)(gen & ((1u << kTimerGenBits) - 1u)) << kTimerSlotBits | slot;
+}
+
+// the held slot a handle names, or nullptr for a released, stale, foreign or malformed handle
+TimerSlot *timer_slot(lh_ctx *ctx, const lh_gpu_timer *t) {
+    if (!t) return nullptr;
+    const uint32_t k = (uint32_t)(t->handle & ((1u << kTimerSlotBits) - 1u));
+    if (k >= ctx->timer_slots.size()) return nullptr;
+    TimerSlot &ts = ctx->timer_slots[k];
+    if (ts.state != TIMER_HELD || t->handle != timer_handle(ctx, k, ts.gen)) return nullptr;
+    return &ts;
+}
+
+// A mark enqueued during capture would run only at replay, against a slot that may belong to another token by then.
+lh_status refuse_capture(lh_ctx *ctx, cudaStream_t s) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    LH_CUDA(ctx, cudaStreamIsCapturing(s, &cs));
+    if (cs != cudaStreamCaptureStatusNone) return fail(ctx, LH_ERR_STATE, "GPU timers cannot be captured into a CUDA graph");
+    return LH_OK;
+}
+
+// every kernel that read or wrote the slot has completed (queried, never waited for)
+bool timer_slot_idle(const TimerSlot &ts) {
+    bool idle = cudaEventQuery(ts.started) == cudaSuccess;
+    for (const auto &w : ts.stops) idle = idle && cudaEventQuery(w.ev) == cudaSuccess;
+    cudaGetLastError();   // cudaErrorNotReady is not an error
+    return idle;
+}
+
+// A slot for a new token: the oldest released slot if its kernels are done, else a fresh one, else any released slot
+// whose kernels are done.
+lh_status timer_take(lh_ctx *ctx, uint32_t *out) {
+    if (!ctx->d_timer_marks) {
+        LH_CUDA(ctx, cudaMalloc(&ctx->d_timer_marks, (size_t)ctx->timer_slots_n * sizeof(unsigned long long)));
+        ctx->timer_slots.resize(ctx->timer_slots_n);
+    }
+    const bool fresh = ctx->timer_fresh < ctx->timer_slots_n;
+    const size_t scan = fresh ? std::min<size_t>(1, ctx->timer_released.size()) : ctx->timer_released.size();
+    for (size_t i = 0; i < scan; i++) {
+        const uint32_t k = ctx->timer_released[i];
+        TimerSlot &ts = ctx->timer_slots[k];
+        if (!timer_slot_idle(ts)) continue;
+        ctx->timer_released.erase(ctx->timer_released.begin() + (long)i);
+        for (auto &w : ts.stops) ctx->timer_spare_events.push_back(w.ev);
+        ts.stops.clear();
+        *out = k;
+        return LH_OK;
+    }
+    if (fresh) { *out = ctx->timer_fresh++; return LH_OK; }
+    return fail(ctx, LH_ERR_RANGE, "every GPU timer slot is held or still in use on the device");
+}
+}  // namespace
+
+extern "C" lh_status lh_gpu_timer_start(lh_ctx *ctx, void *stream, lh_gpu_timer *out) {
+    LH_ENTER(ctx);
+    if (!out) return fail(ctx, LH_ERR_INVALID, "out is NULL");
+    cudaStream_t s = pick_stream(ctx, stream);
+    lh_status st = refuse_capture(ctx, s);
+    if (st != LH_OK) return st;
+    uint32_t k = 0;
+    st = timer_take(ctx, &k);
+    if (st != LH_OK) return st;
+    TimerSlot &ts = ctx->timer_slots[k];
+    cudaError_t e = ts.started ? cudaSuccess : cudaEventCreateWithFlags(&ts.started, cudaEventDisableTiming);
+    if (e == cudaSuccess) {
+        k_gpu_timer_mark<<<1, 1, 0, s>>>(ctx->d_timer_marks + k);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaEventRecord(ts.started, s);
+    if (e != cudaSuccess) {   // back to the pool, behind whatever may have been enqueued
+        ts.state = TIMER_RELEASED;
+        ctx->timer_released.push_back(k);
+        return fail(ctx, LH_ERR_CUDA, "lh_gpu_timer_start", e);
+    }
+    ctx->stats.kernel_launches++;
+    ts.state = TIMER_HELD;
+    ts.start_stream = s;
+    out->handle = timer_handle(ctx, k, ts.gen);
+    return LH_OK;
+}
+
+extern "C" lh_status lh_gpu_timer_stop(lh_ctx *ctx, const lh_gpu_timer *t, uint32_t hid, void *stream, int64_t *d_out) {
+    LH_ENTER(ctx);
+    cudaStream_t s = pick_stream(ctx, stream);
+    lh_status st = refuse_capture(ctx, s);
+    if (st != LH_OK) return st;
+    if (hid >= ctx->H) return fail(ctx, LH_ERR_RANGE, "histogram_id >= max_histograms");
+    TimerSlot *ts = timer_slot(ctx, t);
+    if (!ts) return fail(ctx, LH_ERR_INVALID, "released, stale or foreign GPU timer handle");
+    if (((uintptr_t)d_out & 7u) != 0) return fail(ctx, LH_ERR_INVALID, "d_duration_ns must be 8-byte aligned");
+    if (s != ts->start_stream) LH_CUDA(ctx, cudaStreamWaitEvent(s, ts->started, 0));
+    const unsigned long long *mark = ctx->d_timer_marks + (ts - ctx->timer_slots.data());
+    st = write_bracket(ctx, s, [&](int b) -> lh_status {
+        k_gpu_timer_stop<<<1, 1, 0, s>>>(mark, ctx->buf[b].d_buckets + (size_t)hid * 65536u, ctx->buf[b].d_flags + hid,
+                                         reinterpret_cast<long long *>(d_out), ctx->pc);
+        LH_CUDA(ctx, cudaGetLastError());
+        ctx->stats.kernel_launches++;
+        ctx->stats.samples++;
+        return LH_OK;
+    });
+    if (st != LH_OK) return st;
+    // the slot is not handed out again before this stop has run (one event per stream that stopped the token)
+    for (auto &w : ts->stops)
+        if (w.stream == s) { LH_CUDA(ctx, cudaEventRecord(w.ev, s)); return LH_OK; }
+    WriterEvent w{s, nullptr};
+    if (!ctx->timer_spare_events.empty()) {
+        w.ev = ctx->timer_spare_events.back();
+        ctx->timer_spare_events.pop_back();
+    } else {
+        LH_CUDA(ctx, cudaEventCreateWithFlags(&w.ev, cudaEventDisableTiming));
+    }
+    ts->stops.push_back(w);
+    LH_CUDA(ctx, cudaEventRecord(w.ev, s));
+    return LH_OK;
+}
+
+extern "C" lh_status lh_gpu_timer_release(lh_ctx *ctx, const lh_gpu_timer *t) {
+    LH_ENTER(ctx);
+    TimerSlot *ts = timer_slot(ctx, t);
+    if (!ts) return fail(ctx, LH_ERR_INVALID, "released, stale or foreign GPU timer handle");
+    ts->state = TIMER_RELEASED;
+    ts->gen++;
+    ctx->timer_released.push_back((uint32_t)(ts - ctx->timer_slots.data()));
+    return LH_OK;
 }
 
 // =========================================================== snapshot
@@ -1908,6 +2064,12 @@ extern "C" lh_status lh_tune(lh_ctx *ctx, const char *key, int64_t value) {
     if (!strcmp(key, "kp_chunk")) {
         if (value < (1 << 16) || value > ((int64_t)1 << 28)) return fail(ctx, LH_ERR_RANGE, "kp_chunk out of range");
         ctx->kp_chunk = value;
+        return LH_OK;
+    }
+    if (!strcmp(key, "gpu_timer_slots")) {
+        if (value < 1 || value > (1 << 20)) return fail(ctx, LH_ERR_RANGE, "gpu_timer_slots is 1 ... 2^20");
+        if (ctx->d_timer_marks) return fail(ctx, LH_ERR_STATE, "gpu_timer_slots is set before the first lh_gpu_timer_start");
+        ctx->timer_slots_n = (uint32_t)value;
         return LH_OK;
     }
     if (!strcmp(key, "keyed_blocks_per_sm")) {

@@ -1649,6 +1649,19 @@ k_peer_allreduce(PeerParams p) {
     }
 }
 
+// ----------------------------------------------------------- GPU timers (lh_gpu_timer_*)
+// One thread each: their cost is the launch, not the body.  The start writes %globaltimer into the token's slot; the
+// stop records float64(now - start) into one histogram row through the same bucket function and row writer every
+// device caller uses (what lh::record_ns does, without the warp combining a single thread cannot use).
+__global__ void k_gpu_timer_mark(unsigned long long *__restrict__ slot) { *slot = globaltimer_ns(); }
+
+__global__ void k_gpu_timer_stop(const unsigned long long *__restrict__ slot, unsigned long long *__restrict__ row,
+                                 uint32_t *flag, long long *out, Prec pc) {
+    const long long ns = (long long)(globaltimer_ns() - *slot);
+    add_bucket_global(row, flag, key16_of(__ll2double_rn(ns), pc), 1ull, pc.win);
+    if (out) *out = ns;
+}
+
 // ----------------------------------------------------------- probes / tables
 __global__ void k_fill_decompress(double *__restrict__ table, double precision) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;

@@ -49,6 +49,19 @@ def _stream(s) -> int:
     raise TypeError(f"not a stream: {type(s)!r}")
 
 
+CUDA_STREAM_LEGACY = 1   # cudaStreamLegacy
+
+
+def _timer_stream(s) -> int:
+    """_stream for the GPU timers.  torch's default stream has cuda_stream == 0, which the C ABI reads as the context's
+    ingest stream; a timer given that stream object must time torch's default stream, so it gets cudaStreamLegacy.
+    None and plain ints keep their ABI meaning (None / 0 = the ingest stream)."""
+    h = _stream(s)
+    if h == 0 and s is not None and not isinstance(s, int):
+        return CUDA_STREAM_LEGACY
+    return h
+
+
 class DeviceArray:
     """Device memory owned through lh_device_alloc; exposes __cuda_array_interface__."""
 
@@ -349,6 +362,21 @@ class Engine:
             yield rec
         finally:
             self.record_end(rec)
+
+    # ---- GPU timers (StartTimer / Stop with both ends on the device)
+    def gpu_timer_start(self, stream=None) -> L.lh_gpu_timer:
+        """Enqueue a start mark on `stream` (None = the ingest stream; torch's default stream is timed as itself)."""
+        t = L.lh_gpu_timer()
+        self._check(self.lib.lh_gpu_timer_start(self.h, _timer_stream(stream), C.byref(t)))
+        return t
+
+    def gpu_timer_stop(self, t: L.lh_gpu_timer, histogram_id: int, stream=None, d_out=None):
+        """Record float64(now - start) into `histogram_id` on the device; with `d_out` (8 bytes of device memory) the
+        kernel also writes the int64 duration there.  A token may be stopped any number of times."""
+        self._check(self.lib.lh_gpu_timer_stop(self.h, C.byref(t), histogram_id, _timer_stream(stream), _ptr(d_out)))
+
+    def gpu_timer_release(self, t: L.lh_gpu_timer):
+        self._check(self.lib.lh_gpu_timer_release(self.h, C.byref(t)))
 
     # ---- snapshot
     def snapshot_begin(self):

@@ -23,6 +23,10 @@
 #pragma weak lh_record_begin
 #pragma weak lh_record_end
 #pragma weak lh_ingest_f64
+// And for GPU timers: over a build without them, StartGpuTimer hands out tokens whose Stop drops and counts.
+#pragma weak lh_gpu_timer_start
+#pragma weak lh_gpu_timer_stop
+#pragma weak lh_gpu_timer_release
 
 namespace loghisto {
 
@@ -708,6 +712,49 @@ void RecordScope::Histogram(size_t i, const double *d_values, size_t n) {
     check(ms_->ctx_, lh_ingest_f64(ms_->ctx_, id, d_values, n, stream_), "lh_ingest_f64");
 }
 
+// ---- GPU timers ------------------------------------------------------------------------------------------------
+void *const GpuTimerToken::kStartStream = reinterpret_cast<void *>(~(uintptr_t)0);
+
+GpuTimerToken MetricSystem::StartGpuTimer(const std::string &name, void *stream) {
+    GpuTimerToken t;
+    t.ms_ = this;
+    t.name_ = name;
+    t.stream_ = stream;
+    if (!lh_gpu_timer_start || !lh_gpu_timer_stop || !lh_gpu_timer_release) return t;
+    const lh_status st = lh_gpu_timer_start(ctx_, stream, &t.t_);
+    if (st == LH_ERR_RANGE) return t;   // every slot is in use: as StartTimer, this does not fail; Stop drops and counts
+    check(ctx_, st, "lh_gpu_timer_start");
+    t.held_ = true;
+    return t;
+}
+
+// The name is bound at stop time through a record scope on the stop's stream, so the id the sample lands on keeps
+// the name until the interval is collected (see bind_names), however long the token was held.
+void GpuTimerToken::Stop(void *stream, int64_t *d_duration_ns) {
+    if (!ms_) throw std::runtime_error("GpuTimerToken::Stop on an empty token");
+    if (stream == kStartStream) stream = stream_;
+    if (!held_) { ms_->dropped_over_limit_.fetch_add(1, std::memory_order_relaxed); return; }
+    RecordScope s = ms_->BeginRecording(stream, {name_}, {});
+    const uint32_t id = s.histogram_id(0);
+    if (id == RecordScope::kUnbound) { ms_->dropped_over_limit_.fetch_add(1, std::memory_order_relaxed); return; }
+    const lh_status st = lh_gpu_timer_stop(ms_->ctx_, &t_, id, stream, d_duration_ns);
+    s.End();
+    check(ms_->ctx_, st, "lh_gpu_timer_stop");
+}
+
+GpuTimerToken &GpuTimerToken::operator=(GpuTimerToken &&o) noexcept {
+    if (this != &o) {
+        if (held_ && ms_) lh_gpu_timer_release(ms_->ctx_, &t_);
+        ms_ = o.ms_; name_ = std::move(o.name_); stream_ = o.stream_; t_ = o.t_; held_ = o.held_;
+        o.ms_ = nullptr;
+        o.held_ = false;
+    }
+    return *this;
+}
+GpuTimerToken::~GpuTimerToken() {
+    if (held_ && ms_) lh_gpu_timer_release(ms_->ctx_, &t_);
+}
+
 void MetricSystem::RegisterGaugeFunc(const std::string &name, std::function<double()> f) {
     std::lock_guard<std::mutex> lk(gauge_mu_);
     gauge_funcs_[name] = std::move(f);
@@ -1224,6 +1271,24 @@ LHMS_API int lhms_record_ingest_f64(void *ms, const lh_recorder *rec, uint32_t n
     if (it == g_scopes.end()) return LH_ERR_INVALID;
     try { it->second.Histogram(name_index, d_values, n); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
 }
+// GPU timers (MetricSystem::StartGpuTimer).  start returns a token, or NULL with *status set; stop may be called
+// repeatedly on `stream` (passed as given: NULL = the context's ingest stream); free releases the token's slot.
+LHMS_API void *lhms_gpu_timer_start(void *ms, const char *name, void *stream, int *status) {
+    if (!ms || !name || !status) { if (status) *status = LH_ERR_INVALID; return nullptr; }
+    try {
+        auto *t = new GpuTimerToken(static_cast<MetricSystem *>(ms)->StartGpuTimer(name, stream));
+        *status = LH_OK;
+        return t;
+    } catch (const std::exception &e) {
+        *status = scope_status(e);
+        return nullptr;
+    }
+}
+LHMS_API int lhms_gpu_timer_stop(void *token, void *stream, int64_t *d_duration_ns) {
+    if (!token) return LH_ERR_INVALID;
+    try { static_cast<GpuTimerToken *>(token)->Stop(stream, d_duration_ns); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
+}
+LHMS_API void lhms_gpu_timer_free(void *token) { delete static_cast<GpuTimerToken *>(token); }
 LHMS_API void lhms_start(void *ms) { static_cast<MetricSystem *>(ms)->Start(); }
 LHMS_API void lhms_stop(void *ms) { static_cast<MetricSystem *>(ms)->Stop(); }
 LHMS_API uint64_t lhms_dropped(void *ms) { return static_cast<MetricSystem *>(ms)->dropped_samples(); }

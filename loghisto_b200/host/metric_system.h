@@ -152,6 +152,44 @@ class RecordScope {
     lh_recorder rec_{};
 };
 
+// StartTimer / Stop with both ends on the GPU (MetricSystem::StartGpuTimer): the start and every Stop are stream-ordered
+// marks on the device's %globaltimer, and the duration is recorded on the device under the name; nothing synchronises
+// with the host.  Use it around CUDA work, where a host timer would measure only the enqueue.
+//
+//   loghisto::GpuTimerToken t = ms.StartGpuTimer("decode_step", stream);
+//   decode<<<g, b, 0, stream>>>(...);
+//   t.Stop();                          // on the start's stream; t.Stop(other, d_ns) elsewhere and/or with the duration
+//
+// Stop binds the name at stop time (BeginRecording), so the sample lands in the interval that is open when Stop is
+// called, under the name, however long the token was held.  Like Go's Stop it may be called repeatedly, one sample each
+// from the same start.  A name that finds no free id, and every Stop of a token that got no pool slot (the pool of the
+// context is exhausted), drop the sample and count it in dropped_samples().  Move-only; the slot goes back to the pool
+// on destruction (it is reused only after the token's kernels have run).
+class GpuTimerToken {
+ public:
+    static void *const kStartStream;   // Stop's default: the stream the token was started on
+    GpuTimerToken() = default;
+    GpuTimerToken(GpuTimerToken &&o) noexcept { *this = std::move(o); }
+    GpuTimerToken &operator=(GpuTimerToken &&o) noexcept;
+    GpuTimerToken(const GpuTimerToken &) = delete;
+    GpuTimerToken &operator=(const GpuTimerToken &) = delete;
+    ~GpuTimerToken();
+
+    // Records the duration on the device.  d_duration_ns (device memory, 8-byte aligned, nullable) also receives it as
+    // int64.  Throws std::runtime_error when the library refuses the call (e.g. a misaligned d_duration_ns).  GPU
+    // timers do not time work captured into CUDA graphs.
+    void Stop(void *stream = kStartStream, int64_t *d_duration_ns = nullptr);
+    bool has_slot() const { return held_; }
+
+ private:
+    friend class MetricSystem;
+    MetricSystem *ms_ = nullptr;
+    std::string name_;
+    void *stream_ = nullptr;
+    lh_gpu_timer t_{};
+    bool held_ = false;
+};
+
 struct Options {
     int device = 0;
     uint32_t max_histograms = 1024;
@@ -175,6 +213,10 @@ class MetricSystem {
     void SubscribeToProcessedMetrics(std::shared_ptr<Channel<std::shared_ptr<ProcessedMetricSet>>> ch);   // :218
     void UnsubscribeFromProcessedMetrics(std::shared_ptr<Channel<std::shared_ptr<ProcessedMetricSet>>> ch);
     TimerToken StartTimer(const std::string &name);                       // :232
+    // StartTimer timed on the GPU: enqueues the start mark on `stream` (NULL = the context's ingest stream).  Never
+    // fails for want of a pool slot (see GpuTimerToken); throws std::runtime_error when the library refuses the call
+    // (e.g. a stream in CUDA-graph capture).
+    GpuTimerToken StartGpuTimer(const std::string &name, void *stream);
     // Ingest never throws and never fails the caller (problems are logged, samples dropped and counted).
     void Counter(const std::string &name, uint64_t amount) noexcept;      // :251
     void Histogram(const std::string &name, double value) noexcept;       // :273
@@ -249,6 +291,7 @@ class MetricSystem {
     void reaper();
     // record scopes (BeginRecording)
     friend class RecordScope;
+    friend class GpuTimerToken;
     void bind_names(NameTable &t, const std::vector<std::string> &names, std::vector<uint32_t> &ids, std::vector<uint32_t> &gens);
     bool pin_names(NameTable &t, const std::vector<uint32_t> &ids, const std::vector<uint32_t> &gens);
     void end_scope(RecordScope &s);

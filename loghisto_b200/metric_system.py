@@ -10,7 +10,7 @@ import ctypes as C
 
 from . import _lib as _L
 from . import build as _build
-from .engine import _stream
+from .engine import _stream, _timer_stream
 
 _EMIT = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_char_p, C.c_int, C.c_uint64, C.c_double)
 _lib = None
@@ -71,6 +71,11 @@ def _bind(L):
     L.lhms_record_end.argtypes = [vp, rec]
     L.lhms_record_ingest_f64.restype = C.c_int
     L.lhms_record_ingest_f64.argtypes = [vp, rec, C.c_uint32, vp, C.c_size_t]
+    L.lhms_gpu_timer_start.restype = vp
+    L.lhms_gpu_timer_start.argtypes = [vp, C.c_char_p, vp, C.POINTER(C.c_int)]
+    L.lhms_gpu_timer_stop.restype = C.c_int
+    L.lhms_gpu_timer_stop.argtypes = [vp, vp, vp]
+    L.lhms_gpu_timer_free.argtypes = [vp]
     for kind in ("processed", "raw"):
         getattr(L, "lhms_subscribe_" + kind).restype = vp
         getattr(L, "lhms_subscribe_" + kind).argtypes = [vp, C.c_int]
@@ -121,6 +126,41 @@ class TimerToken:
             if self._h is not None:      # never stopped: release the C++ token
                 self._lib.lhms_timer_free(self._h)
                 self._h = None
+        except Exception:
+            pass
+
+
+class GpuTimerToken:
+    """A timer whose start and stop are marks on the GPU's clock (MetricSystem.StartGpuTimer)."""
+
+    def __init__(self, ms, handle, stream: int):
+        self._ms, self._h, self._stream = ms, handle, stream
+
+    def Stop(self, stream=None, out=None):
+        """Records the duration on the device under the token's name; nothing is returned to the host.  `stream`:
+        None = the stream the timer was started on, else an int handle or a torch.cuda.Stream.  `out`: an optional
+        contiguous int64 CUDA tensor whose first element receives the duration in ns.  Consumed by the first call, as
+        TimerToken: later calls do nothing."""
+        if self._h is None:
+            return
+        ptr = 0
+        if out is not None:
+            if not (out.is_cuda and str(out.dtype) == "torch.int64" and out.is_contiguous() and out.numel() >= 1):
+                raise TypeError("out must be a contiguous int64 CUDA tensor")
+            ptr = out.data_ptr()
+        st = self._ms._lib.lhms_gpu_timer_stop(self._h, self._stream if stream is None else _timer_stream(stream), ptr)
+        self._free()
+        if st != 0:
+            raise RuntimeError("lhms_gpu_timer_stop failed (status %d)" % st)
+
+    def _free(self):
+        if self._h is not None and self._ms._h:   # a closed MetricSystem already freed the pool
+            self._ms._lib.lhms_gpu_timer_free(self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self._free()
         except Exception:
             pass
 
@@ -249,6 +289,28 @@ class MetricSystem:
 
     def StartTimer(self, name: str) -> TimerToken:
         return TimerToken(self._lib, self._lib.lhms_start_timer(self._h, name.encode()))
+
+    def StartGpuTimer(self, name: str, stream=None) -> GpuTimerToken:
+        """StartTimer for stream work: the start is a mark on the GPU's clock enqueued on `stream` (None = the
+        engine's ingest stream, an int handle, or a torch.cuda.Stream; torch's default stream is timed as itself), and
+        Stop() records the span on the device.  Does not fail when the timer pool is exhausted: that token's Stop
+        drops the sample and counts it in dropped()."""
+        h = _timer_stream(stream)
+        st = C.c_int()
+        tok = self._lib.lhms_gpu_timer_start(self._h, name.encode(), h, C.byref(st))
+        if not tok:
+            raise RuntimeError("lhms_gpu_timer_start failed (status %d)" % st.value)
+        return GpuTimerToken(self, tok, h)
+
+    @contextlib.contextmanager
+    def gpu_timer(self, name: str, stream=None):
+        """`with ms.gpu_timer(name, stream):` -- StartGpuTimer before the block, Stop() on the same stream after it:
+        records the GPU time of the stream work enqueued in between, plus the launch latency of the two marks."""
+        t = self.StartGpuTimer(name, stream)
+        try:
+            yield t
+        finally:
+            t.Stop()
 
     @contextlib.contextmanager
     def recording(self, stream=None, histograms=(), counters=()):
