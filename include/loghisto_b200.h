@@ -15,7 +15,9 @@
  *   - every function returns an lh_status (0 = LH_OK, negative = error); nothing
  *     throws, nothing calls back into the caller;
  *   - all functions are thread-safe; ingest may run concurrently with a
- *     snapshot (double-buffered bucket arrays);
+ *     snapshot (double-buffered bucket arrays), and may be issued from any
+ *     number of streams and of contexts on one device (launches of the
+ *     write-combining keyed kernel on a device are serialised);
  *   - `stream` arguments are a cudaStream_t passed as void* (NULL = the
  *     context's own ingest stream); device pointers are plain pointers;
  *   - names never cross the boundary: the caller interns name -> dense id.

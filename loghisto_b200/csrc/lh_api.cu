@@ -391,6 +391,25 @@ void launch_keyed_scalar(lh_ctx *ctx, const KeyedOut &ko, const IdT *ids, const 
 // passes but P owner CTAs (one per SM) can hold them all, and the batch is big enough to amortise the
 // cooperative launch.
 constexpr size_t kSmemBudget = 227 * 1024;
+
+// Every write-combining launch on a device is ordered after the previous one, whatever its stream or context.  A
+// context's scratch (record sub-queues, grid-barrier word) is shared by all the streams it ingests from, and a launch
+// zeroes the barrier word on its own stream: two launches in flight together could clear it under a running grid and
+// mix their records.  Ordering across contexts as well means no two cooperative grids are ever outstanding at once.
+// A grid holds one CTA on every SM it uses, so two of them never ran side by side anyway.
+std::mutex g_wc_mu;                      // guards g_wc_done; held from the wait through the record of each launch
+std::vector<cudaEvent_t> g_wc_done;      // [device]: after the device's last write-combining launch
+
+// the device's completion event (created on first use; lives as long as the process); call with g_wc_mu held
+cudaError_t wc_done_event(int device, cudaEvent_t *out) {
+    if ((size_t)device >= g_wc_done.size()) g_wc_done.resize((size_t)device + 1, nullptr);
+    if (!g_wc_done[device]) {
+        cudaError_t e = cudaEventCreateWithFlags(&g_wc_done[device], cudaEventDisableTiming);
+        if (e != cudaSuccess) { g_wc_done[device] = nullptr; return e; }
+    }
+    *out = g_wc_done[device];
+    return cudaSuccess;
+}
 // Processes the first *taken samples (whole tiles only); the caller sends the rest to the scalar kernel.
 // Optional second segment (ids2, vals2, n2): int64 nanosecond samples binned by the SAME launch (ValT = double only).
 template <typename IdT, typename ValT, int SPT>
@@ -428,6 +447,15 @@ lh_status launch_keyed_wc_spt(lh_ctx *ctx, int b, const IdT *ids, const ValT *va
     const size_t expect = slice_max * S::TILE / P;       // sized for the nominal slice: the allocation does not follow the batch size
     const size_t cap = ((expect * 5 / 4 + 3 * WC_LINE + WC_LINE - 1) / WC_LINE) * WC_LINE;
     if (!ctx->d_kp_queues || ctx->kp_cap != cap || ctx->kp_parts != P) {
+        if (ctx->d_kp_queues) {
+            // a launch on another stream may still be using the old scratch
+            cudaEvent_t done;
+            {
+                std::lock_guard<std::mutex> lk(g_wc_mu);
+                LH_CUDA(ctx, wc_done_event(ctx->device, &done));
+            }
+            LH_CUDA(ctx, cudaEventSynchronize(done));
+        }
         cudaFree(ctx->d_kp_queues); cudaFree(ctx->d_kp_cnt); cudaFree(ctx->d_kp_rare);
         ctx->d_kp_queues = nullptr; ctx->d_kp_cnt = nullptr; ctx->d_kp_rare = nullptr;
         LH_CUDA(ctx, cudaMalloc(&ctx->d_kp_rare, (size_t)P * WC_RARE_CAP * sizeof(uint4)));
@@ -439,9 +467,9 @@ lh_status launch_keyed_wc_spt(lh_ctx *ctx, int b, const IdT *ids, const ValT *va
     if constexpr (std::is_same<ValT, double>::value) {
         if (n2) fn = (const void *)k_ingest_keyed_wc<IdT, double, SPT, true>;
     }
-    LH_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // the attribute belongs to the function on the device, not to this context: one value for every context
+    LH_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
     unsigned int *d_barrier = ctx->d_kp_cnt + (size_t)2 * P * P;
-    LH_CUDA(ctx, cudaMemsetAsync(d_barrier, 0, sizeof(unsigned int), s));
     WcParams prm{};
     prm.ids = ids; prm.vals = vals; prm.n = n4x4; prm.ids_per = ids_per; prm.cap = (uint32_t)cap;
     prm.ids2 = ids2; prm.vals2 = vals2; prm.n2 = n2;
@@ -461,7 +489,15 @@ lh_status launch_keyed_wc_spt(lh_ctx *ctx, int b, const IdT *ids, const ValT *va
     prm.barrier = d_barrier; prm.rare = ctx->d_kp_rare; prm.o = keyed_out(ctx, b);
     Prec pc = ctx->pc;
     void *args[] = {&prm, &pc};
-    LH_CUDA(ctx, cudaLaunchCooperativeKernel(fn, dim3(P), dim3(S::THREADS), args, smem, s));
+    {
+        std::lock_guard<std::mutex> lk(g_wc_mu);
+        cudaEvent_t done;
+        LH_CUDA(ctx, wc_done_event(ctx->device, &done));
+        LH_CUDA(ctx, cudaStreamWaitEvent(s, done, 0));
+        LH_CUDA(ctx, cudaMemsetAsync(d_barrier, 0, sizeof(unsigned int), s));
+        LH_CUDA(ctx, cudaLaunchCooperativeKernel(fn, dim3(P), dim3(S::THREADS), args, smem, s));
+        LH_CUDA(ctx, cudaEventRecord(done, s));
+    }
     ctx->stats.kernel_launches++;
     *used = true;
     *taken = n4x4;
@@ -487,7 +523,14 @@ lh_status launch_keyed(lh_ctx *ctx, int b, const IdT *d_ids, const ValT *d_vals,
     while (done < n) {
         // no uint32 cell of the hot window may wrap: drain it before 2^32 samples have gone in
         const unsigned long long kCap = 0xFFFFFFFFull;
-        if (ctx->buf[b].hot_pending >= kCap - (1ull << 30)) { lh_status st = fold_hot(ctx, b, s); if (st != LH_OK) return st; }
+        if (ctx->buf[b].hot_pending >= kCap - (1ull << 30)) {
+            // the tally is host-side and counts what every stream has issued: the fold must come after all of it, not
+            // only after this stream's kernels (each writer event follows the last bracket issued on its stream)
+            for (const WriterEvent &w : ctx->buf[b].writers)
+                if (w.stream != s) LH_CUDA(ctx, cudaStreamWaitEvent(s, w.ev, 0));
+            lh_status st = fold_hot(ctx, b, s);
+            if (st != LH_OK) return st;
+        }
         size_t m = (size_t)std::min<unsigned long long>(n - done, kCap - ctx->buf[b].hot_pending);
         const IdT *ids = d_ids + done;
         const ValT *vals = d_vals + done;
@@ -506,7 +549,9 @@ lh_status launch_keyed(lh_ctx *ctx, int b, const IdT *d_ids, const ValT *d_vals,
                 const uint32_t per = (ctx->H + passes - 1) / passes;
                 const size_t smem = ((size_t)per * ctx->pc.win + 4) * 4;
                 const void *fn = (const void *)k_ingest_keyed_small<IdT, ValT>;
-                LH_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                // per device, not per context: a value of this context's H could be overwritten by another context's
+                // between here and the launch
+                LH_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
                 // one CTA per SM; fewer when the batch is small, so that the per-CTA flush stays negligible
                 int grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)(ctx->sm_count - ctx->k1_reserve_sms),
                                                                       n4 / (KS_THREADS * 16)));
@@ -859,7 +904,9 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
                 }
             }
         }
-        LH_CREATE_CUDA(cudaFuncSetAttribute(ctx->k1[i].func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ctx->k1[i].smem));
+        // the limit is an attribute of the function on the device, shared by every context: a value of this precision
+        // would make an older context of a higher precision fail its launches.  Every launch asks for at most the budget.
+        LH_CREATE_CUDA(cudaFuncSetAttribute(ctx->k1[i].func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
         int nb = 0;
         LH_CREATE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, ctx->k1[i].func, ctx->k1[i].threads, ctx->k1[i].smem));
         ctx->k1[i].blocks_per_sm = std::max(nb, 1);

@@ -580,7 +580,8 @@ k_ingest_keyed_small(const IdT *__restrict__ ids, const ValT *__restrict__ vals,
 //   phase B  every owner drains its P sub-queues (L2 hits) into its shared-memory windows (ATOMS.POPC.INC).
 // Samples the window does not cover (negative, |v| >= 2^63, NaN/Inf, estimates within eps of a bucket boundary),
 // ids >= H, and records that do not fit their buffer or sub-queue (heavily skewed ids) take the exact L2-atomic
-// route of keyed_one().  At the end each CTA adds its windows into the uint32 hot window.
+// route of keyed_one().  At the end each CTA adds its windows straight into the uint64 bucket arrays: nothing goes
+// through the uint32 hot window, so these launches add nothing to the host's tally of it (hot_pending).
 constexpr int WC_MAX_PARTS = 160;             // owners = CTAs (one per SM)
 constexpr int WC_LINE = 64;                   // records per line (128 B)
 
