@@ -108,6 +108,39 @@ LH_API lh_status lh_ingest_keyed_i64ns_u16(lh_ctx *ctx, const uint16_t *d_ids, c
  * lh_ingest_keyed_i64ns_u16; either count may be 0. */
 LH_API lh_status lh_ingest_keyed_pair_u16(lh_ctx *ctx, const uint16_t *d_ids_f64, const double *d_values, size_t n_f64,
                                           const uint16_t *d_ids_ns, const int64_t *d_nanos, size_t n_ns, void *stream);
+/* Many device arrays, each under its own histogram id, in one call (per-layer tensors, per-endpoint latency batches):
+ * the bucket counts are exactly those of issuing, for every item,
+ *   LH_VALUES_F64    lh_ingest_f64(ctx, histogram_id, d_values, n, stream)           Histogram(name, v), metrics.go:273-295
+ *   LH_VALUES_I64NS  the int64 nanoseconds of lh_ingest_keyed_i64ns_u16, float64(ns) round-to-nearest
+ *                                                                                     TimerToken.Stop, metrics.go:242-246
+ * but the call is ONE write bracket: one sequence number (lh_kernel_ms covers all its launches), lh_stats.samples += the
+ * sum of n, and every item lands in the same interval (a concurrent lh_snapshot_begin comes before all of it or after
+ * all of it).  Items may repeat ids, alias or overlap each other's memory and come in any order.
+ *
+ * Routing: an F64 item of at least 2^20 samples is ingested by the single-histogram kernel, as lh_ingest_f64 would;
+ * every other item goes to one kernel that deals the concatenation of the items to CTAs in pieces and counts them
+ * through a shared-memory combining table, up to 1024 items per launch.  A batch of a few hundred samples runs on one
+ * CTA, not the whole machine.
+ * Measured on an H100 80GB HBM3 at 700 W (DESIGN.md section 5): 64 arrays of 64 samples take 0.050 ms to a
+ * synchronise, against 0.73 ms as 64 lh_ingest_f64 calls; 4096 arrays of 1024 samples 0.36 ms against 48 ms.  A single
+ * short array is slower than one lh_ingest_f64 (17 vs 9 us of kernel time).
+ *
+ * Every item is validated before anything is enqueued; on error nothing is launched, counted or sequenced:
+ * LH_ERR_INVALID for h_items NULL with n_items > 0 or an unknown kind, and, for an item with n > 0, d_values NULL or
+ * not 8-byte aligned; LH_ERR_RANGE for an item with n > 0 and histogram_id >= max_histograms (as lh_ingest_f64, not
+ * the keyed calls' drop-and-count).  Items with n == 0 are skipped; a call without samples returns LH_OK with no
+ * bracket and no launch.  h_items may be reused when the call returns; the device arrays must stay valid until the
+ * stream's work completes.  The call never waits for the device and allocates nothing. */
+#define LH_VALUES_F64 0     /* float64 values */
+#define LH_VALUES_I64NS 1   /* int64 nanoseconds */
+typedef struct lh_batch_item {
+    const void *d_values;   /* device memory, 8-byte aligned */
+    uint64_t n;
+    uint32_t histogram_id;
+    uint32_t kind;          /* LH_VALUES_* */
+} lh_batch_item;
+LH_API lh_status lh_ingest_batch(lh_ctx *ctx, const lh_batch_item *h_items, uint32_t n_items, void *stream);
+
 /* Counter(name, amount), metrics.go:251-269: wrapping uint64 adds. */
 LH_API lh_status lh_counter_add_u16(lh_ctx *ctx, const uint16_t *d_ids, const uint64_t *d_amounts,
                              size_t n, void *stream);
@@ -393,7 +426,7 @@ LH_API const char *lh_k1_variant_name(lh_ctx *ctx, int32_t i);
 /* name of the kernel the most recent keyed ingest dispatched to */
 LH_API const char *lh_keyed_kernel_name(lh_ctx *ctx);
 /* Ingest timing: two CUDA events on the launch stream bracket the kernels of one sequence number, which is
- *   - one device-pointer ingest call, lh_ingest_keyed_pair_u16 included whichever kernels it takes;
+ *   - one device-pointer ingest call, lh_ingest_keyed_pair_u16 and lh_ingest_batch included whichever kernels they take;
  *   - one staging chunk of a host-fed call (lh_*_host); its H2D copy is outside the bracket;
  *   - one lh_staging_commit_* call;
  *   - one lh_gpu_timer_stop.

@@ -79,6 +79,15 @@ class lh_recorder(C.Structure):
     ]
 
 
+LH_VALUES_F64 = 0      # lh_batch_item.kind: float64 values
+LH_VALUES_I64NS = 1    # int64 nanoseconds, recorded as float64(ns)
+
+
+class lh_batch_item(C.Structure):
+    """One (histogram id, device array) item of lh_ingest_batch."""
+    _fields_ = [("d_values", C.c_void_p), ("n", C.c_uint64), ("histogram_id", C.c_uint32), ("kind", C.c_uint32)]
+
+
 class lh_gpu_timer(C.Structure):
     """Opaque handle of a GPU timer (lh_gpu_timer_start)."""
     _fields_ = [("handle", C.c_uint64)]
@@ -98,6 +107,7 @@ SIGNATURES = {
     "lh_ingest_keyed_f64_u32": (_i32, [_vp, _vp, _vp, _sz, _vp]),
     "lh_ingest_keyed_i64ns_u16": (_i32, [_vp, _vp, _vp, _sz, _vp]),
     "lh_ingest_keyed_pair_u16": (_i32, [_vp, _vp, _vp, _sz, _vp, _vp, _sz, _vp]),
+    "lh_ingest_batch": (_i32, [_vp, C.POINTER(lh_batch_item), _u32, _vp]),
     "lh_counter_add_u16": (_i32, [_vp, _vp, _vp, _sz, _vp]),
     "lh_counter_add_u32": (_i32, [_vp, _vp, _vp, _sz, _vp]),
     "lh_ingest_f64_host": (_i32, [_vp, _u32, _vp, _sz]),

@@ -206,6 +206,9 @@ struct lh_ctx {
     size_t kp_cap = 0;
     int kp_parts = 0;
     const char *keyed_kernel = "";       // kernel the last keyed launch used
+    // lh_ingest_batch: CTAs of k_ingest_batch per SM (filled at create) and the parameter block being filled (locked)
+    int batch_blocks_per_sm = 1;
+    BatchParams batch_prm{};
     // multi-GPU (lh_comm_*): peer mappings of every rank's arrays + this rank's reduced output arrays
     uint32_t comm_rank = 0, comm_world = 0;
     unsigned long long *d_comm = nullptr;         // this rank's comm block (uint64[kCommWords])
@@ -662,6 +665,73 @@ lh_status launch_counter(lh_ctx *ctx, int b, const IdT *d_ids, const uint64_t *d
     return LH_OK;
 }
 
+// lh_ingest_batch routing.  An F64 item this long pays back K1's full-grid launch (launch_single); shorter ones and every
+// I64NS item go to k_ingest_batch.
+constexpr size_t kBatchK1Min = 1024 * 1024;
+
+// Items of a validated batch (lh_ingest_batch): the long float64 ones through launch_single, the rest through as few
+// launches of k_ingest_batch as the parameter block and the uint32 table counts allow.  An item that does not fit the
+// launch being filled is split across launches.
+lh_status launch_batch(lh_ctx *ctx, int b, const lh_batch_item *items, uint32_t n_items, cudaStream_t s) {
+    BatchParams &prm = ctx->batch_prm;
+    lh_recorder &rec = prm.rec;
+    memset(&rec, 0, sizeof rec);
+    rec.d_buckets = reinterpret_cast<uint64_t *>(ctx->buf[b].d_buckets);
+    rec.d_flags = ctx->buf[b].d_flags;
+    rec.d_counters = reinterpret_cast<uint64_t *>(ctx->buf[b].d_counters);
+    rec.d_dropped = reinterpret_cast<uint64_t *>(ctx->d_dropped);
+    rec.max_histograms = ctx->H;
+    rec.max_counters = ctx->C;
+    memcpy(rec.prec, &ctx->pc, sizeof ctx->pc);
+    // pieces are dealt round-robin, so at most 2^31 samples per CTA of the full grid keeps every table count below 2^32
+    const int grid_max = std::max(1, ctx->sm_count - ctx->k1_reserve_sms) * ctx->batch_blocks_per_sm;
+    const unsigned long long cap = std::min<unsigned long long>(1ull << 36, (unsigned long long)grid_max << 31);
+    uint32_t k = 0;
+    unsigned long long total = 0, batched = 0;
+    auto launch = [&]() -> lh_status {
+        if (!k) return LH_OK;
+        prm.n_items = k;
+        const unsigned long long pieces = (total + BI_PIECE - 1) / BI_PIECE;
+        const int grid = (int)std::min<unsigned long long>((unsigned long long)grid_max, pieces);
+        k_ingest_batch<<<grid, BI_THREADS, BlockRecorder::smem_bytes(BI_TABLE_ENTRIES), s>>>(prm);
+        LH_CUDA(ctx, cudaGetLastError());
+        ctx->stats.kernel_launches++;
+        batched += total;
+        k = 0;
+        total = 0;
+        return LH_OK;
+    };
+    for (uint32_t i = 0; i < n_items; i++) {
+        const lh_batch_item &it = items[i];
+        if (it.n == 0) continue;
+        if (it.kind == LH_VALUES_F64 && it.n >= kBatchK1Min) {
+            lh_status st = launch_single(ctx, b, it.histogram_id, (const double *)it.d_values, (size_t)it.n, s);
+            if (st != LH_OK) return st;
+            continue;
+        }
+        const unsigned long long *p = (const unsigned long long *)it.d_values;
+        unsigned long long left = it.n;
+        while (left) {
+            if (k == (uint32_t)BI_MAX_ITEMS || total == cap) {
+                lh_status st = launch();
+                if (st != LH_OK) return st;
+            }
+            const unsigned long long m = std::min(left, cap - total);
+            prm.seg[k] = BatchSeg{p, it.histogram_id, it.kind};
+            prm.start[k] = total;
+            total += m;
+            prm.start[k + 1] = total;
+            k++;
+            p += m;
+            left -= m;
+        }
+    }
+    lh_status st = launch();
+    if (st != LH_OK) return st;
+    ctx->stats.samples += batched;
+    return LH_OK;
+}
+
 // ---- staging ring (locked) ----
 // Called with ctx->mu held through `lk`.  The host-side wait for an in-flight slot happens with the mutex RELEASED
 // (the slot is parked as SLOT_WAITED meanwhile so nobody else takes it): other ingest threads are never held up by
@@ -911,6 +981,13 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
         LH_CREATE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, ctx->k1[i].func, ctx->k1[i].threads, ctx->k1[i].smem));
         ctx->k1[i].blocks_per_sm = std::max(nb, 1);
     }
+    {   // the attribute is per function on the device, so the same budget as every other kernel with a large table
+        const void *fn = (const void *)k_ingest_batch;
+        LH_CREATE_CUDA(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
+        int nb = 0;
+        LH_CREATE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, fn, BI_THREADS, BlockRecorder::smem_bytes(BI_TABLE_ENTRIES)));
+        ctx->batch_blocks_per_sm = std::max(nb, 1);
+    }
     LH_CREATE_CUDA(cudaStreamSynchronize(ctx->snap_stream));
 #undef LH_CREATE_CUDA
     *out = ctx;
@@ -1038,6 +1115,23 @@ extern "C" lh_status lh_counter_add_u32(lh_ctx *ctx, const uint32_t *d_ids, cons
     if (n && (!d_ids || !d_amounts)) return fail(ctx, LH_ERR_INVALID, "NULL input");
     cudaStream_t s = pick_stream(ctx, stream);
     return write_bracket(ctx, s, [&](int b) { return launch_counter<unsigned int>(ctx, b, d_ids, d_amounts, n, s); });
+}
+extern "C" lh_status lh_ingest_batch(lh_ctx *ctx, const lh_batch_item *h_items, uint32_t n_items, void *stream) {
+    LH_ENTER(ctx);
+    if (n_items && !h_items) return fail(ctx, LH_ERR_INVALID, "h_items is NULL");
+    unsigned long long n = 0;
+    for (uint32_t i = 0; i < n_items; i++) {
+        const lh_batch_item &it = h_items[i];
+        if (it.kind != LH_VALUES_F64 && it.kind != LH_VALUES_I64NS) return fail(ctx, LH_ERR_INVALID, "unknown item kind");
+        if (it.n == 0) continue;
+        if (!it.d_values) return fail(ctx, LH_ERR_INVALID, "item d_values is NULL");
+        if (((uintptr_t)it.d_values & 7u) != 0) return fail(ctx, LH_ERR_INVALID, "item d_values must be 8-byte aligned");
+        if (it.histogram_id >= ctx->H) return fail(ctx, LH_ERR_RANGE, "item histogram_id >= max_histograms");
+        n += it.n;
+    }
+    if (n == 0) return LH_OK;
+    cudaStream_t s = pick_stream(ctx, stream);
+    return write_bracket(ctx, s, [&](int b) { return launch_batch(ctx, b, h_items, n_items, s); });
 }
 
 // =========================================================== ingest (host)

@@ -1650,6 +1650,75 @@ k_peer_allreduce(PeerParams p) {
     }
 }
 
+// ----------------------------------------------------------- batch ingest (lh_ingest_batch)
+// Many short device arrays, each under its own histogram id, in one launch.  The item table travels in the parameter
+// block (no copy, no allocation): descriptors plus prefix offsets of their lengths.  The concatenation of the items is
+// cut into pieces of BI_PIECE samples, dealt round-robin to the CTAs; a piece may span several items.  Every CTA counts
+// into one lh::BlockRecorder combining table over the interval's rows and flushes it once, so a sample costs shared
+// atomics wherever the CTA's distinct (id, bucket) pairs fit the table, and the table's direct path otherwise: the
+// count is exact whatever the fill.  The host bounds the samples of a launch so that no CTA counts more than 2^31 of
+// them (the table's counts are uint32).
+constexpr int BI_THREADS = 512;
+constexpr uint32_t BI_TABLE_ENTRIES = 8192;  // 96 KB of combining table: two CTAs per SM
+constexpr uint32_t BI_PIECE = 2048;          // samples per piece: 4 per thread
+constexpr int BI_MAX_ITEMS = 1024;           // items per launch: 24 B each in the parameter block
+
+struct BatchSeg {
+    const unsigned long long *vals;          // 8-byte samples (float64 or int64 ns)
+    uint32_t id;
+    uint32_t kind;                           // LH_VALUES_*
+};
+struct BatchParams {
+    lh_recorder rec;                         // the interval's rows, built by the library (no scope)
+    uint32_t n_items;
+    uint32_t pad;
+    unsigned long long start[BI_MAX_ITEMS + 1];   // prefix offsets of the items' lengths
+    BatchSeg seg[BI_MAX_ITEMS];
+};
+
+__global__ void __launch_bounds__(BI_THREADS, 2)
+k_ingest_batch(const __grid_constant__ BatchParams p) {
+    extern __shared__ __align__(16) unsigned char bi_smem[];
+    BlockRecorder br(p.rec, bi_smem, BI_TABLE_ENTRIES);
+    br.init();
+    const unsigned long long total = p.start[p.n_items];
+    const unsigned long long pieces = (total + BI_PIECE - 1) / BI_PIECE;
+    for (unsigned long long pc = blockIdx.x; pc < pieces; pc += gridDim.x) {
+        unsigned long long lo = pc * BI_PIECE;
+        const unsigned long long hi = min(lo + BI_PIECE, total);
+        // the item holding sample lo: the last one whose start is <= lo (uniform over the CTA)
+        uint32_t a = 0, b = p.n_items - 1;
+        while (a < b) {
+            const uint32_t m = (a + b + 1) / 2;
+            if (p.start[m] <= lo) a = m; else b = m - 1;
+        }
+        // every thread walks the piece's samples across item boundaries (its item index only grows), so the loads of a
+        // piece are in flight together however short the items are
+        uint32_t it = a;
+        for (unsigned long long g0 = lo + threadIdx.x; g0 < hi; g0 += 2 * BI_THREADS) {
+            unsigned long long raw[2];
+            uint32_t id[2];
+            bool ns[2];
+#pragma unroll
+            for (int k = 0; k < 2; k++) {
+                const unsigned long long g = g0 + k * BI_THREADS;
+                raw[k] = 0ull; id[k] = 0u; ns[k] = false;
+                if (g < hi) {
+                    while (p.start[it + 1] <= g) ++it;
+                    id[k] = p.seg[it].id;
+                    ns[k] = p.seg[it].kind == LH_VALUES_I64NS;
+                    raw[k] = __ldcs(p.seg[it].vals + (g - p.start[it]));
+                }
+            }
+#pragma unroll
+            for (int k = 0; k < 2; k++)
+                if (g0 + k * BI_THREADS < hi)
+                    br.record(id[k], ns[k] ? __ll2double_rn((long long)raw[k]) : __longlong_as_double((long long)raw[k]));
+        }
+    }
+    br.flush();
+}
+
 // ----------------------------------------------------------- GPU timers (lh_gpu_timer_*)
 // One thread each: their cost is the launch, not the body.  The start writes %globaltimer into the token's slot; the
 // stop records float64(now - start) into one histogram row through the same bucket function and row writer every

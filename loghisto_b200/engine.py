@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import contextlib
 import ctypes as C
+import math
 from dataclasses import dataclass
 
 import numpy as np
@@ -47,6 +48,43 @@ def _stream(s) -> int:
     if hasattr(s, "cuda_stream"):   # torch.cuda.Stream
         return int(s.cuda_stream)
     raise TypeError(f"not a stream: {type(s)!r}")
+
+
+_BATCH_KINDS = {"float64": L.LH_VALUES_F64, "int64": L.LH_VALUES_I64NS}
+_TYPESTRS = {t: np.dtype(t) for t in ("<f8", "<i8")}
+
+
+def _batch_array(x):
+    """(address, length, LH_VALUES_* kind) of one device array of a batch: a CUDA torch tensor, a DeviceArray or an
+    object with __cuda_array_interface__, contiguous, of dtype float64 or int64.  TypeError otherwise."""
+    if hasattr(x, "is_cuda") and hasattr(x, "data_ptr"):        # torch.Tensor
+        if not x.is_cuda:
+            raise TypeError("batch arrays must be in device memory, not a CPU tensor")
+        if not x.is_contiguous():
+            raise TypeError("batch arrays must be contiguous")
+        dtype = str(x.dtype).replace("torch.", "")
+        ptr, n = int(x.data_ptr()), int(x.numel())
+    elif isinstance(x, DeviceArray):
+        dtype, ptr, n = x.dtype.name, x.ptr, x.n
+    elif hasattr(x, "__cuda_array_interface__"):
+        cai = x.__cuda_array_interface__
+        dt = _TYPESTRS.get(cai["typestr"]) or np.dtype(cai["typestr"])
+        shape = cai["shape"]
+        n = math.prod(shape)
+        strides = cai.get("strides")
+        if strides is not None and n > 1:
+            want, step = [], dt.itemsize
+            for d in reversed(shape):
+                want.append(step)
+                step *= d
+            if tuple(strides) != tuple(reversed(want)):
+                raise TypeError("batch arrays must be contiguous")
+        dtype, ptr = dt.name if dt.byteorder in "=<|" else "", int(cai["data"][0])
+    else:
+        raise TypeError(f"not a device array: {type(x)!r}")
+    if dtype not in _BATCH_KINDS:
+        raise TypeError(f"batch arrays must be float64 (Histogram) or int64 (Timer nanoseconds), not {dtype or 'big-endian'}")
+    return ptr, n, _BATCH_KINDS[dtype]
 
 
 CUDA_STREAM_LEGACY = 1   # cudaStreamLegacy
@@ -281,6 +319,20 @@ class Engine:
         """Histogram samples and Timer samples of one batch in one call (one launch of the write-combining kernel)."""
         self._check(self.lib.lh_ingest_keyed_pair_u16(self.h, _ptr(d_ids_f64), _ptr(d_values), n_f64, _ptr(d_ids_ns), _ptr(d_nanos), n_ns,
                                                       _stream(stream)))
+
+    def ingest_batch(self, items, stream=None):
+        """Many device arrays, each under its own histogram id, in one call (lh_ingest_batch): `items` is a list of
+        (histogram id, array) pairs; the array is a CUDA torch tensor, a DeviceArray or a __cuda_array_interface__
+        object, contiguous, float64 (Histogram samples) or int64 (Timer nanoseconds).  TypeError before the call for
+        anything else."""
+        items = list(items)
+        arr = (L.lh_batch_item * max(len(items), 1))()
+        for i, (hid, a) in enumerate(items):
+            ptr, n, kind = _batch_array(a)
+            if not 0 <= int(hid) < 1 << 32:
+                raise ValueError(f"histogram id {hid} is not a uint32")
+            arr[i] = L.lh_batch_item(ptr, n, int(hid), kind)
+        self._check(self.lib.lh_ingest_batch(self.h, arr, len(items), _stream(stream)))
 
     def counter_add_u16(self, d_ids, d_amounts, n: int, stream=None):
         self._check(self.lib.lh_counter_add_u16(self.h, _ptr(d_ids), _ptr(d_amounts), n, _stream(stream)))

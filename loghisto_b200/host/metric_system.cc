@@ -23,6 +23,7 @@
 #pragma weak lh_record_begin
 #pragma weak lh_record_end
 #pragma weak lh_ingest_f64
+#pragma weak lh_ingest_batch
 // And for GPU timers: over a build without them, StartGpuTimer hands out tokens whose Stop drops and counts.
 #pragma weak lh_gpu_timer_start
 #pragma weak lh_gpu_timer_stop
@@ -711,6 +712,21 @@ void RecordScope::Histogram(size_t i, const double *d_values, size_t n) {
     if (id == kUnbound) { ms_->dropped_over_limit_.fetch_add(n, std::memory_order_relaxed); return; }
     check(ms_->ctx_, lh_ingest_f64(ms_->ctx_, id, d_values, n, stream_), "lh_ingest_f64");
 }
+void RecordScope::Histograms(const std::vector<Item> &items) {
+    if (!ms_) throw std::runtime_error("RecordScope::Histograms after End()");
+    for (const Item &it : items) (void)hids_.at(it.name);   // std::out_of_range before anything is issued
+    if (!lh_ingest_batch) throw std::runtime_error("lh_ingest_batch: not in this build of the library");
+    std::vector<lh_batch_item> batch;
+    batch.reserve(items.size());
+    uint64_t unbound = 0;
+    for (const Item &it : items) {
+        const uint32_t id = hids_[it.name];
+        if (id == kUnbound) { unbound += it.n; continue; }
+        batch.push_back(lh_batch_item{it.d_values, (uint64_t)it.n, id, it.kind});
+    }
+    check(ms_->ctx_, lh_ingest_batch(ms_->ctx_, batch.data(), (uint32_t)batch.size(), stream_), "lh_ingest_batch");
+    ms_->dropped_over_limit_.fetch_add(unbound, std::memory_order_relaxed);
+}
 
 // ---- GPU timers ------------------------------------------------------------------------------------------------
 void *const GpuTimerToken::kStartStream = reinterpret_cast<void *>(~(uintptr_t)0);
@@ -1270,6 +1286,24 @@ LHMS_API int lhms_record_ingest_f64(void *ms, const lh_recorder *rec, uint32_t n
     auto it = g_scopes.find(std::make_pair(ms, rec->scope));
     if (it == g_scopes.end()) return LH_ERR_INVALID;
     try { it->second.Histogram(name_index, d_values, n); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
+}
+// RecordScope::Histograms: item i is n[i] samples of kind kinds[i] (LH_VALUES_*) at d_values[i] under histogram name
+// name_index[i] of the scope.
+LHMS_API int lhms_scope_histograms(void *ms, const lh_recorder *rec, const uint32_t *name_index,
+                                      const void *const *d_values, const uint64_t *n, const uint32_t *kinds,
+                                      uint32_t n_items) {
+    if (!ms || !rec || (n_items && (!name_index || !d_values || !n || !kinds))) return LH_ERR_INVALID;
+    std::lock_guard<std::mutex> lk(g_scopes_mu);
+    auto it = g_scopes.find(std::make_pair(ms, rec->scope));
+    if (it == g_scopes.end()) return LH_ERR_INVALID;
+    try {
+        std::vector<RecordScope::Item> items(n_items);
+        for (uint32_t i = 0; i < n_items; i++) items[i] = RecordScope::Item{name_index[i], d_values[i], (size_t)n[i], kinds[i]};
+        it->second.Histograms(items);
+        return LH_OK;
+    } catch (const std::exception &e) {
+        return scope_status(e);
+    }
 }
 // GPU timers (MetricSystem::StartGpuTimer).  start returns a token, or NULL with *status set; stop may be called
 // repeatedly on `stream` (passed as given: NULL = the context's ingest stream); free releases the token's slot.

@@ -140,6 +140,17 @@ class RecordScope {
     // name the samples are dropped and counted.  Throws std::out_of_range for a bad index, std::runtime_error when the
     // library refuses the call (e.g. a misaligned pointer) or the scope has ended.
     void Histogram(size_t i, const double *d_values, size_t n);
+    // Many device arrays in one lh_ingest_batch on the scope's stream: n samples at d_values (8-byte aligned device
+    // memory) under histogram name `name`, of kind LH_VALUES_F64 (float64) or LH_VALUES_I64NS (int64 ns, recorded as
+    // float64(ns)).  Names may repeat.  Items under unbound names are dropped and counted; the others are one call.
+    // Throws as Histogram does, before anything is issued for a bad index.
+    struct Item {
+        size_t name;
+        const void *d_values;
+        size_t n;
+        uint32_t kind;
+    };
+    void Histograms(const std::vector<Item> &items);
     void End();
     bool open() const { return ms_ != nullptr; }
 

@@ -10,7 +10,7 @@ import ctypes as C
 
 from . import _lib as _L
 from . import build as _build
-from .engine import _stream, _timer_stream
+from .engine import _batch_array, _stream, _timer_stream
 
 _EMIT = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_char_p, C.c_int, C.c_uint64, C.c_double)
 _lib = None
@@ -71,6 +71,8 @@ def _bind(L):
     L.lhms_record_end.argtypes = [vp, rec]
     L.lhms_record_ingest_f64.restype = C.c_int
     L.lhms_record_ingest_f64.argtypes = [vp, rec, C.c_uint32, vp, C.c_size_t]
+    L.lhms_scope_histograms.restype = C.c_int
+    L.lhms_scope_histograms.argtypes = [vp, rec, u32p, C.POINTER(vp), C.POINTER(C.c_uint64), u32p, C.c_uint32]
     L.lhms_gpu_timer_start.restype = vp
     L.lhms_gpu_timer_start.argtypes = [vp, C.c_char_p, vp, C.POINTER(C.c_int)]
     L.lhms_gpu_timer_stop.restype = C.c_int
@@ -195,6 +197,24 @@ class RecordScope:
                                                   values.data_ptr(), values.numel())
         if st != 0:
             raise RuntimeError("lhms_record_ingest_f64 failed (status %d)" % st)
+
+    def histograms(self, arrays):
+        """Histogram(name, v) for every element of several device arrays in one call (lh_ingest_batch), on the scope's
+        stream: `arrays` is {name: array} or a list of (name, array) pairs, names among the scope's histograms and
+        possibly repeated.  An array is a contiguous CUDA tensor (or DeviceArray / __cuda_array_interface__ object):
+        float64 values, or int64 nanoseconds recorded as float64(ns) like a Timer's Stop.  TypeError for any other
+        array and KeyError for a name the scope was not opened with, before anything is issued."""
+        pairs = list(arrays.items()) if isinstance(arrays, dict) else list(arrays)
+        k = max(len(pairs), 1)
+        idx, ptrs, ns, kinds = (C.c_uint32 * k)(), (C.c_void_p * k)(), (C.c_uint64 * k)(), (C.c_uint32 * k)()
+        for i, (name, a) in enumerate(pairs):
+            if name not in self._hnames:
+                raise KeyError("%r is not a histogram of this scope" % (name,))
+            idx[i] = self._hnames.index(name)
+            ptrs[i], ns[i], kinds[i] = _batch_array(a)
+        st = self._ms._lib.lhms_scope_histograms(self._ms._h, C.byref(self.recorder), idx, ptrs, ns, kinds, len(pairs))
+        if st != 0:
+            raise RuntimeError("lhms_scope_histograms failed (status %d)" % st)
 
     def end(self):
         if self._open:

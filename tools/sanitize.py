@@ -4,6 +4,15 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import loghisto_b200 as lh
 
 PS = [0.0, 0.5, 0.99, 1.0]
+
+
+class View:
+    """n 8-byte elements at a device address, as a __cuda_array_interface__ object (an item of ingest_batch)."""
+    def __init__(self, ptr, n, typestr="<f8"):
+        self.n = n
+        self.__cuda_array_interface__ = {"shape": (n,), "typestr": typestr, "data": (ptr, False), "version": 3}
+
+
 n = 300_001
 total = 0
 with lh.Engine(device=0, max_histograms=64, max_counters=64) as e:
@@ -26,6 +35,9 @@ with lh.Engine(device=0, max_histograms=64, max_counters=64) as e:
         e.ingest_keyed_f64_u16(ids, d, n); total += n
     e.ingest_keyed_pair_u16(ids, d, n, ids, ns, n); total += 2 * n   # float64 + int64 segments in one launch
     e.tune("keyed_mode", 0)
+    items = [(i % 64, View(d.offset(i * 700), 700 + 3 * i)) for i in range(300)]   # batch kernel, pieces across items
+    items += [(5, View(ns.offset(1), 20_000, "<i8")), (6, View(d.offset(3), 9_000))]       # int64 ns, misaligned starts
+    e.ingest_batch(items); total += sum(v.n for _, v in items)
     e.counter_add_u16(ids, amt, n)                      # vector + scalar counter kernels
     e.counter_add_u16(ids.offset(1), amt.offset(1), n - 1)
     e.snapshot_begin()
