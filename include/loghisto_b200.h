@@ -347,14 +347,23 @@ LH_API lh_status lh_reduce_sparse_host(lh_ctx *ctx, uint32_t n_histograms, const
  *   lh_snapshot_allreduce  collective, between lh_snapshot_begin and lh_snapshot_reduce/_export: ranks must take
  *                    their snapshots in lock-step (same number, same order).  Enqueued on the snapshot stream; the
  *                    kernel waits on the device for the peers' frozen arrays (no host synchronisation) and returns
- *                    LH_OK immediately.  A peer that never arrives makes the kernel give up after 10 s; that is
- *                    reported by lh_comm_info.status != 0 (the snapshot's counts are then this rank's own only)
+ *                    LH_OK immediately.  A peer that never arrives makes the kernel give up after 10 s (status 1);
+ *                    ranks that froze different halves of their double buffers, because one took a snapshot
+ *                    without the collective, are found at once (status 2, on every rank).  Either way the snapshot's
+ *                    reduction, export and counter deltas are then this rank's own frozen counts only, and nothing
+ *                    was written into a peer's arrays by this rank.  lh_comm_info.status and last_bytes_from_peers
+ *                    describe the most recent all-reduce (0 bytes when it failed): a failure does not outlive it,
+ *                    so the all-reduce after the ranks are back in lock-step sums again.  Limit: a timeout can be
+ *                    one-sided -- a peer that did arrive may still read this rank's frozen arrays, or (two-shot
+ *                    form) push its sums into this rank's reduced arrays, after this rank gave up; only status 2 is
+ *                    known to be seen by every rank alike
  *   lh_comm_allreduce_ms   device time of all-reduce `seq` (CUDA events around the kernel on the snapshot stream)
  */
 typedef struct lh_peer_handle { uint8_t bytes[LH_PEER_HANDLE_BYTES]; } lh_peer_handle;
 typedef struct lh_comm_stats {
     uint32_t rank, world;
-    uint32_t status;                 /* 0 ok, 1 a peer did not arrive in time, 2 peers froze different buffers */
+    uint32_t status;                 /* most recent all-reduce: 0 ok, 1 a peer did not arrive in time, 2 peers froze
+                                        different buffers (1 and 2: the snapshot holds this rank's counts only) */
     uint32_t reserved;
     uint64_t allreduces;
     uint64_t last_bytes_from_peers;  /* bytes read over NVLink by the most recent all-reduce */

@@ -212,7 +212,7 @@ struct lh_ctx {
     // multi-GPU (lh_comm_*): peer mappings of every rank's arrays + this rank's reduced output arrays
     uint32_t comm_rank = 0, comm_world = 0;
     unsigned long long *d_comm = nullptr;         // this rank's comm block (uint64[kCommWords])
-    unsigned int *d_comm_aux = nullptr;           // [0] block counter, [1] status
+    unsigned int *d_comm_aux = nullptr;           // [0] block counter, [1] status, [2..3] cells (both of the last all-reduce)
     PeerMap peers[kMaxRanks];
     unsigned long long *d_red_buckets = nullptr;  // [H][65536] sums over ranks (valid for the open snapshot after lh_snapshot_allreduce)
     uint32_t *d_red_flags = nullptr;
@@ -1946,6 +1946,8 @@ extern "C" lh_status lh_snapshot_allreduce(lh_ctx *ctx, uint32_t include_counter
     if (ctx->view_reduced) return fail(ctx, LH_ERR_STATE, "this snapshot has already been all-reduced");
     const int f = ctx->active ^ 1;
     cudaStream_t s = ctx->snap_stream;
+    // status and cells describe this all-reduce only: zeroed behind the previous one on the same stream
+    LH_CUDA(ctx, cudaMemsetAsync(ctx->d_comm_aux + 1, 0, 12, s));
     PeerParams p{};
     p.rank = ctx->comm_rank; p.world = ctx->comm_world; p.H = ctx->H; p.C = ctx->C; p.win = ctx->pc.win;
     p.do_counters = include_counters ? 1u : 0u; p.frozen = (uint32_t)f;

@@ -1553,21 +1553,25 @@ k_peer_allreduce(PeerParams p) {
     //    one-shot (small payload): every rank sums every item into its own array - one NVLink round trip.
     //    two-shot (large payload): the rank that owns an item sums it and pushes the sum into every rank's array, so a
     //    rank moves 2 * (world - 1) / world of the payload over NVLink instead of (world - 1) times the payload.
-    if (ok) {
+    //    When a peer did not arrive or froze the other buffer (status != 0), the one-shot form runs over this rank
+    //    alone: its reduced arrays get its own frozen cells, flags and counters, and nothing goes to a peer's arrays.
+    {
+        const uint32_t r0 = ok ? 0u : p.rank, r1 = ok ? p.world : p.rank + 1u;
+        const bool push = ok && p.two_shot;
         const uint32_t wcells = 2u * p.win - 1u;
         constexpr uint32_t PER_H = 65536u / K5_CHUNK;         // items are indexed as if every histogram were dense
         const uint32_t chunks_w = (wcells + K5_CHUNK - 1) / K5_CHUNK;
         unsigned long long cells = 0;
         for (uint32_t h = t; h < p.H; h += K5_THREADS) {
             uint32_t lv = 0;
-            for (uint32_t r = 0; r < p.world; r++) lv |= ld_sys_u32(p.flags[r] + h);
+            for (uint32_t r = r0; r < r1; r++) lv |= ld_sys_u32(p.flags[r] + h);
             s_level[h] = (unsigned char)lv;
             if (blockIdx.x == 0 && lv) { p.out_flags[h] = lv; cells += (lv & 2u) ? 65536u : wcells; }
         }
         if (blockIdx.x == 0 && cells) atomicAdd(&s_cells, cells);
         __syncthreads();
-        if (blockIdx.x == 0 && t == 0) *p.cells = s_cells;
-        if (!p.two_shot) {
+        if (ok && blockIdx.x == 0 && t == 0) *p.cells = s_cells;      // nothing was read from a peer otherwise
+        if (!push) {
             const size_t nitems = (size_t)p.H * PER_H;
             for (size_t item = blockIdx.x; item < nitems; item += gridDim.x) {
                 const uint32_t h = (uint32_t)(item / PER_H), chunk = (uint32_t)(item % PER_H);
@@ -1583,7 +1587,7 @@ k_peer_allreduce(PeerParams p) {
                     if (i >= ncell) continue;
                     const size_t cell = (size_t)h * 65536u + (dense ? i : window_cell(i, p.win));
                     unsigned long long sum = 0;
-                    for (uint32_t r = 0; r < p.world; r++) sum += ld_peer_u64(p.buckets[r] + cell);
+                    for (uint32_t r = r0; r < r1; r++) sum += ld_peer_u64(p.buckets[r] + cell);
                     if (sum) p.out_buckets[cell] = sum;
                 }
             }
@@ -1625,11 +1629,11 @@ k_peer_allreduce(PeerParams p) {
         if (p.do_counters && blockIdx.x == 0) {
             for (uint32_t i = t; i < p.C; i += K5_THREADS) {
                 unsigned long long sum = 0;
-                for (uint32_t r = 0; r < p.world; r++) sum += ld_sys_u64(p.counters[r] + i);
+                for (uint32_t r = r0; r < r1; r++) sum += ld_sys_u64(p.counters[r] + i);
                 p.out_counters[i] = sum;
             }
         }
-        if (p.two_shot) __threadfence_system();              // my pushes are performed before this CTA checks out
+        if (push) __threadfence_system();                    // my pushes are performed before this CTA checks out
     }
     // 4. depart: the last CTA of this rank tells every peer it has finished reading them and that the sums it pushed
     //    are visible (every CTA fences at system scope before it checks out), then waits for the same from every peer
