@@ -221,6 +221,56 @@ typedef struct lh_recorder {          /* passed by value to kernels; valid only 
 LH_API lh_status lh_record_begin(lh_ctx *ctx, void *stream, lh_recorder *out);
 LH_API lh_status lh_record_end(lh_ctx *ctx, const lh_recorder *rec);
 
+/* ---- recording from CUDA graphs ---------------------------------------------------------------------------------
+ * A record scope hands out the active interval's rows, which a captured kernel would keep writing at every replay,
+ * after the snapshot froze them.  A graph recorder owns its rows instead: `rec` is an ordinary lh_recorder whose
+ * d_buckets / d_flags / d_counters are k histogram rows (local ids 0 .. k-1) and kc counters that no snapshot swaps or
+ * clears, so lh::record / record_ns / count / stop / BlockHistogram / BlockRecorder work unchanged in kernels captured
+ * into a CUDA graph and replayed any number of times.  Each lh_snapshot_begin drains every live recorder into the
+ * interval it freezes: one kernel on the snapshot stream takes every non-zero cell with an atomic exchange to 0 and
+ * adds it to the row of the histogram (counter) id the local row is bound to at that moment.  Replays running
+ * meanwhile keep adding, so each count is taken by exactly one drain; the host never waits for a replay.  A count
+ * lands in the interval of the first collection whose drain finds it, so a caller that wants a replay in a given
+ * interval synchronises the replay's stream before collecting.
+ *
+ *   lh_graph_recorder_create   allocates and zeroes k rows of uint64[65536] (512 KiB each), k flags and kc counters,
+ *                              k <= max_histograms, kc <= max_counters, k + kc >= 1, and binds them: hist_ids[i] /
+ *                              counter_ids[i] (NULL = all unbound) is the context id local row i drains into.  The
+ *                              recorder has max_histograms = k and max_counters = kc (a local id >= k is dropped and
+ *                              counted, as in a scope), the context's d_dropped and precision, and a `scope` that
+ *                              lh_record_end refuses with LH_ERR_INVALID.  Call it outside any stream capture; it
+ *                              waits for the zeroing.
+ *   lh_graph_recorder_bind     sets the target ids of the rows (either array may be NULL: unchanged).  Takes effect at
+ *                              the next drain.  LH_GRAPH_UNBOUND: that row's drained counts are dropped and counted in
+ *                              lh_stats.dropped (for a counter, its drained amount).
+ *   lh_graph_recorder_ingest   lh_ingest_batch into the recorder's rows: the same items, kinds, validation (ids are
+ *                              local: LH_ERR_RANGE for histogram_id >= k) and kernels, but no write bracket, event,
+ *                              sequence number, lh_stats.samples or allocation -- it only enqueues kernels, so it may be
+ *                              captured into a CUDA graph (or called on an ordinary stream).  On error nothing is
+ *                              enqueued.
+ *   lh_graph_recorder_destroy  enqueues a final drain on `stream` (NULL = the ingest stream) into the active interval
+ *                              as one write bracket, as an ingest call, and frees the rows, stream-ordered, after it and
+ *                              after every collection drain already issued.  The caller guarantees that no replay that
+ *                              uses the recorder is pending or will be launched.  lh_destroy frees every recorder left.
+ *
+ * A handle carries its context: a destroyed or foreign handle gets LH_ERR_INVALID and touches nothing.  Every call
+ * that takes the context's lock (the snapshot calls, lh_sync, lh_destroy and the host-fed ingest calls among them)
+ * switches the calling thread to cudaStreamCaptureModeRelaxed for its duration, so a collection from another thread
+ * neither fails nor invalidates a capture that some thread runs in the global mode (torch.cuda.graph's default). */
+#define LH_GRAPH_UNBOUND 0xFFFFFFFFu
+typedef struct lh_graph_recorder {
+    uint64_t handle;          /* opaque */
+    lh_recorder rec;          /* pass by value to captured kernels */
+} lh_graph_recorder;
+LH_API lh_status lh_graph_recorder_create(lh_ctx *ctx, uint32_t n_histograms, uint32_t n_counters,
+                                          const uint32_t *hist_ids, const uint32_t *counter_ids,
+                                          lh_graph_recorder *out);
+LH_API lh_status lh_graph_recorder_bind(lh_ctx *ctx, const lh_graph_recorder *g, const uint32_t *hist_ids,
+                                        const uint32_t *counter_ids);
+LH_API lh_status lh_graph_recorder_ingest(lh_ctx *ctx, const lh_graph_recorder *g, const lh_batch_item *h_items,
+                                          uint32_t n_items, void *stream);
+LH_API lh_status lh_graph_recorder_destroy(lh_ctx *ctx, const lh_graph_recorder *g, void *stream);
+
 /* ---- GPU timers: StartTimer / Stop (metrics.go:232-246) from host code, timed on the device ------------------
  * Host StartTimer / Stop around CUDA work time the enqueue.  These calls put the two ends of the span on the GPU
  * instead: each end is a one-thread kernel on `stream` that reads %globaltimer (the clock of lh::start_timer), and

@@ -93,6 +93,14 @@ class lh_gpu_timer(C.Structure):
     _fields_ = [("handle", C.c_uint64)]
 
 
+LH_GRAPH_UNBOUND = 0xFFFFFFFF   # target id of a graph recorder row whose drained counts are dropped and counted
+
+
+class lh_graph_recorder(C.Structure):
+    """A graph recorder (lh_graph_recorder_create): `rec` is passed by value to kernels captured into CUDA graphs."""
+    _fields_ = [("handle", C.c_uint64), ("rec", lh_recorder)]
+
+
 _vp, _sz, _u32, _u64, _i32 = C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint64, C.c_int32
 
 # name -> (restype, argtypes); every symbol include/loghisto_b200.h declares
@@ -122,6 +130,10 @@ SIGNATURES = {
     "lh_staging_abandon": (_i32, [_vp, C.POINTER(lh_staging)]),
     "lh_record_begin": (_i32, [_vp, _vp, C.POINTER(lh_recorder)]),
     "lh_record_end": (_i32, [_vp, C.POINTER(lh_recorder)]),
+    "lh_graph_recorder_create": (_i32, [_vp, _u32, _u32, _vp, _vp, C.POINTER(lh_graph_recorder)]),
+    "lh_graph_recorder_bind": (_i32, [_vp, C.POINTER(lh_graph_recorder), _vp, _vp]),
+    "lh_graph_recorder_ingest": (_i32, [_vp, C.POINTER(lh_graph_recorder), C.POINTER(lh_batch_item), _u32, _vp]),
+    "lh_graph_recorder_destroy": (_i32, [_vp, C.POINTER(lh_graph_recorder), _vp]),
     "lh_gpu_timer_start": (_i32, [_vp, _vp, C.POINTER(lh_gpu_timer)]),
     "lh_gpu_timer_stop": (_i32, [_vp, C.POINTER(lh_gpu_timer), _u32, _vp, _vp]),
     "lh_gpu_timer_release": (_i32, [_vp, C.POINTER(lh_gpu_timer)]),

@@ -39,6 +39,13 @@ struct TimerSlot {
     std::vector<WriterEvent> stops;    // after the latest stop on each stream that stopped the token
 };
 
+// a graph recorder (lh_graph_recorder_*): rows it owns, drained into the frozen interval at every lh_snapshot_begin
+struct GraphRec {
+    uint64_t handle;
+    lh_recorder rec;                 // what the caller was given (rows, flags, counters in one allocation)
+    std::vector<uint32_t> hid, cid;  // target id of each local row / counter (LH_GRAPH_UNBOUND = drop and count)
+};
+
 struct Buffer {
     unsigned long long *d_buckets = nullptr;   // [H][65536]
     unsigned long long *d_counters = nullptr;  // [C]
@@ -246,6 +253,11 @@ struct lh_ctx {
     std::vector<uint32_t> timer_released;            // released slots, oldest first, reused once their kernels are done
     uint32_t timer_fresh = 0;                         // slots [timer_fresh, n) have never been handed out
     std::vector<cudaEvent_t> timer_spare_events;      // stop events of recycled slots
+    // graph recorders, and the parameter block of their drain kernel (filled under the lock)
+    std::vector<GraphRec> graphs;
+    uint64_t next_graph = 1;
+    cudaEvent_t graph_drained = nullptr;               // after the latest collection drain (created with the first recorder)
+    DrainParams drain_prm{};
     // stats
     lh_stats stats{};
     std::mutex mu;
@@ -267,6 +279,16 @@ lh_status fail(lh_ctx *ctx, lh_status st, const char *what, cudaError_t e = cuda
     }
     return st;
 }
+
+// The calling thread in cudaStreamCaptureModeRelaxed for the scope of one entry point.  In the global mode (what
+// torch.cuda.graph uses by default) a capture on ANY thread makes calls such as cudaEventSynchronize or cudaMalloc fail
+// on every other thread and invalidates the capture; the library's own calls never touch a capturing stream, so a
+// collection from a reaper thread may run beside a capture.
+struct RelaxedCapture {
+    cudaStreamCaptureMode prev = cudaStreamCaptureModeRelaxed;
+    RelaxedCapture() { cudaThreadExchangeStreamCaptureMode(&prev); }
+    ~RelaxedCapture() { cudaThreadExchangeStreamCaptureMode(&prev); }
+};
 
 #define LH_CUDA(ctx, call)                                                      \
     do {                                                                        \
@@ -322,10 +344,23 @@ lh_status write_bracket(lh_ctx *ctx, cudaStream_t s, Body body) {
     return after_write(ctx, b, s);
 }
 
-// ---- ingest bodies (run inside write_bracket, on validated input) ----
-lh_status launch_single(lh_ctx *ctx, int b, uint32_t hid, const double *d_values, size_t n, cudaStream_t s) {
-    unsigned long long *counts = ctx->buf[b].d_buckets + (size_t)hid * 65536u;
-    uint32_t *flag = ctx->buf[b].d_flags + hid;
+// ---- ingest bodies (run on validated input: inside write_bracket, or into a graph recorder's rows) ----
+// The rows of buffer b as a recorder: the target the bodies below write, like a graph recorder's.
+lh_recorder buffer_target(lh_ctx *ctx, int b) {
+    lh_recorder rec;
+    memset(&rec, 0, sizeof rec);
+    rec.d_buckets = reinterpret_cast<uint64_t *>(ctx->buf[b].d_buckets);
+    rec.d_flags = ctx->buf[b].d_flags;
+    rec.d_counters = reinterpret_cast<uint64_t *>(ctx->buf[b].d_counters);
+    rec.d_dropped = reinterpret_cast<uint64_t *>(ctx->d_dropped);
+    rec.max_histograms = ctx->H;
+    rec.max_counters = ctx->C;
+    memcpy(rec.prec, &ctx->pc, sizeof ctx->pc);
+    return rec;
+}
+
+// K1 into one row (counts, flag); the caller counts the samples in stats
+lh_status launch_single(lh_ctx *ctx, unsigned long long *counts, uint32_t *flag, const double *d_values, size_t n, cudaStream_t s) {
     const K1Variant &kv = ctx->k1[ctx->k1_variant];
     // a CTA's uint32 sub-histogram must not overflow: tiles are dealt round-robin, so bounding a launch to
     // 2^31 samples per CTA keeps every cell below 2^32 whatever the grid size (reserved SMs shrink it)
@@ -348,8 +383,13 @@ lh_status launch_single(lh_ctx *ctx, int b, uint32_t hid, const double *d_values
         ctx->stats.kernel_launches++;
         done += m;
     }
-    ctx->stats.samples += n;
     return LH_OK;
+}
+// n samples of histogram hid into buffer b, counted in stats
+lh_status ingest_single(lh_ctx *ctx, int b, uint32_t hid, const double *d_values, size_t n, cudaStream_t s) {
+    lh_status st = launch_single(ctx, ctx->buf[b].d_buckets + (size_t)hid * 65536u, ctx->buf[b].d_flags + hid, d_values, n, s);
+    if (st == LH_OK) ctx->stats.samples += n;
+    return st;
 }
 
 lh_status fold_hot(lh_ctx *ctx, int b, cudaStream_t s) {
@@ -669,25 +709,18 @@ lh_status launch_counter(lh_ctx *ctx, int b, const IdT *d_ids, const uint64_t *d
 // I64NS item go to k_ingest_batch.
 constexpr size_t kBatchK1Min = 1024 * 1024;
 
-// Items of a validated batch (lh_ingest_batch): the long float64 ones through launch_single, the rest through as few
-// launches of k_ingest_batch as the parameter block and the uint32 table counts allow.  An item that does not fit the
-// launch being filled is split across launches.
-lh_status launch_batch(lh_ctx *ctx, int b, const lh_batch_item *items, uint32_t n_items, cudaStream_t s) {
+// Items of a validated batch (lh_ingest_batch, lh_graph_recorder_ingest) into the rows of `target`: the long float64
+// ones through launch_single, the rest through as few launches of k_ingest_batch as the parameter block and the uint32
+// table counts allow.  An item that does not fit the launch being filled is split across launches.  Kernels only (the
+// graph recorder's form is captured); the caller counts the samples in stats.
+lh_status launch_batch(lh_ctx *ctx, const lh_recorder &target, const lh_batch_item *items, uint32_t n_items, cudaStream_t s) {
     BatchParams &prm = ctx->batch_prm;
-    lh_recorder &rec = prm.rec;
-    memset(&rec, 0, sizeof rec);
-    rec.d_buckets = reinterpret_cast<uint64_t *>(ctx->buf[b].d_buckets);
-    rec.d_flags = ctx->buf[b].d_flags;
-    rec.d_counters = reinterpret_cast<uint64_t *>(ctx->buf[b].d_counters);
-    rec.d_dropped = reinterpret_cast<uint64_t *>(ctx->d_dropped);
-    rec.max_histograms = ctx->H;
-    rec.max_counters = ctx->C;
-    memcpy(rec.prec, &ctx->pc, sizeof ctx->pc);
+    prm.rec = target;
     // pieces are dealt round-robin, so at most 2^31 samples per CTA of the full grid keeps every table count below 2^32
     const int grid_max = std::max(1, ctx->sm_count - ctx->k1_reserve_sms) * ctx->batch_blocks_per_sm;
     const unsigned long long cap = std::min<unsigned long long>(1ull << 36, (unsigned long long)grid_max << 31);
     uint32_t k = 0;
-    unsigned long long total = 0, batched = 0;
+    unsigned long long total = 0;
     auto launch = [&]() -> lh_status {
         if (!k) return LH_OK;
         prm.n_items = k;
@@ -696,7 +729,6 @@ lh_status launch_batch(lh_ctx *ctx, int b, const lh_batch_item *items, uint32_t 
         k_ingest_batch<<<grid, BI_THREADS, BlockRecorder::smem_bytes(BI_TABLE_ENTRIES), s>>>(prm);
         LH_CUDA(ctx, cudaGetLastError());
         ctx->stats.kernel_launches++;
-        batched += total;
         k = 0;
         total = 0;
         return LH_OK;
@@ -705,7 +737,8 @@ lh_status launch_batch(lh_ctx *ctx, int b, const lh_batch_item *items, uint32_t 
         const lh_batch_item &it = items[i];
         if (it.n == 0) continue;
         if (it.kind == LH_VALUES_F64 && it.n >= kBatchK1Min) {
-            lh_status st = launch_single(ctx, b, it.histogram_id, (const double *)it.d_values, (size_t)it.n, s);
+            unsigned long long *row = reinterpret_cast<unsigned long long *>(target.d_buckets) + (size_t)it.histogram_id * 65536u;
+            lh_status st = launch_single(ctx, row, target.d_flags + it.histogram_id, (const double *)it.d_values, (size_t)it.n, s);
             if (st != LH_OK) return st;
             continue;
         }
@@ -726,10 +759,66 @@ lh_status launch_batch(lh_ctx *ctx, int b, const lh_batch_item *items, uint32_t 
             left -= m;
         }
     }
-    lh_status st = launch();
-    if (st != LH_OK) return st;
-    ctx->stats.samples += batched;
+    return launch();
+}
+
+// Validation of lh_ingest_batch / lh_graph_recorder_ingest against `limit` histogram ids; the samples of the batch
+lh_status check_batch(lh_ctx *ctx, const lh_batch_item *h_items, uint32_t n_items, uint32_t limit, unsigned long long *n_out) {
+    if (n_items && !h_items) return fail(ctx, LH_ERR_INVALID, "h_items is NULL");
+    unsigned long long n = 0;
+    for (uint32_t i = 0; i < n_items; i++) {
+        const lh_batch_item &it = h_items[i];
+        if (it.kind != LH_VALUES_F64 && it.kind != LH_VALUES_I64NS) return fail(ctx, LH_ERR_INVALID, "unknown item kind");
+        if (it.n == 0) continue;
+        if (!it.d_values) return fail(ctx, LH_ERR_INVALID, "item d_values is NULL");
+        if (((uintptr_t)it.d_values & 7u) != 0) return fail(ctx, LH_ERR_INVALID, "item d_values must be 8-byte aligned");
+        if (it.histogram_id >= limit) return fail(ctx, LH_ERR_RANGE, "item histogram_id >= max_histograms");
+        n += it.n;
+    }
+    *n_out = n;
     return LH_OK;
+}
+
+// One launch of k_graph_drain per DR_MAX_ENTRIES rows and counters of `graphs` (all live recorders, or one), into the
+// rows of buffer b, on s.
+lh_status drain_graphs(lh_ctx *ctx, const GraphRec *graphs, size_t n_graphs, int b, cudaStream_t s) {
+    DrainParams &p = ctx->drain_prm;
+    p.buckets = ctx->buf[b].d_buckets;
+    p.flags = ctx->buf[b].d_flags;
+    p.counters = ctx->buf[b].d_counters;
+    p.dropped = ctx->d_dropped;
+    p.win = ctx->pc.win;
+    p.n = 0;
+    auto launch = [&]() -> lh_status {
+        if (!p.n) return LH_OK;
+        k_graph_drain<<<p.n, DR_THREADS, 0, s>>>(p);
+        LH_CUDA(ctx, cudaGetLastError());
+        ctx->stats.kernel_launches++;
+        p.n = 0;
+        return LH_OK;
+    };
+    auto add = [&](unsigned long long *src, uint32_t *flag, uint32_t target) -> lh_status {
+        if (p.n == (uint32_t)DR_MAX_ENTRIES) {
+            lh_status st = launch();
+            if (st != LH_OK) return st;
+        }
+        p.e[p.n++] = DrainEntry{src, flag, target, 0};
+        return LH_OK;
+    };
+    for (size_t g = 0; g < n_graphs; g++) {
+        const GraphRec &gr = graphs[g];
+        unsigned long long *rows = reinterpret_cast<unsigned long long *>(gr.rec.d_buckets);
+        unsigned long long *ctrs = reinterpret_cast<unsigned long long *>(gr.rec.d_counters);
+        for (uint32_t i = 0; i < gr.rec.max_histograms; i++) {
+            lh_status st = add(rows + (size_t)i * 65536u, gr.rec.d_flags + i, gr.hid[i]);
+            if (st != LH_OK) return st;
+        }
+        for (uint32_t i = 0; i < gr.rec.max_counters; i++) {
+            lh_status st = add(ctrs + i, nullptr, gr.cid[i]);
+            if (st != LH_OK) return st;
+        }
+    }
+    return launch();
 }
 
 // ---- staging ring (locked) ----
@@ -996,12 +1085,15 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
 
 extern "C" lh_status lh_destroy(lh_ctx *ctx) {
     if (!ctx) return LH_OK;
+    RelaxedCapture relaxed;
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
         if (!ctx->scopes.empty()) return fail(ctx, LH_ERR_STATE, "lh_destroy with record scopes open");
     }
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
+    for (auto &g : ctx->graphs) cudaFree(g.rec.d_buckets);
+    if (ctx->graph_drained) cudaEventDestroy(ctx->graph_drained);
     comm_unmap(ctx);
     cudaFree(ctx->d_comm); cudaFree(ctx->d_comm_aux);
     cudaFree(ctx->d_red_buckets); cudaFree(ctx->d_red_flags); cudaFree(ctx->d_red_counters);
@@ -1056,6 +1148,7 @@ extern "C" lh_status lh_destroy(lh_ctx *ctx) {
 // =========================================================== ingest (device)
 #define LH_ENTER(ctx)                                   \
     if (!(ctx)) return LH_ERR_INVALID;                  \
+    RelaxedCapture _relaxed;                            \
     std::unique_lock<std::mutex> _lk((ctx)->mu);        \
     LH_CUDA((ctx), cudaSetDevice((ctx)->device))
 
@@ -1077,7 +1170,7 @@ extern "C" lh_status lh_ingest_f64(lh_ctx *ctx, uint32_t hid, const double *d_va
     if (hid >= ctx->H) return fail(ctx, LH_ERR_RANGE, "histogram_id >= max_histograms");
     if (((uintptr_t)d_values & 7u) != 0) return fail(ctx, LH_ERR_INVALID, "d_values must be 8-byte aligned");
     cudaStream_t s = pick_stream(ctx, stream);
-    return write_bracket(ctx, s, [&](int b) { return launch_single(ctx, b, hid, d_values, n, s); });
+    return write_bracket(ctx, s, [&](int b) { return ingest_single(ctx, b, hid, d_values, n, s); });
 }
 extern "C" lh_status lh_ingest_keyed_f64_u16(lh_ctx *ctx, const uint16_t *d_ids, const double *d_values, size_t n, void *stream) {
     LH_ENTER(ctx);
@@ -1118,20 +1211,15 @@ extern "C" lh_status lh_counter_add_u32(lh_ctx *ctx, const uint32_t *d_ids, cons
 }
 extern "C" lh_status lh_ingest_batch(lh_ctx *ctx, const lh_batch_item *h_items, uint32_t n_items, void *stream) {
     LH_ENTER(ctx);
-    if (n_items && !h_items) return fail(ctx, LH_ERR_INVALID, "h_items is NULL");
     unsigned long long n = 0;
-    for (uint32_t i = 0; i < n_items; i++) {
-        const lh_batch_item &it = h_items[i];
-        if (it.kind != LH_VALUES_F64 && it.kind != LH_VALUES_I64NS) return fail(ctx, LH_ERR_INVALID, "unknown item kind");
-        if (it.n == 0) continue;
-        if (!it.d_values) return fail(ctx, LH_ERR_INVALID, "item d_values is NULL");
-        if (((uintptr_t)it.d_values & 7u) != 0) return fail(ctx, LH_ERR_INVALID, "item d_values must be 8-byte aligned");
-        if (it.histogram_id >= ctx->H) return fail(ctx, LH_ERR_RANGE, "item histogram_id >= max_histograms");
-        n += it.n;
-    }
-    if (n == 0) return LH_OK;
+    lh_status st = check_batch(ctx, h_items, n_items, ctx->H, &n);
+    if (st != LH_OK || n == 0) return st;
     cudaStream_t s = pick_stream(ctx, stream);
-    return write_bracket(ctx, s, [&](int b) { return launch_batch(ctx, b, h_items, n_items, s); });
+    return write_bracket(ctx, s, [&](int b) {
+        lh_status bs = launch_batch(ctx, buffer_target(ctx, b), h_items, n_items, s);
+        if (bs == LH_OK) ctx->stats.samples += n;
+        return bs;
+    });
 }
 
 // =========================================================== ingest (host)
@@ -1161,7 +1249,7 @@ lh_status staging_step(lh_ctx *ctx, Slot &sl, HostKind kind, uint32_t hid, const
         ctx->stats.h2d_bytes += n * (kind == HK_SINGLE ? 8 : 10);
         st = write_bracket(ctx, s, [&](int b) {
             switch (kind) {
-            case HK_SINGLE: return launch_single(ctx, b, hid, (const double *)d_a, n, s);
+            case HK_SINGLE: return ingest_single(ctx, b, hid, (const double *)d_a, n, s);
             case HK_KEYED_U16: return launch_keyed<unsigned short, double>(ctx, b, d_i, (const double *)d_a, n, s);
             case HK_KEYED_I64_U16: return launch_keyed<unsigned short, long long>(ctx, b, d_i, (const long long *)d_a, n, s);
             default: return launch_counter<unsigned short>(ctx, b, d_i, (const uint64_t *)d_a, n, s);   // HK_COUNTER_U16
@@ -1359,6 +1447,108 @@ extern "C" lh_status lh_record_end(lh_ctx *ctx, const lh_recorder *rec) {
     return fail(ctx, LH_ERR_INVALID, "unknown or already ended record scope");
 }
 
+// =========================================================== graph recorders
+namespace {
+// handle = context tag (16 bits) | serial (48 bits)
+uint64_t graph_handle(const lh_ctx *ctx, uint64_t serial) {
+    return (ctx->ctx_id % 0xFFFFu + 1u) << 48 | (serial & 0xFFFFFFFFFFFFull);
+}
+
+// the live recorder a handle names (its rows must match too), or nullptr
+GraphRec *graph_of(lh_ctx *ctx, const lh_graph_recorder *g) {
+    if (!g) return nullptr;
+    for (auto &gr : ctx->graphs)
+        if (gr.handle == g->handle && gr.rec.d_buckets == g->rec.d_buckets) return &gr;
+    return nullptr;
+}
+
+// target ids: each < limit or LH_GRAPH_UNBOUND
+bool ids_ok(const uint32_t *ids, uint32_t n, uint32_t limit) {
+    for (uint32_t i = 0; ids && i < n; i++)
+        if (ids[i] >= limit && ids[i] != LH_GRAPH_UNBOUND) return false;
+    return true;
+}
+}  // namespace
+
+extern "C" lh_status lh_graph_recorder_create(lh_ctx *ctx, uint32_t k, uint32_t kc, const uint32_t *hist_ids,
+                                              const uint32_t *counter_ids, lh_graph_recorder *out) {
+    LH_ENTER(ctx);
+    if (!out) return fail(ctx, LH_ERR_INVALID, "out is NULL");
+    if (k == 0 && kc == 0) return fail(ctx, LH_ERR_INVALID, "a graph recorder needs a histogram or a counter");
+    if (k > ctx->H || kc > ctx->C) return fail(ctx, LH_ERR_RANGE, "more rows than max_histograms / max_counters");
+    if (!ids_ok(hist_ids, k, ctx->H) || !ids_ok(counter_ids, kc, ctx->C))
+        return fail(ctx, LH_ERR_RANGE, "target id >= max_histograms / max_counters");
+    if (!ctx->graph_drained) LH_CUDA(ctx, cudaEventCreateWithFlags(&ctx->graph_drained, cudaEventDisableTiming));
+    // one allocation: rows [k][65536], counters [kc], flags [k]
+    const size_t row_bytes = (size_t)k * 65536u * 8u, bytes = row_bytes + (size_t)kc * 8u + (size_t)k * 4u;
+    cudaStream_t s = ctx->snap_stream;
+    char *base = nullptr;
+    LH_CUDA(ctx, cudaMallocAsync((void **)&base, bytes, s));
+    cudaError_t e = cudaMemsetAsync(base, 0, bytes, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) {
+        cudaFreeAsync(base, s);
+        return fail(ctx, LH_ERR_CUDA, "lh_graph_recorder_create", e);
+    }
+    GraphRec gr;
+    gr.handle = graph_handle(ctx, ctx->next_graph++);
+    memset(&gr.rec, 0, sizeof gr.rec);
+    gr.rec.d_buckets = reinterpret_cast<uint64_t *>(base);
+    gr.rec.d_counters = reinterpret_cast<uint64_t *>(base + row_bytes);
+    gr.rec.d_flags = reinterpret_cast<uint32_t *>(base + row_bytes + (size_t)kc * 8u);
+    gr.rec.d_dropped = reinterpret_cast<uint64_t *>(ctx->d_dropped);
+    gr.rec.max_histograms = k;
+    gr.rec.max_counters = kc;
+    gr.rec.block_smem_bytes = subhist_words(ctx->pc.win) * 4u;
+    gr.rec.scope = 0;   // never a scope ticket: lh_record_end refuses it
+    memcpy(gr.rec.prec, &ctx->pc, sizeof ctx->pc);
+    gr.hid.assign(k, LH_GRAPH_UNBOUND);
+    gr.cid.assign(kc, LH_GRAPH_UNBOUND);
+    if (hist_ids) gr.hid.assign(hist_ids, hist_ids + k);
+    if (counter_ids) gr.cid.assign(counter_ids, counter_ids + kc);
+    ctx->graphs.push_back(gr);
+    out->handle = gr.handle;
+    out->rec = gr.rec;
+    return LH_OK;
+}
+
+extern "C" lh_status lh_graph_recorder_bind(lh_ctx *ctx, const lh_graph_recorder *g, const uint32_t *hist_ids,
+                                            const uint32_t *counter_ids) {
+    LH_ENTER(ctx);
+    GraphRec *gr = graph_of(ctx, g);
+    if (!gr) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign graph recorder");
+    if (!ids_ok(hist_ids, gr->rec.max_histograms, ctx->H) || !ids_ok(counter_ids, gr->rec.max_counters, ctx->C))
+        return fail(ctx, LH_ERR_RANGE, "target id >= max_histograms / max_counters");
+    if (hist_ids) gr->hid.assign(hist_ids, hist_ids + gr->rec.max_histograms);
+    if (counter_ids) gr->cid.assign(counter_ids, counter_ids + gr->rec.max_counters);
+    return LH_OK;
+}
+
+extern "C" lh_status lh_graph_recorder_ingest(lh_ctx *ctx, const lh_graph_recorder *g, const lh_batch_item *h_items,
+                                              uint32_t n_items, void *stream) {
+    LH_ENTER(ctx);
+    GraphRec *gr = graph_of(ctx, g);
+    if (!gr) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign graph recorder");
+    unsigned long long n = 0;
+    lh_status st = check_batch(ctx, h_items, n_items, gr->rec.max_histograms, &n);
+    if (st != LH_OK || n == 0) return st;
+    return launch_batch(ctx, gr->rec, h_items, n_items, pick_stream(ctx, stream));
+}
+
+extern "C" lh_status lh_graph_recorder_destroy(lh_ctx *ctx, const lh_graph_recorder *g, void *stream) {
+    LH_ENTER(ctx);
+    GraphRec *gr = graph_of(ctx, g);
+    if (!gr) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign graph recorder");
+    cudaStream_t s = pick_stream(ctx, stream);
+    // after every collection drain issued so far, then the final drain, then the free: all stream-ordered on s
+    LH_CUDA(ctx, cudaStreamWaitEvent(s, ctx->graph_drained, 0));
+    lh_status st = write_bracket(ctx, s, [&](int b) { return drain_graphs(ctx, gr, 1, b, s); });
+    if (st != LH_OK) return st;
+    LH_CUDA(ctx, cudaFreeAsync(gr->rec.d_buckets, s));
+    ctx->graphs.erase(ctx->graphs.begin() + (gr - ctx->graphs.data()));
+    return LH_OK;
+}
+
 // =========================================================== GPU timers
 namespace {
 // handle = context tag (16 bits) | generation (28 bits) | slot (20 bits)
@@ -1517,6 +1707,11 @@ extern "C" lh_status lh_snapshot_begin(lh_ctx *ctx) {
     }
     // order the snapshot stream after every ingest launch that wrote the buffer being frozen
     for (auto &w : ctx->buf[f].writers) LH_CUDA(ctx, cudaStreamWaitEvent(ctx->snap_stream, w.ev, 0));
+    if (!ctx->graphs.empty()) {   // what graph recorders hold so far joins the interval being frozen
+        lh_status st = drain_graphs(ctx, ctx->graphs.data(), ctx->graphs.size(), f, ctx->snap_stream);
+        if (st != LH_OK) return st;
+        LH_CUDA(ctx, cudaEventRecord(ctx->graph_drained, ctx->snap_stream));
+    }
     if (ctx->buf[f].hot_pending) {   // drain the keyed path's uint32 window into the uint64 buckets
         lh_status st = fold_hot(ctx, f, ctx->snap_stream);
         if (st != LH_OK) return st;
@@ -1624,6 +1819,7 @@ extern "C" lh_status lh_snapshot_reduce_async(lh_ctx *ctx, const double *percent
 extern "C" lh_status lh_snapshot_result(lh_ctx *ctx, uint64_t ticket, uint64_t *counts, double *sums, double *avgs,
                                         int32_t *pkeys, double *pvals) {
     if (!ctx) return LH_ERR_INVALID;
+    RelaxedCapture relaxed;
     const int slot = (int)(ticket & 1);
     cudaEvent_t ev;
     {

@@ -20,6 +20,8 @@
 //                               mappings (SURVEY.md section 8e) -- no library collective
 //   K6   k_scatter_segments, k_sparse_epilogue   caller-supplied sparse histograms -> scratch rows -> K3
 //                               (lh_reduce_sparse_host)
+//   k_ingest_batch          many device arrays under many ids (lh_ingest_batch, lh_graph_recorder_ingest)
+//   k_graph_drain           graph recorders' rows -> the interval being frozen (lh_snapshot_begin)
 //   misc k_clear_touched, k_fill_decompress, k_compress_probe, k_fastpath_margin, k_stream_probe, k_gen_stream,
 //        k_gen_ids_u16
 //
@@ -1721,6 +1723,80 @@ k_ingest_batch(const __grid_constant__ BatchParams p) {
         }
     }
     br.flush();
+}
+
+// ----------------------------------------------------------- graph recorder drain (lh_graph_recorder_*)
+// Moves the counts of graph-owned rows into an interval's rows.  One CTA per entry of the table, which travels in the
+// parameter block: a histogram row (src, src_flag, target id) or a counter (src, no flag, target id).  A row whose flag
+// is 0 is skipped; otherwise its window (every cell when flag & 2) is read with 16-byte loads through L2, and every
+// non-zero cell is taken with an atomic exchange to 0 and added to the target row with add_bucket_global, which raises
+// the target flag for the key as every writer does.  Unbound targets (LH_GRAPH_UNBOUND) add the total to `dropped`.
+//
+// Exactness while replays keep recording into the source rows: a replay's add and the drain's exchange are atomics on
+// the same cell, so every add is taken by exactly one exchange, this one or a later drain's; nothing is lost or counted
+// twice.  Source flags are never cleared: a writer adds to the cell before it raises the flag, but another SM may see
+// the flag first or the cell first.  A drain that reads a stale flag (0, or 1 where an out-of-window cell was just
+// written) or a stale zero cell skips counts that a later drain will find, since the flag stays raised; it never takes
+// a count twice.  The cost is one scan per touched row per drain, bounded by the rows the recorders declare.
+constexpr int DR_THREADS = 256;
+constexpr int DR_MAX_ENTRIES = 1024;         // entries per launch: 24 B each in the parameter block
+
+struct DrainEntry {
+    unsigned long long *src;                 // row [65536], or one counter
+    uint32_t *src_flag;                      // nullptr for a counter
+    uint32_t target;                         // histogram / counter id of the interval, or LH_GRAPH_UNBOUND
+    uint32_t pad;
+};
+struct DrainParams {
+    unsigned long long *buckets;             // the interval's rows [H][65536]
+    uint32_t *flags;                         // [H]
+    unsigned long long *counters;            // [C]
+    unsigned long long *dropped;
+    uint32_t win;
+    uint32_t n;
+    DrainEntry e[DR_MAX_ENTRIES];
+};
+
+__device__ __forceinline__ ulonglong2 ld_cg_u64x2(const unsigned long long *p) {
+    ulonglong2 r;
+    asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(r.x), "=l"(r.y) : "l"(p) : "memory");
+    return r;
+}
+
+__global__ void __launch_bounds__(DR_THREADS)
+k_graph_drain(const __grid_constant__ DrainParams p) {
+    const DrainEntry &e = p.e[blockIdx.x];
+    const bool unbound = e.target == LH_GRAPH_UNBOUND;
+    unsigned long long lost = 0;
+    if (!e.src_flag) {
+        if (threadIdx.x == 0 && *reinterpret_cast<volatile unsigned long long *>(e.src)) {
+            const unsigned long long c = atomicExch(e.src, 0ull);
+            if (unbound) lost = c;
+            else if (c) atomicAdd(p.counters + e.target, c);
+        }
+    } else {
+        const uint32_t level = *reinterpret_cast<volatile uint32_t *>(e.src_flag);
+        if (level == 0) return;
+        unsigned long long *row = unbound ? nullptr : p.buckets + (size_t)e.target * 65536u;
+        uint32_t *flag = unbound ? nullptr : p.flags + e.target;
+        auto take = [&](uint32_t key) {
+            const unsigned long long c = atomicExch(e.src + key, 0ull);
+            if (!c) return;
+            if (unbound) lost += c;
+            else add_bucket_global(row, flag, key, c, p.win);
+        };
+        // cell pairs to scan: all 32768, or the pairs holding keys [0, win) and [65536 - win + 1, 65536)
+        const uint32_t lo_pairs = (level & 2u) ? 32768u : (p.win + 1u) / 2u;
+        const uint32_t hi_first = (level & 2u) ? 32768u : (65536u - p.win + 1u) / 2u;
+        const uint32_t n_pairs = lo_pairs + (32768u - hi_first);
+        for (uint32_t j = threadIdx.x; j < n_pairs; j += DR_THREADS) {
+            const uint32_t pair = j < lo_pairs ? j : hi_first + (j - lo_pairs);
+            const ulonglong2 v = ld_cg_u64x2(e.src + 2u * pair);
+            if (v.x) take(2u * pair);
+            if (v.y) take(2u * pair + 1u);
+        }
+    }
+    if (lost) atomicAdd(p.dropped, lost);
 }
 
 // ----------------------------------------------------------- GPU timers (lh_gpu_timer_*)

@@ -185,6 +185,75 @@ class Sparse:
         return {int(k): int(c) for k, c in zip(self.keys[a:b], self.counts[a:b])}
 
 
+def _capture_stream(s) -> int:
+    """Stream of a graph recorder call: None = torch's current stream (inside torch.cuda.graph, the capturing stream;
+    torch's default stream as itself) where torch has CUDA, else the context's ingest stream; otherwise as _timer_stream."""
+    if s is None:
+        try:
+            import torch
+        except ImportError:
+            return 0
+        if not torch.cuda.is_available():
+            return 0
+        s = torch.cuda.current_stream()
+    return _timer_stream(s)
+
+
+def _batch_items(items, limit_name: str):
+    """lh_batch_item array of (id, array) pairs; TypeError / ValueError before any call."""
+    items = list(items)
+    arr = (L.lh_batch_item * max(len(items), 1))()
+    for i, (hid, a) in enumerate(items):
+        ptr, n, kind = _batch_array(a)
+        if not 0 <= int(hid) < 1 << 32:
+            raise ValueError(f"{limit_name} {hid} is not a uint32")
+        arr[i] = L.lh_batch_item(ptr, n, int(hid), kind)
+    return arr, len(items)
+
+
+def _ids(ids):
+    ids = [int(x) for x in ids]
+    return (C.c_uint32 * max(len(ids), 1))(*ids), len(ids)
+
+
+class GraphRecorder:
+    """A graph recorder of an Engine (Engine.graph_recorder): `recorder` is the lh_recorder to pass by value to kernels
+    captured into CUDA graphs, recording under local ids 0 .. len(hist_ids) - 1 (counters 0 .. len(counter_ids) - 1)."""
+
+    def __init__(self, engine: "Engine", hist_ids, counter_ids):
+        self._eng = engine
+        self.g = L.lh_graph_recorder()
+        h, k = _ids(hist_ids)
+        c, kc = _ids(counter_ids)
+        engine._check(engine.lib.lh_graph_recorder_create(engine.h, k, kc, h, c, C.byref(self.g)))
+        self.recorder = self.g.rec
+        self._open = True
+
+    def bind(self, hist_ids=None, counter_ids=None):
+        """Target ids from the next snapshot_begin on (None = unchanged)."""
+        h = _ids(hist_ids)[0] if hist_ids is not None else None
+        c = _ids(counter_ids)[0] if counter_ids is not None else None
+        self._eng._check(self._eng.lib.lh_graph_recorder_bind(self._eng.h, C.byref(self.g), h, c))
+
+    def ingest(self, items, stream=None):
+        """lh_graph_recorder_ingest of (local id, array) pairs, arrays as Engine.ingest_batch takes them, on `stream`
+        (None = torch's current stream, so that it is captured inside torch.cuda.graph)."""
+        arr, n = _batch_items(items, "local histogram id")
+        self._eng._check(self._eng.lib.lh_graph_recorder_ingest(self._eng.h, C.byref(self.g), arr, n, _capture_stream(stream)))
+
+    def close(self, stream=None):
+        """Final drain into the current interval on `stream` (None = torch's current stream), then the rows are freed."""
+        if self._open:
+            self._open = False
+            self._eng._check(self._eng.lib.lh_graph_recorder_destroy(self._eng.h, C.byref(self.g), _capture_stream(stream)))
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+
 class Engine:
     def __init__(self, device: int = 0, max_histograms: int = 1, max_counters: int = 1,
                  staging_bytes: int = 0, staging_slots: int = 0, precision: int = 0):
@@ -325,14 +394,8 @@ class Engine:
         (histogram id, array) pairs; the array is a CUDA torch tensor, a DeviceArray or a __cuda_array_interface__
         object, contiguous, float64 (Histogram samples) or int64 (Timer nanoseconds).  TypeError before the call for
         anything else."""
-        items = list(items)
-        arr = (L.lh_batch_item * max(len(items), 1))()
-        for i, (hid, a) in enumerate(items):
-            ptr, n, kind = _batch_array(a)
-            if not 0 <= int(hid) < 1 << 32:
-                raise ValueError(f"histogram id {hid} is not a uint32")
-            arr[i] = L.lh_batch_item(ptr, n, int(hid), kind)
-        self._check(self.lib.lh_ingest_batch(self.h, arr, len(items), _stream(stream)))
+        arr, n = _batch_items(items, "histogram id")
+        self._check(self.lib.lh_ingest_batch(self.h, arr, n, _stream(stream)))
 
     def counter_add_u16(self, d_ids, d_amounts, n: int, stream=None):
         self._check(self.lib.lh_counter_add_u16(self.h, _ptr(d_ids), _ptr(d_amounts), n, _stream(stream)))
@@ -414,6 +477,12 @@ class Engine:
             yield rec
         finally:
             self.record_end(rec)
+
+    def graph_recorder(self, hist_ids=(), counter_ids=()) -> "GraphRecorder":
+        """A recorder for kernels captured into CUDA graphs (lh_graph_recorder_create): local histogram row i drains
+        into histogram id hist_ids[i] of the interval at every snapshot_begin, local counter i into counter_ids[i]
+        (LH_GRAPH_UNBOUND: dropped and counted).  Usable as a context manager that closes it on exit."""
+        return GraphRecorder(self, hist_ids, counter_ids)
 
     # ---- GPU timers (StartTimer / Stop with both ends on the device)
     def gpu_timer_start(self, stream=None) -> L.lh_gpu_timer:

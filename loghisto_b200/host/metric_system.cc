@@ -28,8 +28,20 @@
 #pragma weak lh_gpu_timer_start
 #pragma weak lh_gpu_timer_stop
 #pragma weak lh_gpu_timer_release
+// And for graph recorders: over a build without them, NewGraphRecorder throws.
+#pragma weak lh_graph_recorder_create
+#pragma weak lh_graph_recorder_bind
+#pragma weak lh_graph_recorder_ingest
+#pragma weak lh_graph_recorder_destroy
 
 namespace loghisto {
+
+// an open graph recorder, shared by its GraphRecorder and the system's list of open recorders
+struct GraphRecorder::State {
+    MetricSystem *ms;                   // nullptr once closed (or once the system is gone)
+    lh_graph_recorder g{};
+    std::vector<std::string> hnames, cnames;
+};
 
 namespace {
 
@@ -402,6 +414,10 @@ MetricSystem::~MetricSystem() {
     }
     try { Stop(); } catch (...) {}
     if (reaper_thread_.joinable()) reaper_thread_.join();
+    {   // recorders left open are freed by lh_destroy; their objects only forget the system
+        std::lock_guard<std::mutex> lk(graph_mu_);
+        for (auto &g : graphs_) g->ms = nullptr;
+    }
     lh_destroy(ctx_);
 }
 
@@ -425,29 +441,37 @@ bool MetricSystem::intern(NameTable &t, const char *p, size_t n, uint32_t *id, u
         }
     }
     std::unique_lock<std::shared_mutex> wl(t.mu);
+    *id = intern_locked(t, name);
+    if (*id == RecordScope::kUnbound) return false;
+    *gen = t.gen[*id].load(std::memory_order_relaxed);
+    return true;
+}
+
+// The write-locked half of intern: the name's id, revived or taken from the free ids, live and used this interval;
+// RecordScope::kUnbound when no id is free.
+uint32_t MetricSystem::intern_locked(NameTable &t, const std::string &name) {
+    uint32_t id;
     auto it = t.ids.find(name);
     if (it != t.ids.end()) {
-        *id = it->second;
-        if (t.state[*id] == kRetiring) { t.state[*id] = kLive; t.used[*id] = 1; }
+        id = it->second;
     } else {
         if (!t.free_ids.empty()) {
-            *id = t.free_ids.back();
+            id = t.free_ids.back();
             t.free_ids.pop_back();
-            t.names[*id] = name;
+            t.names[id] = name;
         } else if (t.names.size() < t.capacity) {
-            *id = (uint32_t)t.names.size();
+            id = (uint32_t)t.names.size();
             t.names.push_back(name);
             t.state.push_back(kFree);
             t.used.push_back(0);
         } else {
-            return false;
+            return RecordScope::kUnbound;
         }
-        t.ids.emplace(name, *id);
-        t.state[*id] = kLive;
-        t.used[*id] = 1;
+        t.ids.emplace(name, id);
     }
-    *gen = t.gen[*id].load(std::memory_order_relaxed);
-    return true;
+    t.state[id] = kLive;
+    t.used[id] = 1;
+    return id;
 }
 
 // The id lifecycle step of collectRawMetrics, with t.mu held for writing (NameTable).  touched[id]: a sample or
@@ -728,6 +752,86 @@ void RecordScope::Histograms(const std::vector<Item> &items) {
     ms_->dropped_over_limit_.fetch_add(unbound, std::memory_order_relaxed);
 }
 
+// ---- graph recorders -------------------------------------------------------------------------------------------
+// Interns (or revives) every name of an open recorder, marking it used in this interval so that it keeps its id while
+// the recorder is open, and binds the rows to the ids; with graph_mu_ held.  Each drain (lh_snapshot_begin of
+// collectRawMetrics, lh_graph_recorder_destroy of Close) follows a call of this in the same collection or Close, so the
+// ids it drains into are live in the interval it drains into, and that interval's collection labels them with these
+// names.
+void MetricSystem::bind_graph(GraphRecorder::State &g) {
+    std::vector<uint32_t> hids(g.hnames.size()), cids(g.cnames.size());
+    {
+        std::unique_lock<std::shared_mutex> wl(histos_.mu);
+        for (size_t i = 0; i < hids.size(); i++) hids[i] = intern_locked(histos_, g.hnames[i]);
+    }
+    {
+        std::unique_lock<std::shared_mutex> wl(counters_.mu);
+        for (size_t i = 0; i < cids.size(); i++) cids[i] = intern_locked(counters_, g.cnames[i]);
+    }
+    if (g.g.handle)
+        check(ctx_, lh_graph_recorder_bind(ctx_, &g.g, hids.data(), cids.data()), "lh_graph_recorder_bind");
+    else
+        check(ctx_, lh_graph_recorder_create(ctx_, (uint32_t)hids.size(), (uint32_t)cids.size(), hids.data(), cids.data(), &g.g),
+              "lh_graph_recorder_create");
+}
+
+GraphRecorder MetricSystem::NewGraphRecorder(const std::vector<std::string> &histograms, const std::vector<std::string> &counters) {
+    if (!lh_graph_recorder_create || !lh_graph_recorder_bind || !lh_graph_recorder_ingest || !lh_graph_recorder_destroy)
+        throw std::runtime_error("NewGraphRecorder: this libloghisto_b200 has no graph recorders");
+    auto st = std::make_shared<GraphRecorder::State>();
+    st->ms = this;
+    st->hnames = histograms;
+    st->cnames = counters;
+    std::lock_guard<std::mutex> lk(graph_mu_);
+    bind_graph(*st);
+    graphs_.push_back(st);
+    GraphRecorder g;
+    g.st_ = std::move(st);
+    return g;
+}
+
+const lh_recorder &GraphRecorder::recorder() const {
+    if (!st_) throw std::runtime_error("GraphRecorder::recorder of a closed recorder");
+    return st_->g.rec;
+}
+
+void GraphRecorder::Histograms(const std::vector<Item> &items, void *stream) {
+    if (!st_ || !st_->ms) throw std::runtime_error("GraphRecorder::Histograms of a closed recorder");
+    std::vector<lh_batch_item> batch;
+    batch.reserve(items.size());
+    for (const Item &it : items) {
+        if (it.name >= st_->hnames.size()) throw std::out_of_range("GraphRecorder::Histograms: no such histogram name");
+        batch.push_back(lh_batch_item{it.d_values, (uint64_t)it.n, (uint32_t)it.name, it.kind});
+    }
+    MetricSystem *ms = st_->ms;
+    check(ms->ctx_, lh_graph_recorder_ingest(ms->ctx_, &st_->g, batch.data(), (uint32_t)batch.size(), stream),
+          "lh_graph_recorder_ingest");
+}
+
+void GraphRecorder::Close(void *stream) {
+    if (!st_) return;
+    std::shared_ptr<State> st = std::move(st_);
+    MetricSystem *ms = st->ms;
+    if (!ms) return;
+    std::lock_guard<std::mutex> lk(ms->graph_mu_);
+    auto &v = ms->graphs_;
+    v.erase(std::remove(v.begin(), v.end(), st), v.end());
+    st->ms = nullptr;
+    ms->bind_graph(*st);   // the final drain's ids are used in the interval it drains into
+    check(ms->ctx_, lh_graph_recorder_destroy(ms->ctx_, &st->g, stream), "lh_graph_recorder_destroy");
+}
+
+GraphRecorder &GraphRecorder::operator=(GraphRecorder &&o) noexcept {
+    if (this != &o) {
+        try { Close(); } catch (...) {}
+        st_ = std::move(o.st_);
+    }
+    return *this;
+}
+GraphRecorder::~GraphRecorder() {
+    try { Close(); } catch (...) {}
+}
+
 // ---- GPU timers ------------------------------------------------------------------------------------------------
 void *const GpuTimerToken::kStartStream = reinterpret_cast<void *>(~(uintptr_t)0);
 
@@ -828,6 +932,10 @@ std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
     for (auto &s : shards_) flush_shard(*s, &touched);
     for (size_t c = 0; c < carried_touched_.size(); c++) touched[c] |= carried_touched_[c];
     carried_touched_.clear();
+    {   // the drain in lh_snapshot_begin moves graph recorders' counts under the ids their names have now
+        std::lock_guard<std::mutex> lk(graph_mu_);
+        for (auto &g : graphs_) bind_graph(*g);
+    }
     if (const lh_status st = lh_snapshot_begin(ctx_); st != LH_OK) {   // the marks stay for the next collection
         carried_touched_ = std::move(touched);
         check(ctx_, st, "lh_snapshot_begin");
@@ -1323,6 +1431,43 @@ LHMS_API int lhms_gpu_timer_stop(void *token, void *stream, int64_t *d_duration_
     try { static_cast<GpuTimerToken *>(token)->Stop(stream, d_duration_ns); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
 }
 LHMS_API void lhms_gpu_timer_free(void *token) { delete static_cast<GpuTimerToken *>(token); }
+// MetricSystem::NewGraphRecorder: a GraphRecorder handle (NULL with *status set on failure); *out receives its
+// recorder.  Free it with lhms_graph_recorder_free, which closes it if lhms_graph_recorder_close has not.
+LHMS_API void *lhms_graph_recorder_new(void *ms, uint32_t n_h, const char *const *h_names, uint32_t n_c,
+                                       const char *const *c_names, lh_recorder *out, int *status) {
+    int dummy;
+    if (!status) status = &dummy;
+    *status = LH_ERR_INVALID;
+    if (!ms || !out || (n_h && !h_names) || (n_c && !c_names)) return nullptr;
+    try {
+        std::vector<std::string> hs(h_names, h_names + n_h), cs(c_names, c_names + n_c);
+        auto *g = new GraphRecorder(static_cast<MetricSystem *>(ms)->NewGraphRecorder(hs, cs));
+        *out = g->recorder();
+        *status = LH_OK;
+        return g;
+    } catch (const std::exception &e) {
+        *status = scope_status(e);
+        return nullptr;
+    }
+}
+// GraphRecorder::Histograms: item i is n[i] samples of kind kinds[i] at d_values[i] under histogram name name_index[i].
+LHMS_API int lhms_graph_recorder_histograms(void *g, const uint32_t *name_index, const void *const *d_values,
+                                            const uint64_t *n, const uint32_t *kinds, uint32_t n_items, void *stream) {
+    if (!g || (n_items && (!name_index || !d_values || !n || !kinds))) return LH_ERR_INVALID;
+    try {
+        std::vector<GraphRecorder::Item> items(n_items);
+        for (uint32_t i = 0; i < n_items; i++) items[i] = GraphRecorder::Item{name_index[i], d_values[i], (size_t)n[i], kinds[i]};
+        static_cast<GraphRecorder *>(g)->Histograms(items, stream);
+        return LH_OK;
+    } catch (const std::exception &e) {
+        return scope_status(e);
+    }
+}
+LHMS_API int lhms_graph_recorder_close(void *g, void *stream) {
+    if (!g) return LH_ERR_INVALID;
+    try { static_cast<GraphRecorder *>(g)->Close(stream); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
+}
+LHMS_API void lhms_graph_recorder_free(void *g) { delete static_cast<GraphRecorder *>(g); }
 LHMS_API void lhms_start(void *ms) { static_cast<MetricSystem *>(ms)->Start(); }
 LHMS_API void lhms_stop(void *ms) { static_cast<MetricSystem *>(ms)->Stop(); }
 LHMS_API uint64_t lhms_dropped(void *ms) { return static_cast<MetricSystem *>(ms)->dropped_samples(); }

@@ -201,6 +201,54 @@ class GpuTimerToken {
     bool held_ = false;
 };
 
+// Recording from kernels captured into CUDA graphs, under names (MetricSystem::NewGraphRecorder).  The recorder owns its
+// rows (lh_graph_recorder_create), so a captured kernel may be replayed any number of times, in any interval; every
+// collection drains what the replays recorded so far into the interval it collects, labelled with the recorder's names.
+//
+//   loghisto::GraphRecorder g = ms.NewGraphRecorder({"step_latency", "logit_max"}, {"tokens"});
+//   cudaStreamBeginCapture(stream, cudaStreamCaptureModeGlobal);
+//   kernel<<<grid, block, 0, stream>>>(g.recorder(), /* histogram "step_latency" = local id */ 0, ...);
+//   g.Histograms({{1, d_logits, n, LH_VALUES_F64}}, stream);   // optional: device arrays, captured too
+//   cudaStreamEndCapture(stream, &graph);  ...  cudaGraphLaunch(exec, stream);   // any number of times
+//   g.Close(stream);   // once no replay is pending; also on destruction
+//
+// The local id of histogram name i is i, and of counter name i is i.  While the recorder is open its names keep their
+// ids (they count as used in every interval).  A name that finds no free id at a collection is unbound there: what the
+// replays recorded under it since the previous drain is dropped and counted in dropped_samples() (for a counter, its
+// amount).  Close the recorder before the MetricSystem is destroyed.
+class GraphRecorder {
+ public:
+    GraphRecorder() = default;
+    GraphRecorder(GraphRecorder &&o) noexcept { *this = std::move(o); }
+    GraphRecorder &operator=(GraphRecorder &&o) noexcept;
+    GraphRecorder(const GraphRecorder &) = delete;
+    GraphRecorder &operator=(const GraphRecorder &) = delete;
+    ~GraphRecorder();
+
+    const lh_recorder &recorder() const;
+    // lh_graph_recorder_ingest on `stream`: n samples at d_values (8-byte aligned device memory) under histogram name
+    // `name` (its index), of kind LH_VALUES_F64 or LH_VALUES_I64NS.  Kernels only, so it may be captured.  Throws
+    // std::out_of_range for a bad index before anything is issued, std::runtime_error when the library refuses the call
+    // or the recorder is closed.
+    struct Item {
+        size_t name;
+        const void *d_values;
+        size_t n;
+        uint32_t kind;
+    };
+    void Histograms(const std::vector<Item> &items, void *stream);
+    // Drains what the recorder still holds into the current interval, on `stream`, and frees it (stream-ordered).
+    // Idempotent.
+    void Close(void *stream = nullptr);
+    bool open() const { return st_ != nullptr; }
+
+    struct State;
+
+ private:
+    friend class MetricSystem;
+    std::shared_ptr<State> st_;
+};
+
 struct Options {
     int device = 0;
     uint32_t max_histograms = 1024;
@@ -240,6 +288,10 @@ class MetricSystem {
     // a full name table never makes it fail.
     RecordScope BeginRecording(void *stream, const std::vector<std::string> &histograms,
                                const std::vector<std::string> &counters);
+    // A recorder for kernels captured into CUDA graphs, with these names (GraphRecorder).  Call it outside any stream
+    // capture.  Throws std::runtime_error when the library refuses lh_graph_recorder_create (e.g. more names than
+    // max_histograms / max_counters); a full name table never makes it fail.
+    GraphRecorder NewGraphRecorder(const std::vector<std::string> &histograms, const std::vector<std::string> &counters);
     void RegisterGaugeFunc(const std::string &name, std::function<double()> f);   // :299
     void DeregisterGaugeFunc(const std::string &name);                    // :306
     void Start();                                                         // :644
@@ -309,6 +361,12 @@ class MetricSystem {
     std::mutex scope_mu_;
     std::unordered_map<std::thread::id, uint32_t> scope_threads_;   // open scopes per opening thread
     std::vector<uint8_t> carried_touched_;   // touched-counter marks of a collection that lh_snapshot_begin refused
+    // graph recorders (NewGraphRecorder)
+    friend class GraphRecorder;
+    uint32_t intern_locked(NameTable &t, const std::string &name);
+    void bind_graph(GraphRecorder::State &g);
+    std::mutex graph_mu_;
+    std::vector<std::shared_ptr<GraphRecorder::State>> graphs_;   // open recorders
 
     lh_ctx *ctx_ = nullptr;
     std::chrono::nanoseconds interval_;

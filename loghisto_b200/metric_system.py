@@ -10,7 +10,7 @@ import ctypes as C
 
 from . import _lib as _L
 from . import build as _build
-from .engine import _batch_array, _stream, _timer_stream
+from .engine import _batch_array, _capture_stream, _stream, _timer_stream
 
 _EMIT = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_char_p, C.c_int, C.c_uint64, C.c_double)
 _lib = None
@@ -78,6 +78,13 @@ def _bind(L):
     L.lhms_gpu_timer_stop.restype = C.c_int
     L.lhms_gpu_timer_stop.argtypes = [vp, vp, vp]
     L.lhms_gpu_timer_free.argtypes = [vp]
+    L.lhms_graph_recorder_new.restype = vp
+    L.lhms_graph_recorder_new.argtypes = [vp, C.c_uint32, names, C.c_uint32, names, rec, C.POINTER(C.c_int)]
+    L.lhms_graph_recorder_histograms.restype = C.c_int
+    L.lhms_graph_recorder_histograms.argtypes = [vp, u32p, C.POINTER(vp), C.POINTER(C.c_uint64), u32p, C.c_uint32, vp]
+    L.lhms_graph_recorder_close.restype = C.c_int
+    L.lhms_graph_recorder_close.argtypes = [vp, vp]
+    L.lhms_graph_recorder_free.argtypes = [vp]
     for kind in ("processed", "raw"):
         getattr(L, "lhms_subscribe_" + kind).restype = vp
         getattr(L, "lhms_subscribe_" + kind).argtypes = [vp, C.c_int]
@@ -224,6 +231,64 @@ class RecordScope:
                 raise RuntimeError("lhms_record_end failed (status %d)" % st)
 
 
+class GraphRecorder:
+    """A graph recorder of a MetricSystem (MetricSystem.graph_recorder).  `recorder` is the lh_recorder to pass by value
+    to kernels captured into CUDA graphs; `histogram_ids` / `counter_ids` map each name to the local id those kernels
+    record under (its position in the list).  Every collection drains what the replays recorded so far into the
+    interval it collects, under the names."""
+
+    def __init__(self, ms, histograms, counters):
+        self._ms = ms
+        self._hnames, cnames = [str(x) for x in histograms], [str(x) for x in counters]
+        self.recorder = _L.lh_recorder()
+        hn = (C.c_char_p * max(len(self._hnames), 1))(*[x.encode() for x in self._hnames])
+        cn = (C.c_char_p * max(len(cnames), 1))(*[x.encode() for x in cnames])
+        st = C.c_int()
+        self._h = ms._lib.lhms_graph_recorder_new(ms._h, len(self._hnames), hn, len(cnames), cn,
+                                                 C.byref(self.recorder), C.byref(st))
+        if not self._h:
+            raise RuntimeError("lhms_graph_recorder_new failed (status %d)" % st.value)
+        self.histogram_ids = {nm: i for i, nm in enumerate(self._hnames)}
+        self.counter_ids = {nm: i for i, nm in enumerate(cnames)}
+
+    def histograms(self, arrays, stream=None):
+        """Histogram(name, v) for every element of several device arrays (lh_graph_recorder_ingest): `arrays` as
+        RecordScope.histograms takes them.  Kernels only, on `stream` (None = torch's current stream), so inside
+        torch.cuda.graph the call is captured and every replay records the arrays' contents at that time."""
+        pairs = list(arrays.items()) if isinstance(arrays, dict) else list(arrays)
+        k = max(len(pairs), 1)
+        idx, ptrs, ns, kinds = (C.c_uint32 * k)(), (C.c_void_p * k)(), (C.c_uint64 * k)(), (C.c_uint32 * k)()
+        for i, (name, a) in enumerate(pairs):
+            if name not in self.histogram_ids:
+                raise KeyError("%r is not a histogram of this recorder" % (name,))
+            idx[i] = self.histogram_ids[name]
+            ptrs[i], ns[i], kinds[i] = _batch_array(a)
+        if self._h is None:
+            raise RuntimeError("the graph recorder is closed")
+        st = self._ms._lib.lhms_graph_recorder_histograms(self._h, idx, ptrs, ns, kinds, len(pairs), _capture_stream(stream))
+        if st != 0:
+            raise RuntimeError("lhms_graph_recorder_histograms failed (status %d)" % st)
+
+    def close(self, stream=None):
+        """Drains what the recorder holds into the current interval on `stream` (None = torch's current stream) and
+        frees it.  No replay that uses it may be pending.  Idempotent."""
+        if self._h is None:
+            return
+        h, self._h = self._h, None
+        st = 0
+        if self._ms._h:   # a closed MetricSystem already freed the recorder
+            st = self._ms._lib.lhms_graph_recorder_close(h, _capture_stream(stream))
+        self._ms._lib.lhms_graph_recorder_free(h)
+        if st != 0:
+            raise RuntimeError("lhms_graph_recorder_close failed (status %d)" % st)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class Subscription:
     def __init__(self, ms, kind, capacity):
         self._ms, self._kind = ms, kind
@@ -344,6 +409,18 @@ class MetricSystem:
             yield scope
         finally:
             scope.end()
+
+    @contextlib.contextmanager
+    def graph_recorder(self, histograms=(), counters=()):
+        """`with ms.graph_recorder(histograms=[...], counters=[...]) as g:` -- a recorder for kernels captured into CUDA
+        graphs (GraphRecorder), closed on exit (on torch's current stream).  Create it outside the capture; inside, pass
+        g.recorder to captured kernels with ids from g.histogram_ids / g.counter_ids, or capture g.histograms(...).
+        Leave the block only once no replay that uses it is pending."""
+        g = GraphRecorder(self, histograms, counters)
+        try:
+            yield g
+        finally:
+            g.close()
 
     def RegisterConstantGauge(self, name: str, value: float):
         self._lib.lhms_register_constant_gauge(self._h, name.encode(), float(value))

@@ -56,6 +56,16 @@ with lh.Engine(device=0, max_histograms=4, max_counters=4) as e:    # few histog
     e.ingest_keyed_f64_u16(ids, d, n)
     red, sp2 = e.snapshot(PS)
     assert int(red.counts.sum()) == n
+with lh.Engine(device=0, max_histograms=4, max_counters=4) as e:    # graph recorder: batch ingest into its rows, drains
+    d = e.gen_stream(lh.STREAM_S, n, lh.DEFAULT_SEED)
+    with e.graph_recorder([2, 3, 0xFFFFFFFF], [1]) as g:      # local row 2 unbound: dropped and counted
+        g.ingest([(0, View(d.ptr, n)), (1, View(d.offset(1), 5_000)), (2, View(d.offset(2), 700))], stream=0)
+        red, _ = e.snapshot(PS)                          # collection drain: window and full rows, one unbound row
+        assert int(red.counts[2]) == n and int(red.counts[3]) == 5_000
+        g.ingest([(1, View(d.ptr, 3_000))], stream=0)
+        g.close(stream=0)                                # final drain
+    red, _ = e.snapshot(PS)
+    assert int(red.counts[3]) == 3_000
 # two contexts on one device: the peer all-reduce kernel
 engs = [lh.Engine(device=0, max_histograms=3, max_counters=2) for _ in range(2)]
 handles = b"".join(x.comm_export() for x in engs)
