@@ -438,6 +438,27 @@ LH_API lh_status lh_fastpath_margin(lh_ctx *ctx, const double *d_values, size_t 
 /* the same per estimator (1: fast_candidate, 2: the packed-FP32 form of the single-histogram kernels), for the
  * inputs of the last lh_fastpath_margin call */
 LH_API lh_status lh_fastpath_margin_detail(lh_ctx *ctx, double *h_err_estimator1, double *h_err_estimator2);
+/* Exhaustive check of the FP32 estimate behind every fast path, on the device, at every precision of
+ * [p_lo, p_hi] (1 <= p_lo <= p_hi <= LH_MAX_PRECISION; independent of the context's own precision).  Every cell of
+ * x = 1+|v| in [1, 2^64) (biased exponent, top 23 mantissa bits: the estimate depends on nothing else) is fed with
+ * both signs through each shipped form of the estimate and compared with FP64 P*ln at both ends of the cell.
+ * h_out[(p - p_lo) * 4 + form], form 0: fast_candidate (keyed vec / scalar kernels, fix-ups, device API),
+ * 1: the packed form of the single-histogram kernels with the sign folded into the slot, 2: the same with negatives
+ * flagged (also the few-histogram keyed kernel), 3: the slot-index form of the write-combining keyed kernel.
+ * A correct form has wrong == out_of_range == unflagged_outside == over_flagged == input_mismatch == 0. */
+typedef struct lh_certify_form {
+    uint64_t samples;            /* samples inside the window (x < 2^63; v >= 0 for forms 2 and 3) */
+    uint64_t flagged;            /* ... of them sent to the exact path */
+    uint64_t wrong;              /* unflagged, and some double of the cell is not in the returned bucket, or lies
+                                  * within 2^-30 bucket units of its boundary */
+    uint64_t out_of_range;       /* unflagged, with a slot outside the window's sub-histogram */
+    uint64_t unflagged_outside;  /* unflagged although outside the window (x >= 2^63; v < 0 for forms 2 and 3) */
+    uint64_t over_flagged;       /* flagged, though farther from every bucket boundary than eps plus its error */
+    uint64_t input_mismatch;     /* inputs v for which 1+|v| did not land on the intended cell */
+    double max_err;              /* max |estimate - P*ln x| over samples with x < 2^63, bucket units */
+    double min_margin;           /* smallest distance of an unflagged cell from a bucket boundary, bucket units */
+} lh_certify_form;
+LH_API lh_status lh_fastpath_certify(lh_ctx *ctx, uint32_t p_lo, uint32_t p_hi, lh_certify_form *h_out);
 
 /* ---- synthetic streams (bench / tests; SURVEY.md section 8d) ------------- */
 /* kind: 0=U log-uniform, 1=L latency-like, 2=S signed/edge mix, 3=C constant, 4=Z heavy hitter,

@@ -93,6 +93,13 @@ class lh_gpu_timer(C.Structure):
     _fields_ = [("handle", C.c_uint64)]
 
 
+class lh_certify_form(C.Structure):
+    """One (precision, form) row of lh_fastpath_certify."""
+    _fields_ = [("samples", C.c_uint64), ("flagged", C.c_uint64), ("wrong", C.c_uint64), ("out_of_range", C.c_uint64),
+                ("unflagged_outside", C.c_uint64), ("over_flagged", C.c_uint64), ("input_mismatch", C.c_uint64),
+                ("max_err", C.c_double), ("min_margin", C.c_double)]
+
+
 LH_GRAPH_UNBOUND = 0xFFFFFFFF   # target id of a graph recorder row whose drained counts are dropped and counted
 
 
@@ -156,6 +163,7 @@ SIGNATURES = {
     "lh_decompress_table": (_i32, [_vp, _vp]),
     "lh_fastpath_margin": (_i32, [_vp, _vp, _sz, C.POINTER(C.c_double), C.POINTER(_u64), _vp]),
     "lh_fastpath_margin_detail": (_i32, [_vp, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
+    "lh_fastpath_certify": (_i32, [_vp, _u32, _u32, C.POINTER(lh_certify_form)]),
     "lh_gen_stream_f64": (_i32, [_vp, C.c_int, _u64, _u64, _sz, _vp, _vp]),
     "lh_gen_ids_u16": (_i32, [_vp, C.c_int, _u64, _u64, _sz, _u32, _vp, _vp]),
     "lh_get_stats": (_i32, [_vp, C.POINTER(lh_stats)]),

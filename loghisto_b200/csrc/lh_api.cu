@@ -2277,6 +2277,31 @@ extern "C" lh_status lh_fastpath_margin_detail(lh_ctx *ctx, double *h_err_estima
     return LH_OK;
 }
 
+// every cell of the fast window at every precision of [p_lo, p_hi], one launch of k_fastpath_certify per precision
+extern "C" lh_status lh_fastpath_certify(lh_ctx *ctx, uint32_t p_lo, uint32_t p_hi, lh_certify_form *h_out) {
+    LH_ENTER(ctx);
+    static_assert(sizeof(lh_certify_form) == FC_FIELDS * 8, "lh_certify_form mirrors the FC_* words");
+    if (!h_out) return fail(ctx, LH_ERR_INVALID, "h_out is NULL");
+    if (p_lo < 1 || p_hi > LH_MAX_PRECISION || p_lo > p_hi) return fail(ctx, LH_ERR_RANGE, "precisions must satisfy 1 <= p_lo <= p_hi <= 250");
+    const size_t rows = (size_t)(p_hi - p_lo + 1) * FC_FORMS;
+    std::vector<unsigned long long> h(rows * FC_FIELDS, 0ull);
+    for (size_t r = 0; r < rows; r++) h[r * FC_FIELDS + FC_MIN_MARGIN] = 0x7FF0000000000000ull;   // +Inf
+    cudaStream_t s = ctx->ingest_stream;
+    unsigned long long *d = nullptr;
+    LH_CUDA(ctx, cudaMalloc(&d, h.size() * 8));
+    cudaError_t e = cudaMemcpyAsync(d, h.data(), h.size() * 8, cudaMemcpyHostToDevice, s);
+    for (uint32_t p = p_lo; p <= p_hi && e == cudaSuccess; p++) {
+        k_fastpath_certify<<<ctx->sm_count * 8, FC_THREADS, 0, s>>>(d + (size_t)(p - p_lo) * FC_FORMS * FC_FIELDS, make_prec(p));
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h.data(), d, h.size() * 8, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    cudaFree(d);
+    if (e != cudaSuccess) return fail(ctx, LH_ERR_CUDA, "lh_fastpath_certify", e);
+    memcpy(h_out, h.data(), h.size() * 8);
+    return LH_OK;
+}
+
 // =========================================================== streams
 extern "C" lh_status lh_gen_stream_f64(lh_ctx *ctx, int kind, uint64_t seed, uint64_t start, size_t n, double *d_out, void *stream) {
     LH_ENTER(ctx);

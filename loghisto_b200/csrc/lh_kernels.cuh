@@ -22,8 +22,8 @@
 //                               (lh_reduce_sparse_host)
 //   k_ingest_batch          many device arrays under many ids (lh_ingest_batch, lh_graph_recorder_ingest)
 //   k_graph_drain           graph recorders' rows -> the interval being frozen (lh_snapshot_begin)
-//   misc k_clear_touched, k_fill_decompress, k_compress_probe, k_fastpath_margin, k_stream_probe, k_gen_stream,
-//        k_gen_ids_u16
+//   misc k_clear_touched, k_fill_decompress, k_compress_probe, k_fastpath_margin, k_fastpath_certify, k_stream_probe,
+//        k_gen_stream, k_gen_ids_u16
 //
 // Per-histogram flags (uint32[H], one array per bucket buffer): 0 = untouched since the buffer was cleared,
 // 1 = counts inside the fast window only, 3 = some count outside it.  Every kernel that adds into the uint64
@@ -188,13 +188,17 @@ k_ingest_single_ldg(const double *__restrict__ vals32, size_t nvec, const double
 //   * the sign of v is folded into the slot (negative values land in [win, 2*win)) instead of being flagged, so a
 //     stream with many negative durations (readme.md:43) stays on the fast path;
 //   * the shared-memory byte offset is built as eb*a4 + (rounded bits << 2) + const: one IMAD and one LEA.
-// Extra estimate error vs fast_candidate(): the float constant -1023*c2 (|err| <= 1.6e-5 bucket units at
-// precision 100), still well inside eps.
+// Extra estimate error vs fast_candidate(): the float constant -1023*c2, at most half an ulp of a float below 1024:
+// <= 1.53e-5 bucket units at precision 100 (|1023*c2| = 321.9), <= 3.1e-5 at any precision.  Certified worst case of
+// this form over every input and precision 1..250: 6.69e-5 (fast_candidate: 4.61e-5), eps at least 5.2 times that
+// (lh_fastpath_certify).
 // FOLD_SIGN = false: positive-only layout (rows of `win` slots); negative samples are flagged instead.
 // SHIFT = 2: byte offsets into a uint32 sub-histogram; SHIFT = 0: slot indices.
+// est[i]: the FP32 part of sample i's estimate, precision*ln(1+|v|) ~= (eb - 1023) * a_int + est (as fast_candidate's w;
+// k_fastpath_certify reads it, the kernels use the form without it).
 template <int NS, bool FOLD_SIGN, int SHIFT = 2>
 __device__ __forceinline__ void bucket_offsets_v2(const double (&v)[NS], const Prec &pc, uint32_t one_bits,
-                                                  uint32_t (&off)[NS], bool (&flag)[NS]) {
+                                                  uint32_t (&off)[NS], bool (&flag)[NS], float (&est)[NS]) {
     static_assert(NS % 2 == 0, "pairs");
     constexpr float MAGIC = 12582912.0f;
     const uint32_t negoff = pc.win << SHIFT;
@@ -215,6 +219,7 @@ __device__ __forceinline__ void bucket_offsets_v2(const double (&v)[NS], const P
         const float2 ef = make_float2(__uint2float_rn(e0), __uint2float_rn(e1));
         const float2 a = make_float2(__fmaf_rn(ef.x, pc.c2, pc.kb), __fmaf_rn(ef.y, pc.c2, pc.kb));
         const float2 w = make_float2(__fmaf_rn(lg.x, pc.c1, a.x), __fmaf_rn(lg.y, pc.c1, a.y));
+        est[i] = w.x; est[i + 1] = w.y;
         const float2 r = make_float2(__fadd_rn(w.x, MAGIC), __fadd_rn(w.y, MAGIC));
         const float2 s = make_float2(__fadd_rn(r.x, -MAGIC), __fadd_rn(r.y, -MAGIC));
         const float2 d = make_float2(__fmaf_rn(s.x, -1.0f, w.x), __fmaf_rn(s.y, -1.0f, w.y));   // w - s, one rounding
@@ -232,6 +237,12 @@ __device__ __forceinline__ void bucket_offsets_v2(const double (&v)[NS], const P
             off[i + 1] = e1 * am + (__float_as_uint(r.y) << SHIFT) + cm;
         }
     }
+}
+template <int NS, bool FOLD_SIGN, int SHIFT = 2>
+__device__ __forceinline__ void bucket_offsets_v2(const double (&v)[NS], const Prec &pc, uint32_t one_bits,
+                                                  uint32_t (&off)[NS], bool (&flag)[NS]) {
+    float est[NS];
+    bucket_offsets_v2<NS, FOLD_SIGN, SHIFT>(v, pc, one_bits, off, flag, est);
 }
 
 template <int NS, bool FOLD_SIGN>
@@ -1852,6 +1863,163 @@ __global__ void k_fastpath_margin(const double *__restrict__ v, size_t n, unsign
         float a = __fmaf_rn(__uint2float_rn(eb), pc.c2, pc.kb);
         float w = __fmaf_rn(lg, pc.c1, a);
         atomicMax(&out[2], (unsigned long long)__double_as_longlong(fabs(base + (double)w - truth)));
+    }
+}
+
+// Exhaustive certification of the fast path at one precision (lh_fastpath_certify; one launch per precision).
+// The forms' outputs depend on v only through its sign and the cell of x = 1+|v|: the biased exponent eb and the top
+// 23 mantissa bits t.  Every cell with eb in 1023..1086 (x in [1, 2^64)) is visited with v = X_lo - 1 and -v, X_lo
+// the cell's smallest double, through the inline functions the kernels call with the arguments they pass:
+//   form 0  fast_candidate()                  (key16_of, the keyed vec / scalar kernels, K1 ldg, the fix-ups, device API)
+//   form 1  bucket_offsets_v2<4, true, 2>     (K1 bulk, sign folded into the slot)
+//   form 2  bucket_offsets_v2<4, false, 2>    (K1 bulk, negatives flagged; k_ingest_keyed_small)
+//   form 3  bucket_offsets_v2<4, false, 0>    (k_ingest_keyed_wc)
+// and each output is decoded as the kernels decode it (slot -> key16).  The reference is FP64 log at both ends of the
+// cell, L_lo = P ln X_lo and L_hi = P ln X_hi (X_hi the next cell's X_lo); ln is monotone, so [L_lo, L_hi] holds
+// P ln x for every double of the cell.  Per form, as FC_* words of out[form * FC_FIELDS]:
+//   samples            samples inside the window: x < 2^63, and v >= 0 for the positive-only forms 2 and 3
+//   flagged            ... of them handed to the exact path
+//   wrong              unflagged, but [L_lo, L_hi] not inside (key - 0.5 + 2^-30, key + 0.5 - 2^-30): some double of
+//                      the cell could get another key than Go's (FP64 log errs by far less than 2^-30 bucket units)
+//   out_of_range       unflagged with a slot outside the sub-histogram ([0, 2 win), [0, win) for forms 2 and 3): a
+//                      shared-memory write past the window
+//   unflagged_outside  a sample outside the window (x >= 2^63; a negative one for forms 2 and 3) left unflagged
+//   over_flagged       flagged although [L_lo, L_hi] lies farther than eps + (this sample's estimate error) + 2^-20
+//                      from every half-integer: a flag the eps band does not explain
+//   input_mismatch     fl(1 + |v|) != X_lo (the same count for every form)
+//   max_err            max |estimate - L| at both ends over every sample with x < 2^63 (double bits)
+//   min_margin         min distance of an unflagged interval from a bucket boundary, floored at 0 (double bits)
+constexpr int FC_FORMS = 4;
+constexpr int FC_FIELDS = 9;
+constexpr int FC_SAMPLES = 0, FC_FLAGGED = 1, FC_WRONG = 2, FC_OUT_OF_RANGE = 3, FC_UNFLAGGED_OUTSIDE = 4,
+              FC_OVER_FLAGGED = 5, FC_INPUT_MISMATCH = 6, FC_MAX_ERR = 7, FC_MIN_MARGIN = 8;
+constexpr int FC_THREADS = 256;
+constexpr uint32_t FC_CELL_BITS = 29;        // 64 exponents x 2^23 mantissa prefixes
+constexpr uint32_t FC_RUN = 64;              // consecutive cells per thread and run: one FP64 log per cell
+
+struct FcAcc {
+    uint32_t n[FC_INPUT_MISMATCH];           // FC_SAMPLES .. FC_OVER_FLAGGED
+    double max_err, min_margin;
+};
+
+// One sample of one form.  slot = the sub-histogram slot the form produced (0xFFFFFFFF: not a slot), nslots = the
+// sub-histogram's length, pos_only = positive-only layout (slot == key), w = the FP32 part of the estimate.
+__device__ __forceinline__ void fc_account(FcAcc &a, bool flag, uint32_t slot, uint32_t nslots, bool pos_only, bool neg,
+                                           uint32_t eb, float w, double L_lo, double L_hi, double eps, const Prec &pc) {
+    const double E = (double)((int)eb - 1023) * (double)pc.a_int + (double)w;
+    const double err = fmax(fabs(E - L_lo), fabs(E - L_hi));
+    const bool in_range = eb < 1086u;                    // x < 2^63
+    if (in_range) a.max_err = fmax(a.max_err, err);
+    if (!in_range || (pos_only && neg)) {
+        if (!flag) a.n[FC_UNFLAGGED_OUTSIDE]++;
+        return;
+    }
+    a.n[FC_SAMPLES]++;
+    if (flag) {
+        a.n[FC_FLAGGED]++;
+        // distance of [L_lo, L_hi] from the nearest half-integer (the interval is far shorter than one bucket)
+        const double h0 = floor(L_lo) + 0.5, h1 = floor(L_hi) + 0.5;
+        const double dist = fmin(fmax(0.0, fmax(L_lo - h0, h0 - L_hi)), fmax(0.0, fmax(L_lo - h1, h1 - L_hi)));
+        if (dist > eps + err + 0x1p-20) a.n[FC_OVER_FLAGGED]++;
+        return;
+    }
+    if (slot >= nslots) { a.n[FC_OUT_OF_RANGE]++; return; }
+    const uint32_t key16 = pos_only ? slot : slot_to_key16(slot, pc.win);
+    const double key = (double)(short)key16, mag = neg ? -key : key;
+    const double margin = fmin(L_lo - (mag - 0.5), (mag + 0.5) - L_hi);
+    if (!(margin > 0x1p-30)) a.n[FC_WRONG]++;
+    a.min_margin = fmin(a.min_margin, fmax(margin, 0.0));
+}
+
+__global__ void __launch_bounds__(FC_THREADS)
+k_fastpath_certify(unsigned long long *__restrict__ out, Prec pc) {
+    __shared__ unsigned long long s_red[FC_FORMS][FC_FIELDS];
+    for (int i = threadIdx.x; i < FC_FORMS * FC_FIELDS; i += FC_THREADS) {
+        const int f = i % FC_FIELDS;
+        s_red[i / FC_FIELDS][f] = f == FC_MIN_MARGIN ? 0x7FF0000000000000ull : 0ull;   // +Inf: the identity of min
+    }
+    __syncthreads();
+    uint32_t one_bits;
+    asm volatile("mov.b32 %0, 0x3F800000;" : "=r"(one_bits));
+    const double eps = 0.5 - (double)pc.thresh;
+    FcAcc acc[FC_FORMS];
+#pragma unroll
+    for (int f = 0; f < FC_FORMS; f++) {
+#pragma unroll
+        for (int i = 0; i < FC_INPUT_MISMATCH; i++) acc[f].n[i] = 0;
+        acc[f].max_err = 0.0;
+        acc[f].min_margin = __longlong_as_double(0x7FF0000000000000ll);
+    }
+    uint32_t mismatch = 0;
+    const uint64_t one = 0x3FF0000000000000ull;          // X_lo of cell c: bits one + (c << 29)
+    const uint32_t nruns = (1u << FC_CELL_BITS) / FC_RUN;
+    for (uint32_t run = blockIdx.x * FC_THREADS + threadIdx.x; run < nruns; run += gridDim.x * FC_THREADS) {
+        const uint64_t c0 = (uint64_t)run * FC_RUN;
+        const uint32_t eb = 1023u + (uint32_t)(c0 >> 23);                  // a run never crosses an exponent
+        double L_prev = pc.precision * log(u64_as_f64(one + (c0 << 29)));
+        for (uint32_t j = 0; j < FC_RUN; j += 2) {                         // two cells: the forms take 4 samples
+            const uint64_t c = c0 + j;
+            const double X0 = u64_as_f64(one + (c << 29)), X1 = u64_as_f64(one + ((c + 1) << 29));
+            const double L[3] = {L_prev, pc.precision * log(X1), pc.precision * log(u64_as_f64(one + ((c + 2) << 29)))};
+            L_prev = L[2];
+            const double v0 = __dsub_rn(X0, 1.0), v1 = __dsub_rn(X1, 1.0);
+            const double v[4] = {v0, -v0, v1, -v1};
+            mismatch += 2u * ((__dadd_rn(1.0, v0) != X0) + (__dadd_rn(1.0, v1) != X1));
+            {   // form 0
+#pragma unroll
+                for (int s = 0; s < 4; s++) {
+                    uint32_t idx; bool slow; float w;
+                    fast_candidate(v[s], pc, idx, slow, w);
+                    fc_account(acc[0], slow, idx, 2u * pc.win, false, s & 1, eb, w, L[s >> 1], L[(s >> 1) + 1], eps, pc);
+                }
+            }
+            uint32_t off[4]; bool flag[4]; float est[4];
+            bucket_offsets_v2<4, true, 2>(v, pc, one_bits, off, flag, est);
+#pragma unroll
+            for (int s = 0; s < 4; s++)
+                fc_account(acc[1], flag[s], (off[s] & 3u) ? 0xFFFFFFFFu : off[s] >> 2, 2u * pc.win, false, s & 1, eb, est[s],
+                           L[s >> 1], L[(s >> 1) + 1], eps, pc);
+            bucket_offsets_v2<4, false, 2>(v, pc, one_bits, off, flag, est);
+#pragma unroll
+            for (int s = 0; s < 4; s++)
+                fc_account(acc[2], flag[s], (off[s] & 3u) ? 0xFFFFFFFFu : off[s] >> 2, pc.win, true, s & 1, eb, est[s],
+                           L[s >> 1], L[(s >> 1) + 1], eps, pc);
+            bucket_offsets_v2<4, false, 0>(v, pc, one_bits, off, flag, est);
+#pragma unroll
+            for (int s = 0; s < 4; s++)
+                fc_account(acc[3], flag[s], off[s], pc.win, true, s & 1, eb, est[s], L[s >> 1], L[(s >> 1) + 1], eps, pc);
+        }
+    }
+    // warp, then CTA, then one global atomic per word and CTA
+#pragma unroll
+    for (int f = 0; f < FC_FORMS; f++) {
+        unsigned long long w[FC_FIELDS];
+#pragma unroll
+        for (int i = 0; i < FC_INPUT_MISMATCH; i++) w[i] = acc[f].n[i];
+        w[FC_INPUT_MISMATCH] = mismatch;
+        double mx = acc[f].max_err, mn = acc[f].min_margin;
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+#pragma unroll
+            for (int i = 0; i <= FC_INPUT_MISMATCH; i++) w[i] += __shfl_xor_sync(0xFFFFFFFFu, w[i], o);
+            mx = fmax(mx, __shfl_xor_sync(0xFFFFFFFFu, mx, o));
+            mn = fmin(mn, __shfl_xor_sync(0xFFFFFFFFu, mn, o));
+        }
+        if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+            for (int i = 0; i <= FC_INPUT_MISMATCH; i++) atomicAdd(&s_red[f][i], w[i]);
+            atomicMax(&s_red[f][FC_MAX_ERR], (unsigned long long)__double_as_longlong(mx));    // both >= 0: bits order
+            atomicMin(&s_red[f][FC_MIN_MARGIN], (unsigned long long)__double_as_longlong(mn));
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x < FC_FORMS * FC_FIELDS) {
+        const int f = threadIdx.x / FC_FIELDS, i = threadIdx.x % FC_FIELDS;
+        const unsigned long long x = s_red[f][i];
+        unsigned long long *dst = out + f * FC_FIELDS + i;
+        if (i == FC_MAX_ERR) atomicMax(dst, x);
+        else if (i == FC_MIN_MARGIN) atomicMin(dst, x);
+        else if (x) atomicAdd(dst, x);
     }
 }
 

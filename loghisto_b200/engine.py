@@ -622,6 +622,13 @@ class Engine:
         self._check(self.lib.lh_fastpath_margin_detail(self.h, C.byref(a), C.byref(b)))
         return float(a.value), float(b.value)
 
+    def fastpath_certify(self, p_lo: int = 1, p_hi: int = 250) -> np.ndarray:
+        """lh_fastpath_certify: a structured array [p_hi - p_lo + 1, 4] (precision, form) with the fields of
+        lh_certify_form; row i is precision p_lo + i."""
+        out = (L.lh_certify_form * ((p_hi - p_lo + 1) * 4))() if p_hi >= p_lo else None
+        self._check(self.lib.lh_fastpath_certify(self.h, p_lo, p_hi, out))
+        return np.ctypeslib.as_array(out).reshape(p_hi - p_lo + 1, 4).copy()
+
     def gen_stream(self, kind: int, n: int, seed: int, start: int = 0, out: DeviceArray | None = None,
                    stream=None) -> DeviceArray:
         if out is None:

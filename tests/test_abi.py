@@ -40,7 +40,8 @@ def test_struct_layouts_match_header(tmp_path):
     import subprocess
     from loghisto_b200 import _lib
     structs = {"lh_config": _lib.lh_config, "lh_staging": _lib.lh_staging, "lh_device_view": _lib.lh_device_view,
-               "lh_sparse": _lib.lh_sparse, "lh_stats": _lib.lh_stats, "lh_comm_stats": _lib.lh_comm_stats}
+               "lh_sparse": _lib.lh_sparse, "lh_stats": _lib.lh_stats, "lh_comm_stats": _lib.lh_comm_stats,
+               "lh_certify_form": _lib.lh_certify_form}
     src = ['#include <stdio.h>', '#include <stddef.h>', '#include "loghisto_b200.h"', 'int main(void) {']
     for name, cls in structs.items():
         src.append('printf("%s %%zu\\n", sizeof(%s));' % (name, name))
