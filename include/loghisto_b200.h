@@ -271,6 +271,84 @@ LH_API lh_status lh_graph_recorder_ingest(lh_ctx *ctx, const lh_graph_recorder *
                                           uint32_t n_items, void *stream);
 LH_API lh_status lh_graph_recorder_destroy(lh_ctx *ctx, const lh_graph_recorder *g, void *stream);
 
+/* ---- device subscriptions: each collection's processed metrics in device memory --------------------------------
+ * SubscribeToProcessedMetrics (metrics.go:218, 508-525) for consumers on the GPU.  A board is device memory the library
+ * owns; lh_snapshot_publish writes the named rows of the open snapshot's reduction into it, on the snapshot stream,
+ * and kernels (include/loghisto_b200_device.cuh: lh::read_histogram / lh::read_counter) or lh_board_read read the
+ * latest publish from there with no host call, also from CUDA-graph replays.  A board is guarded by a seqlock:
+ * `seq` is odd while a publish writes it and advances by 2 per publish, so every read is of one publish.
+ *
+ * Layout (bytes): lh_board_header at 0, k lh_board_hist_row, then kc lh_board_counter_row.
+ *
+ *   lh_board_create      allocates a board of k histogram rows and kc counter rows (k <= max_histograms,
+ *                        kc <= max_counters, k + kc >= 1) and zeroes it: every row unbound, np = 0, publishes = 0.
+ *                        Call it outside any stream capture; it waits for the zeroing.
+ *   lh_snapshot_publish  fills every row from the most recent lh_snapshot_reduce / lh_snapshot_reduce_async of the
+ *                        open snapshot (LH_ERR_STATE without one, or outside a snapshot):
+ *                          histogram row i, hist_ids[i] = h: count, sum, avg, pkeys[0..np), pvals[0..np) bit for bit
+ *                            as that reduction reports h (the all-reduced values after lh_snapshot_allreduce), and
+ *                            present = (count != 0);
+ *                          hist_ids[i] = LH_GRAPH_UNBOUND (or hist_ids NULL): an untouched histogram as the reduction
+ *                            reports one (count 0, sum 0, avg NaN, keys INT32_MIN, values NaN), present = 0;
+ *                          counter row i, counter_ids[i] = c: rate = the interval delta lh_snapshot_export reports in
+ *                            counter_deltas[c], present = 1; LH_GRAPH_UNBOUND (or counter_ids NULL): rate 0, present 0;
+ *                            total = counter_totals[i] either way (0 when counter_totals is NULL).
+ *                        Percentile slots j >= np hold INT32_MIN / NaN.  LH_ERR_RANGE for an id >= max_histograms /
+ *                        max_counters other than LH_GRAPH_UNBOUND.  The publish is enqueued on the snapshot stream after
+ *                        that reduction (so it may follow lh_snapshot_reduce_async before lh_snapshot_result); it never
+ *                        waits and never allocates.
+ *   lh_board_read        enqueues ONE kernel on `stream` (NULL = the ingest stream) that copies a consistent image of the
+ *                        whole board (b->bytes, the board's layout, even seq) to device memory d_out (8-byte aligned).
+ *                        It only enqueues a kernel, so it may be captured into a CUDA graph: a replay copies whatever
+ *                        publish is the latest when it runs.
+ *   lh_board_destroy     frees the board, stream-ordered after every publish already issued.  The caller guarantees
+ *                        that no read of the board (lh_board_read or a kernel) is pending.  lh_destroy frees every
+ *                        board left.
+ * A destroyed or foreign handle gets LH_ERR_INVALID. */
+typedef struct lh_board_header {
+    uint64_t seq;                             /* seqlock word: odd while a publish writes, +2 per publish */
+    uint64_t publishes;                       /* publishes so far (= seq / 2 when even) */
+    uint32_t np;                              /* percentiles of the latest publish */
+    uint32_t reserved[3];
+    double percentiles[LH_MAX_PERCENTILES];   /* [0, np) of the latest publish, NaN beyond */
+} lh_board_header;
+typedef struct lh_board_hist_row {
+    uint64_t count;
+    double sum, avg;
+    uint32_t present;                         /* count != 0 */
+    uint32_t reserved;
+    double pvals[LH_MAX_PERCENTILES];         /* NaN where pkeys is INT32_MIN, and beyond np */
+    int32_t pkeys[LH_MAX_PERCENTILES];
+} lh_board_hist_row;
+typedef struct lh_board_counter_row {
+    uint64_t rate;                            /* interval delta */
+    uint64_t total;                           /* the caller's running total */
+    uint32_t present;
+    uint32_t reserved;
+} lh_board_counter_row;
+typedef struct lh_board {                     /* pass by value to kernels */
+    uint64_t handle;                          /* opaque */
+    void *d_board;                            /* device memory: header, k histogram rows, kc counter rows */
+    uint32_t k, kc;
+    uint64_t bytes;                           /* size of an image (lh_board_read) */
+} lh_board;
+#ifdef __cplusplus
+#define LH_STATIC_ASSERT(c, m) static_assert(c, m)
+#else
+#define LH_STATIC_ASSERT(c, m) _Static_assert(c, m)
+#endif
+LH_STATIC_ASSERT(sizeof(lh_board_header) == 288 && offsetof(lh_board_header, percentiles) == 32,
+                 "lh_board_header is 288 bytes: seq, publishes, np, reserved, percentiles");
+LH_STATIC_ASSERT(sizeof(lh_board_hist_row) == 416 && offsetof(lh_board_hist_row, pvals) == 32 &&
+                 offsetof(lh_board_hist_row, pkeys) == 288, "lh_board_hist_row is 416 bytes");
+LH_STATIC_ASSERT(sizeof(lh_board_counter_row) == 24, "lh_board_counter_row is 24 bytes");
+LH_STATIC_ASSERT(sizeof(lh_board) == 32, "lh_board is 32 bytes");
+LH_API lh_status lh_board_create(lh_ctx *ctx, uint32_t k, uint32_t kc, lh_board *out);
+LH_API lh_status lh_snapshot_publish(lh_ctx *ctx, const lh_board *b, const uint32_t *hist_ids,
+                                     const uint32_t *counter_ids, const uint64_t *counter_totals);
+LH_API lh_status lh_board_read(lh_ctx *ctx, const lh_board *b, void *d_out, void *stream);
+LH_API lh_status lh_board_destroy(lh_ctx *ctx, const lh_board *b);
+
 /* ---- GPU timers: StartTimer / Stop (metrics.go:232-246) from host code, timed on the device ------------------
  * Host StartTimer / Stop around CUDA work time the enqueue.  These calls put the two ends of the span on the GPU
  * instead: each end is a one-thread kernel on `stream` that reads %globaltimer (the clock of lh::start_timer), and

@@ -9,6 +9,9 @@
 //                                 StartTimer(name) / Stop()   metrics.go:232-246  durations on the GPU's clock
 //   lh::BlockHistogram            one CTA feeding one histogram through a shared-memory sub-histogram
 //   lh::BlockRecorder             one CTA feeding any number of histograms through a shared-memory combining table
+//   lh::read_histogram / lh::read_counter
+//                                 the latest collection's processed metrics of a name, from a device subscription
+//                                 board (lh_board, MetricSystem::NewDeviceSubscription)   metrics.go:218, 508-525
 //
 // `rec` is an lh_recorder (include/loghisto_b200.h) obtained from lh_record_begin on the host and passed to the kernel
 // by value.  Kernels that use it must be enqueued on the recorder's stream between lh_record_begin and lh_record_end;
@@ -474,5 +477,120 @@ class BlockRecorder {
     unsigned long long *tags_;
     uint32_t *counts_;
 };
+
+// ================================================================ reading a device subscription (lh_board)
+// A board (lh_board_create) holds the processed metrics of the latest collection that published into it: what the
+// reference hands SubscribeToProcessedMetrics subscribers (metrics.go:508-525), for kernels and CUDA-graph replays.
+//
+//   lh::HistogramStats s;
+//   if (lh::read_histogram(board, row, &s) && s.present && s.np > 2) clip = s.pvals[2];   // e.g. the p99 label
+//
+// Each read is a seqlock-consistent copy of one row: the sequence word is loaded with ld.acquire.gpu and retried while
+// odd (a publish is writing), the row with strong relaxed loads, which go to L2 (a plain load could hit an L1 line that
+// a persistent kernel cached before the latest publish), then fence.acq_rel.gpu and the word again: a changed word
+// means the row may mix two publishes, and the read is retried.  A publish is one CTA that never waits on anything, so
+// the retry loop ends as soon as it has run.  The value returned is the publish number the row belongs to (the number
+// of publishes into the board so far), 0 if nothing has been published yet.  A kernel must not wait for the next
+// publish: collections run on the host, which may never run another.
+namespace board {
+__device__ __forceinline__ unsigned long long ld_acquire(const unsigned long long *p) {
+    unsigned long long v;
+    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ unsigned long long ld_relaxed(const void *p) {
+    unsigned long long v;
+    asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ uint32_t ld_relaxed_u32(const void *p) {
+    uint32_t v;
+    asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_relaxed(void *p, unsigned long long v) {
+    asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
+}
+__device__ __forceinline__ void st_relaxed_u32(void *p, uint32_t v) {
+    asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" :: "l"(p), "r"(v) : "memory");
+}
+__device__ __forceinline__ void st_release(unsigned long long *p, unsigned long long v) {
+    asm volatile("st.release.gpu.global.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
+}
+__device__ __forceinline__ void fence_acq_rel() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
+
+__device__ __forceinline__ char *hist_row(const lh_board &b, uint32_t row) {
+    return (char *)b.d_board + sizeof(lh_board_header) + (size_t)row * sizeof(lh_board_hist_row);
+}
+__device__ __forceinline__ char *counter_row(const lh_board &b, uint32_t row) {
+    return (char *)b.d_board + sizeof(lh_board_header) + (size_t)b.k * sizeof(lh_board_hist_row) +
+           (size_t)row * sizeof(lh_board_counter_row);
+}
+// the even sequence word a consistent read starts from
+__device__ __forceinline__ unsigned long long begin_read(const lh_board &b) {
+    for (;;) {
+        const unsigned long long s = ld_acquire((const unsigned long long *)b.d_board);
+        if (!(s & 1ull)) return s;
+        __nanosleep(64);
+    }
+}
+// true when nothing was published while the loads before it ran
+__device__ __forceinline__ bool end_read(const lh_board &b, unsigned long long s) {
+    fence_acq_rel();
+    return ld_relaxed(b.d_board) == s;
+}
+}  // namespace board
+
+struct HistogramStats {          // one histogram row of the latest publish (lh_board_hist_row)
+    uint64_t count;              // the name's _count (as uint64)
+    double sum, avg;             // _sum, _avg
+    bool present;                // the name was in that collection's Histograms (count != 0)
+    uint32_t np;                 // percentile labels of that collection
+    double pvals[LH_MAX_PERCENTILES];    // value of label j, j < np; NaN where pkeys[j] is INT32_MIN (label omitted)
+    int32_t pkeys[LH_MAX_PERCENTILES];   // bucket key of label j
+};
+struct CounterStats {            // one counter row of the latest publish (lh_board_counter_row)
+    uint64_t rate;               // the name's _rate: the interval delta
+    uint64_t total;              // its running total (Counters[name]) as the publisher passed it
+    bool present;                // the name was in that collection's Rates
+};
+
+// A consistent copy of histogram row `row` (< b.k) of board b; returns its publish number (0: nothing published yet,
+// or row out of range: *out is then all zero).
+__device__ __forceinline__ uint64_t read_histogram(const lh_board &b, uint32_t row, HistogramStats *out) {
+    if (row >= b.k) { *out = HistogramStats{}; return 0; }
+    const char *r = board::hist_row(b, row);
+    for (;;) {
+        const unsigned long long s = board::begin_read(b);
+        out->np = board::ld_relaxed_u32((const char *)b.d_board + offsetof(lh_board_header, np));
+        out->count = board::ld_relaxed(r + offsetof(lh_board_hist_row, count));
+        out->sum = __longlong_as_double((long long)board::ld_relaxed(r + offsetof(lh_board_hist_row, sum)));
+        out->avg = __longlong_as_double((long long)board::ld_relaxed(r + offsetof(lh_board_hist_row, avg)));
+        out->present = board::ld_relaxed_u32(r + offsetof(lh_board_hist_row, present)) != 0;
+#pragma unroll 8
+        for (int j = 0; j < LH_MAX_PERCENTILES; j++)
+            out->pvals[j] = __longlong_as_double((long long)board::ld_relaxed(r + offsetof(lh_board_hist_row, pvals) + 8 * j));
+#pragma unroll 8
+        for (int j = 0; j < LH_MAX_PERCENTILES; j += 2) {
+            const unsigned long long two = board::ld_relaxed(r + offsetof(lh_board_hist_row, pkeys) + 4 * j);
+            out->pkeys[j] = (int32_t)(uint32_t)two;
+            out->pkeys[j + 1] = (int32_t)(uint32_t)(two >> 32);
+        }
+        if (board::end_read(b, s)) return s >> 1;
+    }
+}
+
+// A consistent copy of counter row `row` (< b.kc) of board b; returns its publish number as read_histogram does.
+__device__ __forceinline__ uint64_t read_counter(const lh_board &b, uint32_t row, CounterStats *out) {
+    if (row >= b.kc) { *out = CounterStats{}; return 0; }
+    const char *r = board::counter_row(b, row);
+    for (;;) {
+        const unsigned long long s = board::begin_read(b);
+        out->rate = board::ld_relaxed(r + offsetof(lh_board_counter_row, rate));
+        out->total = board::ld_relaxed(r + offsetof(lh_board_counter_row, total));
+        out->present = board::ld_relaxed_u32(r + offsetof(lh_board_counter_row, present)) != 0;
+        if (board::end_read(b, s)) return s >> 1;
+    }
+}
 
 }  // namespace lh

@@ -108,6 +108,29 @@ class lh_graph_recorder(C.Structure):
     _fields_ = [("handle", C.c_uint64), ("rec", lh_recorder)]
 
 
+class lh_board_header(C.Structure):
+    """Header of a device subscription board (include/loghisto_b200.h)."""
+    _fields_ = [("seq", C.c_uint64), ("publishes", C.c_uint64), ("np", C.c_uint32), ("reserved", C.c_uint32 * 3),
+                ("percentiles", C.c_double * LH_MAX_PERCENTILES)]
+
+
+class lh_board_hist_row(C.Structure):
+    _fields_ = [("count", C.c_uint64), ("sum", C.c_double), ("avg", C.c_double), ("present", C.c_uint32),
+                ("reserved", C.c_uint32), ("pvals", C.c_double * LH_MAX_PERCENTILES),
+                ("pkeys", C.c_int32 * LH_MAX_PERCENTILES)]
+
+
+class lh_board_counter_row(C.Structure):
+    _fields_ = [("rate", C.c_uint64), ("total", C.c_uint64), ("present", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+class lh_board(C.Structure):
+    """A device subscription board (lh_board_create): passed by value to the caller's kernels, which read it with
+    lh::read_histogram / lh::read_counter."""
+    _fields_ = [("handle", C.c_uint64), ("d_board", C.c_void_p), ("k", C.c_uint32), ("kc", C.c_uint32),
+                ("bytes", C.c_uint64)]
+
+
 _vp, _sz, _u32, _u64, _i32 = C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint64, C.c_int32
 
 # name -> (restype, argtypes); every symbol include/loghisto_b200.h declares
@@ -141,6 +164,10 @@ SIGNATURES = {
     "lh_graph_recorder_bind": (_i32, [_vp, C.POINTER(lh_graph_recorder), _vp, _vp]),
     "lh_graph_recorder_ingest": (_i32, [_vp, C.POINTER(lh_graph_recorder), C.POINTER(lh_batch_item), _u32, _vp]),
     "lh_graph_recorder_destroy": (_i32, [_vp, C.POINTER(lh_graph_recorder), _vp]),
+    "lh_board_create": (_i32, [_vp, _u32, _u32, C.POINTER(lh_board)]),
+    "lh_snapshot_publish": (_i32, [_vp, C.POINTER(lh_board), _vp, _vp, _vp]),
+    "lh_board_read": (_i32, [_vp, C.POINTER(lh_board), _vp, _vp]),
+    "lh_board_destroy": (_i32, [_vp, C.POINTER(lh_board)]),
     "lh_gpu_timer_start": (_i32, [_vp, _vp, C.POINTER(lh_gpu_timer)]),
     "lh_gpu_timer_stop": (_i32, [_vp, C.POINTER(lh_gpu_timer), _u32, _vp, _vp]),
     "lh_gpu_timer_release": (_i32, [_vp, C.POINTER(lh_gpu_timer)]),

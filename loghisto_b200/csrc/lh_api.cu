@@ -258,6 +258,12 @@ struct lh_ctx {
     uint64_t next_graph = 1;
     cudaEvent_t graph_drained = nullptr;               // after the latest collection drain (created with the first recorder)
     DrainParams drain_prm{};
+    // device subscriptions (lh_board_*): live boards, and the parameter block of their publish kernel (filled under the
+    // lock); pub_slot is the result slot of the open snapshot's latest lh_snapshot_reduce(_async), -1 when there is none
+    std::vector<lh_board> boards;
+    uint64_t next_board = 1;
+    int pub_slot = -1;
+    BoardParams board_prm{};
     // stats
     lh_stats stats{};
     std::mutex mu;
@@ -1093,6 +1099,7 @@ extern "C" lh_status lh_destroy(lh_ctx *ctx) {
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
     for (auto &g : ctx->graphs) cudaFree(g.rec.d_buckets);
+    for (auto &b : ctx->boards) cudaFree(b.d_board);
     if (ctx->graph_drained) cudaEventDestroy(ctx->graph_drained);
     comm_unmap(ctx);
     cudaFree(ctx->d_comm); cudaFree(ctx->d_comm_aux);
@@ -1718,6 +1725,7 @@ extern "C" lh_status lh_snapshot_begin(lh_ctx *ctx) {
     }
     ctx->active = f ^ 1;
     ctx->frozen = true;
+    ctx->pub_slot = -1;
     ctx->nnz_valid = false;
     ctx->view_reduced = false;
     ctx->view_counters_reduced = false;
@@ -1811,6 +1819,7 @@ extern "C" lh_status lh_snapshot_reduce_async(lh_ctx *ctx, const double *percent
     }
     lh_status st = enqueue_reduce(ctx, percentiles, np, slot);
     if (st != LH_OK) return st;
+    ctx->pub_slot = slot;
     ctx->res_ticket[slot] = t;
     *ticket = t;
     return LH_OK;
@@ -1928,8 +1937,128 @@ extern "C" lh_status lh_snapshot_end(lh_ctx *ctx) {
     LH_CUDA(ctx, cudaMemsetAsync(ctx->buf[f].d_counters, 0, (size_t)ctx->C * 8u, s));
     LH_CUDA(ctx, cudaEventRecord(ctx->buf[f].cleared, s));
     ctx->frozen = false;
+    ctx->pub_slot = -1;
     ctx->view_reduced = false;
     ctx->view_counters_reduced = false;
+    return LH_OK;
+}
+
+// =========================================================== device subscriptions
+namespace {
+// the image, then the id table of k_board_stage (16-byte aligned)
+size_t board_image_bytes(uint32_t k, uint32_t kc) {
+    return sizeof(lh_board_header) + (size_t)k * sizeof(lh_board_hist_row) + (size_t)kc * sizeof(lh_board_counter_row);
+}
+size_t board_table_offset(uint32_t k, uint32_t kc) { return (board_image_bytes(k, kc) + 15u) & ~(size_t)15u; }
+
+// the live board a handle names (its memory must match too), or nullptr
+const lh_board *board_of(lh_ctx *ctx, const lh_board *b) {
+    if (!b) return nullptr;
+    for (auto &x : ctx->boards)
+        if (x.handle == b->handle && x.d_board == b->d_board) return &x;
+    return nullptr;
+}
+}  // namespace
+
+extern "C" lh_status lh_board_create(lh_ctx *ctx, uint32_t k, uint32_t kc, lh_board *out) {
+    LH_ENTER(ctx);
+    if (!out) return fail(ctx, LH_ERR_INVALID, "out is NULL");
+    if (k == 0 && kc == 0) return fail(ctx, LH_ERR_INVALID, "a board needs a histogram or a counter row");
+    if (k > ctx->H || kc > ctx->C) return fail(ctx, LH_ERR_RANGE, "more rows than max_histograms / max_counters");
+    const size_t bytes = board_table_offset(k, kc) + (size_t)(k + kc) * sizeof(BoardEntry);
+    cudaStream_t s = ctx->snap_stream;
+    char *base = nullptr;
+    LH_CUDA(ctx, cudaMallocAsync((void **)&base, bytes, s));
+    cudaError_t e = cudaMemsetAsync(base, 0, bytes, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) {
+        cudaFreeAsync(base, s);
+        return fail(ctx, LH_ERR_CUDA, "lh_board_create", e);
+    }
+    lh_board b{};
+    b.handle = graph_handle(ctx, ctx->next_board++);
+    b.d_board = base;
+    b.k = k;
+    b.kc = kc;
+    b.bytes = board_image_bytes(k, kc);
+    ctx->boards.push_back(b);
+    *out = b;
+    return LH_OK;
+}
+
+// One k_board_publish on the snapshot stream, after the reduction it reads.  Entries that do not fit its parameter
+// block are first copied into the board's table by k_board_stage launches (see lh_kernels.cuh: the word is odd only
+// inside the one publish kernel).
+extern "C" lh_status lh_snapshot_publish(lh_ctx *ctx, const lh_board *b, const uint32_t *hist_ids,
+                                         const uint32_t *counter_ids, const uint64_t *counter_totals) {
+    LH_ENTER(ctx);
+    const lh_board *bd = board_of(ctx, b);
+    if (!bd) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign board");
+    if (!ctx->frozen || ctx->pub_slot < 0)
+        return fail(ctx, LH_ERR_STATE, "lh_snapshot_publish needs a reduction of the open snapshot");
+    if (!ids_ok(hist_ids, bd->k, ctx->H) || !ids_ok(counter_ids, bd->kc, ctx->C))
+        return fail(ctx, LH_ERR_RANGE, "id >= max_histograms / max_counters");
+    const int slot = ctx->pub_slot;
+    const uint32_t np = ctx->res_np[slot];
+    const ResLayout l = res_layout(ctx->H, np);
+    const char *d = ctx->d_res[slot];
+    cudaStream_t s = ctx->snap_stream;
+    BoardParams &p = ctx->board_prm;
+    p.board = (char *)bd->d_board;
+    p.table = reinterpret_cast<BoardEntry *>(p.board + board_table_offset(bd->k, bd->kc));
+    p.count = (const unsigned long long *)(d + l.count);
+    p.sum = (const double *)(d + l.sum);
+    p.avg = (const double *)(d + l.avg);
+    p.pvals = (const double *)(d + l.pvals);
+    p.pkeys = (const int *)(d + l.pkeys);
+    p.ps = ctx->d_ps[slot];
+    p.counters = snapshot_view(ctx).counters;
+    p.np = np;
+    p.k = bd->k;
+    const uint32_t rows = bd->k + bd->kc;
+    for (uint32_t r0 = 0;; r0 += BP_MAX_ENTRIES) {
+        const uint32_t n = std::min<uint32_t>(BP_MAX_ENTRIES, rows - r0);
+        p.n_staged = r0;
+        p.n = n;
+        for (uint32_t i = 0; i < n; i++) {
+            const uint32_t row = r0 + i;
+            if (row < bd->k) {
+                p.e[i] = BoardEntry{row, hist_ids ? hist_ids[row] : LH_GRAPH_UNBOUND, 0ull};
+            } else {
+                const uint32_t c = row - bd->k;
+                p.e[i] = BoardEntry{row, counter_ids ? counter_ids[c] : LH_GRAPH_UNBOUND,
+                                    counter_totals ? (unsigned long long)counter_totals[c] : 0ull};
+            }
+        }
+        if (r0 + n == rows) break;
+        k_board_stage<<<1, BP_THREADS, 0, s>>>(p);
+        LH_CUDA(ctx, cudaGetLastError());
+        ctx->stats.kernel_launches++;
+    }
+    k_board_publish<<<1, BP_THREADS, 0, s>>>(p);
+    LH_CUDA(ctx, cudaGetLastError());
+    ctx->stats.kernel_launches++;
+    return LH_OK;
+}
+
+extern "C" lh_status lh_board_read(lh_ctx *ctx, const lh_board *b, void *d_out, void *stream) {
+    LH_ENTER(ctx);
+    const lh_board *bd = board_of(ctx, b);
+    if (!bd) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign board");
+    if (!d_out || ((uintptr_t)d_out & 7u)) return fail(ctx, LH_ERR_INVALID, "d_out is NULL or not 8-byte aligned");
+    k_board_read<<<1, BR_THREADS, 0, pick_stream(ctx, stream)>>>((const unsigned long long *)bd->d_board,
+                                                                 (unsigned long long *)d_out, (uint32_t)(bd->bytes / 8u));
+    LH_CUDA(ctx, cudaGetLastError());
+    ctx->stats.kernel_launches++;
+    return LH_OK;
+}
+
+extern "C" lh_status lh_board_destroy(lh_ctx *ctx, const lh_board *b) {
+    LH_ENTER(ctx);
+    const lh_board *bd = board_of(ctx, b);
+    if (!bd) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign board");
+    LH_CUDA(ctx, cudaFreeAsync(bd->d_board, ctx->snap_stream));   // after every publish issued (all on this stream)
+    ctx->boards.erase(ctx->boards.begin() + (bd - ctx->boards.data()));
     return LH_OK;
 }
 

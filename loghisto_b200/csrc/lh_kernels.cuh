@@ -1810,6 +1810,141 @@ k_graph_drain(const __grid_constant__ DrainParams p) {
     if (lost) atomicAdd(p.dropped, lost);
 }
 
+// ----------------------------------------------------------- device subscriptions (lh_board_*, lh_snapshot_publish)
+// k_board_publish writes one collection's rows into a board (layout and row semantics: include/loghisto_b200.h), one
+// CTA, under a seqlock whose word is the board's first uint64:
+//   1. thread 0 makes the word odd, fence.acq_rel.gpu, __syncthreads;
+//   2. every thread gathers rows from the result slot of the reduction (count / sum / avg / pvals / pkeys at the
+//      res_layout offsets for that reduction's np; the percentiles from its d_ps) and the counter deltas of the
+//      snapshot view, and writes them with strong relaxed stores;
+//   3. __threadfence, __syncthreads;
+//   4. thread 0 writes the publish count and makes the word even with st.release.gpu.
+// A reader (k_board_read, lh::read_histogram / read_counter) loads the word with ld.acquire.gpu and retries while it
+// is odd, loads the rows with strong relaxed loads, then fence.acq_rel.gpu and the word again, and retries if it
+// changed.  A reader that saw a row store of this publish synchronises with step 1's fence, so its second load of the
+// word sees the odd value or a later one and the read is retried; a reader that saw the even word of step 4 sees every
+// row store before it.
+//
+// Termination: the writer waits on nothing -- no lock, no flag, no other kernel -- so once its CTA is resident it
+// finishes in a bounded number of steps, and the word is odd only while it is resident.  A reader therefore spins only
+// while a resident writer runs, whatever else occupies the GPU.  That is why the whole odd window lies inside one
+// kernel: an id table too large for one parameter block is first copied into the board's table area by k_board_stage
+// launches, which do not touch the word.
+constexpr int BP_THREADS = 512;
+constexpr int BP_MAX_ENTRIES = 1536;         // entries per launch: 16 B each in the parameter block
+
+struct BoardEntry {
+    uint32_t row;                            // < k: histogram row; else counter row (row - k)
+    uint32_t id;                             // histogram / counter id of the snapshot, or LH_GRAPH_UNBOUND
+    unsigned long long total;                // counter rows: the caller's total
+};
+struct BoardParams {
+    char *board;                             // header, k histogram rows, kc counter rows
+    BoardEntry *table;                       // entries staged by k_board_stage, [n_staged]
+    const unsigned long long *count;         // the reduction's result slot
+    const double *sum, *avg, *pvals;
+    const int *pkeys;
+    const double *ps;                        // its percentiles [np]
+    const unsigned long long *counters;      // counter deltas of the snapshot view
+    uint32_t np, k;
+    uint32_t n_staged, n;                    // entries in `table`, then in e[]
+    BoardEntry e[BP_MAX_ENTRIES];
+};
+
+__global__ void __launch_bounds__(BP_THREADS)
+k_board_stage(const __grid_constant__ BoardParams p) {
+    for (uint32_t i = threadIdx.x; i < p.n; i += BP_THREADS) p.table[p.n_staged + i] = p.e[i];
+}
+
+__global__ void __launch_bounds__(BP_THREADS)
+k_board_publish(const __grid_constant__ BoardParams p) {
+    unsigned long long *seq = reinterpret_cast<unsigned long long *>(p.board);
+    const uint32_t t = threadIdx.x, lane = t & 31u, warp = t >> 5;
+    if (t == 0) {
+        board::st_relaxed(seq, board::ld_relaxed(seq) + 1ull);   // odd: the previous publish ended (stream order)
+        board::fence_acq_rel();
+    }
+    __syncthreads();
+    const double qnan = __longlong_as_double(0x7FF8000000000000ll);
+    char *hdr = p.board;
+    if (t < LH_MAX_PERCENTILES)
+        board::st_relaxed(hdr + offsetof(lh_board_header, percentiles) + 8 * t,
+                          (unsigned long long)__double_as_longlong(t < p.np ? p.ps[t] : qnan));
+    if (t == 0) board::st_relaxed_u32(hdr + offsetof(lh_board_header, np), p.np);
+    const uint32_t total = p.n_staged + p.n;
+    auto entry = [&](uint32_t i) { return i < p.n_staged ? p.table[i] : p.e[i - p.n_staged]; };
+    // histogram rows: one warp each, lane j writes percentile slot j
+    for (uint32_t i = warp; i < total; i += BP_THREADS / 32) {
+        const BoardEntry e = entry(i);
+        if (e.row >= p.k) continue;
+        char *r = p.board + sizeof(lh_board_header) + (size_t)e.row * sizeof(lh_board_hist_row);
+        const bool bound = e.id != LH_GRAPH_UNBOUND;
+        int key = (int)0x80000000;
+        double val = qnan;
+        if (bound && lane < p.np) {
+            key = p.pkeys[(size_t)e.id * p.np + lane];
+            val = p.pvals[(size_t)e.id * p.np + lane];
+        }
+        board::st_relaxed(r + offsetof(lh_board_hist_row, pvals) + 8 * lane, (unsigned long long)__double_as_longlong(val));
+        board::st_relaxed_u32(r + offsetof(lh_board_hist_row, pkeys) + 4 * lane, (uint32_t)key);
+        if (lane == 0) {
+            const unsigned long long c = bound ? p.count[e.id] : 0ull;
+            board::st_relaxed(r + offsetof(lh_board_hist_row, count), c);
+            board::st_relaxed(r + offsetof(lh_board_hist_row, sum), (unsigned long long)__double_as_longlong(bound ? p.sum[e.id] : 0.0));
+            board::st_relaxed(r + offsetof(lh_board_hist_row, avg), (unsigned long long)__double_as_longlong(bound ? p.avg[e.id] : qnan));
+            board::st_relaxed_u32(r + offsetof(lh_board_hist_row, present), c != 0ull);
+        }
+    }
+    // counter rows: one thread each
+    char *crows = p.board + sizeof(lh_board_header) + (size_t)p.k * sizeof(lh_board_hist_row);
+    for (uint32_t i = t; i < total; i += BP_THREADS) {
+        const BoardEntry e = entry(i);
+        if (e.row < p.k) continue;
+        char *r = crows + (size_t)(e.row - p.k) * sizeof(lh_board_counter_row);
+        const bool bound = e.id != LH_GRAPH_UNBOUND;
+        board::st_relaxed(r + offsetof(lh_board_counter_row, rate), bound ? p.counters[e.id] : 0ull);
+        board::st_relaxed(r + offsetof(lh_board_counter_row, total), e.total);
+        board::st_relaxed_u32(r + offsetof(lh_board_counter_row, present), bound ? 1u : 0u);
+    }
+    __threadfence();
+    __syncthreads();
+    if (t == 0) {
+        const unsigned long long s = board::ld_relaxed(seq) + 1ull;   // even
+        board::st_relaxed(hdr + offsetof(lh_board_header, publishes), s >> 1);
+        board::st_release(seq, s);
+    }
+}
+
+// Copies a consistent image of a board (`words` uint64) to `out`, one CTA: the seqlock read of k_board_publish's
+// comment over the whole board, each thread fencing its own loads before thread 0 re-reads the word.  A torn copy is
+// overwritten by the retry; the image's word is the even value it was read under.
+constexpr int BR_THREADS = 512;
+
+__global__ void __launch_bounds__(BR_THREADS)
+k_board_read(const unsigned long long *__restrict__ board, unsigned long long *__restrict__ out, uint32_t words) {
+    __shared__ unsigned long long s_seq;
+    __shared__ int s_ok;
+    const uint32_t t = threadIdx.x;
+    for (;;) {
+        if (t == 0) {
+            unsigned long long s;
+            while ((s = board::ld_acquire(board)) & 1ull) __nanosleep(64);
+            s_seq = s;
+        }
+        __syncthreads();
+        const unsigned long long s = s_seq;
+        for (uint32_t i = t + 1; i < words; i += BR_THREADS) out[i] = board::ld_relaxed(board + i);
+        board::fence_acq_rel();
+        __syncthreads();
+        if (t == 0) s_ok = board::ld_relaxed(board) == s;
+        __syncthreads();
+        if (s_ok) {
+            if (t == 0) out[0] = s;
+            return;
+        }
+    }
+}
+
 // ----------------------------------------------------------- GPU timers (lh_gpu_timer_*)
 // One thread each: their cost is the launch, not the body.  The start writes %globaltimer into the token's slot; the
 // stop records float64(now - start) into one histogram row through the same bucket function and row writer every

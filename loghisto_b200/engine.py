@@ -254,6 +254,96 @@ class GraphRecorder:
         self.close()
 
 
+_BOARD_HDR_WORDS = C.sizeof(L.lh_board_header) // 8        # 36
+_BOARD_ROW_WORDS = C.sizeof(L.lh_board_hist_row) // 8      # 52
+_BOARD_CTR_WORDS = C.sizeof(L.lh_board_counter_row) // 8   # 3
+
+
+def board_out(out, nbytes: int, device: int):
+    """The uint8 CUDA tensor a board image is read into: `out` checked (contiguous uint8 on the device, at least
+    `nbytes` long, 8-byte aligned), or a new one when out is None."""
+    import torch
+    if out is None:
+        return torch.empty(nbytes, dtype=torch.uint8, device=torch.device("cuda", device))
+    if not (out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and out.numel() >= nbytes
+            and out.data_ptr() % 8 == 0):
+        raise TypeError("out must be a contiguous 8-byte aligned uint8 CUDA tensor of at least %d bytes" % nbytes)
+    return out
+
+
+def board_views(buf, k: int, kc: int) -> dict:
+    """Torch views of the board image in `buf` (layout of include/loghisto_b200.h), no copy and no synchronisation:
+      collection       int64 [], the publish number of the image (0: nothing published yet)
+      np               int32 [], percentiles of that publish
+      percentiles      float64 [LH_MAX_PERCENTILES], NaN from np on
+      present          int32 [k]; count int64 [k] (the uint64 bits); sum, avg float64 [k]
+      pvals            float64 [k, LH_MAX_PERCENTILES]; pkeys int32 [k, LH_MAX_PERCENTILES] (INT32_MIN = label omitted)
+      counter_present  int32 [kc]; rate, total int64 [kc] (the uint64 bits)
+    Percentile columns j >= np hold NaN / INT32_MIN."""
+    import torch
+    nbytes = (_BOARD_HDR_WORDS + _BOARD_ROW_WORDS * k + _BOARD_CTR_WORDS * kc) * 8
+    w64 = buf[:nbytes].view(torch.int64)
+    f64 = buf[:nbytes].view(torch.float64)
+    i32 = buf[:nbytes].view(torch.int32)
+    b8, b4 = w64.storage_offset(), i32.storage_offset()
+    h, rw, cb = _BOARD_HDR_WORDS, _BOARD_ROW_WORDS, _BOARD_HDR_WORDS + _BOARD_ROW_WORDS * k
+    P = L.LH_MAX_PERCENTILES
+    return {
+        "image": buf[:nbytes],
+        "collection": w64.as_strided((), (), b8 + 1),
+        "np": i32.as_strided((), (), b4 + 4),
+        "percentiles": f64.as_strided((P,), (1,), b8 + 4),
+        "count": w64.as_strided((k,), (rw,), b8 + h),
+        "sum": f64.as_strided((k,), (rw,), b8 + h + 1),
+        "avg": f64.as_strided((k,), (rw,), b8 + h + 2),
+        "present": i32.as_strided((k,), (2 * rw,), b4 + 2 * h + 6),
+        "pvals": f64.as_strided((k, P), (rw, 1), b8 + h + 4),
+        "pkeys": i32.as_strided((k, P), (2 * rw, 1), b4 + 2 * h + 72),
+        "rate": w64.as_strided((kc,), (_BOARD_CTR_WORDS,), b8 + cb),
+        "total": w64.as_strided((kc,), (_BOARD_CTR_WORDS,), b8 + cb + 1),
+        "counter_present": i32.as_strided((kc,), (2 * _BOARD_CTR_WORDS,), b4 + 2 * cb + 4),
+    }
+
+
+class Board:
+    """A device subscription board of an Engine (Engine.board): `board` is the lh_board to pass by value to kernels,
+    which read it with lh::read_histogram / lh::read_counter."""
+
+    def __init__(self, engine: "Engine", k: int, kc: int):
+        self._eng = engine
+        self.board = L.lh_board()
+        engine._check(engine.lib.lh_board_create(engine.h, int(k), int(kc), C.byref(self.board)))
+        self.k, self.kc = int(k), int(kc)
+        self._open = True
+
+    def publish(self, hist_ids=None, counter_ids=None, totals=None):
+        """lh_snapshot_publish: row i from the open snapshot's latest reduction for hist_ids[i] / counter_ids[i]
+        (None = every row unbound; L.LH_GRAPH_UNBOUND = that row), with counter totals `totals` (None = 0)."""
+        h = _ids(hist_ids)[0] if hist_ids is not None else None
+        c = _ids(counter_ids)[0] if counter_ids is not None else None
+        t = (C.c_uint64 * max(len(totals), 1))(*[int(x) for x in totals]) if totals is not None else None
+        self._eng._check(self._eng.lib.lh_snapshot_publish(self._eng.h, C.byref(self.board), h, c, t))
+
+    def read(self, out=None, stream=None) -> dict:
+        """lh_board_read into `out` (None = a new uint8 CUDA tensor) on `stream` (None = torch's current stream, so
+        that it is captured inside torch.cuda.graph); returns board_views of it.  Nothing is synchronised."""
+        buf = board_out(out, self.board.bytes, self._eng.device)
+        self._eng._check(self._eng.lib.lh_board_read(self._eng.h, C.byref(self.board), buf.data_ptr(), _capture_stream(stream)))
+        return board_views(buf, self.k, self.kc)
+
+    def close(self):
+        """lh_board_destroy (stream-ordered after every publish issued); no read of the board may be pending."""
+        if self._open:
+            self._open = False
+            self._eng._check(self._eng.lib.lh_board_destroy(self._eng.h, C.byref(self.board)))
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+
 class Engine:
     def __init__(self, device: int = 0, max_histograms: int = 1, max_counters: int = 1,
                  staging_bytes: int = 0, staging_slots: int = 0, precision: int = 0):
@@ -485,6 +575,10 @@ class Engine:
         return GraphRecorder(self, hist_ids, counter_ids)
 
     # ---- GPU timers (StartTimer / Stop with both ends on the device)
+    def board(self, k: int = 0, kc: int = 0) -> "Board":
+        """A device subscription board of k histogram rows and kc counter rows (lh_board_create)."""
+        return Board(self, k, kc)
+
     def gpu_timer_start(self, stream=None) -> L.lh_gpu_timer:
         """Enqueue a start mark on `stream` (None = the ingest stream; torch's default stream is timed as itself)."""
         t = L.lh_gpu_timer()

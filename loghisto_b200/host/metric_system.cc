@@ -33,6 +33,11 @@
 #pragma weak lh_graph_recorder_bind
 #pragma weak lh_graph_recorder_ingest
 #pragma weak lh_graph_recorder_destroy
+// And for device subscriptions: over a build without them, NewDeviceSubscription throws.
+#pragma weak lh_board_create
+#pragma weak lh_snapshot_publish
+#pragma weak lh_board_read
+#pragma weak lh_board_destroy
 
 namespace loghisto {
 
@@ -40,6 +45,13 @@ namespace loghisto {
 struct GraphRecorder::State {
     MetricSystem *ms;                   // nullptr once closed (or once the system is gone)
     lh_graph_recorder g{};
+    std::vector<std::string> hnames, cnames;
+};
+
+// an open device subscription, shared by its DeviceSubscription and the system's list of open subscriptions
+struct DeviceSubscription::State {
+    MetricSystem *ms;                   // nullptr once closed (or once the system is gone)
+    lh_board b{};
     std::vector<std::string> hnames, cnames;
 };
 
@@ -417,6 +429,10 @@ MetricSystem::~MetricSystem() {
     {   // recorders left open are freed by lh_destroy; their objects only forget the system
         std::lock_guard<std::mutex> lk(graph_mu_);
         for (auto &g : graphs_) g->ms = nullptr;
+    }
+    {   // likewise for subscriptions' boards
+        std::lock_guard<std::mutex> lk(sub_mu_);
+        for (auto &d : subs_) d->ms = nullptr;
     }
     lh_destroy(ctx_);
 }
@@ -832,6 +848,82 @@ GraphRecorder::~GraphRecorder() {
     try { Close(); } catch (...) {}
 }
 
+// ---- device subscriptions ----------------------------------------------------------------------------------------
+DeviceSubscription MetricSystem::NewDeviceSubscription(const std::vector<std::string> &histograms,
+                                                       const std::vector<std::string> &counters) {
+    if (!lh_board_create || !lh_snapshot_publish || !lh_board_read || !lh_board_destroy)
+        throw std::runtime_error("NewDeviceSubscription: this libloghisto_b200 has no device subscriptions");
+    auto st = std::make_shared<DeviceSubscription::State>();
+    st->ms = this;
+    st->hnames = histograms;
+    st->cnames = counters;
+    check(ctx_, lh_board_create(ctx_, (uint32_t)histograms.size(), (uint32_t)counters.size(), &st->b), "lh_board_create");
+    std::lock_guard<std::mutex> lk(sub_mu_);
+    subs_.push_back(st);
+    DeviceSubscription d;
+    d.st_ = std::move(st);
+    return d;
+}
+
+// With sub_mu_ held, between the reduction of collectRawMetrics and lh_snapshot_end: row i of every open subscription
+// is bound to the id that carries its name in this collection's labels, if the name is in Histograms (hid_of) or
+// Rates (cid_of); totals are the Counters values.  The first failure is returned; the other boards still publish.
+lh_status MetricSystem::publish_subscriptions(const RawMetricSet &raw, const std::unordered_map<std::string, uint32_t> &hid_of,
+                                              const std::unordered_map<std::string, uint32_t> &cid_of) {
+    lh_status first = LH_OK;
+    for (auto &d : subs_) {
+        std::vector<uint32_t> hids(d->hnames.size()), cids(d->cnames.size());
+        std::vector<uint64_t> totals(d->cnames.size());
+        for (size_t i = 0; i < hids.size(); i++) {
+            auto it = hid_of.find(d->hnames[i]);
+            hids[i] = it == hid_of.end() ? LH_GRAPH_UNBOUND : it->second;
+        }
+        for (size_t i = 0; i < cids.size(); i++) {
+            auto it = cid_of.find(d->cnames[i]);
+            cids[i] = it == cid_of.end() ? LH_GRAPH_UNBOUND : it->second;
+            auto t = raw.Counters.find(d->cnames[i]);
+            totals[i] = t == raw.Counters.end() ? 0 : t->second;
+        }
+        const lh_status st = lh_snapshot_publish(ctx_, &d->b, hids.data(), cids.data(), totals.data());
+        if (st != LH_OK && first == LH_OK) first = st;
+    }
+    return first;
+}
+
+const lh_board &DeviceSubscription::board() const {
+    if (!st_) throw std::runtime_error("DeviceSubscription::board of a closed subscription");
+    return st_->b;
+}
+
+void DeviceSubscription::Read(void *d_out, void *stream) {
+    if (!st_ || !st_->ms) throw std::runtime_error("DeviceSubscription::Read of a closed subscription");
+    MetricSystem *ms = st_->ms;
+    check(ms->ctx_, lh_board_read(ms->ctx_, &st_->b, d_out, stream), "lh_board_read");
+}
+
+void DeviceSubscription::Close() {
+    if (!st_) return;
+    std::shared_ptr<State> st = std::move(st_);
+    MetricSystem *ms = st->ms;
+    if (!ms) return;
+    std::lock_guard<std::mutex> lk(ms->sub_mu_);   // not during a collection's publish
+    auto &v = ms->subs_;
+    v.erase(std::remove(v.begin(), v.end(), st), v.end());
+    st->ms = nullptr;
+    check(ms->ctx_, lh_board_destroy(ms->ctx_, &st->b), "lh_board_destroy");
+}
+
+DeviceSubscription &DeviceSubscription::operator=(DeviceSubscription &&o) noexcept {
+    if (this != &o) {
+        try { Close(); } catch (...) {}
+        st_ = std::move(o.st_);
+    }
+    return *this;
+}
+DeviceSubscription::~DeviceSubscription() {
+    try { Close(); } catch (...) {}
+}
+
 // ---- GPU timers ------------------------------------------------------------------------------------------------
 void *const GpuTimerToken::kStartStream = reinterpret_cast<void *>(~(uintptr_t)0);
 
@@ -999,6 +1091,18 @@ std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
             }
         }
         raw->Counters = counter_store_;
+    }
+    {   // device subscriptions: this collection's rows, from the reduction above, before the snapshot ends
+        std::lock_guard<std::mutex> lk(sub_mu_);
+        if (!subs_.empty()) {
+            std::unordered_map<std::string, uint32_t> hid_of, cid_of;   // names of Histograms / Rates -> their ids
+            for (size_t h = 0; h < hnames.size(); h++)
+                if (sp.offsets[h] != sp.offsets[h + 1]) hid_of.emplace(hnames[h], (uint32_t)h);
+            for (size_t c = 0; c < cnames.size(); c++)
+                if (sp.counter_deltas[c] || touched[c]) cid_of.emplace(cnames[c], (uint32_t)c);
+            if (publish_subscriptions(*raw, hid_of, cid_of) != LH_OK)   // the host's metric set is still delivered
+                fprintf(stderr, "loghisto: lh_snapshot_publish failed: %s\n", lh_last_error(ctx_));
+        }
     }
     check(ctx_, lh_snapshot_end(ctx_), "lh_snapshot_end");
     {
@@ -1468,6 +1572,35 @@ LHMS_API int lhms_graph_recorder_close(void *g, void *stream) {
     try { static_cast<GraphRecorder *>(g)->Close(stream); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
 }
 LHMS_API void lhms_graph_recorder_free(void *g) { delete static_cast<GraphRecorder *>(g); }
+// MetricSystem::NewDeviceSubscription: a DeviceSubscription handle (NULL with *status set on failure); *out receives
+// its board.  Free it with lhms_subscription_free, which closes it if lhms_subscription_close has not.
+LHMS_API void *lhms_subscription_new(void *ms, uint32_t n_h, const char *const *h_names, uint32_t n_c,
+                                     const char *const *c_names, lh_board *out, int *status) {
+    int dummy;
+    if (!status) status = &dummy;
+    *status = LH_ERR_INVALID;
+    if (!ms || !out || (n_h && !h_names) || (n_c && !c_names)) return nullptr;
+    try {
+        std::vector<std::string> hs(h_names, h_names + n_h), cs(c_names, c_names + n_c);
+        auto *d = new DeviceSubscription(static_cast<MetricSystem *>(ms)->NewDeviceSubscription(hs, cs));
+        *out = d->board();
+        *status = LH_OK;
+        return d;
+    } catch (const std::exception &e) {
+        *status = scope_status(e);
+        return nullptr;
+    }
+}
+// DeviceSubscription::Read of the board image into d_out on `stream`.
+LHMS_API int lhms_subscription_read(void *d, void *d_out, void *stream) {
+    if (!d) return LH_ERR_INVALID;
+    try { static_cast<DeviceSubscription *>(d)->Read(d_out, stream); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
+}
+LHMS_API int lhms_subscription_close(void *d) {
+    if (!d) return LH_ERR_INVALID;
+    try { static_cast<DeviceSubscription *>(d)->Close(); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
+}
+LHMS_API void lhms_subscription_free(void *d) { delete static_cast<DeviceSubscription *>(d); }
 LHMS_API void lhms_start(void *ms) { static_cast<MetricSystem *>(ms)->Start(); }
 LHMS_API void lhms_stop(void *ms) { static_cast<MetricSystem *>(ms)->Stop(); }
 LHMS_API uint64_t lhms_dropped(void *ms) { return static_cast<MetricSystem *>(ms)->dropped_samples(); }

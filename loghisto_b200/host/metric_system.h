@@ -249,6 +249,45 @@ class GraphRecorder {
     std::shared_ptr<State> st_;
 };
 
+// SubscribeToProcessedMetrics for consumers on the GPU (MetricSystem::NewDeviceSubscription).  Every collection, after
+// its reduction, publishes the subscribed names' processed metrics into a board in device memory (lh_board_create,
+// lh_snapshot_publish), where kernels and CUDA-graph replays read the latest collection with lh::read_histogram /
+// lh::read_counter (include/loghisto_b200_device.cuh) or an lh_board_read copy, with no host call.
+//
+//   loghisto::DeviceSubscription sub = ms.NewDeviceSubscription({"step_latency"}, {"requests"});
+//   shed_load<<<1, 32, 0, stream>>>(sub.board(), /* histogram row of "step_latency" */ 0);   // reads p99 on the device
+//   sub.Close();   // once no read of the board is pending; also on destruction
+//
+// Histogram row i is name histograms[i], counter row i is counters[i].  At a collection a histogram row holds what
+// processMetrics emits for that name when the name is in the collection's Histograms (count = <name>_count as uint64,
+// sum, avg and every labelled percentile bit for bit; a percentile whose key is INT32_MIN is a label processMetrics
+// omits), and present = 0 otherwise.  A counter row holds the name's Rates entry (rate, present = 1) when the name is
+// in Rates, and its Counters value as total in any case (0 for a name never counted).  A subscription reads; it does
+// not keep its names' ids alive.  Move-only.
+class DeviceSubscription {
+ public:
+    DeviceSubscription() = default;
+    DeviceSubscription(DeviceSubscription &&o) noexcept { *this = std::move(o); }
+    DeviceSubscription &operator=(DeviceSubscription &&o) noexcept;
+    DeviceSubscription(const DeviceSubscription &) = delete;
+    DeviceSubscription &operator=(const DeviceSubscription &) = delete;
+    ~DeviceSubscription();
+
+    const lh_board &board() const;
+    // lh_board_read: one kernel on `stream` copies a consistent image of the board (board().bytes) to d_out.  It may
+    // be captured into a CUDA graph.  Throws std::runtime_error when the library refuses the call or it is closed.
+    void Read(void *d_out, void *stream);
+    // Frees the board, after every publish issued (idempotent); no read of it may be pending.
+    void Close();
+    bool open() const { return st_ != nullptr; }
+
+    struct State;
+
+ private:
+    friend class MetricSystem;
+    std::shared_ptr<State> st_;
+};
+
 struct Options {
     int device = 0;
     uint32_t max_histograms = 1024;
@@ -292,6 +331,11 @@ class MetricSystem {
     // capture.  Throws std::runtime_error when the library refuses lh_graph_recorder_create (e.g. more names than
     // max_histograms / max_counters); a full name table never makes it fail.
     GraphRecorder NewGraphRecorder(const std::vector<std::string> &histograms, const std::vector<std::string> &counters);
+    // A device subscription to these names (DeviceSubscription): every collection from now on, the reaper's included,
+    // publishes into it.  Call it outside any stream capture.  Throws std::runtime_error when the library refuses
+    // lh_board_create (e.g. more names than max_histograms / max_counters, or none).
+    DeviceSubscription NewDeviceSubscription(const std::vector<std::string> &histograms,
+                                             const std::vector<std::string> &counters);
     void RegisterGaugeFunc(const std::string &name, std::function<double()> f);   // :299
     void DeregisterGaugeFunc(const std::string &name);                    // :306
     void Start();                                                         // :644
@@ -367,6 +411,12 @@ class MetricSystem {
     void bind_graph(GraphRecorder::State &g);
     std::mutex graph_mu_;
     std::vector<std::shared_ptr<GraphRecorder::State>> graphs_;   // open recorders
+    // device subscriptions (NewDeviceSubscription)
+    friend class DeviceSubscription;
+    std::mutex sub_mu_;
+    std::vector<std::shared_ptr<DeviceSubscription::State>> subs_;   // open subscriptions
+    lh_status publish_subscriptions(const RawMetricSet &raw, const std::unordered_map<std::string, uint32_t> &hid_of,
+                                    const std::unordered_map<std::string, uint32_t> &cid_of);
 
     lh_ctx *ctx_ = nullptr;
     std::chrono::nanoseconds interval_;

@@ -10,7 +10,7 @@ import ctypes as C
 
 from . import _lib as _L
 from . import build as _build
-from .engine import _batch_array, _capture_stream, _stream, _timer_stream
+from .engine import _batch_array, _capture_stream, _stream, _timer_stream, board_out, board_views
 
 _EMIT = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_char_p, C.c_int, C.c_uint64, C.c_double)
 _lib = None
@@ -85,6 +85,13 @@ def _bind(L):
     L.lhms_graph_recorder_close.restype = C.c_int
     L.lhms_graph_recorder_close.argtypes = [vp, vp]
     L.lhms_graph_recorder_free.argtypes = [vp]
+    L.lhms_subscription_new.restype = vp
+    L.lhms_subscription_new.argtypes = [vp, C.c_uint32, names, C.c_uint32, names, C.POINTER(_L.lh_board), C.POINTER(C.c_int)]
+    L.lhms_subscription_read.restype = C.c_int
+    L.lhms_subscription_read.argtypes = [vp, vp, vp]
+    L.lhms_subscription_close.restype = C.c_int
+    L.lhms_subscription_close.argtypes = [vp]
+    L.lhms_subscription_free.argtypes = [vp]
     for kind in ("processed", "raw"):
         getattr(L, "lhms_subscribe_" + kind).restype = vp
         getattr(L, "lhms_subscribe_" + kind).argtypes = [vp, C.c_int]
@@ -289,6 +296,65 @@ class GraphRecorder:
             pass
 
 
+class DeviceSubscription:
+    """A device subscription of a MetricSystem (MetricSystem.device_subscription): every collection publishes the
+    processed metrics of its names into `board`, an lh_board in device memory that kernels read with
+    lh::read_histogram / lh::read_counter (row numbers in histogram_rows / counter_rows), and read() copies on a stream.
+    Usable as a context manager; close() (also on exit) frees the board once no read of it is pending."""
+
+    def __init__(self, ms, histograms, counters):
+        self._ms = ms
+        hnames, cnames = [str(x) for x in histograms], [str(x) for x in counters]
+        self.board = _L.lh_board()
+        hn = (C.c_char_p * max(len(hnames), 1))(*[x.encode() for x in hnames])
+        cn = (C.c_char_p * max(len(cnames), 1))(*[x.encode() for x in cnames])
+        st = C.c_int()
+        self._h = ms._lib.lhms_subscription_new(ms._h, len(hnames), hn, len(cnames), cn, C.byref(self.board), C.byref(st))
+        if not self._h:
+            raise RuntimeError("lhms_subscription_new failed (status %d)" % st.value)
+        self.histogram_rows = {nm: i for i, nm in enumerate(hnames)}
+        self.counter_rows = {nm: i for i, nm in enumerate(cnames)}
+        self._device = ms._device
+
+    def read(self, out=None, stream=None) -> dict:
+        """One kernel on `stream` (None = torch's current stream, so that it is captured inside torch.cuda.graph)
+        copies a consistent image of the latest publish into `out` (a contiguous uint8 CUDA tensor of at least
+        board.bytes, or None for a new one); returns torch views of it (engine.board_views: collection, np,
+        percentiles, present, count, sum, avg, pvals, pkeys, counter_present, rate, total).  Nothing is synchronised:
+        the views are valid once the stream has run the copy.  A graph replay copies the publish latest at its run."""
+        if self._h is None:
+            raise RuntimeError("the device subscription is closed")
+        buf = board_out(out, self.board.bytes, self._device)
+        st = self._ms._lib.lhms_subscription_read(self._h, buf.data_ptr(), _capture_stream(stream))
+        if st != 0:
+            raise RuntimeError("lhms_subscription_read failed (status %d)" % st)
+        return board_views(buf, self.board.k, self.board.kc)
+
+    def close(self):
+        """Frees the board after every publish issued.  No read of it may be pending.  Idempotent."""
+        if self._h is None:
+            return
+        h, self._h = self._h, None
+        st = 0
+        if self._ms._h:   # a closed MetricSystem already freed the board
+            st = self._ms._lib.lhms_subscription_close(h)
+        self._ms._lib.lhms_subscription_free(h)
+        if st != 0:
+            raise RuntimeError("lhms_subscription_close failed (status %d)" % st)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class Subscription:
     def __init__(self, ms, kind, capacity):
         self._ms, self._kind = ms, kind
@@ -344,6 +410,7 @@ class MetricSystem:
             self._h = self._lib.lhms_new(max(int(interval_s * 1e9), 1), device, max_histograms, max_counters, err, 512)
         if not self._h:
             raise RuntimeError(err.value.decode())
+        self._device = device
 
     def close(self):
         if self._h:
@@ -421,6 +488,13 @@ class MetricSystem:
             yield g
         finally:
             g.close()
+
+    def device_subscription(self, histograms=(), counters=()) -> DeviceSubscription:
+        """SubscribeToProcessedMetrics for the GPU: every collection from now on (the reaper's included) publishes the
+        processed metrics of these names into device memory, for kernels and captured graphs (DeviceSubscription).
+        `with ms.device_subscription(histograms=[...], counters=[...]) as sub:` closes it on exit.  Create it outside
+        any stream capture."""
+        return DeviceSubscription(self, histograms, counters)
 
     def RegisterConstantGauge(self, name: str, value: float):
         self._lib.lhms_register_constant_gauge(self._h, name.encode(), float(value))

@@ -66,6 +66,18 @@ with lh.Engine(device=0, max_histograms=4, max_counters=4) as e:    # graph reco
         g.close(stream=0)                                # final drain
     red, _ = e.snapshot(PS)
     assert int(red.counts[3]) == 3_000
+with lh.Engine(device=0, max_histograms=4, max_counters=2) as e:    # device subscription: publish (staged too), read
+    d = e.gen_stream(lh.STREAM_S, n, lh.DEFAULT_SEED)
+    e.ingest_f64(1, d, n)
+    e.snapshot_begin()
+    e.snapshot_reduce_async(PS)
+    with e.board(4, 2) as b:
+        b.publish([1, 0xFFFFFFFF, 0, 3], [1, 0xFFFFFFFF], [7, 8])
+        e.snapshot_end()
+        e.sync()
+        v = b.read(stream=0)
+        e.sync()
+        assert int(v["count"][0].item()) == n and int(v["collection"].item()) == 1
 # two contexts on one device: the peer all-reduce kernel
 engs = [lh.Engine(device=0, max_histograms=3, max_counters=2) for _ in range(2)]
 handles = b"".join(x.comm_export() for x in engs)
