@@ -349,6 +349,45 @@ LH_API lh_status lh_snapshot_publish(lh_ctx *ctx, const lh_board *b, const uint3
 LH_API lh_status lh_board_read(lh_ctx *ctx, const lh_board *b, void *d_out, void *stream);
 LH_API lh_status lh_board_destroy(lh_ctx *ctx, const lh_board *b);
 
+/* ---- device gauges: RegisterGaugeFunc (metrics.go:299-310) for values that live in device memory -----------------
+ * lh_gauges_read reads n scalars from device memory, one per lh_gauge_src, and returns them to the host as float64.  It
+ * is stateless: the registry of names lives in the caller (MetricSystem::RegisterDeviceGauge).
+ *
+ *   Values    h_out[i] is Go's float64(x) of the value x at d_value: exact for F64, F32, F16, BF16 and I32;
+ *             round-to-nearest-even for I64 and U64 (what amd64 Go does: CVTSQ2SD, and the halve-and-double
+ *             sequence for uint64 >= 2^63).  A NaN stays a NaN; its payload is unspecified.
+ *   Loads     each value is read with one naturally aligned strong load (ld.relaxed.gpu), so a value written by a
+ *             single aligned store is never torn (see lh::set_gauge in include/loghisto_b200_device.cuh).
+ *   Ordering  the read is enqueued on the context's snapshot stream only.  It never waits for ingest streams, record
+ *             scopes, graph replays or any caller stream: it reads whatever is in memory when the kernel runs, as a Go
+ *             gauge function reads the current state.
+ *   Waiting   the call returns once the values are in h_out.  It does not hold the context's lock while it waits for
+ *             the device, so ingest calls from other threads are not held up.
+ *   Checks    everything is validated before anything is launched; on a failed check nothing is launched:
+ *             h_srcs / h_out NULL with n > 0, an unknown dtype, a non-zero `reserved`, a NULL d_value or one not
+ *             naturally aligned for its dtype, and a d_value that is not device or managed memory of the context's
+ *             device (cudaPointerGetAttributes: host memory, pinned or not, and another GPU's memory are refused) all
+ *             return LH_ERR_INVALID.  The last check is what keeps the kernel from ever faulting on a bad address.
+ *   Sizes     n == 0 returns LH_OK with no launch.  Any n is accepted: tables larger than one launch's parameter block
+ *             (1 024 entries) are split across launches on the same stream, with one wait at the end.
+ * The call returns host values, so it cannot be captured into a CUDA graph.  It does not change lh_stats.samples,
+ * lh_stats.counter_ops or the ingest sequence. */
+#define LH_GAUGE_F64 0
+#define LH_GAUGE_F32 1
+#define LH_GAUGE_F16 2
+#define LH_GAUGE_BF16 3
+#define LH_GAUGE_I64 4
+#define LH_GAUGE_I32 5
+#define LH_GAUGE_U64 6
+typedef struct lh_gauge_src {
+    const void *d_value;                      /* device or managed memory of the context's device */
+    uint32_t dtype;                           /* LH_GAUGE_* */
+    uint32_t reserved;                        /* 0 */
+} lh_gauge_src;
+LH_STATIC_ASSERT(sizeof(lh_gauge_src) == 16 && offsetof(lh_gauge_src, dtype) == 8 &&
+                 offsetof(lh_gauge_src, reserved) == 12, "lh_gauge_src is 16 bytes: d_value, dtype, reserved");
+LH_API lh_status lh_gauges_read(lh_ctx *ctx, const lh_gauge_src *h_srcs, uint32_t n, double *h_out);
+
 /* ---- GPU timers: StartTimer / Stop (metrics.go:232-246) from host code, timed on the device ------------------
  * Host StartTimer / Stop around CUDA work time the enqueue.  These calls put the two ends of the span on the GPU
  * instead: each end is a one-thread kernel on `stream` that reads %globaltimer (the clock of lh::start_timer), and

@@ -593,4 +593,38 @@ __device__ __forceinline__ uint64_t read_counter(const lh_board &b, uint32_t row
     }
 }
 
+// ================================================================ writing a device gauge (lh_gauges_read)
+// A device gauge (MetricSystem::RegisterDeviceGauge) is a scalar in device memory that every collection reads with one
+// naturally aligned strong load (ld.relaxed.gpu).  The PTX memory model promises an untorn read only against a strong
+// store of the same size, which is what lh::set_gauge issues (st.relaxed.gpu):
+//
+//   lh::set_gauge(d_loss, loss);     // T = double, float, __half, __nv_bfloat16, int64_t, int32_t or uint64_t
+//
+// Plain aligned stores of one value -- what torch's fill_ / copy_ kernels emit -- are single instructions of the same
+// width on sm_90 and are read whole in practice (tests/test_gpu_device_gauges.py checks both), but only set_gauge is
+// covered by the memory model.  T must be one of the seven gauge types, matching the dtype registered for p.
+namespace gauge_store {
+template <int N> struct bits;
+template <> struct bits<2> { typedef unsigned short type; };
+template <> struct bits<4> { typedef unsigned int type; };
+template <> struct bits<8> { typedef unsigned long long type; };
+__device__ __forceinline__ void st(void *p, unsigned short u) {
+    asm volatile("st.relaxed.gpu.b16 [%0], %1;" :: "l"(p), "h"(u) : "memory");
+}
+__device__ __forceinline__ void st(void *p, unsigned int u) {
+    asm volatile("st.relaxed.gpu.b32 [%0], %1;" :: "l"(p), "r"(u) : "memory");
+}
+__device__ __forceinline__ void st(void *p, unsigned long long u) {
+    asm volatile("st.relaxed.gpu.b64 [%0], %1;" :: "l"(p), "l"(u) : "memory");
+}
+}  // namespace gauge_store
+
+template <typename T>
+__device__ __forceinline__ void set_gauge(T *p, T v) {
+    static_assert(sizeof(T) == 2 || sizeof(T) == 4 || sizeof(T) == 8, "a gauge is a 2-, 4- or 8-byte scalar");
+    typename gauge_store::bits<(int)sizeof(T)>::type u;
+    __builtin_memcpy(&u, &v, sizeof u);
+    gauge_store::st(p, u);
+}
+
 }  // namespace lh

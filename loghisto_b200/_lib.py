@@ -131,6 +131,14 @@ class lh_board(C.Structure):
                 ("bytes", C.c_uint64)]
 
 
+LH_GAUGE_F64, LH_GAUGE_F32, LH_GAUGE_F16, LH_GAUGE_BF16, LH_GAUGE_I64, LH_GAUGE_I32, LH_GAUGE_U64 = range(7)
+
+
+class lh_gauge_src(C.Structure):
+    """One device gauge of lh_gauges_read: a scalar of dtype LH_GAUGE_* at d_value (include/loghisto_b200.h)."""
+    _fields_ = [("d_value", C.c_void_p), ("dtype", C.c_uint32), ("reserved", C.c_uint32)]
+
+
 _vp, _sz, _u32, _u64, _i32 = C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint64, C.c_int32
 
 # name -> (restype, argtypes); every symbol include/loghisto_b200.h declares
@@ -168,6 +176,7 @@ SIGNATURES = {
     "lh_snapshot_publish": (_i32, [_vp, C.POINTER(lh_board), _vp, _vp, _vp]),
     "lh_board_read": (_i32, [_vp, C.POINTER(lh_board), _vp, _vp]),
     "lh_board_destroy": (_i32, [_vp, C.POINTER(lh_board)]),
+    "lh_gauges_read": (_i32, [_vp, C.POINTER(lh_gauge_src), _u32, _vp]),
     "lh_gpu_timer_start": (_i32, [_vp, _vp, C.POINTER(lh_gpu_timer)]),
     "lh_gpu_timer_stop": (_i32, [_vp, C.POINTER(lh_gpu_timer), _u32, _vp, _vp]),
     "lh_gpu_timer_release": (_i32, [_vp, C.POINTER(lh_gpu_timer)]),

@@ -264,6 +264,13 @@ struct lh_ctx {
     uint64_t next_board = 1;
     int pub_slot = -1;
     BoardParams board_prm{};
+    // device gauges (lh_gauges_read): calls are serialised by gauge_mu (taken before mu), since they share the output
+    // buffer, mapped pinned memory that k_gauge_read writes into (grown on demand); gauge_done follows the last launch
+    std::mutex gauge_mu;
+    double *h_gauges = nullptr, *d_gauges = nullptr;
+    uint32_t gauge_cap = 0;
+    cudaEvent_t gauge_done = nullptr;
+    GaugeParams gauge_prm{};
     // stats
     lh_stats stats{};
     std::mutex mu;
@@ -1100,6 +1107,8 @@ extern "C" lh_status lh_destroy(lh_ctx *ctx) {
     cudaDeviceSynchronize();
     for (auto &g : ctx->graphs) cudaFree(g.rec.d_buckets);
     for (auto &b : ctx->boards) cudaFree(b.d_board);
+    if (ctx->h_gauges) cudaFreeHost(ctx->h_gauges);
+    if (ctx->gauge_done) cudaEventDestroy(ctx->gauge_done);
     if (ctx->graph_drained) cudaEventDestroy(ctx->graph_drained);
     comm_unmap(ctx);
     cudaFree(ctx->d_comm); cudaFree(ctx->d_comm_aux);
@@ -2059,6 +2068,74 @@ extern "C" lh_status lh_board_destroy(lh_ctx *ctx, const lh_board *b) {
     if (!bd) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign board");
     LH_CUDA(ctx, cudaFreeAsync(bd->d_board, ctx->snap_stream));   // after every publish issued (all on this stream)
     ctx->boards.erase(ctx->boards.begin() + (bd - ctx->boards.data()));
+    return LH_OK;
+}
+
+// =========================================================== device gauges
+namespace {
+constexpr uint32_t kGaugeBytes[] = {8, 4, 2, 2, 8, 4, 8};   // by LH_GAUGE_*
+static_assert(sizeof(GaugeEntry) == sizeof(lh_gauge_src), "one table entry per lh_gauge_src");
+
+// LH_OK when k_gauge_read may load the entry: a known dtype, a naturally aligned address in device or managed memory of
+// the context's device.  Anything else could fault the kernel, so it is refused before any launch.
+lh_status check_gauge(lh_ctx *ctx, uint32_t i, const lh_gauge_src &s) {
+    char what[160];
+    if (s.dtype >= sizeof kGaugeBytes / sizeof kGaugeBytes[0] || s.reserved) {
+        snprintf(what, sizeof what, "gauge %u: unknown dtype %u or non-zero reserved", i, s.dtype);
+        return fail(ctx, LH_ERR_INVALID, what);
+    }
+    if (!s.d_value || ((uintptr_t)s.d_value & (kGaugeBytes[s.dtype] - 1u))) {
+        snprintf(what, sizeof what, "gauge %u: d_value is NULL or not %u-byte aligned", i, kGaugeBytes[s.dtype]);
+        return fail(ctx, LH_ERR_INVALID, what);
+    }
+    cudaPointerAttributes a{};
+    const cudaError_t e = cudaPointerGetAttributes(&a, s.d_value);
+    if (e != cudaSuccess) cudaGetLastError();
+    if (e != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != ctx->device) {
+        snprintf(what, sizeof what, "gauge %u: d_value is not device or managed memory of device %d", i, ctx->device);
+        return fail(ctx, LH_ERR_INVALID, what);
+    }
+    return LH_OK;
+}
+}  // namespace
+
+extern "C" lh_status lh_gauges_read(lh_ctx *ctx, const lh_gauge_src *h_srcs, uint32_t n, double *h_out) {
+    if (!ctx) return LH_ERR_INVALID;
+    std::lock_guard<std::mutex> one_read(ctx->gauge_mu);
+    LH_ENTER(ctx);
+    if (n && (!h_srcs || !h_out)) return fail(ctx, LH_ERR_INVALID, "h_srcs / h_out is NULL");
+    for (uint32_t i = 0; i < n; i++)
+        if (lh_status st = check_gauge(ctx, i, h_srcs[i]); st != LH_OK) return st;
+    if (n == 0) return LH_OK;
+    if (n > ctx->gauge_cap) {
+        const uint32_t cap = std::max<uint32_t>(n, 4096);
+        if (ctx->h_gauges) cudaFreeHost(ctx->h_gauges);   // no read is in flight: every call waits for its launches
+        ctx->h_gauges = ctx->d_gauges = nullptr;
+        ctx->gauge_cap = 0;
+        LH_CUDA(ctx, cudaHostAlloc((void **)&ctx->h_gauges, (size_t)cap * 8u, cudaHostAllocMapped));
+        LH_CUDA(ctx, cudaHostGetDevicePointer((void **)&ctx->d_gauges, ctx->h_gauges, 0));
+        ctx->gauge_cap = cap;
+    }
+    if (!ctx->gauge_done) LH_CUDA(ctx, cudaEventCreateWithFlags(&ctx->gauge_done, cudaEventDisableTiming));
+    cudaStream_t s = ctx->snap_stream;
+    GaugeParams &p = ctx->gauge_prm;
+    for (uint32_t i0 = 0; i0 < n; i0 += GR_MAX_ENTRIES) {
+        const uint32_t m = std::min<uint32_t>(GR_MAX_ENTRIES, n - i0);
+        p.out = ctx->d_gauges + i0;
+        p.n = m;
+        for (uint32_t j = 0; j < m; j++) p.e[j] = GaugeEntry{h_srcs[i0 + j].d_value, h_srcs[i0 + j].dtype, 0u};
+        k_gauge_read<<<(m + GR_THREADS - 1) / GR_THREADS, GR_THREADS, 0, s>>>(p);
+        LH_CUDA(ctx, cudaGetLastError());
+        ctx->stats.kernel_launches++;
+    }
+    LH_CUDA(ctx, cudaEventRecord(ctx->gauge_done, s));
+    // wait outside the lock so ingest threads are not held up; gauge_mu keeps the buffer ours
+    cudaEvent_t ev = ctx->gauge_done;
+    _lk.unlock();
+    const cudaError_t e = cudaEventSynchronize(ev);
+    _lk.lock();
+    if (e != cudaSuccess) return fail(ctx, LH_ERR_CUDA, "cudaEventSynchronize(gauges)", e);
+    memcpy(h_out, ctx->h_gauges, (size_t)n * 8u);
     return LH_OK;
 }
 

@@ -1945,6 +1945,71 @@ k_board_read(const unsigned long long *__restrict__ board, unsigned long long *_
     }
 }
 
+// ----------------------------------------------------------- device gauges (lh_gauges_read)
+// One thread per gauge.  Each value is read with one naturally aligned ld.relaxed.gpu (a strong load: never torn
+// against a strong store of the same size, and served from L2, never from a stale L1 line), then converted to float64
+// as Go's float64(x) does: exact widening for f32 (and f16 / bf16 through f32) and s32, cvt.rn for s64 / u64.  The
+// table comes by value in the parameter block; the values go to host-mapped pinned memory.
+constexpr int GR_THREADS = 128;
+constexpr int GR_MAX_ENTRIES = 1024;         // entries per launch: 16 B each in the parameter block
+
+struct GaugeEntry {
+    const void *p;
+    uint32_t dtype;                          // LH_GAUGE_*, checked on the host
+    uint32_t reserved;
+};
+struct GaugeParams {
+    double *out;                             // [n], device view of mapped pinned memory
+    uint32_t n, reserved;
+    GaugeEntry e[GR_MAX_ENTRIES];
+};
+
+namespace gauge {
+__device__ __forceinline__ unsigned long long ld64(const void *p) {
+    unsigned long long v;
+    asm volatile("ld.relaxed.gpu.b64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ uint32_t ld32(const void *p) {
+    uint32_t v;
+    asm volatile("ld.relaxed.gpu.b32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ unsigned short ld16(const void *p) {
+    unsigned short v;
+    asm volatile("ld.relaxed.gpu.b16 %0, [%1];" : "=h"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ double f32(float x) {   // exact, subnormals kept (no .ftz)
+    double d;
+    asm("cvt.f64.f32 %0, %1;" : "=d"(d) : "f"(x));
+    return d;
+}
+}  // namespace gauge
+
+__global__ void __launch_bounds__(GR_THREADS)
+k_gauge_read(const __grid_constant__ GaugeParams p) {
+    const uint32_t i = blockIdx.x * GR_THREADS + threadIdx.x;
+    if (i >= p.n) return;
+    const GaugeEntry e = p.e[i];
+    double v;
+    switch (e.dtype) {
+    case LH_GAUGE_F64: v = __longlong_as_double((long long)gauge::ld64(e.p)); break;
+    case LH_GAUGE_F32: v = gauge::f32(__uint_as_float(gauge::ld32(e.p))); break;
+    case LH_GAUGE_F16: {
+        float f;
+        asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(gauge::ld16(e.p)));
+        v = gauge::f32(f);
+        break;
+    }
+    case LH_GAUGE_BF16: v = gauge::f32(__uint_as_float((uint32_t)gauge::ld16(e.p) << 16)); break;
+    case LH_GAUGE_I64: asm("cvt.rn.f64.s64 %0, %1;" : "=d"(v) : "l"(gauge::ld64(e.p))); break;
+    case LH_GAUGE_I32: asm("cvt.rn.f64.s32 %0, %1;" : "=d"(v) : "r"(gauge::ld32(e.p))); break;
+    default: asm("cvt.rn.f64.u64 %0, %1;" : "=d"(v) : "l"(gauge::ld64(e.p))); break;   // LH_GAUGE_U64
+    }
+    p.out[i] = v;
+}
+
 // ----------------------------------------------------------- GPU timers (lh_gpu_timer_*)
 // One thread each: their cost is the launch, not the body.  The start writes %globaltimer into the token's slot; the
 // stop records float64(now - start) into one histogram row through the same bucket function and row writer every

@@ -305,6 +305,26 @@ def board_views(buf, k: int, kc: int) -> dict:
     }
 
 
+_GAUGE_DTYPES = {"torch.float64": L.LH_GAUGE_F64, "torch.float32": L.LH_GAUGE_F32, "torch.float16": L.LH_GAUGE_F16,
+                 "torch.bfloat16": L.LH_GAUGE_BF16, "torch.int64": L.LH_GAUGE_I64, "torch.int32": L.LH_GAUGE_I32,
+                 "torch.uint64": L.LH_GAUGE_U64}
+
+
+def gauge_src(t, device: int) -> tuple:
+    """(address, LH_GAUGE_* dtype) of a device gauge: a CUDA tensor (or a view such as t[i]) with exactly one element,
+    on `device`, of dtype float64 / float32 / float16 / bfloat16 / int64 / int32 / uint64.  TypeError otherwise."""
+    if not (hasattr(t, "is_cuda") and hasattr(t, "data_ptr")):
+        raise TypeError(f"a device gauge is a CUDA tensor, not {type(t)!r}")
+    if not t.is_cuda or t.device.index != device:
+        raise TypeError(f"a device gauge must be on cuda:{device}, not {t.device}")
+    if t.numel() != 1:
+        raise TypeError(f"a device gauge has exactly one element, not {t.numel()}")
+    dtype = _GAUGE_DTYPES.get(str(t.dtype))
+    if dtype is None:
+        raise TypeError(f"a device gauge must be float64/32/16, bfloat16, int64/32 or uint64, not {t.dtype}")
+    return int(t.data_ptr()), dtype
+
+
 class Board:
     """A device subscription board of an Engine (Engine.board): `board` is the lh_board to pass by value to kernels,
     which read it with lh::read_histogram / lh::read_counter."""
@@ -578,6 +598,17 @@ class Engine:
     def board(self, k: int = 0, kc: int = 0) -> "Board":
         """A device subscription board of k histogram rows and kc counter rows (lh_board_create)."""
         return Board(self, k, kc)
+
+    def read_gauges(self, tensors) -> np.ndarray:
+        """lh_gauges_read of one-element CUDA tensors (gauge_src): float64(value) of each, read on the snapshot stream
+        without waiting for any other stream."""
+        tensors = list(tensors)
+        srcs = (L.lh_gauge_src * max(len(tensors), 1))()
+        for i, t in enumerate(tensors):
+            srcs[i].d_value, srcs[i].dtype = gauge_src(t, self.device)
+        out = np.empty(len(tensors), dtype=np.float64)
+        self._check(self.lib.lh_gauges_read(self.h, srcs, len(tensors), out.ctypes.data))
+        return out
 
     def gpu_timer_start(self, stream=None) -> L.lh_gpu_timer:
         """Enqueue a start mark on `stream` (None = the ingest stream; torch's default stream is timed as itself)."""

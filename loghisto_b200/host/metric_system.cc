@@ -38,6 +38,8 @@
 #pragma weak lh_snapshot_publish
 #pragma weak lh_board_read
 #pragma weak lh_board_destroy
+// And for device gauges: over a build without them, RegisterDeviceGauge throws.
+#pragma weak lh_gauges_read
 
 namespace loghisto {
 
@@ -969,11 +971,25 @@ GpuTimerToken::~GpuTimerToken() {
 
 void MetricSystem::RegisterGaugeFunc(const std::string &name, std::function<double()> f) {
     std::lock_guard<std::mutex> lk(gauge_mu_);
+    device_gauges_.erase(name);
     gauge_funcs_[name] = std::move(f);
+}
+void MetricSystem::RegisterDeviceGauge(const std::string &name, const void *d_value, uint32_t dtype) {
+    if (!lh_gauges_read) throw std::runtime_error("RegisterDeviceGauge: this libloghisto_b200 has no device gauges");
+    const lh_gauge_src src{d_value, dtype, 0u};
+    double v = 0;
+    const lh_status st = lh_gauges_read(ctx_, &src, 1, &v);
+    if (st == LH_ERR_INVALID)
+        throw std::invalid_argument(std::string("RegisterDeviceGauge(") + name + "): " + lh_last_error(ctx_));
+    check(ctx_, st, "lh_gauges_read");
+    std::lock_guard<std::mutex> lk(gauge_mu_);
+    gauge_funcs_.erase(name);
+    device_gauges_[name] = src;
 }
 void MetricSystem::DeregisterGaugeFunc(const std::string &name) {
     std::lock_guard<std::mutex> lk(gauge_mu_);
     gauge_funcs_.erase(name);
+    device_gauges_.erase(name);
 }
 
 // commit whatever the shard holds and hand over (and clear) its touched-counter marks
@@ -1108,6 +1124,18 @@ std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
     {
         std::lock_guard<std::mutex> lk(gauge_mu_);
         for (auto &g : gauge_funcs_) raw->Gauges[g.first] = g.second();   // :465-470
+        if (!device_gauges_.empty()) {   // every device gauge in one read; none at all when it fails
+            std::vector<lh_gauge_src> srcs;
+            srcs.reserve(device_gauges_.size());
+            for (auto &g : device_gauges_) srcs.push_back(g.second);
+            std::vector<double> vals(srcs.size());
+            if (lh_gauges_read(ctx_, srcs.data(), (uint32_t)srcs.size(), vals.data()) == LH_OK) {
+                size_t i = 0;
+                for (auto &g : device_gauges_) raw->Gauges[g.first] = vals[i++];
+            } else {   // the host's metric set is still delivered
+                fprintf(stderr, "loghisto: lh_gauges_read failed: %s\n", lh_last_error(ctx_));
+            }
+        }
     }
     return raw;
 }
@@ -1389,6 +1417,26 @@ LHMS_API void lhms_specify_percentiles(void *ms, int n, const char *const *label
 }
 LHMS_API void lhms_register_constant_gauge(void *ms, const char *name, double v) {
     static_cast<MetricSystem *>(ms)->RegisterGaugeFunc(name, [v] { return v; });
+}
+// RegisterDeviceGauge: LH_OK, LH_ERR_INVALID when the address or dtype is refused, LH_ERR_STATE for any other failure.
+LHMS_API int lhms_register_device_gauge(void *ms, const char *name, const void *d_value, uint32_t dtype) {
+    if (!ms || !name) return LH_ERR_INVALID;
+    try {
+        static_cast<MetricSystem *>(ms)->RegisterDeviceGauge(name, d_value, dtype);
+        return LH_OK;
+    } catch (const std::invalid_argument &) {
+        return LH_ERR_INVALID;
+    } catch (const std::exception &) {
+        return LH_ERR_STATE;
+    }
+}
+// DeregisterGaugeFunc: removes a gauge function or a device gauge
+LHMS_API void lhms_deregister_gauge(void *ms, const char *name) {
+    static_cast<MetricSystem *>(ms)->DeregisterGaugeFunc(name);
+}
+// lh_get_stats of the system's context (e.g. the kernel launches a collection issues)
+LHMS_API int lhms_stats(void *ms, lh_stats *out) {
+    return lh_get_stats(static_cast<MetricSystem *>(ms)->context(), out);
 }
 
 static void emit_raw(const RawMetricSet &raw, lhms_emit_fn emit, void *ctx) {

@@ -7,7 +7,8 @@
 //
 // Differences from the Go type, all outside the hot path:
 //   * sysStats gauges (sys.Alloc, sys.NumGC, ... metrics.go:172-193) are Go-runtime facts and are not provided;
-//     RegisterGaugeFunc / DeregisterGaugeFunc work as in the reference.
+//     RegisterGaugeFunc / DeregisterGaugeFunc work as in the reference, and RegisterDeviceGauge adds gauges whose
+//     values live in device memory.
 //   * channels are loghisto::Channel<T>: bounded, non-blocking send, closable (Go's `select { case ch <- x: default: }`).
 //   * names map to dense ids on the device, and ids of idle names are recycled (NameTable below): max_histograms /
 //     max_counters bound the distinct names used in any three consecutive intervals.  The reference has no limit.
@@ -337,7 +338,15 @@ class MetricSystem {
     DeviceSubscription NewDeviceSubscription(const std::vector<std::string> &histograms,
                                              const std::vector<std::string> &counters);
     void RegisterGaugeFunc(const std::string &name, std::function<double()> f);   // :299
-    void DeregisterGaugeFunc(const std::string &name);                    // :306
+    // A gauge whose value lives in device memory: a scalar of type `dtype` (LH_GAUGE_*) at d_value, device or managed
+    // memory of this system's device, which must stay allocated while registered.  Every collection reads all device
+    // gauges in one lh_gauges_read, which waits for no caller stream, and puts float64(value) in Gauges under `name`,
+    // as a RegisterGaugeFunc value.  Gauge functions and device gauges share one name space: registering either kind
+    // replaces the other under that name.  Throws std::invalid_argument when lh_gauges_read refuses the address or dtype
+    // (checked with one read now, so a bad pointer never reaches a collection), std::runtime_error when this
+    // libloghisto_b200 has no device gauges or the read fails otherwise.
+    void RegisterDeviceGauge(const std::string &name, const void *d_value, uint32_t dtype);
+    void DeregisterGaugeFunc(const std::string &name);                    // :306, device gauges too
     void Start();                                                         // :644
     void Stop();                                                          // :651
 
@@ -437,8 +446,10 @@ class MetricSystem {
     std::mutex histogram_count_mu_;
     std::map<std::string, uint64_t> histogram_count_store_;    // metrics.go:122-126
 
+    // held across a collection's device read, so a gauge deregistered (and then freed) is never read
     std::mutex gauge_mu_;
     std::map<std::string, std::function<double()>> gauge_funcs_;
+    std::map<std::string, lh_gauge_src> device_gauges_;   // no name is in both maps
 
     std::mutex subscribers_mu_;
     std::vector<std::shared_ptr<Channel<std::shared_ptr<RawMetricSet>>>> raw_subscribers_;

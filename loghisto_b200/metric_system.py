@@ -10,7 +10,7 @@ import ctypes as C
 
 from . import _lib as _L
 from . import build as _build
-from .engine import _batch_array, _capture_stream, _stream, _timer_stream, board_out, board_views
+from .engine import _batch_array, _capture_stream, _stream, _timer_stream, board_out, board_views, gauge_src
 
 _EMIT = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_char_p, C.c_int, C.c_uint64, C.c_double)
 _lib = None
@@ -43,6 +43,11 @@ def _bind(L):
     L.lhms_timer_stop.argtypes = [vp]
     L.lhms_specify_percentiles.argtypes = [vp, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_double)]
     L.lhms_register_constant_gauge.argtypes = [vp, C.c_char_p, C.c_double]
+    L.lhms_register_device_gauge.restype = C.c_int
+    L.lhms_register_device_gauge.argtypes = [vp, C.c_char_p, vp, C.c_uint32]
+    L.lhms_deregister_gauge.argtypes = [vp, C.c_char_p]
+    L.lhms_stats.restype = C.c_int
+    L.lhms_stats.argtypes = [vp, C.POINTER(_L.lh_stats)]
     L.lhms_collect_and_process.restype = C.c_int
     L.lhms_collect_and_process.argtypes = [vp, _EMIT, vp, C.c_char_p, C.c_int]
     names, u64p = C.POINTER(C.c_char_p), C.POINTER(C.c_uint64)
@@ -411,11 +416,13 @@ class MetricSystem:
         if not self._h:
             raise RuntimeError(err.value.decode())
         self._device = device
+        self._device_gauges = {}   # name -> tensor: keeps the memory of every registered device gauge allocated
 
     def close(self):
         if self._h:
             self._lib.lhms_free(self._h)
             self._h = None
+            self._device_gauges.clear()
 
     def __del__(self):
         try:
@@ -498,6 +505,25 @@ class MetricSystem:
 
     def RegisterConstantGauge(self, name: str, value: float):
         self._lib.lhms_register_constant_gauge(self._h, name.encode(), float(value))
+        self._device_gauges.pop(name, None)
+
+    def RegisterDeviceGauge(self, name: str, tensor):
+        """A gauge whose value lives on the GPU: `tensor` is a CUDA tensor (or a view such as t[i]) with exactly one
+        element, on this system's device, of dtype float64 / float32 / float16 / bfloat16 / int64 / int32 / uint64
+        (TypeError otherwise).  Every collection reads all device gauges in one kernel that waits for no stream, and puts
+        float64(value) in Gauges under `name`.  Replaces a gauge of either kind under that name.  The system keeps a
+        reference to the tensor while it is registered, so its memory is not reused."""
+        ptr, dtype = gauge_src(tensor, self._device)
+        st = self._lib.lhms_register_device_gauge(self._h, name.encode(), ptr, dtype)
+        if st != 0:
+            raise (ValueError if st == _L.LH_ERR_INVALID else RuntimeError)(
+                "lhms_register_device_gauge refused %r (status %d)" % (name, st))
+        self._device_gauges[name] = tensor
+
+    def DeregisterGaugeFunc(self, name: str):
+        """Removes the gauge registered under `name`, a function or a device gauge (metrics.go:306)."""
+        self._lib.lhms_deregister_gauge(self._h, name.encode())
+        self._device_gauges.pop(name, None)
 
     def SubscribeToProcessedMetrics(self, capacity: int = 128) -> Subscription:
         return Subscription(self, "processed", capacity)
@@ -547,6 +573,13 @@ class MetricSystem:
         if rc != 0:
             raise RuntimeError(err.value.decode())
         return col.metrics
+
+    def stats(self) -> dict:
+        """lh_get_stats of the system's context, as Engine.stats."""
+        st = _L.lh_stats()
+        if self._lib.lhms_stats(self._h, C.byref(st)) != 0:
+            raise RuntimeError("lhms_stats failed")
+        return {f: int(getattr(st, f)) for f, _ in _L.lh_stats._fields_}
 
     def dropped(self) -> int:
         """Samples and counter ops not recorded so far: those of new names that found no free id (more distinct names

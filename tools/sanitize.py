@@ -78,6 +78,15 @@ with lh.Engine(device=0, max_histograms=4, max_counters=2) as e:    # device sub
         v = b.read(stream=0)
         e.sync()
         assert int(v["count"][0].item()) == n and int(v["collection"].item()) == 1
+with lh.Engine(device=0, max_histograms=1, max_counters=1) as e:     # device gauges: a read split over two launches
+    import ctypes as C
+    import numpy as np
+    from loghisto_b200 import _lib as L
+    g = e.upload(np.arange(1025, dtype=np.float64))
+    srcs = (L.lh_gauge_src * 1025)(*[L.lh_gauge_src(g.offset(i), L.LH_GAUGE_F64, 0) for i in range(1025)])
+    vals = np.zeros(1025)
+    e._check(e.lib.lh_gauges_read(e.h, srcs, 1025, vals.ctypes.data))
+    assert (vals == np.arange(1025)).all()
 # two contexts on one device: the peer all-reduce kernel
 engs = [lh.Engine(device=0, max_histograms=3, max_counters=2) for _ in range(2)]
 handles = b"".join(x.comm_export() for x in engs)
