@@ -422,18 +422,6 @@ KeyedOut keyed_out(lh_ctx *ctx, int b) {
     return o;
 }
 
-// The passes of k_ingest_keyed_small over id sub-ranges that cover all H histograms' positive windows.
-uint32_t ks_passes(const lh_ctx *ctx) {
-    const uint32_t per_max = std::max<uint32_t>(1, (uint32_t)(KS_SMEM_BYTES / ((size_t)ctx->pc.win * 4)));
-    return (ctx->H + per_max - 1) / per_max;
-}
-
-// Few histograms: their windows fit in shared memory (K1-style privatisation).  Up to KS_MAX_PASSES passes over id
-// sub-ranges match or beat the L2-atomic kernel (each pass is HBM-bound at 10 B/sample) and, unlike it, do not depend
-// on how clustered the values are.  launch_keyed also wants a vector body of at least 4096 groups of 4.
-constexpr uint32_t KS_MAX_PASSES = 4;
-bool small_route(const lh_ctx *ctx) { return ks_passes(ctx) <= KS_MAX_PASSES && ctx->keyed_mode == 0; }
-
 // The scalar keyed kernel over a ragged piece (a head before the aligned body, a tail after it); nothing when n == 0.
 template <typename IdT, typename ValT>
 void launch_keyed_scalar(lh_ctx *ctx, const KeyedOut &ko, const IdT *ids, const ValT *vals, size_t n, cudaStream_t s) {
@@ -443,10 +431,111 @@ void launch_keyed_scalar(lh_ctx *ctx, const KeyedOut &ko, const IdT *ids, const 
     ctx->stats.kernel_launches++;
 }
 
+// Few histograms: their windows fit in shared memory (K1-style privatisation).  Up to KS_MAX_PASSES passes over id
+// sub-ranges match or beat the L2-atomic kernel (each pass is HBM-bound at 10 B/sample) and, unlike it, do not depend
+// on how clustered the values are.
+constexpr uint32_t KS_MAX_PASSES = 4;
+
 // Owner-partitioned write-combining kernel: used when the histograms cannot be privatised per CTA in a few
 // passes but P owner CTAs (one per SM) can hold them all, and the batch is big enough to amortise the
 // cooperative launch.
 constexpr size_t kSmemBudget = 227 * 1024;
+
+// What launch_keyed issues for one piece of a batch, or launch_keyed_pair for a pair (plan_keyed).
+struct KeyedPlan {
+    // the kernel of the vector body (the ragged ends always go through k_ingest_keyed); APART: a pair the
+    // write-combining kernel does not take, ingested one array after the other
+    enum Route { SCALAR /* no vector body */, SMALL, WC, VEC, APART } route = SCALAR;
+    const char *name = "k_ingest_keyed";  // what lh_keyed_kernel_name reports after the launch
+    size_t head = 0, n4 = 0;              // scalar samples before the vector body (32-byte aligned values), groups of 4 in it
+    size_t taken = 0, taken2 = 0;         // samples the body kernel bins, of each array; the rest is the scalar tail
+    int grid = 0;                         // CTAs: small, or P, the owners of the write-combining kernel
+    size_t smem = 0;                      // dynamic shared memory (small, write-combining)
+    uint32_t per = 0;                     // small: ids per pass
+    int spt = 0, threads = 0;             // write-combining: tile shape (wc_spt resolved to 3, 4, 6 or 8)
+    WcParams wc{};                        // write-combining: the parameter block but for the arrays and the scratch
+};
+
+// The route of keyed samples (ids, vals, n) and everything its launches need; no CUDA call and no change to ctx.
+// A pair (float64 samples ids/vals/n, int64 samples ids2/vals2/n2) is one write-combining launch for both arrays when
+// both are vector-aligned and that kernel takes them, else APART.
+KeyedPlan plan_keyed(const lh_ctx *ctx, size_t id_bytes, const void *ids, const void *vals, size_t n, bool pair = false,
+                     const void *ids2 = nullptr, const void *vals2 = nullptr, size_t n2 = 0) {
+    KeyedPlan p;
+    const uint32_t ks_per_max = std::max<uint32_t>(1, (uint32_t)(KS_SMEM_BYTES / ((size_t)ctx->pc.win * 4)));
+    const uint32_t ks_passes = (ctx->H + ks_per_max - 1) / ks_per_max;
+    const bool small = ks_passes <= KS_MAX_PASSES && ctx->keyed_mode == 0;
+    const uintptr_t id_mask = 4 * id_bytes - 1;
+    if (pair) {
+        // few histograms: the shared-memory privatised kernel of launch_keyed is the better one, per array
+        auto aligned = [&](const void *v, const void *i) { return ((uintptr_t)v & 31u) == 0 && ((uintptr_t)i & id_mask) == 0; };
+        p.route = KeyedPlan::APART;
+        if (!n || !n2 || ctx->keyed_mode == 1 || small || !aligned(vals, ids) || !aligned(vals2, ids2)) return p;
+    } else {
+        // scalar head until the values are 32-byte aligned; the vector body also needs ids aligned to 4 ids
+        p.head = std::min<size_t>(n, ((32u - ((uintptr_t)vals & 31u)) & 31u) / 8u);
+        if (((uintptr_t)ids + p.head * id_bytes) & id_mask) { p.head = 0; return p; }   // misaligned: the scalar kernel only
+        p.n4 = (n - p.head) / 4;
+        if (!p.n4) return p;                                                              // short: the scalar kernel only
+        n = p.taken = p.n4 * 4;                                  // the vector body, all the write-combining kernel is offered
+        if (small && p.n4 >= 4096) {
+            p.route = KeyedPlan::SMALL; p.name = "k_ingest_keyed_small";
+            p.per = (ctx->H + ks_passes - 1) / ks_passes;
+            p.smem = ((size_t)p.per * ctx->pc.win + 4) * 4;
+            // one CTA per SM; fewer when the batch is small, so that the per-CTA flush stays negligible
+            p.grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)(ctx->sm_count - ctx->k1_reserve_sms),
+                                                               p.n4 / (KS_THREADS * 16)));
+            return p;
+        }
+        p.route = KeyedPlan::VEC; p.name = "k_ingest_keyed_vec";
+        if (ctx->keyed_mode == 1) return p;
+    }
+    // the write-combining kernel, or keep the route above when it declines
+    const int P = std::min(ctx->sm_count - ctx->k1_reserve_sms, (int)WC_MAX_PARTS);
+    if (P < 8) return p;
+    const uint32_t ids_per = (ctx->H + P - 1) / P;
+    const size_t hist_bytes = (((size_t)ids_per * ctx->pc.win + 3) & ~(size_t)3) * 4;
+    // the owners' windows first, then the largest per-owner buffers that still fit (fewer SMs for ingest = more ids per
+    // owner = less room; on H100, 256 records at P = 131 for H = 1024)
+    uint32_t row_cap = 0;
+    size_t smem = 0;
+    for (uint32_t cap_try : {256u, 192u, 128u}) {
+        smem = hist_bytes + 2 * WC_MAX_PARTS * 4 + (size_t)(P + 1) * (cap_try + WC_ROW_EXTRA) * 2;
+        if (smem <= kSmemBudget) { row_cap = cap_try; break; }
+    }
+    if (!row_cap || (size_t)ids_per * ctx->pc.win > 65535) return p;           // records are 16-bit (lid*win + slot)
+    if (ctx->keyed_mode != 2 && n + n2 < ((size_t)1 << 22)) return p;          // small batches: the L2-atomic kernel
+    const int spt = ctx->wc_spt == 6 || ctx->wc_spt == 4 || ctx->wc_spt == 3 ? ctx->wc_spt : 8;
+    const int tile = spt == 6 ? WcShape<6>::TILE : spt == 4 ? WcShape<4>::TILE : spt == 3 ? WcShape<3>::TILE : WcShape<8>::TILE;
+    const size_t taken = n / tile * tile, taken2 = n2 / tile * tile;   // whole tiles only
+    if (taken + taken2 == 0) return p;
+    p.route = KeyedPlan::WC; p.name = "k_ingest_keyed_wc";
+    p.taken = taken; p.taken2 = taken2; p.grid = P; p.smem = smem; p.spt = spt;
+    p.threads = spt == 6 ? WcShape<6>::THREADS : spt == 4 ? WcShape<4>::THREADS : spt == 3 ? WcShape<3>::THREADS : WcShape<8>::THREADS;
+    WcParams &w = p.wc;
+    w.n = taken; w.n2 = taken2; w.ids_per = ids_per; w.row_cap = row_cap; w.row_stride = row_cap + WC_ROW_EXTRA;
+    w.inv_p = (uint32_t)(((uint64_t)1 << 32) / (uint64_t)P) + 1u;
+    w.pf_tiles = ctx->wc_pf_tiles;
+    // chunks of about kp_chunk samples, EQUAL in size: with the nominal slice a short last chunk would be binned by a
+    // few CTAs at full slice length while the others idle, a whole chunk time per launch)
+    const size_t slice_max = std::max<size_t>(1, ((size_t)ctx->kp_chunk + (size_t)P * tile - 1) / ((size_t)P * tile));
+    const size_t tiles_all = taken / tile + taken2 / tile;
+    const size_t nchunks = (tiles_all + slice_max * P - 1) / (slice_max * P);
+    w.slice_tiles = (uint32_t)std::max<size_t>(1, (tiles_all + nchunks * P - 1) / (nchunks * P));
+    // every (owner, writer) pair has its own sub-queue: 1.25x the expected records per pair per chunk, plus slack
+    // (records that do not fit take the exact L2 route, so this only trades speed on heavily skewed ids)
+    const size_t expect = slice_max * tile / P;       // sized for the nominal slice: the allocation does not follow the batch size
+    w.cap = (uint32_t)(((expect * 5 / 4 + 3 * WC_LINE + WC_LINE - 1) / WC_LINE) * WC_LINE);
+    // samples between two flushes of the shared-memory owner buffers: the flush costs about the same whatever it moves,
+    // so as many as the buffers hold at 4 sigma (wc_flush_samples; default 24576)
+    // ... and an owner's expected share m of one interval must leave room for the carried-over remainder (< 64) and the
+    // binomial spread: m + 3.5 sqrt(m) + 63 <= row_cap
+    const double room = (double)row_cap - 63.0;
+    const double m_max = std::pow((-3.5 + std::sqrt(3.5 * 3.5 + 4.0 * room)) / 2.0, 2.0);
+    const uint32_t flush_samples = std::min<uint32_t>(ctx->wc_flush_samples, (uint32_t)(m_max * P));
+    w.flush_tiles = std::max<uint32_t>(1u, flush_samples / tile);
+    return p;
+}
 
 // Every write-combining launch on a device is ordered after the previous one, whatever its stream or context.  A
 // context's scratch (record sub-queues, grid-barrier word) is shared by all the streams it ingests from, and a launch
@@ -466,43 +555,14 @@ cudaError_t wc_done_event(int device, cudaEvent_t *out) {
     *out = g_wc_done[device];
     return cudaSuccess;
 }
-// Processes the first *taken samples (whole tiles only); the caller sends the rest to the scalar kernel.
-// Optional second segment (ids2, vals2, n2): int64 nanosecond samples binned by the SAME launch (ValT = double only).
-template <typename IdT, typename ValT, int SPT>
-lh_status launch_keyed_wc_spt(lh_ctx *ctx, int b, const IdT *ids, const ValT *vals, size_t n4x4, cudaStream_t s, bool *used, size_t *taken,
-                              const IdT *ids2 = nullptr, const long long *vals2 = nullptr, size_t n2 = 0, size_t *taken2 = nullptr) {
-    *used = false;
-    *taken = 0;
-    if (taken2) *taken2 = 0;
-    const int P = std::min(ctx->sm_count - ctx->k1_reserve_sms, (int)WC_MAX_PARTS);
-    if (P < 8 || n4x4 + n2 == 0) return LH_OK;
-    const uint32_t ids_per = (ctx->H + P - 1) / P;
-    using S = WcShape<SPT>;
-    const size_t hist_bytes = (((size_t)ids_per * ctx->pc.win + 3) & ~(size_t)3) * 4;
-    // the owners' windows first, then the largest per-owner buffers that still fit (fewer SMs for ingest = more ids per
-    // owner = less room; on H100, 256 records at P = 131 for H = 1024)
-    uint32_t row_cap = 0;
-    size_t smem = 0;
-    for (uint32_t cap_try : {256u, 192u, 128u}) {
-        smem = hist_bytes + 2 * WC_MAX_PARTS * 4 + (size_t)(P + 1) * (cap_try + WC_ROW_EXTRA) * 2;
-        if (smem <= kSmemBudget) { row_cap = cap_try; break; }
-    }
-    if (!row_cap || (size_t)ids_per * ctx->pc.win > 65535) return LH_OK;               // records are 16-bit (lid*win + slot)
-    if (ctx->keyed_mode != 2 && n4x4 + n2 < ((size_t)1 << 22)) return LH_OK;           // small batches: the L2-atomic kernel
-    n4x4 = n4x4 / S::TILE * S::TILE;
-    n2 = n2 / S::TILE * S::TILE;
-    if (n4x4 + n2 == 0) return LH_OK;
-    // chunks of about kp_chunk samples, EQUAL in size: with the nominal slice a short last chunk would be binned by a
-    // few CTAs at full slice length while the others idle, a whole chunk time per launch)
-    const size_t slice_max = std::max<size_t>(1, ((size_t)ctx->kp_chunk + (size_t)P * S::TILE - 1) / ((size_t)P * S::TILE));
-    const size_t tiles_all = n4x4 / S::TILE + n2 / S::TILE;
-    const size_t nchunks = (tiles_all + slice_max * P - 1) / (slice_max * P);
-    const size_t slice_tiles = std::max<size_t>(1, (tiles_all + nchunks * P - 1) / (nchunks * P));
-    // every (owner, writer) pair has its own sub-queue: 1.25x the expected records per pair per chunk, plus slack
-    // (records that do not fit take the exact L2 route, so this only trades speed on heavily skewed ids)
-    const size_t expect = slice_max * S::TILE / P;       // sized for the nominal slice: the allocation does not follow the batch size
-    const size_t cap = ((expect * 5 / 4 + 3 * WC_LINE + WC_LINE - 1) / WC_LINE) * WC_LINE;
-    if (!ctx->d_kp_queues || ctx->kp_cap != cap || ctx->kp_parts != P) {
+
+// The write-combining launch of plan p: its first p.taken samples of (ids, vals) and, in a fused pair, the first
+// p.taken2 int64 samples of (ids2, vals2).
+template <typename IdT, typename ValT>
+lh_status launch_keyed_wc(lh_ctx *ctx, int b, const KeyedPlan &p, const IdT *ids, const ValT *vals, cudaStream_t s,
+                          const IdT *ids2 = nullptr, const long long *vals2 = nullptr) {
+    const int P = p.grid;
+    if (!ctx->d_kp_queues || ctx->kp_cap != p.wc.cap || ctx->kp_parts != P) {
         if (ctx->d_kp_queues) {
             // a launch on another stream may still be using the old scratch
             cudaEvent_t done;
@@ -515,34 +575,20 @@ lh_status launch_keyed_wc_spt(lh_ctx *ctx, int b, const IdT *ids, const ValT *va
         cudaFree(ctx->d_kp_queues); cudaFree(ctx->d_kp_cnt); cudaFree(ctx->d_kp_rare);
         ctx->d_kp_queues = nullptr; ctx->d_kp_cnt = nullptr; ctx->d_kp_rare = nullptr;
         LH_CUDA(ctx, cudaMalloc(&ctx->d_kp_rare, (size_t)P * WC_RARE_CAP * sizeof(uint4)));
-        LH_CUDA(ctx, cudaMalloc(&ctx->d_kp_queues, (size_t)2 * P * P * cap * sizeof(unsigned short)));
+        LH_CUDA(ctx, cudaMalloc(&ctx->d_kp_queues, (size_t)2 * P * P * p.wc.cap * sizeof(unsigned short)));
         LH_CUDA(ctx, cudaMalloc(&ctx->d_kp_cnt, ((size_t)2 * P * P + 1) * sizeof(unsigned int)));
-        ctx->kp_cap = cap; ctx->kp_parts = P;
+        ctx->kp_cap = p.wc.cap; ctx->kp_parts = P;
     }
-    const void *fn = (const void *)k_ingest_keyed_wc<IdT, ValT, SPT, false>;
-    if constexpr (std::is_same<ValT, double>::value) {
-        if (n2) fn = (const void *)k_ingest_keyed_wc<IdT, double, SPT, true>;
-    }
+    // the kernel of the planned tile shape; with an int64 second segment, its PAIR form (on the float64 instantiation)
+#define LH_WC_KERNEL(SPT) (!p.taken2 ? (const void *)k_ingest_keyed_wc<IdT, ValT, SPT, false> : (const void *)k_ingest_keyed_wc<IdT, double, SPT, true>)
+    const void *fn = p.spt == 6 ? LH_WC_KERNEL(6) : p.spt == 4 ? LH_WC_KERNEL(4) : p.spt == 3 ? LH_WC_KERNEL(3) : LH_WC_KERNEL(8);
+#undef LH_WC_KERNEL
     // the attribute belongs to the function on the device, not to this context: one value for every context
     LH_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
-    unsigned int *d_barrier = ctx->d_kp_cnt + (size_t)2 * P * P;
-    WcParams prm{};
-    prm.ids = ids; prm.vals = vals; prm.n = n4x4; prm.ids_per = ids_per; prm.cap = (uint32_t)cap;
-    prm.ids2 = ids2; prm.vals2 = vals2; prm.n2 = n2;
-    prm.inv_p = (uint32_t)(((uint64_t)1 << 32) / (uint64_t)P) + 1u;
-    // samples between two flushes of the shared-memory owner buffers: the flush costs about the same whatever it moves,
-    // so as many as the buffers hold at 4 sigma (wc_flush_samples; default 24576)
-    // ... and an owner's expected share m of one interval must leave room for the carried-over remainder (< 64) and the
-    // binomial spread: m + 3.5 sqrt(m) + 63 <= row_cap
-    const double room = (double)row_cap - 63.0;
-    const double m_max = std::pow((-3.5 + std::sqrt(3.5 * 3.5 + 4.0 * room)) / 2.0, 2.0);
-    const uint32_t flush_samples = std::min<uint32_t>(ctx->wc_flush_samples, (uint32_t)(m_max * P));
-    prm.flush_tiles = std::max<uint32_t>(1u, flush_samples / S::TILE);
-    prm.pf_tiles = ctx->wc_pf_tiles;
-    prm.row_cap = row_cap;
-    prm.row_stride = row_cap + WC_ROW_EXTRA;
-    prm.slice_tiles = (uint32_t)slice_tiles; prm.queues = ctx->d_kp_queues; prm.q_cnt = ctx->d_kp_cnt;
-    prm.barrier = d_barrier; prm.rare = ctx->d_kp_rare; prm.o = keyed_out(ctx, b);
+    WcParams prm = p.wc;
+    prm.ids = ids; prm.vals = vals; prm.ids2 = ids2; prm.vals2 = vals2;
+    prm.queues = ctx->d_kp_queues; prm.q_cnt = ctx->d_kp_cnt; prm.barrier = ctx->d_kp_cnt + (size_t)2 * P * P;
+    prm.rare = ctx->d_kp_rare; prm.o = keyed_out(ctx, b);
     Prec pc = ctx->pc;
     void *args[] = {&prm, &pc};
     {
@@ -550,25 +596,12 @@ lh_status launch_keyed_wc_spt(lh_ctx *ctx, int b, const IdT *ids, const ValT *va
         cudaEvent_t done;
         LH_CUDA(ctx, wc_done_event(ctx->device, &done));
         LH_CUDA(ctx, cudaStreamWaitEvent(s, done, 0));
-        LH_CUDA(ctx, cudaMemsetAsync(d_barrier, 0, sizeof(unsigned int), s));
-        LH_CUDA(ctx, cudaLaunchCooperativeKernel(fn, dim3(P), dim3(S::THREADS), args, smem, s));
+        LH_CUDA(ctx, cudaMemsetAsync(prm.barrier, 0, sizeof(unsigned int), s));
+        LH_CUDA(ctx, cudaLaunchCooperativeKernel(fn, dim3(P), dim3(p.threads), args, p.smem, s));
         LH_CUDA(ctx, cudaEventRecord(done, s));
     }
     ctx->stats.kernel_launches++;
-    *used = true;
-    *taken = n4x4;
-    if (taken2) *taken2 = n2;
     return LH_OK;
-}
-template <typename IdT, typename ValT>
-lh_status launch_keyed_wc(lh_ctx *ctx, int b, const IdT *ids, const ValT *vals, size_t n4x4, cudaStream_t s, bool *used, size_t *taken,
-                          const IdT *ids2 = nullptr, const long long *vals2 = nullptr, size_t n2 = 0, size_t *taken2 = nullptr) {
-#define LH_WC_SHAPE(code) case code: return launch_keyed_wc_spt<IdT, ValT, code>(ctx, b, ids, vals, n4x4, s, used, taken, ids2, vals2, n2, taken2);
-    switch (ctx->wc_spt) {
-        LH_WC_SHAPE(6) LH_WC_SHAPE(4) LH_WC_SHAPE(3)
-        default: return launch_keyed_wc_spt<IdT, ValT, 8>(ctx, b, ids, vals, n4x4, s, used, taken, ids2, vals2, n2, taken2);
-    }
-#undef LH_WC_SHAPE
 }
 
 template <typename IdT, typename ValT>
@@ -590,58 +623,30 @@ lh_status launch_keyed(lh_ctx *ctx, int b, const IdT *d_ids, const ValT *d_vals,
         size_t m = (size_t)std::min<unsigned long long>(n - done, kCap - ctx->buf[b].hot_pending);
         const IdT *ids = d_ids + done;
         const ValT *vals = d_vals + done;
-        // scalar head until the values are 32-byte aligned; the vector body also needs ids aligned to 4 ids
-        size_t head = std::min<size_t>(m, ((32u - ((uintptr_t)vals & 31u)) & 31u) / 8u);
-        bool vec_ok = (((uintptr_t)(ids + head)) & (4 * sizeof(IdT) - 1)) == 0;
-        size_t n4 = vec_ok ? (m - head) / 4 : 0;
-        size_t tail_off = head + n4 * 4;
-        if (!vec_ok) { head = 0; tail_off = 0; }
-        launch_keyed_scalar(ctx, ko, ids, vals, head, s);
-        size_t hot_used = 0;
-        if (n4) {
-            bool used = false;
-            if (small_route(ctx) && n4 >= 4096) {
-                const uint32_t passes = ks_passes(ctx);
-                const uint32_t per = (ctx->H + passes - 1) / passes;
-                const size_t smem = ((size_t)per * ctx->pc.win + 4) * 4;
-                const void *fn = (const void *)k_ingest_keyed_small<IdT, ValT>;
-                // per device, not per context: a value of this context's H could be overwritten by another context's
-                // between here and the launch
-                LH_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
-                // one CTA per SM; fewer when the batch is small, so that the per-CTA flush stays negligible
-                int grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)(ctx->sm_count - ctx->k1_reserve_sms),
-                                                                      n4 / (KS_THREADS * 16)));
-                for (uint32_t lo = 0; lo < ctx->H; lo += per) {
-                    const uint32_t cnt = std::min(per, ctx->H - lo);
-                    k_ingest_keyed_small<IdT, ValT><<<grid, KS_THREADS, smem, s>>>(ids + head, vals + head, n4, lo, cnt, ko, ctx->pc);
-                    ctx->stats.kernel_launches++;
-                }
-                used = true;
-                hot_used = n4 * 4;
-                ctx->keyed_kernel = "k_ingest_keyed_small";
-            }
-            if (!used && ctx->keyed_mode != 1) {
-                size_t taken = 0;
-                lh_status st = launch_keyed_wc<IdT, ValT>(ctx, b, ids + head, vals + head, n4 * 4, s, &used, &taken);
-                if (st != LH_OK) return st;
-                if (used) {
-                    ctx->keyed_kernel = "k_ingest_keyed_wc";
-                    tail_off = head + taken;          // whole tiles only: the ragged remainder goes through the scalar kernel below
-                }
-            }
-            if (!used) {
-                int grid = grid_1d(ctx, n4, T, 1, ctx->keyed_blocks_per_sm);
-                k_ingest_keyed_vec<IdT, ValT, T><<<grid, T, 0, s>>>(ids + head, vals + head, n4, ctx->hot_replicas, ko, ctx->pc);
+        const KeyedPlan p = plan_keyed(ctx, sizeof(IdT), ids, vals, m);
+        launch_keyed_scalar(ctx, ko, ids, vals, p.head, s);
+        if (p.route == KeyedPlan::SMALL) {
+            // per device, not per context: a value of this context's H could be overwritten by another context's
+            // between here and the launch
+            LH_CUDA(ctx, cudaFuncSetAttribute((const void *)k_ingest_keyed_small<IdT, ValT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
+            for (uint32_t lo = 0; lo < ctx->H; lo += p.per) {
+                const uint32_t cnt = std::min(p.per, ctx->H - lo);
+                k_ingest_keyed_small<IdT, ValT><<<p.grid, KS_THREADS, p.smem, s>>>(ids + p.head, vals + p.head, p.n4, lo, cnt, ko, ctx->pc);
                 ctx->stats.kernel_launches++;
-                hot_used = n4 * 4;
-                ctx->keyed_kernel = "k_ingest_keyed_vec";
             }
-        } else {
-            ctx->keyed_kernel = "k_ingest_keyed";   // no vector body (short or misaligned batch): the scalar kernel only
+        } else if (p.route == KeyedPlan::WC) {
+            lh_status st = launch_keyed_wc<IdT, ValT>(ctx, b, p, ids + p.head, vals + p.head, s);
+            if (st != LH_OK) return st;
+        } else if (p.route == KeyedPlan::VEC) {
+            k_ingest_keyed_vec<IdT, ValT, T><<<grid_1d(ctx, p.n4, T, 1, ctx->keyed_blocks_per_sm), T, 0, s>>>(ids + p.head, vals + p.head, p.n4, ctx->hot_replicas, ko, ctx->pc);
+            ctx->stats.kernel_launches++;
         }
+        ctx->keyed_kernel = p.name;
+        const size_t tail_off = p.head + p.taken;   // after whole tiles of the write-combining kernel: a ragged remainder
         launch_keyed_scalar(ctx, ko, ids + tail_off, vals + tail_off, m - tail_off, s);
         LH_CUDA(ctx, cudaGetLastError());
-        ctx->buf[b].hot_pending += hot_used;     // only k_ingest_keyed_small / _vec count into the uint32 hot window
+        // only k_ingest_keyed_small / _vec count into the uint32 hot window
+        if (p.route == KeyedPlan::SMALL || p.route == KeyedPlan::VEC) ctx->buf[b].hot_pending += p.taken;
         done += m;
     }
     ctx->stats.samples += n;
@@ -650,33 +655,25 @@ lh_status launch_keyed(lh_ctx *ctx, int b, const IdT *d_ids, const ValT *d_vals,
 
 // Histogram samples (float64) and Timer samples (int64 ns, metrics.go:242-246) of one batch in ONE launch of the
 // write-combining kernel: its fixed costs (zeroing and flushing the owners' windows, the last partly filled chunk) are
-// paid once.  Needs both arrays vector-aligned and the write-combining kernel eligible; otherwise launch_keyed for
-// each array in turn.  Either way one body, so one sequence number.
+// paid once.  Unless plan_keyed fuses them, launch_keyed for each array in turn; either way one body, one sequence number.
 template <typename IdT>
 lh_status launch_keyed_pair(lh_ctx *ctx, int b, const IdT *ids_f, const double *vals_f, size_t n_f, const IdT *ids_ns,
                             const long long *vals_ns, size_t n_ns, cudaStream_t s) {
-    auto aligned = [](const void *v, const void *i) { return (((uintptr_t)v & 31u) == 0) && (((uintptr_t)i & (4 * sizeof(IdT) - 1)) == 0); };
-    // few histograms: the shared-memory privatised kernel of launch_keyed() is the better one, per array
-    const bool fuse = n_f && n_ns && ctx->keyed_mode != 1 && !small_route(ctx) && aligned(vals_f, ids_f) && aligned(vals_ns, ids_ns);
-    if (fuse) {
-        bool used = false;
-        size_t took_f = 0, took_ns = 0;
-        lh_status st = launch_keyed_wc<IdT, double>(ctx, b, ids_f, vals_f, n_f, s, &used, &took_f, ids_ns, vals_ns, n_ns, &took_ns);
+    const KeyedPlan p = plan_keyed(ctx, sizeof(IdT), ids_f, vals_f, n_f, true, ids_ns, vals_ns, n_ns);
+    if (p.route == KeyedPlan::APART) {
+        lh_status st = launch_keyed<IdT, double>(ctx, b, ids_f, vals_f, n_f, s);
         if (st != LH_OK) return st;
-        if (used) {
-            const KeyedOut ko = keyed_out(ctx, b);
-            ctx->keyed_kernel = "k_ingest_keyed_wc";
-            launch_keyed_scalar(ctx, ko, ids_f + took_f, vals_f + took_f, n_f - took_f, s);   // the ragged ends
-            launch_keyed_scalar(ctx, ko, ids_ns + took_ns, vals_ns + took_ns, n_ns - took_ns, s);
-            LH_CUDA(ctx, cudaGetLastError());
-            ctx->stats.samples += n_f + n_ns;
-            return LH_OK;
-        }
-        // declined (too many histograms for the owners' windows, too few SMs, a small batch): one array at a time
+        return launch_keyed<IdT, long long>(ctx, b, ids_ns, vals_ns, n_ns, s);
     }
-    lh_status st = launch_keyed<IdT, double>(ctx, b, ids_f, vals_f, n_f, s);
+    lh_status st = launch_keyed_wc<IdT, double>(ctx, b, p, ids_f, vals_f, s, ids_ns, vals_ns);
     if (st != LH_OK) return st;
-    return launch_keyed<IdT, long long>(ctx, b, ids_ns, vals_ns, n_ns, s);
+    ctx->keyed_kernel = p.name;
+    const KeyedOut ko = keyed_out(ctx, b);
+    launch_keyed_scalar(ctx, ko, ids_f + p.taken, vals_f + p.taken, n_f - p.taken, s);   // the ragged ends
+    launch_keyed_scalar(ctx, ko, ids_ns + p.taken2, vals_ns + p.taken2, n_ns - p.taken2, s);
+    LH_CUDA(ctx, cudaGetLastError());
+    ctx->stats.samples += n_f + n_ns;
+    return LH_OK;
 }
 
 template <typename IdT>
