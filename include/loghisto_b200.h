@@ -233,7 +233,8 @@ LH_API lh_status lh_record_end(lh_ctx *ctx, const lh_recorder *rec);
  * lands in the interval of the first collection whose drain finds it, so a caller that wants a replay in a given
  * interval synchronises the replay's stream before collecting.
  *
- *   lh_graph_recorder_create   allocates and zeroes k rows of uint64[65536] (512 KiB each), k flags and kc counters,
+ *   lh_graph_recorder_create   allocates and zeroes k rows of uint64[65536] (512 KiB each), k flags and kc counters
+ *                              (and k timer start marks, set to never started, in the same allocation),
  *                              k <= max_histograms, kc <= max_counters, k + kc >= 1, and binds them: hist_ids[i] /
  *                              counter_ids[i] (NULL = all unbound) is the context id local row i drains into.  The
  *                              recorder has max_histograms = k and max_counters = kc (a local id >= k is dropped and
@@ -248,6 +249,31 @@ LH_API lh_status lh_record_end(lh_ctx *ctx, const lh_recorder *rec);
  *                              sequence number, lh_stats.samples or allocation -- it only enqueues kernels, so it may be
  *                              captured into a CUDA graph (or called on an ordinary stream).  On error nothing is
  *                              enqueued.
+ *   lh_graph_recorder_ingest_keyed_u16 / _u32
+ *                              n (local id, value) pairs into the recorder's rows: values of `kind` LH_VALUES_F64 or
+ *                              LH_VALUES_I64NS as in lh_ingest_batch, ids local (an id >= k is dropped and counted in
+ *                              lh_stats.dropped, also when k = 0).  Validation as lh_ingest_keyed_*: NULL inputs with
+ *                              n > 0, values not 8-byte aligned, ids not naturally aligned or any other kind give
+ *                              LH_ERR_INVALID.  One sm_90a kernel (k_ingest_keyed_graph) per up to 2^31 samples per CTA.
+ *   lh_graph_recorder_counter_add_u16 / _u32
+ *                              n (local id, amount) pairs: wrapping uint64 adds into the recorder's kc counters; an op
+ *                              with id >= kc counts 1 in lh_stats.dropped.  NULL inputs with n > 0, or amounts / ids not
+ *                              naturally aligned, give LH_ERR_INVALID.
+ *   lh_graph_recorder_timer_start / _stop
+ *                              a GPU-timed span of local histogram `histogram` (LH_ERR_RANGE when >= k): the start
+ *                              writes the device clock into the histogram's start mark, the stop records
+ *                              float64(now - mark) into its row and, when d_duration_ns is not NULL (8-byte aligned
+ *                              device memory, else LH_ERR_INVALID), writes the int64 duration there.  A stop whose mark
+ *                              was never started records nothing, writes nothing and counts 1 in lh_stats.dropped.  The
+ *                              mark stays after a stop, so a span may be stopped again.  The caller orders a start
+ *                              before its stop: the same stream, or its own fork / join inside the capture.  A histogram
+ *                              has one mark per recorder, so one open span at a time; sequential spans (one per layer)
+ *                              are fine, concurrent spans of one histogram on parallel branches need two recorders or
+ *                              lh::start_timer in a kernel.
+ *                              These six calls, like lh_graph_recorder_ingest, only enqueue kernels on `stream` (NULL =
+ *                              the ingest stream): no event, host wait, allocation, write bracket, sequence number or
+ *                              lh_stats.samples / counter_ops, so they may be captured in any capture mode or called on
+ *                              an ordinary stream.  Every check runs first; on error, and for n = 0, nothing is enqueued.
  *   lh_graph_recorder_destroy  enqueues a final drain on `stream` (NULL = the ingest stream) into the active interval
  *                              as one write bracket, as an ingest call, and frees the rows, stream-ordered, after it and
  *                              after every collection drain already issued.  The caller guarantees that no replay that
@@ -269,6 +295,17 @@ LH_API lh_status lh_graph_recorder_bind(lh_ctx *ctx, const lh_graph_recorder *g,
                                         const uint32_t *counter_ids);
 LH_API lh_status lh_graph_recorder_ingest(lh_ctx *ctx, const lh_graph_recorder *g, const lh_batch_item *h_items,
                                           uint32_t n_items, void *stream);
+LH_API lh_status lh_graph_recorder_ingest_keyed_u16(lh_ctx *ctx, const lh_graph_recorder *g, const uint16_t *d_ids,
+                                                    const void *d_values, uint32_t kind, size_t n, void *stream);
+LH_API lh_status lh_graph_recorder_ingest_keyed_u32(lh_ctx *ctx, const lh_graph_recorder *g, const uint32_t *d_ids,
+                                                    const void *d_values, uint32_t kind, size_t n, void *stream);
+LH_API lh_status lh_graph_recorder_counter_add_u16(lh_ctx *ctx, const lh_graph_recorder *g, const uint16_t *d_ids,
+                                                   const uint64_t *d_amounts, size_t n, void *stream);
+LH_API lh_status lh_graph_recorder_counter_add_u32(lh_ctx *ctx, const lh_graph_recorder *g, const uint32_t *d_ids,
+                                                   const uint64_t *d_amounts, size_t n, void *stream);
+LH_API lh_status lh_graph_recorder_timer_start(lh_ctx *ctx, const lh_graph_recorder *g, uint32_t histogram, void *stream);
+LH_API lh_status lh_graph_recorder_timer_stop(lh_ctx *ctx, const lh_graph_recorder *g, uint32_t histogram, void *stream,
+                                              int64_t *d_duration_ns);
 LH_API lh_status lh_graph_recorder_destroy(lh_ctx *ctx, const lh_graph_recorder *g, void *stream);
 
 /* ---- device subscriptions: each collection's processed metrics in device memory --------------------------------

@@ -171,6 +171,12 @@ SIGNATURES = {
     "lh_graph_recorder_create": (_i32, [_vp, _u32, _u32, _vp, _vp, C.POINTER(lh_graph_recorder)]),
     "lh_graph_recorder_bind": (_i32, [_vp, C.POINTER(lh_graph_recorder), _vp, _vp]),
     "lh_graph_recorder_ingest": (_i32, [_vp, C.POINTER(lh_graph_recorder), C.POINTER(lh_batch_item), _u32, _vp]),
+    "lh_graph_recorder_ingest_keyed_u16": (_i32, [_vp, C.POINTER(lh_graph_recorder), _vp, _vp, _u32, _sz, _vp]),
+    "lh_graph_recorder_ingest_keyed_u32": (_i32, [_vp, C.POINTER(lh_graph_recorder), _vp, _vp, _u32, _sz, _vp]),
+    "lh_graph_recorder_counter_add_u16": (_i32, [_vp, C.POINTER(lh_graph_recorder), _vp, _vp, _sz, _vp]),
+    "lh_graph_recorder_counter_add_u32": (_i32, [_vp, C.POINTER(lh_graph_recorder), _vp, _vp, _sz, _vp]),
+    "lh_graph_recorder_timer_start": (_i32, [_vp, C.POINTER(lh_graph_recorder), _u32, _vp]),
+    "lh_graph_recorder_timer_stop": (_i32, [_vp, C.POINTER(lh_graph_recorder), _u32, _vp, _vp]),
     "lh_graph_recorder_destroy": (_i32, [_vp, C.POINTER(lh_graph_recorder), _vp]),
     "lh_board_create": (_i32, [_vp, _u32, _u32, C.POINTER(lh_board)]),
     "lh_snapshot_publish": (_i32, [_vp, C.POINTER(lh_board), _vp, _vp, _vp]),

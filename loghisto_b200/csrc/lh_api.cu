@@ -43,6 +43,7 @@ struct TimerSlot {
 struct GraphRec {
     uint64_t handle;
     lh_recorder rec;                 // what the caller was given (rows, flags, counters in one allocation)
+    unsigned long long *d_marks;     // [k] start marks of lh_graph_recorder_timer_* (kTimerNeverStarted until a start)
     std::vector<uint32_t> hid, cid;  // target id of each local row / counter (LH_GRAPH_UNBOUND = drop and count)
 };
 
@@ -676,12 +677,14 @@ lh_status launch_keyed_pair(lh_ctx *ctx, int b, const IdT *ids_f, const double *
     return LH_OK;
 }
 
+// (id, amount) pairs into `counters` (C of them, ids >= C dropped and counted); the caller counts the ops in stats
 template <typename IdT>
-lh_status launch_counter(lh_ctx *ctx, int b, const IdT *d_ids, const uint64_t *d_amounts, size_t n, cudaStream_t s) {
+lh_status launch_counter(lh_ctx *ctx, unsigned long long *counters, uint32_t C, const IdT *d_ids, const uint64_t *d_amounts,
+                         size_t n, cudaStream_t s) {
     if (n) {
         constexpr int T = 512;
         const unsigned long long *amts = reinterpret_cast<const unsigned long long *>(d_amounts);
-        if (ctx->C <= (uint32_t)K2_SMEM_COUNTERS) {
+        if (C <= (uint32_t)K2_SMEM_COUNTERS) {
             // privatised per CTA (lo/hi halves in shared memory).  Vector body where the alignment allows: 4 ops per
             // thread and iteration; ragged head / tail through the scalar form of the same kernel.
             size_t head = std::min<size_t>(n, ((32u - ((uintptr_t)amts & 31u)) & 31u) / 8u);
@@ -690,29 +693,35 @@ lh_status launch_counter(lh_ctx *ctx, int b, const IdT *d_ids, const uint64_t *d
             if (n4 < 4096) { head = 0; n4 = 0; }
             const size_t tail_off = head + n4 * 4;
             if (head) {
-                k_counter_add_smem<IdT, T><<<1, T, (size_t)ctx->C * 8, s>>>(d_ids, amts, head, ctx->buf[b].d_counters, ctx->C, ctx->d_dropped);
+                k_counter_add_smem<IdT, T><<<1, T, (size_t)C * 8, s>>>(d_ids, amts, head, counters, C, ctx->d_dropped);
                 ctx->stats.kernel_launches++;
             }
             if (n4) {
                 // one CTA per SM (the per-CTA flush is C global atomics), fewer for small batches
                 const int grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)std::max(1, ctx->sm_count - ctx->k1_reserve_sms) * 2, n4 / (T * 4)));
-                k_counter_add_smem_vec<IdT, T><<<grid, T, (size_t)ctx->C * 8, s>>>(d_ids + head, amts + head, n4, ctx->buf[b].d_counters, ctx->C, ctx->d_dropped);
+                k_counter_add_smem_vec<IdT, T><<<grid, T, (size_t)C * 8, s>>>(d_ids + head, amts + head, n4, counters, C, ctx->d_dropped);
                 ctx->stats.kernel_launches++;
             }
             if (tail_off < n) {
                 int grid = grid_1d(ctx, n - tail_off, T, 8, 2);
-                k_counter_add_smem<IdT, T><<<grid, T, (size_t)ctx->C * 8, s>>>(d_ids + tail_off, amts + tail_off, n - tail_off, ctx->buf[b].d_counters, ctx->C, ctx->d_dropped);
+                k_counter_add_smem<IdT, T><<<grid, T, (size_t)C * 8, s>>>(d_ids + tail_off, amts + tail_off, n - tail_off, counters, C, ctx->d_dropped);
                 ctx->stats.kernel_launches++;
             }
         } else {
             int grid = grid_1d(ctx, n, T, 4, 4);
-            k_counter_add<IdT, T><<<grid, T, 0, s>>>(d_ids, amts, n, ctx->buf[b].d_counters, ctx->C, ctx->d_dropped);
+            k_counter_add<IdT, T><<<grid, T, 0, s>>>(d_ids, amts, n, counters, C, ctx->d_dropped);
             ctx->stats.kernel_launches++;
         }
         LH_CUDA(ctx, cudaGetLastError());
     }
-    ctx->stats.counter_ops += n;
     return LH_OK;
+}
+// n counter ops into buffer b, counted in stats
+template <typename IdT>
+lh_status add_counters(lh_ctx *ctx, int b, const IdT *d_ids, const uint64_t *d_amounts, size_t n, cudaStream_t s) {
+    lh_status st = launch_counter<IdT>(ctx, ctx->buf[b].d_counters, ctx->C, d_ids, d_amounts, n, s);
+    if (st == LH_OK) ctx->stats.counter_ops += n;
+    return st;
 }
 
 // lh_ingest_batch routing.  An F64 item this long pays back K1's full-grid launch (launch_single); shorter ones and every
@@ -723,12 +732,17 @@ constexpr size_t kBatchK1Min = 1024 * 1024;
 // ones through launch_single, the rest through as few launches of k_ingest_batch as the parameter block and the uint32
 // table counts allow.  An item that does not fit the launch being filled is split across launches.  Kernels only (the
 // graph recorder's form is captured); the caller counts the samples in stats.
+// The grid of k_ingest_batch (and of k_ingest_keyed_graph, which has its launch bounds and table), and the samples one
+// launch of it may take: pieces are dealt round-robin, so at most 2^31 samples per CTA of the full grid keeps every
+// table count below 2^32.
+int batch_grid_max(const lh_ctx *ctx) { return std::max(1, ctx->sm_count - ctx->k1_reserve_sms) * ctx->batch_blocks_per_sm; }
+unsigned long long batch_cap(int grid_max) { return std::min<unsigned long long>(1ull << 36, (unsigned long long)grid_max << 31); }
+
 lh_status launch_batch(lh_ctx *ctx, const lh_recorder &target, const lh_batch_item *items, uint32_t n_items, cudaStream_t s) {
     BatchParams &prm = ctx->batch_prm;
     prm.rec = target;
-    // pieces are dealt round-robin, so at most 2^31 samples per CTA of the full grid keeps every table count below 2^32
-    const int grid_max = std::max(1, ctx->sm_count - ctx->k1_reserve_sms) * ctx->batch_blocks_per_sm;
-    const unsigned long long cap = std::min<unsigned long long>(1ull << 36, (unsigned long long)grid_max << 31);
+    const int grid_max = batch_grid_max(ctx);
+    const unsigned long long cap = batch_cap(grid_max);
     uint32_t k = 0;
     unsigned long long total = 0;
     auto launch = [&]() -> lh_status {
@@ -770,6 +784,32 @@ lh_status launch_batch(lh_ctx *ctx, const lh_recorder &target, const lh_batch_it
         }
     }
     return launch();
+}
+
+// Validated (id, value) pairs into the rows of `target` (lh_graph_recorder_ingest_keyed_*): k_ingest_keyed_graph, over
+// as many launches as launch_batch's bound on the samples of one launch requires, with launch_batch's grid.  The
+// vector body starts at the first 32-byte aligned value; when the ids are not 4*sizeof(IdT)-aligned there, every sample
+// goes one per thread.  Kernels only, so it may be captured; the caller counts nothing in stats but the launches.
+template <typename IdT>
+lh_status launch_keyed_graph(lh_ctx *ctx, const lh_recorder &target, const IdT *ids, const unsigned long long *vals, size_t n,
+                             bool ns, cudaStream_t s) {
+    const int grid_max = batch_grid_max(ctx);
+    const size_t cap = (size_t)batch_cap(grid_max);
+    for (size_t done = 0; done < n;) {
+        const size_t m = std::min(n - done, cap);
+        const IdT *ip = ids + done;
+        const unsigned long long *vp = vals + done;
+        size_t head = std::min<size_t>(m, ((32u - ((uintptr_t)vp & 31u)) & 31u) / 8u);
+        const bool vec_ok = ((uintptr_t)(ip + head) & (4 * sizeof(IdT) - 1)) == 0;
+        const size_t n4 = vec_ok ? (m - head) / 4 : 0;
+        if (!vec_ok) head = m;
+        const int grid = (int)std::min<size_t>((size_t)grid_max, (m + BI_PIECE - 1) / BI_PIECE);
+        k_ingest_keyed_graph<IdT><<<grid, BI_THREADS, BlockRecorder::smem_bytes(BI_TABLE_ENTRIES), s>>>(target, ip, vp, head, n4, m, ns);
+        LH_CUDA(ctx, cudaGetLastError());
+        ctx->stats.kernel_launches++;
+        done += m;
+    }
+    return LH_OK;
 }
 
 // Validation of lh_ingest_batch / lh_graph_recorder_ingest against `limit` histogram ids; the samples of the batch
@@ -1086,6 +1126,9 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
         int nb = 0;
         LH_CREATE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, fn, BI_THREADS, BlockRecorder::smem_bytes(BI_TABLE_ENTRIES)));
         ctx->batch_blocks_per_sm = std::max(nb, 1);
+        // k_ingest_keyed_graph: the same launch bounds and table, so the same occupancy and grid (batch_grid_max)
+        LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_ingest_keyed_graph<unsigned short>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
+        LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_ingest_keyed_graph<unsigned int>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
     }
     LH_CREATE_CUDA(cudaStreamSynchronize(ctx->snap_stream));
 #undef LH_CREATE_CUDA
@@ -1214,13 +1257,13 @@ extern "C" lh_status lh_counter_add_u16(lh_ctx *ctx, const uint16_t *d_ids, cons
     LH_ENTER(ctx);
     if (n && (!d_ids || !d_amounts)) return fail(ctx, LH_ERR_INVALID, "NULL input");
     cudaStream_t s = pick_stream(ctx, stream);
-    return write_bracket(ctx, s, [&](int b) { return launch_counter<unsigned short>(ctx, b, d_ids, d_amounts, n, s); });
+    return write_bracket(ctx, s, [&](int b) { return add_counters<unsigned short>(ctx, b, d_ids, d_amounts, n, s); });
 }
 extern "C" lh_status lh_counter_add_u32(lh_ctx *ctx, const uint32_t *d_ids, const uint64_t *d_amounts, size_t n, void *stream) {
     LH_ENTER(ctx);
     if (n && (!d_ids || !d_amounts)) return fail(ctx, LH_ERR_INVALID, "NULL input");
     cudaStream_t s = pick_stream(ctx, stream);
-    return write_bracket(ctx, s, [&](int b) { return launch_counter<unsigned int>(ctx, b, d_ids, d_amounts, n, s); });
+    return write_bracket(ctx, s, [&](int b) { return add_counters<unsigned int>(ctx, b, d_ids, d_amounts, n, s); });
 }
 extern "C" lh_status lh_ingest_batch(lh_ctx *ctx, const lh_batch_item *h_items, uint32_t n_items, void *stream) {
     LH_ENTER(ctx);
@@ -1265,7 +1308,7 @@ lh_status staging_step(lh_ctx *ctx, Slot &sl, HostKind kind, uint32_t hid, const
             case HK_SINGLE: return ingest_single(ctx, b, hid, (const double *)d_a, n, s);
             case HK_KEYED_U16: return launch_keyed<unsigned short, double>(ctx, b, d_i, (const double *)d_a, n, s);
             case HK_KEYED_I64_U16: return launch_keyed<unsigned short, long long>(ctx, b, d_i, (const long long *)d_a, n, s);
-            default: return launch_counter<unsigned short>(ctx, b, d_i, (const uint64_t *)d_a, n, s);   // HK_COUNTER_U16
+            default: return add_counters<unsigned short>(ctx, b, d_i, (const uint64_t *)d_a, n, s);   // HK_COUNTER_U16
             }
         });
     }
@@ -1492,12 +1535,15 @@ extern "C" lh_status lh_graph_recorder_create(lh_ctx *ctx, uint32_t k, uint32_t 
     if (!ids_ok(hist_ids, k, ctx->H) || !ids_ok(counter_ids, kc, ctx->C))
         return fail(ctx, LH_ERR_RANGE, "target id >= max_histograms / max_counters");
     if (!ctx->graph_drained) LH_CUDA(ctx, cudaEventCreateWithFlags(&ctx->graph_drained, cudaEventDisableTiming));
-    // one allocation: rows [k][65536], counters [kc], flags [k]
-    const size_t row_bytes = (size_t)k * 65536u * 8u, bytes = row_bytes + (size_t)kc * 8u + (size_t)k * 4u;
+    // one allocation: rows [k][65536], counters [kc], timer marks [k], flags [k]
+    const size_t row_bytes = (size_t)k * 65536u * 8u, mark_off = row_bytes + (size_t)kc * 8u, flag_off = mark_off + (size_t)k * 8u;
+    const size_t bytes = flag_off + (size_t)k * 4u;
     cudaStream_t s = ctx->snap_stream;
     char *base = nullptr;
     LH_CUDA(ctx, cudaMallocAsync((void **)&base, bytes, s));
     cudaError_t e = cudaMemsetAsync(base, 0, bytes, s);
+    static_assert(kTimerNeverStarted == ~0ull, "marks are set bytewise");
+    if (e == cudaSuccess) e = cudaMemsetAsync(base + mark_off, 0xFF, (size_t)k * 8u, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     if (e != cudaSuccess) {
         cudaFreeAsync(base, s);
@@ -1508,7 +1554,8 @@ extern "C" lh_status lh_graph_recorder_create(lh_ctx *ctx, uint32_t k, uint32_t 
     memset(&gr.rec, 0, sizeof gr.rec);
     gr.rec.d_buckets = reinterpret_cast<uint64_t *>(base);
     gr.rec.d_counters = reinterpret_cast<uint64_t *>(base + row_bytes);
-    gr.rec.d_flags = reinterpret_cast<uint32_t *>(base + row_bytes + (size_t)kc * 8u);
+    gr.rec.d_flags = reinterpret_cast<uint32_t *>(base + flag_off);
+    gr.d_marks = reinterpret_cast<unsigned long long *>(base + mark_off);
     gr.rec.d_dropped = reinterpret_cast<uint64_t *>(ctx->d_dropped);
     gr.rec.max_histograms = k;
     gr.rec.max_counters = kc;
@@ -1546,6 +1593,84 @@ extern "C" lh_status lh_graph_recorder_ingest(lh_ctx *ctx, const lh_graph_record
     lh_status st = check_batch(ctx, h_items, n_items, gr->rec.max_histograms, &n);
     if (st != LH_OK || n == 0) return st;
     return launch_batch(ctx, gr->rec, h_items, n_items, pick_stream(ctx, stream));
+}
+
+namespace {
+template <typename IdT>
+lh_status graph_keyed(lh_ctx *ctx, const lh_graph_recorder *g, const IdT *d_ids, const void *d_values, uint32_t kind, size_t n,
+                      void *stream) {
+    GraphRec *gr = graph_of(ctx, g);
+    if (!gr) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign graph recorder");
+    if (kind != LH_VALUES_F64 && kind != LH_VALUES_I64NS) return fail(ctx, LH_ERR_INVALID, "unknown values kind");
+    if (n && (!d_ids || !d_values)) return fail(ctx, LH_ERR_INVALID, "NULL input");
+    if (((uintptr_t)d_values & 7u) || ((uintptr_t)d_ids & (sizeof(IdT) - 1)))
+        return fail(ctx, LH_ERR_INVALID, "ids / values are not naturally aligned");
+    if (n == 0) return LH_OK;
+    return launch_keyed_graph<IdT>(ctx, gr->rec, d_ids, static_cast<const unsigned long long *>(d_values), n,
+                                   kind == LH_VALUES_I64NS, pick_stream(ctx, stream));
+}
+
+template <typename IdT>
+lh_status graph_counters(lh_ctx *ctx, const lh_graph_recorder *g, const IdT *d_ids, const uint64_t *d_amounts, size_t n,
+                         void *stream) {
+    GraphRec *gr = graph_of(ctx, g);
+    if (!gr) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign graph recorder");
+    if (n && (!d_ids || !d_amounts)) return fail(ctx, LH_ERR_INVALID, "NULL input");
+    if (((uintptr_t)d_amounts & 7u) || ((uintptr_t)d_ids & (sizeof(IdT) - 1)))
+        return fail(ctx, LH_ERR_INVALID, "ids / amounts are not naturally aligned");
+    if (n == 0) return LH_OK;
+    return launch_counter<IdT>(ctx, reinterpret_cast<unsigned long long *>(gr->rec.d_counters), gr->rec.max_counters, d_ids,
+                               d_amounts, n, pick_stream(ctx, stream));
+}
+}  // namespace
+
+extern "C" lh_status lh_graph_recorder_ingest_keyed_u16(lh_ctx *ctx, const lh_graph_recorder *g, const uint16_t *d_ids,
+                                                        const void *d_values, uint32_t kind, size_t n, void *stream) {
+    LH_ENTER(ctx);
+    return graph_keyed<unsigned short>(ctx, g, d_ids, d_values, kind, n, stream);
+}
+extern "C" lh_status lh_graph_recorder_ingest_keyed_u32(lh_ctx *ctx, const lh_graph_recorder *g, const uint32_t *d_ids,
+                                                        const void *d_values, uint32_t kind, size_t n, void *stream) {
+    LH_ENTER(ctx);
+    return graph_keyed<unsigned int>(ctx, g, d_ids, d_values, kind, n, stream);
+}
+extern "C" lh_status lh_graph_recorder_counter_add_u16(lh_ctx *ctx, const lh_graph_recorder *g, const uint16_t *d_ids,
+                                                       const uint64_t *d_amounts, size_t n, void *stream) {
+    LH_ENTER(ctx);
+    return graph_counters<unsigned short>(ctx, g, d_ids, d_amounts, n, stream);
+}
+extern "C" lh_status lh_graph_recorder_counter_add_u32(lh_ctx *ctx, const lh_graph_recorder *g, const uint32_t *d_ids,
+                                                       const uint64_t *d_amounts, size_t n, void *stream) {
+    LH_ENTER(ctx);
+    return graph_counters<unsigned int>(ctx, g, d_ids, d_amounts, n, stream);
+}
+
+// A span of the recorder's local histogram: the start writes the row's mark, the stop records now - mark into the row.
+// No event or host state, so both may be captured; the caller orders them (see the header).
+extern "C" lh_status lh_graph_recorder_timer_start(lh_ctx *ctx, const lh_graph_recorder *g, uint32_t histogram, void *stream) {
+    LH_ENTER(ctx);
+    GraphRec *gr = graph_of(ctx, g);
+    if (!gr) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign graph recorder");
+    if (histogram >= gr->rec.max_histograms) return fail(ctx, LH_ERR_RANGE, "histogram >= the recorder's histograms");
+    k_gpu_timer_mark<<<1, 1, 0, pick_stream(ctx, stream)>>>(gr->d_marks + histogram);
+    LH_CUDA(ctx, cudaGetLastError());
+    ctx->stats.kernel_launches++;
+    return LH_OK;
+}
+
+extern "C" lh_status lh_graph_recorder_timer_stop(lh_ctx *ctx, const lh_graph_recorder *g, uint32_t histogram, void *stream,
+                                                  int64_t *d_duration_ns) {
+    LH_ENTER(ctx);
+    GraphRec *gr = graph_of(ctx, g);
+    if (!gr) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign graph recorder");
+    if (histogram >= gr->rec.max_histograms) return fail(ctx, LH_ERR_RANGE, "histogram >= the recorder's histograms");
+    if (((uintptr_t)d_duration_ns & 7u) != 0) return fail(ctx, LH_ERR_INVALID, "d_duration_ns must be 8-byte aligned");
+    k_gpu_timer_stop<<<1, 1, 0, pick_stream(ctx, stream)>>>(
+        gr->d_marks + histogram, reinterpret_cast<unsigned long long *>(gr->rec.d_buckets) + (size_t)histogram * 65536u,
+        gr->rec.d_flags + histogram, reinterpret_cast<long long *>(d_duration_ns), ctx->d_dropped, ctx->pc);
+    LH_CUDA(ctx, cudaGetLastError());
+    ctx->stats.kernel_launches++;
+    return LH_OK;
 }
 
 extern "C" lh_status lh_graph_recorder_destroy(lh_ctx *ctx, const lh_graph_recorder *g, void *stream) {
@@ -1663,7 +1788,7 @@ extern "C" lh_status lh_gpu_timer_stop(lh_ctx *ctx, const lh_gpu_timer *t, uint3
     const unsigned long long *mark = ctx->d_timer_marks + (ts - ctx->timer_slots.data());
     st = write_bracket(ctx, s, [&](int b) -> lh_status {
         k_gpu_timer_stop<<<1, 1, 0, s>>>(mark, ctx->buf[b].d_buckets + (size_t)hid * 65536u, ctx->buf[b].d_flags + hid,
-                                         reinterpret_cast<long long *>(d_out), ctx->pc);
+                                         reinterpret_cast<long long *>(d_out), ctx->d_dropped, ctx->pc);
         LH_CUDA(ctx, cudaGetLastError());
         ctx->stats.kernel_launches++;
         ctx->stats.samples++;

@@ -21,6 +21,7 @@
 //   K6   k_scatter_segments, k_sparse_epilogue   caller-supplied sparse histograms -> scratch rows -> K3
 //                               (lh_reduce_sparse_host)
 //   k_ingest_batch          many device arrays under many ids (lh_ingest_batch, lh_graph_recorder_ingest)
+//   k_ingest_keyed_graph    (id,value) pairs into a graph recorder's rows (lh_graph_recorder_ingest_keyed_*)
 //   k_graph_drain           graph recorders' rows -> the interval being frozen (lh_snapshot_begin)
 //   misc k_clear_touched, k_fill_decompress, k_compress_probe, k_fastpath_margin, k_fastpath_certify, k_stream_probe,
 //        k_gen_stream, k_gen_ids_u16
@@ -1736,6 +1737,45 @@ k_ingest_batch(const __grid_constant__ BatchParams p) {
     br.flush();
 }
 
+// ----------------------------------------------------------- captured keyed ingest (lh_graph_recorder_ingest_keyed_*)
+// (id, value) pairs into a graph recorder's rows, ids local.  The keyed kernels above cannot be captured (the hot window
+// needs a host-tallied fold, the write-combining kernel cross-launch scratch and events), so this one counts like
+// k_ingest_batch instead: every CTA through one lh::BlockRecorder over the recorder, flushed once, with the id taken per
+// sample; an id >= max_histograms is dropped and counted by the recorder.  Samples [0, nhead) and [nhead + 4 n4, n) go
+// one per thread (all of them when the id and value alignments do not line up); the vector body in between takes
+// 4 samples per thread and iteration (two 16-byte value loads, one IdPack id load), the next group loaded while the
+// current one is counted.  vals + nhead is 32-byte aligned and ids + nhead 4*sizeof(IdT)-aligned.  The host bounds a
+// launch as it bounds k_ingest_batch's, so no CTA counts more than 2^31 samples.
+template <typename IdT>
+__global__ void __launch_bounds__(BI_THREADS, 2)
+k_ingest_keyed_graph(const __grid_constant__ lh_recorder rec, const IdT *__restrict__ ids,
+                     const unsigned long long *__restrict__ vals, size_t nhead, size_t n4, size_t n, bool ns) {
+    extern __shared__ __align__(16) unsigned char kg_smem[];
+    BlockRecorder br(rec, kg_smem, BI_TABLE_ENTRIES);
+    br.init();
+    auto value = [ns](unsigned long long raw) { return ns ? __ll2double_rn((long long)raw) : __longlong_as_double((long long)raw); };
+    const size_t stride = (size_t)gridDim.x * BI_THREADS;
+    const size_t t0 = (size_t)blockIdx.x * BI_THREADS + threadIdx.x;
+    for (size_t i = t0; i < nhead; i += stride) br.record((uint32_t)ids[i], value(__ldcs(vals + i)));
+    const IdT *bid = ids + nhead;
+    const unsigned long long *bv = vals + nhead;
+    size_t g = t0;
+    unsigned long long cur[4], nxt[4];
+    IdPack<IdT> cid, nid;
+    if (g < n4) { load_vals4(bv, g, cur); cid.load(bid, g); }
+    for (; g < n4; g += stride) {
+        const size_t gn = g + stride;
+        if (gn < n4) { load_vals4(bv, gn, nxt); nid.load(bid, gn); }
+#pragma unroll
+        for (int j = 0; j < 4; j++) br.record(cid.get(j), value(cur[j]));
+#pragma unroll
+        for (int j = 0; j < 4; j++) cur[j] = nxt[j];
+        cid = nid;
+    }
+    for (size_t i = nhead + 4 * n4 + t0; i < n; i += stride) br.record((uint32_t)ids[i], value(__ldcs(vals + i)));
+    br.flush();
+}
+
 // ----------------------------------------------------------- graph recorder drain (lh_graph_recorder_*)
 // Moves the counts of graph-owned rows into an interval's rows.  One CTA per entry of the table, which travels in the
 // parameter block: a histogram row (src, src_flag, target id) or a counter (src, no flag, target id).  A row whose flag
@@ -2013,12 +2053,16 @@ k_gauge_read(const __grid_constant__ GaugeParams p) {
 // ----------------------------------------------------------- GPU timers (lh_gpu_timer_*)
 // One thread each: their cost is the launch, not the body.  The start writes %globaltimer into the token's slot; the
 // stop records float64(now - start) into one histogram row through the same bucket function and row writer every
-// device caller uses (what lh::record_ns does, without the warp combining a single thread cannot use).
+// device caller uses (what lh::record_ns does, without the warp combining a single thread cannot use).  A slot that
+// holds kTimerNeverStarted (a graph recorder's mark before its first start) records nothing and counts 1 in `dropped`.
+constexpr unsigned long long kTimerNeverStarted = ~0ull;
 __global__ void k_gpu_timer_mark(unsigned long long *__restrict__ slot) { *slot = globaltimer_ns(); }
 
 __global__ void k_gpu_timer_stop(const unsigned long long *__restrict__ slot, unsigned long long *__restrict__ row,
-                                 uint32_t *flag, long long *out, Prec pc) {
-    const long long ns = (long long)(globaltimer_ns() - *slot);
+                                 uint32_t *flag, long long *out, unsigned long long *dropped, Prec pc) {
+    const unsigned long long start = *slot;
+    if (start == kTimerNeverStarted) { atomicAdd(dropped, 1ull); return; }
+    const long long ns = (long long)(globaltimer_ns() - start);
     add_bucket_global(row, flag, key16_of(__ll2double_rn(ns), pc), 1ull, pc.win);
     if (out) *out = ns;
 }

@@ -54,14 +54,14 @@ _BATCH_KINDS = {"float64": L.LH_VALUES_F64, "int64": L.LH_VALUES_I64NS}
 _TYPESTRS = {t: np.dtype(t) for t in ("<f8", "<i8")}
 
 
-def _batch_array(x):
-    """(address, length, LH_VALUES_* kind) of one device array of a batch: a CUDA torch tensor, a DeviceArray or an
-    object with __cuda_array_interface__, contiguous, of dtype float64 or int64.  TypeError otherwise."""
+def _device_array(x, what="batch arrays"):
+    """(address, length, dtype name) of a CUDA torch tensor, a DeviceArray or an object with __cuda_array_interface__,
+    contiguous ("" for a big-endian dtype).  TypeError otherwise; `what` names the array in the message."""
     if hasattr(x, "is_cuda") and hasattr(x, "data_ptr"):        # torch.Tensor
         if not x.is_cuda:
-            raise TypeError("batch arrays must be in device memory, not a CPU tensor")
+            raise TypeError(f"{what} must be in device memory, not a CPU tensor")
         if not x.is_contiguous():
-            raise TypeError("batch arrays must be contiguous")
+            raise TypeError(f"{what} must be contiguous")
         dtype = str(x.dtype).replace("torch.", "")
         ptr, n = int(x.data_ptr()), int(x.numel())
     elif isinstance(x, DeviceArray):
@@ -78,10 +78,17 @@ def _batch_array(x):
                 want.append(step)
                 step *= d
             if tuple(strides) != tuple(reversed(want)):
-                raise TypeError("batch arrays must be contiguous")
+                raise TypeError(f"{what} must be contiguous")
         dtype, ptr = dt.name if dt.byteorder in "=<|" else "", int(cai["data"][0])
     else:
         raise TypeError(f"not a device array: {type(x)!r}")
+    return ptr, n, dtype
+
+
+def _batch_array(x):
+    """(address, length, LH_VALUES_* kind) of one device array of a batch: a CUDA torch tensor, a DeviceArray or an
+    object with __cuda_array_interface__, contiguous, of dtype float64 or int64.  TypeError otherwise."""
+    ptr, n, dtype = _device_array(x)
     if dtype not in _BATCH_KINDS:
         raise TypeError(f"batch arrays must be float64 (Histogram) or int64 (Timer nanoseconds), not {dtype or 'big-endian'}")
     return ptr, n, _BATCH_KINDS[dtype]
@@ -211,6 +218,45 @@ def _batch_items(items, limit_name: str):
     return arr, len(items)
 
 
+_ID_BYTES = {"uint16": 2, "int32": 4, "uint32": 4}   # a negative int32 id reads as a large uint32: dropped and counted
+
+
+def graph_keyed_args(ids, values):
+    """(id bytes, ids address, values address, LH_VALUES_* kind, n) of keyed samples for a graph recorder: ids uint16,
+    int32 or uint32, values float64 or int64 (as batch arrays), of one length.  TypeError / ValueError otherwise."""
+    ip, n, idt = _device_array(ids, "ids")
+    if idt not in _ID_BYTES:
+        raise TypeError(f"ids must be uint16, int32 or uint32, not {idt or 'big-endian'}")
+    vp, nv, kind = _batch_array(values)
+    if nv != n:
+        raise ValueError(f"{n} ids but {nv} values")
+    return _ID_BYTES[idt], ip, vp, kind, n
+
+
+def graph_counter_args(ids, amounts):
+    """(id bytes, ids address, amounts address, n) of counter adds for a graph recorder: ids as graph_keyed_args takes
+    them, amounts int64 or uint64 (added as uint64 bits), of one length.  TypeError / ValueError otherwise."""
+    ip, n, idt = _device_array(ids, "ids")
+    if idt not in _ID_BYTES:
+        raise TypeError(f"ids must be uint16, int32 or uint32, not {idt or 'big-endian'}")
+    ap, na, adt = _device_array(amounts, "amounts")
+    if adt not in ("int64", "uint64"):
+        raise TypeError(f"amounts must be int64 or uint64, not {adt or 'big-endian'}")
+    if na != n:
+        raise ValueError(f"{n} ids but {na} amounts")
+    return _ID_BYTES[idt], ip, ap, n
+
+
+def graph_duration_out(out) -> int:
+    """Address of the int64 a graph recorder's timer stop writes its duration to (None = 0: not written)."""
+    if out is None:
+        return 0
+    ptr, n, dtype = _device_array(out, "out")
+    if dtype != "int64" or n < 1:
+        raise TypeError("out must be a device array of at least one int64")
+    return ptr
+
+
 def _ids(ids):
     ids = [int(x) for x in ids]
     return (C.c_uint32 * max(len(ids), 1))(*ids), len(ids)
@@ -240,6 +286,38 @@ class GraphRecorder:
         (None = torch's current stream, so that it is captured inside torch.cuda.graph)."""
         arr, n = _batch_items(items, "local histogram id")
         self._eng._check(self._eng.lib.lh_graph_recorder_ingest(self._eng.h, C.byref(self.g), arr, n, _capture_stream(stream)))
+
+    def keyed(self, ids, values, stream=None):
+        """lh_graph_recorder_ingest_keyed_u16 / _u32: values[i] into local histogram ids[i], on `stream` (None =
+        torch's current stream).  ids uint16 (_u16), int32 or uint32 (_u32); values float64 or int64 nanoseconds."""
+        id_bytes, ip, vp, kind, n = graph_keyed_args(ids, values)
+        fn = self._eng.lib.lh_graph_recorder_ingest_keyed_u16 if id_bytes == 2 else self._eng.lib.lh_graph_recorder_ingest_keyed_u32
+        self._eng._check(fn(self._eng.h, C.byref(self.g), ip, vp, kind, n, _capture_stream(stream)))
+
+    def counters(self, ids, amounts, stream=None):
+        """lh_graph_recorder_counter_add_u16 / _u32: amounts[i] into local counter ids[i] (wrapping uint64)."""
+        id_bytes, ip, ap, n = graph_counter_args(ids, amounts)
+        fn = self._eng.lib.lh_graph_recorder_counter_add_u16 if id_bytes == 2 else self._eng.lib.lh_graph_recorder_counter_add_u32
+        self._eng._check(fn(self._eng.h, C.byref(self.g), ip, ap, n, _capture_stream(stream)))
+
+    def start_timer(self, histogram: int, stream=None):
+        """lh_graph_recorder_timer_start: mark the start of a span of local histogram `histogram` on `stream`."""
+        self._eng._check(self._eng.lib.lh_graph_recorder_timer_start(self._eng.h, C.byref(self.g), int(histogram),
+                                                                     _capture_stream(stream)))
+
+    def stop_timer(self, histogram: int, stream=None, out=None):
+        """lh_graph_recorder_timer_stop: record now - start into local histogram `histogram`; `out` (an int64 device
+        array) also receives the duration in ns."""
+        ptr = graph_duration_out(out)
+        self._eng._check(self._eng.lib.lh_graph_recorder_timer_stop(self._eng.h, C.byref(self.g), int(histogram),
+                                                                    _capture_stream(stream), ptr))
+
+    @contextlib.contextmanager
+    def timer(self, histogram: int, stream=None):
+        """`with g.timer(h):` -- start_timer before the block and stop_timer after it, on one stream."""
+        self.start_timer(histogram, stream)
+        yield
+        self.stop_timer(histogram, stream)
 
     def close(self, stream=None):
         """Final drain into the current interval on `stream` (None = torch's current stream), then the rows are freed."""

@@ -33,6 +33,13 @@
 #pragma weak lh_graph_recorder_bind
 #pragma weak lh_graph_recorder_ingest
 #pragma weak lh_graph_recorder_destroy
+// The later graph recorder calls: over a build without them, the GraphRecorder method that needs one throws.
+#pragma weak lh_graph_recorder_ingest_keyed_u16
+#pragma weak lh_graph_recorder_ingest_keyed_u32
+#pragma weak lh_graph_recorder_counter_add_u16
+#pragma weak lh_graph_recorder_counter_add_u32
+#pragma weak lh_graph_recorder_timer_start
+#pragma weak lh_graph_recorder_timer_stop
 // And for device subscriptions: over a build without them, NewDeviceSubscription throws.
 #pragma weak lh_board_create
 #pragma weak lh_snapshot_publish
@@ -826,6 +833,47 @@ void GraphRecorder::Histograms(const std::vector<Item> &items, void *stream) {
           "lh_graph_recorder_ingest");
 }
 
+void GraphRecorder::Keyed(const void *d_ids, size_t id_bytes, const void *d_values, uint32_t kind, size_t n, void *stream) {
+    if (!st_ || !st_->ms) throw std::runtime_error("GraphRecorder::Keyed of a closed recorder");
+    MetricSystem *ms = st_->ms;
+    if (id_bytes != 2 && id_bytes != 4) throw std::invalid_argument("GraphRecorder::Keyed: id_bytes must be 2 or 4");
+    auto fn16 = lh_graph_recorder_ingest_keyed_u16;
+    auto fn32 = lh_graph_recorder_ingest_keyed_u32;
+    if (id_bytes == 2 ? !fn16 : !fn32) throw std::runtime_error("GraphRecorder::Keyed: this libloghisto_b200 has no captured keyed ingest");
+    lh_status st = id_bytes == 2 ? fn16(ms->ctx_, &st_->g, static_cast<const uint16_t *>(d_ids), d_values, kind, n, stream)
+                                 : fn32(ms->ctx_, &st_->g, static_cast<const uint32_t *>(d_ids), d_values, kind, n, stream);
+    check(ms->ctx_, st, "lh_graph_recorder_ingest_keyed");
+}
+
+void GraphRecorder::Counters(const void *d_ids, size_t id_bytes, const uint64_t *d_amounts, size_t n, void *stream) {
+    if (!st_ || !st_->ms) throw std::runtime_error("GraphRecorder::Counters of a closed recorder");
+    MetricSystem *ms = st_->ms;
+    if (id_bytes != 2 && id_bytes != 4) throw std::invalid_argument("GraphRecorder::Counters: id_bytes must be 2 or 4");
+    auto fn16 = lh_graph_recorder_counter_add_u16;
+    auto fn32 = lh_graph_recorder_counter_add_u32;
+    if (id_bytes == 2 ? !fn16 : !fn32) throw std::runtime_error("GraphRecorder::Counters: this libloghisto_b200 has no captured counter adds");
+    lh_status st = id_bytes == 2 ? fn16(ms->ctx_, &st_->g, static_cast<const uint16_t *>(d_ids), d_amounts, n, stream)
+                                 : fn32(ms->ctx_, &st_->g, static_cast<const uint32_t *>(d_ids), d_amounts, n, stream);
+    check(ms->ctx_, st, "lh_graph_recorder_counter_add");
+}
+
+void GraphRecorder::StartTimer(size_t name, void *stream) {
+    if (!st_ || !st_->ms) throw std::runtime_error("GraphRecorder::StartTimer of a closed recorder");
+    MetricSystem *ms = st_->ms;
+    if (name >= st_->hnames.size()) throw std::out_of_range("GraphRecorder::StartTimer: no such histogram name");
+    if (!lh_graph_recorder_timer_start) throw std::runtime_error("GraphRecorder::StartTimer: this libloghisto_b200 has no graph timers");
+    check(ms->ctx_, lh_graph_recorder_timer_start(ms->ctx_, &st_->g, (uint32_t)name, stream), "lh_graph_recorder_timer_start");
+}
+
+void GraphRecorder::StopTimer(size_t name, void *stream, int64_t *d_duration_ns) {
+    if (!st_ || !st_->ms) throw std::runtime_error("GraphRecorder::StopTimer of a closed recorder");
+    MetricSystem *ms = st_->ms;
+    if (name >= st_->hnames.size()) throw std::out_of_range("GraphRecorder::StopTimer: no such histogram name");
+    if (!lh_graph_recorder_timer_stop) throw std::runtime_error("GraphRecorder::StopTimer: this libloghisto_b200 has no graph timers");
+    check(ms->ctx_, lh_graph_recorder_timer_stop(ms->ctx_, &st_->g, (uint32_t)name, stream, d_duration_ns),
+          "lh_graph_recorder_timer_stop");
+}
+
 void GraphRecorder::Close(void *stream) {
     if (!st_) return;
     std::shared_ptr<State> st = std::move(st_);
@@ -1614,6 +1662,24 @@ LHMS_API int lhms_graph_recorder_histograms(void *g, const uint32_t *name_index,
     } catch (const std::exception &e) {
         return scope_status(e);
     }
+}
+// GraphRecorder::Keyed / Counters / StartTimer / StopTimer.
+LHMS_API int lhms_graph_keyed(void *g, uint32_t id_bytes, const void *d_ids, const void *d_values, uint32_t kind, size_t n,
+                              void *stream) {
+    if (!g) return LH_ERR_INVALID;
+    try { static_cast<GraphRecorder *>(g)->Keyed(d_ids, id_bytes, d_values, kind, n, stream); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
+}
+LHMS_API int lhms_graph_counters(void *g, uint32_t id_bytes, const void *d_ids, const uint64_t *d_amounts, size_t n, void *stream) {
+    if (!g) return LH_ERR_INVALID;
+    try { static_cast<GraphRecorder *>(g)->Counters(d_ids, id_bytes, d_amounts, n, stream); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
+}
+LHMS_API int lhms_graph_timer_start(void *g, uint32_t name_index, void *stream) {
+    if (!g) return LH_ERR_INVALID;
+    try { static_cast<GraphRecorder *>(g)->StartTimer(name_index, stream); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
+}
+LHMS_API int lhms_graph_timer_stop(void *g, uint32_t name_index, void *stream, int64_t *d_duration_ns) {
+    if (!g) return LH_ERR_INVALID;
+    try { static_cast<GraphRecorder *>(g)->StopTimer(name_index, stream, d_duration_ns); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
 }
 LHMS_API int lhms_graph_recorder_close(void *g, void *stream) {
     if (!g) return LH_ERR_INVALID;

@@ -188,8 +188,8 @@ class GpuTimerToken {
     ~GpuTimerToken();
 
     // Records the duration on the device.  d_duration_ns (device memory, 8-byte aligned, nullable) also receives it as
-    // int64.  Throws std::runtime_error when the library refuses the call (e.g. a misaligned d_duration_ns).  GPU
-    // timers do not time work captured into CUDA graphs.
+    // int64.  Throws std::runtime_error when the library refuses the call (e.g. a misaligned d_duration_ns).  These
+    // tokens do not time work captured into CUDA graphs; GraphRecorder::StartTimer / StopTimer do.
     void Stop(void *stream = kStartStream, int64_t *d_duration_ns = nullptr);
     bool has_slot() const { return held_; }
 
@@ -238,6 +238,19 @@ class GraphRecorder {
         uint32_t kind;
     };
     void Histograms(const std::vector<Item> &items, void *stream);
+    // Kernels only, like Histograms, so each may be captured; each throws before anything is issued (std::out_of_range
+    // for a bad name index, std::invalid_argument for id_bytes other than 2 or 4, std::runtime_error when the library
+    // lacks the call or refuses it, or the recorder is closed).
+    // lh_graph_recorder_ingest_keyed_u16 (id_bytes 2) / _u32 (4): values[i] of `kind` under local histogram id ids[i]
+    // (the index of its name); ids >= the number of names are dropped and counted.
+    void Keyed(const void *d_ids, size_t id_bytes, const void *d_values, uint32_t kind, size_t n, void *stream);
+    // lh_graph_recorder_counter_add_u16 / _u32: amounts[i] into local counter ids[i] (wrapping uint64).
+    void Counters(const void *d_ids, size_t id_bytes, const uint64_t *d_amounts, size_t n, void *stream);
+    // lh_graph_recorder_timer_start / _stop: a GPU-timed span of histogram name `name` (its index).  The caller orders
+    // the start before the stop; one open span per name and recorder (see the header).  d_duration_ns (nullable, 8-byte
+    // aligned device memory) also receives the duration.
+    void StartTimer(size_t name, void *stream);
+    void StopTimer(size_t name, void *stream, int64_t *d_duration_ns = nullptr);
     // Drains what the recorder still holds into the current interval, on `stream`, and frees it (stream-ordered).
     // Idempotent.
     void Close(void *stream = nullptr);

@@ -10,7 +10,8 @@ import ctypes as C
 
 from . import _lib as _L
 from . import build as _build
-from .engine import _batch_array, _capture_stream, _stream, _timer_stream, board_out, board_views, gauge_src
+from .engine import (_batch_array, _capture_stream, _stream, _timer_stream, board_out, board_views, gauge_src,
+                     graph_counter_args, graph_duration_out, graph_keyed_args)
 
 _EMIT = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_char_p, C.c_int, C.c_uint64, C.c_double)
 _lib = None
@@ -90,6 +91,14 @@ def _bind(L):
     L.lhms_graph_recorder_close.restype = C.c_int
     L.lhms_graph_recorder_close.argtypes = [vp, vp]
     L.lhms_graph_recorder_free.argtypes = [vp]
+    L.lhms_graph_keyed.restype = C.c_int
+    L.lhms_graph_keyed.argtypes = [vp, C.c_uint32, vp, vp, C.c_uint32, C.c_size_t, vp]
+    L.lhms_graph_counters.restype = C.c_int
+    L.lhms_graph_counters.argtypes = [vp, C.c_uint32, vp, vp, C.c_size_t, vp]
+    L.lhms_graph_timer_start.restype = C.c_int
+    L.lhms_graph_timer_start.argtypes = [vp, C.c_uint32, vp]
+    L.lhms_graph_timer_stop.restype = C.c_int
+    L.lhms_graph_timer_stop.argtypes = [vp, C.c_uint32, vp, vp]
     L.lhms_subscription_new.restype = vp
     L.lhms_subscription_new.argtypes = [vp, C.c_uint32, names, C.c_uint32, names, C.POINTER(_L.lh_board), C.POINTER(C.c_int)]
     L.lhms_subscription_read.restype = C.c_int
@@ -280,6 +289,53 @@ class GraphRecorder:
         st = self._ms._lib.lhms_graph_recorder_histograms(self._h, idx, ptrs, ns, kinds, len(pairs), _capture_stream(stream))
         if st != 0:
             raise RuntimeError("lhms_graph_recorder_histograms failed (status %d)" % st)
+
+    def _call(self, what, *args):
+        if self._h is None:
+            raise RuntimeError("the graph recorder is closed")
+        st = getattr(self._ms._lib, what)(self._h, *args)
+        if st != 0:
+            raise RuntimeError("%s failed (status %d)" % (what, st))
+
+    def _name(self, name):
+        if name not in self.histogram_ids:
+            raise KeyError("%r is not a histogram of this recorder" % (name,))
+        return self.histogram_ids[name]
+
+    def keyed(self, ids, values, stream=None):
+        """Histogram(name, values[i]) with name the histogram of local id ids[i] (its position in histogram_ids), for
+        every i (lh_graph_recorder_ingest_keyed_*).  ids: uint16, int32 or uint32 device array (an id past the names,
+        a negative int32 among them, is dropped and counted); values: float64, or int64 nanoseconds recorded as
+        float64(ns).  Kernels only, on `stream` (None = torch's current stream), so inside torch.cuda.graph the call
+        is captured.  TypeError / ValueError before anything is issued."""
+        id_bytes, ip, vp, kind, n = graph_keyed_args(ids, values)
+        self._call("lhms_graph_keyed", id_bytes, ip, vp, kind, n, _capture_stream(stream))
+
+    def counters(self, ids, amounts, stream=None):
+        """Counter(name, amounts[i]) with name the counter of local id ids[i] (lh_graph_recorder_counter_add_*): ids as
+        keyed() takes them, amounts int64 or uint64 (added as uint64 bits, wrapping).  Capturable like keyed()."""
+        id_bytes, ip, ap, n = graph_counter_args(ids, amounts)
+        self._call("lhms_graph_counters", id_bytes, ip, ap, n, _capture_stream(stream))
+
+    def start_timer(self, name, stream=None):
+        """Start a GPU-timed span of histogram `name` on `stream` (lh_graph_recorder_timer_start); capturable.  One open
+        span per name: sequential spans are fine, concurrent ones on parallel branches need another recorder."""
+        idx = self._name(name)
+        self._call("lhms_graph_timer_start", idx, _capture_stream(stream))
+
+    def stop_timer(self, name, stream=None, out=None):
+        """Record the span's duration under `name` (lh_graph_recorder_timer_stop), ordered after its start by the
+        caller; `out` (an int64 device array) also receives it in ns.  A stop with no start is dropped and counted."""
+        idx = self._name(name)
+        ptr = graph_duration_out(out)
+        self._call("lhms_graph_timer_stop", idx, _capture_stream(stream), ptr)
+
+    @contextlib.contextmanager
+    def timer(self, name, stream=None):
+        """`with g.timer("layer"):` -- start_timer before the block and stop_timer after it, on one stream."""
+        self.start_timer(name, stream)
+        yield
+        self.stop_timer(name, stream)
 
     def close(self, stream=None):
         """Drains what the recorder holds into the current interval on `stream` (None = torch's current stream) and
