@@ -386,6 +386,77 @@ LH_API lh_status lh_snapshot_publish(lh_ctx *ctx, const lh_board *b, const uint3
 LH_API lh_status lh_board_read(lh_ctx *ctx, const lh_board *b, void *d_out, void *stream);
 LH_API lh_status lh_board_destroy(lh_ctx *ctx, const lh_board *b);
 
+/* ---- raw device subscriptions: each collection's bucket counts in device memory ---------------------------------
+ * SubscribeToRawMetrics (metrics.go:203-215, 508-525) for consumers on the GPU.  A raw board holds k histogram rows;
+ * lh_snapshot_publish_raw writes the running bucket counts of the open snapshot's histograms into them, and kernels
+ * (include/loghisto_b200_device.cuh: lh::raw_percentile / raw_rank / raw_bucket_count) or the capturable query calls
+ * below answer exact percentile, rank and bucket queries from the latest publish with no host call.
+ *
+ * Layout (bytes, from d_rows): k lh_raw_row_header, then from LH_RAW_CELLS_OFFSET(k) k rows of uint64[65536]: cell
+ * key + 32768 of row i holds the number of samples of that publish whose int16 bucket key is <= key (ascending int16
+ * key order, the order K3 and lh_snapshot_reduce rank in).  Only keys [key_lo, key_hi] of the header are written by a
+ * publish: a key below key_lo reads as 0 and a key above key_hi as total.  An empty row has total 0 and key_lo > key_hi.
+ * Each row has its own seqlock: `seq` is odd while a publish writes the row and advances by 2 per publish, so
+ * seq / 2 is the publish number (0 before the first) and every query answer is of one publish.
+ *
+ *   lh_raw_board_create      allocates a board of 1 <= k <= max_histograms rows and writes every header as an empty
+ *                            row of publish 0 (total 0, key_lo 0, key_hi -1), so that queries before the first publish
+ *                            answer as for an empty row and read no cell.  512 KiB per row.  Call it outside any stream
+ *                            capture; it waits for the headers to be written.
+ *   lh_snapshot_publish_raw  writes row i from histogram hist_ids[i] of the open snapshot (its frozen counts, or the
+ *                            all-reduced ones after lh_snapshot_allreduce: publish after the all-reduce, before
+ *                            lh_snapshot_end).  hist_ids[i] = LH_GRAPH_UNBOUND (or hist_ids NULL), or a histogram the
+ *                            interval never touched: an empty row.  No reduction is needed.  LH_ERR_STATE outside a
+ *                            snapshot, LH_ERR_RANGE for an id >= max_histograms other than LH_GRAPH_UNBOUND.  Enqueued on
+ *                            the snapshot stream; it never waits and never allocates.
+ *   lh_raw_percentiles       query i: (d_keys[i], d_vals[i]) = what lh_snapshot_reduce reports for row d_rows[i]'s
+ *                            histogram with percentile d_ps[i], bit for bit (INT32_MIN / NaN for p > 1, NaN or an
+ *                            empty row; the smallest non-empty key for p <= 0).
+ *   lh_raw_ranks             query i: d_ranks[i] = samples of row d_rows[i] whose key is <= compress(d_values[i]) (the
+ *                            bucket lh::record gives the value; NaN and +-Inf have key 0), d_totals[i] = its total.
+ *   lh_raw_percentiles_grid / lh_raw_ranks_grid
+ *                            the same for every row r < k and input j < m: answers at [r * m + j]; d_totals[r] is the
+ *                            total of the publish query (r, 0) read.  LH_ERR_RANGE when k * m >= 2^32.
+ *                            Every query call writes d_publish[i] = the publish number its answer comes from, enqueues ONE
+ *                            kernel on `stream` (NULL = the ingest stream) and nothing else, so it may be captured into a
+ *                            CUDA graph: a replay answers from the publish latest when it runs.  Different queries may
+ *                            come from different publishes.  A row >= k answers as an empty row of publish 0.  Arrays are
+ *                            device memory, naturally aligned (LH_ERR_INVALID otherwise, or NULL, with n > 0: nothing is
+ *                            enqueued); n == 0 enqueues nothing.
+ *   lh_raw_board_destroy     frees the board, stream-ordered after every publish already issued.  The caller guarantees
+ *                            that no query of the board is pending.  lh_destroy frees every raw board left.
+ * A destroyed or foreign handle gets LH_ERR_INVALID. */
+typedef struct lh_raw_row_header {
+    uint64_t seq;                             /* seqlock word: odd while a publish writes the row, +2 per publish */
+    uint64_t publishes;                       /* publishes so far (= seq / 2 when even) */
+    uint64_t total;                           /* samples of the row in the latest publish */
+    int32_t key_lo, key_hi;                   /* the key range that publish wrote (key_lo > key_hi: empty row) */
+} lh_raw_row_header;
+typedef struct lh_raw_board {                 /* pass by value to kernels */
+    uint64_t handle;                          /* opaque */
+    void *d_rows;                             /* device memory: k headers, then k rows of running counts */
+    const double *d_decomp;                   /* the context's decompress table, indexed by (uint16)key */
+    uint32_t k;
+    uint32_t reserved;
+    uint8_t prec[48];                         /* lh::Prec of the context (raw_rank's bucket function), opaque to C */
+} lh_raw_board;
+LH_STATIC_ASSERT(sizeof(lh_raw_row_header) == 32 && offsetof(lh_raw_row_header, key_lo) == 24,
+                 "lh_raw_row_header is 32 bytes: seq, publishes, total, key_lo, key_hi");
+LH_STATIC_ASSERT(sizeof(lh_raw_board) == 80 && offsetof(lh_raw_board, prec) == 32, "lh_raw_board is 80 bytes");
+/* byte offset of row 0's cells from d_rows: the headers rounded up to 256 bytes */
+#define LH_RAW_CELLS_OFFSET(k) ((((uint64_t)(k) * 32u) + 255u) & ~(uint64_t)255u)
+LH_API lh_status lh_raw_board_create(lh_ctx *ctx, uint32_t k, lh_raw_board *out);
+LH_API lh_status lh_snapshot_publish_raw(lh_ctx *ctx, const lh_raw_board *b, const uint32_t *hist_ids);
+LH_API lh_status lh_raw_percentiles(lh_ctx *ctx, const lh_raw_board *b, const uint32_t *d_rows, const double *d_ps,
+                                    uint32_t n, int32_t *d_keys, double *d_vals, uint64_t *d_publish, void *stream);
+LH_API lh_status lh_raw_ranks(lh_ctx *ctx, const lh_raw_board *b, const uint32_t *d_rows, const double *d_values,
+                              uint32_t n, uint64_t *d_ranks, uint64_t *d_totals, uint64_t *d_publish, void *stream);
+LH_API lh_status lh_raw_percentiles_grid(lh_ctx *ctx, const lh_raw_board *b, const double *d_ps, uint32_t m,
+                                         int32_t *d_keys, double *d_vals, uint64_t *d_publish, void *stream);
+LH_API lh_status lh_raw_ranks_grid(lh_ctx *ctx, const lh_raw_board *b, const double *d_values, uint32_t m,
+                                   uint64_t *d_ranks, uint64_t *d_totals, uint64_t *d_publish, void *stream);
+LH_API lh_status lh_raw_board_destroy(lh_ctx *ctx, const lh_raw_board *b);
+
 /* ---- device gauges: RegisterGaugeFunc (metrics.go:299-310) for values that live in device memory -----------------
  * lh_gauges_read reads n scalars from device memory, one per lh_gauge_src, and returns them to the host as float64.  It
  * is stateless: the registry of names lives in the caller (MetricSystem::RegisterDeviceGauge).

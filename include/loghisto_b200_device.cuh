@@ -12,6 +12,10 @@
 //   lh::read_histogram / lh::read_counter
 //                                 the latest collection's processed metrics of a name, from a device subscription
 //                                 board (lh_board, MetricSystem::NewDeviceSubscription)   metrics.go:218, 508-525
+//   lh::raw_percentile / lh::raw_rank / lh::raw_bucket_count
+//                                 exact percentile, rank and bucket queries over the latest collection's bucket counts
+//                                 of a name, from a raw device subscription board (lh_raw_board,
+//                                 MetricSystem::NewRawDeviceSubscription)                 metrics.go:203-215, 508-525
 //
 // `rec` is an lh_recorder (include/loghisto_b200.h) obtained from lh_record_begin on the host and passed to the kernel
 // by value.  Kernels that use it must be enqueued on the recorder's stream between lh_record_begin and lh_record_end;
@@ -590,6 +594,150 @@ __device__ __forceinline__ uint64_t read_counter(const lh_board &b, uint32_t row
         out->total = board::ld_relaxed(r + offsetof(lh_board_counter_row, total));
         out->present = board::ld_relaxed_u32(r + offsetof(lh_board_counter_row, present)) != 0;
         if (board::end_read(b, s)) return s >> 1;
+    }
+}
+
+// ================================================================ querying a raw device subscription (lh_raw_board)
+// A raw board (lh_raw_board_create) holds, per row, the running bucket counts of one histogram of the latest
+// collection that published into it: the buckets the reference hands SubscribeToRawMetrics subscribers
+// (metrics.go:508-525), for kernels and CUDA-graph replays.  Three exact queries, each one seqlock read of one row:
+//
+//   int32_t key; double v;
+//   lh::raw_percentile(raw, row, p, &key, &v);        // p read at run time: the same (key, value) K3 gives for p
+//   uint64_t below, total;
+//   lh::raw_rank(raw, row, budget, &below, &total);   // samples in buckets at or below budget's bucket
+//
+// A read is the protocol of lh::read_histogram applied to the row's own sequence word: ld.acquire.gpu of the word
+// (retried while odd), the header and the cells the query needs with strong relaxed loads, fence.acq_rel.gpu, and the
+// word again; a changed word retries the query.  A row is written by one CTA of k_raw_publish that waits on nothing,
+// so the retry loop ends as soon as that CTA has run.  Each query returns the publish number its answer comes from
+// (0 before the first publish, or for a row >= b.k, which answers as an empty row).  A kernel must not wait for the
+// next publish: collections run on the host, which may never run another.
+
+// Smallest s in [0, total] with float64(s)/float64(total) >= p -- the reference's rule (metrics.go:413) turned into an
+// integer threshold on the running count: the quotient is monotone in s, so "first non-empty bucket whose running count
+// satisfies the rule" == "first non-empty bucket whose running count reaches T".  Returns false when no s satisfies
+// the rule (p > 1 or NaN: percentile() returns its error).
+__device__ __forceinline__ bool percentile_threshold(double p, unsigned long long total, unsigned long long *T) {
+    const double ft = (double)total;
+    if (!(__ddiv_rn(ft, ft) >= p)) return false;                 // even s = total fails (p > 1, NaN)
+    auto ok = [&](unsigned long long s) { return __ddiv_rn((double)s, ft) >= p; };
+    unsigned long long s = 0;
+    if (p > 0.0) {
+        const double est = ceil(p * ft);
+        s = est >= ft ? total : (unsigned long long)est;
+    }
+    int steps = 0;
+    while (s > 0 && ok(s - 1) && steps < 8) { s--; steps++; }
+    while (!ok(s) && steps < 16) { s++; steps++; }
+    if (steps >= 8 && (!ok(s) || (s > 0 && ok(s - 1)))) {        // long plateaus of float64(s) (totals beyond 2^53): bisection
+        unsigned long long lo = 0, hi = total;                  // ok(hi) holds
+        while (lo < hi) { const unsigned long long mid = lo + (hi - lo) / 2; if (ok(mid)) hi = mid; else lo = mid + 1; }
+        s = lo;
+    }
+    *T = s;
+    return true;
+}
+
+namespace raw {
+__device__ __forceinline__ const char *header(const lh_raw_board &b, uint32_t row) {
+    return (const char *)b.d_rows + (size_t)row * sizeof(lh_raw_row_header);
+}
+// cell key + 32768 of the row: running count at key
+__device__ __forceinline__ const char *cells(const lh_raw_board &b, uint32_t row) {
+    return (const char *)b.d_rows + LH_RAW_CELLS_OFFSET(b.k) + (size_t)row * (65536u * 8u);
+}
+__device__ __forceinline__ unsigned long long begin_read(const char *h) {
+    for (;;) {
+        const unsigned long long s = board::ld_acquire((const unsigned long long *)h);
+        if (!(s & 1ull)) return s;
+        __nanosleep(64);
+    }
+}
+__device__ __forceinline__ bool end_read(const char *h, unsigned long long s) {
+    board::fence_acq_rel();
+    return board::ld_relaxed(h) == s;
+}
+struct Range {
+    unsigned long long total;
+    int lo, hi;                  // written keys; lo > hi: empty
+};
+__device__ __forceinline__ Range range(const char *h) {
+    const unsigned long long two = board::ld_relaxed(h + offsetof(lh_raw_row_header, key_lo));
+    return Range{board::ld_relaxed(h + offsetof(lh_raw_row_header, total)), (int)(uint32_t)two, (int)(uint32_t)(two >> 32)};
+}
+// running count at key: 0 below the written range, total above it
+__device__ __forceinline__ unsigned long long running(const char *c, const Range &r, int key) {
+    if (key < r.lo) return 0ull;
+    if (key > r.hi) return r.total;
+    return board::ld_relaxed(c + (size_t)(key + 32768) * 8u);
+}
+}  // namespace raw
+
+// (key, value) of percentile p of row `row`: bit for bit what lh_snapshot_reduce reports for the row's histogram with
+// that p.  INT32_MIN / NaN for p > 1, NaN or an empty row; p <= 0 gives the smallest non-empty key.
+__device__ __forceinline__ uint64_t raw_percentile(const lh_raw_board &b, uint32_t row, double p, int32_t *key, double *val) {
+    *key = (int32_t)0x80000000;
+    *val = __longlong_as_double(0x7FF8000000000000ll);
+    if (row >= b.k) return 0;
+    const char *h = raw::header(b, row), *c = raw::cells(b, row);
+    for (;;) {
+        const unsigned long long s = raw::begin_read(h);
+        const raw::Range r = raw::range(h);
+        unsigned long long T;
+        bool found = false;
+        int lo = r.lo, hi = r.hi;
+        if (r.total && lo <= hi && percentile_threshold(p, r.total, &T)) {
+            if (T == 0) T = 1;                                    // p <= 0: the smallest non-empty bucket
+            while (lo < hi) {                                     // running(hi) == total >= T
+                const int mid = lo + ((hi - lo) >> 1);
+                if (board::ld_relaxed(c + (size_t)(mid + 32768) * 8u) >= T) hi = mid; else lo = mid + 1;
+            }
+            found = true;
+        }
+        if (raw::end_read(h, s)) {
+            if (found) {
+                *key = lo;
+                *val = b.d_decomp[(uint32_t)lo & 0xFFFFu];
+            }
+            return s >> 1;
+        }
+    }
+}
+
+// Samples of row `row` whose bucket key is <= the key lh::record gives v (NaN and +-Inf: key 0), and the row's total.
+__device__ __forceinline__ uint64_t raw_rank(const lh_raw_board &b, uint32_t row, double v, uint64_t *rank, uint64_t *total) {
+    *rank = 0;
+    *total = 0;
+    if (row >= b.k) return 0;
+    const int key = (int)(int16_t)(uint16_t)key16_of(v, *reinterpret_cast<const Prec *>(b.prec));
+    const char *h = raw::header(b, row), *c = raw::cells(b, row);
+    for (;;) {
+        const unsigned long long s = raw::begin_read(h);
+        const raw::Range r = raw::range(h);
+        const unsigned long long n = raw::running(c, r, key);
+        if (raw::end_read(h, s)) {
+            *rank = n;
+            *total = r.total;
+            return s >> 1;
+        }
+    }
+}
+
+// Samples of row `row` in bucket `key` (0 for a key with none, or outside int16).
+__device__ __forceinline__ uint64_t raw_bucket_count(const lh_raw_board &b, uint32_t row, int32_t key, uint64_t *count) {
+    *count = 0;
+    if (row >= b.k) return 0;
+    const char *h = raw::header(b, row), *c = raw::cells(b, row);
+    for (;;) {
+        const unsigned long long s = raw::begin_read(h);
+        const raw::Range r = raw::range(h);
+        const unsigned long long n = key < -32768 || key > 32767 ? 0ull
+                                   : raw::running(c, r, key) - raw::running(c, r, key - 1);
+        if (raw::end_read(h, s)) {
+            *count = n;
+            return s >> 1;
+        }
     }
 }
 

@@ -131,6 +131,24 @@ class lh_board(C.Structure):
                 ("bytes", C.c_uint64)]
 
 
+class lh_raw_row_header(C.Structure):
+    """Header of one row of a raw device subscription board (include/loghisto_b200.h)."""
+    _fields_ = [("seq", C.c_uint64), ("publishes", C.c_uint64), ("total", C.c_uint64), ("key_lo", C.c_int32),
+                ("key_hi", C.c_int32)]
+
+
+class lh_raw_board(C.Structure):
+    """A raw device subscription board (lh_raw_board_create): passed by value to the caller's kernels, which query it
+    with lh::raw_percentile / lh::raw_rank / lh::raw_bucket_count."""
+    _fields_ = [("handle", C.c_uint64), ("d_rows", C.c_void_p), ("d_decomp", C.c_void_p), ("k", C.c_uint32),
+                ("reserved", C.c_uint32), ("prec", C.c_uint8 * 48)]
+
+
+def LH_RAW_CELLS_OFFSET(k: int) -> int:
+    """Byte offset of row 0's running counts from lh_raw_board.d_rows."""
+    return (k * 32 + 255) & ~255
+
+
 LH_GAUGE_F64, LH_GAUGE_F32, LH_GAUGE_F16, LH_GAUGE_BF16, LH_GAUGE_I64, LH_GAUGE_I32, LH_GAUGE_U64 = range(7)
 
 
@@ -182,6 +200,13 @@ SIGNATURES = {
     "lh_snapshot_publish": (_i32, [_vp, C.POINTER(lh_board), _vp, _vp, _vp]),
     "lh_board_read": (_i32, [_vp, C.POINTER(lh_board), _vp, _vp]),
     "lh_board_destroy": (_i32, [_vp, C.POINTER(lh_board)]),
+    "lh_raw_board_create": (_i32, [_vp, _u32, C.POINTER(lh_raw_board)]),
+    "lh_snapshot_publish_raw": (_i32, [_vp, C.POINTER(lh_raw_board), _vp]),
+    "lh_raw_percentiles": (_i32, [_vp, C.POINTER(lh_raw_board), _vp, _vp, _u32, _vp, _vp, _vp, _vp]),
+    "lh_raw_ranks": (_i32, [_vp, C.POINTER(lh_raw_board), _vp, _vp, _u32, _vp, _vp, _vp, _vp]),
+    "lh_raw_percentiles_grid": (_i32, [_vp, C.POINTER(lh_raw_board), _vp, _u32, _vp, _vp, _vp, _vp]),
+    "lh_raw_ranks_grid": (_i32, [_vp, C.POINTER(lh_raw_board), _vp, _u32, _vp, _vp, _vp, _vp]),
+    "lh_raw_board_destroy": (_i32, [_vp, C.POINTER(lh_raw_board)]),
     "lh_gauges_read": (_i32, [_vp, C.POINTER(lh_gauge_src), _u32, _vp]),
     "lh_gpu_timer_start": (_i32, [_vp, _vp, C.POINTER(lh_gpu_timer)]),
     "lh_gpu_timer_stop": (_i32, [_vp, C.POINTER(lh_gpu_timer), _u32, _vp, _vp]),

@@ -106,16 +106,21 @@ BOARD_CLIENT_LIB = os.path.join(ROOT, "tests", "_build", "libboard_read_client.s
 GAUGE_CLIENT_SRC = os.path.join(ROOT, "tests", "gauge_write_client.cu")
 GAUGE_CLIENT_LIB = os.path.join(ROOT, "tests", "_build", "libgauge_write_client.so")
 
+RAW_CLIENT_SRC = os.path.join(ROOT, "tests", "raw_read_client.cu")
+RAW_CLIENT_LIB = os.path.join(ROOT, "tests", "_build", "libraw_read_client.so")
+
 
 def build_device_client(force: bool = False) -> str:
     """CUDA clients of the device API (tests/device_record_client.cu, tests/named_record_client.cu,
     tests/block_recorder_client.cu, tests/gpu_timer_client.cu, tests/graph_record_client.cu,
-    tests/board_read_client.cu, tests/gauge_write_client.cu): separate shared libraries that record into a context from
-    their own kernels, give the GPU timers spans to measure, read device subscriptions, or write device gauges, knowing
-    the library only through the public headers.  Returns the path of the first."""
+    tests/board_read_client.cu, tests/gauge_write_client.cu, tests/raw_read_client.cu): separate shared libraries that
+    record into a context from their own kernels, give the GPU timers spans to measure, read device subscriptions,
+    write device gauges, or query raw device subscriptions, knowing the library only through the public headers.
+    Returns the path of the first."""
     for src, lib in ((CLIENT_SRC, CLIENT_LIB), (NAMED_CLIENT_SRC, NAMED_CLIENT_LIB), (BLOCK_CLIENT_SRC, BLOCK_CLIENT_LIB),
                      (TIMER_CLIENT_SRC, TIMER_CLIENT_LIB), (GRAPH_CLIENT_SRC, GRAPH_CLIENT_LIB),
-                     (BOARD_CLIENT_SRC, BOARD_CLIENT_LIB), (GAUGE_CLIENT_SRC, GAUGE_CLIENT_LIB)):
+                     (BOARD_CLIENT_SRC, BOARD_CLIENT_LIB), (GAUGE_CLIENT_SRC, GAUGE_CLIENT_LIB),
+                     (RAW_CLIENT_SRC, RAW_CLIENT_LIB)):
         deps = [src, DEVICE_HEADER, os.path.join(ROOT, "include", "loghisto_b200.h")]
         if not force and os.path.exists(lib) and _newest(deps) <= os.path.getmtime(lib):
             continue

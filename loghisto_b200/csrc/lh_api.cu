@@ -265,6 +265,11 @@ struct lh_ctx {
     uint64_t next_board = 1;
     int pub_slot = -1;
     BoardParams board_prm{};
+    // raw device subscriptions (lh_raw_board_*): live boards, and the parameter block of their publish kernel (filled
+    // under the lock)
+    std::vector<lh_raw_board> raw_boards;
+    uint64_t next_raw_board = 1;
+    RawPublishParams raw_prm{};
     // device gauges (lh_gauges_read): calls are serialised by gauge_mu (taken before mu), since they share the output
     // buffer, mapped pinned memory that k_gauge_read writes into (grown on demand); gauge_done follows the last launch
     std::mutex gauge_mu;
@@ -1147,6 +1152,7 @@ extern "C" lh_status lh_destroy(lh_ctx *ctx) {
     cudaDeviceSynchronize();
     for (auto &g : ctx->graphs) cudaFree(g.rec.d_buckets);
     for (auto &b : ctx->boards) cudaFree(b.d_board);
+    for (auto &b : ctx->raw_boards) cudaFree(b.d_rows);
     if (ctx->h_gauges) cudaFreeHost(ctx->h_gauges);
     if (ctx->gauge_done) cudaEventDestroy(ctx->gauge_done);
     if (ctx->graph_drained) cudaEventDestroy(ctx->graph_drained);
@@ -2190,6 +2196,151 @@ extern "C" lh_status lh_board_destroy(lh_ctx *ctx, const lh_board *b) {
     if (!bd) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign board");
     LH_CUDA(ctx, cudaFreeAsync(bd->d_board, ctx->snap_stream));   // after every publish issued (all on this stream)
     ctx->boards.erase(ctx->boards.begin() + (bd - ctx->boards.data()));
+    return LH_OK;
+}
+
+// =========================================================== raw device subscriptions
+namespace {
+// headers, the k rows of cells, then the id table of k_raw_stage
+size_t raw_table_offset(uint32_t k) { return LH_RAW_CELLS_OFFSET(k) + (size_t)k * 65536u * 8u; }
+
+// the live raw board a handle names (its memory must match too), or nullptr
+const lh_raw_board *raw_board_of(lh_ctx *ctx, const lh_raw_board *b) {
+    if (!b) return nullptr;
+    for (auto &x : ctx->raw_boards)
+        if (x.handle == b->handle && x.d_rows == b->d_rows) return &x;
+    return nullptr;
+}
+
+// non-NULL and a-byte aligned
+bool arg_ok(const void *p, uintptr_t a) { return p && ((uintptr_t)p & (a - 1u)) == 0; }
+}  // namespace
+
+extern "C" lh_status lh_raw_board_create(lh_ctx *ctx, uint32_t k, lh_raw_board *out) {
+    LH_ENTER(ctx);
+    if (!out) return fail(ctx, LH_ERR_INVALID, "out is NULL");
+    if (k == 0) return fail(ctx, LH_ERR_INVALID, "a raw board needs a row");
+    if (k > ctx->H) return fail(ctx, LH_ERR_RANGE, "more rows than max_histograms");
+    const size_t bytes = raw_table_offset(k) + (size_t)k * 4u;
+    cudaStream_t s = ctx->snap_stream;
+    char *base = nullptr;
+    LH_CUDA(ctx, cudaMallocAsync((void **)&base, bytes, s));
+    // only the headers, each an empty row (publish 0, total 0, key_lo > key_hi): a row's cells are read only inside
+    // the key range its latest publish wrote, so the cells of a row never published are never read
+    std::vector<lh_raw_row_header> empty(k);
+    for (auto &h : empty) { h.key_lo = 0; h.key_hi = -1; }
+    cudaError_t e = cudaMemcpyAsync(base, empty.data(), (size_t)k * sizeof(lh_raw_row_header), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (e != cudaSuccess) {
+        cudaFreeAsync(base, s);
+        return fail(ctx, LH_ERR_CUDA, "lh_raw_board_create", e);
+    }
+    lh_raw_board b{};
+    b.handle = graph_handle(ctx, ctx->next_raw_board++);
+    b.d_rows = base;
+    b.d_decomp = ctx->d_decomp;
+    b.k = k;
+    memcpy(b.prec, &ctx->pc, sizeof(Prec));
+    ctx->raw_boards.push_back(b);
+    *out = b;
+    return LH_OK;
+}
+
+// One k_raw_publish (a CTA per row) on the snapshot stream, after whatever wrote the snapshot view it reads.  Ids that
+// do not fit its parameter block are first copied into the board's table by k_raw_stage launches (see lh_kernels.cuh:
+// a row's word is odd only inside the CTA that writes the row).
+extern "C" lh_status lh_snapshot_publish_raw(lh_ctx *ctx, const lh_raw_board *b, const uint32_t *hist_ids) {
+    LH_ENTER(ctx);
+    const lh_raw_board *bd = raw_board_of(ctx, b);
+    if (!bd) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign raw board");
+    if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "lh_snapshot_publish_raw needs an open snapshot");
+    if (!ids_ok(hist_ids, bd->k, ctx->H)) return fail(ctx, LH_ERR_RANGE, "id >= max_histograms");
+    const View v = snapshot_view(ctx);
+    cudaStream_t s = ctx->snap_stream;
+    RawPublishParams &p = ctx->raw_prm;
+    p.rows = (char *)bd->d_rows;
+    p.cells = reinterpret_cast<unsigned long long *>(p.rows + LH_RAW_CELLS_OFFSET(bd->k));
+    p.table = reinterpret_cast<uint32_t *>(p.rows + raw_table_offset(bd->k));
+    p.buckets = v.buckets;
+    p.flags = v.flags;
+    p.win = ctx->pc.win;
+    for (uint32_t r0 = 0;; r0 += RP_MAX_IDS) {
+        const uint32_t n = std::min<uint32_t>(RP_MAX_IDS, bd->k - r0);
+        p.n_staged = r0;
+        p.n = n;
+        for (uint32_t i = 0; i < n; i++) p.ids[i] = hist_ids ? hist_ids[r0 + i] : LH_GRAPH_UNBOUND;
+        if (r0 + n == bd->k) break;
+        k_raw_stage<<<1, RP_THREADS, 0, s>>>(p);
+        LH_CUDA(ctx, cudaGetLastError());
+        ctx->stats.kernel_launches++;
+    }
+    k_raw_publish<<<bd->k, RP_THREADS, 0, s>>>(p);
+    LH_CUDA(ctx, cudaGetLastError());
+    ctx->stats.kernel_launches++;
+    return LH_OK;
+}
+
+namespace {
+// One k_raw_percentiles / k_raw_ranks over n queries (rows == nullptr: the grid form, m inputs per row), every
+// argument checked before it is enqueued.
+lh_status raw_query(lh_ctx *ctx, const lh_raw_board *b, bool pct, const uint32_t *d_rows, const double *d_x,
+                    uint64_t n, uint32_t m, void *d_out1, void *d_out2, uint64_t *d_publish, void *stream) {
+    const lh_raw_board *bd = raw_board_of(ctx, b);
+    if (!bd) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign raw board");
+    if (n == 0) return LH_OK;
+    if (n > UINT32_MAX) return fail(ctx, LH_ERR_RANGE, "more than 2^32 - 1 queries");
+    const bool grid = m != 0;
+    if ((!grid && !arg_ok(d_rows, 4)) || !arg_ok(d_x, 8) || !arg_ok(d_out1, pct ? 4 : 8) || !arg_ok(d_out2, 8) ||
+        !arg_ok(d_publish, 8))
+        return fail(ctx, LH_ERR_INVALID, "a query array is NULL or not naturally aligned");
+    const uint32_t blocks = (uint32_t)((n + RQ_THREADS - 1) / RQ_THREADS);
+    cudaStream_t s = pick_stream(ctx, stream);
+    if (pct)
+        k_raw_percentiles<<<blocks, RQ_THREADS, 0, s>>>(*bd, grid ? nullptr : d_rows, d_x, (uint32_t)n, m, (int32_t *)d_out1,
+                                                         (double *)d_out2, (unsigned long long *)d_publish);
+    else
+        k_raw_ranks<<<blocks, RQ_THREADS, 0, s>>>(*bd, grid ? nullptr : d_rows, d_x, (uint32_t)n, m,
+                                                   (unsigned long long *)d_out1, (unsigned long long *)d_out2,
+                                                   (unsigned long long *)d_publish);
+    LH_CUDA(ctx, cudaGetLastError());
+    ctx->stats.kernel_launches++;
+    return LH_OK;
+}
+}  // namespace
+
+extern "C" lh_status lh_raw_percentiles(lh_ctx *ctx, const lh_raw_board *b, const uint32_t *d_rows, const double *d_ps,
+                                        uint32_t n, int32_t *d_keys, double *d_vals, uint64_t *d_publish, void *stream) {
+    LH_ENTER(ctx);
+    return raw_query(ctx, b, true, d_rows, d_ps, n, 0, d_keys, d_vals, d_publish, stream);
+}
+
+extern "C" lh_status lh_raw_ranks(lh_ctx *ctx, const lh_raw_board *b, const uint32_t *d_rows, const double *d_values,
+                                  uint32_t n, uint64_t *d_ranks, uint64_t *d_totals, uint64_t *d_publish, void *stream) {
+    LH_ENTER(ctx);
+    return raw_query(ctx, b, false, d_rows, d_values, n, 0, d_ranks, d_totals, d_publish, stream);
+}
+
+extern "C" lh_status lh_raw_percentiles_grid(lh_ctx *ctx, const lh_raw_board *b, const double *d_ps, uint32_t m,
+                                             int32_t *d_keys, double *d_vals, uint64_t *d_publish, void *stream) {
+    LH_ENTER(ctx);
+    const lh_raw_board *bd = raw_board_of(ctx, b);
+    return raw_query(ctx, b, true, nullptr, d_ps, bd ? (uint64_t)bd->k * m : 0, m, d_keys, d_vals, d_publish, stream);
+}
+
+extern "C" lh_status lh_raw_ranks_grid(lh_ctx *ctx, const lh_raw_board *b, const double *d_values, uint32_t m,
+                                       uint64_t *d_ranks, uint64_t *d_totals, uint64_t *d_publish, void *stream) {
+    LH_ENTER(ctx);
+    const lh_raw_board *bd = raw_board_of(ctx, b);
+    return raw_query(ctx, b, false, nullptr, d_values, bd ? (uint64_t)bd->k * m : 0, m, d_ranks, d_totals, d_publish,
+                     stream);
+}
+
+extern "C" lh_status lh_raw_board_destroy(lh_ctx *ctx, const lh_raw_board *b) {
+    LH_ENTER(ctx);
+    const lh_raw_board *bd = raw_board_of(ctx, b);
+    if (!bd) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign raw board");
+    LH_CUDA(ctx, cudaFreeAsync(bd->d_rows, ctx->snap_stream));   // after every publish issued (all on this stream)
+    ctx->raw_boards.erase(ctx->raw_boards.begin() + (bd - ctx->raw_boards.data()));
     return LH_OK;
 }
 

@@ -23,6 +23,8 @@
 //   k_ingest_batch          many device arrays under many ids (lh_ingest_batch, lh_graph_recorder_ingest)
 //   k_ingest_keyed_graph    (id,value) pairs into a graph recorder's rows (lh_graph_recorder_ingest_keyed_*)
 //   k_graph_drain           graph recorders' rows -> the interval being frozen (lh_snapshot_begin)
+//   k_raw_publish, k_raw_percentiles, k_raw_ranks   running bucket counts of a snapshot -> raw device subscription rows,
+//                           and exact percentile / rank queries over them (lh_snapshot_publish_raw, lh_raw_*)
 //   misc k_clear_touched, k_fill_decompress, k_compress_probe, k_fastpath_margin, k_fastpath_certify, k_stream_probe,
 //        k_gen_stream, k_gen_ids_u16
 //
@@ -1178,30 +1180,8 @@ __device__ __forceinline__ void reduce_dense(uint32_t level, const unsigned long
     }
 }
 
-// Smallest s in [0, total] with float64(s)/float64(total) >= p -- the reference's rule (metrics.go:413) turned into an
-// integer threshold on the running count: the quotient is monotone in s, so "first non-empty bucket whose running count
-// satisfies the rule" == "first non-empty bucket whose running count reaches T".  Returns false when no s satisfies
-// the rule (p > 1 or NaN: percentile() returns its error).
-__device__ __forceinline__ bool percentile_threshold(double p, unsigned long long total, unsigned long long *T) {
-    const double ft = (double)total;
-    if (!(__ddiv_rn(ft, ft) >= p)) return false;                 // even s = total fails (p > 1, NaN)
-    auto ok = [&](unsigned long long s) { return __ddiv_rn((double)s, ft) >= p; };
-    unsigned long long s = 0;
-    if (p > 0.0) {
-        const double est = ceil(p * ft);
-        s = est >= ft ? total : (unsigned long long)est;
-    }
-    int steps = 0;
-    while (s > 0 && ok(s - 1) && steps < 8) { s--; steps++; }
-    while (!ok(s) && steps < 16) { s++; steps++; }
-    if (steps >= 8 && (!ok(s) || (s > 0 && ok(s - 1)))) {        // long plateaus of float64(s) (totals beyond 2^53): bisection
-        unsigned long long lo = 0, hi = total;                  // ok(hi) holds
-        while (lo < hi) { const unsigned long long mid = lo + (hi - lo) / 2; if (ok(mid)) hi = mid; else lo = mid + 1; }
-        s = lo;
-    }
-    *T = s;
-    return true;
-}
+// percentile_threshold (the integer form of the reference's percentile rule) lives in the public device header,
+// where lh::raw_percentile shares it.
 
 // One CTA per histogram.  Untouched histograms are answered without reading a bucket.  A histogram whose counts all
 // lie in the fast window (flag 1; the normal case) is reduced from shared memory: its 2*win-1 cells are loaded once
@@ -2048,6 +2028,162 @@ k_gauge_read(const __grid_constant__ GaugeParams p) {
     default: asm("cvt.rn.f64.u64 %0, %1;" : "=d"(v) : "l"(gauge::ld64(e.p))); break;   // LH_GAUGE_U64
     }
     p.out[i] = v;
+}
+
+// ----------------------------------------------------------- raw device subscriptions (lh_raw_*, lh_snapshot_publish_raw)
+// k_raw_publish writes the running bucket counts of one collection into a raw board (layout: include/loghisto_b200.h),
+// one CTA per row, each row under its own seqlock whose word is the row header's first uint64:
+//   1. thread 0 makes the word odd, fence.acq_rel.gpu, __syncthreads;
+//   2. the row's id picks its source row of the snapshot view and that row's flag picks the cells: none (flag 0 or
+//      unbound: an empty row), the 2*win-1 keys of the fast window (flag 1), or all 65 536 keys (flag & 2).  The cells
+//      are loaded in ascending key order in chunks of RP_CHUNK, block-scanned with the running total of the chunks
+//      before as carry (the window of precision 250 is 43 669 cells, more than shared memory holds at once), and
+//      written with strong relaxed stores to cell key + 32768 of the row;
+//   3. thread 0 writes total and the key range into the header, __threadfence, __syncthreads;
+//   4. thread 0 writes the publish count and makes the word even with st.release.gpu.
+// Readers (include/loghisto_b200_device.cuh: lh::raw_percentile / raw_rank / raw_bucket_count, which k_raw_percentiles
+// and k_raw_ranks call) load the word with ld.acquire.gpu and retry while it is odd, load the header and the cells they
+// need with strong relaxed loads, then fence.acq_rel.gpu and the word again, and retry if it changed.  A reader that
+// saw a store of this publish synchronises with step 1's fence, so its second load of the word sees the odd value or a
+// later one and it retries; a reader that saw step 4's even word sees every store before it.  Cells outside the header's
+// range are never read (they read as 0 below it and total above it), so a dense row published earlier leaves nothing a
+// later window-only publish of the row has to clear.
+//
+// Termination: the CTA that writes a row waits on nothing -- no lock, no flag, no other CTA or kernel -- so once it is
+// resident it finishes in a bounded number of steps, and the row's word is odd only while that CTA is resident.  A
+// reader therefore spins only while a resident writer runs, whatever else occupies the GPU (CTAs of the same launch
+// that have not started yet leave their rows' words even).  An id table too large for one parameter block is first
+// copied into the board's table area by k_raw_stage launches, which touch no word.
+constexpr int RP_THREADS = 512;
+constexpr int RP_PER = 8;                        // contiguous cells per thread in the scan
+constexpr int RP_CHUNK = RP_THREADS * RP_PER;    // cells per chunk
+constexpr int RP_MAX_IDS = 4096;                 // ids per launch: 4 B each in the parameter block
+
+// shared-memory index of chunk cell i: one pad word per 8 cells, so that the scan's per-thread runs of 8 hit distinct
+// banks
+__device__ __forceinline__ uint32_t rp_slot(uint32_t i) { return i + (i >> 3); }
+
+struct RawPublishParams {
+    char *rows;                              // k lh_raw_row_header
+    unsigned long long *cells;               // k rows of uint64[65536]
+    uint32_t *table;                         // ids staged by k_raw_stage, [n_staged]
+    const unsigned long long *buckets;       // the snapshot view's rows and flags
+    const uint32_t *flags;
+    uint32_t win;
+    uint32_t n_staged, n;                    // ids in `table`, then in ids[]
+    uint32_t ids[RP_MAX_IDS];
+};
+
+__global__ void __launch_bounds__(RP_THREADS)
+k_raw_stage(const __grid_constant__ RawPublishParams p) {
+    for (uint32_t i = threadIdx.x; i < p.n; i += RP_THREADS) p.table[p.n_staged + i] = p.ids[i];
+}
+
+__global__ void __launch_bounds__(RP_THREADS)
+k_raw_publish(const __grid_constant__ RawPublishParams p) {
+    __shared__ unsigned long long s_cells[RP_CHUNK + RP_CHUNK / 8];
+    __shared__ unsigned long long s_warp[RP_THREADS / 32];
+    const uint32_t row = blockIdx.x, t = threadIdx.x, lane = t & 31u, warp = t >> 5;
+    const uint32_t id = row < p.n_staged ? p.table[row] : p.ids[row - p.n_staged];
+    const uint32_t level = id == LH_GRAPH_UNBOUND ? 0u : p.flags[id];
+    char *h = p.rows + (size_t)row * sizeof(lh_raw_row_header);
+    unsigned long long *seq = reinterpret_cast<unsigned long long *>(h);
+    if (t == 0) {
+        board::st_relaxed(seq, board::ld_relaxed(seq) + 1ull);   // odd: the previous publish ended (stream order)
+        board::fence_acq_rel();
+    }
+    __syncthreads();
+    int lo = 0, hi = -1;                                          // empty
+    unsigned long long carry = 0;
+    if (level) {
+        lo = (level & 2u) ? -32768 : -(int)(p.win - 1u);
+        hi = (level & 2u) ? 32767 : (int)(p.win - 1u);
+        const uint32_t n = (uint32_t)(hi - lo + 1);
+        const unsigned long long *src = p.buckets + (size_t)id * 65536u;
+        unsigned long long *dst = p.cells + (size_t)row * 65536u + (uint32_t)(lo + 32768);
+        for (uint32_t c0 = 0; c0 < n; c0 += RP_CHUNK) {
+#pragma unroll
+            for (int j = 0; j < RP_PER; j++) {                    // coalesced: chunk cell i is key lo + c0 + i
+                const uint32_t i = (uint32_t)j * RP_THREADS + t;
+                s_cells[rp_slot(i)] = c0 + i < n ? src[(uint32_t)(lo + (int)(c0 + i)) & 0xFFFFu] : 0ull;
+            }
+            __syncthreads();
+            unsigned long long v[RP_PER], local = 0;
+#pragma unroll
+            for (int j = 0; j < RP_PER; j++) { v[j] = s_cells[rp_slot(t * RP_PER + j)]; local += v[j]; }
+            unsigned long long incl = local;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+                if (lane >= (uint32_t)o) incl += y;
+            }
+            if (lane == 31) s_warp[warp] = incl;
+            __syncthreads();
+            if (warp == 0) {
+                const unsigned long long w = lane < RP_THREADS / 32 ? s_warp[lane] : 0ull;
+                unsigned long long wi = w;
+#pragma unroll
+                for (int o = 1; o < RP_THREADS / 32; o <<= 1) {
+                    const unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, wi, o);
+                    if (lane >= (uint32_t)o) wi += y;
+                }
+                if (lane < RP_THREADS / 32) s_warp[lane] = wi - w;   // exclusive prefix of the warp totals
+            }
+            __syncthreads();
+            unsigned long long run = carry + s_warp[warp] + incl - local;
+#pragma unroll
+            for (int j = 0; j < RP_PER; j++) { run += v[j]; s_cells[rp_slot(t * RP_PER + j)] = run; }
+            __syncthreads();
+#pragma unroll
+            for (int j = 0; j < RP_PER; j++) {
+                const uint32_t i = (uint32_t)j * RP_THREADS + t;
+                if (c0 + i < n) board::st_relaxed(dst + c0 + i, s_cells[rp_slot(i)]);
+            }
+            carry = s_cells[rp_slot(RP_CHUNK - 1)];                // the running count after this chunk
+            __syncthreads();                                      // before the next chunk overwrites s_cells / s_warp
+        }
+    }
+    if (t == 0) {
+        board::st_relaxed(h + offsetof(lh_raw_row_header, total), carry);
+        board::st_relaxed(h + offsetof(lh_raw_row_header, key_lo),
+                          (unsigned long long)(uint32_t)lo | (unsigned long long)(uint32_t)hi << 32);
+    }
+    __threadfence();
+    __syncthreads();
+    if (t == 0) {
+        const unsigned long long s = board::ld_relaxed(seq) + 1ull;   // even
+        board::st_relaxed(h + offsetof(lh_raw_row_header, publishes), s >> 1);
+        board::st_release(seq, s);
+    }
+}
+
+// One thread per query; the answers are the device API's (one definition of the read).  rows == nullptr: the grid
+// form, query i is row i / m with input i % m.
+constexpr int RQ_THREADS = 256;
+
+__global__ void __launch_bounds__(RQ_THREADS)
+k_raw_percentiles(const lh_raw_board b, const uint32_t *__restrict__ rows, const double *__restrict__ ps, uint32_t n,
+                  uint32_t m, int32_t *__restrict__ keys, double *__restrict__ vals, unsigned long long *__restrict__ publish) {
+    const uint32_t i = blockIdx.x * RQ_THREADS + threadIdx.x;
+    if (i >= n) return;
+    int32_t key;
+    double val;
+    publish[i] = raw_percentile(b, rows ? rows[i] : i / m, ps[rows ? i : i % m], &key, &val);
+    keys[i] = key;
+    vals[i] = val;
+}
+
+__global__ void __launch_bounds__(RQ_THREADS)
+k_raw_ranks(const lh_raw_board b, const uint32_t *__restrict__ rows, const double *__restrict__ values, uint32_t n,
+            uint32_t m, unsigned long long *__restrict__ ranks, unsigned long long *__restrict__ totals,
+            unsigned long long *__restrict__ publish) {
+    const uint32_t i = blockIdx.x * RQ_THREADS + threadIdx.x;
+    if (i >= n) return;
+    uint64_t rank, total;
+    publish[i] = raw_rank(b, rows ? rows[i] : i / m, values[rows ? i : i % m], &rank, &total);
+    ranks[i] = rank;
+    if (rows) totals[i] = total;
+    else if (i % m == 0) totals[i / m] = total;
 }
 
 // ----------------------------------------------------------- GPU timers (lh_gpu_timer_*)

@@ -442,6 +442,112 @@ class Board:
         self.close()
 
 
+def _raw_input(x, what: str, device: int):
+    """(address, length) of the query inputs of a raw board: a contiguous 1-D float64 CUDA tensor on `device`.
+    TypeError otherwise, before anything is issued."""
+    import torch
+    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float64 and x.dim() == 1
+            and x.is_contiguous() and x.device.index == device):
+        raise TypeError(f"{what} must be a contiguous 1-D float64 CUDA tensor on cuda:{device}")
+    return x.data_ptr(), x.numel()
+
+
+def raw_percentiles(call, k: int, ps, device: int, stream):
+    """Every row of a raw board for each p of `ps` (a float64 CUDA tensor of length m), through `call` (the
+    lh_raw_percentiles_grid form: d_ps, m, d_keys, d_vals, d_publish, stream): returns keys int32 [k, m], values
+    float64 [k, m] and publish numbers int64 [k, m].  One kernel on `stream` (None = torch's current stream), no
+    synchronisation: the tensors hold the answers once the stream has run it."""
+    import torch
+    ptr, m = _raw_input(ps, "ps", device)
+    dev = torch.device("cuda", device)
+    keys = torch.empty((k, m), dtype=torch.int32, device=dev)
+    vals = torch.empty((k, m), dtype=torch.float64, device=dev)
+    pub = torch.empty((k, m), dtype=torch.int64, device=dev)
+    if m:
+        call(ptr, m, keys.data_ptr(), vals.data_ptr(), pub.data_ptr(), _capture_stream(stream))
+    return keys, vals, pub
+
+
+def raw_ranks(call, k: int, values, device: int, stream):
+    """Every row of a raw board for each value of `values` (a float64 CUDA tensor of length m), through `call` (the
+    lh_raw_ranks_grid form): returns ranks int64 [k, m] (samples at or below each value's bucket), totals int64 [k]
+    (row r's total in the publish its query (r, 0) read) and publish numbers int64 [k, m].  Counts are the uint64 bits.
+    As raw_percentiles: one kernel, no synchronisation."""
+    import torch
+    ptr, m = _raw_input(values, "values", device)
+    dev = torch.device("cuda", device)
+    ranks = torch.empty((k, m), dtype=torch.int64, device=dev)
+    pub = torch.empty((k, m), dtype=torch.int64, device=dev)
+    if not m:
+        return ranks, torch.zeros(k, dtype=torch.int64, device=dev), pub
+    totals = torch.empty(k, dtype=torch.int64, device=dev)
+    call(ptr, m, ranks.data_ptr(), totals.data_ptr(), pub.data_ptr(), _capture_stream(stream))
+    return ranks, totals, pub
+
+
+class RawBoard:
+    """A raw device subscription board of an Engine (Engine.raw_board): `board` is the lh_raw_board to pass by value to
+    kernels, which query it with lh::raw_percentile / lh::raw_rank / lh::raw_bucket_count."""
+
+    def __init__(self, engine: "Engine", k: int):
+        self._eng = engine
+        self.board = L.lh_raw_board()
+        engine._check(engine.lib.lh_raw_board_create(engine.h, int(k), C.byref(self.board)))
+        self.k = int(k)
+        self._open = True
+
+    def publish(self, hist_ids=None):
+        """lh_snapshot_publish_raw: row i from histogram hist_ids[i] of the open snapshot (None = every row unbound;
+        L.LH_GRAPH_UNBOUND = that row)."""
+        h = _ids(hist_ids)[0] if hist_ids is not None else None
+        self._eng._check(self._eng.lib.lh_snapshot_publish_raw(self._eng.h, C.byref(self.board), h))
+
+    def _pairs(self, fn, rows, x, what, out_dtypes, stream):
+        import torch
+        ptr, n = _raw_input(x, what, self._eng.device)
+        if not (isinstance(rows, torch.Tensor) and rows.is_cuda and rows.dtype in (torch.int32, torch.uint32)
+                and rows.dim() == 1 and rows.is_contiguous() and rows.device.index == self._eng.device):
+            raise TypeError(f"rows must be a contiguous 1-D int32 or uint32 CUDA tensor on cuda:{self._eng.device}")
+        if rows.numel() != n:
+            raise ValueError(f"{rows.numel()} rows but {n} {what}")
+        outs = [torch.empty(n, dtype=dt, device=rows.device) for dt in out_dtypes]
+        self._eng._check(fn(self._eng.h, C.byref(self.board), rows.data_ptr(), ptr, n,
+                            *[o.data_ptr() for o in outs], _capture_stream(stream)))
+        return tuple(outs)
+
+    def percentiles(self, ps, rows=None, stream=None):
+        """rows None: lh_raw_percentiles_grid, (keys, values, publish) [k, m] for every row and each p of `ps`.
+        Otherwise lh_raw_percentiles, one query (rows[i], ps[i]) each: (keys, values, publish) [n]."""
+        import torch
+        lib, h = self._eng.lib, self._eng.h
+        if rows is not None:
+            return self._pairs(lib.lh_raw_percentiles, rows, ps, "ps", (torch.int32, torch.float64, torch.int64), stream)
+        return raw_percentiles(lambda *a: self._eng._check(lib.lh_raw_percentiles_grid(h, C.byref(self.board), *a)),
+                               self.k, ps, self._eng.device, stream)
+
+    def ranks(self, values, rows=None, stream=None):
+        """rows None: lh_raw_ranks_grid, (ranks [k, m], totals [k], publish [k, m]).  Otherwise lh_raw_ranks, one query
+        (rows[i], values[i]) each: (ranks, totals, publish) [n]."""
+        import torch
+        lib, h = self._eng.lib, self._eng.h
+        if rows is not None:
+            return self._pairs(lib.lh_raw_ranks, rows, values, "values", (torch.int64, torch.int64, torch.int64), stream)
+        return raw_ranks(lambda *a: self._eng._check(lib.lh_raw_ranks_grid(h, C.byref(self.board), *a)),
+                         self.k, values, self._eng.device, stream)
+
+    def close(self):
+        """lh_raw_board_destroy (stream-ordered after every publish issued); no query of the board may be pending."""
+        if self._open:
+            self._open = False
+            self._eng._check(self._eng.lib.lh_raw_board_destroy(self._eng.h, C.byref(self.board)))
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+
 class Engine:
     def __init__(self, device: int = 0, max_histograms: int = 1, max_counters: int = 1,
                  staging_bytes: int = 0, staging_slots: int = 0, precision: int = 0):
@@ -676,6 +782,10 @@ class Engine:
     def board(self, k: int = 0, kc: int = 0) -> "Board":
         """A device subscription board of k histogram rows and kc counter rows (lh_board_create)."""
         return Board(self, k, kc)
+
+    def raw_board(self, k: int) -> "RawBoard":
+        """A raw device subscription board of k histogram rows (lh_raw_board_create)."""
+        return RawBoard(self, k)
 
     def read_gauges(self, tensors) -> np.ndarray:
         """lh_gauges_read of one-element CUDA tensors (gauge_src): float64(value) of each, read on the snapshot stream

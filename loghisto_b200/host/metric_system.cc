@@ -45,6 +45,12 @@
 #pragma weak lh_snapshot_publish
 #pragma weak lh_board_read
 #pragma weak lh_board_destroy
+// And for raw device subscriptions: over a build without them, NewRawDeviceSubscription throws.
+#pragma weak lh_raw_board_create
+#pragma weak lh_snapshot_publish_raw
+#pragma weak lh_raw_percentiles_grid
+#pragma weak lh_raw_ranks_grid
+#pragma weak lh_raw_board_destroy
 // And for device gauges: over a build without them, RegisterDeviceGauge throws.
 #pragma weak lh_gauges_read
 
@@ -62,6 +68,13 @@ struct DeviceSubscription::State {
     MetricSystem *ms;                   // nullptr once closed (or once the system is gone)
     lh_board b{};
     std::vector<std::string> hnames, cnames;
+};
+
+// an open raw device subscription, shared like DeviceSubscription::State
+struct RawDeviceSubscription::State {
+    MetricSystem *ms;                   // nullptr once closed (or once the system is gone)
+    lh_raw_board b{};
+    std::vector<std::string> hnames;
 };
 
 namespace {
@@ -442,6 +455,7 @@ MetricSystem::~MetricSystem() {
     {   // likewise for subscriptions' boards
         std::lock_guard<std::mutex> lk(sub_mu_);
         for (auto &d : subs_) d->ms = nullptr;
+        for (auto &d : raw_subs_) d->ms = nullptr;
     }
     lh_destroy(ctx_);
 }
@@ -915,6 +929,18 @@ DeviceSubscription MetricSystem::NewDeviceSubscription(const std::vector<std::st
     return d;
 }
 
+namespace {
+// the id each name carries in this collection's labels (id_of: the names of Histograms / Rates), or LH_GRAPH_UNBOUND
+std::vector<uint32_t> bind_rows(const std::vector<std::string> &names, const std::unordered_map<std::string, uint32_t> &id_of) {
+    std::vector<uint32_t> ids(names.size());
+    for (size_t i = 0; i < ids.size(); i++) {
+        auto it = id_of.find(names[i]);
+        ids[i] = it == id_of.end() ? LH_GRAPH_UNBOUND : it->second;
+    }
+    return ids;
+}
+}  // namespace
+
 // With sub_mu_ held, between the reduction of collectRawMetrics and lh_snapshot_end: row i of every open subscription
 // is bound to the id that carries its name in this collection's labels, if the name is in Histograms (hid_of) or
 // Rates (cid_of); totals are the Counters values.  The first failure is returned; the other boards still publish.
@@ -922,15 +948,9 @@ lh_status MetricSystem::publish_subscriptions(const RawMetricSet &raw, const std
                                               const std::unordered_map<std::string, uint32_t> &cid_of) {
     lh_status first = LH_OK;
     for (auto &d : subs_) {
-        std::vector<uint32_t> hids(d->hnames.size()), cids(d->cnames.size());
+        const std::vector<uint32_t> hids = bind_rows(d->hnames, hid_of), cids = bind_rows(d->cnames, cid_of);
         std::vector<uint64_t> totals(d->cnames.size());
-        for (size_t i = 0; i < hids.size(); i++) {
-            auto it = hid_of.find(d->hnames[i]);
-            hids[i] = it == hid_of.end() ? LH_GRAPH_UNBOUND : it->second;
-        }
-        for (size_t i = 0; i < cids.size(); i++) {
-            auto it = cid_of.find(d->cnames[i]);
-            cids[i] = it == cid_of.end() ? LH_GRAPH_UNBOUND : it->second;
+        for (size_t i = 0; i < totals.size(); i++) {
             auto t = raw.Counters.find(d->cnames[i]);
             totals[i] = t == raw.Counters.end() ? 0 : t->second;
         }
@@ -971,6 +991,78 @@ DeviceSubscription &DeviceSubscription::operator=(DeviceSubscription &&o) noexce
     return *this;
 }
 DeviceSubscription::~DeviceSubscription() {
+    try { Close(); } catch (...) {}
+}
+
+// ---- raw device subscriptions --------------------------------------------------------------------------------------
+RawDeviceSubscription MetricSystem::NewRawDeviceSubscription(const std::vector<std::string> &histograms) {
+    if (!lh_raw_board_create || !lh_snapshot_publish_raw || !lh_raw_percentiles_grid || !lh_raw_ranks_grid ||
+        !lh_raw_board_destroy)
+        throw std::runtime_error("NewRawDeviceSubscription: this libloghisto_b200 has no raw device subscriptions");
+    auto st = std::make_shared<RawDeviceSubscription::State>();
+    st->ms = this;
+    st->hnames = histograms;
+    check(ctx_, lh_raw_board_create(ctx_, (uint32_t)histograms.size(), &st->b), "lh_raw_board_create");
+    std::lock_guard<std::mutex> lk(sub_mu_);
+    raw_subs_.push_back(st);
+    RawDeviceSubscription d;
+    d.st_ = std::move(st);
+    return d;
+}
+
+// With sub_mu_ held, before lh_snapshot_end: row i of every open raw subscription is bound as publish_subscriptions
+// binds histogram rows.  The first failure is returned; the other boards still publish.
+lh_status MetricSystem::publish_raw_subscriptions(const std::unordered_map<std::string, uint32_t> &hid_of) {
+    lh_status first = LH_OK;
+    for (auto &d : raw_subs_) {
+        const std::vector<uint32_t> hids = bind_rows(d->hnames, hid_of);
+        const lh_status st = lh_snapshot_publish_raw(ctx_, &d->b, hids.data());
+        if (st != LH_OK && first == LH_OK) first = st;
+    }
+    return first;
+}
+
+const lh_raw_board &RawDeviceSubscription::board() const {
+    if (!st_) throw std::runtime_error("RawDeviceSubscription::board of a closed subscription");
+    return st_->b;
+}
+
+void RawDeviceSubscription::Percentiles(const double *d_ps, uint32_t m, int32_t *d_keys, double *d_vals,
+                                        uint64_t *d_publish, void *stream) {
+    if (!st_ || !st_->ms) throw std::runtime_error("RawDeviceSubscription::Percentiles of a closed subscription");
+    MetricSystem *ms = st_->ms;
+    check(ms->ctx_, lh_raw_percentiles_grid(ms->ctx_, &st_->b, d_ps, m, d_keys, d_vals, d_publish, stream),
+          "lh_raw_percentiles_grid");
+}
+
+void RawDeviceSubscription::Ranks(const double *d_values, uint32_t m, uint64_t *d_ranks, uint64_t *d_totals,
+                                  uint64_t *d_publish, void *stream) {
+    if (!st_ || !st_->ms) throw std::runtime_error("RawDeviceSubscription::Ranks of a closed subscription");
+    MetricSystem *ms = st_->ms;
+    check(ms->ctx_, lh_raw_ranks_grid(ms->ctx_, &st_->b, d_values, m, d_ranks, d_totals, d_publish, stream),
+          "lh_raw_ranks_grid");
+}
+
+void RawDeviceSubscription::Close() {
+    if (!st_) return;
+    std::shared_ptr<State> st = std::move(st_);
+    MetricSystem *ms = st->ms;
+    if (!ms) return;
+    std::lock_guard<std::mutex> lk(ms->sub_mu_);   // not during a collection's publish
+    auto &v = ms->raw_subs_;
+    v.erase(std::remove(v.begin(), v.end(), st), v.end());
+    st->ms = nullptr;
+    check(ms->ctx_, lh_raw_board_destroy(ms->ctx_, &st->b), "lh_raw_board_destroy");
+}
+
+RawDeviceSubscription &RawDeviceSubscription::operator=(RawDeviceSubscription &&o) noexcept {
+    if (this != &o) {
+        try { Close(); } catch (...) {}
+        st_ = std::move(o.st_);
+    }
+    return *this;
+}
+RawDeviceSubscription::~RawDeviceSubscription() {
     try { Close(); } catch (...) {}
 }
 
@@ -1158,7 +1250,7 @@ std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
     }
     {   // device subscriptions: this collection's rows, from the reduction above, before the snapshot ends
         std::lock_guard<std::mutex> lk(sub_mu_);
-        if (!subs_.empty()) {
+        if (!subs_.empty() || !raw_subs_.empty()) {
             std::unordered_map<std::string, uint32_t> hid_of, cid_of;   // names of Histograms / Rates -> their ids
             for (size_t h = 0; h < hnames.size(); h++)
                 if (sp.offsets[h] != sp.offsets[h + 1]) hid_of.emplace(hnames[h], (uint32_t)h);
@@ -1166,6 +1258,8 @@ std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
                 if (sp.counter_deltas[c] || touched[c]) cid_of.emplace(cnames[c], (uint32_t)c);
             if (publish_subscriptions(*raw, hid_of, cid_of) != LH_OK)   // the host's metric set is still delivered
                 fprintf(stderr, "loghisto: lh_snapshot_publish failed: %s\n", lh_last_error(ctx_));
+            if (publish_raw_subscriptions(hid_of) != LH_OK)
+                fprintf(stderr, "loghisto: lh_snapshot_publish_raw failed: %s\n", lh_last_error(ctx_));
         }
     }
     check(ctx_, lh_snapshot_end(ctx_), "lh_snapshot_end");
@@ -1715,6 +1809,47 @@ LHMS_API int lhms_subscription_close(void *d) {
     try { static_cast<DeviceSubscription *>(d)->Close(); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
 }
 LHMS_API void lhms_subscription_free(void *d) { delete static_cast<DeviceSubscription *>(d); }
+// MetricSystem::NewRawDeviceSubscription: a RawDeviceSubscription handle (NULL with *status set on failure); *out
+// receives its board.  Free it with lhms_raw_subscription_free, which closes it if lhms_raw_subscription_close has not.
+LHMS_API void *lhms_raw_subscription_new(void *ms, uint32_t n_h, const char *const *h_names, lh_raw_board *out,
+                                         int *status) {
+    int dummy;
+    if (!status) status = &dummy;
+    *status = LH_ERR_INVALID;
+    if (!ms || !out || (n_h && !h_names)) return nullptr;
+    try {
+        std::vector<std::string> hs(h_names, h_names + n_h);
+        auto *d = new RawDeviceSubscription(static_cast<MetricSystem *>(ms)->NewRawDeviceSubscription(hs));
+        *out = d->board();
+        *status = LH_OK;
+        return d;
+    } catch (const std::exception &e) {
+        *status = scope_status(e);
+        return nullptr;
+    }
+}
+// RawDeviceSubscription::Percentiles / Ranks on `stream`.
+LHMS_API int lhms_raw_subscription_percentiles(void *d, const double *d_ps, uint32_t m, int32_t *d_keys, double *d_vals,
+                                               uint64_t *d_publish, void *stream) {
+    if (!d) return LH_ERR_INVALID;
+    try {
+        static_cast<RawDeviceSubscription *>(d)->Percentiles(d_ps, m, d_keys, d_vals, d_publish, stream);
+        return LH_OK;
+    } catch (const std::exception &e) { return scope_status(e); }
+}
+LHMS_API int lhms_raw_subscription_ranks(void *d, const double *d_values, uint32_t m, uint64_t *d_ranks,
+                                         uint64_t *d_totals, uint64_t *d_publish, void *stream) {
+    if (!d) return LH_ERR_INVALID;
+    try {
+        static_cast<RawDeviceSubscription *>(d)->Ranks(d_values, m, d_ranks, d_totals, d_publish, stream);
+        return LH_OK;
+    } catch (const std::exception &e) { return scope_status(e); }
+}
+LHMS_API int lhms_raw_subscription_close(void *d) {
+    if (!d) return LH_ERR_INVALID;
+    try { static_cast<RawDeviceSubscription *>(d)->Close(); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
+}
+LHMS_API void lhms_raw_subscription_free(void *d) { delete static_cast<RawDeviceSubscription *>(d); }
 LHMS_API void lhms_start(void *ms) { static_cast<MetricSystem *>(ms)->Start(); }
 LHMS_API void lhms_stop(void *ms) { static_cast<MetricSystem *>(ms)->Stop(); }
 LHMS_API uint64_t lhms_dropped(void *ms) { return static_cast<MetricSystem *>(ms)->dropped_samples(); }

@@ -302,6 +302,47 @@ class DeviceSubscription {
     std::shared_ptr<State> st_;
 };
 
+// SubscribeToRawMetrics for consumers on the GPU (MetricSystem::NewRawDeviceSubscription).  Every collection publishes
+// the running bucket counts of the subscribed histograms into a raw board in device memory (lh_raw_board_create,
+// lh_snapshot_publish_raw), where kernels and CUDA-graph replays answer exact percentile, rank and bucket queries over
+// the latest collection with lh::raw_percentile / lh::raw_rank / lh::raw_bucket_count
+// (include/loghisto_b200_device.cuh), or Percentiles / Ranks below, with no host call.
+//
+//   loghisto::RawDeviceSubscription raw = ms.NewRawDeviceSubscription({"step_latency"});
+//   admit<<<1, 32, 0, stream>>>(raw.board(), /* row of "step_latency" */ 0, d_budget);   // share under budget, on the GPU
+//   raw.Close();   // once no query of the board is pending; also on destruction
+//
+// Row i is name histograms[i].  At a collection it holds that name's buckets of the collection's RawMetricSet when
+// the name is in Histograms, and is empty otherwise (percentiles INT32_MIN / NaN, ranks and totals 0).  A percentile
+// query with p equals what processMetrics reports for a label with that p, bit for bit.  A raw subscription reads; it
+// does not keep its names' ids alive.  Move-only.
+class RawDeviceSubscription {
+ public:
+    RawDeviceSubscription() = default;
+    RawDeviceSubscription(RawDeviceSubscription &&o) noexcept { *this = std::move(o); }
+    RawDeviceSubscription &operator=(RawDeviceSubscription &&o) noexcept;
+    RawDeviceSubscription(const RawDeviceSubscription &) = delete;
+    RawDeviceSubscription &operator=(const RawDeviceSubscription &) = delete;
+    ~RawDeviceSubscription();
+
+    const lh_raw_board &board() const;
+    // lh_raw_percentiles_grid / lh_raw_ranks_grid: one kernel on `stream` answers every row for each of the m device
+    // inputs (answers at [row * m + j]; Ranks' d_totals[row] is the total of query (row, 0)).  They may be captured
+    // into a CUDA graph.  Throws std::runtime_error when the library refuses the call or the subscription is closed.
+    void Percentiles(const double *d_ps, uint32_t m, int32_t *d_keys, double *d_vals, uint64_t *d_publish, void *stream);
+    void Ranks(const double *d_values, uint32_t m, uint64_t *d_ranks, uint64_t *d_totals, uint64_t *d_publish,
+               void *stream);
+    // Frees the board, after every publish issued (idempotent); no query of it may be pending.
+    void Close();
+    bool open() const { return st_ != nullptr; }
+
+    struct State;
+
+ private:
+    friend class MetricSystem;
+    std::shared_ptr<State> st_;
+};
+
 struct Options {
     int device = 0;
     uint32_t max_histograms = 1024;
@@ -350,6 +391,11 @@ class MetricSystem {
     // lh_board_create (e.g. more names than max_histograms / max_counters, or none).
     DeviceSubscription NewDeviceSubscription(const std::vector<std::string> &histograms,
                                              const std::vector<std::string> &counters);
+    // A raw device subscription to these histogram names (RawDeviceSubscription): every collection from now on, the
+    // reaper's included, publishes their bucket counts into it.  Call it outside any stream capture.  Throws
+    // std::runtime_error when the library refuses lh_raw_board_create (more names than max_histograms, or none) or
+    // has no raw device subscriptions.
+    RawDeviceSubscription NewRawDeviceSubscription(const std::vector<std::string> &histograms);
     void RegisterGaugeFunc(const std::string &name, std::function<double()> f);   // :299
     // A gauge whose value lives in device memory: a scalar of type `dtype` (LH_GAUGE_*) at d_value, device or managed
     // memory of this system's device, which must stay allocated while registered.  Every collection reads all device
@@ -439,6 +485,10 @@ class MetricSystem {
     std::vector<std::shared_ptr<DeviceSubscription::State>> subs_;   // open subscriptions
     lh_status publish_subscriptions(const RawMetricSet &raw, const std::unordered_map<std::string, uint32_t> &hid_of,
                                     const std::unordered_map<std::string, uint32_t> &cid_of);
+    // raw device subscriptions (NewRawDeviceSubscription), under sub_mu_ too
+    friend class RawDeviceSubscription;
+    std::vector<std::shared_ptr<RawDeviceSubscription::State>> raw_subs_;   // open raw subscriptions
+    lh_status publish_raw_subscriptions(const std::unordered_map<std::string, uint32_t> &hid_of);
 
     lh_ctx *ctx_ = nullptr;
     std::chrono::nanoseconds interval_;

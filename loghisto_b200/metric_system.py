@@ -11,7 +11,7 @@ import ctypes as C
 from . import _lib as _L
 from . import build as _build
 from .engine import (_batch_array, _capture_stream, _stream, _timer_stream, board_out, board_views, gauge_src,
-                     graph_counter_args, graph_duration_out, graph_keyed_args)
+                     graph_counter_args, graph_duration_out, graph_keyed_args, raw_percentiles, raw_ranks)
 
 _EMIT = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_char_p, C.c_int, C.c_uint64, C.c_double)
 _lib = None
@@ -106,6 +106,14 @@ def _bind(L):
     L.lhms_subscription_close.restype = C.c_int
     L.lhms_subscription_close.argtypes = [vp]
     L.lhms_subscription_free.argtypes = [vp]
+    L.lhms_raw_subscription_new.restype = vp
+    L.lhms_raw_subscription_new.argtypes = [vp, C.c_uint32, names, C.POINTER(_L.lh_raw_board), C.POINTER(C.c_int)]
+    for q in ("percentiles", "ranks"):
+        getattr(L, "lhms_raw_subscription_" + q).restype = C.c_int
+        getattr(L, "lhms_raw_subscription_" + q).argtypes = [vp, vp, C.c_uint32, vp, vp, vp, vp]
+    L.lhms_raw_subscription_close.restype = C.c_int
+    L.lhms_raw_subscription_close.argtypes = [vp]
+    L.lhms_raw_subscription_free.argtypes = [vp]
     for kind in ("processed", "raw"):
         getattr(L, "lhms_subscribe_" + kind).restype = vp
         getattr(L, "lhms_subscribe_" + kind).argtypes = [vp, C.c_int]
@@ -416,6 +424,76 @@ class DeviceSubscription:
             pass
 
 
+class RawDeviceSubscription:
+    """A raw device subscription of a MetricSystem (MetricSystem.raw_device_subscription): every collection publishes
+    the bucket counts of its histogram names into `board`, an lh_raw_board in device memory that kernels query with
+    lh::raw_percentile / lh::raw_rank / lh::raw_bucket_count (row numbers in `rows`), and percentiles() / ranks()
+    query from torch.  Usable as a context manager; close() (also on exit) frees the board once no query of it is
+    pending."""
+
+    def __init__(self, ms, histograms):
+        self._ms = ms
+        hnames = [str(x) for x in histograms]
+        self.board = _L.lh_raw_board()
+        hn = (C.c_char_p * max(len(hnames), 1))(*[x.encode() for x in hnames])
+        st = C.c_int()
+        self._h = ms._lib.lhms_raw_subscription_new(ms._h, len(hnames), hn, C.byref(self.board), C.byref(st))
+        if not self._h:
+            raise RuntimeError("lhms_raw_subscription_new failed (status %d)" % st.value)
+        self.rows = {nm: i for i, nm in enumerate(hnames)}
+        self._device = ms._device
+
+    def _call(self, fn, what):
+        if self._h is None:
+            raise RuntimeError("the raw device subscription is closed")
+
+        def call(*a):
+            st = fn(self._h, *a)
+            if st != 0:
+                raise RuntimeError("%s failed (status %d)" % (what, st))
+        return call
+
+    def percentiles(self, ps, stream=None):
+        """For every row and each p of `ps` (a float64 CUDA tensor of length m): keys int32 [k, m], values float64
+        [k, m] and publish numbers int64 [k, m], bit for bit what processMetrics reports for a label with that p
+        (INT32_MIN / NaN where it omits one).  One kernel on `stream` (None = torch's current stream, so that it is
+        captured inside torch.cuda.graph) and no synchronisation; a graph replay answers from the publish latest at
+        its run."""
+        call = self._call(self._ms._lib.lhms_raw_subscription_percentiles, "lhms_raw_subscription_percentiles")
+        return raw_percentiles(call, self.board.k, ps, self._device, stream)
+
+    def ranks(self, values, stream=None):
+        """For every row and each value of `values` (a float64 CUDA tensor of length m): ranks int64 [k, m] (samples
+        whose bucket is at or below the value's), totals int64 [k] (of the publish query (r, 0) read) and publish
+        numbers int64 [k, m].  One kernel, as percentiles()."""
+        call = self._call(self._ms._lib.lhms_raw_subscription_ranks, "lhms_raw_subscription_ranks")
+        return raw_ranks(call, self.board.k, values, self._device, stream)
+
+    def close(self):
+        """Frees the board after every publish issued.  No query of it may be pending.  Idempotent."""
+        if self._h is None:
+            return
+        h, self._h = self._h, None
+        st = 0
+        if self._ms._h:   # a closed MetricSystem already freed the board
+            st = self._ms._lib.lhms_raw_subscription_close(h)
+        self._ms._lib.lhms_raw_subscription_free(h)
+        if st != 0:
+            raise RuntimeError("lhms_raw_subscription_close failed (status %d)" % st)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *a):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class Subscription:
     def __init__(self, ms, kind, capacity):
         self._ms, self._kind = ms, kind
@@ -558,6 +636,13 @@ class MetricSystem:
         `with ms.device_subscription(histograms=[...], counters=[...]) as sub:` closes it on exit.  Create it outside
         any stream capture."""
         return DeviceSubscription(self, histograms, counters)
+
+    def raw_device_subscription(self, histograms=()) -> RawDeviceSubscription:
+        """SubscribeToRawMetrics for the GPU: every collection from now on (the reaper's included) publishes the bucket
+        counts of these histogram names into device memory, where kernels, captured graphs and torch callers ask exact
+        percentile and rank queries (RawDeviceSubscription).  `with ms.raw_device_subscription(histograms=[...]) as
+        raw:` closes it on exit.  Create it outside any stream capture."""
+        return RawDeviceSubscription(self, histograms)
 
     def RegisterConstantGauge(self, name: str, value: float):
         self._lib.lhms_register_constant_gauge(self._h, name.encode(), float(value))
