@@ -324,7 +324,7 @@ LH_API lh_status lh_graph_recorder_destroy(lh_ctx *ctx, const lh_graph_recorder 
  *                        open snapshot (LH_ERR_STATE without one, or outside a snapshot):
  *                          histogram row i, hist_ids[i] = h: count, sum, avg, pkeys[0..np), pvals[0..np) bit for bit
  *                            as that reduction reports h (the all-reduced values after lh_snapshot_allreduce), and
- *                            present = (count != 0);
+ *                            present = whether h holds a non-empty bucket (count != 0, or a count that wrapped);
  *                          hist_ids[i] = LH_GRAPH_UNBOUND (or hist_ids NULL): an untouched histogram as the reduction
  *                            reports one (count 0, sum 0, avg NaN, keys INT32_MIN, values NaN), present = 0;
  *                          counter row i, counter_ids[i] = c: rate = the interval delta lh_snapshot_export reports in
@@ -352,7 +352,7 @@ typedef struct lh_board_header {
 typedef struct lh_board_hist_row {
     uint64_t count;
     double sum, avg;
-    uint32_t present;                         /* count != 0 */
+    uint32_t present;                         /* a non-empty bucket (count != 0 unless the uint64 count wrapped) */
     uint32_t reserved;
     double pvals[LH_MAX_PERCENTILES];         /* NaN where pkeys is INT32_MIN, and beyond np */
     int32_t pkeys[LH_MAX_PERCENTILES];
@@ -394,8 +394,11 @@ LH_API lh_status lh_board_destroy(lh_ctx *ctx, const lh_board *b);
  *
  * Layout (bytes, from d_rows): k lh_raw_row_header, then from LH_RAW_CELLS_OFFSET(k) k rows of uint64[65536]: cell
  * key + 32768 of row i holds the number of samples of that publish whose int16 bucket key is <= key (ascending int16
- * key order, the order K3 and lh_snapshot_reduce rank in).  Only keys [key_lo, key_hi] of the header are written by a
- * publish: a key below key_lo reads as 0 and a key above key_hi as total.  An empty row has total 0 and key_lo > key_hi.
+ * key order, the order K3 and lh_snapshot_reduce rank in), mod 2^64 as Go's uint64 running count.  Only keys
+ * [key_lo, key_hi] of the header are written by a publish: a key below key_lo reads as 0 and a key above key_hi as
+ * total.  A row whose running count passed 2^64 (counts summing to 2^64 or more: the cells are not monotone and total
+ * may be 0) stores key_hi + LH_RAW_KEY_WRAPPED, so a stored key_hi above 32767 marks it; the device queries then apply
+ * the percentile rule to every written key.  An empty row has key_lo > key_hi (and total 0).
  * Each row has its own seqlock: `seq` is odd while a publish writes the row and advances by 2 per publish, so
  * seq / 2 is the publish number (0 before the first) and every query answer is of one publish.
  *
@@ -410,8 +413,9 @@ LH_API lh_status lh_board_destroy(lh_ctx *ctx, const lh_board *b);
  *                            snapshot, LH_ERR_RANGE for an id >= max_histograms other than LH_GRAPH_UNBOUND.  Enqueued on
  *                            the snapshot stream; it never waits and never allocates.
  *   lh_raw_percentiles       query i: (d_keys[i], d_vals[i]) = what lh_snapshot_reduce reports for row d_rows[i]'s
- *                            histogram with percentile d_ps[i], bit for bit (INT32_MIN / NaN for p > 1, NaN or an
- *                            empty row; the smallest non-empty key for p <= 0).
+ *                            histogram with percentile d_ps[i], bit for bit (INT32_MIN / NaN where no bucket satisfies
+ *                            the rule: p > 1 unless the row's running counts wrapped, NaN, an empty row; the smallest
+ *                            non-empty key for p <= 0).
  *   lh_raw_ranks             query i: d_ranks[i] = samples of row d_rows[i] whose key is <= compress(d_values[i]) (the
  *                            bucket lh::record gives the value; NaN and +-Inf have key 0), d_totals[i] = its total.
  *   lh_raw_percentiles_grid / lh_raw_ranks_grid
@@ -430,8 +434,10 @@ typedef struct lh_raw_row_header {
     uint64_t seq;                             /* seqlock word: odd while a publish writes the row, +2 per publish */
     uint64_t publishes;                       /* publishes so far (= seq / 2 when even) */
     uint64_t total;                           /* samples of the row in the latest publish */
-    int32_t key_lo, key_hi;                   /* the key range that publish wrote (key_lo > key_hi: empty row) */
+    int32_t key_lo, key_hi;                   /* the key range that publish wrote (key_lo > key_hi: empty row); key_hi
+                                               * + LH_RAW_KEY_WRAPPED when the running counts wrapped */
 } lh_raw_row_header;
+#define LH_RAW_KEY_WRAPPED 65536
 typedef struct lh_raw_board {                 /* pass by value to kernels */
     uint64_t handle;                          /* opaque */
     void *d_rows;                             /* device memory: k headers, then k rows of running counts */
@@ -557,10 +563,14 @@ LH_API lh_status lh_snapshot_begin(lh_ctx *ctx);
 LH_API lh_status lh_snapshot_device(lh_ctx *ctx, lh_device_view *out);
 
 /* Output arrays are caller-allocated host memory:
- *   counts[H]           exact uint64 totals (0 => histogram absent this interval)
- *   sums[H], avgs[H]    as the reference's float64 map values (avg NaN when count==0)
+ *   counts[H]           uint64 totals, mod 2^64 as Go's (0 when the histogram is absent this interval, and also when
+ *                       counts merged into it sum to a multiple of 2^64: presence is a non-empty bucket, which the
+ *                       export's offsets show)
+ *   sums[H], avgs[H]    as the reference's float64 map values (avg = sum / float64(count): NaN when absent, +-Inf or
+ *                       NaN for a wrapped count of 0)
  *   pkeys[H*np]         chosen bucket key per percentile, INT32_MIN where the
- *                       reference's percentile() returns its error (p>1, NaN)
+ *                       reference's percentile() returns its error (no bucket satisfies the rule: p>1 unless the
+ *                       running count wrapped, NaN, absent)
  *   pvals[H*np]         decompress(key); NaN where pkeys is INT32_MIN
  * Any output pointer may be NULL to skip it. */
 LH_API lh_status lh_snapshot_reduce(lh_ctx *ctx, const double *percentiles, uint32_t np,

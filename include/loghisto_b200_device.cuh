@@ -548,7 +548,8 @@ __device__ __forceinline__ bool end_read(const lh_board &b, unsigned long long s
 struct HistogramStats {          // one histogram row of the latest publish (lh_board_hist_row)
     uint64_t count;              // the name's _count (as uint64)
     double sum, avg;             // _sum, _avg
-    bool present;                // the name was in that collection's Histograms (count != 0)
+    bool present;                // the name was in that collection's Histograms: a non-empty bucket (count != 0 unless
+                                 // the uint64 count wrapped to 0)
     uint32_t np;                 // percentile labels of that collection
     double pvals[LH_MAX_PERCENTILES];    // value of label j, j < np; NaN where pkeys[j] is INT32_MIN (label omitted)
     int32_t pkeys[LH_MAX_PERCENTILES];   // bucket key of label j
@@ -616,8 +617,11 @@ __device__ __forceinline__ uint64_t read_counter(const lh_board &b, uint32_t row
 
 // Smallest s in [0, total] with float64(s)/float64(total) >= p -- the reference's rule (metrics.go:413) turned into an
 // integer threshold on the running count: the quotient is monotone in s, so "first non-empty bucket whose running count
-// satisfies the rule" == "first non-empty bucket whose running count reaches T".  Returns false when no s satisfies
-// the rule (p > 1 or NaN: percentile() returns its error).
+// satisfies the rule" == "first non-empty bucket whose running count reaches T".  Returns false when no s in
+// [0, total] satisfies the rule (p > 1 or NaN).  That settles percentile() only while the running counts are exact:
+// once Go's uint64 running count wraps (counts summing to 2^64 or more) it is not monotone, can exceed the wrapped
+// total (ratios above 1, so p > 1 may answer) and the total may be 0 (ratios +Inf, or NaN at 0), and callers apply the
+// rule to every non-empty bucket instead.
 __device__ __forceinline__ bool percentile_threshold(double p, unsigned long long total, unsigned long long *T) {
     const double ft = (double)total;
     if (!(__ddiv_rn(ft, ft) >= p)) return false;                 // even s = total fails (p > 1, NaN)
@@ -661,10 +665,14 @@ __device__ __forceinline__ bool end_read(const char *h, unsigned long long s) {
 struct Range {
     unsigned long long total;
     int lo, hi;                  // written keys; lo > hi: empty
+    bool wrapped;                // a running count passed 2^64 (key_hi was stored + LH_RAW_KEY_WRAPPED)
 };
 __device__ __forceinline__ Range range(const char *h) {
     const unsigned long long two = board::ld_relaxed(h + offsetof(lh_raw_row_header, key_lo));
-    return Range{board::ld_relaxed(h + offsetof(lh_raw_row_header, total)), (int)(uint32_t)two, (int)(uint32_t)(two >> 32)};
+    const int hi = (int)(uint32_t)(two >> 32);
+    const bool wrapped = hi > 32767;
+    return Range{board::ld_relaxed(h + offsetof(lh_raw_row_header, total)), (int)(uint32_t)two,
+                 wrapped ? hi - LH_RAW_KEY_WRAPPED : hi, wrapped};
 }
 // running count at key: 0 below the written range, total above it
 __device__ __forceinline__ unsigned long long running(const char *c, const Range &r, int key) {
@@ -675,7 +683,9 @@ __device__ __forceinline__ unsigned long long running(const char *c, const Range
 }  // namespace raw
 
 // (key, value) of percentile p of row `row`: bit for bit what lh_snapshot_reduce reports for the row's histogram with
-// that p.  INT32_MIN / NaN for p > 1, NaN or an empty row; p <= 0 gives the smallest non-empty key.
+// that p.  INT32_MIN / NaN where no bucket satisfies the rule (p > 1 unless the running counts wrapped, NaN, an empty
+// row); p <= 0 gives the smallest non-empty key.  A row whose running counts wrapped is answered by a linear scan of
+// its written keys.
 __device__ __forceinline__ uint64_t raw_percentile(const lh_raw_board &b, uint32_t row, double p, int32_t *key, double *val) {
     *key = (int32_t)0x80000000;
     *val = __longlong_as_double(0x7FF8000000000000ll);
@@ -687,7 +697,15 @@ __device__ __forceinline__ uint64_t raw_percentile(const lh_raw_board &b, uint32
         unsigned long long T;
         bool found = false;
         int lo = r.lo, hi = r.hi;
-        if (r.total && lo <= hi && percentile_threshold(p, r.total, &T)) {
+        if (r.wrapped) {                                          // Go's rule on each non-empty bucket, in key order
+            const double ft = (double)r.total;
+            unsigned long long prev = 0;
+            for (int k = lo; k <= hi; k++) {
+                const unsigned long long run = board::ld_relaxed(c + (size_t)(k + 32768) * 8u);
+                if (run != prev && __ddiv_rn((double)run, ft) >= p) { lo = k; found = true; break; }
+                prev = run;
+            }
+        } else if (r.total && lo <= hi && percentile_threshold(p, r.total, &T)) {
             if (T == 0) T = 1;                                    // p <= 0: the smallest non-empty bucket
             while (lo < hi) {                                     // running(hi) == total >= T
                 const int mid = lo + ((hi - lo) >> 1);

@@ -185,7 +185,8 @@ struct lh_ctx {
     uint32_t res_np[3] = {0, 0, 0};
     uint64_t res_ticket[2] = {0, 0};
     uint64_t next_ticket = 1;
-    uint32_t *d_nnz = nullptr, *d_offsets = nullptr;
+    uint32_t *d_nnz = nullptr, *d_offsets = nullptr;     // d_nnz: [3][H], the non-empty buckets K3 counted per result slot
+    int nnz_slot = 0;                                    // the slot whose counts k_scan_nnz reads (the latest K3)
     short *d_x_keys = nullptr; unsigned long long *d_x_counts = nullptr; size_t x_cap = 0;
     // pinned host mirrors
     uint32_t *h_offsets = nullptr;
@@ -1082,7 +1083,7 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
         LH_CREATE_CUDA(cudaMallocHost(&ctx->h_res[i], res_bytes));
         LH_CREATE_CUDA(cudaEventCreateWithFlags(&ctx->res_done[i], cudaEventDisableTiming));
     }
-    LH_CREATE_CUDA(cudaMalloc(&ctx->d_nnz, (size_t)ctx->H * 4));
+    LH_CREATE_CUDA(cudaMalloc(&ctx->d_nnz, (size_t)3 * ctx->H * 4));
     LH_CREATE_CUDA(cudaMalloc(&ctx->d_offsets, ((size_t)ctx->H + 1) * 4));
     LH_CREATE_CUDA(cudaMallocHost(&ctx->h_offsets, ((size_t)ctx->H + 1) * 4));
     LH_CREATE_CUDA(cudaMallocHost(&ctx->h_counter_deltas, counter_bytes));
@@ -1925,13 +1926,15 @@ lh_status enqueue_reduce(lh_ctx *ctx, const double *ps, uint32_t np, int slot) {
     const uint32_t smem_cells = k3_smem_cells(ctx->pc.win);
     k_reduce<<<ctx->H, K3_THREADS, (size_t)smem_cells * 8, s>>>(v.buckets, v.flags, ctx->pc.win, ctx->d_decomp, ctx->d_ps[slot], (int)np,
                                            (unsigned long long *)(d + l.count), (double *)(d + l.sum), (double *)(d + l.avg),
-                                           (int *)(d + l.pkeys), (double *)(d + l.pvals), ctx->d_nnz, smem_cells);
+                                           (int *)(d + l.pkeys), (double *)(d + l.pvals), ctx->d_nnz + (size_t)slot * ctx->H,
+                                           smem_cells);
     LH_CUDA(ctx, cudaGetLastError());
     LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_res[slot], d, l.total, cudaMemcpyDeviceToHost, s));
     LH_CUDA(ctx, cudaEventRecord(ctx->res_done[slot], s));
     ctx->stats.kernel_launches++;
     ctx->stats.d2h_bytes += l.total;
     ctx->nnz_valid = true;
+    ctx->nnz_slot = slot;
     ctx->res_np[slot] = np;
     return LH_OK;
 }
@@ -2010,7 +2013,7 @@ extern "C" lh_status lh_snapshot_export(lh_ctx *ctx, lh_sparse *out) {
         lh_status st = enqueue_reduce(ctx, nullptr, 0, 2);
         if (st != LH_OK) return st;
     }
-    k_scan_nnz<<<1, 1024, 0, s>>>(ctx->d_nnz, ctx->H, ctx->d_offsets);
+    k_scan_nnz<<<1, 1024, 0, s>>>(ctx->d_nnz + (size_t)ctx->nnz_slot * ctx->H, ctx->H, ctx->d_offsets);
     LH_CUDA(ctx, cudaGetLastError());
     LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_offsets, ctx->d_offsets, ((size_t)ctx->H + 1) * 4, cudaMemcpyDeviceToHost, s));
     LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_counter_deltas, v.counters, (size_t)ctx->C * 8, cudaMemcpyDeviceToHost, s));
@@ -2148,6 +2151,7 @@ extern "C" lh_status lh_snapshot_publish(lh_ctx *ctx, const lh_board *b, const u
     p.avg = (const double *)(d + l.avg);
     p.pvals = (const double *)(d + l.pvals);
     p.pkeys = (const int *)(d + l.pkeys);
+    p.nnz = ctx->d_nnz + (size_t)slot * ctx->H;
     p.ps = ctx->d_ps[slot];
     p.counters = snapshot_view(ctx).counters;
     p.np = np;

@@ -1094,17 +1094,32 @@ __device__ __forceinline__ void reduce_dense(uint32_t level, const unsigned long
     unsigned long long mine = 0;
     double msum = 0.0;
     unsigned int nnz = 0;
+    unsigned int high = 0;   // OR of the counts' high words: 64 counts below 2^58 cannot pass 2^64
     if (scans) {
 #pragma unroll 16
         for (int r = 0; r < K3_WARP_KEYS / 32; r++) {      // 16 independent 256-byte rows in flight per warp
             unsigned int slot = (unsigned int)(key0 + r * 32 + lane) & 0xFFFFu;
             unsigned long long c = hb[slot];
+            high |= (unsigned int)(c >> 32);
             if (c) { mine += c; msum += decomp[slot] * (double)c; nnz++; }
+        }
+    }
+    // an addition of the count reduction or scan passed 2^64 (the exact total is >= 2^64).  A lane with a count of
+    // 2^58 or more adds its cells again with a check per addition; the reduction and the scan below check each step.
+    int wrap = 0;
+    if (high >> 26) {
+        unsigned long long again = 0;
+        for (int r = 0; r < K3_WARP_KEYS / 32; r++) {
+            const unsigned long long c = hb[(unsigned int)(key0 + r * 32 + lane) & 0xFFFFu];
+            again += c;
+            wrap |= again < c;
         }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
-        mine += __shfl_xor_sync(0xFFFFFFFFu, mine, o);
+        const unsigned long long y = __shfl_xor_sync(0xFFFFFFFFu, mine, o);
+        mine += y;
+        wrap |= mine < y;
         msum += __shfl_xor_sync(0xFFFFFFFFu, msum, o);
         nnz += __shfl_xor_sync(0xFFFFFFFFu, nnz, o);
     }
@@ -1116,7 +1131,7 @@ __device__ __forceinline__ void reduce_dense(uint32_t level, const unsigned long
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
             unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, wi, o);
-            if (lane >= o) wi += y;
+            if (lane >= o) { wi += y; wrap |= wi < y; }
         }
         s_cnt[lane] = wi - w;
         if (lane == 31) s_total = wi;
@@ -1129,47 +1144,82 @@ __device__ __forceinline__ void reduce_dense(uint32_t level, const unsigned long
         }
         if (lane == 0) { s_sum[0] = ts; s_nnz[0] = tn; }
     }
-    __syncthreads();
+    const bool wrapped = __syncthreads_or(wrap);
     const unsigned long long total = s_total;
     const double ftotal = (double)total;
-    // owner of percentile j = first non-empty warp whose inclusive prefix satisfies the rule
-    if (lane == 0 && s_tot[warp]) {
-        const unsigned long long end_incl = s_cnt[warp] + s_tot[warp];
-        for (int j = 0; j < np; j++)
-            if (__ddiv_rn((double)end_incl, ftotal) >= ps[j]) atomicMin(&s_owner[j], warp);
-    }
-    __syncthreads();
-    unsigned int pending = 0;
-    for (int j = 0; j < np; j++) if (s_owner[j] == warp) pending |= 1u << j;
-    if (pending) {
-        unsigned long long sofar = s_cnt[warp];
-        for (int r = 0; r < K3_WARP_KEYS / 32 && pending; r++) {
-            int key = key0 + r * 32 + lane;
-            unsigned long long c = hb[(unsigned int)key & 0xFFFFu];
-            unsigned long long incl = c;
+    if (wrapped) {
+        // Go's uint64 running count wrapped: a crossing inside a warp need not survive to the warp's end, so every
+        // scanning warp applies the rule to each of its non-empty cells (running counts mod 2^64, as Go's) and the
+        // block keeps the smallest key per percentile.
+        if (scans) {
+            unsigned long long sofar = s_cnt[warp];
+            unsigned int pending = np == 32 ? 0xFFFFFFFFu : (1u << np) - 1u;
+            for (int r = 0; r < K3_WARP_KEYS / 32 && pending; r++) {
+                const int key = key0 + r * 32 + lane;
+                const unsigned long long c = hb[(unsigned int)key & 0xFFFFu];
+                unsigned long long incl = c;
 #pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-                if (lane >= o) incl += y;
-            }
-            const double frac = __ddiv_rn((double)(sofar + incl), ftotal);
-            for (int j = 0; j < np; j++) {
-                if (!(pending >> j & 1u)) continue;
-                unsigned int hit = __ballot_sync(0xFFFFFFFFu, c != 0 && frac >= ps[j]);
-                if (hit) {
-                    if (lane == __ffs(hit) - 1) {
-                        out_pkeys[(size_t)h * np + j] = key;
-                        out_pvals[(size_t)h * np + j] = decomp[(unsigned int)key & 0xFFFFu];
-                    }
-                    pending &= ~(1u << j);
+                for (int o = 1; o < 32; o <<= 1) {
+                    const unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+                    if (lane >= o) incl += y;
                 }
+                const double frac = __ddiv_rn((double)(sofar + incl), ftotal);
+                for (int j = 0; j < np; j++) {
+                    if (!(pending >> j & 1u)) continue;
+                    const unsigned int hit = __ballot_sync(0xFFFFFFFFu, c != 0 && frac >= ps[j]);
+                    if (hit) {
+                        if (lane == __ffs(hit) - 1) atomicMin(&s_owner[j], key);
+                        pending &= ~(1u << j);
+                    }
+                }
+                sofar += __shfl_sync(0xFFFFFFFFu, incl, 31);
             }
-            sofar += __shfl_sync(0xFFFFFFFFu, incl, 31);
+        }
+        __syncthreads();
+        if (t < np && s_owner[t] != 0x7FFFFFFF) {
+            out_pkeys[(size_t)h * np + t] = s_owner[t];
+            out_pvals[(size_t)h * np + t] = decomp[(unsigned int)s_owner[t] & 0xFFFFu];
+        }
+    } else {
+        // owner of percentile j = first non-empty warp whose inclusive prefix satisfies the rule
+        if (lane == 0 && s_tot[warp]) {
+            const unsigned long long end_incl = s_cnt[warp] + s_tot[warp];
+            for (int j = 0; j < np; j++)
+                if (__ddiv_rn((double)end_incl, ftotal) >= ps[j]) atomicMin(&s_owner[j], warp);
+        }
+        __syncthreads();
+        unsigned int pending = 0;
+        for (int j = 0; j < np; j++) if (s_owner[j] == warp) pending |= 1u << j;
+        if (pending) {
+            unsigned long long sofar = s_cnt[warp];
+            for (int r = 0; r < K3_WARP_KEYS / 32 && pending; r++) {
+                int key = key0 + r * 32 + lane;
+                unsigned long long c = hb[(unsigned int)key & 0xFFFFu];
+                unsigned long long incl = c;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+                    if (lane >= o) incl += y;
+                }
+                const double frac = __ddiv_rn((double)(sofar + incl), ftotal);
+                for (int j = 0; j < np; j++) {
+                    if (!(pending >> j & 1u)) continue;
+                    unsigned int hit = __ballot_sync(0xFFFFFFFFu, c != 0 && frac >= ps[j]);
+                    if (hit) {
+                        if (lane == __ffs(hit) - 1) {
+                            out_pkeys[(size_t)h * np + j] = key;
+                            out_pvals[(size_t)h * np + j] = decomp[(unsigned int)key & 0xFFFFu];
+                        }
+                        pending &= ~(1u << j);
+                    }
+                }
+                sofar += __shfl_sync(0xFFFFFFFFu, incl, 31);
+            }
         }
     }
     if (t == 0) {
         for (int j = 0; j < np; j++)
-            if (s_owner[j] == 0x7FFFFFFF) {   // percentile() error (p > 1, NaN, empty): key omitted by the caller
+            if (s_owner[j] == 0x7FFFFFFF) {   // percentile() error (no bucket satisfies the rule): key omitted by the caller
                 out_pkeys[(size_t)h * np + j] = (int)0x80000000;
                 out_pvals[(size_t)h * np + j] = __longlong_as_double(0x7FF8000000000000ll);
             }
@@ -1223,10 +1273,12 @@ k_reduce(const unsigned long long *__restrict__ buckets, const uint32_t *__restr
     unsigned long long mine = 0;
     double msum = 0.0;
     unsigned int nnz = 0;
+    unsigned int high = 0;                                        // OR of the counts' high words
     for (uint32_t i = t; i < n; i += K3_THREADS) {
         const unsigned int slot = (unsigned int)((int)i - (int)(win - 1u)) & 0xFFFFu;
         const unsigned long long c = hb[slot];
         k3_cells[i] = c;
+        high |= (unsigned int)(c >> 32);
         if (c) { mine += c; msum += decomp[slot] * (double)c; nnz++; }
     }
 #pragma unroll
@@ -1236,7 +1288,9 @@ k_reduce(const unsigned long long *__restrict__ buckets, const uint32_t *__restr
         nnz += __shfl_xor_sync(0xFFFFFFFFu, nnz, o);
     }
     if (lane == 0) { s_c[warp] = mine; s_s[warp] = msum; s_n[warp] = nnz; }
-    __syncthreads();
+    // at most 2^15 cells below 2^49 each cannot sum to 2^64: only a window holding a count of 2^49 or more checks its
+    // scan for a running count that passes 2^64
+    const int big = __syncthreads_or(high >> 17);
     if (warp == 0) {
         unsigned long long c = s_c[lane];
         double sm = s_s[lane];
@@ -1280,10 +1334,48 @@ k_reduce(const unsigned long long *__restrict__ buckets, const uint32_t *__restr
     }
     __syncthreads();
     unsigned long long run = s_c[warp] + incl - local;
-    for (uint32_t i = first; i < last; i++) { run += k3_cells[i]; k3_cells[i] = run; }
-    __syncthreads();
+    int wrap = 0;                                                 // a step of the running count passed 2^64
+    if (big) {
+        for (uint32_t i = first; i < last; i++) { const unsigned long long c = k3_cells[i]; run += c; k3_cells[i] = run; wrap |= run < c; }
+    } else {
+        for (uint32_t i = first; i < last; i++) { run += k3_cells[i]; k3_cells[i] = run; }
+    }
+    if (__syncthreads_or(wrap)) {
+        // Go's uint64 running count wrapped (the counts sum to 2^64 or more): it is no longer monotone and the total
+        // may be 0, so apply the rule literally.  Cell i is non-empty iff its running count differs from cell i-1's;
+        // percentile j is the first non-empty cell with float64(run) / float64(total) >= p (x / 0.0 = +Inf, 0 / 0.0 =
+        // NaN), the minimum over the threads' first hits in their own cells.
+        if (t < LH_MAX_PCT) s_c[t] = ~0ull;
+        __syncthreads();
+        const double ftotal = (double)s_total;
+        for (int j = 0; j < np; j++) {
+            const double p = ps[j];
+            unsigned int hit = 0xFFFFFFFFu;
+            unsigned long long prev = first && first < last ? k3_cells[first - 1] : 0ull;
+            for (uint32_t i = first; i < last; i++) {
+                const unsigned long long r = k3_cells[i];
+                if (r != prev && __ddiv_rn((double)r, ftotal) >= p) { hit = i; break; }
+                prev = r;
+            }
+            hit = __reduce_min_sync(0xFFFFFFFFu, hit);
+            if (lane == 0 && hit != 0xFFFFFFFFu) atomicMin(&s_c[j], (unsigned long long)hit);
+        }
+        __syncthreads();
+        if (t < np) {
+            int key = (int)0x80000000;
+            double val = __longlong_as_double(0x7FF8000000000000ll);
+            if (s_c[t] != ~0ull) {
+                key = (int)s_c[t] - (int)(win - 1u);
+                val = decomp[(unsigned int)key & 0xFFFFu];
+            }
+            out_pkeys[(size_t)h * np + t] = key;
+            out_pvals[(size_t)h * np + t] = val;
+        }
+        return;
+    }
     (void)PER;
-    // one thread per percentile: integer threshold, then the first cell whose running count reaches it
+    // one thread per percentile: integer threshold, then the first cell whose running count reaches it.  Without a
+    // wrap the running counts are exact and monotone, and a total of 0 means no non-empty cell.
     if (t < np) {
         const unsigned long long total = s_total;
         unsigned long long T;
@@ -1406,8 +1498,9 @@ k_scatter_segments(const uint32_t *__restrict__ offsets, uint32_t nb, uint32_t b
 
 // One CTA per segment of the batch, after K3 and before the clear.  Go's map keeps a key whose counts summed to 0
 // (metrics.go:342-347), the dense row does not, and two answers depend on it:
-//   * p <= 0 with total > 0: percentile() returns the first entry in value order whatever its count
-//     (float64(0)/float64(total) >= p), i.e. the smallest key present; K3 gives the smallest non-empty one;
+//   * p <= 0 with total > 0 (the uint64 total, which wraps at 2^64): percentile() returns the first entry in value
+//     order whatever its count (float64(0)/float64(total) >= p), i.e. the smallest key present; K3 gives the smallest
+//     non-empty one;
 //   * decompress(key) = +-Inf with count 0 (precision <= 46, the ends of the key range): Inf * 0 makes the sum and
 //     the average NaN; K3 skips empty cells.
 // out_* point at the batch's first result.
@@ -1439,7 +1532,10 @@ k_sparse_epilogue(const uint32_t *__restrict__ offsets, uint32_t base, const sho
         out_sum[s] = __longlong_as_double(0x7FF8000000000000ll);
         out_avg[s] = __longlong_as_double(0x7FF8000000000000ll);
     }
-    if (out_count[s] == 0ull) return;                 // every percentile is an error (0/0 is never >= p)
+    // total 0: the segment is empty (every percentile an error) or its counts wrapped to 0 (sums of 2^64, 2^65 ...).
+    // Then a key before the first non-empty one has running count 0 and ratio 0/0.0 = NaN, which fails every p, so
+    // p <= 0 picks the first non-empty key (ratio x/0.0 = +Inf): K3's answer stands either way.
+    if (out_count[s] == 0ull) return;
     for (int j = 0; j < np; j++)
         if (ps[j] <= 0.0) {                           // false for NaN
             out_pkeys[(size_t)s * np + j] = kmin;
@@ -1869,6 +1965,7 @@ struct BoardParams {
     uint32_t np, k;
     uint32_t n_staged, n;                    // entries in `table`, then in e[]
     BoardEntry e[BP_MAX_ENTRIES];
+    const uint32_t *nnz;                     // the reduction's non-empty bucket counts: presence (a count can wrap to 0)
 };
 
 __global__ void __launch_bounds__(BP_THREADS)
@@ -1912,7 +2009,7 @@ k_board_publish(const __grid_constant__ BoardParams p) {
             board::st_relaxed(r + offsetof(lh_board_hist_row, count), c);
             board::st_relaxed(r + offsetof(lh_board_hist_row, sum), (unsigned long long)__double_as_longlong(bound ? p.sum[e.id] : 0.0));
             board::st_relaxed(r + offsetof(lh_board_hist_row, avg), (unsigned long long)__double_as_longlong(bound ? p.avg[e.id] : qnan));
-            board::st_relaxed_u32(r + offsetof(lh_board_hist_row, present), c != 0ull);
+            board::st_relaxed_u32(r + offsetof(lh_board_hist_row, present), bound && p.nnz[e.id] != 0u);
         }
     }
     // counter rows: one thread each
@@ -2039,7 +2136,8 @@ k_gauge_read(const __grid_constant__ GaugeParams p) {
 //      are loaded in ascending key order in chunks of RP_CHUNK, block-scanned with the running total of the chunks
 //      before as carry (the window of precision 250 is 43 669 cells, more than shared memory holds at once), and
 //      written with strong relaxed stores to cell key + 32768 of the row;
-//   3. thread 0 writes total and the key range into the header, __threadfence, __syncthreads;
+//   3. thread 0 writes total and the key range into the header (key_hi + LH_RAW_KEY_WRAPPED when a running count
+//      passed 2^64, seen as a step whose sum is below its addend), __threadfence, __syncthreads;
 //   4. thread 0 writes the publish count and makes the word even with st.release.gpu.
 // Readers (include/loghisto_b200_device.cuh: lh::raw_percentile / raw_rank / raw_bucket_count, which k_raw_percentiles
 // and k_raw_ranks call) load the word with ld.acquire.gpu and retry while it is odd, load the header and the cells they
@@ -2095,6 +2193,7 @@ k_raw_publish(const __grid_constant__ RawPublishParams p) {
     __syncthreads();
     int lo = 0, hi = -1;                                          // empty
     unsigned long long carry = 0;
+    int wrap = 0;                                                 // a running count passed 2^64
     if (level) {
         lo = (level & 2u) ? -32768 : -(int)(p.win - 1u);
         hi = (level & 2u) ? 32767 : (int)(p.win - 1u);
@@ -2132,7 +2231,7 @@ k_raw_publish(const __grid_constant__ RawPublishParams p) {
             __syncthreads();
             unsigned long long run = carry + s_warp[warp] + incl - local;
 #pragma unroll
-            for (int j = 0; j < RP_PER; j++) { run += v[j]; s_cells[rp_slot(t * RP_PER + j)] = run; }
+            for (int j = 0; j < RP_PER; j++) { run += v[j]; wrap |= run < v[j]; s_cells[rp_slot(t * RP_PER + j)] = run; }
             __syncthreads();
 #pragma unroll
             for (int j = 0; j < RP_PER; j++) {
@@ -2143,6 +2242,7 @@ k_raw_publish(const __grid_constant__ RawPublishParams p) {
             __syncthreads();                                      // before the next chunk overwrites s_cells / s_warp
         }
     }
+    if (__syncthreads_or(wrap)) hi += LH_RAW_KEY_WRAPPED;          // readers fall back to Go's literal rule
     if (t == 0) {
         board::st_relaxed(h + offsetof(lh_raw_row_header, total), carry);
         board::st_relaxed(h + offsetof(lh_raw_row_header, key_lo),

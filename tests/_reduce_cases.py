@@ -51,27 +51,21 @@ def expected_flag(hist: dict, precision: int) -> int:
 class Reference:
     """processHistograms + percentile (metrics.go:336-356, 406-418) on one {int16 key: count} histogram, restated
     independently of the oracle's key-ordered loop: buckets sorted by decompressed value as metrics.go:409 sorts
-    (ties, which occur only at +-Inf for precisions <= 46, broken by key), running count and total as Python ints,
-    the rule float64(sofar) / float64(total) >= p in Python floats (correctly rounded int -> float, IEEE division),
-    and the sum of decompress(key) * count as an exact rational."""
+    (ties, which occur only at +-Inf for precisions <= 46, broken by key), running count and total as Go's uint64 (mod
+    2^64), the rule float64(sofar) / float64(total) >= p in Python floats (correctly rounded int -> float, IEEE
+    division: x / 0.0 is +Inf and 0 / 0.0 NaN when the total wraps to 0), and the sum of decompress(key) * count as an
+    exact rational."""
 
     def __init__(self, hist: dict, table: np.ndarray, name: str = ""):
         self.name = name
-        items = sorted(((float(table[k & 0xFFFF]), k, c) for k, c in hist.items() if c), key=lambda t: (t[0], t[1]))
-        self.order = [k for _, k, _ in items]
         self.table = table
-        self.count = sum(c for _, _, c in items)
-        self.nnz = len(items)
-        self.cums = []
-        ratios = []
-        sofar = 0
-        for _, _, c in items:
-            sofar += c
-            self.cums.append(sofar)
-            ratios.append(float(sofar) / float(self.count))
-        self.ratios = np.array(ratios, dtype=np.float64)
+        self.nnz = sum(1 for c in hist.values() if c)
+        self._rank([(k, c) for k, c in hist.items() if c])
         exact, mag, infs = 0, 0, set()
-        for v, _, c in items:
+        for k, c in hist.items():
+            v = float(table[k & 0xFFFF])
+            if not c:
+                continue
             if math.isinf(v):
                 infs.add(v)
                 continue
@@ -88,9 +82,23 @@ class Reference:
         self.keys = np.array([k for k, _ in by_key], dtype=np.int16)
         self.counts = np.array([c for _, c in by_key], dtype=np.uint64)
 
+    def _rank(self, entries):
+        """Value order, running counts and rule ratios of the (key, count) entries percentile() sorts."""
+        items = sorted(((float(self.table[k & 0xFFFF]), k, c) for k, c in entries), key=lambda t: (t[0], t[1]))
+        self.order = [k for _, k, _ in items]
+        self.count = sum(c for _, _, c in items) % 2 ** 64
+        self.cums = []
+        ratios = []
+        sofar = 0
+        for _, _, c in items:
+            sofar = (sofar + c) % 2 ** 64
+            self.cums.append(sofar)
+            ratios.append(go_div(float(sofar), self.count))
+        self.ratios = np.array(ratios, dtype=np.float64)
+
     def percentile(self, p: float):
         """Key of the first bucket (in value order) whose running count satisfies the rule; None where percentile()
-        returns its error (p > 1, NaN, empty histogram)."""
+        returns its error (no bucket satisfies it: p above every ratio, NaN, an empty histogram)."""
         hit = np.flatnonzero(self.ratios >= p)
         return self.order[hit[0]] if hit.size else None
 
@@ -103,6 +111,17 @@ class Reference:
 def reference(hist: dict, ps, table: np.ndarray) -> dict:
     """Keys (None = percentile() error), values, count, exact sum and sum of |terms| of `hist` for percentiles `ps`."""
     return Reference(hist, table).results(ps)
+
+
+def go_div(x: float, count: int) -> float:
+    """Go's x / float64(count) in IEEE arithmetic (metrics.go:356, 413): x / 0.0 is +-Inf, 0 / 0.0 and NaN / y NaN."""
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return float(np.float64(x) / np.float64(float(count)))
+
+
+def avg_of(s: float, ref: "Reference") -> float:
+    """The average processHistograms reports beside a float64 sum `s` of the histogram: s / float64(total)."""
+    return go_div(s, ref.count)
 
 
 def sum_ok(got: float, ref: Reference) -> bool:
@@ -240,6 +259,150 @@ def make_cases(precision: int, table: np.ndarray, seed: int) -> list:
     return cases
 
 
+def _split_wrapping(total: int, parts: int, floor: int, rng: random.Random) -> list:
+    """`parts` counts in [floor, 2^64 - 1] summing to `total` exactly."""
+    assert parts * floor <= total <= parts * (2 ** 64 - 1)
+    while True:
+        cuts = sorted(rng.randrange(total + 1) for _ in range(parts - 1))
+        sizes = [b - a for a, b in zip([0] + cuts, cuts + [total])]
+        if all(floor <= x < 2 ** 64 for x in sizes):
+            return sizes
+
+
+def _wrapping_run(wrapped: int, giants: int, run: int, start: int, rng: random.Random) -> dict:
+    """_giants_and_ones whose exact sum is 2^64 + `wrapped`: the running count wraps at one of the giant buckets, and
+    past 2^53 the count-1 runs barely move float64(sofar) / float64(total)."""
+    hist, k = {}, start
+    sizes = _split_wrapping(2 ** 64 + wrapped - run * (giants + 1), giants, 2, rng)
+    for g in range(giants + 1):
+        for _ in range(run):
+            hist[k] = 1
+            k += 1
+        if g < giants:
+            hist[k] = sizes[g]
+            k += 1
+    return hist
+
+
+WRAPPED_TOTALS = (0, 1, 2, 12345, 2 ** 53 - 1, 2 ** 53 + 1, 2 ** 60 + 2 ** 41 + 7)   # totals mod 2^64 every precision covers
+
+
+def make_wrapped_cases(precision: int, table: np.ndarray, seed: int) -> list:
+    """Histograms whose counts sum to 2^64 or more, so that Go's uint64 total and running counts (metrics.go:406-418)
+    wrap: the running count is no longer monotone in the bucket order and the total may be 0.  Cases as make_cases
+    gives them (name, hist, form, total = the exact sum) plus `wraps`, the number of times the running count passes
+    2^64.  Every window case has a dense form that holds the same running counts at the window keys: one count moves
+    from the last window bucket to the out-of-window key w, so that the total stays (the zero-sum case moves its two
+    buckets to -w and w instead).
+
+    The window shapes put a wrap where a search that assumes monotone running counts goes wrong: a "valley", where
+    the running count at key 0 (the window's middle cell, where a bisection over the window starts) is below the
+    threshold of some p in [0, 1] while an earlier bucket already satisfies the rule, and wraps at the end of warp
+    15 (keys -2048 .. -1 of the dense path's 2 048-key warps), inside it and inside one 32-key row, so that warp 15's
+    end-of-warp running count fails some p that a bucket inside it satisfies.  The runs of count-1 buckets lie in warp
+    15 too, so that the running count at its end is the total while earlier ones exceed it."""
+    rng = random.Random(seed * 1_000_003 + precision + 7)
+    w = window(precision)
+    K = w - 1
+    H = 2 ** 63
+    a, b = (K * 9) // 10, K // 2                      # every key below is inside the window for K >= 2009
+    base = [
+        # total 0: ratios x / 0.0 = +Inf (every p but NaN), 0 / 0.0 = NaN; the average is +-Inf, or NaN for a zero sum
+        ("wrap0_sum", {-7: H, 9: H}),
+        ("wrap0_zero_sum", {-b: H, b: H}),
+        ("valley", {-1800: H, -10: H, a: 5}),
+        ("wrap_at_last", {-1900: H, -1000: 2 ** 62, -2: H}),
+        ("two_wraps", {-1900: H + 1, -1000: H + 1, -5: H, -3: H, a: 5}),
+        ("wrap_at_warp_end", {-100: H, -1: H, 5: 3}),
+        ("wrap_in_warp", {-1500: H + 10, -700: H, -3: 1, 600: 4}),
+        ("wrap_in_row", {-37: H, -35: H, -33: 2, 900: 3}),
+    ]
+    for wrapped, giants, run in ((0, 2, 300), (1, 2, 300), (2, 2, 300), (12345, 3, 200), (2 ** 53 - 1, 2, 500),
+                                 (2 ** 53 + 1, 2, 500), (2 ** 60 + 2 ** 41 + 7, 3, 400)):
+        start = rng.randrange(-min(K, 2048), 1 - run * (giants + 1) - giants)      # inside warp 15 and the window
+        base.append(("wrap_total_%#x" % wrapped, _wrapping_run(wrapped, giants, run, start, rng)))
+
+    cases = []
+    for name, hist in base:
+        cases.append({"name": name, "hist": hist, "form": "window"})
+        d = dict(hist)
+        if name == "wrap0_zero_sum":                       # a zero sum in any summation order
+            d = {-w: H, w: H}
+        else:
+            last = max(d)
+            d[last] -= 1
+            if not d[last]:
+                del d[last]
+            d[w] = 1
+        cases.append({"name": name + "+%d" % w, "hist": d, "form": "dense"})
+    # the dense path's own shapes: a wrap inside a warp outside the window, and at precision 46
+    # +-Inf buckets (the ends of the key range) with a wrap between them
+    k0 = -32768 + 2048 * ((32768 - w) // 2048 - 1)                    # first key of a warp wholly below -w
+    cases.append({"name": "far_warp_wrap", "hist": {k0 + 100: H, k0 + 1000: H, -k0 - 100: 5}, "form": "outside"})
+    cases.append({"name": "inf_wrap", "hist": {-32768: 3, -5: H, -3: H, 32767: 2}, "form": "outside"})
+    cases.append({"name": "inf_wrap_to_0", "hist": {-32767: H, -32766: H}, "form": "outside"})
+    for c in cases:
+        c["total"] = sum(c["hist"].values())
+        c["wraps"] = c["total"] >> 64
+    return cases
+
+
+def wrapped_percentile_pool(cases: list, table: np.ndarray, seed: int) -> list:
+    """percentile_pool's sample, 1.5, and every crossing float64(s) / float64(total) of a bucket whose count is not 1,
+    with the doubles on either side; each value once."""
+    pool = percentile_pool(cases, table, seed) + [1.5]
+    for c in cases:
+        ref = Reference(c["hist"], table)
+        for k, q in zip(ref.order, ref.ratios):
+            if c["hist"][k] != 1:
+                pool += [math.nextafter(q, -math.inf), q, math.nextafter(q, math.inf)]
+    seen, out = set(), []
+    for p in pool:
+        b = np.float64(p).view(np.uint64)
+        if b not in seen:
+            seen.add(b)
+            out.append(p)
+    return out
+
+
+def monotone_search(ref: Reference, p: float, w: int):
+    """What a search that assumes monotone running counts answers for a window histogram: the integer threshold of
+    the rule on the wrapped total (None when float64(total) / float64(total) fails p, or the total is 0), then a
+    bisection of the 2w-1 window cells for the first running count at or above it."""
+    T = threshold(ref.count, p)
+    if T is None:
+        return None
+    T = max(T, 1)
+    run, cells = 0, []
+    at = dict(zip(ref.order, ref.cums))
+    for k in range(-(w - 1), w):
+        run = at.get(k, run)
+        cells.append(run)
+    lo, hi = 0, len(cells) - 1
+    while lo < hi:
+        mid = (lo + hi) // 2
+        if cells[mid] >= T:
+            hi = mid
+        else:
+            lo = mid + 1
+    return lo - (w - 1)
+
+
+def end_of_warp_owner(ref: Reference, p: float):
+    """What the dense path answers when percentile p's owner is the first 2048-key warp with a non-zero total whose
+    running count at its end satisfies the rule: the first non-empty bucket of that warp that satisfies it."""
+    warps = {}
+    for k, s in zip(ref.order, ref.cums):
+        warps.setdefault((k + 32768) // 2048, []).append((k, s))
+    prev = 0
+    for wi in sorted(warps):
+        end = warps[wi][-1][1]
+        if (end - prev) % 2 ** 64 and go_div(float(end), ref.count) >= p:
+            return next((k for k, s in warps[wi] if go_div(float(s), ref.count) >= p), None)
+        prev = end
+    return None
+
+
 def percentile_pool(cases: list, table: np.ndarray, seed: int) -> list:
     """SPECIAL_PS, then for a sample of crossings s of each case (the first bucket, the middle of the count-1 run after
     the largest bucket, one at random): q = float(s) / float(total) and the doubles on either side of it."""
@@ -256,7 +419,7 @@ def percentile_pool(cases: list, table: np.ndarray, seed: int) -> list:
         while end < n and counts[end] == 1:
             end += 1
         for i in sorted({0, min(n - 1, top + 1 + (end - top - 1) // 2), rng.randrange(n)}):
-            q = float(ref.cums[i]) / float(ref.count)
+            q = float(ref.ratios[i])
             pool += [math.nextafter(q, -math.inf), q, math.nextafter(q, math.inf)]
     return pool
 

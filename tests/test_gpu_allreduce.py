@@ -171,7 +171,8 @@ def split_hist(hist: dict, layout: str, world: int, precision: int, rng: random.
     """[(key, count)] per rank for one histogram.  "one": every triple on one rank.  "mixed": out-of-window keys on one
     rank, window keys on a second (both on two ranks, alternating, when there are only window keys), the others
     untouched.  "all": every key on every rank, the count cut at random points, so that parts of 0 occur and the
-    parts sum to the count exactly."""
+    parts sum to the count exactly.  "spread": every key on every rank with a world-th of its count (the remainder on
+    random ranks), so that a histogram whose counts sum to 2^64 or more reaches each rank as a share below 2^64."""
     w = rc.window(precision)
     pick = rng.sample(range(world), 2)
     parts = [[] for _ in range(world)]
@@ -182,6 +183,13 @@ def split_hist(hist: dict, layout: str, world: int, precision: int, rng: random.
         for i, (k, c) in enumerate(sorted(hist.items())):
             inside = -w < k < w
             parts[pick[i % 2] if window_only else pick[1 if inside else 0]].append((k, c))
+    elif layout == "spread":
+        for k, c in hist.items():
+            amounts = [c // world] * world
+            for r in rng.sample(range(world), c % world):
+                amounts[r] += 1
+            for r in range(world):
+                parts[r].append((k, amounts[r]))
     else:
         for k, c in hist.items():
             cuts = sorted(rng.randrange(c + 1) for _ in range(world - 1))
@@ -234,7 +242,7 @@ class Expect:
         self.counts = np.array([r.count for r in refs], np.uint64)
         self.pkeys = np.full((H, n), rc.INT32_MIN, np.int32)
         self.pvals = np.full((H, n), math.nan)
-        self.live = [h for h, r in enumerate(refs) if r.count]
+        self.live = [h for h, r in enumerate(refs) if r.nnz]        # a count that wrapped to 0 is live
         for h in self.live:
             res = refs[h].results(ps)
             self.pkeys[h] = [rc.INT32_MIN if k is None else k for k in res["keys"]]
@@ -249,12 +257,12 @@ class Expect:
         bad = np.flatnonzero((red.pkeys != self.pkeys).any(axis=1))
         assert bad.size == 0, (what, [(int(h), self.refs[h].name) for h in bad[:5]])
         assert rc.same_bits(red.pvals, self.pvals).all(), (what, np.flatnonzero(~rc.same_bits(red.pvals, self.pvals).all(axis=1))[:5])
-        dead = np.flatnonzero(self.counts == 0)
+        dead = [h for h, r in enumerate(self.refs) if not r.nnz]
         assert (red.sums[dead] == 0).all() and np.isnan(red.avgs[dead]).all(), what
         for h in self.live:
             s = float(red.sums[h])
             assert rc.sum_ok(s, self.refs[h]), (what, h, self.refs[h].name, s, float(self.refs[h].sum))
-            assert rc.same_bits(red.avgs[h], s / float(self.refs[h].count)), (what, h, self.refs[h].name)
+            assert rc.same_bits(red.avgs[h], rc.avg_of(s, self.refs[h])), (what, h, self.refs[h].name)
         if sp is not None:
             assert (sp.offsets.astype(np.int64) == self.offsets).all(), what
             assert (sp.keys == self.keys).all() and (sp.counts == self.xcounts).all(), what
@@ -276,13 +284,21 @@ _CASES = {}
 
 
 def cases_for(oracle, precision):
-    """(table, cases, {case index: Reference}, percentile batches), built once per precision."""
+    """(table, cases, {case index: Reference}, percentile batches, number of make_cases cases, batches of the wrapped
+    cases), built once per precision.  The cases of make_wrapped_cases (precisions of tests/_reduce_cases.py) follow
+    those of make_cases."""
     if precision not in _CASES:
         table = oracle.decompress_table(precision)
         cases = rc.make_cases(precision, table, SEED)
-        refs = [rc.Reference(c["hist"], table, c["name"]) for c in cases]
         batches = rc.percentile_batches(rc.percentile_pool(cases, table, SEED))
-        _CASES[precision] = (table, cases, refs, batches)
+        n_plain = len(cases)
+        wbatches = []
+        if precision in rc.PRECISIONS:
+            wrapped = rc.make_wrapped_cases(precision, table, SEED)
+            cases = cases + wrapped
+            wbatches = rc.percentile_batches(rc.wrapped_percentile_pool(wrapped, table, SEED))
+        refs = [rc.Reference(c["hist"], table, c["name"]) for c in cases]
+        _CASES[precision] = (table, cases, refs, batches, n_plain, wbatches)
     return _CASES[precision]
 
 
@@ -293,19 +309,25 @@ def cases_for(oracle, precision):
 def test_allreduce_constructed_cases(lh, oracle, ndev, spin, precision, form, world):
     """Every constructed case of the precision, packed into intervals of H - 1 histograms at random ids (at least one
     id untouched), each split over the ranks by a layout that rotates over the cases; one rank held back per
-    interval; counters included in every other interval; then an empty interval."""
+    interval; counters included in every other interval; then an empty interval.  Then the cases whose counts sum to
+    2^64 or more, each spread so that every rank's share stays below 2^64 (those that need more ranks are left out)."""
     if world == "all":
         world = min(8, ndev)
         if world <= 4:
             pytest.skip("needs more than 4 GPUs")
     H = form_H(precision, form)
-    table, cases, case_refs, batches = cases_for(oracle, precision)
+    table, cases, case_refs, batches, n_plain, wbatches = cases_for(oracle, precision)
     empty = rc.Reference({}, table, "untouched")
     rng = random.Random(SEED ^ (precision * 1009 + world * 7 + H))
     per = H - 1
-    order = list(range(len(cases)))
+    order = list(range(n_plain))
     rng.shuffle(order)
-    intervals = [order[i:i + per] for i in range(0, len(order), per)] + [[]]
+    intervals = [order[i:i + per] for i in range(0, len(order), per)]
+    wrapped = [ci for ci in range(n_plain, len(cases)) if cases[ci]["total"] // world + len(cases[ci]["hist"]) < 2 ** 64]
+    assert not wbatches or len(wrapped) >= len(cases) - n_plain - 2         # only two_wraps (both forms) needs three ranks
+    rng.shuffle(wrapped)
+    n_wrapped_intervals = -(-len(wrapped) // per)
+    intervals += [wrapped[i:i + per] for i in range(0, len(wrapped), per)] + [[]]
     with contexts(lh, ndev, world, H, NC, precision) as (engs, ref):
         for i, chosen in enumerate(intervals):
             ids = rng.sample(range(H), len(chosen))
@@ -317,14 +339,22 @@ def test_allreduce_constructed_cases(lh, oracle, ndev, spin, precision, form, wo
                 refs[h] = case_refs[ci]
                 hists[h] = cases[ci]["hist"]
                 flags[h] = rc.expected_flag(cases[ci]["hist"], precision)
-                layout = ("one", "mixed", "all")[(ci + i) % 3]
-                for r, share in enumerate(split_hist(cases[ci]["hist"], layout, world, precision, rng)):
+                wraps = cases[ci]["total"] >= 2 ** 64
+                layout = "spread" if wraps else ("one", "mixed", "all")[(ci + i) % 3]
+                split = split_hist(cases[ci]["hist"], layout, world, precision, rng)
+                if wraps:
+                    assert all(sum(c for _, c in share) < 2 ** 64 for share in split), (cases[ci]["name"], world)
+                for r, share in enumerate(split):
                     parts[r] += [(h, k, c) for k, c in share]
             shares = [triples(p) for p in parts]
             counters = counter_shares(world, SEED + i)
             with_counters = i % 2 == 0
             skewed = i % world
-            ps = batches[i % len(batches)]
+            first_wrapped = len(intervals) - 1 - n_wrapped_intervals
+            if first_wrapped <= i < len(intervals) - 1:
+                ps = wbatches[(i - first_wrapped) % len(wbatches)]
+            else:
+                ps = batches[i % len(batches)]
             what = (precision, form, world, i)
 
             for r, e in enumerate(engs):

@@ -94,11 +94,13 @@ def kernel_bucket_counts(torch, client, board, rows, keys):
 
 
 def reference_keys(ref, ps):
-    """Reference.percentile for every p at once: the first bucket in the reference's order whose ratio reaches p."""
+    """Reference.percentile for every p at once: the first bucket in the reference's order whose ratio reaches p (the
+    ratios are not monotone once the running count wraps at 2^64, and 0/0.0 is NaN, which reaches nothing)."""
     ps = np.asarray(ps, dtype=np.float64)
     if not ref.nnz:
         return np.full(ps.size, INT32_MIN, np.int32)
-    i = np.searchsorted(ref.ratios, ps, side="left")
+    best = np.fmax.accumulate(np.where(np.isnan(ref.ratios), -np.inf, ref.ratios))   # the largest ratio so far
+    i = np.searchsorted(best, ps, side="left")
     order = np.array(ref.order + [INT32_MIN], dtype=np.int64)
     i[np.isnan(ps)] = ref.nnz
     return order[np.minimum(i, ref.nnz)].astype(np.int32)
@@ -131,15 +133,23 @@ def test_exact_on_constructed_histograms(lh, oracle, torch, client, precision):
     """Every case of tests/_reduce_cases.py in its own row: percentiles for the special ps, the crossings and one ulp
     beside them and 10^4 random ps equal lh_snapshot_reduce (batches of 32) and the reference bit for bit, from the grid
     call, the pair call and a kernel; every key's bucket count equals the export; ranks equal the export's running
-    sums.  The last row is unbound and row k answers as empty, with publish number 0."""
-    H = 64
+    sums.  The last row is unbound and row k answers as empty, with publish number 0.  The cases of make_cases, then
+    those whose counts wrap at 2^64 (running counts mod 2^64, as np.cumsum of uint64 gives them)."""
     table = oracle.decompress_table(precision)
-    cases = rc.make_cases(precision, table, SEED)
+    plain = rc.make_cases(precision, table, SEED)
+    wrapped = rc.make_wrapped_cases(precision, table, SEED)
+    for cases, pool in ((plain, rc.percentile_pool(plain, table, SEED)),
+                        (wrapped, rc.wrapped_percentile_pool(wrapped, table, SEED))):
+        exact_on_cases(lh, oracle, torch, client, table, precision, cases, pool)
+
+
+def exact_on_cases(lh, oracle, torch, client, table, precision, cases, pool):
+    H = 64
     assert len(cases) < H
     refs = [rc.Reference(c["hist"], table, c["name"]) for c in cases] + [rc.Reference({}, table, "untouched")] * (H - len(cases))
     refs[H - 1] = rc.Reference({}, table, "unbound")
     rng = np.random.default_rng(SEED + precision)
-    ps = np.array(rc.percentile_pool(cases, table, SEED) + list(rng.random(10_000) * 1.1 - 0.05), dtype=np.float64)
+    ps = np.array(pool + list(rng.random(10_000) * 1.1 - 0.05), dtype=np.float64)
     ids, keys, counts = rc.merge_triples(cases)
     hid = list(range(H - 1)) + [UNBOUND]
     with lh.Engine(device=0, max_histograms=H, max_counters=1, precision=precision) as eng, eng.raw_board(H) as rb:

@@ -25,6 +25,11 @@ def lh():
     return loghisto_b200
 
 
+@pytest.fixture(scope="module")
+def torch():
+    return pytest.importorskip("torch")
+
+
 def frozen_flags(eng) -> np.ndarray:
     """Per-histogram flags of the open snapshot's frozen buffer."""
     v = eng.snapshot_device()
@@ -44,7 +49,7 @@ def check_reduced(red, refs, ps, table, what):
         assert rc.same_bits(red.pvals[h], want["values"]).all(), tag
         s = float(red.sums[h])
         assert rc.sum_ok(s, ref), (tag, s, float(ref.sum), float(ref.abs_sum))
-        assert rc.same_bits(red.avgs[h], s / float(ref.count) if ref.count else math.nan), (tag, red.avgs[h], s)
+        assert rc.same_bits(red.avgs[h], rc.avg_of(s, ref)), (tag, red.avgs[h], s)
 
 
 def check_export(sp, refs, what):
@@ -55,17 +60,29 @@ def check_export(sp, refs, what):
         assert (sp.keys[a:b] == ref.keys).all() and (sp.counts[a:b] == ref.counts).all(), (what, h, ref.name)
 
 
+def case_sets(precision, table):
+    """(kind, cases, percentile pool): the constructed cases of make_cases, then those whose counts wrap at 2^64."""
+    cases = rc.make_cases(precision, table, SEED)
+    wrapped = rc.make_wrapped_cases(precision, table, SEED)
+    return [("plain", cases, rc.percentile_pool(cases, table, SEED)),
+            ("wrapped", wrapped, rc.wrapped_percentile_pool(wrapped, table, SEED))]
+
+
 @pytest.mark.parametrize("precision", rc.PRECISIONS)
 def test_reduce_and_export_constructed_cases(lh, oracle, precision):
     """Every case in its own histogram id, merged again before each reduction (a snapshot clears): every p batch
     against every case, one reduction through lh_snapshot_reduce_async, one with the export first, one with no
     percentiles.  Merging the same counts into the two halves of the double buffer in turn also checks that each
-    snapshot cleared what it froze."""
+    snapshot cleared what it froze.  The cases of make_cases, then the wrapped ones, in an engine each."""
     table = oracle.decompress_table(precision)
-    cases = rc.make_cases(precision, table, SEED)
+    for kind, cases, pool in case_sets(precision, table):
+        reduce_and_export(lh, table, precision, cases, pool, kind)
+
+
+def reduce_and_export(lh, table, precision, cases, pool, kind):
     refs = [rc.Reference(c["hist"], table, c["name"]) for c in cases]
     refs += [rc.Reference({}, table, "untouched")] * (H - len(cases))
-    batches = rc.percentile_batches(rc.percentile_pool(cases, table, SEED))
+    batches = rc.percentile_batches(pool)
     ids, keys, counts = rc.merge_triples(cases)
     flags = np.array([rc.expected_flag(c["hist"], precision) for c in cases] + [0] * (H - len(cases)), np.uint32)
     with lh.Engine(device=0, max_histograms=H, max_counters=1, precision=precision) as eng:
@@ -87,8 +104,8 @@ def test_reduce_and_export_constructed_cases(lh, oracle, precision):
                     sp = eng.snapshot_export()
             finally:
                 eng.snapshot_end()
-            check_reduced(red, refs, ps, table, (precision, r))
-            check_export(sp, refs, (precision, r))
+            check_reduced(red, refs, ps, table, (precision, kind, r))
+            check_export(sp, refs, (precision, kind, r))
         for _ in range(2):                    # both halves of the double buffer are empty again
             red, sp = eng.snapshot(rc.SPECIAL_PS)
             empty = [rc.Reference({}, table, "empty")] * H
@@ -130,3 +147,33 @@ def test_intervals_after_out_of_window_counts(lh, oracle, precision):
             refs = [rc.Reference(hists.get(h, {}), table, "interval %d" % i) for h in range(4)]
             check_reduced(red, refs, ps, table, (precision, i))
             check_export(sp, refs, (precision, i))
+
+
+@pytest.mark.parametrize("precision", [100, 250])
+def test_board_rows_of_wrapped_histograms(lh, oracle, torch, precision):
+    """lh_snapshot_publish of wrapped histograms: each row is present, including those whose count wrapped to 0, and
+    holds the reduction's count, sum, average and percentiles; an untouched id and an unbound row are absent."""
+    table = oracle.decompress_table(precision)
+    cases = rc.make_wrapped_cases(precision, table, SEED)
+    ps = [0.0, 0.5, 1.0, 1.5, math.inf, math.nan]
+    refs = [rc.Reference(c["hist"], table, c["name"]) for c in cases]
+    k = len(cases) + 2
+    hid = np.array(list(range(len(cases))) + [len(cases), 0xFFFFFFFF], np.uint32)    # an untouched id, an unbound row
+    with lh.Engine(device=0, max_histograms=H, max_counters=1, precision=precision) as eng, eng.board(k, 0) as b:
+        eng.merge_counts_host(*rc.merge_triples(cases))
+        eng.snapshot_begin()
+        try:
+            red = eng.snapshot_reduce(ps)
+            b.publish(hid)
+        finally:
+            eng.snapshot_end()
+        check_reduced(red, refs + [rc.Reference({}, table, "untouched")] * (H - len(cases)), ps, table, precision)
+        v = {name: a.cpu().numpy() for name, a in b.read().items()}
+    n = len(cases)
+    assert (v["present"][:n] == 1).all() and (v["present"][n:] == 0).all()
+    assert any(r.count == 0 for r in refs)
+    assert (v["count"].view(np.uint64)[:n] == red.counts[:n]).all() and (v["count"][n:] == 0).all()
+    assert (v["sum"][:n].view(np.uint64) == red.sums[:n].view(np.uint64)).all()
+    assert (v["avg"][:n].view(np.uint64) == red.avgs[:n].view(np.uint64)).all()
+    assert (v["pkeys"][:n, :len(ps)] == red.pkeys[:n]).all()
+    assert (v["pvals"][:n, :len(ps)].view(np.uint64) == red.pvals[:n].view(np.uint64)).all()

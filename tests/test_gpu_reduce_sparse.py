@@ -75,12 +75,29 @@ def csr(hists: list, rng: random.Random):
     return np.array(offsets, np.uint32), np.array(keys, np.int16), np.array(counts, np.uint64)
 
 
+def wrapped_zero_count_cases(precision: int) -> list:
+    """Wrapped maps with zero-count keys: with a total of 0 a key before the first non-empty one has ratio 0/0.0 = NaN,
+    so p <= 0 answers the first non-empty key; with a wrapped total above 0 it answers the smallest key present."""
+    w, H = rc.window(precision), 2 ** 63
+    return [
+        ("wrap0_zero_keys", {-9: 0, -7: H, 9: H, 20: 0}),
+        ("wrap0_zero_keys_outside", {-w - 3: 0, -7: H, 5: 0, 9: H}),
+        ("wrap5_zero_keys", {-9: 0, -7: H, -3: H, 9: 5}),
+    ]
+
+
 @pytest.mark.parametrize("precision", rc.PRECISIONS)
 def test_constructed_cases_as_split_shuffled_segments(lh, oracle, precision):
     table = oracle.decompress_table(precision)
     cases = [(c["name"], c["hist"]) for c in rc.make_cases(precision, table, SEED)] + zero_count_cases(precision)
+    wrapped = [(c["name"], c["hist"]) for c in rc.make_wrapped_cases(precision, table, SEED)]
+    wrapped += wrapped_zero_count_cases(precision)
+    pool = rc.percentile_pool([{"hist": h} for _, h in cases], table, SEED)
+    pool += rc.wrapped_percentile_pool([{"hist": h} for _, h in wrapped if all(h.values())], table, SEED)
+    cases += wrapped
     refs = [GoMapReference(h, table, name) for name, h in cases]
-    batches = rc.percentile_batches(rc.percentile_pool([{"hist": h} for _, h in cases], table, SEED))
+    assert refs[-3].percentile(0.0) == -7 and refs[-1].percentile(0.0) == -9
+    batches = rc.percentile_batches(pool)
     rng = random.Random(SEED + precision)
     with lh.Engine(device=0, max_histograms=1, max_counters=1, precision=precision) as eng:
         for r, ps in enumerate(batches):
@@ -255,3 +272,28 @@ def test_mirror_empty_map(MS):
 
 def test_mirror_collected_set_fed_back(MS):
     pmc.check_collected_set_fed_back(MS)
+
+
+def test_mirror_wrapped_count(MS, oracle):
+    """processMetrics of a hand-built set whose counts sum past 2^64: _count is the uint64 total (wrapped), _avg is
+    sum / float64(count), a percentile above 1 is emitted where Go's ratio reaches it, and the aggregate count store
+    adds the wrapped count."""
+    table = oracle.decompress_table(100)
+    hist = {-1800: 2 ** 63, -10: 2 ** 63, 3000: 5}
+    ms = MS()
+    ms.SpecifyPercentiles({"%s_p50": 0.5, "%s_p150": 1.5, "%s_pbig": 1e18})
+    ref = GoMapReference(hist, table)
+    assert ref.count == 5 and ref.percentile(1.5) == -1800 and ref.percentile(1e18) == -1800
+    m = ms.processMetrics({"Histograms": {"lat": hist}}, aggregates=True)
+    assert m["lat_count"] == 5.0
+    assert rc.sum_ok(m["lat_sum"], ref) and rc.same_bits(m["lat_avg"], rc.avg_of(m["lat_sum"], ref))
+    for label in ("p50", "p150", "pbig"):
+        assert m["lat_" + label] == float(table[-1800 & 0xFFFF]), label
+    assert m["lat_agg_count"] == 5.0
+    # a total of 0: no _agg_ metrics (the store holds 0), every percentile but NaN answers the first bucket
+    m = ms.processMetrics({"Histograms": {"zero": {-7: 2 ** 63, 9: 2 ** 63}}}, aggregates=True)
+    assert m["zero_count"] == 0.0 and math.isinf(m["zero_avg"])
+    assert m["zero_p50"] == m["zero_p150"] == float(table[-7 & 0xFFFF])
+    assert "zero_agg_count" not in m
+    m = ms.processMetrics({"Histograms": {"lat": hist}}, aggregates=True)
+    assert m["lat_agg_count"] == 10.0

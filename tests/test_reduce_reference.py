@@ -2,6 +2,7 @@
 of its case generator.  Runs without a GPU: both restatements must agree before either judges the engine
 (tests/test_gpu_reduce.py)."""
 import math
+from fractions import Fraction
 
 import numpy as np
 import pytest
@@ -19,8 +20,15 @@ def generated(request, oracle):
     return p, table, cases, rc.percentile_pool(cases, table, SEED)
 
 
-def test_reference_matches_oracle(generated, oracle):
-    precision, table, cases, ps = generated
+@pytest.fixture(scope="module", params=rc.PRECISIONS)
+def wrapped(request, oracle):
+    p = request.param
+    table = oracle.decompress_table(p)
+    cases = rc.make_wrapped_cases(p, table, SEED)
+    return p, table, cases, rc.wrapped_percentile_pool(cases, table, SEED)
+
+
+def check_against_oracle(precision, table, cases, ps, oracle):
     for c in cases:
         ref = rc.Reference(c["hist"], table)
         got = oracle.process_histogram(rc.dense(c["hist"]), ps, precision)
@@ -29,10 +37,14 @@ def test_reference_matches_oracle(generated, oracle):
         bad = np.flatnonzero(got["pkeys"] != keys)
         assert bad.size == 0, (c["name"], [(ps[j], got["pkeys"][j], keys[j]) for j in bad[:5]])
         assert rc.same_bits(got["pvals"], want["values"]).all(), c["name"]
-        assert got["total"] == ref.count == c["total"]
+        assert got["total"] == ref.count == c["total"] % 2 ** 64
         # the oracle's sequential sum obeys the bound the engine is held to, and avg = sum / float64(count)
         assert rc.sum_ok(got["sum"], ref), (c["name"], got["sum"], float(ref.sum))
-        assert rc.same_bits(got["avg"], got["sum"] / float(ref.count) if ref.count else math.nan), c["name"]
+        assert rc.same_bits(got["avg"], rc.avg_of(got["sum"], ref)), c["name"]
+
+
+def test_reference_matches_oracle(generated, oracle):
+    check_against_oracle(*generated, oracle)
 
 
 def test_case_generator_promises(generated):
@@ -71,7 +83,7 @@ def test_case_generator_promises(generated):
         ref = rc.Reference(c["hist"], table)
         hits = 0
         for s in ref.cums:
-            q = float(s) / float(ref.count)
+            q = rc.go_div(float(s), ref.count)
             hits += all(np.float64(x).view(np.uint64) in bits
                         for x in (math.nextafter(q, -math.inf), q, math.nextafter(q, math.inf)))
         assert hits >= min(ref.nnz, 1), c["name"]
@@ -111,3 +123,83 @@ def test_threshold_rule():
     assert float(s) / float(t) >= 0.75 > float(s - 1) / float(t)
     assert rc.forces_bisection(2 ** 64 - 1, float(2 ** 64 - 5000) / float(2 ** 64 - 1))
     assert not rc.forces_bisection(1000, 0.5)
+
+
+def test_wrapped_reference_matches_oracle(wrapped, oracle):
+    """Go's uint64 total and running counts wrap at 2^64: the reference and the oracle agree on every wrapped case."""
+    check_against_oracle(*wrapped, oracle)
+
+
+def test_wrapped_case_generator_promises(wrapped):
+    precision, table, cases, ps = wrapped
+    w = rc.window(precision)
+    assert len(cases) < 64
+    names = {c["name"] for c in cases}
+    assert len(names) == len(cases)
+    refs = {c["name"]: rc.Reference(c["hist"], table, c["name"]) for c in cases}
+    for c in cases:
+        assert c["total"] == sum(c["hist"].values()) >= 2 ** 64, c["name"]          # the exact sum wraps
+        assert all(0 < n < 2 ** 64 for n in c["hist"].values()) and all(-32768 <= k <= 32767 for k in c["hist"])
+        inside = all(-w < k < w for k in c["hist"])
+        assert inside == (c["form"] == "window"), c["name"]
+        assert refs[c["name"]].count == c["total"] % 2 ** 64
+    for form in ("window", "dense"):
+        totals = {c["total"] % 2 ** 64 for c in cases if c["form"] == form}
+        assert set(rc.WRAPPED_TOTALS) <= totals, form
+        assert any(c["wraps"] == 2 for c in cases if c["form"] == form), form
+    # total 0 with a non-zero sum (average +-Inf) and with an exact zero sum (average 0 / 0 = NaN), in both forms
+    zero = [refs[c["name"]] for c in cases if c["total"] % 2 ** 64 == 0 and c["form"] != "outside"]
+    assert sum(r.sum == 0 for r in zero) >= 2 and sum(isinstance(r.sum, Fraction) and r.sum != 0 for r in zero) >= 2
+    # a wrap only at the last bucket
+    last = refs["wrap_at_last"]
+    assert all(a < b for a, b in zip(last.cums, last.cums[1:-1])) and last.cums[-1] < last.cums[-2]
+
+    # every window case has a p at which a bisection that assumes monotone running counts answers another bucket, and
+    # the valleys do so at some p in [0, 1]: the running count at key 0 (the middle cell) is below the threshold
+    # while an earlier bucket already satisfies the rule
+    unit = [p for p in ps if 0.0 <= p <= 1.0]
+    for c in cases:
+        ref = refs[c["name"]]
+        if c["form"] == "window":
+            assert any(rc.monotone_search(ref, p, w) != ref.percentile(p) for p in ps), c["name"]
+    for name in ("valley", "two_wraps", "wrap_at_warp_end", "wrap_in_warp", "wrap_in_row"):
+        ref = refs[name]
+        at0 = ref.cums[max(i for i, k in enumerate(ref.order) if k <= 0)]
+        valley = [p for p in unit if ref.percentile(p) < 0 and at0 < max(rc.threshold(ref.count, p), 1)]
+        assert valley and all(rc.monotone_search(ref, p, w) > 0 for p in valley), name
+
+    # every dense-path case whose total is not 0 has a p at which the first warp (2048 keys) whose end-of-warp running
+    # count satisfies the rule holds no bucket that does; with a total of 0 every non-empty running count gives +Inf,
+    # and the count alone no longer tells an empty histogram
+    for c in cases:
+        ref = refs[c["name"]]
+        if c["form"] != "window" and ref.count:
+            assert any(rc.end_of_warp_owner(ref, p) != ref.percentile(p) for p in ps), c["name"]
+    for name in ("wrap_at_warp_end", "wrap_in_warp", "wrap_in_row"):
+        ref = refs[name + "+%d" % w]
+        assert any(rc.end_of_warp_owner(ref, p) != ref.percentile(p) for p in unit), name
+        ks = [k for k in ref.order if -2048 <= k < 0]
+        at = dict(zip(ref.order, ref.cums))
+        assert any(at[b] < at[a] for a, b in zip(ks, ks[1:])), name                   # the wrap lies in warp 15
+    row = [k for k in refs["wrap_in_row"].order if k < 0]
+    assert len({(k + 32768) // 32 for k in row}) == 1                                  # ... inside one 32-key row
+    end = refs["wrap_at_warp_end"]
+    assert dict(zip(end.order, end.cums))[-1] == 0                                     # ... ending at the warp's end
+    assert any(c["form"] == "outside" and refs[c["name"]].count == 0 and c["hist"] for c in cases)
+
+    # crossings: every case has p on each crossing float64(s) / float64(total) of a bucket whose count is not 1 and
+    # one ulp on either side; some lie above 1, so 1.5 and +Inf answer too; NaN never does
+    bits = {np.float64(p).view(np.uint64) for p in ps}
+    for c in cases:
+        ref = refs[c["name"]]
+        for k, q in zip(ref.order, ref.ratios):
+            if c["hist"][k] != 1:
+                assert all(np.float64(x).view(np.uint64) in bits
+                           for x in (math.nextafter(q, -math.inf), q, math.nextafter(q, math.inf))), c["name"]
+    assert 1.5 in ps and math.inf in ps and any(math.isnan(p) for p in ps)
+    assert any(r.percentile(1.5) is not None for r in refs.values())
+    assert any(r.percentile(math.inf) is not None for r in refs.values())
+    if precision <= 46:
+        inf = refs["inf_wrap"]
+        assert math.isinf(float(table[-32768 & 0xFFFF])) and math.isinf(float(table[32767]))
+        assert math.isnan(inf.sum)
