@@ -147,6 +147,27 @@ LH_API lh_status lh_counter_add_u16(lh_ctx *ctx, const uint16_t *d_ids, const ui
 LH_API lh_status lh_counter_add_u32(lh_ctx *ctx, const uint32_t *d_ids, const uint64_t *d_amounts,
                              size_t n, void *stream);
 
+/* Keyed samples and counter adds under local ids, for callers whose global ids are not stable (MetricSystem record
+ * scopes: interned names whose ids are recycled).  h_map (host memory, k entries, reusable when the call returns) maps
+ * local id l < k to histogram / counter h_map[l]; a local id >= k, or an entry of LH_GRAPH_UNBOUND, drops the sample or
+ * op and counts 1 in lh_stats.dropped (k = 0 drops everything).  Entries may repeat.  Otherwise the semantics are those
+ * of lh_ingest_keyed_* (values of `kind` LH_VALUES_F64, or LH_VALUES_I64NS recorded as float64(ns)) and
+ * lh_counter_add_* (wrapping uint64): one write bracket and sequence number, lh_stats.samples / counter_ops, and
+ * lh_keyed_kernel_name reports the route.  The keyed kernels are those of lh_ingest_keyed_*, planned on k ids instead of
+ * max_histograms, so a call over a few names takes the shared-memory privatised kernel.
+ * Errors, before anything is enqueued: LH_ERR_INVALID for k > 4096, h_map NULL with k > 0, an unknown kind, NULL
+ * inputs with n > 0, values / amounts not 8-byte aligned or ids not naturally aligned; LH_ERR_RANGE for an entry
+ * >= max_histograms (max_counters) other than LH_GRAPH_UNBOUND.  n = 0 returns LH_OK with no bracket. */
+#define LH_MAP_MAX_IDS 4096
+LH_API lh_status lh_ingest_keyed_mapped_u16(lh_ctx *ctx, const uint32_t *h_map, uint32_t k, const uint16_t *d_ids,
+                                            const void *d_values, uint32_t kind, size_t n, void *stream);
+LH_API lh_status lh_ingest_keyed_mapped_u32(lh_ctx *ctx, const uint32_t *h_map, uint32_t k, const uint32_t *d_ids,
+                                            const void *d_values, uint32_t kind, size_t n, void *stream);
+LH_API lh_status lh_counter_add_mapped_u16(lh_ctx *ctx, const uint32_t *h_map, uint32_t kc, const uint16_t *d_ids,
+                                           const uint64_t *d_amounts, size_t n, void *stream);
+LH_API lh_status lh_counter_add_mapped_u32(lh_ctx *ctx, const uint32_t *h_map, uint32_t kc, const uint32_t *d_ids,
+                                           const uint64_t *d_amounts, size_t n, void *stream);
+
 /* ---- ingest, host-resident inputs ----------------------------------------
  * Same semantics, inputs in host memory.  Copies are chunked and overlapped
  * with the kernels.  On return the host buffers may be reused; the work may

@@ -174,6 +174,10 @@ SIGNATURES = {
     "lh_ingest_batch": (_i32, [_vp, C.POINTER(lh_batch_item), _u32, _vp]),
     "lh_counter_add_u16": (_i32, [_vp, _vp, _vp, _sz, _vp]),
     "lh_counter_add_u32": (_i32, [_vp, _vp, _vp, _sz, _vp]),
+    "lh_ingest_keyed_mapped_u16": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _sz, _vp]),
+    "lh_ingest_keyed_mapped_u32": (_i32, [_vp, _vp, _u32, _vp, _vp, _u32, _sz, _vp]),
+    "lh_counter_add_mapped_u16": (_i32, [_vp, _vp, _u32, _vp, _vp, _sz, _vp]),
+    "lh_counter_add_mapped_u32": (_i32, [_vp, _vp, _u32, _vp, _vp, _sz, _vp]),
     "lh_ingest_f64_host": (_i32, [_vp, _u32, _vp, _sz]),
     "lh_ingest_keyed_f64_u16_host": (_i32, [_vp, _vp, _vp, _sz]),
     "lh_ingest_keyed_i64ns_u16_host": (_i32, [_vp, _vp, _vp, _sz]),

@@ -430,11 +430,15 @@ KeyedOut keyed_out(lh_ctx *ctx, int b) {
 }
 
 // The scalar keyed kernel over a ragged piece (a head before the aligned body, a tail after it); nothing when n == 0.
+// With a map (record-scope ids), its mapped form, which copies the map into shared memory.
 template <typename IdT, typename ValT>
-void launch_keyed_scalar(lh_ctx *ctx, const KeyedOut &ko, const IdT *ids, const ValT *vals, size_t n, cudaStream_t s) {
+void launch_keyed_scalar(lh_ctx *ctx, const KeyedOut &ko, const IdT *ids, const ValT *vals, size_t n, cudaStream_t s,
+                         const IdMap *map = nullptr) {
     if (!n) return;
     constexpr int T = 256;
-    k_ingest_keyed<IdT, ValT, T><<<grid_1d(ctx, n, T, 1, ctx->keyed_blocks_per_sm), T, 0, s>>>(ids, vals, n, ko, ctx->pc);
+    const int grid = grid_1d(ctx, n, T, 1, ctx->keyed_blocks_per_sm);
+    if (map) k_ingest_keyed<IdT, ValT, T, IdMap><<<grid, T, (size_t)map->k * 4, s>>>(ids, vals, n, ko, ctx->pc, *map);
+    else k_ingest_keyed<IdT, ValT, T><<<grid, T, 0, s>>>(ids, vals, n, ko, ctx->pc, IdIdentity{});
     ctx->stats.kernel_launches++;
 }
 
@@ -463,14 +467,16 @@ struct KeyedPlan {
     WcParams wc{};                        // write-combining: the parameter block but for the arrays and the scratch
 };
 
-// The route of keyed samples (ids, vals, n) and everything its launches need; no CUDA call and no change to ctx.
+// The route of keyed samples (ids, vals, n) over `nids` ids in play (ctx->H; a mapped call's k) and everything its
+// launches need; no CUDA call and no change to ctx.  No ids in play: the scalar kernel, which drops every sample.
 // A pair (float64 samples ids/vals/n, int64 samples ids2/vals2/n2) is one write-combining launch for both arrays when
 // both are vector-aligned and that kernel takes them, else APART.
-KeyedPlan plan_keyed(const lh_ctx *ctx, size_t id_bytes, const void *ids, const void *vals, size_t n, bool pair = false,
+KeyedPlan plan_keyed(const lh_ctx *ctx, uint32_t nids, size_t id_bytes, const void *ids, const void *vals, size_t n, bool pair = false,
                      const void *ids2 = nullptr, const void *vals2 = nullptr, size_t n2 = 0) {
     KeyedPlan p;
+    if (!nids) return p;
     const uint32_t ks_per_max = std::max<uint32_t>(1, (uint32_t)(KS_SMEM_BYTES / ((size_t)ctx->pc.win * 4)));
-    const uint32_t ks_passes = (ctx->H + ks_per_max - 1) / ks_per_max;
+    const uint32_t ks_passes = (nids + ks_per_max - 1) / ks_per_max;
     const bool small = ks_passes <= KS_MAX_PASSES && ctx->keyed_mode == 0;
     const uintptr_t id_mask = 4 * id_bytes - 1;
     if (pair) {
@@ -487,7 +493,7 @@ KeyedPlan plan_keyed(const lh_ctx *ctx, size_t id_bytes, const void *ids, const 
         n = p.taken = p.n4 * 4;                                  // the vector body, all the write-combining kernel is offered
         if (small && p.n4 >= 4096) {
             p.route = KeyedPlan::SMALL; p.name = "k_ingest_keyed_small";
-            p.per = (ctx->H + ks_passes - 1) / ks_passes;
+            p.per = (nids + ks_passes - 1) / ks_passes;
             p.smem = ((size_t)p.per * ctx->pc.win + 4) * 4;
             // one CTA per SM; fewer when the batch is small, so that the per-CTA flush stays negligible
             p.grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)(ctx->sm_count - ctx->k1_reserve_sms),
@@ -500,7 +506,7 @@ KeyedPlan plan_keyed(const lh_ctx *ctx, size_t id_bytes, const void *ids, const 
     // the write-combining kernel, or keep the route above when it declines
     const int P = std::min(ctx->sm_count - ctx->k1_reserve_sms, (int)WC_MAX_PARTS);
     if (P < 8) return p;
-    const uint32_t ids_per = (ctx->H + P - 1) / P;
+    const uint32_t ids_per = (nids + P - 1) / P;
     const size_t hist_bytes = (((size_t)ids_per * ctx->pc.win + 3) & ~(size_t)3) * 4;
     // the owners' windows first, then the largest per-owner buffers that still fit (fewer SMs for ingest = more ids per
     // owner = less room; on H100, 256 records at P = 131 for H = 1024)
@@ -567,7 +573,7 @@ cudaError_t wc_done_event(int device, cudaEvent_t *out) {
 // p.taken2 int64 samples of (ids2, vals2).
 template <typename IdT, typename ValT>
 lh_status launch_keyed_wc(lh_ctx *ctx, int b, const KeyedPlan &p, const IdT *ids, const ValT *vals, cudaStream_t s,
-                          const IdT *ids2 = nullptr, const long long *vals2 = nullptr) {
+                          const IdT *ids2 = nullptr, const long long *vals2 = nullptr, const IdMap *map = nullptr) {
     const int P = p.grid;
     if (!ctx->d_kp_queues || ctx->kp_cap != p.wc.cap || ctx->kp_parts != P) {
         if (ctx->d_kp_queues) {
@@ -590,6 +596,9 @@ lh_status launch_keyed_wc(lh_ctx *ctx, int b, const KeyedPlan &p, const IdT *ids
 #define LH_WC_KERNEL(SPT) (!p.taken2 ? (const void *)k_ingest_keyed_wc<IdT, ValT, SPT, false> : (const void *)k_ingest_keyed_wc<IdT, double, SPT, true>)
     const void *fn = p.spt == 6 ? LH_WC_KERNEL(6) : p.spt == 4 ? LH_WC_KERNEL(4) : p.spt == 3 ? LH_WC_KERNEL(3) : LH_WC_KERNEL(8);
 #undef LH_WC_KERNEL
+#define LH_WC_MAPPED(SPT) (const void *)k_ingest_keyed_wc<IdT, ValT, SPT, false, IdMap>
+    if (map) fn = p.spt == 6 ? LH_WC_MAPPED(6) : p.spt == 4 ? LH_WC_MAPPED(4) : p.spt == 3 ? LH_WC_MAPPED(3) : LH_WC_MAPPED(8);
+#undef LH_WC_MAPPED
     // the attribute belongs to the function on the device, not to this context: one value for every context
     LH_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
     WcParams prm = p.wc;
@@ -597,7 +606,8 @@ lh_status launch_keyed_wc(lh_ctx *ctx, int b, const KeyedPlan &p, const IdT *ids
     prm.queues = ctx->d_kp_queues; prm.q_cnt = ctx->d_kp_cnt; prm.barrier = ctx->d_kp_cnt + (size_t)2 * P * P;
     prm.rare = ctx->d_kp_rare; prm.o = keyed_out(ctx, b);
     Prec pc = ctx->pc;
-    void *args[] = {&prm, &pc};
+    IdIdentity ident;
+    void *args[] = {&prm, &pc, map ? (void *)map : (void *)&ident};
     {
         std::lock_guard<std::mutex> lk(g_wc_mu);
         cudaEvent_t done;
@@ -611,9 +621,12 @@ lh_status launch_keyed_wc(lh_ctx *ctx, int b, const KeyedPlan &p, const IdT *ids
     return LH_OK;
 }
 
+// With a map, ids are local to it (record-scope calls): the plan counts map->k ids and the kernels are the mapped forms.
 template <typename IdT, typename ValT>
-lh_status launch_keyed(lh_ctx *ctx, int b, const IdT *d_ids, const ValT *d_vals, size_t n, cudaStream_t s) {
+lh_status launch_keyed(lh_ctx *ctx, int b, const IdT *d_ids, const ValT *d_vals, size_t n, cudaStream_t s,
+                       const IdMap *map = nullptr) {
     constexpr int T = 256;
+    const uint32_t nids = map ? map->k : ctx->H;
     const KeyedOut ko = keyed_out(ctx, b);
     size_t done = 0;
     while (done < n) {
@@ -630,27 +643,35 @@ lh_status launch_keyed(lh_ctx *ctx, int b, const IdT *d_ids, const ValT *d_vals,
         size_t m = (size_t)std::min<unsigned long long>(n - done, kCap - ctx->buf[b].hot_pending);
         const IdT *ids = d_ids + done;
         const ValT *vals = d_vals + done;
-        const KeyedPlan p = plan_keyed(ctx, sizeof(IdT), ids, vals, m);
-        launch_keyed_scalar(ctx, ko, ids, vals, p.head, s);
+        const KeyedPlan p = plan_keyed(ctx, nids, sizeof(IdT), ids, vals, m);
+        launch_keyed_scalar(ctx, ko, ids, vals, p.head, s, map);
         if (p.route == KeyedPlan::SMALL) {
             // per device, not per context: a value of this context's H could be overwritten by another context's
             // between here and the launch
-            LH_CUDA(ctx, cudaFuncSetAttribute((const void *)k_ingest_keyed_small<IdT, ValT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
-            for (uint32_t lo = 0; lo < ctx->H; lo += p.per) {
-                const uint32_t cnt = std::min(p.per, ctx->H - lo);
-                k_ingest_keyed_small<IdT, ValT><<<p.grid, KS_THREADS, p.smem, s>>>(ids + p.head, vals + p.head, p.n4, lo, cnt, ko, ctx->pc);
+            const void *fn = map ? (const void *)k_ingest_keyed_small<IdT, ValT, IdMap> : (const void *)k_ingest_keyed_small<IdT, ValT>;
+            LH_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
+            for (uint32_t lo = 0; lo < nids; lo += p.per) {
+                const uint32_t cnt = std::min(p.per, nids - lo);
+                if (map)
+                    k_ingest_keyed_small<IdT, ValT, IdMap><<<p.grid, KS_THREADS, p.smem, s>>>(ids + p.head, vals + p.head, p.n4, lo, cnt, ko, ctx->pc, *map);
+                else
+                    k_ingest_keyed_small<IdT, ValT><<<p.grid, KS_THREADS, p.smem, s>>>(ids + p.head, vals + p.head, p.n4, lo, cnt, ko, ctx->pc, IdIdentity{});
                 ctx->stats.kernel_launches++;
             }
         } else if (p.route == KeyedPlan::WC) {
-            lh_status st = launch_keyed_wc<IdT, ValT>(ctx, b, p, ids + p.head, vals + p.head, s);
+            lh_status st = launch_keyed_wc<IdT, ValT>(ctx, b, p, ids + p.head, vals + p.head, s, nullptr, nullptr, map);
             if (st != LH_OK) return st;
         } else if (p.route == KeyedPlan::VEC) {
-            k_ingest_keyed_vec<IdT, ValT, T><<<grid_1d(ctx, p.n4, T, 1, ctx->keyed_blocks_per_sm), T, 0, s>>>(ids + p.head, vals + p.head, p.n4, ctx->hot_replicas, ko, ctx->pc);
+            const int grid = grid_1d(ctx, p.n4, T, 1, ctx->keyed_blocks_per_sm);
+            if (map)
+                k_ingest_keyed_vec<IdT, ValT, T, IdMap><<<grid, T, (size_t)map->k * 4, s>>>(ids + p.head, vals + p.head, p.n4, ctx->hot_replicas, ko, ctx->pc, *map);
+            else
+                k_ingest_keyed_vec<IdT, ValT, T><<<grid, T, 0, s>>>(ids + p.head, vals + p.head, p.n4, ctx->hot_replicas, ko, ctx->pc, IdIdentity{});
             ctx->stats.kernel_launches++;
         }
         ctx->keyed_kernel = p.name;
         const size_t tail_off = p.head + p.taken;   // after whole tiles of the write-combining kernel: a ragged remainder
-        launch_keyed_scalar(ctx, ko, ids + tail_off, vals + tail_off, m - tail_off, s);
+        launch_keyed_scalar(ctx, ko, ids + tail_off, vals + tail_off, m - tail_off, s, map);
         LH_CUDA(ctx, cudaGetLastError());
         // only k_ingest_keyed_small / _vec count into the uint32 hot window
         if (p.route == KeyedPlan::SMALL || p.route == KeyedPlan::VEC) ctx->buf[b].hot_pending += p.taken;
@@ -666,7 +687,7 @@ lh_status launch_keyed(lh_ctx *ctx, int b, const IdT *d_ids, const ValT *d_vals,
 template <typename IdT>
 lh_status launch_keyed_pair(lh_ctx *ctx, int b, const IdT *ids_f, const double *vals_f, size_t n_f, const IdT *ids_ns,
                             const long long *vals_ns, size_t n_ns, cudaStream_t s) {
-    const KeyedPlan p = plan_keyed(ctx, sizeof(IdT), ids_f, vals_f, n_f, true, ids_ns, vals_ns, n_ns);
+    const KeyedPlan p = plan_keyed(ctx, ctx->H, sizeof(IdT), ids_f, vals_f, n_f, true, ids_ns, vals_ns, n_ns);
     if (p.route == KeyedPlan::APART) {
         lh_status st = launch_keyed<IdT, double>(ctx, b, ids_f, vals_f, n_f, s);
         if (st != LH_OK) return st;
@@ -683,10 +704,12 @@ lh_status launch_keyed_pair(lh_ctx *ctx, int b, const IdT *ids_f, const double *
     return LH_OK;
 }
 
-// (id, amount) pairs into `counters` (C of them, ids >= C dropped and counted); the caller counts the ops in stats
+// (id, amount) pairs into `counters` (C of them, ids >= C dropped and counted); the caller counts the ops in stats.
+// With a map, ids are local: C is map->k (<= LH_MAP_MAX, so always the shared-memory kernels, whose mapped forms take
+// the map after the 2C halves: 12 B per id, 48 KiB at most) and an op under an unbound row is dropped and counted.
 template <typename IdT>
 lh_status launch_counter(lh_ctx *ctx, unsigned long long *counters, uint32_t C, const IdT *d_ids, const uint64_t *d_amounts,
-                         size_t n, cudaStream_t s) {
+                         size_t n, cudaStream_t s, const IdMap *map = nullptr) {
     if (n) {
         constexpr int T = 512;
         const unsigned long long *amts = reinterpret_cast<const unsigned long long *>(d_amounts);
@@ -698,21 +721,21 @@ lh_status launch_counter(lh_ctx *ctx, unsigned long long *counters, uint32_t C, 
             size_t n4 = vec_ok ? (n - head) / 4 : 0;
             if (n4 < 4096) { head = 0; n4 = 0; }
             const size_t tail_off = head + n4 * 4;
-            if (head) {
-                k_counter_add_smem<IdT, T><<<1, T, (size_t)C * 8, s>>>(d_ids, amts, head, counters, C, ctx->d_dropped);
+            const size_t smem = (size_t)C * 8 + (map ? (size_t)C * 4 : 0);
+            auto scalar = [&](int grid, size_t off, size_t cnt) {
+                if (map) k_counter_add_smem<IdT, T, IdMap><<<grid, T, smem, s>>>(d_ids + off, amts + off, cnt, counters, C, ctx->d_dropped, *map);
+                else k_counter_add_smem<IdT, T><<<grid, T, smem, s>>>(d_ids + off, amts + off, cnt, counters, C, ctx->d_dropped, IdIdentity{});
                 ctx->stats.kernel_launches++;
-            }
+            };
+            if (head) scalar(1, 0, head);
             if (n4) {
                 // one CTA per SM (the per-CTA flush is C global atomics), fewer for small batches
                 const int grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)std::max(1, ctx->sm_count - ctx->k1_reserve_sms) * 2, n4 / (T * 4)));
-                k_counter_add_smem_vec<IdT, T><<<grid, T, (size_t)C * 8, s>>>(d_ids + head, amts + head, n4, counters, C, ctx->d_dropped);
+                if (map) k_counter_add_smem_vec<IdT, T, IdMap><<<grid, T, smem, s>>>(d_ids + head, amts + head, n4, counters, C, ctx->d_dropped, *map);
+                else k_counter_add_smem_vec<IdT, T><<<grid, T, smem, s>>>(d_ids + head, amts + head, n4, counters, C, ctx->d_dropped, IdIdentity{});
                 ctx->stats.kernel_launches++;
             }
-            if (tail_off < n) {
-                int grid = grid_1d(ctx, n - tail_off, T, 8, 2);
-                k_counter_add_smem<IdT, T><<<grid, T, (size_t)C * 8, s>>>(d_ids + tail_off, amts + tail_off, n - tail_off, counters, C, ctx->d_dropped);
-                ctx->stats.kernel_launches++;
-            }
+            if (tail_off < n) scalar(grid_1d(ctx, n - tail_off, T, 8, 2), tail_off, n - tail_off);
         } else {
             int grid = grid_1d(ctx, n, T, 4, 4);
             k_counter_add<IdT, T><<<grid, T, 0, s>>>(d_ids, amts, n, counters, C, ctx->d_dropped);
@@ -1271,6 +1294,75 @@ extern "C" lh_status lh_counter_add_u32(lh_ctx *ctx, const uint32_t *d_ids, cons
     if (n && (!d_ids || !d_amounts)) return fail(ctx, LH_ERR_INVALID, "NULL input");
     cudaStream_t s = pick_stream(ctx, stream);
     return write_bracket(ctx, s, [&](int b) { return add_counters<unsigned int>(ctx, b, d_ids, d_amounts, n, s); });
+}
+static_assert(LH_MAP_MAX == LH_MAP_MAX_IDS, "the header and the kernels agree on the map size");
+namespace {
+// The host map of a mapped call into the parameter block's form; LH_ERR_INVALID / LH_ERR_RANGE as the header says.
+lh_status make_map(lh_ctx *ctx, const uint32_t *h_map, uint32_t k, uint32_t limit, IdMap &m) {
+    if (k > LH_MAP_MAX) return fail(ctx, LH_ERR_INVALID, "more than 4096 mapped ids");
+    if (k && !h_map) return fail(ctx, LH_ERR_INVALID, "h_map is NULL");
+    for (uint32_t i = 0; i < k; i++)
+        if (h_map[i] != LH_GRAPH_UNBOUND && h_map[i] >= limit) return fail(ctx, LH_ERR_RANGE, "map entry >= max_histograms / max_counters");
+    m.k = k;
+    m.any_unbound = std::find(h_map, h_map + k, LH_GRAPH_UNBOUND) != h_map + k;
+    std::copy(h_map, h_map + k, m.row);
+    return LH_OK;
+}
+
+template <typename IdT>
+lh_status ingest_keyed_mapped(lh_ctx *ctx, const uint32_t *h_map, uint32_t k, const IdT *d_ids, const void *d_values,
+                              uint32_t kind, size_t n, void *stream) {
+    if (kind != LH_VALUES_F64 && kind != LH_VALUES_I64NS) return fail(ctx, LH_ERR_INVALID, "unknown values kind");
+    if (n && (!d_ids || !d_values)) return fail(ctx, LH_ERR_INVALID, "NULL input");
+    if (((uintptr_t)d_values & 7u) || ((uintptr_t)d_ids & (sizeof(IdT) - 1)))
+        return fail(ctx, LH_ERR_INVALID, "ids / values are not naturally aligned");
+    IdMap m;
+    lh_status st = make_map(ctx, h_map, k, ctx->H, m);
+    if (st != LH_OK || n == 0) return st;
+    cudaStream_t s = pick_stream(ctx, stream);
+    return write_bracket(ctx, s, [&](int b) {
+        return kind == LH_VALUES_F64 ? launch_keyed<IdT, double>(ctx, b, d_ids, static_cast<const double *>(d_values), n, s, &m)
+                                     : launch_keyed<IdT, long long>(ctx, b, d_ids, static_cast<const long long *>(d_values), n, s, &m);
+    });
+}
+
+template <typename IdT>
+lh_status counter_add_mapped(lh_ctx *ctx, const uint32_t *h_map, uint32_t kc, const IdT *d_ids, const uint64_t *d_amounts,
+                             size_t n, void *stream) {
+    if (n && (!d_ids || !d_amounts)) return fail(ctx, LH_ERR_INVALID, "NULL input");
+    if (((uintptr_t)d_amounts & 7u) || ((uintptr_t)d_ids & (sizeof(IdT) - 1)))
+        return fail(ctx, LH_ERR_INVALID, "ids / amounts are not naturally aligned");
+    IdMap m;
+    lh_status st = make_map(ctx, h_map, kc, ctx->C, m);
+    if (st != LH_OK || n == 0) return st;
+    cudaStream_t s = pick_stream(ctx, stream);
+    return write_bracket(ctx, s, [&](int b) {
+        lh_status r = launch_counter<IdT>(ctx, ctx->buf[b].d_counters, kc, d_ids, d_amounts, n, s, &m);
+        if (r == LH_OK) ctx->stats.counter_ops += n;
+        return r;
+    });
+}
+}  // namespace
+
+extern "C" lh_status lh_ingest_keyed_mapped_u16(lh_ctx *ctx, const uint32_t *h_map, uint32_t k, const uint16_t *d_ids,
+                                                const void *d_values, uint32_t kind, size_t n, void *stream) {
+    LH_ENTER(ctx);
+    return ingest_keyed_mapped<unsigned short>(ctx, h_map, k, d_ids, d_values, kind, n, stream);
+}
+extern "C" lh_status lh_ingest_keyed_mapped_u32(lh_ctx *ctx, const uint32_t *h_map, uint32_t k, const uint32_t *d_ids,
+                                                const void *d_values, uint32_t kind, size_t n, void *stream) {
+    LH_ENTER(ctx);
+    return ingest_keyed_mapped<unsigned int>(ctx, h_map, k, d_ids, d_values, kind, n, stream);
+}
+extern "C" lh_status lh_counter_add_mapped_u16(lh_ctx *ctx, const uint32_t *h_map, uint32_t kc, const uint16_t *d_ids,
+                                               const uint64_t *d_amounts, size_t n, void *stream) {
+    LH_ENTER(ctx);
+    return counter_add_mapped<unsigned short>(ctx, h_map, kc, d_ids, d_amounts, n, stream);
+}
+extern "C" lh_status lh_counter_add_mapped_u32(lh_ctx *ctx, const uint32_t *h_map, uint32_t kc, const uint32_t *d_ids,
+                                               const uint64_t *d_amounts, size_t n, void *stream) {
+    LH_ENTER(ctx);
+    return counter_add_mapped<unsigned int>(ctx, h_map, kc, d_ids, d_amounts, n, stream);
 }
 extern "C" lh_status lh_ingest_batch(lh_ctx *ctx, const lh_batch_item *h_items, uint32_t n_items, void *stream) {
     LH_ENTER(ctx);

@@ -400,9 +400,57 @@ struct KeyedOut {
     uint32_t H;
 };
 
-template <typename ValT>
-__device__ __forceinline__ void keyed_one(uint32_t id, ValT raw, const Prec &pc, const KeyedOut &o, unsigned int *hot, uint64_t pol) {
-    if (id >= o.H) { atomicAdd(o.dropped, 1ull); return; }
+// Id-map policies of the keyed and counter kernels (their last template parameter, passed by value as their last
+// argument).  IdIdentity: an id is a row (the raw calls).  IdMap: ids are local to a record scope; local id l < k means
+// row row[l], and an id >= k or a row of LH_GRAPH_UNBOUND drops the sample (counted).  Binning and privatisation stay in
+// local-id space; the map is read only where a row address is formed.  The kernels read it through a view, MapRows,
+// over the parameter block (indexed loads from the constant bank; the parameter is not __grid_constant__, which would
+// change how the other by-value parameters are loaded) or over a copy in shared memory; IdIdentity is its own view and
+// compiles to the unmapped code.
+constexpr uint32_t LH_MAP_MAX = 4096;          // entries of an IdMap (16 KiB of the parameter block)
+struct IdIdentity {
+    __device__ __forceinline__ uint32_t bound(uint32_t H) const { return H; }
+    __device__ __forceinline__ bool lookup(uint32_t id, uint32_t H, uint32_t &) const { return id < H; }   // row = id
+    __device__ __forceinline__ uint32_t row(uint32_t id) const { return id; }
+    __device__ __forceinline__ bool drops(uint32_t id, uint32_t C) const { return id >= C; }
+};
+struct IdMap {
+    uint32_t k;
+    uint32_t any_unbound;            // some row[l] is unbound: the counter kernels check every op
+    uint32_t row[LH_MAP_MAX];
+};
+struct MapRows {
+    const uint32_t *rows;
+    uint32_t k;
+    bool any_unbound;
+    __device__ __forceinline__ uint32_t bound(uint32_t) const { return k; }
+    // a counter op under local id l is dropped (the op count of an unbound row is not known at the flush)
+    __device__ __forceinline__ bool drops(uint32_t l, uint32_t) const { return l >= k || (any_unbound && rows[l] == 0xFFFFFFFFu); }
+    // local id l -> its row in r (r may alias l); false: drop the sample
+    __device__ __forceinline__ bool lookup(uint32_t l, uint32_t, uint32_t &r) const {
+        if (l >= k) return false;
+        const uint32_t x = rows[l];
+        r = x;
+        return x != 0xFFFFFFFFu;
+    }
+    __device__ __forceinline__ uint32_t row(uint32_t l) const { return rows[l]; }   // l < k; may be unbound
+};
+template <typename Map> constexpr bool kMapped = !std::is_same<Map, IdIdentity>::value;
+// the map as read from the parameter block (flushes and rare paths)
+__device__ __forceinline__ IdIdentity map_view(const IdIdentity &) { return {}; }
+__device__ __forceinline__ MapRows map_view(const IdMap &m) { return MapRows{m.row, m.k, m.any_unbound != 0}; }
+// the map copied into shared memory `s` (k words) by the whole CTA, for kernels that look up every sample
+__device__ __forceinline__ IdIdentity map_to_smem(const IdIdentity &, uint32_t *) { return {}; }
+__device__ __forceinline__ MapRows map_to_smem(const IdMap &m, uint32_t *s) {
+    for (uint32_t i = threadIdx.x; i < m.k; i += blockDim.x) s[i] = m.row[i];
+    __syncthreads();
+    return MapRows{s, m.k, m.any_unbound != 0};
+}
+
+template <typename ValT, typename V = IdIdentity>
+__device__ __forceinline__ void keyed_one(uint32_t id, ValT raw, const Prec &pc, const KeyedOut &o, unsigned int *hot, uint64_t pol,
+                                          const V &m = {}) {
+    if (!m.lookup(id, o.H, id)) { atomicAdd(o.dropped, 1ull); return; }
     double v = sample_to_f64<ValT>(raw);
     uint32_t idx; bool slow;
     fast_candidate(v, pc, idx, slow);
@@ -416,9 +464,13 @@ __device__ __forceinline__ void keyed_one(uint32_t id, ValT raw, const Prec &pc,
 // The same sample straight into the uint64 arrays (one 64-bit atomic + the histogram's flag): for the few samples
 // that reach the scalar kernel (ragged heads / tails) and the rare paths of the write-combining kernel, so that those
 // launches leave nothing in the uint32 hot window for the snapshot to fold.
-template <typename ValT>
-__device__ __forceinline__ void keyed_one_direct(uint32_t id, ValT raw, const Prec &pc, const KeyedOut &o) {
-    if (id >= o.H) { atomicAdd(o.dropped, 1ull); return; }
+template <typename ValT, typename V = IdIdentity>
+__device__ __forceinline__ void keyed_one_direct(uint32_t id, ValT raw, const Prec &pc, const KeyedOut &o, const V &m = {}) {
+    if constexpr (kMapped<V>) {
+        if (!m.lookup(id, o.H, id)) { atomicAdd(o.dropped, 1ull); return; }
+    } else {
+        if (id >= o.H) { atomicAdd(o.dropped, 1ull); return; }   // (written out: through lookup() the value load moves)
+    }
     add_bucket_global(o.buckets + (size_t)id * 65536u, o.flags + id, key16_of(sample_to_f64<ValT>(raw), pc), 1ull, pc.win);
 }
 
@@ -429,6 +481,16 @@ __device__ __noinline__ void keyed_one_slow(uint32_t id, unsigned long long raw,
     ValT r;
     memcpy(&r, &raw, 8);
     keyed_one_direct<ValT>(id, r, pc, o);
+}
+// Mapped: the row is resolved here, so that the map (in the parameter block) is only read inline.
+template <typename ValT>
+__device__ __forceinline__ void keyed_one_slow_v(uint32_t id, unsigned long long raw, const Prec &pc, const KeyedOut &o, IdIdentity) {
+    keyed_one_slow<ValT>(id, raw, pc, o);
+}
+template <typename ValT>
+__device__ __forceinline__ void keyed_one_slow_v(uint32_t id, unsigned long long raw, const Prec &pc, const KeyedOut &o, const MapRows &m) {
+    if (!m.lookup(id, o.H, id)) { atomicAdd(o.dropped, 1ull); return; }
+    keyed_one_slow<ValT>(id, raw, pc, o);
 }
 
 template <typename IdT>
@@ -471,9 +533,13 @@ template <> struct IdPack<unsigned int> {
 // `hot` holds `replicas` copies of the window ([replicas][H][2*win]); CTA b updates copy b % replicas, which
 // divides the same-address pressure on hot cells (clustered, latency-like data) by the replica count while every
 // copy stays L2-resident.  k_fold_hot sums the copies.
-template <typename IdT, typename ValT, int THREADS>
+// Mapped: the map is copied into dynamic shared memory (k words) and the sample goes to its row's window.
+template <typename IdT, typename ValT, int THREADS, typename Map = IdIdentity>
 __global__ void __launch_bounds__(THREADS)
-k_ingest_keyed_vec(const IdT *__restrict__ ids, const ValT *__restrict__ vals, size_t n4, uint32_t replicas, KeyedOut o, Prec pc) {
+k_ingest_keyed_vec(const IdT *__restrict__ ids, const ValT *__restrict__ vals, size_t n4, uint32_t replicas, KeyedOut o, Prec pc,
+                   const Map map) {
+    extern __shared__ uint32_t kv_map[];
+    const auto mv = map_to_smem(map, kv_map);
     unsigned int *hot = o.hot + (size_t)(blockIdx.x % replicas) * o.H * (2u * pc.win);
     const uint64_t pol = policy_evict_last();
     const size_t stride = (size_t)gridDim.x * THREADS;
@@ -486,18 +552,21 @@ k_ingest_keyed_vec(const IdT *__restrict__ ids, const ValT *__restrict__ vals, s
         for (int j = 0; j < 4; j++) {
             ValT r;
             memcpy(&r, &raw[j], 8);
-            keyed_one<ValT>(id4[j], r, pc, o, hot, pol);
+            keyed_one<ValT>(id4[j], r, pc, o, hot, pol, mv);
         }
     }
 }
 
-// Scalar version for ragged heads/tails and misaligned inputs.
-template <typename IdT, typename ValT, int THREADS>
+// Scalar version for ragged heads/tails and misaligned inputs.  Mapped: as k_ingest_keyed_vec.
+template <typename IdT, typename ValT, int THREADS, typename Map = IdIdentity>
 __global__ void __launch_bounds__(THREADS)
-k_ingest_keyed(const IdT *__restrict__ ids, const ValT *__restrict__ vals, size_t n, KeyedOut o, Prec pc) {
+k_ingest_keyed(const IdT *__restrict__ ids, const ValT *__restrict__ vals, size_t n, KeyedOut o, Prec pc,
+               const Map map) {
+    extern __shared__ uint32_t ks_map[];
+    const auto mv = map_to_smem(map, ks_map);
     const size_t stride = (size_t)gridDim.x * THREADS;
     for (size_t i = (size_t)blockIdx.x * THREADS + threadIdx.x; i < n; i += stride)
-        keyed_one_direct<ValT>((uint32_t)ids[i], vals[i], pc, o);
+        keyed_one_direct<ValT>((uint32_t)ids[i], vals[i], pc, o, mv);
 }
 
 // ------------------------------------------------------------------ K1k/small
@@ -510,13 +579,15 @@ k_ingest_keyed(const IdT *__restrict__ ids, const ValT *__restrict__ vals, size_
 constexpr int KS_THREADS = 1024;
 constexpr int KS_SMEM_BYTES = 196608;        // shared memory the windows of one pass may take (11 ids at precision 100)
 
-template <typename IdT, typename ValT>
+template <typename IdT, typename ValT, typename Map = IdIdentity>
 __global__ void __launch_bounds__(KS_THREADS, 1)
 k_ingest_keyed_small(const IdT *__restrict__ ids, const ValT *__restrict__ vals, size_t n4,
-                     uint32_t id_lo, uint32_t id_cnt, KeyedOut o, Prec pc) {
+                     uint32_t id_lo, uint32_t id_cnt, KeyedOut o, Prec pc, const Map map) {
     // This launch owns ids [id_lo, id_lo + id_cnt); with more histograms than fit, the host
     // runs one pass per id sub-range over the same batch.  Samples of other valid ids are skipped; ids >= H are
-    // dropped (and counted) by the pass that starts at id 0.
+    // dropped (and counted) by the pass that starts at id 0.  Mapped: ids, passes and windows are local (H is k); the
+    // flush adds a window to its row, or counts an unbound row's total as dropped.
+    const auto mv = map_view(map);
     extern __shared__ __align__(16) uint32_t ks_hist[];          // [id_cnt][win] + trash word
     const uint32_t row = pc.win;
     const uint32_t words = id_cnt * row;
@@ -549,7 +620,7 @@ k_ingest_keyed_small(const IdT *__restrict__ ids, const ValT *__restrict__ vals,
         for (int i = 0; i < 4; i++) {
             const uint32_t l = cur_id[i] - id_lo;                                  // local id (wraps when below id_lo)
             const bool mine = valid & (l < id_cnt);
-            const bool bad = valid & (cur_id[i] >= o.H) & (id_lo == 0);
+            const bool bad = valid & (cur_id[i] >= mv.bound(o.H)) & (id_lo == 0);
             flag[i] = (mine & flag[i]) | bad;
             off[i] = mine ? off[i] + l * (row * 4u) : trash_off;
             any |= flag[i];
@@ -562,7 +633,7 @@ k_ingest_keyed_small(const IdT *__restrict__ ids, const ValT *__restrict__ vals,
                 memcpy(&rv, &cur[i], 8);
                 // uncertain samples of a valid id could stay in shared memory; the L2 route is exact too
                 // and keeps this path trivial (it handles ~0.05 % of the samples)
-                keyed_one<ValT>(cur_id[i], rv, pc, o, o.hot, pol);
+                keyed_one<ValT>(cur_id[i], rv, pc, o, o.hot, pol, mv);
                 off[i] = trash_off;
             }
         }
@@ -576,7 +647,9 @@ k_ingest_keyed_small(const IdT *__restrict__ ids, const ValT *__restrict__ vals,
         const uint32_t c = ks_hist[i];
         if (!c) continue;
         const uint32_t lid = i / row, slot = i - lid * row;
-        atomicAdd(&o.hot[(size_t)(id_lo + lid) * (2u * pc.win) + slot], c);
+        const uint32_t r = mv.row(id_lo + lid);
+        if (kMapped<Map> && r == 0xFFFFFFFFu) atomicAdd(o.dropped, (unsigned long long)c);
+        else atomicAdd(&o.hot[(size_t)r * (2u * pc.win) + slot], c);
     }
 }
 
@@ -652,15 +725,21 @@ __device__ __forceinline__ void grid_barrier(unsigned int *bar, unsigned int tar
 }
 
 // a record that could not be queued: add it to its bucket directly (exact, one L2 atomic; positive rows: slot == key)
-__device__ __forceinline__ void wc_spill(uint32_t rec, uint32_t owner, uint32_t P, const Prec &pc, const KeyedOut &o) {
-    const uint32_t lid = rec / pc.win, slot = rec - lid * pc.win, id = lid * P + owner;
+template <typename V = IdIdentity>
+__device__ __forceinline__ void wc_spill(uint32_t rec, uint32_t owner, uint32_t P, const Prec &pc, const KeyedOut &o, const V &m = {}) {
+    const uint32_t lid = rec / pc.win, slot = rec - lid * pc.win, id = m.row(lid * P + owner);
+    if (kMapped<V> && id == 0xFFFFFFFFu) { atomicAdd(o.dropped, 1ull); return; }
     add_bucket_global(o.buckets + (size_t)id * 65536u, o.flags + id, slot, 1ull, pc.win);
 }
 
-template <typename IdT, typename ValT, int SPT, bool PAIR = false>      // PAIR: a second, int64 segment follows the float64 one
+// Mapped (non-PAIR only): ids are local, owners hold ceil(k / P) windows (ids_per) and o.H's bound is k; the map is read
+// by the spills, the rare path and the final flush, which counts an unbound row's window total as dropped.
+template <typename IdT, typename ValT, int SPT, bool PAIR = false, typename Map = IdIdentity>   // PAIR: a second, int64 segment follows the float64 one
 __global__ void __launch_bounds__(WcShape<SPT>::THREADS, 1)
-k_ingest_keyed_wc(WcParams prm, Prec pc) {
+k_ingest_keyed_wc(WcParams prm, Prec pc, const Map map) {
     static_assert(!PAIR || std::is_same<ValT, double>::value, "the int64 segment rides on the float64 instantiation");
+    static_assert(!PAIR || !kMapped<Map>, "pairs are not mapped");
+    const auto mv = map_view(map);
     using S = WcShape<SPT>;
     constexpr int WC_THREADS = S::THREADS;
     constexpr int GROUPS = S::PER / 4;
@@ -746,7 +825,7 @@ k_ingest_keyed_wc(WcParams prm, Prec pc) {
                     const uint32_t id = idp[g].get(j);
                     const uint32_t lid = __umulhi(id, prm.inv_p), owner = lid * negP + id;   // id / P, id % P
                     const uint32_t rec = lid * pc.win + idx[j];
-                    const bool rare = flag[j] | (id >= prm.o.H);
+                    const bool rare = flag[j] | (id >= mv.bound(prm.o.H));
                     // branch-free append: rare samples draw from a trash counter (a predicated atomic makes ptxas branch and spill)
                     const uint32_t oe = rare ? P : owner;
                     uint32_t pos;
@@ -764,7 +843,7 @@ k_ingest_keyed_wc(WcParams prm, Prec pc) {
                         if (flag[j]) {
                             const unsigned int at = atomicAdd(s_rare, 1u);
                             if (at < WC_RARE_CAP) rareq[at] = make_uint4((unsigned int)raw[g][j], (unsigned int)(raw[g][j] >> 32), idp[g].get(j), 0u);
-                            else keyed_one_slow<ValT>(idp[g].get(j), raw[g][j], pc, prm.o);
+                            else keyed_one_slow_v<ValT>(idp[g].get(j), raw[g][j], pc, prm.o, mv);
                         }
                 }
             }
@@ -799,7 +878,7 @@ k_ingest_keyed_wc(WcParams prm, Prec pc) {
                                 off0 += WC_LINE;
                             } else if (k4 == 0) {                                          // sub-queue full: these records go the L2 route
                                 const unsigned short *r = s_buf + o * row_stride + l * WC_LINE;
-                                for (unsigned int k = 0; k < (unsigned int)WC_LINE; k++) wc_spill(r[k], o, P, pc, prm.o);
+                                for (unsigned int k = 0; k < (unsigned int)WC_LINE; k++) wc_spill(r[k], o, P, pc, prm.o, mv);
                             }
                         }
                     }
@@ -854,7 +933,7 @@ k_ingest_keyed_wc(WcParams prm, Prec pc) {
                 ValT r;
                 const unsigned long long raw = ((unsigned long long)e.y << 32) | e.x;
                 memcpy(&r, &raw, 8);
-                keyed_one_direct<ValT>(e.z, r, pc, prm.o);
+                keyed_one_direct<ValT>(e.z, r, pc, prm.o, mv);
             }
             __syncthreads();
             if (tid == 0) *s_rare = 0;
@@ -874,7 +953,7 @@ k_ingest_keyed_wc(WcParams prm, Prec pc) {
                         off0 += nrec;
                     } else {
                         const unsigned short *r = s_buf + o * row_stride + l * WC_LINE;
-                        for (unsigned int k = 0; k < nrec; k++) wc_spill(r[k], o, P, pc, prm.o);
+                        for (unsigned int k = 0; k < nrec; k++) wc_spill(r[k], o, P, pc, prm.o, mv);
                     }
                 }
                 s_off[o] = off0;
@@ -922,8 +1001,14 @@ k_ingest_keyed_wc(WcParams prm, Prec pc) {
     // ---------------- flush my windows straight into the uint64 bucket arrays (positive rows: slot == key) and raise the
     // flags of the histograms that received counts; nothing of the common path goes through the uint32 hot window
     for (uint32_t lid = 0; lid < prm.ids_per; lid++) {
-        const uint32_t id = lid * P + p;
-        if (id >= prm.o.H) break;
+        if (lid * P + p >= mv.bound(prm.o.H)) break;
+        const uint32_t id = mv.row(lid * P + p);
+        if (kMapped<Map> && id == 0xFFFFFFFFu) {
+            unsigned long long lost = 0;
+            for (uint32_t slot = tid; slot < pc.win; slot += WC_THREADS) lost += s_hist[lid * pc.win + slot];
+            if (lost) atomicAdd(prm.o.dropped, lost);
+            continue;
+        }
         int any = 0;
         for (uint32_t slot = tid; slot < pc.win; slot += WC_THREADS) {
             const unsigned int cnt = s_hist[lid * pc.win + slot];
@@ -962,20 +1047,23 @@ __global__ void k_fold_hot(unsigned int *__restrict__ hot, unsigned long long *_
 // high half only when the amount has high bits or the low half carried.
 constexpr int K2_SMEM_COUNTERS = 8192;
 
-template <typename IdT, int THREADS>
+// Mapped (k_counter_add_smem{,_vec}): C is the number of local ids; the map follows the 2C halves in shared memory, an
+// op is dropped per op when its local id is >= C or unbound, and the flush adds counter i into its row.
+template <typename IdT, int THREADS, typename Map = IdIdentity>
 __global__ void __launch_bounds__(THREADS)
 k_counter_add_smem(const IdT *__restrict__ ids, const unsigned long long *__restrict__ amounts, size_t n,
                    unsigned long long *__restrict__ counters, uint32_t C,
-                   unsigned long long *__restrict__ dropped) {
+                   unsigned long long *__restrict__ dropped, const Map map) {
     extern __shared__ unsigned int s_cnt[];          // [C] low halves, [C] high halves
     unsigned int *lo = s_cnt, *hi = s_cnt + C;
     for (uint32_t i = threadIdx.x; i < 2 * C; i += THREADS) s_cnt[i] = 0;
+    const auto mv = map_to_smem(map, s_cnt + 2 * C);
     __syncthreads();
     const size_t stride = (size_t)gridDim.x * THREADS;
     for (size_t i = (size_t)blockIdx.x * THREADS + threadIdx.x; i < n; i += stride) {
         uint32_t id = (uint32_t)ids[i];
         unsigned long long amt = amounts[i];
-        if (id >= C) { atomicAdd(dropped, 1ull); continue; }
+        if (mv.drops(id, C)) { atomicAdd(dropped, 1ull); continue; }
         unsigned int a_lo = (unsigned int)amt, a_hi = (unsigned int)(amt >> 32);
         unsigned int old = atomicAdd(&lo[id], a_lo);
         a_hi += (old + a_lo < old) ? 1u : 0u;        // carry out of the low half
@@ -984,19 +1072,21 @@ k_counter_add_smem(const IdT *__restrict__ ids, const unsigned long long *__rest
     __syncthreads();
     for (uint32_t i = threadIdx.x; i < C; i += THREADS) {
         unsigned long long v = ((unsigned long long)hi[i] << 32) | lo[i];
-        if (v) atomicAdd(&counters[i], v);
+        if (v) atomicAdd(&counters[mv.row(i)], v);            // v == 0 for an unbound row: its ops were dropped
     }
 }
 
 // Vector body: 4 consecutive (id, amount) pairs per thread and iteration (two 128-bit amount loads, one 64/128-bit id
 // load), the next group prefetched while the current one is added.  amounts 32-byte aligned, ids 4*sizeof(IdT)-aligned.
-template <typename IdT, int THREADS>
+template <typename IdT, int THREADS, typename Map = IdIdentity>
 __global__ void __launch_bounds__(THREADS)
 k_counter_add_smem_vec(const IdT *__restrict__ ids, const unsigned long long *__restrict__ amounts, size_t n4,
-                       unsigned long long *__restrict__ counters, uint32_t C, unsigned long long *__restrict__ dropped) {
+                       unsigned long long *__restrict__ counters, uint32_t C, unsigned long long *__restrict__ dropped,
+                       const Map map) {
     extern __shared__ unsigned int s_cnt[];          // [C] low halves, [C] high halves
     unsigned int *lo = s_cnt, *hi = s_cnt + C;
     for (uint32_t i = threadIdx.x; i < 2 * C; i += THREADS) s_cnt[i] = 0;
+    const auto mv = map_to_smem(map, s_cnt + 2 * C);
     __syncthreads();
     const size_t stride = (size_t)gridDim.x * THREADS;
     size_t g = (size_t)blockIdx.x * THREADS + threadIdx.x;
@@ -1010,7 +1100,7 @@ k_counter_add_smem_vec(const IdT *__restrict__ ids, const unsigned long long *__
         for (int j = 0; j < 4; j++) {
             const uint32_t id = cid.get(j);
             const unsigned long long amt = cur[j];
-            if (id >= C) { atomicAdd(dropped, 1ull); continue; }
+            if (mv.drops(id, C)) { atomicAdd(dropped, 1ull); continue; }
             const unsigned int a_lo = (unsigned int)amt;
             unsigned int a_hi = (unsigned int)(amt >> 32);
             const unsigned int old = atomicAdd(&lo[id], a_lo);
@@ -1024,7 +1114,7 @@ k_counter_add_smem_vec(const IdT *__restrict__ ids, const unsigned long long *__
     __syncthreads();
     for (uint32_t i = threadIdx.x; i < C; i += THREADS) {
         unsigned long long v = ((unsigned long long)hi[i] << 32) | lo[i];
-        if (v) atomicAdd(&counters[i], v);
+        if (v) atomicAdd(&counters[mv.row(i)], v);            // v == 0 for an unbound row: its ops were dropped
     }
 }
 

@@ -697,6 +697,24 @@ class Engine:
     def counter_add_u32(self, d_ids, d_amounts, n: int, stream=None):
         self._check(self.lib.lh_counter_add_u32(self.h, _ptr(d_ids), _ptr(d_amounts), n, _stream(stream)))
 
+    def ingest_keyed_mapped_u16(self, h_map, d_ids, d_values, kind: int, n: int, stream=None):
+        """lh_ingest_keyed_mapped_u16: local id l < len(h_map) is histogram h_map[l] (a list of ids)."""
+        m, k = _ids(h_map)
+        self._check(self.lib.lh_ingest_keyed_mapped_u16(self.h, m, k, _ptr(d_ids), _ptr(d_values), kind, n, _stream(stream)))
+
+    def ingest_keyed_mapped_u32(self, h_map, d_ids, d_values, kind: int, n: int, stream=None):
+        m, k = _ids(h_map)
+        self._check(self.lib.lh_ingest_keyed_mapped_u32(self.h, m, k, _ptr(d_ids), _ptr(d_values), kind, n, _stream(stream)))
+
+    def counter_add_mapped_u16(self, h_map, d_ids, d_amounts, n: int, stream=None):
+        """lh_counter_add_mapped_u16: local id l < len(h_map) is counter h_map[l]."""
+        m, k = _ids(h_map)
+        self._check(self.lib.lh_counter_add_mapped_u16(self.h, m, k, _ptr(d_ids), _ptr(d_amounts), n, _stream(stream)))
+
+    def counter_add_mapped_u32(self, h_map, d_ids, d_amounts, n: int, stream=None):
+        m, k = _ids(h_map)
+        self._check(self.lib.lh_counter_add_mapped_u32(self.h, m, k, _ptr(d_ids), _ptr(d_amounts), n, _stream(stream)))
+
     # ---- ingest, host inputs
     def ingest_f64_host(self, histogram_id: int, h_values, n: int | None = None):
         if isinstance(h_values, np.ndarray):

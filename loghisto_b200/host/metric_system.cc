@@ -40,6 +40,11 @@
 #pragma weak lh_graph_recorder_counter_add_u32
 #pragma weak lh_graph_recorder_timer_start
 #pragma weak lh_graph_recorder_timer_stop
+
+#pragma weak lh_ingest_keyed_mapped_u16
+#pragma weak lh_ingest_keyed_mapped_u32
+#pragma weak lh_counter_add_mapped_u16
+#pragma weak lh_counter_add_mapped_u32
 // And for device subscriptions: over a build without them, NewDeviceSubscription throws.
 #pragma weak lh_board_create
 #pragma weak lh_snapshot_publish
@@ -789,6 +794,28 @@ void RecordScope::Histograms(const std::vector<Item> &items) {
     }
     check(ms_->ctx_, lh_ingest_batch(ms_->ctx_, batch.data(), (uint32_t)batch.size(), stream_), "lh_ingest_batch");
     ms_->dropped_over_limit_.fetch_add(unbound, std::memory_order_relaxed);
+}
+void RecordScope::Keyed(const void *d_ids, size_t id_bytes, const void *d_values, uint32_t kind, size_t n) {
+    if (!ms_) throw std::runtime_error("RecordScope::Keyed after End()");
+    if (id_bytes != 2 && id_bytes != 4) throw std::invalid_argument("RecordScope::Keyed: id_bytes must be 2 or 4");
+    auto fn16 = lh_ingest_keyed_mapped_u16;
+    auto fn32 = lh_ingest_keyed_mapped_u32;
+    if (id_bytes == 2 ? !fn16 : !fn32) throw std::runtime_error("RecordScope::Keyed: this libloghisto_b200 has no mapped keyed ingest");
+    const uint32_t k = (uint32_t)hids_.size();
+    lh_status st = id_bytes == 2 ? fn16(ms_->ctx_, hids_.data(), k, static_cast<const uint16_t *>(d_ids), d_values, kind, n, stream_)
+                                 : fn32(ms_->ctx_, hids_.data(), k, static_cast<const uint32_t *>(d_ids), d_values, kind, n, stream_);
+    check(ms_->ctx_, st, "lh_ingest_keyed_mapped");
+}
+void RecordScope::Counters(const void *d_ids, size_t id_bytes, const uint64_t *d_amounts, size_t n) {
+    if (!ms_) throw std::runtime_error("RecordScope::Counters after End()");
+    if (id_bytes != 2 && id_bytes != 4) throw std::invalid_argument("RecordScope::Counters: id_bytes must be 2 or 4");
+    auto fn16 = lh_counter_add_mapped_u16;
+    auto fn32 = lh_counter_add_mapped_u32;
+    if (id_bytes == 2 ? !fn16 : !fn32) throw std::runtime_error("RecordScope::Counters: this libloghisto_b200 has no mapped counter adds");
+    const uint32_t kc = (uint32_t)cids_.size();
+    lh_status st = id_bytes == 2 ? fn16(ms_->ctx_, cids_.data(), kc, static_cast<const uint16_t *>(d_ids), d_amounts, n, stream_)
+                                 : fn32(ms_->ctx_, cids_.data(), kc, static_cast<const uint32_t *>(d_ids), d_amounts, n, stream_);
+    check(ms_->ctx_, st, "lh_counter_add_mapped");
 }
 
 // ---- graph recorders -------------------------------------------------------------------------------------------
@@ -1706,6 +1733,23 @@ LHMS_API int lhms_scope_histograms(void *ms, const lh_recorder *rec, const uint3
     } catch (const std::exception &e) {
         return scope_status(e);
     }
+}
+// RecordScope::Keyed / Counters (id_bytes 2 or 4: uint16 or uint32 local ids).
+LHMS_API int lhms_scoped_keyed(void *ms, const lh_recorder *rec, uint32_t id_bytes, const void *d_ids, const void *d_values,
+                               uint32_t kind, size_t n) {
+    if (!ms || !rec) return LH_ERR_INVALID;
+    std::lock_guard<std::mutex> lk(g_scopes_mu);
+    auto it = g_scopes.find(std::make_pair(ms, rec->scope));
+    if (it == g_scopes.end()) return LH_ERR_INVALID;
+    try { it->second.Keyed(d_ids, id_bytes, d_values, kind, n); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
+}
+LHMS_API int lhms_scoped_counters(void *ms, const lh_recorder *rec, uint32_t id_bytes, const void *d_ids,
+                                  const uint64_t *d_amounts, size_t n) {
+    if (!ms || !rec) return LH_ERR_INVALID;
+    std::lock_guard<std::mutex> lk(g_scopes_mu);
+    auto it = g_scopes.find(std::make_pair(ms, rec->scope));
+    if (it == g_scopes.end()) return LH_ERR_INVALID;
+    try { it->second.Counters(d_ids, id_bytes, d_amounts, n); return LH_OK; } catch (const std::exception &e) { return scope_status(e); }
 }
 // GPU timers (MetricSystem::StartGpuTimer).  start returns a token, or NULL with *status set; stop may be called
 // repeatedly on `stream` (passed as given: NULL = the context's ingest stream); free releases the token's slot.

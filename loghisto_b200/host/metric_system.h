@@ -152,6 +152,15 @@ class RecordScope {
         uint32_t kind;
     };
     void Histograms(const std::vector<Item> &items);
+    // (local id, value) pairs in device memory on the scope's stream, local id i being histogram name i
+    // (lh_ingest_keyed_mapped_u16 for id_bytes 2, _u32 for 4): values of `kind` as in Histograms.  An id >= the number
+    // of names, or under an unbound name, is dropped and counted in dropped_samples().  Names may repeat.
+    // Throws before anything is issued: std::invalid_argument for id_bytes other than 2 or 4, std::runtime_error when
+    // the scope has ended, the library lacks the call or refuses it (e.g. a misaligned pointer).
+    void Keyed(const void *d_ids, size_t id_bytes, const void *d_values, uint32_t kind, size_t n);
+    // (local id, amount) pairs, local id i being counter name i (lh_counter_add_mapped_*): wrapping uint64 adds; throws
+    // as Keyed.
+    void Counters(const void *d_ids, size_t id_bytes, const uint64_t *d_amounts, size_t n);
     void End();
     bool open() const { return ms_ != nullptr; }
 

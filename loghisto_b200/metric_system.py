@@ -79,6 +79,10 @@ def _bind(L):
     L.lhms_record_ingest_f64.argtypes = [vp, rec, C.c_uint32, vp, C.c_size_t]
     L.lhms_scope_histograms.restype = C.c_int
     L.lhms_scope_histograms.argtypes = [vp, rec, u32p, C.POINTER(vp), C.POINTER(C.c_uint64), u32p, C.c_uint32]
+    L.lhms_scoped_keyed.restype = C.c_int
+    L.lhms_scoped_keyed.argtypes = [vp, rec, C.c_uint32, vp, vp, C.c_uint32, C.c_size_t]
+    L.lhms_scoped_counters.restype = C.c_int
+    L.lhms_scoped_counters.argtypes = [vp, rec, C.c_uint32, vp, vp, C.c_size_t]
     L.lhms_gpu_timer_start.restype = vp
     L.lhms_gpu_timer_start.argtypes = [vp, C.c_char_p, vp, C.POINTER(C.c_int)]
     L.lhms_gpu_timer_stop.restype = C.c_int
@@ -251,6 +255,24 @@ class RecordScope:
         st = self._ms._lib.lhms_scope_histograms(self._ms._h, C.byref(self.recorder), idx, ptrs, ns, kinds, len(pairs))
         if st != 0:
             raise RuntimeError("lhms_scope_histograms failed (status %d)" % st)
+
+    def keyed(self, ids, values):
+        """Histogram(name, values[i]) with name the scope's histogram at position ids[i], for every i, in one call on
+        the scope's stream (lh_ingest_keyed_mapped_*).  ids and values as GraphRecorder.keyed takes them (uint16, int32
+        or uint32 ids; float64 values, or int64 nanoseconds recorded as float64(ns)); TypeError / ValueError before
+        anything is issued.  An id past the names, or under an unbound name, is dropped and counted."""
+        id_bytes, ip, vp, kind, n = graph_keyed_args(ids, values)
+        st = self._ms._lib.lhms_scoped_keyed(self._ms._h, C.byref(self.recorder), id_bytes, ip, vp, kind, n)
+        if st != 0:
+            raise RuntimeError("lhms_scoped_keyed failed (status %d)" % st)
+
+    def counters(self, ids, amounts):
+        """Counter(name, amounts[i]) with name the scope's counter at position ids[i] (lh_counter_add_mapped_*): ids
+        as keyed() takes them, amounts int64 or uint64 (added as uint64 bits, wrapping)."""
+        id_bytes, ip, ap, n = graph_counter_args(ids, amounts)
+        st = self._ms._lib.lhms_scoped_counters(self._ms._h, C.byref(self.recorder), id_bytes, ip, ap, n)
+        if st != 0:
+            raise RuntimeError("lhms_scoped_counters failed (status %d)" % st)
 
     def end(self):
         if self._open:

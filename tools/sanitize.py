@@ -56,6 +56,22 @@ with lh.Engine(device=0, max_histograms=4, max_counters=4) as e:    # few histog
     e.ingest_keyed_f64_u16(ids, d, n)
     red, sp2 = e.snapshot(PS)
     assert int(red.counts.sum()) == n
+with lh.Engine(device=0, max_histograms=64, max_counters=64) as e:  # mapped (record-scope) keyed and counter calls
+    d = e.gen_stream(lh.STREAM_S, n, lh.DEFAULT_SEED)
+    ns = e.gen_stream(lh.STREAM_TIMER_NS, n, lh.DEFAULT_SEED)
+    amt = e.gen_stream(lh.STREAM_AMOUNTS, n, lh.DEFAULT_SEED)
+    ids = e.gen_ids_u16(0, n, 64, lh.DEFAULT_SEED)
+    m = [(i * 7) % 64 for i in range(62)] + [0xFFFFFFFF]       # ids 62 unbound, 63 past the map
+    e.ingest_keyed_mapped_u16(m, ids, d, 0, n)                  # vector body
+    e.ingest_keyed_mapped_u16(m, ids.offset(1), ns.offset(1), 1, n - 1)   # scalar kernel only
+    e.ingest_keyed_mapped_u16(m[:8], ids, d, 0, n)              # shared-memory privatised kernel, most samples dropped
+    e.tune("keyed_mode", 2); e.tune("kp_chunk", 65536)
+    e.ingest_keyed_mapped_u16(m, ids, d, 0, n)                  # write-combining owner kernel
+    e.tune("keyed_mode", 0)
+    e.counter_add_mapped_u16(m, ids, amt, n)
+    e.counter_add_mapped_u16(m, ids.offset(1), amt.offset(1), n - 1)
+    red, _ = e.snapshot(PS)
+    assert int(red.counts.sum()) + e.stats()["dropped"] > 0
 with lh.Engine(device=0, max_histograms=4, max_counters=4) as e:    # graph recorder: batch ingest into its rows, drains
     d = e.gen_stream(lh.STREAM_S, n, lh.DEFAULT_SEED)
     with e.graph_recorder([2, 3, 0xFFFFFFFF], [1]) as g:      # local row 2 unbound: dropped and counted
