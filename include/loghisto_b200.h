@@ -680,6 +680,35 @@ LH_API lh_status lh_snapshot_allreduce(lh_ctx *ctx, uint32_t include_counters, u
 LH_API lh_status lh_comm_allreduce_ms(lh_ctx *ctx, uint64_t seq, float *ms);
 LH_API lh_status lh_comm_info(lh_ctx *ctx, lh_comm_stats *out);
 
+/* ---- multi-GPU by rows: the all-reduce over job-wide rows whose ids differ per rank ---------------------------------
+ * lh_snapshot_allreduce sums row h of every rank into row h.  When each rank keeps a name under its own id (MetricSystem
+ * interns and recycles per rank), the ranks first agree on job-wide rows g and then sum through maps:
+ *
+ *   lh_snapshot_rows  between lh_snapshot_begin and any all-reduce: hist_touched[h] = 1 when histogram row h of the
+ *                     frozen interval holds data (flag != 0), counter_deltas[c] = the frozen counter delta of c, and
+ *                     *frozen = the half of the double buffer this snapshot froze (0 or 1), which the ranks exchange
+ *                     for lh_snapshot_allreduce_rows (any pointer may be NULL).  One D2H on the snapshot stream, behind
+ *                     what lh_snapshot_begin ordered there.  LH_ERR_STATE without a snapshot or after an all-reduce.
+ *   lh_snapshot_allreduce_rows  collective, as lh_snapshot_allreduce, over job-wide rows: rank r contributes its frozen
+ *                     row hist_map[r * n_rows + g] to row g (nothing for LH_ROW_ABSENT), and counter_map[r *
+ *                     n_counter_rows + g] to counter g.  Afterwards the snapshot's reduce, export, publish and
+ *                     lh_snapshot_copy_histogram see job-wide row g at index g, and nothing at or above n_rows
+ *                     (n_counter_rows).  seq and frozen[world] (the buffer each rank froze: 0 or 1) come from the
+ *                     host's own exchange, so every rank uses one agreed sequence number and reads each peer's own
+ *                     frozen half; seq must exceed this context's last all-reduce.  The form (one-shot / two-shot) is
+ *                     chosen from n_rows * (2*win - 1) * 8 bytes.  On failure (lh_comm_info.status != 0) the
+ *                     snapshot holds this rank's own counts through hist_map[rank] / counter_map[rank].  Errors
+ *                     before anything is launched: LH_ERR_STATE without a snapshot or lh_comm_import, LH_ERR_INVALID
+ *                     for n_rows > max_histograms, n_counter_rows > max_counters, a NULL map with rows, a NULL frozen,
+ *                     a frozen[r] > 1, frozen[rank] other than this snapshot's buffer, or seq not above the last,
+ *                     LH_ERR_RANGE for a map entry neither LH_ROW_ABSENT nor below max_histograms (max_counters).
+ */
+#define LH_ROW_ABSENT 0xFFFFFFFFu
+LH_API lh_status lh_snapshot_rows(lh_ctx *ctx, uint8_t *hist_touched, uint64_t *counter_deltas, uint32_t *frozen);
+LH_API lh_status lh_snapshot_allreduce_rows(lh_ctx *ctx, uint64_t seq, const uint32_t *frozen, uint32_t n_rows,
+                                            const uint32_t *hist_map, uint32_t n_counter_rows,
+                                            const uint32_t *counter_map, uint64_t *seq_out);
+
 /* ---- scalar helpers, evaluated ON THE DEVICE (parity probes for tests) --- */
 /* out[i] = compress(values[i]) exactly as the ingest kernels compute it
  * (mode 0: production fast path + exact fallback; mode 1: exact path only) */

@@ -45,6 +45,8 @@ class lh_device_view(C.Structure):
 
 
 LH_PEER_HANDLE_BYTES = 1024
+LH_MAX_RANKS = 16
+LH_ROW_ABSENT = 0xFFFFFFFF   # map entry of lh_snapshot_allreduce_rows: this rank has nothing under that row
 
 
 class lh_comm_stats(C.Structure):
@@ -229,6 +231,8 @@ SIGNATURES = {
     "lh_snapshot_allreduce": (_i32, [_vp, _u32, C.POINTER(_u64)]),
     "lh_comm_allreduce_ms": (_i32, [_vp, _u64, C.POINTER(C.c_float)]),
     "lh_comm_info": (_i32, [_vp, C.POINTER(lh_comm_stats)]),
+    "lh_snapshot_rows": (_i32, [_vp, _vp, _vp, C.POINTER(_u32)]),
+    "lh_snapshot_allreduce_rows": (_i32, [_vp, _u64, _vp, _u32, _vp, _u32, _vp, C.POINTER(_u64)]),
     "lh_keyed_kernel_name": (C.c_char_p, [_vp]),
     "lh_compress_f64": (_i32, [_vp, _vp, _sz, _vp, C.c_int, _vp]),
     "lh_decompress_table": (_i32, [_vp, _vp]),

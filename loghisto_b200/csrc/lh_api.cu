@@ -232,6 +232,13 @@ struct lh_ctx {
     bool comm_two_shot = false;                    // form of the last all-reduce (lh_comm_info's byte count)
     static constexpr int kCommRing = 8;
     cudaEvent_t comm_t0[kCommRing] = {}, comm_t1[kCommRing] = {};
+    // lh_snapshot_allreduce_rows: the row maps ([world][H] then [world][C] uint32, allocated at lh_comm_import), their
+    // pinned staging, and an event behind the last upload (staging is rewritten only after it)
+    uint32_t *d_row_maps = nullptr, *h_row_maps = nullptr;
+    cudaEvent_t row_maps_copied = nullptr;
+    // lh_snapshot_rows: pinned staging of the frozen flags and counters (allocated on first use)
+    uint32_t *h_rows_flags = nullptr;
+    unsigned long long *h_rows_counters = nullptr;
     uint64_t ctx_id = 0;
     // lh_reduce_sparse_host: its own stream and K6_BATCH scratch rows (allocated on first use), serialised by rs_mu;
     // none of the arrays above is touched by it
@@ -985,6 +992,16 @@ lh_status comm_alloc_reduced(lh_ctx *ctx) {
     return LH_OK;
 }
 
+// the row maps of lh_snapshot_allreduce_rows, sized for the largest world
+lh_status comm_alloc_row_maps(lh_ctx *ctx) {
+    if (ctx->d_row_maps) return LH_OK;
+    const size_t bytes = (size_t)kMaxRanks * ((size_t)ctx->H + ctx->C) * 4u;
+    LH_CUDA(ctx, cudaMalloc(&ctx->d_row_maps, bytes));
+    LH_CUDA(ctx, cudaMallocHost(&ctx->h_row_maps, bytes));
+    LH_CUDA(ctx, cudaEventCreateWithFlags(&ctx->row_maps_copied, cudaEventDisableTiming));
+    return LH_OK;
+}
+
 bool is_pinned_or_managed(const void *p) {
     cudaPointerAttributes a;
     if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
@@ -1119,6 +1136,7 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
 
     LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_reduce, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
     LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_peer_allreduce, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
+    LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_peer_allreduce_rows, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
     LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_counter_add_smem<unsigned short, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, K2_SMEM_COUNTERS * 8));
     LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_counter_add_smem<unsigned int, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, K2_SMEM_COUNTERS * 8));
     LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_counter_add_smem_vec<unsigned short, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, K2_SMEM_COUNTERS * 8));
@@ -1183,6 +1201,11 @@ extern "C" lh_status lh_destroy(lh_ctx *ctx) {
     comm_unmap(ctx);
     cudaFree(ctx->d_comm); cudaFree(ctx->d_comm_aux);
     cudaFree(ctx->d_red_buckets); cudaFree(ctx->d_red_flags); cudaFree(ctx->d_red_counters);
+    cudaFree(ctx->d_row_maps);
+    if (ctx->h_row_maps) cudaFreeHost(ctx->h_row_maps);
+    if (ctx->row_maps_copied) cudaEventDestroy(ctx->row_maps_copied);
+    if (ctx->h_rows_flags) cudaFreeHost(ctx->h_rows_flags);
+    if (ctx->h_rows_counters) cudaFreeHost(ctx->h_rows_counters);
     for (int i = 0; i < lh_ctx::kCommRing; i++) {
         if (ctx->comm_t0[i]) cudaEventDestroy(ctx->comm_t0[i]);
         if (ctx->comm_t1[i]) cudaEventDestroy(ctx->comm_t1[i]);
@@ -2705,16 +2728,21 @@ extern "C" lh_status lh_comm_import(lh_ctx *ctx, uint32_t rank, uint32_t world, 
             LH_CUDA(ctx, cudaIpcOpenMemHandle((void **)&pm.red, w.ipc_red, cudaIpcMemLazyEnablePeerAccess));
         }
     }
+    if (lh_status st = comm_alloc_row_maps(ctx)) return st;
     ctx->comm_rank = rank;
     ctx->comm_world = world;
     return LH_OK;
 }
 
-extern "C" lh_status lh_snapshot_allreduce(lh_ctx *ctx, uint32_t include_counters, uint64_t *seq_out) {
-    LH_ENTER(ctx);
-    if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
-    if (ctx->comm_world < 2) return fail(ctx, LH_ERR_STATE, "lh_comm_import has not been called with world >= 2");
-    if (ctx->view_reduced) return fail(ctx, LH_ERR_STATE, "this snapshot has already been all-reduced");
+namespace {
+// The launches of one all-reduce (both forms), with ctx->mu held and every argument checked.  frozen[r]: the buffer
+// rank r froze; n_rows: the histogram rows in play (H for the identity form), which set the payload and the grid.
+void k5_launch(int grid, size_t smem, cudaStream_t s, const PeerParams &p, RowIdentity) { k_peer_allreduce<<<grid, K5_THREADS, smem, s>>>(p); }
+void k5_launch(int grid, size_t smem, cudaStream_t s, const PeerParams &p, const RowMap &m) { k_peer_allreduce_rows<<<grid, K5_THREADS, smem, s>>>(p, m); }
+
+template <typename Rows>
+lh_status launch_allreduce(lh_ctx *ctx, uint64_t seq, const uint32_t *frozen, uint32_t n_rows, uint32_t include_counters,
+                           Rows rows, uint64_t *seq_out) {
     const int f = ctx->active ^ 1;
     cudaStream_t s = ctx->snap_stream;
     // status and cells describe this all-reduce only: zeroed behind the previous one on the same stream
@@ -2722,12 +2750,14 @@ extern "C" lh_status lh_snapshot_allreduce(lh_ctx *ctx, uint32_t include_counter
     PeerParams p{};
     p.rank = ctx->comm_rank; p.world = ctx->comm_world; p.H = ctx->H; p.C = ctx->C; p.win = ctx->pc.win;
     p.do_counters = include_counters ? 1u : 0u; p.frozen = (uint32_t)f;
-    p.seq = ++ctx->comm_seq;
+    p.seq = seq;
+    ctx->comm_seq = seq;
     p.timeout_ns = 10ull * 1000ull * 1000ull * 1000ull;
     for (uint32_t r = 0; r < ctx->comm_world; r++) {
-        p.buckets[r] = ctx->peers[r].buckets[f];
-        p.flags[r] = ctx->peers[r].flags[f];
-        p.counters[r] = ctx->peers[r].counters[f];
+        const int fr = frozen ? (int)frozen[r] : f;
+        p.buckets[r] = ctx->peers[r].buckets[fr];
+        p.flags[r] = ctx->peers[r].flags[fr];
+        p.counters[r] = ctx->peers[r].counters[fr];
         p.comm[r] = ctx->peers[r].comm;
     }
     p.out_buckets = ctx->d_red_buckets; p.out_flags = ctx->d_red_flags; p.out_counters = ctx->d_red_counters;
@@ -2735,14 +2765,14 @@ extern "C" lh_status lh_snapshot_allreduce(lh_ctx *ctx, uint32_t include_counter
     p.cells = reinterpret_cast<unsigned long long *>(ctx->d_comm_aux + 2);
     for (uint32_t r = 0; r < ctx->comm_world; r++) p.out_peer[r] = ctx->peers[r].red;
     // payload = the window cells of every histogram that can be live; above 1 MiB the reduce-scatter + push form wins
-    const size_t payload = (size_t)ctx->H * (2u * ctx->pc.win - 1u) * 8u;
+    const size_t payload = (size_t)n_rows * (2u * ctx->pc.win - 1u) * 8u;
     p.two_shot = payload >= (1u << 20) ? 1u : 0u;
     ctx->comm_two_shot = p.two_shot != 0;
     const int ring = (int)(p.seq % lh_ctx::kCommRing);
     // a few CTAs: the kernel shares the GPU with the next interval's ingest (which leaves k1_reserve_sms SMs free);
     // CTAs that are not resident yet simply start later (no CTA waits for another CTA of its own grid before the end)
-    const size_t items = (size_t)ctx->H * (65536u / K5_CHUNK);
-    int grid = (int)std::min<size_t>(items, ctx->H == 1 ? 5 : 16);
+    const size_t items = (size_t)std::max(1u, n_rows) * (65536u / K5_CHUNK);
+    int grid = (int)std::min<size_t>(items, n_rows <= 1 ? 5 : 16);
     LH_CUDA(ctx, cudaEventRecord(ctx->comm_t0[ring], s));
     if (p.two_shot) {
         // An SM sustains only ~4 GB/s of NVLink loads (measured, tools/peer_probe.py: 36 MB take 9.1 / 2.3 / 0.64 / 0.21 ms
@@ -2752,12 +2782,12 @@ extern "C" lh_status lh_snapshot_allreduce(lh_ctx *ctx, uint32_t include_counter
         // start as those finish.
         PeerParams pa = p;
         pa.arrive_only = 1;
-        k_peer_allreduce<<<1, K5_THREADS, ctx->H, s>>>(pa);
+        k5_launch(1, ctx->H, s, pa, rows);
         LH_CUDA(ctx, cudaGetLastError());
         ctx->stats.kernel_launches++;
-        grid = (int)std::min<size_t>((ctx->H + ctx->comm_world - 1) / ctx->comm_world, (size_t)std::max(1, std::min(128, ctx->sm_count - 20)));
+        grid = (int)std::min<size_t>((n_rows + ctx->comm_world - 1) / ctx->comm_world, (size_t)std::max(1, std::min(128, ctx->sm_count - 20)));
     }
-    k_peer_allreduce<<<grid, K5_THREADS, ctx->H, s>>>(p);
+    k5_launch(grid, ctx->H, s, p, rows);
     LH_CUDA(ctx, cudaGetLastError());
     LH_CUDA(ctx, cudaEventRecord(ctx->comm_t1[ring], s));
     ctx->stats.kernel_launches++;
@@ -2766,6 +2796,76 @@ extern "C" lh_status lh_snapshot_allreduce(lh_ctx *ctx, uint32_t include_counter
     ctx->nnz_valid = false;
     if (seq_out) *seq_out = p.seq;
     return LH_OK;
+}
+}  // namespace
+
+extern "C" lh_status lh_snapshot_allreduce(lh_ctx *ctx, uint32_t include_counters, uint64_t *seq_out) {
+    LH_ENTER(ctx);
+    if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
+    if (ctx->comm_world < 2) return fail(ctx, LH_ERR_STATE, "lh_comm_import has not been called with world >= 2");
+    if (ctx->view_reduced) return fail(ctx, LH_ERR_STATE, "this snapshot has already been all-reduced");
+    return launch_allreduce(ctx, ctx->comm_seq + 1, nullptr, ctx->H, include_counters, RowIdentity{}, seq_out);
+}
+
+extern "C" lh_status lh_snapshot_rows(lh_ctx *ctx, uint8_t *hist_touched, uint64_t *counter_deltas, uint32_t *frozen) {
+    LH_ENTER(ctx);
+    if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
+    if (ctx->view_reduced) return fail(ctx, LH_ERR_STATE, "this snapshot has already been all-reduced");
+    const int f = ctx->active ^ 1;
+    cudaStream_t s = ctx->snap_stream;
+    if (!ctx->h_rows_flags) {
+        LH_CUDA(ctx, cudaMallocHost(&ctx->h_rows_flags, (size_t)ctx->H * 4));
+        LH_CUDA(ctx, cudaMallocHost(&ctx->h_rows_counters, (size_t)ctx->C * 8));
+    }
+    // behind the writer events, the graph drain and the hot-window fold lh_snapshot_begin ordered on this stream
+    if (hist_touched) LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_rows_flags, ctx->buf[f].d_flags, (size_t)ctx->H * 4, cudaMemcpyDeviceToHost, s));
+    if (counter_deltas) LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_rows_counters, ctx->buf[f].d_counters, (size_t)ctx->C * 8, cudaMemcpyDeviceToHost, s));
+    LH_CUDA(ctx, cudaStreamSynchronize(s));
+    if (hist_touched)
+        for (uint32_t h = 0; h < ctx->H; h++) hist_touched[h] = ctx->h_rows_flags[h] != 0;
+    if (counter_deltas) memcpy(counter_deltas, ctx->h_rows_counters, (size_t)ctx->C * 8);
+    if (frozen) *frozen = (uint32_t)f;
+    ctx->stats.d2h_bytes += (hist_touched ? (size_t)ctx->H * 4 : 0) + (counter_deltas ? (size_t)ctx->C * 8 : 0);
+    return LH_OK;
+}
+
+extern "C" lh_status lh_snapshot_allreduce_rows(lh_ctx *ctx, uint64_t seq, const uint32_t *frozen, uint32_t n_rows,
+                                                const uint32_t *hist_map, uint32_t n_counter_rows,
+                                                const uint32_t *counter_map, uint64_t *seq_out) {
+    LH_ENTER(ctx);
+    if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
+    if (ctx->comm_world < 2) return fail(ctx, LH_ERR_STATE, "lh_comm_import has not been called with world >= 2");
+    if (ctx->view_reduced) return fail(ctx, LH_ERR_STATE, "this snapshot has already been all-reduced");
+    const uint32_t W = ctx->comm_world;
+    if (!frozen) return fail(ctx, LH_ERR_INVALID, "frozen is NULL");
+    for (uint32_t r = 0; r < W; r++)
+        if (frozen[r] > 1) return fail(ctx, LH_ERR_INVALID, "frozen[r] is not 0 or 1");
+    if (frozen[ctx->comm_rank] != (uint32_t)(ctx->active ^ 1)) return fail(ctx, LH_ERR_INVALID, "frozen[rank] is not the buffer this snapshot froze");
+    if (n_rows > ctx->H) return fail(ctx, LH_ERR_INVALID, "n_rows > max_histograms");
+    if (n_counter_rows > ctx->C) return fail(ctx, LH_ERR_INVALID, "n_counter_rows > max_counters");
+    if ((n_rows && !hist_map) || (n_counter_rows && !counter_map)) return fail(ctx, LH_ERR_INVALID, "map is NULL with rows");
+    if (seq <= ctx->comm_seq) return fail(ctx, LH_ERR_INVALID, "seq does not exceed this context's last all-reduce");
+    const size_t nh = (size_t)W * n_rows, nc = (size_t)W * n_counter_rows;
+    for (size_t i = 0; i < nh; i++)
+        if (hist_map[i] != LH_ROW_ABSENT && hist_map[i] >= ctx->H) return fail(ctx, LH_ERR_RANGE, "histogram map entry >= max_histograms");
+    for (size_t i = 0; i < nc; i++)
+        if (counter_map[i] != LH_ROW_ABSENT && counter_map[i] >= ctx->C) return fail(ctx, LH_ERR_RANGE, "counter map entry >= max_counters");
+    if (lh_status st = comm_alloc_row_maps(ctx)) return st;
+    // the staging is rewritten only after the previous upload from it has run
+    LH_CUDA(ctx, cudaEventSynchronize(ctx->row_maps_copied));
+    if (nh) memcpy(ctx->h_row_maps, hist_map, nh * 4);
+    if (nc) memcpy(ctx->h_row_maps + nh, counter_map, nc * 4);
+    cudaStream_t s = ctx->snap_stream;
+    if (nh + nc) {
+        LH_CUDA(ctx, cudaMemcpyAsync(ctx->d_row_maps, ctx->h_row_maps, (nh + nc) * 4, cudaMemcpyHostToDevice, s));
+        ctx->stats.h2d_bytes += (nh + nc) * 4;
+    }
+    LH_CUDA(ctx, cudaEventRecord(ctx->row_maps_copied, s));
+    RowMap m{};
+    m.hist = ctx->d_row_maps; m.ctr = ctx->d_row_maps + nh;
+    m.n_rows = n_rows; m.n_counter_rows = n_counter_rows;
+    for (uint32_t r = 0; r < W; r++) m.frozen_mask |= frozen[r] << r;
+    return launch_allreduce(ctx, seq, frozen, n_rows, 1u, m, seq_out);
 }
 
 extern "C" lh_status lh_comm_allreduce_ms(lh_ctx *ctx, uint64_t seq, float *ms) {

@@ -1707,9 +1707,120 @@ __device__ __forceinline__ bool wait_token(const unsigned long long *slot, unsig
     }
 }
 
-__global__ void __launch_bounds__(K5_THREADS, 1)
-k_peer_allreduce(PeerParams p) {
-    extern __shared__ unsigned char s_level[];               // [H]: OR over ranks of the histogram's flag
+// Row policy of K5 (its last template parameter and argument).  RowIdentity: row h of every rank sums into row h
+// (lh_snapshot_allreduce).  RowMap: job-wide rows g < n_rows (lh_snapshot_allreduce_rows): rank r contributes its
+// frozen row hist[r * n_rows + g], or nothing for LH_ROW_ABSENT; counters alike over n_counter_rows.  Everything the
+// kernel iterates (flag OR, sums, two-shot ownership, pushes) is over g, and the reduced arrays are indexed by g on
+// every rank.  The maps live in device memory (up to 16 x 4 096 entries: too large for the parameter block).
+struct RowIdentity {};
+struct RowMap {
+    const uint32_t *hist;          // [world][n_rows]
+    const uint32_t *ctr;           // [world][n_counter_rows]
+    uint32_t n_rows, n_counter_rows;
+    uint32_t frozen_mask;          // bit r: the buffer rank r froze (announced in its token)
+};
+constexpr uint32_t K5_ROW_ABSENT = 0xFFFFFFFFu;
+
+// Step 3 of K5 over job-wide rows: the identity form's sums with every row address taken through the maps.  ok false
+// (a peer did not arrive, or froze another half than announced): this rank alone, through its own map.
+__device__ __forceinline__ void k5_sum_mapped(const PeerParams &p, const RowMap &m, bool ok, unsigned char *s_level,
+                                              unsigned long long *s_cells) {
+    const uint32_t t = threadIdx.x;
+    const uint32_t r0 = ok ? 0u : p.rank, r1 = ok ? p.world : p.rank + 1u;
+    const bool push = ok && p.two_shot;
+    const uint32_t wcells = 2u * p.win - 1u;
+    const uint32_t n = m.n_rows;
+    constexpr uint32_t PER_H = 65536u / K5_CHUNK;
+    const uint32_t chunks_w = (wcells + K5_CHUNK - 1) / K5_CHUNK;
+    unsigned long long cells = 0;
+    for (uint32_t g = t; g < n; g += K5_THREADS) {
+        uint32_t lv = 0;
+        for (uint32_t r = r0; r < r1; r++) {
+            const uint32_t h = __ldg(m.hist + (size_t)r * n + g);
+            if (h != K5_ROW_ABSENT) lv |= ld_sys_u32(p.flags[r] + h);
+        }
+        s_level[g] = (unsigned char)lv;
+        if (blockIdx.x == 0 && lv) { p.out_flags[g] = lv; cells += (lv & 2u) ? 65536u : wcells; }
+    }
+    if (blockIdx.x == 0 && cells) atomicAdd(s_cells, cells);
+    __syncthreads();
+    if (ok && blockIdx.x == 0 && t == 0) *p.cells = *s_cells;
+    if (!push) {
+        const size_t nitems = (size_t)n * PER_H;
+        for (size_t item = blockIdx.x; item < nitems; item += gridDim.x) {
+            const uint32_t g = (uint32_t)(item / PER_H), chunk = (uint32_t)(item % PER_H);
+            const uint32_t level = s_level[g];
+            if (level == 0) continue;
+            const bool dense = (level & 2u) != 0;
+            if (!dense && chunk >= chunks_w) continue;
+            const uint32_t ncell = dense ? 65536u : wcells;
+            constexpr int K = K5_CHUNK / K5_THREADS;
+#pragma unroll
+            for (int k = 0; k < K; k++) {
+                const uint32_t i = chunk * K5_CHUNK + k * K5_THREADS + t;
+                if (i >= ncell) continue;
+                const uint32_t c = dense ? i : window_cell(i, p.win);
+                unsigned long long sum = 0;
+                for (uint32_t r = r0; r < r1; r++) {
+                    const uint32_t h = __ldg(m.hist + (size_t)r * n + g);
+                    if (h != K5_ROW_ABSENT) sum += ld_peer_u64(p.buckets[r] + (size_t)h * 65536u + c);
+                }
+                if (sum) p.out_buckets[(size_t)g * 65536u + c] = sum;
+            }
+        }
+    } else {
+        // two-shot: a rank owns the rows g = rank (mod world); as the identity form, K5_DEEP cells x world loads in
+        // flight per thread
+        for (uint32_t g = p.rank + blockIdx.x * p.world; g < n; g += gridDim.x * p.world) {
+            const uint32_t level = s_level[g];
+            if (level == 0) continue;
+            const bool dense = (level & 2u) != 0;
+            const uint32_t ncell = dense ? 65536u : wcells;
+            for (uint32_t base = 0; base < ncell; base += K5_DEEP * K5_THREADS) {
+                uint32_t cell[K5_DEEP];                  // cell index inside a row
+                unsigned long long sum[K5_DEEP];
+#pragma unroll
+                for (int k = 0; k < K5_DEEP; k++) {
+                    const uint32_t i = base + k * K5_THREADS + t;
+                    cell[k] = i < ncell ? (dense ? i : window_cell(i, p.win)) : 0xFFFFFFFFu;
+                    sum[k] = 0;
+                }
+#pragma unroll 4
+                for (uint32_t r = 0; r < p.world; r++) {
+                    const uint32_t h = __ldg(m.hist + (size_t)r * n + g);
+                    if (h == K5_ROW_ABSENT) continue;
+                    const unsigned long long *src = p.buckets[r] + (size_t)h * 65536u;
+#pragma unroll
+                    for (int k = 0; k < K5_DEEP; k++)
+                        if (cell[k] != 0xFFFFFFFFu) sum[k] += ld_peer_u64(src + cell[k]);
+                }
+#pragma unroll
+                for (int k = 0; k < K5_DEEP; k++) {
+                    if (cell[k] == 0xFFFFFFFFu || sum[k] == 0) continue;
+                    for (uint32_t r = 0; r < p.world; r++) p.out_peer[r][(size_t)g * 65536u + cell[k]] = sum[k];
+                }
+            }
+        }
+    }
+    if (p.do_counters && blockIdx.x == 0) {
+        const uint32_t nc = m.n_counter_rows;
+        for (uint32_t i = t; i < p.C; i += K5_THREADS) {
+            unsigned long long sum = 0;
+            if (i < nc)
+                for (uint32_t r = r0; r < r1; r++) {
+                    const uint32_t c = __ldg(m.ctr + (size_t)r * nc + i);
+                    if (c != K5_ROW_ABSENT) sum += ld_sys_u64(p.counters[r] + c);
+                }
+            p.out_counters[i] = sum;
+        }
+    }
+    if (push) __threadfence_system();
+}
+
+// The body of both K5 kernels.  They are separate __global__ functions, not one template: a template kernel takes the
+// module's largest dynamic shared-memory alignment, which moved the identity form's s_level.
+template <typename Rows>
+__device__ __forceinline__ void k5_body(PeerParams p, Rows rows, unsigned char *s_level) {
     __shared__ unsigned long long s_cells;
     const uint32_t t = threadIdx.x;
     const unsigned long long token = p.seq * 2ull + p.frozen;
@@ -1723,12 +1834,17 @@ k_peer_allreduce(PeerParams p) {
     if (t < p.world && t != p.rank) {
         unsigned long long seen = 0;
         if (!wait_token(mine + t, token, p.timeout_ns, &seen)) atomicMax(p.status, 1u);
-        else if ((seen >> 1) == p.seq && (seen & 1ull) != p.frozen) atomicMax(p.status, 2u);
+        else if constexpr (std::is_same<Rows, RowMap>::value) {
+            if ((seen >> 1) == p.seq && (seen & 1ull) != ((rows.frozen_mask >> t) & 1u)) atomicMax(p.status, 2u);
+        } else if ((seen >> 1) == p.seq && (seen & 1ull) != p.frozen) atomicMax(p.status, 2u);
     }
     if (p.arrive_only) return;
     if (t == 0) s_cells = 0;
     __syncthreads();
     const bool ok = ld_sys_u32(p.status) == 0;
+    if constexpr (std::is_same<Rows, RowMap>::value) {
+        k5_sum_mapped(p, rows, ok, s_level, &s_cells);
+    } else
     // 3. sum.  Work item = (histogram, chunk of K5_CHUNK cells); the set of cells follows the OR of all ranks' flags.
     //    one-shot (small payload): every rank sums every item into its own array - one NVLink round trip.
     //    two-shot (large payload): the rank that owns an item sums it and pushes the sum into every rank's array, so a
@@ -1832,6 +1948,18 @@ k_peer_allreduce(PeerParams p) {
         unsigned long long seen = 0;
         if (!wait_token(mine + LH_MAX_RANKS + t, token, p.timeout_ns, &seen)) atomicMax(p.status, 1u);
     }
+}
+
+__global__ void __launch_bounds__(K5_THREADS, 1)
+k_peer_allreduce(PeerParams p) {
+    extern __shared__ unsigned char s_level[];               // [H]: OR over ranks of the histogram's flag
+    k5_body(p, RowIdentity{}, s_level);
+}
+
+__global__ void __launch_bounds__(K5_THREADS, 1)
+k_peer_allreduce_rows(PeerParams p, RowMap rows) {
+    extern __shared__ unsigned char s_level[];               // [n_rows]: OR over ranks of the row's flag
+    k5_body(p, rows, s_level);
 }
 
 // ----------------------------------------------------------- batch ingest (lh_ingest_batch)

@@ -183,3 +183,21 @@ class ShardedEngine:
         if self.collective == "peer":
             return self.engine.comm_last_bytes()
         return self._bytes
+
+
+def rank_allgather(group=None):
+    """The all-gather MetricSystem.join_ranks takes, over a torch.distributed process group:
+    allgather(bytes) -> list[bytes] of every rank in rank order, through dist.all_gather_object.
+
+    Pass a dedicated gloo group, made on every rank with `dist.new_group(backend="gloo")`.  The reaper exchanges
+    names at every collection from its own thread; on the group the training loop uses, those exchanges would
+    interleave with the loop's collectives and hang both.  The ranks of the group are the ranks given to join_ranks.
+    """
+    import torch.distributed as dist
+
+    def allgather(mine: bytes) -> list:
+        out = [None] * dist.get_world_size(group)
+        dist.all_gather_object(out, bytes(mine), group=group)
+        return [bytes(b) for b in out]
+
+    return allgather

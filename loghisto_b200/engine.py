@@ -634,6 +634,28 @@ class Engine:
         self._check(self.lib.lh_snapshot_allreduce(self.h, 1 if counters else 0, C.byref(seq)))
         return int(seq.value)
 
+    def snapshot_rows(self):
+        """lh_snapshot_rows: (touched uint8[H], counter deltas uint64[C], frozen half) of the frozen interval."""
+        touched = np.zeros(self.H, np.uint8)
+        deltas = np.zeros(self.C, np.uint64)
+        frozen = C.c_uint32()
+        self._check(self.lib.lh_snapshot_rows(self.h, touched.ctypes.data, deltas.ctypes.data, C.byref(frozen)))
+        return touched, deltas, int(frozen.value)
+
+    def snapshot_allreduce_rows(self, seq: int, frozen, hist_map, counter_map) -> int:
+        """lh_snapshot_allreduce_rows: hist_map / counter_map are [world][rows] arrays of frozen rows (LH_ROW_ABSENT for
+        none), frozen[r] the buffer rank r froze."""
+        fr = np.ascontiguousarray(frozen, dtype=np.uint32)
+        hm = np.ascontiguousarray(hist_map, dtype=np.uint32)
+        cm = np.ascontiguousarray(counter_map, dtype=np.uint32)
+        n_rows = hm.shape[1] if hm.ndim == 2 else 0
+        n_counter_rows = cm.shape[1] if cm.ndim == 2 else 0
+        out = C.c_uint64()
+        self._check(self.lib.lh_snapshot_allreduce_rows(self.h, seq, fr.ctypes.data, n_rows, hm.ctypes.data if n_rows else None,
+                                                        n_counter_rows, cm.ctypes.data if n_counter_rows else None,
+                                                        C.byref(out)))
+        return int(out.value)
+
     def comm_allreduce_ms(self, seq: int) -> float:
         ms = C.c_float()
         self._check(self.lib.lh_comm_allreduce_ms(self.h, seq, C.byref(ms)))

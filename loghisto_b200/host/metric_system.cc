@@ -58,6 +58,13 @@
 #pragma weak lh_raw_board_destroy
 // And for device gauges: over a build without them, RegisterDeviceGauge throws.
 #pragma weak lh_gauges_read
+// And for joined ranks: over a build without them, JoinRanks throws.
+#pragma weak lh_comm_export
+#pragma weak lh_comm_import
+#pragma weak lh_comm_info
+#pragma weak lh_snapshot_copy_histogram
+#pragma weak lh_snapshot_rows
+#pragma weak lh_snapshot_allreduce_rows
 
 namespace loghisto {
 
@@ -1179,6 +1186,183 @@ uint64_t MetricSystem::dropped_samples() {
     return d;
 }
 
+// ---- joined ranks ------------------------------------------------------------------------------------------------
+namespace {
+void put_u32(std::string &b, uint32_t v) { b.append(reinterpret_cast<const char *>(&v), 4); }
+void put_u64(std::string &b, uint64_t v) { b.append(reinterpret_cast<const char *>(&v), 8); }
+struct Reader {
+    const std::string &b;
+    size_t at = 0;
+    void need(size_t n) {
+        if (b.size() - at < n) throw std::runtime_error("truncated rank payload");
+    }
+    uint32_t u32() { need(4); uint32_t v; memcpy(&v, b.data() + at, 4); at += 4; return v; }
+    uint64_t u64() { need(8); uint64_t v; memcpy(&v, b.data() + at, 8); at += 8; return v; }
+    std::string str() { const uint32_t n = u32(); need(n); std::string v = b.substr(at, n); at += n; return v; }
+};
+constexpr uint32_t kJoinMagic = 0x4C48524Bu;   // first exchange: handle + shape
+constexpr uint32_t kRowsMagic = 0x4C485253u;   // per collection: sequence, frozen half, touched names
+}  // namespace
+
+void MetricSystem::JoinRanks(uint32_t rank, uint32_t world, AllGather allgather) {
+    if (!lh_comm_export || !lh_comm_import || !lh_comm_info || !lh_snapshot_copy_histogram || !lh_snapshot_rows ||
+        !lh_snapshot_allreduce_rows)
+        throw std::runtime_error("JoinRanks: this libloghisto_b200 has no row-mapped all-reduce");
+    if (world < 2 || world > LH_MAX_RANKS || rank >= world)
+        throw std::invalid_argument("JoinRanks: need 2 <= world <= LH_MAX_RANKS and rank < world");
+    if (!allgather) throw std::invalid_argument("JoinRanks: allgather is empty");
+    std::lock_guard<std::mutex> snap(snapshot_mu_);
+    if (collected_) throw std::runtime_error("JoinRanks on a system that has collected already");
+    if (allgather_) throw std::runtime_error("JoinRanks on a system that has joined already");
+    lh_peer_handle mine{};
+    check(ctx_, lh_comm_export(ctx_, &mine), "lh_comm_export");
+    std::string b;
+    put_u32(b, kJoinMagic);
+    put_u32(b, opt_.max_histograms); put_u32(b, opt_.max_counters); put_u32(b, opt_.precision);
+    b.append(reinterpret_cast<const char *>(mine.bytes), sizeof mine.bytes);
+    const std::vector<std::string> all = allgather(b);
+    if (all.size() != world) throw std::runtime_error("JoinRanks: allgather returned a list of the wrong size");
+    std::vector<lh_peer_handle> handles(world);
+    for (uint32_t r = 0; r < world; r++) {   // every rank checks the same payloads: all refuse alike
+        if (all[r].size() != b.size()) throw std::invalid_argument("JoinRanks: a rank's payload is malformed");
+        Reader rd{all[r]};
+        if (rd.u32() != kJoinMagic) throw std::invalid_argument("JoinRanks: a rank's payload is malformed");
+        const uint32_t h = rd.u32(), c = rd.u32(), p = rd.u32();
+        if (h != opt_.max_histograms || c != opt_.max_counters || p != opt_.precision)
+            throw std::invalid_argument("JoinRanks: the ranks differ in max_histograms, max_counters or precision");
+        memcpy(handles[r].bytes, all[r].data() + rd.at, sizeof handles[r].bytes);
+    }
+    check(ctx_, lh_comm_import(ctx_, rank, world, handles.data()), "lh_comm_import");
+    allgather_ = std::move(allgather);
+    std::lock_guard<std::mutex> lk(ranks_mu_);
+    ranks_.rank = rank;
+    ranks_.world = world;
+}
+
+MetricSystem::RanksState MetricSystem::RanksInfo() {
+    std::lock_guard<std::mutex> lk(ranks_mu_);
+    return ranks_;
+}
+
+// What the exchange of one collection decided: the job-wide rows and, for recycling, this rank's own interval.
+struct MetricSystem::JobRows {
+    std::vector<uint8_t> hist_touched;          // [H] this rank's frozen rows with data
+    std::vector<uint64_t> counter_deltas;       // [C] this rank's frozen counter deltas
+    std::vector<std::string> hnames, cnames;    // job-wide row g -> name
+};
+
+// Steps between lh_snapshot_begin and the reduction of a joined system's collection: lh_snapshot_rows, one exchange,
+// the unions, the maps, lh_snapshot_allreduce_rows.  False when the exchange failed (nothing was launched: the
+// collection is this rank's own).  counter_touched: the host's touched marks (Counter(name, 0) is in Rates).
+bool MetricSystem::join_collection(JobRows &j, const std::vector<uint8_t> &counter_touched) {
+    const uint32_t H = opt_.max_histograms, Cn = opt_.max_counters;
+    const uint32_t rank = ranks_.rank, world = ranks_.world;
+    j.hist_touched.assign(H, 0);
+    j.counter_deltas.assign(Cn, 0);
+    uint32_t frozen = 0;
+    check(ctx_, lh_snapshot_rows(ctx_, j.hist_touched.data(), j.counter_deltas.data(), &frozen), "lh_snapshot_rows");
+    lh_comm_stats cs{};
+    check(ctx_, lh_comm_info(ctx_, &cs), "lh_comm_info");
+    std::vector<std::pair<uint32_t, std::string>> mine_h, mine_c;
+    {
+        std::shared_lock<std::shared_mutex> rl(histos_.mu);
+        for (uint32_t h = 0; h < H && h < histos_.names.size(); h++)
+            if (j.hist_touched[h]) mine_h.emplace_back(h, histos_.names[h]);
+    }
+    {
+        std::shared_lock<std::shared_mutex> rl(counters_.mu);
+        for (uint32_t c = 0; c < Cn && c < counters_.names.size(); c++)
+            if (j.counter_deltas[c] || counter_touched[c]) mine_c.emplace_back(c, counters_.names[c]);
+    }
+    std::string b;
+    put_u32(b, kRowsMagic);
+    put_u64(b, cs.allreduces);
+    put_u32(b, frozen);
+    put_u32(b, (uint32_t)mine_h.size());
+    for (auto &e : mine_h) { put_u32(b, e.first); put_u32(b, (uint32_t)e.second.size()); b += e.second; }
+    put_u32(b, (uint32_t)mine_c.size());
+    for (auto &e : mine_c) { put_u32(b, e.first); put_u32(b, (uint32_t)e.second.size()); b += e.second; }
+
+    std::vector<uint64_t> seqs(world);
+    std::vector<uint32_t> frozens(world);
+    std::vector<std::vector<std::pair<uint32_t, std::string>>> hs(world), cs_(world);
+    try {
+        const std::vector<std::string> all = allgather_(b);
+        if (all.size() != world) throw std::runtime_error("allgather returned a list of the wrong size");
+        for (uint32_t r = 0; r < world; r++) {
+            Reader rd{all[r]};
+            if (rd.u32() != kRowsMagic) throw std::runtime_error("a rank's payload is malformed");
+            seqs[r] = rd.u64();
+            frozens[r] = rd.u32();
+            if (frozens[r] > 1) throw std::runtime_error("a rank's payload is malformed");
+            for (auto *list : {&hs[r], &cs_[r]}) {
+                const uint32_t n = rd.u32();
+                const uint32_t bound = list == &hs[r] ? H : Cn;
+                for (uint32_t i = 0; i < n; i++) {
+                    const uint32_t id = rd.u32();
+                    if (id >= bound) throw std::runtime_error("a rank's payload is malformed");
+                    list->emplace_back(id, rd.str());
+                }
+            }
+        }
+    } catch (const std::exception &e) {
+        std::lock_guard<std::mutex> lk(ranks_mu_);
+        ranks_.status = 3;
+        ranks_.bytes_from_peers = 0;
+        if (!exchange_logged_) {
+            exchange_logged_ = true;
+            fprintf(stderr, "loghisto: rank %u: the collection's exchange failed (%s); collecting this rank alone\n",
+                    rank, e.what());
+        }
+        return false;
+    }
+    // job-wide rows: the byte-sorted union of each list, cut at the bound
+    auto unite = [&](const std::vector<std::vector<std::pair<uint32_t, std::string>>> &per, uint32_t bound,
+                     std::vector<std::string> &names, std::vector<uint32_t> &map) {
+        std::vector<std::string> u;
+        for (auto &l : per) for (auto &e : l) u.push_back(e.second);
+        std::sort(u.begin(), u.end());
+        u.erase(std::unique(u.begin(), u.end()), u.end());
+        const uint64_t dropped_names = u.size() > bound ? u.size() - bound : 0;
+        if (u.size() > bound) u.resize(bound);
+        std::unordered_map<std::string, uint32_t> row;
+        for (uint32_t g = 0; g < u.size(); g++) row.emplace(u[g], g);
+        map.assign((size_t)world * u.size(), LH_ROW_ABSENT);
+        for (uint32_t r = 0; r < world; r++)
+            for (auto &e : per[r]) {
+                auto it = row.find(e.second);
+                if (it != row.end()) map[(size_t)r * u.size() + it->second] = e.first;
+            }
+        names = std::move(u);
+        return dropped_names;
+    };
+    std::vector<uint32_t> hmap, cmap;
+    const uint64_t dropped_names = unite(hs, H, j.hnames, hmap) + unite(cs_, Cn, j.cnames, cmap);
+    if (dropped_names) {   // count what this rank recorded under the names left out (rare: the union is over the bound)
+        std::unordered_map<std::string, uint32_t> kept;
+        for (auto &n : j.hnames) kept.emplace(n, 0);
+        std::vector<uint64_t> row(65536);
+        for (auto &e : mine_h)
+            if (!kept.count(e.second)) {
+                check(ctx_, lh_snapshot_copy_histogram(ctx_, e.first, row.data()), "lh_snapshot_copy_histogram");
+                uint64_t n = 0;
+                for (uint64_t v : row) n += v;
+                dropped_over_limit_.fetch_add(n, std::memory_order_relaxed);
+            }
+        kept.clear();
+        for (auto &n : j.cnames) kept.emplace(n, 0);
+        for (auto &e : mine_c)
+            if (!kept.count(e.second)) dropped_over_limit_.fetch_add(j.counter_deltas[e.first], std::memory_order_relaxed);
+    }
+    const uint64_t seq = *std::max_element(seqs.begin(), seqs.end()) + 1;
+    check(ctx_, lh_snapshot_allreduce_rows(ctx_, seq, frozens.data(), (uint32_t)j.hnames.size(), hmap.data(),
+                                           (uint32_t)j.cnames.size(), cmap.data(), nullptr),
+          "lh_snapshot_allreduce_rows");
+    std::lock_guard<std::mutex> lk(ranks_mu_);
+    ranks_.names_dropped += dropped_names;
+    return true;
+}
+
 // collectRawMetrics, metrics.go:420-479.
 std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
     {   // lh_snapshot_begin would refuse the call after the flush below; refuse it before anything moves
@@ -1187,6 +1371,7 @@ std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
             throw std::runtime_error("collectRawMetrics from a thread that holds an open record scope");
     }
     std::lock_guard<std::mutex> snap(snapshot_mu_);
+    collected_ = true;
     auto raw = std::make_shared<RawMetricSet>();
     const int64_t now = std::chrono::duration_cast<std::chrono::nanoseconds>(
                             std::chrono::system_clock::now().time_since_epoch()).count();
@@ -1224,32 +1409,49 @@ std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
     std::vector<double> sums(H), avgs(H), pvals((size_t)H * np);
     std::vector<int32_t> pkeys((size_t)H * np);
     lh_sparse sp{};
+    JobRows job;
+    bool joined = false;
     try {
+        if (allgather_) {
+            joined = join_collection(job, touched);
+        }
         check(ctx_, lh_snapshot_reduce(ctx_, ps.data(), np, counts.data(), sums.data(), avgs.data(), pkeys.data(), pvals.data()),
               "lh_snapshot_reduce");
         check(ctx_, lh_snapshot_export(ctx_, &sp), "lh_snapshot_export");
+        if (joined) {
+            lh_comm_stats cs{};
+            check(ctx_, lh_comm_info(ctx_, &cs), "lh_comm_info");
+            std::lock_guard<std::mutex> lk(ranks_mu_);
+            ranks_.status = cs.status;
+            ranks_.bytes_from_peers = cs.last_bytes_from_peers;
+            if (cs.status == 0) ranks_.summed++;
+        }
     } catch (...) {
         lh_snapshot_end(ctx_);
         throw;
     }
     // Label the export with the id -> name tables as they stand (retiring ids included), then step every id's
     // lifecycle (NameTable), each under its table's write lock.  A name interned since lh_snapshot_begin has no data
-    // in this export.
+    // in this export.  Joined, the export's rows are the job-wide ones, and each id's lifecycle follows this rank's
+    // own interval (lh_snapshot_rows).
     std::vector<std::string> hnames, cnames;
     {
         std::unique_lock<std::shared_mutex> wl(histos_.mu);
-        hnames = histos_.names;
-        std::vector<uint8_t> landed(hnames.size());
-        for (size_t h = 0; h < hnames.size(); h++) landed[h] = sp.offsets[h] != sp.offsets[h + 1];
+        hnames = joined ? job.hnames : histos_.names;
+        std::vector<uint8_t> landed(histos_.names.size());
+        for (size_t h = 0; h < landed.size(); h++)
+            landed[h] = joined ? job.hist_touched[h] != 0 : sp.offsets[h] != sp.offsets[h + 1];
         recycle(histos_, landed);
     }
     {
         std::unique_lock<std::shared_mutex> wl(counters_.mu);
-        cnames = counters_.names;
-        std::vector<uint8_t> landed(cnames.size());
-        for (size_t c = 0; c < cnames.size(); c++) landed[c] = sp.counter_deltas[c] != 0 || touched[c];
+        cnames = joined ? job.cnames : counters_.names;
+        std::vector<uint8_t> landed(counters_.names.size());
+        for (size_t c = 0; c < landed.size(); c++)
+            landed[c] = (joined ? job.counter_deltas[c] : sp.counter_deltas[c]) != 0 || touched[c];
         recycle(counters_, landed);
     }
+    if (joined) touched.assign(cnames.size(), 1);   // every job-wide counter row was touched on some rank
     // histograms: present only when touched this interval (the swapped-out cache only holds touched names)
     for (size_t h = 0; h < hnames.size(); h++) {
         if (sp.offsets[h] == sp.offsets[h + 1]) continue;
@@ -1632,6 +1834,55 @@ LHMS_API int lhms_collect_and_process(void *ms, lhms_emit_fn emit, void *ctx, ch
         if (err && errlen > 0) snprintf(err, (size_t)errlen, "%s", e.what());
         return -1;
     }
+}
+// MetricSystem::JoinRanks with a C all-gather: allgather(user, mine, len, sink, sink_ctx) calls sink(sink_ctx, r, p,
+// len) once for every rank r with that rank's bytes (the library copies them during the call) and returns 0, or
+// nonzero on failure.  It is called on the collecting thread.  Returns 0, -1 with err filled, or -2 with err filled
+// when the arguments or the ranks' configurations do not fit (std::invalid_argument).
+typedef void (*lhms_ranks_sink_fn)(void *sink_ctx, uint32_t rank, const void *p, uint64_t len);
+typedef int (*lhms_ranks_allgather_fn)(void *user, const void *mine, uint64_t len, lhms_ranks_sink_fn sink, void *sink_ctx);
+namespace {
+struct GatherSink {
+    std::vector<std::string> parts;
+    std::vector<uint8_t> seen;
+};
+void gather_sink(void *sink_ctx, uint32_t rank, const void *p, uint64_t len) {
+    auto *g = static_cast<GatherSink *>(sink_ctx);
+    if (rank >= g->parts.size() || (len && !p)) return;
+    g->parts[rank].assign(static_cast<const char *>(p), (size_t)len);
+    g->seen[rank] = 1;
+}
+}  // namespace
+LHMS_API int lhms_ranks_join(void *ms, uint32_t rank, uint32_t world, lhms_ranks_allgather_fn allgather, void *user,
+                             char *err, int errlen) {
+    try {
+        if (!ms || !allgather) throw std::invalid_argument("lhms_ranks_join: NULL system or allgather");
+        auto fn = [allgather, user, world](const std::string &mine) {
+            GatherSink g;
+            g.parts.resize(world);
+            g.seen.assign(world, 0);
+            if (allgather(user, mine.data(), mine.size(), gather_sink, &g) != 0)
+                throw std::runtime_error("the all-gather callback failed");
+            for (uint32_t r = 0; r < world; r++)
+                if (!g.seen[r]) throw std::runtime_error("the all-gather callback left a rank out");
+            return g.parts;
+        };
+        static_cast<MetricSystem *>(ms)->JoinRanks(rank, world, fn);
+        return 0;
+    } catch (const std::invalid_argument &e) {
+        if (err && errlen > 0) snprintf(err, (size_t)errlen, "%s", e.what());
+        return -2;
+    } catch (const std::exception &e) {
+        if (err && errlen > 0) snprintf(err, (size_t)errlen, "%s", e.what());
+        return -1;
+    }
+}
+// MetricSystem::RanksInfo: out[0..5] = rank, world, status, collections summed, bytes from peers, names dropped.
+LHMS_API void lhms_ranks_info(void *ms, uint64_t *out) {
+    if (!ms || !out) return;
+    const MetricSystem::RanksState r = static_cast<MetricSystem *>(ms)->RanksInfo();
+    out[0] = r.rank; out[1] = r.world; out[2] = r.status; out[3] = r.summed; out[4] = r.bytes_from_peers;
+    out[5] = r.names_dropped;
 }
 // processMetrics(raw) for a RawMetricSet built from flat arrays (a set this system did not collect): histogram i is
 // entries [offsets[i], offsets[i+1]) of keys / counts (repeated keys are summed).  Emits the processed metrics.

@@ -429,6 +429,35 @@ class MetricSystem {
     // to a failed staging call.  Never silent.
     uint64_t dropped_samples();
 
+    // Joins the systems of a multi-GPU job (one system per GPU, e.g. one per torchrun rank) so that each collection
+    // describes the whole job.  Collective: every rank calls it once, with its rank, the world size (2 ..
+    // LH_MAX_RANKS) and an all-gather, before its first collection.  allgather(mine) returns every rank's bytes in rank
+    // order and throws on failure; it is the only way the systems talk to each other, so any transport works
+    // (torch.distributed, MPI, a barrier between threads).  It runs on the collecting thread (the reaper's, once
+    // Start()ed).  Throws std::invalid_argument, on every rank alike and before anything is mapped, when the ranks'
+    // max_histograms, max_counters or precision differ, and std::runtime_error when the system has collected already,
+    // has joined already, or the library lacks lh_snapshot_rows / lh_snapshot_allreduce_rows.
+    //
+    // At each collection of a joined system the ranks exchange the names of the histograms and counters their
+    // interval touched, agree on the byte-sorted union of each (the first max_histograms / max_counters names of it;
+    // samples and counter amounts under the rest are counted in dropped_samples() on the ranks that recorded them),
+    // and one peer-memory all-reduce sums every name's rows wherever each rank keeps them.  Then Histograms, Rates,
+    // Counters, the aggregates of processMetrics, and processed and raw device subscriptions are job-wide and the same
+    // on every rank.  Gauges (functions and device gauges) stay rank-local.  Name ids stay per rank: each rank
+    // recycles them from its own interval, exactly as unjoined.  When the exchange fails on a rank, that rank's
+    // collection is its own interval alone (RanksInfo().status 3, logged once); ranks whose exchange succeeded give up
+    // on it after the all-reduce's 10 s timeout and keep their own counts (status 1).
+    using AllGather = std::function<std::vector<std::string>(const std::string &mine)>;
+    void JoinRanks(uint32_t rank, uint32_t world, AllGather allgather);
+    struct RanksState {
+        uint32_t rank = 0, world = 0;   // world 0: not joined
+        uint32_t status = 0;            // last collection: 0 summed, 1 / 2 as lh_comm_stats, 3 exchange failed
+        uint64_t summed = 0;            // collections summed across the ranks
+        uint64_t bytes_from_peers = 0;  // of the last collection's all-reduce
+        uint64_t names_dropped = 0;     // names left out of the job-wide union by the bounds, over all collections
+    };
+    RanksState RanksInfo();
+
  public:
     struct Shard;
 
@@ -535,6 +564,14 @@ class MetricSystem {
     bool reaping_ = false, shutdown_ = false;
     std::atomic<uint64_t> dropped_over_limit_{0};
     uint64_t system_id_ = 0;
+    // JoinRanks: the exchange and the job-wide rows of a collection (under snapshot_mu_)
+    struct JobRows;
+    bool join_collection(JobRows &j, const std::vector<uint8_t> &counter_touched);
+    AllGather allgather_;
+    bool collected_ = false;
+    bool exchange_logged_ = false;
+    std::mutex ranks_mu_;
+    RanksState ranks_;
 };
 
 // print_benchmark.go:49: run `op` from `concurrency` threads between StartTimer/Stop and print every interval's

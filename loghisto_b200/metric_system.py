@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import contextlib
 import ctypes as C
+import sys
 
 from . import _lib as _L
 from . import build as _build
@@ -14,6 +15,8 @@ from .engine import (_batch_array, _capture_stream, _stream, _timer_stream, boar
                      graph_counter_args, graph_duration_out, graph_keyed_args, raw_percentiles, raw_ranks)
 
 _EMIT = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_char_p, C.c_int, C.c_uint64, C.c_double)
+_RANKS_SINK = C.CFUNCTYPE(None, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64)
+_RANKS_ALLGATHER = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, _RANKS_SINK, C.c_void_p)
 _lib = None
 
 
@@ -125,6 +128,9 @@ def _bind(L):
         getattr(L, "lhms_recv_" + kind).restype = C.c_int
         getattr(L, "lhms_recv_" + kind).argtypes = [vp, C.c_int64, _EMIT, vp]
         getattr(L, "lhms_free_%s_channel" % kind).argtypes = [vp]
+    L.lhms_ranks_join.restype = C.c_int
+    L.lhms_ranks_join.argtypes = [vp, C.c_uint32, C.c_uint32, _RANKS_ALLGATHER, vp, C.c_char_p, C.c_int]
+    L.lhms_ranks_info.argtypes = [vp, C.POINTER(C.c_uint64)]
     return L
 
 
@@ -736,6 +742,55 @@ class MetricSystem:
         if rc != 0:
             raise RuntimeError(err.value.decode())
         return col.metrics
+
+    def join_ranks(self, rank: int, world: int, allgather):
+        """Joins the systems of a multi-GPU job, so that each collection describes the whole job
+        (MetricSystem::JoinRanks).  Collective: every rank calls it once, before its first collection, with
+        allgather(bytes) -> list[bytes], every rank's bytes in rank order (loghisto_b200.distributed.rank_allgather builds
+        one from a process group).  allgather runs on the collecting thread (the reaper's once Start()ed); an exception
+        in it fails that collection's exchange on this rank, which then collects its own interval alone.
+
+        Afterwards Histograms, Rates, Counters, the aggregates and device subscriptions are job-wide and identical on
+        every rank; gauges stay rank-local.  ValueError for a bad rank / world, or when the ranks differ in
+        max_histograms, max_counters or precision (raised on every rank alike); RuntimeError otherwise."""
+        rank, world = int(rank), int(world)
+        if not callable(allgather):
+            raise TypeError("allgather must be callable")
+        if world < 2 or world > _L.LH_MAX_RANKS or not 0 <= rank < world:
+            raise ValueError("join_ranks: need 2 <= world <= %d and 0 <= rank < world" % _L.LH_MAX_RANKS)
+
+        logged = []
+
+        def gather(_user, mine, n, sink, sink_ctx):
+            try:
+                parts = allgather(C.string_at(mine, n) if n else b"")
+                if len(parts) != world:
+                    raise ValueError("allgather returned %d parts for a world of %d" % (len(parts), world))
+                for r, b in enumerate(parts):
+                    b = bytes(b)
+                    sink(sink_ctx, r, b, len(b))
+                return 0
+            except Exception as e:   # the collection goes on with this rank alone; say why, once
+                if not logged:
+                    logged.append(e)
+                    sys.stderr.write("loghisto: rank %d: allgather raised %s: %s\n" % (rank, type(e).__name__, e))
+                return 1
+
+        cb = _RANKS_ALLGATHER(gather)
+        err = C.create_string_buffer(512)
+        rc = self._lib.lhms_ranks_join(self._h, rank, world, cb, None, err, 512)
+        if rc != 0:
+            raise (ValueError if rc == -2 else RuntimeError)(err.value.decode())
+        self._ranks_cb = cb   # called at every collection from now on
+
+    def ranks_info(self) -> dict:
+        """MetricSystem::RanksInfo: rank, world (0: not joined), status of the last collection (0 summed, 1 a peer did
+        not arrive in time, 2 peers froze different buffers, 3 the exchange failed), collections summed, bytes read
+        from peers by the last all-reduce, and names left out of the job-wide unions by the bounds."""
+        out = (C.c_uint64 * 6)()
+        self._lib.lhms_ranks_info(self._h, out)
+        keys = ("rank", "world", "status", "summed", "bytes_from_peers", "names_dropped")
+        return {k: int(v) for k, v in zip(keys, out)}
 
     def stats(self) -> dict:
         """lh_get_stats of the system's context, as Engine.stats."""
