@@ -450,7 +450,24 @@ LH_API lh_status lh_board_destroy(lh_ctx *ctx, const lh_board *b);
  *                            enqueued); n == 0 enqueues nothing.
  *   lh_raw_board_destroy     frees the board, stream-ordered after every publish already issued.  The caller guarantees
  *                            that no query of the board is pending.  lh_destroy frees every raw board left.
- * A destroyed or foreign handle gets LH_ERR_INVALID. */
+ * A destroyed or foreign handle gets LH_ERR_INVALID.
+ *
+ * Window boards: lh_raw_board_create_window(ctx, k, window, out) creates a board whose row i answers for the
+ * histogram whose per-key counts are the sums, mod 2^64, of row i's last `window` publishes (fewer before the board
+ * has seen `window`), i.e. what a board of lh_raw_board_create would answer had those intervals been merged into one
+ * snapshot: the same layout, header, seqlock and LH_RAW_KEY_WRAPPED rule (applied to the window's own running counts,
+ * so a window may wrap when none of its intervals does, and stops being wrapped when the interval that wrapped it
+ * leaves), so every query call, the device functions and the bindings work on it unchanged.
+ *   window == 1 is lh_raw_board_create; window == 0 gives LH_ERR_INVALID, window > LH_RAW_MAX_WINDOW LH_ERR_RANGE, a
+ *   failed allocation LH_ERR_NOMEM with nothing left allocated; the other checks are lh_raw_board_create's.  Device
+ *   memory: (window + 1) x 512 KiB per row beyond the board's 512 KiB (a dense sum row and one slot per publish of the
+ *   window), plus window + 8 bytes of bookkeeping per row.
+ *   lh_snapshot_publish_raw on a window board takes row i's entering interval as on any board (hist_ids[i]'s frozen or
+ *   all-reduced counts; unbound or untouched: empty), drops the row's oldest one from the window and writes the row
+ *   from the new window, all inside the row's seqlock, in one kernel (plus the same staging launches for k > 4096),
+ *   without waiting or allocating.  Its traffic follows the key ranges of the intervals in the window (the fast window's
+ *   keys unless one of them has a count outside it), not `window`.  A second publish to a window board in the same
+ *   snapshot gives LH_ERR_STATE and enqueues nothing, since it would count one interval twice. */
 typedef struct lh_raw_row_header {
     uint64_t seq;                             /* seqlock word: odd while a publish writes the row, +2 per publish */
     uint64_t publishes;                       /* publishes so far (= seq / 2 when even) */
@@ -472,7 +489,9 @@ LH_STATIC_ASSERT(sizeof(lh_raw_row_header) == 32 && offsetof(lh_raw_row_header, 
 LH_STATIC_ASSERT(sizeof(lh_raw_board) == 80 && offsetof(lh_raw_board, prec) == 32, "lh_raw_board is 80 bytes");
 /* byte offset of row 0's cells from d_rows: the headers rounded up to 256 bytes */
 #define LH_RAW_CELLS_OFFSET(k) ((((uint64_t)(k) * 32u) + 255u) & ~(uint64_t)255u)
+#define LH_RAW_MAX_WINDOW 4096
 LH_API lh_status lh_raw_board_create(lh_ctx *ctx, uint32_t k, lh_raw_board *out);
+LH_API lh_status lh_raw_board_create_window(lh_ctx *ctx, uint32_t k, uint32_t window, lh_raw_board *out);
 LH_API lh_status lh_snapshot_publish_raw(lh_ctx *ctx, const lh_raw_board *b, const uint32_t *hist_ids);
 LH_API lh_status lh_raw_percentiles(lh_ctx *ctx, const lh_raw_board *b, const uint32_t *d_rows, const double *d_ps,
                                     uint32_t n, int32_t *d_keys, double *d_vals, uint64_t *d_publish, void *stream);
@@ -774,6 +793,7 @@ LH_API lh_status lh_device_alloc(lh_ctx *ctx, size_t bytes, void **d_out);
 LH_API lh_status lh_device_free(lh_ctx *ctx, void *d_ptr);
 LH_API lh_status lh_host_alloc_pinned(lh_ctx *ctx, size_t bytes, void **h_out);
 LH_API lh_status lh_host_free_pinned(lh_ctx *ctx, void *h_ptr);
+/* lh_memcpy_h2d returns once the bytes are in device memory, so that work on any stream may read them */
 LH_API lh_status lh_memcpy_h2d(lh_ctx *ctx, void *d_dst, const void *h_src, size_t bytes);
 LH_API lh_status lh_memcpy_d2h(lh_ctx *ctx, void *h_dst, const void *d_src, size_t bytes);
 /* kernel-variant selection for profiling: key "k1" -> variant number,

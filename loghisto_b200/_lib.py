@@ -151,6 +151,8 @@ def LH_RAW_CELLS_OFFSET(k: int) -> int:
     return (k * 32 + 255) & ~255
 
 
+LH_RAW_MAX_WINDOW = 4096   # publishes a window board may sum per row (lh_raw_board_create_window)
+
 LH_GAUGE_F64, LH_GAUGE_F32, LH_GAUGE_F16, LH_GAUGE_BF16, LH_GAUGE_I64, LH_GAUGE_I32, LH_GAUGE_U64 = range(7)
 
 
@@ -207,6 +209,7 @@ SIGNATURES = {
     "lh_board_read": (_i32, [_vp, C.POINTER(lh_board), _vp, _vp]),
     "lh_board_destroy": (_i32, [_vp, C.POINTER(lh_board)]),
     "lh_raw_board_create": (_i32, [_vp, _u32, C.POINTER(lh_raw_board)]),
+    "lh_raw_board_create_window": (_i32, [_vp, _u32, _u32, C.POINTER(lh_raw_board)]),
     "lh_snapshot_publish_raw": (_i32, [_vp, C.POINTER(lh_raw_board), _vp]),
     "lh_raw_percentiles": (_i32, [_vp, C.POINTER(lh_raw_board), _vp, _vp, _u32, _vp, _vp, _vp, _vp]),
     "lh_raw_ranks": (_i32, [_vp, C.POINTER(lh_raw_board), _vp, _vp, _u32, _vp, _vp, _vp, _vp]),

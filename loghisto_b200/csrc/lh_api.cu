@@ -159,6 +159,14 @@ struct PeerMap {                                   // one remote rank as mapped 
     bool ipc = false;                              // pointers came from cudaIpcOpenMemHandle (must be closed)
 };
 
+// a live raw board (lh_raw_board_create / _window) and the host's bookkeeping of its window
+struct RawBoard {
+    lh_raw_board b{};
+    uint32_t window = 1;          // publishes summed per row (1: a plain board, published by k_raw_publish)
+    uint64_t published = 0;       // publishes issued; a window board's next one replaces slot published % window
+    uint64_t snapshot = 0;        // stats.snapshots at its latest publish: a window board takes one per snapshot
+};
+
 }  // namespace
 
 struct lh_ctx {
@@ -273,9 +281,9 @@ struct lh_ctx {
     uint64_t next_board = 1;
     int pub_slot = -1;
     BoardParams board_prm{};
-    // raw device subscriptions (lh_raw_board_*): live boards, and the parameter block of their publish kernel (filled
+    // raw device subscriptions (lh_raw_board_*): live boards, and the parameter block of their publish kernels (filled
     // under the lock)
-    std::vector<lh_raw_board> raw_boards;
+    std::vector<RawBoard> raw_boards;
     uint64_t next_raw_board = 1;
     RawPublishParams raw_prm{};
     // device gauges (lh_gauges_read): calls are serialised by gauge_mu (taken before mu), since they share the output
@@ -1194,7 +1202,7 @@ extern "C" lh_status lh_destroy(lh_ctx *ctx) {
     cudaDeviceSynchronize();
     for (auto &g : ctx->graphs) cudaFree(g.rec.d_buckets);
     for (auto &b : ctx->boards) cudaFree(b.d_board);
-    for (auto &b : ctx->raw_boards) cudaFree(b.d_rows);
+    for (auto &b : ctx->raw_boards) cudaFree(b.b.d_rows);   // the window's sums and slots too: one allocation
     if (ctx->h_gauges) cudaFreeHost(ctx->h_gauges);
     if (ctx->gauge_done) cudaEventDestroy(ctx->gauge_done);
     if (ctx->graph_drained) cudaEventDestroy(ctx->graph_drained);
@@ -2322,58 +2330,88 @@ extern "C" lh_status lh_board_destroy(lh_ctx *ctx, const lh_board *b) {
 namespace {
 // headers, the k rows of cells, then the id table of k_raw_stage
 size_t raw_table_offset(uint32_t k) { return LH_RAW_CELLS_OFFSET(k) + (size_t)k * 65536u * 8u; }
+// A window board continues, 256-byte aligned, with its k sum rows, the slot counts [k][2] and the slot levels
+// [k][window] (zeroed at creation: every slot empty), then its k * window slots.
+size_t raw_window_offset(uint32_t k) { return (raw_table_offset(k) + (size_t)k * 4u + 255u) & ~(size_t)255u; }
+size_t raw_nlevel_offset(uint32_t k) { return raw_window_offset(k) + (size_t)k * 65536u * 8u; }
+size_t raw_levels_offset(uint32_t k) { return raw_nlevel_offset(k) + (size_t)k * 8u; }
+size_t raw_slots_offset(uint32_t k, uint32_t w) { return (raw_levels_offset(k) + (size_t)k * w + 255u) & ~(size_t)255u; }
 
 // the live raw board a handle names (its memory must match too), or nullptr
-const lh_raw_board *raw_board_of(lh_ctx *ctx, const lh_raw_board *b) {
+RawBoard *raw_board_of(lh_ctx *ctx, const lh_raw_board *b) {
     if (!b) return nullptr;
     for (auto &x : ctx->raw_boards)
-        if (x.handle == b->handle && x.d_rows == b->d_rows) return &x;
+        if (x.b.handle == b->handle && x.b.d_rows == b->d_rows) return &x;
     return nullptr;
 }
 
 // non-NULL and a-byte aligned
 bool arg_ok(const void *p, uintptr_t a) { return p && ((uintptr_t)p & (a - 1u)) == 0; }
-}  // namespace
 
-extern "C" lh_status lh_raw_board_create(lh_ctx *ctx, uint32_t k, lh_raw_board *out) {
-    LH_ENTER(ctx);
+// lh_raw_board_create (window 1) and lh_raw_board_create_window, with ctx->mu held.  One allocation holds the whole
+// board, so that a failure leaves nothing allocated and lh_raw_board_destroy frees everything at once.
+lh_status raw_board_create(lh_ctx *ctx, uint32_t k, uint32_t window, lh_raw_board *out) {
     if (!out) return fail(ctx, LH_ERR_INVALID, "out is NULL");
     if (k == 0) return fail(ctx, LH_ERR_INVALID, "a raw board needs a row");
+    if (window == 0) return fail(ctx, LH_ERR_INVALID, "a window of 0 publishes");
     if (k > ctx->H) return fail(ctx, LH_ERR_RANGE, "more rows than max_histograms");
-    const size_t bytes = raw_table_offset(k) + (size_t)k * 4u;
+    if (window > LH_RAW_MAX_WINDOW) return fail(ctx, LH_ERR_RANGE, "window > LH_RAW_MAX_WINDOW");
+    const size_t bytes = window == 1 ? raw_table_offset(k) + (size_t)k * 4u
+                                     : raw_slots_offset(k, window) + (size_t)k * window * 65536u * 8u;
     cudaStream_t s = ctx->snap_stream;
     char *base = nullptr;
-    LH_CUDA(ctx, cudaMallocAsync((void **)&base, bytes, s));
+    cudaError_t e = cudaMallocAsync((void **)&base, bytes, s);
+    if (e != cudaSuccess)
+        return fail(ctx, e == cudaErrorMemoryAllocation ? LH_ERR_NOMEM : LH_ERR_CUDA, "allocating a raw board", e);
     // only the headers, each an empty row (publish 0, total 0, key_lo > key_hi): a row's cells are read only inside
-    // the key range its latest publish wrote, so the cells of a row never published are never read
+    // the key range its latest publish wrote, so the cells of a row never published are never read.  A window board's
+    // sums, slot counts and levels start at 0; its slots are read only inside the range of the level they record.
     std::vector<lh_raw_row_header> empty(k);
     for (auto &h : empty) { h.key_lo = 0; h.key_hi = -1; }
-    cudaError_t e = cudaMemcpyAsync(base, empty.data(), (size_t)k * sizeof(lh_raw_row_header), cudaMemcpyHostToDevice, s);
+    e = cudaMemcpyAsync(base, empty.data(), (size_t)k * sizeof(lh_raw_row_header), cudaMemcpyHostToDevice, s);
+    if (e == cudaSuccess && window > 1)
+        e = cudaMemsetAsync(base + raw_window_offset(k), 0, raw_levels_offset(k) + (size_t)k * window - raw_window_offset(k), s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
     if (e != cudaSuccess) {
         cudaFreeAsync(base, s);
         return fail(ctx, LH_ERR_CUDA, "lh_raw_board_create", e);
     }
-    lh_raw_board b{};
-    b.handle = graph_handle(ctx, ctx->next_raw_board++);
-    b.d_rows = base;
-    b.d_decomp = ctx->d_decomp;
-    b.k = k;
-    memcpy(b.prec, &ctx->pc, sizeof(Prec));
-    ctx->raw_boards.push_back(b);
-    *out = b;
+    RawBoard rb;
+    rb.b.handle = graph_handle(ctx, ctx->next_raw_board++);
+    rb.b.d_rows = base;
+    rb.b.d_decomp = ctx->d_decomp;
+    rb.b.k = k;
+    memcpy(rb.b.prec, &ctx->pc, sizeof(Prec));
+    rb.window = window;
+    ctx->raw_boards.push_back(rb);
+    *out = rb.b;
     return LH_OK;
 }
+}  // namespace
 
-// One k_raw_publish (a CTA per row) on the snapshot stream, after whatever wrote the snapshot view it reads.  Ids that
-// do not fit its parameter block are first copied into the board's table by k_raw_stage launches (see lh_kernels.cuh:
-// a row's word is odd only inside the CTA that writes the row).
+extern "C" lh_status lh_raw_board_create(lh_ctx *ctx, uint32_t k, lh_raw_board *out) {
+    LH_ENTER(ctx);
+    return raw_board_create(ctx, k, 1, out);
+}
+
+extern "C" lh_status lh_raw_board_create_window(lh_ctx *ctx, uint32_t k, uint32_t window, lh_raw_board *out) {
+    LH_ENTER(ctx);
+    return raw_board_create(ctx, k, window, out);
+}
+
+// One k_raw_publish (a CTA per row) on the snapshot stream, after whatever wrote the snapshot view it reads, or one
+// k_raw_publish_window for a window board.  Ids that do not fit its parameter block are first copied into the board's
+// table by k_raw_stage launches (see lh_kernels.cuh: a row's word is odd only inside the CTA that writes the row).
 extern "C" lh_status lh_snapshot_publish_raw(lh_ctx *ctx, const lh_raw_board *b, const uint32_t *hist_ids) {
     LH_ENTER(ctx);
-    const lh_raw_board *bd = raw_board_of(ctx, b);
-    if (!bd) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign raw board");
+    RawBoard *rb = raw_board_of(ctx, b);
+    if (!rb) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign raw board");
+    const lh_raw_board *bd = &rb->b;
     if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "lh_snapshot_publish_raw needs an open snapshot");
     if (!ids_ok(hist_ids, bd->k, ctx->H)) return fail(ctx, LH_ERR_RANGE, "id >= max_histograms");
+    const bool windowed = rb->window > 1;
+    if (windowed && rb->snapshot == ctx->stats.snapshots)   // the interval would be counted twice
+        return fail(ctx, LH_ERR_STATE, "a window board takes one publish per snapshot");
     const View v = snapshot_view(ctx);
     cudaStream_t s = ctx->snap_stream;
     RawPublishParams &p = ctx->raw_prm;
@@ -2383,6 +2421,12 @@ extern "C" lh_status lh_snapshot_publish_raw(lh_ctx *ctx, const lh_raw_board *b,
     p.buckets = v.buckets;
     p.flags = v.flags;
     p.win = ctx->pc.win;
+    p.sums = windowed ? reinterpret_cast<unsigned long long *>(p.rows + raw_window_offset(bd->k)) : nullptr;
+    p.nlevel = windowed ? reinterpret_cast<uint32_t *>(p.rows + raw_nlevel_offset(bd->k)) : nullptr;
+    p.levels = windowed ? reinterpret_cast<uint8_t *>(p.rows + raw_levels_offset(bd->k)) : nullptr;
+    p.slots = windowed ? reinterpret_cast<unsigned long long *>(p.rows + raw_slots_offset(bd->k, rb->window)) : nullptr;
+    p.window = rb->window;
+    p.slot = (uint32_t)(rb->published % rb->window);
     for (uint32_t r0 = 0;; r0 += RP_MAX_IDS) {
         const uint32_t n = std::min<uint32_t>(RP_MAX_IDS, bd->k - r0);
         p.n_staged = r0;
@@ -2393,9 +2437,12 @@ extern "C" lh_status lh_snapshot_publish_raw(lh_ctx *ctx, const lh_raw_board *b,
         LH_CUDA(ctx, cudaGetLastError());
         ctx->stats.kernel_launches++;
     }
-    k_raw_publish<<<bd->k, RP_THREADS, 0, s>>>(p);
+    if (windowed) k_raw_publish_window<<<bd->k, RP_THREADS, 0, s>>>(p);
+    else k_raw_publish<<<bd->k, RP_THREADS, 0, s>>>(p);
     LH_CUDA(ctx, cudaGetLastError());
     ctx->stats.kernel_launches++;
+    rb->published++;
+    rb->snapshot = ctx->stats.snapshots;
     return LH_OK;
 }
 
@@ -2404,8 +2451,9 @@ namespace {
 // argument checked before it is enqueued.
 lh_status raw_query(lh_ctx *ctx, const lh_raw_board *b, bool pct, const uint32_t *d_rows, const double *d_x,
                     uint64_t n, uint32_t m, void *d_out1, void *d_out2, uint64_t *d_publish, void *stream) {
-    const lh_raw_board *bd = raw_board_of(ctx, b);
-    if (!bd) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign raw board");
+    const RawBoard *rb = raw_board_of(ctx, b);
+    if (!rb) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign raw board");
+    const lh_raw_board *bd = &rb->b;
     if (n == 0) return LH_OK;
     if (n > UINT32_MAX) return fail(ctx, LH_ERR_RANGE, "more than 2^32 - 1 queries");
     const bool grid = m != 0;
@@ -2442,24 +2490,24 @@ extern "C" lh_status lh_raw_ranks(lh_ctx *ctx, const lh_raw_board *b, const uint
 extern "C" lh_status lh_raw_percentiles_grid(lh_ctx *ctx, const lh_raw_board *b, const double *d_ps, uint32_t m,
                                              int32_t *d_keys, double *d_vals, uint64_t *d_publish, void *stream) {
     LH_ENTER(ctx);
-    const lh_raw_board *bd = raw_board_of(ctx, b);
-    return raw_query(ctx, b, true, nullptr, d_ps, bd ? (uint64_t)bd->k * m : 0, m, d_keys, d_vals, d_publish, stream);
+    const RawBoard *rb = raw_board_of(ctx, b);
+    return raw_query(ctx, b, true, nullptr, d_ps, rb ? (uint64_t)rb->b.k * m : 0, m, d_keys, d_vals, d_publish, stream);
 }
 
 extern "C" lh_status lh_raw_ranks_grid(lh_ctx *ctx, const lh_raw_board *b, const double *d_values, uint32_t m,
                                        uint64_t *d_ranks, uint64_t *d_totals, uint64_t *d_publish, void *stream) {
     LH_ENTER(ctx);
-    const lh_raw_board *bd = raw_board_of(ctx, b);
-    return raw_query(ctx, b, false, nullptr, d_values, bd ? (uint64_t)bd->k * m : 0, m, d_ranks, d_totals, d_publish,
+    const RawBoard *rb = raw_board_of(ctx, b);
+    return raw_query(ctx, b, false, nullptr, d_values, rb ? (uint64_t)rb->b.k * m : 0, m, d_ranks, d_totals, d_publish,
                      stream);
 }
 
 extern "C" lh_status lh_raw_board_destroy(lh_ctx *ctx, const lh_raw_board *b) {
     LH_ENTER(ctx);
-    const lh_raw_board *bd = raw_board_of(ctx, b);
-    if (!bd) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign raw board");
-    LH_CUDA(ctx, cudaFreeAsync(bd->d_rows, ctx->snap_stream));   // after every publish issued (all on this stream)
-    ctx->raw_boards.erase(ctx->raw_boards.begin() + (bd - ctx->raw_boards.data()));
+    const RawBoard *rb = raw_board_of(ctx, b);
+    if (!rb) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign raw board");
+    LH_CUDA(ctx, cudaFreeAsync(rb->b.d_rows, ctx->snap_stream));   // after every publish issued (all on this stream)
+    ctx->raw_boards.erase(ctx->raw_boards.begin() + (rb - ctx->raw_boards.data()));
     return LH_OK;
 }
 
@@ -3053,6 +3101,10 @@ extern "C" lh_status lh_host_free_pinned(lh_ctx *ctx, void *h_ptr) {
 extern "C" lh_status lh_memcpy_h2d(lh_ctx *ctx, void *d_dst, const void *h_src, size_t bytes) {
     LH_ENTER(ctx);
     LH_CUDA(ctx, cudaMemcpy(d_dst, h_src, bytes, cudaMemcpyHostToDevice));
+    // From pageable memory cudaMemcpy may return once the source is staged, before the DMA has reached d_dst, and it
+    // runs on the legacy stream, which the context's (and torch's) non-blocking streams are not ordered after: wait
+    // for the DMA, so that a kernel on any stream may read d_dst as soon as this returns.
+    LH_CUDA(ctx, cudaStreamSynchronize(cudaStreamLegacy));
     return LH_OK;
 }
 extern "C" lh_status lh_memcpy_d2h(lh_ctx *ctx, void *h_dst, const void *d_src, size_t bytes) {

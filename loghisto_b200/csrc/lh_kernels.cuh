@@ -23,8 +23,9 @@
 //   k_ingest_batch          many device arrays under many ids (lh_ingest_batch, lh_graph_recorder_ingest)
 //   k_ingest_keyed_graph    (id,value) pairs into a graph recorder's rows (lh_graph_recorder_ingest_keyed_*)
 //   k_graph_drain           graph recorders' rows -> the interval being frozen (lh_snapshot_begin)
-//   k_raw_publish, k_raw_percentiles, k_raw_ranks   running bucket counts of a snapshot -> raw device subscription rows,
-//                           and exact percentile / rank queries over them (lh_snapshot_publish_raw, lh_raw_*)
+//   k_raw_publish, k_raw_publish_window, k_raw_percentiles, k_raw_ranks   running bucket counts of a snapshot (or of
+//                           the last `window` of them) -> raw device subscription rows, and exact percentile / rank
+//                           queries over them (lh_snapshot_publish_raw, lh_raw_*)
 //   misc k_clear_touched, k_fill_decompress, k_compress_probe, k_fastpath_margin, k_fastpath_certify, k_stream_probe,
 //        k_gen_stream, k_gen_ids_u16
 //
@@ -2387,8 +2388,111 @@ struct RawPublishParams {
     const uint32_t *flags;
     uint32_t win;
     uint32_t n_staged, n;                    // ids in `table`, then in ids[]
+    // window boards only (k_raw_publish_window; see below)
+    unsigned long long *sums;                // k rows of uint64[65536], by uint16 key: the window's per-key sums
+    unsigned long long *slots;               // k * window rows of uint64[65536], by uint16 key: row r's slot j at r * window + j
+    uint32_t *nlevel;                        // [k][2]: slots of row r at level 1, at level 2
+    uint8_t *levels;                         // [k][window]: level of each slot (0 empty, 1 window keys, 2 all keys)
+    uint32_t window, slot;                   // slots per row; the slot (the oldest) this publish replaces
     uint32_t ids[RP_MAX_IDS];
 };
+
+// the id of `row` (staged or in the parameter block), and the level of its source row: 0 none (unbound or untouched),
+// 1 the fast window's keys, 2 all keys.  rp_range gives a level's key range (lo > hi: empty).
+__device__ __forceinline__ uint32_t rp_id(const RawPublishParams &p, uint32_t row) {
+    return row < p.n_staged ? p.table[row] : p.ids[row - p.n_staged];
+}
+__device__ __forceinline__ uint32_t rp_level(const RawPublishParams &p, uint32_t id) {
+    const uint32_t f = id == LH_GRAPH_UNBOUND ? 0u : p.flags[id];
+    return f == 0u ? 0u : (f & 2u) ? 2u : 1u;
+}
+__device__ __forceinline__ void rp_range(uint32_t level, uint32_t win, int &lo, int &hi) {
+    lo = level == 2u ? -32768 : level == 1u ? -(int)(win - 1u) : 0;
+    hi = level == 2u ? 32767 : level == 1u ? (int)(win - 1u) : -1;
+}
+
+// The chunked running-count scan of one row, by the whole CTA: keys [lo, hi] of src (indexed by uint16 key, as the
+// snapshot's rows) are loaded in ascending key order in chunks of RP_CHUNK, block-scanned with the running total of
+// the chunks before as carry, and written with strong relaxed stores to cells key + 32768 of dst.  Returns the running
+// count after key hi (0 for lo > hi); wrap becomes nonzero in the threads that saw a running count pass 2^64.  Every
+// thread must call it; it ends with a __syncthreads.
+__device__ __forceinline__ unsigned long long rp_scan_row(const unsigned long long *src, int lo, int hi,
+                                                          unsigned long long *dst, unsigned long long *s_cells,
+                                                          unsigned long long *s_warp, int &wrap) {
+    const uint32_t t = threadIdx.x, lane = t & 31u, warp = t >> 5;
+    unsigned long long carry = 0;
+    if (lo > hi) return carry;
+    const uint32_t n = (uint32_t)(hi - lo + 1);
+    dst += (uint32_t)(lo + 32768);
+    for (uint32_t c0 = 0; c0 < n; c0 += RP_CHUNK) {
+#pragma unroll
+        for (int j = 0; j < RP_PER; j++) {                    // coalesced: chunk cell i is key lo + c0 + i
+            const uint32_t i = (uint32_t)j * RP_THREADS + t;
+            s_cells[rp_slot(i)] = c0 + i < n ? src[(uint32_t)(lo + (int)(c0 + i)) & 0xFFFFu] : 0ull;
+        }
+        __syncthreads();
+        unsigned long long v[RP_PER], local = 0;
+#pragma unroll
+        for (int j = 0; j < RP_PER; j++) { v[j] = s_cells[rp_slot(t * RP_PER + j)]; local += v[j]; }
+        unsigned long long incl = local;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+            if (lane >= (uint32_t)o) incl += y;
+        }
+        if (lane == 31) s_warp[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            const unsigned long long w = lane < RP_THREADS / 32 ? s_warp[lane] : 0ull;
+            unsigned long long wi = w;
+#pragma unroll
+            for (int o = 1; o < RP_THREADS / 32; o <<= 1) {
+                const unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, wi, o);
+                if (lane >= (uint32_t)o) wi += y;
+            }
+            if (lane < RP_THREADS / 32) s_warp[lane] = wi - w;   // exclusive prefix of the warp totals
+        }
+        __syncthreads();
+        unsigned long long run = carry + s_warp[warp] + incl - local;
+#pragma unroll
+        for (int j = 0; j < RP_PER; j++) { run += v[j]; wrap |= run < v[j]; s_cells[rp_slot(t * RP_PER + j)] = run; }
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < RP_PER; j++) {
+            const uint32_t i = (uint32_t)j * RP_THREADS + t;
+            if (c0 + i < n) board::st_relaxed(dst + c0 + i, s_cells[rp_slot(i)]);
+        }
+        carry = s_cells[rp_slot(RP_CHUNK - 1)];                // the running count after this chunk
+        __syncthreads();                                      // before the next chunk overwrites s_cells / s_warp
+    }
+    return carry;
+}
+
+// Steps 1 and 3-4 of the seqlock sequence above, around the body of a publish.
+__device__ __forceinline__ void rp_open(char *h) {
+    if (threadIdx.x == 0) {
+        unsigned long long *seq = reinterpret_cast<unsigned long long *>(h);
+        board::st_relaxed(seq, board::ld_relaxed(seq) + 1ull);   // odd: the previous publish ended (stream order)
+        board::fence_acq_rel();
+    }
+    __syncthreads();
+}
+__device__ __forceinline__ void rp_close(char *h, unsigned long long total, int lo, int hi, int wrap) {
+    if (__syncthreads_or(wrap)) hi += LH_RAW_KEY_WRAPPED;          // readers fall back to Go's literal rule
+    if (threadIdx.x == 0) {
+        board::st_relaxed(h + offsetof(lh_raw_row_header, total), total);
+        board::st_relaxed(h + offsetof(lh_raw_row_header, key_lo),
+                          (unsigned long long)(uint32_t)lo | (unsigned long long)(uint32_t)hi << 32);
+    }
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        unsigned long long *seq = reinterpret_cast<unsigned long long *>(h);
+        const unsigned long long s = board::ld_relaxed(seq) + 1ull;   // even
+        board::st_relaxed(h + offsetof(lh_raw_row_header, publishes), s >> 1);
+        board::st_release(seq, s);
+    }
+}
 
 __global__ void __launch_bounds__(RP_THREADS)
 k_raw_stage(const __grid_constant__ RawPublishParams p) {
@@ -2399,80 +2503,90 @@ __global__ void __launch_bounds__(RP_THREADS)
 k_raw_publish(const __grid_constant__ RawPublishParams p) {
     __shared__ unsigned long long s_cells[RP_CHUNK + RP_CHUNK / 8];
     __shared__ unsigned long long s_warp[RP_THREADS / 32];
-    const uint32_t row = blockIdx.x, t = threadIdx.x, lane = t & 31u, warp = t >> 5;
-    const uint32_t id = row < p.n_staged ? p.table[row] : p.ids[row - p.n_staged];
-    const uint32_t level = id == LH_GRAPH_UNBOUND ? 0u : p.flags[id];
+    const uint32_t row = blockIdx.x;
+    const uint32_t id = rp_id(p, row);
+    const uint32_t level = rp_level(p, id);
     char *h = p.rows + (size_t)row * sizeof(lh_raw_row_header);
-    unsigned long long *seq = reinterpret_cast<unsigned long long *>(h);
-    if (t == 0) {
-        board::st_relaxed(seq, board::ld_relaxed(seq) + 1ull);   // odd: the previous publish ended (stream order)
-        board::fence_acq_rel();
-    }
-    __syncthreads();
-    int lo = 0, hi = -1;                                          // empty
-    unsigned long long carry = 0;
+    rp_open(h);
+    int lo, hi;
+    rp_range(level, p.win, lo, hi);
     int wrap = 0;                                                 // a running count passed 2^64
-    if (level) {
-        lo = (level & 2u) ? -32768 : -(int)(p.win - 1u);
-        hi = (level & 2u) ? 32767 : (int)(p.win - 1u);
-        const uint32_t n = (uint32_t)(hi - lo + 1);
-        const unsigned long long *src = p.buckets + (size_t)id * 65536u;
-        unsigned long long *dst = p.cells + (size_t)row * 65536u + (uint32_t)(lo + 32768);
-        for (uint32_t c0 = 0; c0 < n; c0 += RP_CHUNK) {
+    const unsigned long long total = rp_scan_row(p.buckets + (size_t)(level ? id : 0u) * 65536u, lo, hi,
+                                                 p.cells + (size_t)row * 65536u, s_cells, s_warp, wrap);
+    rp_close(h, total, lo, hi, wrap);
+}
+
+// k_raw_publish_window publishes into a board of `window` > 1 publishes per row (lh_raw_board_create_window): row r
+// answers for the per-key sums, mod 2^64, of its last `window` entering intervals.  Per row the board keeps a dense sum
+// row and `window` slots, each holding one entering interval's counts and its level (0 empty, 1 window keys, 2 all
+// keys), with the number of slots at levels 1 and 2.  The sum's key range is that of the widest level among the slots;
+// a slot's cells are read only inside its own level's range, and the sum's cells outside its range are 0 (below).
+// One CTA per row, inside the row's seqlock exactly as k_raw_publish (steps 1 and 3-4 above), and, like it, waiting on
+// nothing; all the row's bookkeeping is touched only by the CTA that writes the row, and two publishes of a board are
+// ordered by the stream.  In step 2:
+//   a. the entering interval is the row's source row as in k_raw_publish, at level lin; it replaces slot p.slot, at
+//      level lout; the sum's level before is lsum, after it lnew (from the slot counts);
+//   b. over the keys of max(lsum, lin): sum += in - out (in, out read as 0 outside their own ranges), and the slot takes
+//      in over lin's range.  A key outside lnew's range then holds 0 mod 2^64: every slot left is 0 there;
+//   c. __syncthreads (the CTA's own stores of the sum row are visible to it), then the chunked scan of the sum row over
+//      lnew's range, whose wrap rule therefore follows the window's own running counts.
+constexpr int RW_PER = 4;                        // keys per thread in flight in step b
+
+__global__ void __launch_bounds__(RP_THREADS)
+k_raw_publish_window(const __grid_constant__ RawPublishParams p) {
+    __shared__ unsigned long long s_cells[RP_CHUNK + RP_CHUNK / 8];
+    __shared__ unsigned long long s_warp[RP_THREADS / 32];
+    const uint32_t row = blockIdx.x, t = threadIdx.x;
+    const uint32_t id = rp_id(p, row);
+    const uint32_t lin = rp_level(p, id);
+    char *h = p.rows + (size_t)row * sizeof(lh_raw_row_header);
+    rp_open(h);
+    uint8_t *lv = p.levels + (size_t)row * p.window + p.slot;
+    uint32_t *cnt = p.nlevel + (size_t)row * 2u;
+    const uint32_t lout = *lv, n1 = cnt[0], n2 = cnt[1];
+    const uint32_t m1 = n1 - (lout == 1u) + (lin == 1u), m2 = n2 - (lout == 2u) + (lin == 2u);
+    const uint32_t lsum = n2 ? 2u : n1 ? 1u : 0u, lnew = m2 ? 2u : m1 ? 1u : 0u;
+    __syncthreads();                                              // every thread has read the bookkeeping
+    if (t == 0) { *lv = (uint8_t)lin; cnt[0] = m1; cnt[1] = m2; }
+    int ilo, ihi, olo, ohi, ulo, uhi;
+    rp_range(lin, p.win, ilo, ihi);
+    rp_range(lout, p.win, olo, ohi);
+    rp_range(lsum > lin ? lsum : lin, p.win, ulo, uhi);
+    const unsigned long long *src = p.buckets + (size_t)(lin ? id : 0u) * 65536u;
+    unsigned long long *sum = p.sums + (size_t)row * 65536u;
+    unsigned long long *slot = p.slots + ((size_t)row * p.window + p.slot) * 65536u;
+    if (ulo <= uhi) {
+        const uint32_t n = (uint32_t)(uhi - ulo + 1);
+        for (uint32_t c0 = 0; c0 < n; c0 += RP_THREADS * RW_PER) {
+            unsigned long long in[RW_PER], out[RW_PER], s[RW_PER];
 #pragma unroll
-            for (int j = 0; j < RP_PER; j++) {                    // coalesced: chunk cell i is key lo + c0 + i
-                const uint32_t i = (uint32_t)j * RP_THREADS + t;
-                s_cells[rp_slot(i)] = c0 + i < n ? src[(uint32_t)(lo + (int)(c0 + i)) & 0xFFFFu] : 0ull;
+            for (int j = 0; j < RW_PER; j++) {                    // every load of the group before any store
+                const uint32_t i = c0 + (uint32_t)j * RP_THREADS + t;
+                const int key = ulo + (int)i;
+                const uint32_t k16 = (uint32_t)key & 0xFFFFu;
+                const bool live = i < n;
+                in[j] = live && key >= ilo && key <= ihi ? src[k16] : 0ull;
+                out[j] = live && key >= olo && key <= ohi ? slot[k16] : 0ull;
+                s[j] = live ? sum[k16] : 0ull;
             }
-            __syncthreads();
-            unsigned long long v[RP_PER], local = 0;
 #pragma unroll
-            for (int j = 0; j < RP_PER; j++) { v[j] = s_cells[rp_slot(t * RP_PER + j)]; local += v[j]; }
-            unsigned long long incl = local;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-                if (lane >= (uint32_t)o) incl += y;
-            }
-            if (lane == 31) s_warp[warp] = incl;
-            __syncthreads();
-            if (warp == 0) {
-                const unsigned long long w = lane < RP_THREADS / 32 ? s_warp[lane] : 0ull;
-                unsigned long long wi = w;
-#pragma unroll
-                for (int o = 1; o < RP_THREADS / 32; o <<= 1) {
-                    const unsigned long long y = __shfl_up_sync(0xFFFFFFFFu, wi, o);
-                    if (lane >= (uint32_t)o) wi += y;
+            for (int j = 0; j < RW_PER; j++) {
+                const uint32_t i = c0 + (uint32_t)j * RP_THREADS + t;
+                const int key = ulo + (int)i;
+                const uint32_t k16 = (uint32_t)key & 0xFFFFu;
+                if (i < n) {
+                    sum[k16] = s[j] + in[j] - out[j];
+                    if (key >= ilo && key <= ihi) slot[k16] = in[j];
                 }
-                if (lane < RP_THREADS / 32) s_warp[lane] = wi - w;   // exclusive prefix of the warp totals
             }
-            __syncthreads();
-            unsigned long long run = carry + s_warp[warp] + incl - local;
-#pragma unroll
-            for (int j = 0; j < RP_PER; j++) { run += v[j]; wrap |= run < v[j]; s_cells[rp_slot(t * RP_PER + j)] = run; }
-            __syncthreads();
-#pragma unroll
-            for (int j = 0; j < RP_PER; j++) {
-                const uint32_t i = (uint32_t)j * RP_THREADS + t;
-                if (c0 + i < n) board::st_relaxed(dst + c0 + i, s_cells[rp_slot(i)]);
-            }
-            carry = s_cells[rp_slot(RP_CHUNK - 1)];                // the running count after this chunk
-            __syncthreads();                                      // before the next chunk overwrites s_cells / s_warp
         }
     }
-    if (__syncthreads_or(wrap)) hi += LH_RAW_KEY_WRAPPED;          // readers fall back to Go's literal rule
-    if (t == 0) {
-        board::st_relaxed(h + offsetof(lh_raw_row_header, total), carry);
-        board::st_relaxed(h + offsetof(lh_raw_row_header, key_lo),
-                          (unsigned long long)(uint32_t)lo | (unsigned long long)(uint32_t)hi << 32);
-    }
-    __threadfence();
     __syncthreads();
-    if (t == 0) {
-        const unsigned long long s = board::ld_relaxed(seq) + 1ull;   // even
-        board::st_relaxed(h + offsetof(lh_raw_row_header, publishes), s >> 1);
-        board::st_release(seq, s);
-    }
+    int lo, hi;
+    rp_range(lnew, p.win, lo, hi);
+    int wrap = 0;
+    const unsigned long long total = rp_scan_row(sum, lo, hi, p.cells + (size_t)row * 65536u, s_cells, s_warp, wrap);
+    rp_close(h, total, lo, hi, wrap);
 }
 
 // One thread per query; the answers are the device API's (one definition of the read).  rows == nullptr: the grid

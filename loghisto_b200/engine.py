@@ -485,15 +485,31 @@ def raw_ranks(call, k: int, values, device: int, stream):
     return ranks, totals, pub
 
 
+def check_window(window) -> int:
+    """A raw board's window: an int >= 1 (TypeError / ValueError otherwise)."""
+    import numbers
+    if isinstance(window, bool) or not isinstance(window, numbers.Integral):
+        raise TypeError(f"window must be an int >= 1, not {type(window).__name__}")
+    if window < 1:
+        raise ValueError(f"window must be >= 1, not {window}")
+    return int(window)
+
+
 class RawBoard:
     """A raw device subscription board of an Engine (Engine.raw_board): `board` is the lh_raw_board to pass by value to
-    kernels, which query it with lh::raw_percentile / lh::raw_rank / lh::raw_bucket_count."""
+    kernels, which query it with lh::raw_percentile / lh::raw_rank / lh::raw_bucket_count.  With `window` w > 1
+    (lh_raw_board_create_window) each row answers for the sum of its last w publishes."""
 
-    def __init__(self, engine: "Engine", k: int):
+    def __init__(self, engine: "Engine", k: int, window: int = 1):
+        window = check_window(window)
         self._eng = engine
         self.board = L.lh_raw_board()
-        engine._check(engine.lib.lh_raw_board_create(engine.h, int(k), C.byref(self.board)))
+        if window == 1:
+            engine._check(engine.lib.lh_raw_board_create(engine.h, int(k), C.byref(self.board)))
+        else:
+            engine._check(engine.lib.lh_raw_board_create_window(engine.h, int(k), window, C.byref(self.board)))
         self.k = int(k)
+        self.window = window
         self._open = True
 
     def publish(self, hist_ids=None):
@@ -823,9 +839,10 @@ class Engine:
         """A device subscription board of k histogram rows and kc counter rows (lh_board_create)."""
         return Board(self, k, kc)
 
-    def raw_board(self, k: int) -> "RawBoard":
-        """A raw device subscription board of k histogram rows (lh_raw_board_create)."""
-        return RawBoard(self, k)
+    def raw_board(self, k: int, window: int = 1) -> "RawBoard":
+        """A raw device subscription board of k histogram rows (lh_raw_board_create), each summed over its last
+        `window` publishes (lh_raw_board_create_window; an int >= 1)."""
+        return RawBoard(self, k, window)
 
     def read_gauges(self, tensors) -> np.ndarray:
         """lh_gauges_read of one-element CUDA tensors (gauge_src): float64(value) of each, read on the snapshot stream

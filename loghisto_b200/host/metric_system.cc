@@ -56,6 +56,7 @@
 #pragma weak lh_raw_percentiles_grid
 #pragma weak lh_raw_ranks_grid
 #pragma weak lh_raw_board_destroy
+#pragma weak lh_raw_board_create_window   // window boards: over a build without them, a window other than 1 throws
 // And for device gauges: over a build without them, RegisterDeviceGauge throws.
 #pragma weak lh_gauges_read
 // And for joined ranks: over a build without them, JoinRanks throws.
@@ -87,6 +88,7 @@ struct RawDeviceSubscription::State {
     MetricSystem *ms;                   // nullptr once closed (or once the system is gone)
     lh_raw_board b{};
     std::vector<std::string> hnames;
+    uint32_t window = 1;
 };
 
 namespace {
@@ -1029,14 +1031,22 @@ DeviceSubscription::~DeviceSubscription() {
 }
 
 // ---- raw device subscriptions --------------------------------------------------------------------------------------
-RawDeviceSubscription MetricSystem::NewRawDeviceSubscription(const std::vector<std::string> &histograms) {
+RawDeviceSubscription MetricSystem::NewRawDeviceSubscription(const std::vector<std::string> &histograms,
+                                                             uint32_t window) {
     if (!lh_raw_board_create || !lh_snapshot_publish_raw || !lh_raw_percentiles_grid || !lh_raw_ranks_grid ||
         !lh_raw_board_destroy)
         throw std::runtime_error("NewRawDeviceSubscription: this libloghisto_b200 has no raw device subscriptions");
+    if (window != 1 && !lh_raw_board_create_window)
+        throw std::runtime_error("NewRawDeviceSubscription: this libloghisto_b200 has no window boards");
     auto st = std::make_shared<RawDeviceSubscription::State>();
     st->ms = this;
     st->hnames = histograms;
-    check(ctx_, lh_raw_board_create(ctx_, (uint32_t)histograms.size(), &st->b), "lh_raw_board_create");
+    st->window = window;
+    if (window == 1)
+        check(ctx_, lh_raw_board_create(ctx_, (uint32_t)histograms.size(), &st->b), "lh_raw_board_create");
+    else
+        check(ctx_, lh_raw_board_create_window(ctx_, (uint32_t)histograms.size(), window, &st->b),
+              "lh_raw_board_create_window");
     std::lock_guard<std::mutex> lk(sub_mu_);
     raw_subs_.push_back(st);
     RawDeviceSubscription d;
@@ -1060,6 +1070,8 @@ const lh_raw_board &RawDeviceSubscription::board() const {
     if (!st_) throw std::runtime_error("RawDeviceSubscription::board of a closed subscription");
     return st_->b;
 }
+
+uint32_t RawDeviceSubscription::window() const { return st_ ? st_->window : 1u; }
 
 void RawDeviceSubscription::Percentiles(const double *d_ps, uint32_t m, int32_t *d_keys, double *d_vals,
                                         uint64_t *d_publish, void *stream) {
@@ -2115,6 +2127,25 @@ LHMS_API void *lhms_raw_subscription_new(void *ms, uint32_t n_h, const char *con
     try {
         std::vector<std::string> hs(h_names, h_names + n_h);
         auto *d = new RawDeviceSubscription(static_cast<MetricSystem *>(ms)->NewRawDeviceSubscription(hs));
+        *out = d->board();
+        *status = LH_OK;
+        return d;
+    } catch (const std::exception &e) {
+        *status = scope_status(e);
+        return nullptr;
+    }
+}
+// MetricSystem::NewRawDeviceSubscription with a window: as lhms_raw_subscription_new, each row summed over the last
+// `window` collections.
+LHMS_API void *lhms_raw_window_subscription_new(void *ms, uint32_t n_h, const char *const *h_names, uint32_t window,
+                                                lh_raw_board *out, int *status) {
+    int dummy;
+    if (!status) status = &dummy;
+    *status = LH_ERR_INVALID;
+    if (!ms || !out || (n_h && !h_names)) return nullptr;
+    try {
+        std::vector<std::string> hs(h_names, h_names + n_h);
+        auto *d = new RawDeviceSubscription(static_cast<MetricSystem *>(ms)->NewRawDeviceSubscription(hs, window));
         *out = d->board();
         *status = LH_OK;
         return d;

@@ -325,6 +325,11 @@ class DeviceSubscription {
 // the name is in Histograms, and is empty otherwise (percentiles INT32_MIN / NaN, ranks and totals 0).  A percentile
 // query with p equals what processMetrics reports for a label with that p, bit for bit.  A raw subscription reads; it
 // does not keep its names' ids alive.  Move-only.
+//
+// With a window w > 1 (lh_raw_board_create_window), row i answers for the sum of those per-collection histograms over
+// the last w collections (fewer before w have run): every collection publishes each open subscription once, a
+// collection in which the name is absent, recycled away or unbound enters as an empty interval, and rows follow names,
+// not ids.  After JoinRanks each entering interval is the job-wide one, so the window is job-wide too.
 class RawDeviceSubscription {
  public:
     RawDeviceSubscription() = default;
@@ -335,6 +340,8 @@ class RawDeviceSubscription {
     ~RawDeviceSubscription();
 
     const lh_raw_board &board() const;
+    // publishes summed per row (NewRawDeviceSubscription's window; 1 for a closed subscription)
+    uint32_t window() const;
     // lh_raw_percentiles_grid / lh_raw_ranks_grid: one kernel on `stream` answers every row for each of the m device
     // inputs (answers at [row * m + j]; Ranks' d_totals[row] is the total of query (row, 0)).  They may be captured
     // into a CUDA graph.  Throws std::runtime_error when the library refuses the call or the subscription is closed.
@@ -401,10 +408,11 @@ class MetricSystem {
     DeviceSubscription NewDeviceSubscription(const std::vector<std::string> &histograms,
                                              const std::vector<std::string> &counters);
     // A raw device subscription to these histogram names (RawDeviceSubscription): every collection from now on, the
-    // reaper's included, publishes their bucket counts into it.  Call it outside any stream capture.  Throws
-    // std::runtime_error when the library refuses lh_raw_board_create (more names than max_histograms, or none) or
-    // has no raw device subscriptions.
-    RawDeviceSubscription NewRawDeviceSubscription(const std::vector<std::string> &histograms);
+    // reaper's included, publishes their bucket counts into it, each row summed over the last `window` collections.
+    // Call it outside any stream capture.  Throws std::runtime_error when the library refuses lh_raw_board_create /
+    // lh_raw_board_create_window (more names than max_histograms, or none; window 0 or above LH_RAW_MAX_WINDOW) or has
+    // no raw device subscriptions (for window != 1: no window boards).
+    RawDeviceSubscription NewRawDeviceSubscription(const std::vector<std::string> &histograms, uint32_t window = 1);
     void RegisterGaugeFunc(const std::string &name, std::function<double()> f);   // :299
     // A gauge whose value lives in device memory: a scalar of type `dtype` (LH_GAUGE_*) at d_value, device or managed
     // memory of this system's device, which must stay allocated while registered.  Every collection reads all device

@@ -12,7 +12,8 @@ import sys
 from . import _lib as _L
 from . import build as _build
 from .engine import (_batch_array, _capture_stream, _stream, _timer_stream, board_out, board_views, gauge_src,
-                     graph_counter_args, graph_duration_out, graph_keyed_args, raw_percentiles, raw_ranks)
+                     graph_counter_args, graph_duration_out, graph_keyed_args, raw_percentiles, raw_ranks,
+                     check_window)
 
 _EMIT = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_char_p, C.c_int, C.c_uint64, C.c_double)
 _RANKS_SINK = C.CFUNCTYPE(None, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64)
@@ -115,6 +116,9 @@ def _bind(L):
     L.lhms_subscription_free.argtypes = [vp]
     L.lhms_raw_subscription_new.restype = vp
     L.lhms_raw_subscription_new.argtypes = [vp, C.c_uint32, names, C.POINTER(_L.lh_raw_board), C.POINTER(C.c_int)]
+    L.lhms_raw_window_subscription_new.restype = vp
+    L.lhms_raw_window_subscription_new.argtypes = [vp, C.c_uint32, names, C.c_uint32, C.POINTER(_L.lh_raw_board),
+                                                   C.POINTER(C.c_int)]
     for q in ("percentiles", "ranks"):
         getattr(L, "lhms_raw_subscription_" + q).restype = C.c_int
         getattr(L, "lhms_raw_subscription_" + q).argtypes = [vp, vp, C.c_uint32, vp, vp, vp, vp]
@@ -457,17 +461,24 @@ class RawDeviceSubscription:
     the bucket counts of its histogram names into `board`, an lh_raw_board in device memory that kernels query with
     lh::raw_percentile / lh::raw_rank / lh::raw_bucket_count (row numbers in `rows`), and percentiles() / ranks()
     query from torch.  Usable as a context manager; close() (also on exit) frees the board once no query of it is
-    pending."""
+    pending.  With `window` w > 1 every row answers for its name's histograms summed over the last w collections
+    (a collection without the name adds nothing)."""
 
-    def __init__(self, ms, histograms):
+    def __init__(self, ms, histograms, window=1):
+        window = check_window(window)
         self._ms = ms
         hnames = [str(x) for x in histograms]
         self.board = _L.lh_raw_board()
         hn = (C.c_char_p * max(len(hnames), 1))(*[x.encode() for x in hnames])
         st = C.c_int()
-        self._h = ms._lib.lhms_raw_subscription_new(ms._h, len(hnames), hn, C.byref(self.board), C.byref(st))
+        if window == 1:
+            self._h = ms._lib.lhms_raw_subscription_new(ms._h, len(hnames), hn, C.byref(self.board), C.byref(st))
+        else:
+            self._h = ms._lib.lhms_raw_window_subscription_new(ms._h, len(hnames), hn, window, C.byref(self.board),
+                                                                C.byref(st))
         if not self._h:
             raise RuntimeError("lhms_raw_subscription_new failed (status %d)" % st.value)
+        self.window = window
         self.rows = {nm: i for i, nm in enumerate(hnames)}
         self._device = ms._device
 
@@ -665,12 +676,14 @@ class MetricSystem:
         any stream capture."""
         return DeviceSubscription(self, histograms, counters)
 
-    def raw_device_subscription(self, histograms=()) -> RawDeviceSubscription:
+    def raw_device_subscription(self, histograms=(), window=1) -> RawDeviceSubscription:
         """SubscribeToRawMetrics for the GPU: every collection from now on (the reaper's included) publishes the bucket
         counts of these histogram names into device memory, where kernels, captured graphs and torch callers ask exact
         percentile and rank queries (RawDeviceSubscription).  `with ms.raw_device_subscription(histograms=[...]) as
-        raw:` closes it on exit.  Create it outside any stream capture."""
-        return RawDeviceSubscription(self, histograms)
+        raw:` closes it on exit.  Create it outside any stream capture.  `window` (an int >= 1): every row answers for
+        the sum of its name's histograms over the last `window` collections (TypeError / ValueError otherwise, before
+        any call)."""
+        return RawDeviceSubscription(self, histograms, window)
 
     def RegisterConstantGauge(self, name: str, value: float):
         self._lib.lhms_register_constant_gauge(self._h, name.encode(), float(value))
