@@ -11,6 +11,7 @@
 #include <condition_variable>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <string>
@@ -22,7 +23,43 @@ using namespace lh;
 
 namespace {
 
-struct WriterEvent { cudaStream_t stream; cudaEvent_t ev; };
+// Owners of one CUDA handle each (move-only): the handle is released when its owner is reset or destroyed.  out()
+// releases what is held and hands the slot to an allocating call.
+template <typename H, cudaError_t (*Release)(H)>
+class Owned {
+    H h_ = nullptr;
+public:
+    Owned() = default;
+    Owned(Owned &&o) noexcept : h_(o.h_) { o.h_ = nullptr; }
+    Owned &operator=(Owned &&o) noexcept { if (this != &o) { reset(); h_ = o.h_; o.h_ = nullptr; } return *this; }
+    ~Owned() { reset(); }
+    H get() const { return h_; }
+    H *out() { reset(); return &h_; }
+    void reset() { if (h_) Release(h_); h_ = nullptr; }
+};
+template <typename T> cudaError_t free_device(T *p) { return cudaFree(p); }
+template <typename T> cudaError_t free_pinned(T *p) { return cudaFreeHost(p); }
+template <typename T> using DevPtr = Owned<T *, free_device<T>>;      // cudaMalloc
+template <typename T> using PinnedPtr = Owned<T *, free_pinned<T>>;   // cudaMallocHost, cudaHostAlloc
+using Event = Owned<cudaEvent_t, cudaEventDestroy>;
+using Stream = Owned<cudaStream_t, cudaStreamDestroy>;
+
+// stream-ordered device memory (cudaMallocAsync), freed on the stream it was given, or on the one passed to reset
+class AsyncPtr {
+    char *p_ = nullptr;
+    cudaStream_t s_ = nullptr;
+public:
+    explicit AsyncPtr(cudaStream_t s = nullptr) : s_(s) {}
+    AsyncPtr(AsyncPtr &&o) noexcept : p_(o.p_), s_(o.s_) { o.p_ = nullptr; }
+    AsyncPtr &operator=(AsyncPtr &&o) noexcept { if (this != &o) { reset(); p_ = o.p_; s_ = o.s_; o.p_ = nullptr; } return *this; }
+    ~AsyncPtr() { reset(); }
+    char *get() const { return p_; }
+    char **out() { reset(); return &p_; }
+    cudaError_t reset() { return reset(s_); }
+    cudaError_t reset(cudaStream_t s) { const cudaError_t e = p_ ? cudaFreeAsync(p_, s) : cudaSuccess; p_ = nullptr; return e; }
+};
+
+struct WriterEvent { cudaStream_t stream; Event ev; };
 
 // an open record scope (lh_record_begin .. lh_record_end): device code is writing buffer `buf` from `stream`
 struct Scope { uint64_t ticket; int buf; cudaStream_t stream; std::thread::id thread; };
@@ -35,25 +72,26 @@ struct TimerSlot {
     uint32_t gen = 0;                  // bumped at every release: handles of earlier tokens stop matching
     uint8_t state = TIMER_FRESH;
     cudaStream_t start_stream = nullptr;
-    cudaEvent_t started = nullptr;     // after the mark (created on the slot's first use, kept)
+    Event started;                     // after the mark (created on the slot's first use, kept)
     std::vector<WriterEvent> stops;    // after the latest stop on each stream that stopped the token
 };
 
 // a graph recorder (lh_graph_recorder_*): rows it owns, drained into the frozen interval at every lh_snapshot_begin
 struct GraphRec {
     uint64_t handle;
+    AsyncPtr mem;                    // the one allocation behind rec and d_marks
     lh_recorder rec;                 // what the caller was given (rows, flags, counters in one allocation)
     unsigned long long *d_marks;     // [k] start marks of lh_graph_recorder_timer_* (kTimerNeverStarted until a start)
     std::vector<uint32_t> hid, cid;  // target id of each local row / counter (LH_GRAPH_UNBOUND = drop and count)
 };
 
 struct Buffer {
-    unsigned long long *d_buckets = nullptr;   // [H][65536]
-    unsigned long long *d_counters = nullptr;  // [C]
-    uint32_t *d_flags = nullptr;               // [H] 0 untouched / 1 window only / 3 also outside the window
-    unsigned int *d_hot = nullptr;             // [hot_replicas][H][2*win] uint32 window of the keyed path
+    DevPtr<unsigned long long> d_buckets;      // [H][65536]
+    DevPtr<unsigned long long> d_counters;     // [C]
+    DevPtr<uint32_t> d_flags;                  // [H] 0 untouched / 1 window only / 3 also outside the window
+    DevPtr<unsigned int> d_hot;                // [hot_replicas][H][2*win] uint32 window of the keyed path
     unsigned long long hot_pending = 0;        // samples added to d_hot since it was last drained
-    cudaEvent_t cleared = nullptr;             // zeroing finished
+    Event cleared;                             // zeroing finished
     std::vector<WriterEvent> writers;          // last ingest per stream
 };
 
@@ -61,9 +99,9 @@ enum SlotState { SLOT_FREE = 0, SLOT_ACQUIRED = 1 /* handed to the caller (lh_st
                  SLOT_WAITED = 3 /* a thread is waiting for its kernel, mutex released */,
                  SLOT_FILLING = 4 /* lh_*_host is copying pageable memory into it, mutex released */ };
 struct Slot {
-    void *h = nullptr; void *d = nullptr;
-    cudaEvent_t done = nullptr;      // kernel that consumed the slot has finished
-    cudaEvent_t copied = nullptr;    // H2D copy into the slot has landed
+    PinnedPtr<void> h; DevPtr<void> d;
+    Event done;                      // kernel that consumed the slot has finished
+    Event copied;                    // H2D copy into the slot has landed
     int state = SLOT_FREE;
     uint64_t seq = 0;
 };
@@ -162,14 +200,25 @@ struct PeerMap {                                   // one remote rank as mapped 
 // a live raw board (lh_raw_board_create / _window) and the host's bookkeeping of its window
 struct RawBoard {
     lh_raw_board b{};
+    AsyncPtr mem;                 // the one allocation behind b.d_rows
     uint32_t window = 1;          // publishes summed per row (1: a plain board, published by k_raw_publish)
     uint64_t published = 0;       // publishes issued; a window board's next one replaces slot published % window
     uint64_t snapshot = 0;        // stats.snapshots at its latest publish: a window board takes one per snapshot
 };
 
+// a live board (lh_board_create): what the caller was given, and the allocation behind b.d_board
+struct Board {
+    lh_board b{};
+    AsyncPtr mem;
+};
+
 }  // namespace
 
 struct lh_ctx {
+    // The streams come first: members are destroyed in reverse order, and stream-ordered allocations (graph recorders,
+    // boards) are freed on snap_stream, so the streams must outlive every other member.  This order must hold.
+    Stream ingest_stream, snap_stream, copy_stream;
+    Stream rs_stream;                    // lh_reduce_sparse_host's own (created on first use)
     lh_config cfg{};
     int device = 0;
     int sm_count = 0;
@@ -180,26 +229,25 @@ struct lh_ctx {
     bool frozen = false;
     bool freezing = false;               // lh_snapshot_begin flipped the buffers and waits for record scopes to end
     bool nnz_valid = false;
-    cudaStream_t ingest_stream = nullptr, snap_stream = nullptr, copy_stream = nullptr;
-    double *d_decomp = nullptr;
-    unsigned long long *d_dropped = nullptr;
+    DevPtr<double> d_decomp;
+    DevPtr<unsigned long long> d_dropped;
     // reduce / export scratch
     // two result slots (ticket & 1): packed [count H][sum H][avg H][pvals H*np][pkeys H*np]; slot 2 is scratch for
     // lh_snapshot_export when no reduction has produced the non-empty-bucket counts yet (never holds a ticket)
-    double *d_ps[3] = {nullptr, nullptr, nullptr};
-    char *d_res[3] = {nullptr, nullptr, nullptr};
-    char *h_res[3] = {nullptr, nullptr, nullptr};
-    cudaEvent_t res_done[3] = {nullptr, nullptr, nullptr};
+    DevPtr<double> d_ps[3];
+    DevPtr<char> d_res[3];
+    PinnedPtr<char> h_res[3];
+    Event res_done[3];
     uint32_t res_np[3] = {0, 0, 0};
     uint64_t res_ticket[2] = {0, 0};
     uint64_t next_ticket = 1;
-    uint32_t *d_nnz = nullptr, *d_offsets = nullptr;     // d_nnz: [3][H], the non-empty buckets K3 counted per result slot
+    DevPtr<uint32_t> d_nnz, d_offsets;                   // d_nnz: [3][H], the non-empty buckets K3 counted per result slot
     int nnz_slot = 0;                                    // the slot whose counts k_scan_nnz reads (the latest K3)
-    short *d_x_keys = nullptr; unsigned long long *d_x_counts = nullptr; size_t x_cap = 0;
+    DevPtr<short> d_x_keys; DevPtr<unsigned long long> d_x_counts; size_t x_cap = 0;
     // pinned host mirrors
-    uint32_t *h_offsets = nullptr;
-    short *h_x_keys = nullptr; unsigned long long *h_x_counts = nullptr; size_t hx_cap = 0;
-    unsigned long long *h_counter_deltas = nullptr;
+    PinnedPtr<uint32_t> h_offsets;
+    PinnedPtr<short> h_x_keys; PinnedPtr<unsigned long long> h_x_counts; size_t hx_cap = 0;
+    PinnedPtr<unsigned long long> h_counter_deltas;
     // staging ring
     std::vector<Slot> slots;
     uint64_t slot_seq = 0;
@@ -217,9 +265,9 @@ struct lh_ctx {
     uint32_t wc_flush_samples = 24576;  // samples a CTA bins between two flushes of its owner buffers
     int wc_spt = 6;                     // tile shape of that kernel (6: 896 threads x 4 samples; 4: 1024 x 4; 3: 768 x 4; 8: 512 x 8)
     // owner-partitioned keyed kernel scratch (allocated on first use)
-    unsigned short *d_kp_queues = nullptr;
-    unsigned int *d_kp_cnt = nullptr;     // per-(owner, writer) record counts, then the grid-barrier word
-    uint4 *d_kp_rare = nullptr;           // per-CTA lists of samples set aside for the exact path
+    DevPtr<unsigned short> d_kp_queues;
+    DevPtr<unsigned int> d_kp_cnt;        // per-(owner, writer) record counts, then the grid-barrier word
+    DevPtr<uint4> d_kp_rare;              // per-CTA lists of samples set aside for the exact path
     size_t kp_cap = 0;
     int kp_parts = 0;
     const char *keyed_kernel = "";       // kernel the last keyed launch used
@@ -228,56 +276,56 @@ struct lh_ctx {
     BatchParams batch_prm{};
     // multi-GPU (lh_comm_*): peer mappings of every rank's arrays + this rank's reduced output arrays
     uint32_t comm_rank = 0, comm_world = 0;
-    unsigned long long *d_comm = nullptr;         // this rank's comm block (uint64[kCommWords])
-    unsigned int *d_comm_aux = nullptr;           // [0] block counter, [1] status, [2..3] cells (both of the last all-reduce)
+    DevPtr<unsigned long long> d_comm;            // this rank's comm block (uint64[kCommWords])
+    DevPtr<unsigned int> d_comm_aux;              // [0] block counter, [1] status, [2..3] cells (both of the last all-reduce)
     PeerMap peers[kMaxRanks];
-    unsigned long long *d_red_buckets = nullptr;  // [H][65536] sums over ranks (valid for the open snapshot after lh_snapshot_allreduce)
-    uint32_t *d_red_flags = nullptr;
-    unsigned long long *d_red_counters = nullptr;
+    DevPtr<unsigned long long> d_red_buckets;     // [H][65536] sums over ranks (valid for the open snapshot after lh_snapshot_allreduce)
+    DevPtr<uint32_t> d_red_flags;
+    DevPtr<unsigned long long> d_red_counters;
     bool view_reduced = false;                    // the open snapshot's reduce/export read the reduced arrays
     bool view_counters_reduced = false;
     uint64_t comm_seq = 0;
     bool comm_two_shot = false;                    // form of the last all-reduce (lh_comm_info's byte count)
     static constexpr int kCommRing = 8;
-    cudaEvent_t comm_t0[kCommRing] = {}, comm_t1[kCommRing] = {};
+    Event comm_t0[kCommRing], comm_t1[kCommRing];
     // lh_snapshot_allreduce_rows: the row maps ([world][H] then [world][C] uint32, allocated at lh_comm_import), their
     // pinned staging, and an event behind the last upload (staging is rewritten only after it)
-    uint32_t *d_row_maps = nullptr, *h_row_maps = nullptr;
-    cudaEvent_t row_maps_copied = nullptr;
+    DevPtr<uint32_t> d_row_maps;
+    PinnedPtr<uint32_t> h_row_maps;
+    Event row_maps_copied;
     // lh_snapshot_rows: pinned staging of the frozen flags and counters (allocated on first use)
-    uint32_t *h_rows_flags = nullptr;
-    unsigned long long *h_rows_counters = nullptr;
+    PinnedPtr<uint32_t> h_rows_flags;
+    PinnedPtr<unsigned long long> h_rows_counters;
     uint64_t ctx_id = 0;
-    // lh_reduce_sparse_host: its own stream and K6_BATCH scratch rows (allocated on first use), serialised by rs_mu;
-    // none of the arrays above is touched by it
+    // lh_reduce_sparse_host: its own stream (rs_stream) and K6_BATCH scratch rows (allocated on first use), serialised
+    // by rs_mu; none of the arrays above is touched by it
     std::mutex rs_mu;
-    cudaStream_t rs_stream = nullptr;
-    unsigned long long *d_rs_rows = nullptr;      // [K6_BATCH][65536], all zero between calls
-    uint32_t *d_rs_flags = nullptr, *d_rs_nnz = nullptr;
+    DevPtr<unsigned long long> d_rs_rows;         // [K6_BATCH][65536], all zero between calls
+    DevPtr<uint32_t> d_rs_flags, d_rs_nnz;
     bool rs_dirty = false;                        // a call failed part-way: zero the rows before the next one
     K1Variant k1[kNumK1Variants];
     // timing of ingest: CUDA events bracket the kernels of every write_bracket (one sequence number); a ring keeps the
     // last kTimingRing pairs
     static constexpr int kTimingRing = 16;
-    cudaEvent_t ev_t0s[kTimingRing] = {}, ev_t1s[kTimingRing] = {};
+    Event ev_t0s[kTimingRing], ev_t1s[kTimingRing];
     cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;   // the pair of the bracket being issued
     uint64_t ingest_seq = 0;                         // brackets opened so far
     bool timing_valid = false;
     // GPU timers: a pool of 64-bit start marks on the device (allocated by the first lh_gpu_timer_start)
     uint32_t timer_slots_n = 65536;
-    unsigned long long *d_timer_marks = nullptr;
+    DevPtr<unsigned long long> d_timer_marks;
     std::vector<TimerSlot> timer_slots;
     std::vector<uint32_t> timer_released;            // released slots, oldest first, reused once their kernels are done
     uint32_t timer_fresh = 0;                         // slots [timer_fresh, n) have never been handed out
-    std::vector<cudaEvent_t> timer_spare_events;      // stop events of recycled slots
+    std::vector<Event> timer_spare_events;            // stop events of recycled slots
     // graph recorders, and the parameter block of their drain kernel (filled under the lock)
     std::vector<GraphRec> graphs;
     uint64_t next_graph = 1;
-    cudaEvent_t graph_drained = nullptr;               // after the latest collection drain (created with the first recorder)
+    Event graph_drained;                               // after the latest collection drain (created with the first recorder)
     DrainParams drain_prm{};
     // device subscriptions (lh_board_*): live boards, and the parameter block of their publish kernel (filled under the
     // lock); pub_slot is the result slot of the open snapshot's latest lh_snapshot_reduce(_async), -1 when there is none
-    std::vector<lh_board> boards;
+    std::vector<Board> boards;
     uint64_t next_board = 1;
     int pub_slot = -1;
     BoardParams board_prm{};
@@ -289,9 +337,10 @@ struct lh_ctx {
     // device gauges (lh_gauges_read): calls are serialised by gauge_mu (taken before mu), since they share the output
     // buffer, mapped pinned memory that k_gauge_read writes into (grown on demand); gauge_done follows the last launch
     std::mutex gauge_mu;
-    double *h_gauges = nullptr, *d_gauges = nullptr;
+    PinnedPtr<double> h_gauges;
+    double *d_gauges = nullptr;                        // h_gauges as the device sees it
     uint32_t gauge_cap = 0;
-    cudaEvent_t gauge_done = nullptr;
+    Event gauge_done;
     GaugeParams gauge_prm{};
     // stats
     lh_stats stats{};
@@ -333,27 +382,27 @@ struct RelaxedCapture {
 
 // order `s` after the zeroing of buffer b, and remember `s` as a writer of b
 lh_status before_write(lh_ctx *ctx, int b, cudaStream_t s) {
-    LH_CUDA(ctx, cudaStreamWaitEvent(s, ctx->buf[b].cleared, 0));
+    LH_CUDA(ctx, cudaStreamWaitEvent(s, ctx->buf[b].cleared.get(), 0));
     return LH_OK;
 }
 lh_status after_write(lh_ctx *ctx, int b, cudaStream_t s) {
     for (auto &w : ctx->buf[b].writers)
-        if (w.stream == s) { LH_CUDA(ctx, cudaEventRecord(w.ev, s)); return LH_OK; }
-    WriterEvent w{s, nullptr};
-    LH_CUDA(ctx, cudaEventCreateWithFlags(&w.ev, cudaEventDisableTiming));
-    LH_CUDA(ctx, cudaEventRecord(w.ev, s));
-    ctx->buf[b].writers.push_back(w);
+        if (w.stream == s) { LH_CUDA(ctx, cudaEventRecord(w.ev.get(), s)); return LH_OK; }
+    WriterEvent w{s, {}};
+    LH_CUDA(ctx, cudaEventCreateWithFlags(w.ev.out(), cudaEventDisableTiming));
+    LH_CUDA(ctx, cudaEventRecord(w.ev.get(), s));
+    ctx->buf[b].writers.push_back(std::move(w));
     return LH_OK;
 }
 
 void next_timing_slot(lh_ctx *ctx) {
     const int i = (int)(ctx->ingest_seq % lh_ctx::kTimingRing);
-    ctx->ev_t0 = ctx->ev_t0s[i];
-    ctx->ev_t1 = ctx->ev_t1s[i];
+    ctx->ev_t0 = ctx->ev_t0s[i].get();
+    ctx->ev_t1 = ctx->ev_t1s[i].get();
     ctx->ingest_seq++;
 }
 
-cudaStream_t pick_stream(lh_ctx *ctx, void *stream) { return stream ? (cudaStream_t)stream : ctx->ingest_stream; }
+cudaStream_t pick_stream(lh_ctx *ctx, void *stream) { return stream ? (cudaStream_t)stream : ctx->ingest_stream.get(); }
 
 int grid_1d(lh_ctx *ctx, size_t n, int threads, int per_thread, int blocks_per_sm) {
     size_t need = (n + (size_t)threads * per_thread - 1) / ((size_t)threads * per_thread);
@@ -384,10 +433,10 @@ lh_status write_bracket(lh_ctx *ctx, cudaStream_t s, Body body) {
 lh_recorder buffer_target(lh_ctx *ctx, int b) {
     lh_recorder rec;
     memset(&rec, 0, sizeof rec);
-    rec.d_buckets = reinterpret_cast<uint64_t *>(ctx->buf[b].d_buckets);
-    rec.d_flags = ctx->buf[b].d_flags;
-    rec.d_counters = reinterpret_cast<uint64_t *>(ctx->buf[b].d_counters);
-    rec.d_dropped = reinterpret_cast<uint64_t *>(ctx->d_dropped);
+    rec.d_buckets = reinterpret_cast<uint64_t *>(ctx->buf[b].d_buckets.get());
+    rec.d_flags = ctx->buf[b].d_flags.get();
+    rec.d_counters = reinterpret_cast<uint64_t *>(ctx->buf[b].d_counters.get());
+    rec.d_dropped = reinterpret_cast<uint64_t *>(ctx->d_dropped.get());
     rec.max_histograms = ctx->H;
     rec.max_counters = ctx->C;
     memcpy(rec.prec, &ctx->pc, sizeof ctx->pc);
@@ -422,7 +471,7 @@ lh_status launch_single(lh_ctx *ctx, unsigned long long *counts, uint32_t *flag,
 }
 // n samples of histogram hid into buffer b, counted in stats
 lh_status ingest_single(lh_ctx *ctx, int b, uint32_t hid, const double *d_values, size_t n, cudaStream_t s) {
-    lh_status st = launch_single(ctx, ctx->buf[b].d_buckets + (size_t)hid * 65536u, ctx->buf[b].d_flags + hid, d_values, n, s);
+    lh_status st = launch_single(ctx, ctx->buf[b].d_buckets.get() + (size_t)hid * 65536u, ctx->buf[b].d_flags.get() + hid, d_values, n, s);
     if (st == LH_OK) ctx->stats.samples += n;
     return st;
 }
@@ -430,7 +479,7 @@ lh_status ingest_single(lh_ctx *ctx, int b, uint32_t hid, const double *d_values
 lh_status fold_hot(lh_ctx *ctx, int b, cudaStream_t s) {
     const size_t cells = (size_t)ctx->H * 2u * ctx->pc.win;
     int grid = (int)std::min<size_t>((cells + 255) / 256, (size_t)ctx->sm_count * 16);
-    k_fold_hot<<<grid, 256, 0, s>>>(ctx->buf[b].d_hot, ctx->buf[b].d_buckets, ctx->buf[b].d_flags, cells, ctx->hot_replicas, ctx->pc.win);
+    k_fold_hot<<<grid, 256, 0, s>>>(ctx->buf[b].d_hot.get(), ctx->buf[b].d_buckets.get(), ctx->buf[b].d_flags.get(), cells, ctx->hot_replicas, ctx->pc.win);
     LH_CUDA(ctx, cudaGetLastError());
     ctx->stats.kernel_launches++;
     ctx->buf[b].hot_pending = 0;
@@ -439,8 +488,8 @@ lh_status fold_hot(lh_ctx *ctx, int b, cudaStream_t s) {
 
 KeyedOut keyed_out(lh_ctx *ctx, int b) {
     KeyedOut o{};
-    o.hot = ctx->buf[b].d_hot; o.buckets = ctx->buf[b].d_buckets; o.flags = ctx->buf[b].d_flags;
-    o.dropped = ctx->d_dropped; o.H = ctx->H;
+    o.hot = ctx->buf[b].d_hot.get(); o.buckets = ctx->buf[b].d_buckets.get(); o.flags = ctx->buf[b].d_flags.get();
+    o.dropped = ctx->d_dropped.get(); o.H = ctx->H;
     return o;
 }
 
@@ -590,8 +639,8 @@ template <typename IdT, typename ValT>
 lh_status launch_keyed_wc(lh_ctx *ctx, int b, const KeyedPlan &p, const IdT *ids, const ValT *vals, cudaStream_t s,
                           const IdT *ids2 = nullptr, const long long *vals2 = nullptr, const IdMap *map = nullptr) {
     const int P = p.grid;
-    if (!ctx->d_kp_queues || ctx->kp_cap != p.wc.cap || ctx->kp_parts != P) {
-        if (ctx->d_kp_queues) {
+    if (!ctx->d_kp_queues.get() || ctx->kp_cap != p.wc.cap || ctx->kp_parts != P) {
+        if (ctx->d_kp_queues.get()) {
             // a launch on another stream may still be using the old scratch
             cudaEvent_t done;
             {
@@ -600,11 +649,12 @@ lh_status launch_keyed_wc(lh_ctx *ctx, int b, const KeyedPlan &p, const IdT *ids
             }
             LH_CUDA(ctx, cudaEventSynchronize(done));
         }
-        cudaFree(ctx->d_kp_queues); cudaFree(ctx->d_kp_cnt); cudaFree(ctx->d_kp_rare);
-        ctx->d_kp_queues = nullptr; ctx->d_kp_cnt = nullptr; ctx->d_kp_rare = nullptr;
-        LH_CUDA(ctx, cudaMalloc(&ctx->d_kp_rare, (size_t)P * WC_RARE_CAP * sizeof(uint4)));
-        LH_CUDA(ctx, cudaMalloc(&ctx->d_kp_queues, (size_t)2 * P * P * p.wc.cap * sizeof(unsigned short)));
-        LH_CUDA(ctx, cudaMalloc(&ctx->d_kp_cnt, ((size_t)2 * P * P + 1) * sizeof(unsigned int)));
+        ctx->d_kp_queues.reset(); ctx->d_kp_cnt.reset(); ctx->d_kp_rare.reset();
+        DevPtr<unsigned short> queues; DevPtr<unsigned int> cnt; DevPtr<uint4> rare;
+        LH_CUDA(ctx, cudaMalloc(rare.out(), (size_t)P * WC_RARE_CAP * sizeof(uint4)));
+        LH_CUDA(ctx, cudaMalloc(queues.out(), (size_t)2 * P * P * p.wc.cap * sizeof(unsigned short)));
+        LH_CUDA(ctx, cudaMalloc(cnt.out(), ((size_t)2 * P * P + 1) * sizeof(unsigned int)));
+        ctx->d_kp_queues = std::move(queues); ctx->d_kp_cnt = std::move(cnt); ctx->d_kp_rare = std::move(rare);
         ctx->kp_cap = p.wc.cap; ctx->kp_parts = P;
     }
     // the kernel of the planned tile shape; with an int64 second segment, its PAIR form (on the float64 instantiation)
@@ -618,8 +668,8 @@ lh_status launch_keyed_wc(lh_ctx *ctx, int b, const KeyedPlan &p, const IdT *ids
     LH_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
     WcParams prm = p.wc;
     prm.ids = ids; prm.vals = vals; prm.ids2 = ids2; prm.vals2 = vals2;
-    prm.queues = ctx->d_kp_queues; prm.q_cnt = ctx->d_kp_cnt; prm.barrier = ctx->d_kp_cnt + (size_t)2 * P * P;
-    prm.rare = ctx->d_kp_rare; prm.o = keyed_out(ctx, b);
+    prm.queues = ctx->d_kp_queues.get(); prm.q_cnt = ctx->d_kp_cnt.get(); prm.barrier = ctx->d_kp_cnt.get() + (size_t)2 * P * P;
+    prm.rare = ctx->d_kp_rare.get(); prm.o = keyed_out(ctx, b);
     Prec pc = ctx->pc;
     IdIdentity ident;
     void *args[] = {&prm, &pc, map ? (void *)map : (void *)&ident};
@@ -651,7 +701,7 @@ lh_status launch_keyed(lh_ctx *ctx, int b, const IdT *d_ids, const ValT *d_vals,
             // the tally is host-side and counts what every stream has issued: the fold must come after all of it, not
             // only after this stream's kernels (each writer event follows the last bracket issued on its stream)
             for (const WriterEvent &w : ctx->buf[b].writers)
-                if (w.stream != s) LH_CUDA(ctx, cudaStreamWaitEvent(s, w.ev, 0));
+                if (w.stream != s) LH_CUDA(ctx, cudaStreamWaitEvent(s, w.ev.get(), 0));
             lh_status st = fold_hot(ctx, b, s);
             if (st != LH_OK) return st;
         }
@@ -738,22 +788,22 @@ lh_status launch_counter(lh_ctx *ctx, unsigned long long *counters, uint32_t C, 
             const size_t tail_off = head + n4 * 4;
             const size_t smem = (size_t)C * 8 + (map ? (size_t)C * 4 : 0);
             auto scalar = [&](int grid, size_t off, size_t cnt) {
-                if (map) k_counter_add_smem<IdT, T, IdMap><<<grid, T, smem, s>>>(d_ids + off, amts + off, cnt, counters, C, ctx->d_dropped, *map);
-                else k_counter_add_smem<IdT, T><<<grid, T, smem, s>>>(d_ids + off, amts + off, cnt, counters, C, ctx->d_dropped, IdIdentity{});
+                if (map) k_counter_add_smem<IdT, T, IdMap><<<grid, T, smem, s>>>(d_ids + off, amts + off, cnt, counters, C, ctx->d_dropped.get(), *map);
+                else k_counter_add_smem<IdT, T><<<grid, T, smem, s>>>(d_ids + off, amts + off, cnt, counters, C, ctx->d_dropped.get(), IdIdentity{});
                 ctx->stats.kernel_launches++;
             };
             if (head) scalar(1, 0, head);
             if (n4) {
                 // one CTA per SM (the per-CTA flush is C global atomics), fewer for small batches
                 const int grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)std::max(1, ctx->sm_count - ctx->k1_reserve_sms) * 2, n4 / (T * 4)));
-                if (map) k_counter_add_smem_vec<IdT, T, IdMap><<<grid, T, smem, s>>>(d_ids + head, amts + head, n4, counters, C, ctx->d_dropped, *map);
-                else k_counter_add_smem_vec<IdT, T><<<grid, T, smem, s>>>(d_ids + head, amts + head, n4, counters, C, ctx->d_dropped, IdIdentity{});
+                if (map) k_counter_add_smem_vec<IdT, T, IdMap><<<grid, T, smem, s>>>(d_ids + head, amts + head, n4, counters, C, ctx->d_dropped.get(), *map);
+                else k_counter_add_smem_vec<IdT, T><<<grid, T, smem, s>>>(d_ids + head, amts + head, n4, counters, C, ctx->d_dropped.get(), IdIdentity{});
                 ctx->stats.kernel_launches++;
             }
             if (tail_off < n) scalar(grid_1d(ctx, n - tail_off, T, 8, 2), tail_off, n - tail_off);
         } else {
             int grid = grid_1d(ctx, n, T, 4, 4);
-            k_counter_add<IdT, T><<<grid, T, 0, s>>>(d_ids, amts, n, counters, C, ctx->d_dropped);
+            k_counter_add<IdT, T><<<grid, T, 0, s>>>(d_ids, amts, n, counters, C, ctx->d_dropped.get());
             ctx->stats.kernel_launches++;
         }
         LH_CUDA(ctx, cudaGetLastError());
@@ -763,7 +813,7 @@ lh_status launch_counter(lh_ctx *ctx, unsigned long long *counters, uint32_t C, 
 // n counter ops into buffer b, counted in stats
 template <typename IdT>
 lh_status add_counters(lh_ctx *ctx, int b, const IdT *d_ids, const uint64_t *d_amounts, size_t n, cudaStream_t s) {
-    lh_status st = launch_counter<IdT>(ctx, ctx->buf[b].d_counters, ctx->C, d_ids, d_amounts, n, s);
+    lh_status st = launch_counter<IdT>(ctx, ctx->buf[b].d_counters.get(), ctx->C, d_ids, d_amounts, n, s);
     if (st == LH_OK) ctx->stats.counter_ops += n;
     return st;
 }
@@ -877,10 +927,10 @@ lh_status check_batch(lh_ctx *ctx, const lh_batch_item *h_items, uint32_t n_item
 // rows of buffer b, on s.
 lh_status drain_graphs(lh_ctx *ctx, const GraphRec *graphs, size_t n_graphs, int b, cudaStream_t s) {
     DrainParams &p = ctx->drain_prm;
-    p.buckets = ctx->buf[b].d_buckets;
-    p.flags = ctx->buf[b].d_flags;
-    p.counters = ctx->buf[b].d_counters;
-    p.dropped = ctx->d_dropped;
+    p.buckets = ctx->buf[b].d_buckets.get();
+    p.flags = ctx->buf[b].d_flags.get();
+    p.counters = ctx->buf[b].d_counters.get();
+    p.dropped = ctx->d_dropped.get();
     p.win = ctx->pc.win;
     p.n = 0;
     auto launch = [&]() -> lh_status {
@@ -927,25 +977,24 @@ lh_status slot_wait_free(lh_ctx *ctx, std::unique_lock<std::mutex> &lk, int *out
         for (size_t i = 0; i < ctx->slots.size(); i++) {
             if (ctx->slots[i].state == SLOT_WAITED || ctx->slots[i].state == SLOT_FILLING) waited++;   // will come back by itself
             if (ctx->slots[i].state != SLOT_FREE) continue;
-            if (ctx->slots[i].h) { *out = (int)i; return LH_OK; }
+            if (ctx->slots[i].h.get()) { *out = (int)i; return LH_OK; }
             if (fresh < 0) fresh = (int)i;
         }
         for (size_t i = 0; i < ctx->slots.size(); i++)
-            if (ctx->slots[i].state == SLOT_INFLIGHT && cudaEventQuery(ctx->slots[i].done) == cudaSuccess) {
+            if (ctx->slots[i].state == SLOT_INFLIGHT && cudaEventQuery(ctx->slots[i].done.get()) == cudaSuccess) {
                 ctx->slots[i].state = SLOT_FREE;
                 *out = (int)i;
                 return LH_OK;
             }
         cudaGetLastError();   // cudaErrorNotReady from the queries above is not an error
         if (fresh >= 0) {
-            Slot &sl = ctx->slots[fresh];
-            cudaError_t e = cudaMallocHost(&sl.h, ctx->staging_bytes);
-            if (e == cudaSuccess) e = cudaMalloc(&sl.d, ctx->staging_bytes);
-            if (e != cudaSuccess) {
-                if (sl.h) cudaFreeHost(sl.h);
-                sl.h = nullptr; sl.d = nullptr;
+            PinnedPtr<void> h; DevPtr<void> d;
+            cudaError_t e = cudaMallocHost(h.out(), ctx->staging_bytes);
+            if (e == cudaSuccess) e = cudaMalloc(d.out(), ctx->staging_bytes);
+            if (e != cudaSuccess)
                 return fail(ctx, e == cudaErrorMemoryAllocation ? LH_ERR_NOMEM : LH_ERR_CUDA, "allocating a staging slot", e);
-            }
+            ctx->slots[fresh].h = std::move(h);
+            ctx->slots[fresh].d = std::move(d);
             *out = fresh;
             return LH_OK;
         }
@@ -953,7 +1002,7 @@ lh_status slot_wait_free(lh_ctx *ctx, std::unique_lock<std::mutex> &lk, int *out
             if (ctx->slots[i].state == SLOT_INFLIGHT && (best < 0 || ctx->slots[i].seq < ctx->slots[best].seq)) best = (int)i;
         if (best >= 0) {
             ctx->slots[best].state = SLOT_WAITED;
-            cudaEvent_t ev = ctx->slots[best].done;
+            cudaEvent_t ev = ctx->slots[best].done.get();
             lk.unlock();
             cudaError_t e = cudaEventSynchronize(ev);
             lk.lock();
@@ -988,25 +1037,30 @@ void comm_unmap(lh_ctx *ctx) {
 
 // the arrays the all-reduce writes (this rank's own kernel and, for its slices, every peer's)
 lh_status comm_alloc_reduced(lh_ctx *ctx) {
-    if (ctx->d_red_buckets) return LH_OK;
+    if (ctx->d_red_buckets.get()) return LH_OK;
     const size_t bucket_bytes = (size_t)ctx->H * 65536u * 8u;
-    LH_CUDA(ctx, cudaMalloc(&ctx->d_red_buckets, bucket_bytes));
-    LH_CUDA(ctx, cudaMalloc(&ctx->d_red_flags, (size_t)ctx->H * 4));
-    LH_CUDA(ctx, cudaMalloc(&ctx->d_red_counters, (size_t)ctx->C * 8));
-    LH_CUDA(ctx, cudaMemsetAsync(ctx->d_red_buckets, 0, bucket_bytes, ctx->snap_stream));
-    LH_CUDA(ctx, cudaMemsetAsync(ctx->d_red_flags, 0, (size_t)ctx->H * 4, ctx->snap_stream));
-    LH_CUDA(ctx, cudaMemsetAsync(ctx->d_red_counters, 0, (size_t)ctx->C * 8, ctx->snap_stream));
-    LH_CUDA(ctx, cudaStreamSynchronize(ctx->snap_stream));
+    cudaStream_t s = ctx->snap_stream.get();
+    DevPtr<unsigned long long> buckets, counters; DevPtr<uint32_t> flags;
+    LH_CUDA(ctx, cudaMalloc(buckets.out(), bucket_bytes));
+    LH_CUDA(ctx, cudaMalloc(flags.out(), (size_t)ctx->H * 4));
+    LH_CUDA(ctx, cudaMalloc(counters.out(), (size_t)ctx->C * 8));
+    LH_CUDA(ctx, cudaMemsetAsync(buckets.get(), 0, bucket_bytes, s));
+    LH_CUDA(ctx, cudaMemsetAsync(flags.get(), 0, (size_t)ctx->H * 4, s));
+    LH_CUDA(ctx, cudaMemsetAsync(counters.get(), 0, (size_t)ctx->C * 8, s));
+    LH_CUDA(ctx, cudaStreamSynchronize(s));
+    ctx->d_red_buckets = std::move(buckets); ctx->d_red_flags = std::move(flags); ctx->d_red_counters = std::move(counters);
     return LH_OK;
 }
 
 // the row maps of lh_snapshot_allreduce_rows, sized for the largest world
 lh_status comm_alloc_row_maps(lh_ctx *ctx) {
-    if (ctx->d_row_maps) return LH_OK;
+    if (ctx->d_row_maps.get()) return LH_OK;
     const size_t bytes = (size_t)kMaxRanks * ((size_t)ctx->H + ctx->C) * 4u;
-    LH_CUDA(ctx, cudaMalloc(&ctx->d_row_maps, bytes));
-    LH_CUDA(ctx, cudaMallocHost(&ctx->h_row_maps, bytes));
-    LH_CUDA(ctx, cudaEventCreateWithFlags(&ctx->row_maps_copied, cudaEventDisableTiming));
+    DevPtr<uint32_t> d; PinnedPtr<uint32_t> h; Event copied;
+    LH_CUDA(ctx, cudaMalloc(d.out(), bytes));
+    LH_CUDA(ctx, cudaMallocHost(h.out(), bytes));
+    LH_CUDA(ctx, cudaEventCreateWithFlags(copied.out(), cudaEventDisableTiming));
+    ctx->d_row_maps = std::move(d); ctx->h_row_maps = std::move(h); ctx->row_maps_copied = std::move(copied);
     return LH_OK;
 }
 
@@ -1044,7 +1098,8 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return LH_ERR_NO_DEVICE; }
     if (cfg->device < 0 || cfg->device >= ndev) return LH_ERR_NO_DEVICE;
-    lh_ctx *ctx = new (std::nothrow) lh_ctx();
+    // released through lh_destroy on every failure below, handed out at the end
+    std::unique_ptr<lh_ctx, lh_status (*)(lh_ctx *)> ctx(new (std::nothrow) lh_ctx(), lh_destroy);
     if (!ctx) return LH_ERR_NOMEM;
     ctx->cfg = *cfg;
     ctx->device = cfg->device;
@@ -1071,7 +1126,6 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
         cudaError_t _e = (call);                                                        \
         if (_e != cudaSuccess) {                                                        \
             fprintf(stderr, "loghisto_b200: lh_create: %s failed: %s\n", #call, cudaGetErrorString(_e)); \
-            lh_destroy(ctx);                                                            \
             return _e == cudaErrorMemoryAllocation ? LH_ERR_NOMEM : LH_ERR_CUDA;        \
         }                                                                               \
     } while (0)
@@ -1081,65 +1135,64 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
     LH_CREATE_CUDA(cudaGetDeviceProperties(&prop, ctx->device));
     if (prop.major != 9 || prop.minor != 0) {   // sm_90a code runs on compute capability 9.0 only
         fprintf(stderr, "loghisto_b200: device %d is sm_%d%d; this library is built for sm_90a only\n", ctx->device, prop.major, prop.minor);
-        lh_destroy(ctx);
         return LH_ERR_NO_DEVICE;
     }
     ctx->sm_count = prop.multiProcessorCount;
-    LH_CREATE_CUDA(cudaStreamCreateWithFlags(&ctx->ingest_stream, cudaStreamNonBlocking));
-    LH_CREATE_CUDA(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
+    LH_CREATE_CUDA(cudaStreamCreateWithFlags(ctx->ingest_stream.out(), cudaStreamNonBlocking));
+    LH_CREATE_CUDA(cudaStreamCreateWithFlags(ctx->copy_stream.out(), cudaStreamNonBlocking));
     {   // the snapshot stream outranks ingest: its small kernels slot in as soon as any ingest CTA retires
         int least = 0, greatest = 0;
         LH_CREATE_CUDA(cudaDeviceGetStreamPriorityRange(&least, &greatest));
-        LH_CREATE_CUDA(cudaStreamCreateWithPriority(&ctx->snap_stream, cudaStreamNonBlocking, greatest));
+        LH_CREATE_CUDA(cudaStreamCreateWithPriority(ctx->snap_stream.out(), cudaStreamNonBlocking, greatest));
     }
     for (int i = 0; i < lh_ctx::kTimingRing; i++) {
-        LH_CREATE_CUDA(cudaEventCreate(&ctx->ev_t0s[i]));
-        LH_CREATE_CUDA(cudaEventCreate(&ctx->ev_t1s[i]));
+        LH_CREATE_CUDA(cudaEventCreate(ctx->ev_t0s[i].out()));
+        LH_CREATE_CUDA(cudaEventCreate(ctx->ev_t1s[i].out()));
     }
     for (int i = 0; i < lh_ctx::kCommRing; i++) {
-        LH_CREATE_CUDA(cudaEventCreate(&ctx->comm_t0[i]));
-        LH_CREATE_CUDA(cudaEventCreate(&ctx->comm_t1[i]));
+        LH_CREATE_CUDA(cudaEventCreate(ctx->comm_t0[i].out()));
+        LH_CREATE_CUDA(cudaEventCreate(ctx->comm_t1[i].out()));
     }
 
     const size_t bucket_bytes = (size_t)ctx->H * 65536u * 8u, counter_bytes = (size_t)ctx->C * 8u;
     const size_t hot_bytes = (size_t)ctx->hot_replicas * ctx->H * 2u * ctx->pc.win * 4u;
     for (int b = 0; b < 2; b++) {
-        LH_CREATE_CUDA(cudaMalloc(&ctx->buf[b].d_buckets, bucket_bytes));
-        LH_CREATE_CUDA(cudaMalloc(&ctx->buf[b].d_counters, counter_bytes));
-        LH_CREATE_CUDA(cudaMalloc(&ctx->buf[b].d_flags, (size_t)ctx->H * 4u));
-        LH_CREATE_CUDA(cudaMemsetAsync(ctx->buf[b].d_buckets, 0, bucket_bytes, ctx->snap_stream));
-        LH_CREATE_CUDA(cudaMemsetAsync(ctx->buf[b].d_counters, 0, counter_bytes, ctx->snap_stream));
-        LH_CREATE_CUDA(cudaMemsetAsync(ctx->buf[b].d_flags, 0, (size_t)ctx->H * 4u, ctx->snap_stream));
-        LH_CREATE_CUDA(cudaMalloc(&ctx->buf[b].d_hot, hot_bytes));
-        LH_CREATE_CUDA(cudaMemsetAsync(ctx->buf[b].d_hot, 0, hot_bytes, ctx->snap_stream));
-        LH_CREATE_CUDA(cudaEventCreateWithFlags(&ctx->buf[b].cleared, cudaEventDisableTiming));
-        LH_CREATE_CUDA(cudaEventRecord(ctx->buf[b].cleared, ctx->snap_stream));
+        LH_CREATE_CUDA(cudaMalloc(ctx->buf[b].d_buckets.out(), bucket_bytes));
+        LH_CREATE_CUDA(cudaMalloc(ctx->buf[b].d_counters.out(), counter_bytes));
+        LH_CREATE_CUDA(cudaMalloc(ctx->buf[b].d_flags.out(), (size_t)ctx->H * 4u));
+        LH_CREATE_CUDA(cudaMemsetAsync(ctx->buf[b].d_buckets.get(), 0, bucket_bytes, ctx->snap_stream.get()));
+        LH_CREATE_CUDA(cudaMemsetAsync(ctx->buf[b].d_counters.get(), 0, counter_bytes, ctx->snap_stream.get()));
+        LH_CREATE_CUDA(cudaMemsetAsync(ctx->buf[b].d_flags.get(), 0, (size_t)ctx->H * 4u, ctx->snap_stream.get()));
+        LH_CREATE_CUDA(cudaMalloc(ctx->buf[b].d_hot.out(), hot_bytes));
+        LH_CREATE_CUDA(cudaMemsetAsync(ctx->buf[b].d_hot.get(), 0, hot_bytes, ctx->snap_stream.get()));
+        LH_CREATE_CUDA(cudaEventCreateWithFlags(ctx->buf[b].cleared.out(), cudaEventDisableTiming));
+        LH_CREATE_CUDA(cudaEventRecord(ctx->buf[b].cleared.get(), ctx->snap_stream.get()));
     }
-    LH_CREATE_CUDA(cudaMalloc(&ctx->d_decomp, 65536 * sizeof(double)));
-    k_fill_decompress<<<65536 / 256, 256, 0, ctx->snap_stream>>>(ctx->d_decomp, ctx->pc.precision);
+    LH_CREATE_CUDA(cudaMalloc(ctx->d_decomp.out(), 65536 * sizeof(double)));
+    k_fill_decompress<<<65536 / 256, 256, 0, ctx->snap_stream.get()>>>(ctx->d_decomp.get(), ctx->pc.precision);
     LH_CREATE_CUDA(cudaGetLastError());
-    LH_CREATE_CUDA(cudaMalloc(&ctx->d_comm, kCommWords * 8));
-    LH_CREATE_CUDA(cudaMemsetAsync(ctx->d_comm, 0, kCommWords * 8, ctx->snap_stream));
-    LH_CREATE_CUDA(cudaMalloc(&ctx->d_comm_aux, 16));
-    LH_CREATE_CUDA(cudaMemsetAsync(ctx->d_comm_aux, 0, 16, ctx->snap_stream));
-    LH_CREATE_CUDA(cudaMalloc(&ctx->d_dropped, 8));
-    LH_CREATE_CUDA(cudaMemsetAsync(ctx->d_dropped, 0, 8, ctx->snap_stream));
+    LH_CREATE_CUDA(cudaMalloc(ctx->d_comm.out(), kCommWords * 8));
+    LH_CREATE_CUDA(cudaMemsetAsync(ctx->d_comm.get(), 0, kCommWords * 8, ctx->snap_stream.get()));
+    LH_CREATE_CUDA(cudaMalloc(ctx->d_comm_aux.out(), 16));
+    LH_CREATE_CUDA(cudaMemsetAsync(ctx->d_comm_aux.get(), 0, 16, ctx->snap_stream.get()));
+    LH_CREATE_CUDA(cudaMalloc(ctx->d_dropped.out(), 8));
+    LH_CREATE_CUDA(cudaMemsetAsync(ctx->d_dropped.get(), 0, 8, ctx->snap_stream.get()));
     for (int i = 0; i < 3; i++) {
         const size_t res_bytes = (size_t)ctx->H * (24 + LH_MAX_PERCENTILES * 12);
-        LH_CREATE_CUDA(cudaMalloc(&ctx->d_ps[i], LH_MAX_PERCENTILES * sizeof(double)));
-        LH_CREATE_CUDA(cudaMalloc(&ctx->d_res[i], res_bytes));
-        LH_CREATE_CUDA(cudaMallocHost(&ctx->h_res[i], res_bytes));
-        LH_CREATE_CUDA(cudaEventCreateWithFlags(&ctx->res_done[i], cudaEventDisableTiming));
+        LH_CREATE_CUDA(cudaMalloc(ctx->d_ps[i].out(), LH_MAX_PERCENTILES * sizeof(double)));
+        LH_CREATE_CUDA(cudaMalloc(ctx->d_res[i].out(), res_bytes));
+        LH_CREATE_CUDA(cudaMallocHost(ctx->h_res[i].out(), res_bytes));
+        LH_CREATE_CUDA(cudaEventCreateWithFlags(ctx->res_done[i].out(), cudaEventDisableTiming));
     }
-    LH_CREATE_CUDA(cudaMalloc(&ctx->d_nnz, (size_t)3 * ctx->H * 4));
-    LH_CREATE_CUDA(cudaMalloc(&ctx->d_offsets, ((size_t)ctx->H + 1) * 4));
-    LH_CREATE_CUDA(cudaMallocHost(&ctx->h_offsets, ((size_t)ctx->H + 1) * 4));
-    LH_CREATE_CUDA(cudaMallocHost(&ctx->h_counter_deltas, counter_bytes));
+    LH_CREATE_CUDA(cudaMalloc(ctx->d_nnz.out(), (size_t)3 * ctx->H * 4));
+    LH_CREATE_CUDA(cudaMalloc(ctx->d_offsets.out(), ((size_t)ctx->H + 1) * 4));
+    LH_CREATE_CUDA(cudaMallocHost(ctx->h_offsets.out(), ((size_t)ctx->H + 1) * 4));
+    LH_CREATE_CUDA(cudaMallocHost(ctx->h_counter_deltas.out(), counter_bytes));
 
     ctx->slots.resize(nslots);   // pinned + device memory of a slot is allocated the first time it is handed out
     for (auto &sl : ctx->slots) {
-        LH_CREATE_CUDA(cudaEventCreateWithFlags(&sl.done, cudaEventDisableTiming));
-        LH_CREATE_CUDA(cudaEventCreateWithFlags(&sl.copied, cudaEventDisableTiming));
+        LH_CREATE_CUDA(cudaEventCreateWithFlags(sl.done.out(), cudaEventDisableTiming));
+        LH_CREATE_CUDA(cudaEventCreateWithFlags(sl.copied.out(), cudaEventDisableTiming));
     }
 
     LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_reduce, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
@@ -1185,9 +1238,9 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
         LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_ingest_keyed_graph<unsigned short>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
         LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_ingest_keyed_graph<unsigned int>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
     }
-    LH_CREATE_CUDA(cudaStreamSynchronize(ctx->snap_stream));
+    LH_CREATE_CUDA(cudaStreamSynchronize(ctx->snap_stream.get()));
 #undef LH_CREATE_CUDA
-    *out = ctx;
+    *out = ctx.release();
     return LH_OK;
 }
 
@@ -1200,65 +1253,9 @@ extern "C" lh_status lh_destroy(lh_ctx *ctx) {
     }
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
-    for (auto &g : ctx->graphs) cudaFree(g.rec.d_buckets);
-    for (auto &b : ctx->boards) cudaFree(b.d_board);
-    for (auto &b : ctx->raw_boards) cudaFree(b.b.d_rows);   // the window's sums and slots too: one allocation
-    if (ctx->h_gauges) cudaFreeHost(ctx->h_gauges);
-    if (ctx->gauge_done) cudaEventDestroy(ctx->gauge_done);
-    if (ctx->graph_drained) cudaEventDestroy(ctx->graph_drained);
     comm_unmap(ctx);
-    cudaFree(ctx->d_comm); cudaFree(ctx->d_comm_aux);
-    cudaFree(ctx->d_red_buckets); cudaFree(ctx->d_red_flags); cudaFree(ctx->d_red_counters);
-    cudaFree(ctx->d_row_maps);
-    if (ctx->h_row_maps) cudaFreeHost(ctx->h_row_maps);
-    if (ctx->row_maps_copied) cudaEventDestroy(ctx->row_maps_copied);
-    if (ctx->h_rows_flags) cudaFreeHost(ctx->h_rows_flags);
-    if (ctx->h_rows_counters) cudaFreeHost(ctx->h_rows_counters);
-    for (int i = 0; i < lh_ctx::kCommRing; i++) {
-        if (ctx->comm_t0[i]) cudaEventDestroy(ctx->comm_t0[i]);
-        if (ctx->comm_t1[i]) cudaEventDestroy(ctx->comm_t1[i]);
-    }
-    for (int b = 0; b < 2; b++) {
-        cudaFree(ctx->buf[b].d_buckets); cudaFree(ctx->buf[b].d_counters); cudaFree(ctx->buf[b].d_hot); cudaFree(ctx->buf[b].d_flags);
-        if (ctx->buf[b].cleared) cudaEventDestroy(ctx->buf[b].cleared);
-        for (auto &w : ctx->buf[b].writers) cudaEventDestroy(w.ev);
-    }
-    cudaFree(ctx->d_decomp); cudaFree(ctx->d_dropped);
-    cudaFree(ctx->d_kp_queues); cudaFree(ctx->d_kp_cnt); cudaFree(ctx->d_kp_rare);
-    for (int i = 0; i < 3; i++) {
-        cudaFree(ctx->d_ps[i]); cudaFree(ctx->d_res[i]);
-        if (ctx->h_res[i]) cudaFreeHost(ctx->h_res[i]);
-        if (ctx->res_done[i]) cudaEventDestroy(ctx->res_done[i]);
-    }
-    cudaFree(ctx->d_nnz); cudaFree(ctx->d_offsets);
-    cudaFree(ctx->d_rs_rows); cudaFree(ctx->d_rs_flags); cudaFree(ctx->d_rs_nnz);
-    if (ctx->rs_stream) cudaStreamDestroy(ctx->rs_stream);
-    cudaFree(ctx->d_x_keys); cudaFree(ctx->d_x_counts);
-    if (ctx->h_offsets) cudaFreeHost(ctx->h_offsets);
-    if (ctx->h_x_keys) cudaFreeHost(ctx->h_x_keys);
-    if (ctx->h_x_counts) cudaFreeHost(ctx->h_x_counts);
-    if (ctx->h_counter_deltas) cudaFreeHost(ctx->h_counter_deltas);
-    for (auto &sl : ctx->slots) {
-        if (sl.h) cudaFreeHost(sl.h);
-        cudaFree(sl.d);
-        if (sl.done) cudaEventDestroy(sl.done);
-        if (sl.copied) cudaEventDestroy(sl.copied);
-    }
-    for (int i = 0; i < lh_ctx::kTimingRing; i++) {
-        if (ctx->ev_t0s[i]) cudaEventDestroy(ctx->ev_t0s[i]);
-        if (ctx->ev_t1s[i]) cudaEventDestroy(ctx->ev_t1s[i]);
-    }
-    cudaFree(ctx->d_timer_marks);   // whatever tokens are still held
-    for (auto &ts : ctx->timer_slots) {
-        if (ts.started) cudaEventDestroy(ts.started);
-        for (auto &w : ts.stops) cudaEventDestroy(w.ev);
-    }
-    for (cudaEvent_t ev : ctx->timer_spare_events) cudaEventDestroy(ev);
-    if (ctx->ingest_stream) cudaStreamDestroy(ctx->ingest_stream);
-    if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
-    if (ctx->snap_stream) cudaStreamDestroy(ctx->snap_stream);
-    cudaGetLastError();
-    delete ctx;
+    delete ctx;           // every other resource is released by its owner, the streams last (see lh_ctx)
+    cudaGetLastError();   // a release that failed leaves no error behind for the caller's next CUDA call
     return LH_OK;
 }
 
@@ -1368,7 +1365,7 @@ lh_status counter_add_mapped(lh_ctx *ctx, const uint32_t *h_map, uint32_t kc, co
     if (st != LH_OK || n == 0) return st;
     cudaStream_t s = pick_stream(ctx, stream);
     return write_bracket(ctx, s, [&](int b) {
-        lh_status r = launch_counter<IdT>(ctx, ctx->buf[b].d_counters, kc, d_ids, d_amounts, n, s, &m);
+        lh_status r = launch_counter<IdT>(ctx, ctx->buf[b].d_counters.get(), kc, d_ids, d_amounts, n, s, &m);
         if (r == LH_OK) ctx->stats.counter_ops += n;
         return r;
     });
@@ -1420,18 +1417,18 @@ enum HostKind { HK_SINGLE, HK_KEYED_U16, HK_COUNTER_U16, HK_KEYED_I64_U16 };
 // them, so the kernel time excludes the copy.  Unless a copy fails, the slot is in flight afterwards.
 lh_status staging_step(lh_ctx *ctx, Slot &sl, HostKind kind, uint32_t hid, const void *h_a, const void *h_ids, size_t n,
                        size_t ids_off) {
-    cudaStream_t cs = ctx->copy_stream, s = ctx->ingest_stream;
+    cudaStream_t cs = ctx->copy_stream.get(), s = ctx->ingest_stream.get();
     lh_status st = LH_OK;
     if (n) {
-        char *d_a = (char *)sl.d;
+        char *d_a = (char *)sl.d.get();
         const unsigned short *d_i = (const unsigned short *)(d_a + ids_off);
         // the device buffer is free again once the kernel that read it last is done (slot_wait_free already waited
         // on the host for a recycled slot, the event wait covers the rest)
-        if (sl.seq) LH_CUDA(ctx, cudaStreamWaitEvent(cs, sl.done, 0));
+        if (sl.seq) LH_CUDA(ctx, cudaStreamWaitEvent(cs, sl.done.get(), 0));
         LH_CUDA(ctx, cudaMemcpyAsync(d_a, h_a, n * 8, cudaMemcpyHostToDevice, cs));
         if (kind != HK_SINGLE) LH_CUDA(ctx, cudaMemcpyAsync(d_a + ids_off, h_ids, n * 2, cudaMemcpyHostToDevice, cs));
-        LH_CUDA(ctx, cudaEventRecord(sl.copied, cs));
-        LH_CUDA(ctx, cudaStreamWaitEvent(s, sl.copied, 0));
+        LH_CUDA(ctx, cudaEventRecord(sl.copied.get(), cs));
+        LH_CUDA(ctx, cudaStreamWaitEvent(s, sl.copied.get(), 0));
         ctx->stats.h2d_bytes += n * (kind == HK_SINGLE ? 8 : 10);
         st = write_bracket(ctx, s, [&](int b) {
             switch (kind) {
@@ -1442,7 +1439,7 @@ lh_status staging_step(lh_ctx *ctx, Slot &sl, HostKind kind, uint32_t hid, const
             }
         });
     }
-    LH_CUDA(ctx, cudaEventRecord(sl.done, s));
+    LH_CUDA(ctx, cudaEventRecord(sl.done.get(), s));
     sl.state = SLOT_INFLIGHT;
     sl.seq = ++ctx->slot_seq;
     ctx->slot_cv.notify_all();
@@ -1471,15 +1468,15 @@ lh_status ingest_host(lh_ctx *ctx, std::unique_lock<std::mutex> &lk, HostKind ki
             // the context mutex RELEASED -- the slot is parked as SLOT_FILLING so no other thread can take it.
             sl.state = SLOT_FILLING;
             lk.unlock();
-            memcpy(sl.h, src_a, m * 8);
-            if (h_ids) memcpy((char *)sl.h + per * 8, src_i, m * 2);
+            memcpy(sl.h.get(), src_a, m * 8);
+            if (h_ids) memcpy((char *)sl.h.get() + per * 8, src_i, m * 2);
             lk.lock();
-            src_a = sl.h;
-            src_i = (char *)sl.h + per * 8;
+            src_a = sl.h.get();
+            src_i = (char *)sl.h.get() + per * 8;
         }
         st = staging_step(ctx, sl, kind, hid, src_a, src_i, m, per * 8);
         if (st != LH_OK) return st;
-        last_copied = sl.copied;
+        last_copied = sl.copied.get();
         done += m;
     }
     if (pinned && last_copied) {
@@ -1521,23 +1518,24 @@ extern "C" lh_status lh_merge_counts_host(lh_ctx *ctx, const uint32_t *h_ids, co
     LH_ENTER(ctx);
     if (n && (!h_ids || !h_keys || !h_counts)) return fail(ctx, LH_ERR_INVALID, "NULL input");
     if (!n) return LH_OK;
-    cudaStream_t s = ctx->ingest_stream;
+    cudaStream_t s = ctx->ingest_stream.get();
     const int b = ctx->active;
     lh_status st = before_write(ctx, b, s);
     if (st != LH_OK) return st;
-    char *d = nullptr;
+    AsyncPtr buf(s);
     const size_t off_keys = n * 4, off_counts = ((n * 6 + 7) / 8) * 8, total = off_counts + n * 8;
-    LH_CUDA(ctx, cudaMallocAsync((void **)&d, total, s));
+    LH_CUDA(ctx, cudaMallocAsync((void **)buf.out(), total, s));
+    char *d = buf.get();
     cudaError_t e = cudaMemcpyAsync(d, h_ids, n * 4, cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d + off_keys, h_keys, n * 2, cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) e = cudaMemcpyAsync(d + off_counts, h_counts, n * 8, cudaMemcpyHostToDevice, s);
     if (e == cudaSuccess) {
         int grid = grid_1d(ctx, n, 256, 1, 8);
         k_merge_sparse<<<grid, 256, 0, s>>>((const uint32_t *)d, (const short *)(d + off_keys), (const unsigned long long *)(d + off_counts),
-                                            n, ctx->H, ctx->buf[b].d_buckets, ctx->buf[b].d_flags, ctx->d_dropped, ctx->pc.win);
+                                            n, ctx->H, ctx->buf[b].d_buckets.get(), ctx->buf[b].d_flags.get(), ctx->d_dropped.get(), ctx->pc.win);
         e = cudaGetLastError();
     }
-    cudaFreeAsync(d, s);
+    buf.reset();
     if (e != cudaSuccess) return fail(ctx, LH_ERR_CUDA, "lh_merge_counts_host", e);
     ctx->stats.kernel_launches++;
     ctx->stats.h2d_bytes += n * 14;
@@ -1553,7 +1551,7 @@ extern "C" lh_status lh_staging_acquire(lh_ctx *ctx, lh_staging *out) {
     lh_status st = slot_wait_free(ctx, _lk, &si);
     if (st != LH_OK) return st;
     ctx->slots[si].state = SLOT_ACQUIRED;
-    out->host = ctx->slots[si].h;
+    out->host = ctx->slots[si].h.get();
     out->bytes = ctx->staging_bytes;
     out->slot = (uint32_t)si;
     out->reserved = 0;
@@ -1572,7 +1570,7 @@ lh_status staging_commit(lh_ctx *ctx, const lh_staging *sg, HostKind kind, uint3
         if ((ids_offset & 15u) || ids_offset < item_bytes || ids_offset + n * 2 > ctx->staging_bytes)
             return fail(ctx, LH_ERR_RANGE, "ids_offset / n do not fit the staging slot");
     }
-    return staging_step(ctx, sl, kind, hid, sl.h, (char *)sl.h + ids_offset, n, ids_offset);
+    return staging_step(ctx, sl, kind, hid, sl.h.get(), (char *)sl.h.get() + ids_offset, n, ids_offset);
 }
 }  // namespace
 
@@ -1607,10 +1605,10 @@ extern "C" lh_status lh_record_begin(lh_ctx *ctx, void *stream, lh_recorder *out
     lh_status st = before_write(ctx, b, s);
     if (st != LH_OK) return st;
     memset(out, 0, sizeof *out);
-    out->d_buckets = reinterpret_cast<uint64_t *>(ctx->buf[b].d_buckets);
-    out->d_flags = ctx->buf[b].d_flags;
-    out->d_counters = reinterpret_cast<uint64_t *>(ctx->buf[b].d_counters);
-    out->d_dropped = reinterpret_cast<uint64_t *>(ctx->d_dropped);
+    out->d_buckets = reinterpret_cast<uint64_t *>(ctx->buf[b].d_buckets.get());
+    out->d_flags = ctx->buf[b].d_flags.get();
+    out->d_counters = reinterpret_cast<uint64_t *>(ctx->buf[b].d_counters.get());
+    out->d_dropped = reinterpret_cast<uint64_t *>(ctx->d_dropped.get());
     out->max_histograms = ctx->H;
     out->max_counters = ctx->C;
     out->block_smem_bytes = subhist_words(ctx->pc.win) * 4u;
@@ -1664,29 +1662,28 @@ extern "C" lh_status lh_graph_recorder_create(lh_ctx *ctx, uint32_t k, uint32_t 
     if (k > ctx->H || kc > ctx->C) return fail(ctx, LH_ERR_RANGE, "more rows than max_histograms / max_counters");
     if (!ids_ok(hist_ids, k, ctx->H) || !ids_ok(counter_ids, kc, ctx->C))
         return fail(ctx, LH_ERR_RANGE, "target id >= max_histograms / max_counters");
-    if (!ctx->graph_drained) LH_CUDA(ctx, cudaEventCreateWithFlags(&ctx->graph_drained, cudaEventDisableTiming));
+    if (!ctx->graph_drained.get()) LH_CUDA(ctx, cudaEventCreateWithFlags(ctx->graph_drained.out(), cudaEventDisableTiming));
     // one allocation: rows [k][65536], counters [kc], timer marks [k], flags [k]
     const size_t row_bytes = (size_t)k * 65536u * 8u, mark_off = row_bytes + (size_t)kc * 8u, flag_off = mark_off + (size_t)k * 8u;
     const size_t bytes = flag_off + (size_t)k * 4u;
-    cudaStream_t s = ctx->snap_stream;
-    char *base = nullptr;
-    LH_CUDA(ctx, cudaMallocAsync((void **)&base, bytes, s));
+    cudaStream_t s = ctx->snap_stream.get();
+    AsyncPtr mem(s);
+    LH_CUDA(ctx, cudaMallocAsync((void **)mem.out(), bytes, s));
+    char *base = mem.get();
     cudaError_t e = cudaMemsetAsync(base, 0, bytes, s);
     static_assert(kTimerNeverStarted == ~0ull, "marks are set bytewise");
     if (e == cudaSuccess) e = cudaMemsetAsync(base + mark_off, 0xFF, (size_t)k * 8u, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) {
-        cudaFreeAsync(base, s);
-        return fail(ctx, LH_ERR_CUDA, "lh_graph_recorder_create", e);
-    }
+    if (e != cudaSuccess) return fail(ctx, LH_ERR_CUDA, "lh_graph_recorder_create", e);
     GraphRec gr;
+    gr.mem = std::move(mem);
     gr.handle = graph_handle(ctx, ctx->next_graph++);
     memset(&gr.rec, 0, sizeof gr.rec);
     gr.rec.d_buckets = reinterpret_cast<uint64_t *>(base);
     gr.rec.d_counters = reinterpret_cast<uint64_t *>(base + row_bytes);
     gr.rec.d_flags = reinterpret_cast<uint32_t *>(base + flag_off);
     gr.d_marks = reinterpret_cast<unsigned long long *>(base + mark_off);
-    gr.rec.d_dropped = reinterpret_cast<uint64_t *>(ctx->d_dropped);
+    gr.rec.d_dropped = reinterpret_cast<uint64_t *>(ctx->d_dropped.get());
     gr.rec.max_histograms = k;
     gr.rec.max_counters = kc;
     gr.rec.block_smem_bytes = subhist_words(ctx->pc.win) * 4u;
@@ -1696,9 +1693,9 @@ extern "C" lh_status lh_graph_recorder_create(lh_ctx *ctx, uint32_t k, uint32_t 
     gr.cid.assign(kc, LH_GRAPH_UNBOUND);
     if (hist_ids) gr.hid.assign(hist_ids, hist_ids + k);
     if (counter_ids) gr.cid.assign(counter_ids, counter_ids + kc);
-    ctx->graphs.push_back(gr);
     out->handle = gr.handle;
     out->rec = gr.rec;
+    ctx->graphs.push_back(std::move(gr));
     return LH_OK;
 }
 
@@ -1797,7 +1794,7 @@ extern "C" lh_status lh_graph_recorder_timer_stop(lh_ctx *ctx, const lh_graph_re
     if (((uintptr_t)d_duration_ns & 7u) != 0) return fail(ctx, LH_ERR_INVALID, "d_duration_ns must be 8-byte aligned");
     k_gpu_timer_stop<<<1, 1, 0, pick_stream(ctx, stream)>>>(
         gr->d_marks + histogram, reinterpret_cast<unsigned long long *>(gr->rec.d_buckets) + (size_t)histogram * 65536u,
-        gr->rec.d_flags + histogram, reinterpret_cast<long long *>(d_duration_ns), ctx->d_dropped, ctx->pc);
+        gr->rec.d_flags + histogram, reinterpret_cast<long long *>(d_duration_ns), ctx->d_dropped.get(), ctx->pc);
     LH_CUDA(ctx, cudaGetLastError());
     ctx->stats.kernel_launches++;
     return LH_OK;
@@ -1809,10 +1806,10 @@ extern "C" lh_status lh_graph_recorder_destroy(lh_ctx *ctx, const lh_graph_recor
     if (!gr) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign graph recorder");
     cudaStream_t s = pick_stream(ctx, stream);
     // after every collection drain issued so far, then the final drain, then the free: all stream-ordered on s
-    LH_CUDA(ctx, cudaStreamWaitEvent(s, ctx->graph_drained, 0));
+    LH_CUDA(ctx, cudaStreamWaitEvent(s, ctx->graph_drained.get(), 0));
     lh_status st = write_bracket(ctx, s, [&](int b) { return drain_graphs(ctx, gr, 1, b, s); });
     if (st != LH_OK) return st;
-    LH_CUDA(ctx, cudaFreeAsync(gr->rec.d_buckets, s));
+    LH_CUDA(ctx, gr->mem.reset(s));
     ctx->graphs.erase(ctx->graphs.begin() + (gr - ctx->graphs.data()));
     return LH_OK;
 }
@@ -1847,8 +1844,8 @@ lh_status refuse_capture(lh_ctx *ctx, cudaStream_t s) {
 
 // every kernel that read or wrote the slot has completed (queried, never waited for)
 bool timer_slot_idle(const TimerSlot &ts) {
-    bool idle = cudaEventQuery(ts.started) == cudaSuccess;
-    for (const auto &w : ts.stops) idle = idle && cudaEventQuery(w.ev) == cudaSuccess;
+    bool idle = cudaEventQuery(ts.started.get()) == cudaSuccess;
+    for (const auto &w : ts.stops) idle = idle && cudaEventQuery(w.ev.get()) == cudaSuccess;
     cudaGetLastError();   // cudaErrorNotReady is not an error
     return idle;
 }
@@ -1856,9 +1853,11 @@ bool timer_slot_idle(const TimerSlot &ts) {
 // A slot for a new token: the oldest released slot if its kernels are done, else a fresh one, else any released slot
 // whose kernels are done.
 lh_status timer_take(lh_ctx *ctx, uint32_t *out) {
-    if (!ctx->d_timer_marks) {
-        LH_CUDA(ctx, cudaMalloc(&ctx->d_timer_marks, (size_t)ctx->timer_slots_n * sizeof(unsigned long long)));
+    if (!ctx->d_timer_marks.get()) {
+        DevPtr<unsigned long long> marks;
+        LH_CUDA(ctx, cudaMalloc(marks.out(), (size_t)ctx->timer_slots_n * sizeof(unsigned long long)));
         ctx->timer_slots.resize(ctx->timer_slots_n);
+        ctx->d_timer_marks = std::move(marks);
     }
     const bool fresh = ctx->timer_fresh < ctx->timer_slots_n;
     const size_t scan = fresh ? std::min<size_t>(1, ctx->timer_released.size()) : ctx->timer_released.size();
@@ -1867,7 +1866,7 @@ lh_status timer_take(lh_ctx *ctx, uint32_t *out) {
         TimerSlot &ts = ctx->timer_slots[k];
         if (!timer_slot_idle(ts)) continue;
         ctx->timer_released.erase(ctx->timer_released.begin() + (long)i);
-        for (auto &w : ts.stops) ctx->timer_spare_events.push_back(w.ev);
+        for (auto &w : ts.stops) ctx->timer_spare_events.push_back(std::move(w.ev));
         ts.stops.clear();
         *out = k;
         return LH_OK;
@@ -1887,12 +1886,12 @@ extern "C" lh_status lh_gpu_timer_start(lh_ctx *ctx, void *stream, lh_gpu_timer 
     st = timer_take(ctx, &k);
     if (st != LH_OK) return st;
     TimerSlot &ts = ctx->timer_slots[k];
-    cudaError_t e = ts.started ? cudaSuccess : cudaEventCreateWithFlags(&ts.started, cudaEventDisableTiming);
+    cudaError_t e = ts.started.get() ? cudaSuccess : cudaEventCreateWithFlags(ts.started.out(), cudaEventDisableTiming);
     if (e == cudaSuccess) {
-        k_gpu_timer_mark<<<1, 1, 0, s>>>(ctx->d_timer_marks + k);
+        k_gpu_timer_mark<<<1, 1, 0, s>>>(ctx->d_timer_marks.get() + k);
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaEventRecord(ts.started, s);
+    if (e == cudaSuccess) e = cudaEventRecord(ts.started.get(), s);
     if (e != cudaSuccess) {   // back to the pool, behind whatever may have been enqueued
         ts.state = TIMER_RELEASED;
         ctx->timer_released.push_back(k);
@@ -1914,11 +1913,11 @@ extern "C" lh_status lh_gpu_timer_stop(lh_ctx *ctx, const lh_gpu_timer *t, uint3
     TimerSlot *ts = timer_slot(ctx, t);
     if (!ts) return fail(ctx, LH_ERR_INVALID, "released, stale or foreign GPU timer handle");
     if (((uintptr_t)d_out & 7u) != 0) return fail(ctx, LH_ERR_INVALID, "d_duration_ns must be 8-byte aligned");
-    if (s != ts->start_stream) LH_CUDA(ctx, cudaStreamWaitEvent(s, ts->started, 0));
-    const unsigned long long *mark = ctx->d_timer_marks + (ts - ctx->timer_slots.data());
+    if (s != ts->start_stream) LH_CUDA(ctx, cudaStreamWaitEvent(s, ts->started.get(), 0));
+    const unsigned long long *mark = ctx->d_timer_marks.get() + (ts - ctx->timer_slots.data());
     st = write_bracket(ctx, s, [&](int b) -> lh_status {
-        k_gpu_timer_stop<<<1, 1, 0, s>>>(mark, ctx->buf[b].d_buckets + (size_t)hid * 65536u, ctx->buf[b].d_flags + hid,
-                                         reinterpret_cast<long long *>(d_out), ctx->d_dropped, ctx->pc);
+        k_gpu_timer_stop<<<1, 1, 0, s>>>(mark, ctx->buf[b].d_buckets.get() + (size_t)hid * 65536u, ctx->buf[b].d_flags.get() + hid,
+                                         reinterpret_cast<long long *>(d_out), ctx->d_dropped.get(), ctx->pc);
         LH_CUDA(ctx, cudaGetLastError());
         ctx->stats.kernel_launches++;
         ctx->stats.samples++;
@@ -1927,16 +1926,16 @@ extern "C" lh_status lh_gpu_timer_stop(lh_ctx *ctx, const lh_gpu_timer *t, uint3
     if (st != LH_OK) return st;
     // the slot is not handed out again before this stop has run (one event per stream that stopped the token)
     for (auto &w : ts->stops)
-        if (w.stream == s) { LH_CUDA(ctx, cudaEventRecord(w.ev, s)); return LH_OK; }
-    WriterEvent w{s, nullptr};
+        if (w.stream == s) { LH_CUDA(ctx, cudaEventRecord(w.ev.get(), s)); return LH_OK; }
+    WriterEvent w{s, {}};
     if (!ctx->timer_spare_events.empty()) {
-        w.ev = ctx->timer_spare_events.back();
+        w.ev = std::move(ctx->timer_spare_events.back());
         ctx->timer_spare_events.pop_back();
     } else {
-        LH_CUDA(ctx, cudaEventCreateWithFlags(&w.ev, cudaEventDisableTiming));
+        LH_CUDA(ctx, cudaEventCreateWithFlags(w.ev.out(), cudaEventDisableTiming));
     }
-    ts->stops.push_back(w);
-    LH_CUDA(ctx, cudaEventRecord(w.ev, s));
+    ts->stops.push_back(std::move(w));
+    LH_CUDA(ctx, cudaEventRecord(ts->stops.back().ev.get(), s));
     return LH_OK;
 }
 
@@ -1974,14 +1973,14 @@ extern "C" lh_status lh_snapshot_begin(lh_ctx *ctx) {
         ctx->freezing = false;
     }
     // order the snapshot stream after every ingest launch that wrote the buffer being frozen
-    for (auto &w : ctx->buf[f].writers) LH_CUDA(ctx, cudaStreamWaitEvent(ctx->snap_stream, w.ev, 0));
+    for (auto &w : ctx->buf[f].writers) LH_CUDA(ctx, cudaStreamWaitEvent(ctx->snap_stream.get(), w.ev.get(), 0));
     if (!ctx->graphs.empty()) {   // what graph recorders hold so far joins the interval being frozen
-        lh_status st = drain_graphs(ctx, ctx->graphs.data(), ctx->graphs.size(), f, ctx->snap_stream);
+        lh_status st = drain_graphs(ctx, ctx->graphs.data(), ctx->graphs.size(), f, ctx->snap_stream.get());
         if (st != LH_OK) return st;
-        LH_CUDA(ctx, cudaEventRecord(ctx->graph_drained, ctx->snap_stream));
+        LH_CUDA(ctx, cudaEventRecord(ctx->graph_drained.get(), ctx->snap_stream.get()));
     }
     if (ctx->buf[f].hot_pending) {   // drain the keyed path's uint32 window into the uint64 buckets
-        lh_status st = fold_hot(ctx, f, ctx->snap_stream);
+        lh_status st = fold_hot(ctx, f, ctx->snap_stream.get());
         if (st != LH_OK) return st;
     }
     ctx->active = f ^ 1;
@@ -1999,12 +1998,12 @@ extern "C" lh_status lh_snapshot_device(lh_ctx *ctx, lh_device_view *out) {
     if (!out) return fail(ctx, LH_ERR_INVALID, "out is NULL");
     if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
     const int f = ctx->active ^ 1;
-    out->d_buckets = reinterpret_cast<uint64_t *>(ctx->buf[f].d_buckets);
-    out->d_counters = reinterpret_cast<uint64_t *>(ctx->buf[f].d_counters);
+    out->d_buckets = reinterpret_cast<uint64_t *>(ctx->buf[f].d_buckets.get());
+    out->d_counters = reinterpret_cast<uint64_t *>(ctx->buf[f].d_counters.get());
     out->n_bucket_words = (uint64_t)ctx->H * 65536u;
     out->n_counter_words = ctx->C;
-    out->stream = ctx->snap_stream;
-    out->d_flags = ctx->buf[f].d_flags;
+    out->stream = ctx->snap_stream.get();
+    out->d_flags = ctx->buf[f].d_flags.get();
     out->n_flag_words = ctx->H;
     return LH_OK;
 }
@@ -2024,9 +2023,9 @@ struct View { const unsigned long long *buckets; const uint32_t *flags; const un
 View snapshot_view(lh_ctx *ctx) {
     const int f = ctx->active ^ 1;
     View v;
-    v.buckets = ctx->view_reduced ? ctx->d_red_buckets : ctx->buf[f].d_buckets;
-    v.flags = ctx->view_reduced ? ctx->d_red_flags : ctx->buf[f].d_flags;
-    v.counters = ctx->view_counters_reduced ? ctx->d_red_counters : ctx->buf[f].d_counters;
+    v.buckets = ctx->view_reduced ? ctx->d_red_buckets.get() : ctx->buf[f].d_buckets.get();
+    v.flags = ctx->view_reduced ? ctx->d_red_flags.get() : ctx->buf[f].d_flags.get();
+    v.counters = ctx->view_counters_reduced ? ctx->d_red_counters.get() : ctx->buf[f].d_counters.get();
     return v;
 }
 
@@ -2039,21 +2038,21 @@ uint32_t k3_smem_cells(uint32_t win) {
 
 // enqueue K3 + one packed D2H for the open snapshot into result slot `slot`
 lh_status enqueue_reduce(lh_ctx *ctx, const double *ps, uint32_t np, int slot) {
-    cudaStream_t s = ctx->snap_stream;
+    cudaStream_t s = ctx->snap_stream.get();
     const ResLayout l = res_layout(ctx->H, np);
     const View v = snapshot_view(ctx);
     if (np) {
-        LH_CUDA(ctx, cudaMemcpyAsync(ctx->d_ps[slot], ps, np * sizeof(double), cudaMemcpyHostToDevice, s));
+        LH_CUDA(ctx, cudaMemcpyAsync(ctx->d_ps[slot].get(), ps, np * sizeof(double), cudaMemcpyHostToDevice, s));
     }
-    char *d = ctx->d_res[slot];
+    char *d = ctx->d_res[slot].get();
     const uint32_t smem_cells = k3_smem_cells(ctx->pc.win);
-    k_reduce<<<ctx->H, K3_THREADS, (size_t)smem_cells * 8, s>>>(v.buckets, v.flags, ctx->pc.win, ctx->d_decomp, ctx->d_ps[slot], (int)np,
+    k_reduce<<<ctx->H, K3_THREADS, (size_t)smem_cells * 8, s>>>(v.buckets, v.flags, ctx->pc.win, ctx->d_decomp.get(), ctx->d_ps[slot].get(), (int)np,
                                            (unsigned long long *)(d + l.count), (double *)(d + l.sum), (double *)(d + l.avg),
-                                           (int *)(d + l.pkeys), (double *)(d + l.pvals), ctx->d_nnz + (size_t)slot * ctx->H,
+                                           (int *)(d + l.pkeys), (double *)(d + l.pvals), ctx->d_nnz.get() + (size_t)slot * ctx->H,
                                            smem_cells);
     LH_CUDA(ctx, cudaGetLastError());
-    LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_res[slot], d, l.total, cudaMemcpyDeviceToHost, s));
-    LH_CUDA(ctx, cudaEventRecord(ctx->res_done[slot], s));
+    LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_res[slot].get(), d, l.total, cudaMemcpyDeviceToHost, s));
+    LH_CUDA(ctx, cudaEventRecord(ctx->res_done[slot].get(), s));
     ctx->stats.kernel_launches++;
     ctx->stats.d2h_bytes += l.total;
     ctx->nnz_valid = true;
@@ -2073,7 +2072,7 @@ extern "C" lh_status lh_snapshot_reduce_async(lh_ctx *ctx, const double *percent
     // the slot's previous results (ticket t-2) are overwritten: make sure its copy is not still in flight
     // (waited for with the mutex released: ingest threads are not held up)
     if (ctx->res_ticket[slot]) {
-        cudaEvent_t ev = ctx->res_done[slot];
+        cudaEvent_t ev = ctx->res_done[slot].get();
         _lk.unlock();
         cudaError_t e = cudaEventSynchronize(ev);
         _lk.lock();
@@ -2097,7 +2096,7 @@ extern "C" lh_status lh_snapshot_result(lh_ctx *ctx, uint64_t ticket, uint64_t *
     {
         std::lock_guard<std::mutex> lk(ctx->mu);
         if (ticket == 0 || ctx->res_ticket[slot] != ticket) return fail(ctx, LH_ERR_STATE, "ticket expired or unknown");
-        ev = ctx->res_done[slot];
+        ev = ctx->res_done[slot].get();
     }
     // wait outside the lock so ingest threads are not held up by the reaper
     cudaError_t e = cudaEventSynchronize(ev);
@@ -2107,7 +2106,7 @@ extern "C" lh_status lh_snapshot_result(lh_ctx *ctx, uint64_t ticket, uint64_t *
     const size_t H = ctx->H;
     const uint32_t np = ctx->res_np[slot];
     const ResLayout l = res_layout(H, np);
-    const char *h = ctx->h_res[slot];
+    const char *h = ctx->h_res[slot].get();
     if (counts) memcpy(counts, h + l.count, H * 8);
     if (sums) memcpy(sums, h + l.sum, H * 8);
     if (avgs) memcpy(avgs, h + l.avg, H * 8);
@@ -2128,7 +2127,7 @@ extern "C" lh_status lh_snapshot_export(lh_ctx *ctx, lh_sparse *out) {
     LH_ENTER(ctx);
     if (!out) return fail(ctx, LH_ERR_INVALID, "out is NULL");
     if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
-    cudaStream_t s = ctx->snap_stream;
+    cudaStream_t s = ctx->snap_stream.get();
     const View v = snapshot_view(ctx);
     if (!ctx->nnz_valid) {
         // non-empty bucket counts come out of K3: run it with no percentiles into the scratch result slot, which never
@@ -2136,37 +2135,36 @@ extern "C" lh_status lh_snapshot_export(lh_ctx *ctx, lh_sparse *out) {
         lh_status st = enqueue_reduce(ctx, nullptr, 0, 2);
         if (st != LH_OK) return st;
     }
-    k_scan_nnz<<<1, 1024, 0, s>>>(ctx->d_nnz + (size_t)ctx->nnz_slot * ctx->H, ctx->H, ctx->d_offsets);
+    k_scan_nnz<<<1, 1024, 0, s>>>(ctx->d_nnz.get() + (size_t)ctx->nnz_slot * ctx->H, ctx->H, ctx->d_offsets.get());
     LH_CUDA(ctx, cudaGetLastError());
-    LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_offsets, ctx->d_offsets, ((size_t)ctx->H + 1) * 4, cudaMemcpyDeviceToHost, s));
-    LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_counter_deltas, v.counters, (size_t)ctx->C * 8, cudaMemcpyDeviceToHost, s));
+    LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_offsets.get(), ctx->d_offsets.get(), ((size_t)ctx->H + 1) * 4, cudaMemcpyDeviceToHost, s));
+    LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_counter_deltas.get(), v.counters, (size_t)ctx->C * 8, cudaMemcpyDeviceToHost, s));
     LH_CUDA(ctx, cudaStreamSynchronize(s));
-    const size_t total = ctx->h_offsets[ctx->H];
+    const size_t total = ctx->h_offsets.get()[ctx->H];
     if (total > ctx->x_cap) {
         size_t cap = std::max<size_t>(total, 4096) * 2;
-        cudaFree(ctx->d_x_keys); cudaFree(ctx->d_x_counts);
-        if (ctx->h_x_keys) cudaFreeHost(ctx->h_x_keys);
-        if (ctx->h_x_counts) cudaFreeHost(ctx->h_x_counts);
-        ctx->d_x_keys = nullptr; ctx->d_x_counts = nullptr; ctx->h_x_keys = nullptr; ctx->h_x_counts = nullptr; ctx->x_cap = 0;
-        LH_CUDA(ctx, cudaMalloc(&ctx->d_x_keys, cap * 2));
-        LH_CUDA(ctx, cudaMalloc(&ctx->d_x_counts, cap * 8));
-        LH_CUDA(ctx, cudaMallocHost(&ctx->h_x_keys, cap * 2));
-        LH_CUDA(ctx, cudaMallocHost(&ctx->h_x_counts, cap * 8));
-        ctx->x_cap = cap;
+        ctx->d_x_keys.reset(); ctx->d_x_counts.reset(); ctx->h_x_keys.reset(); ctx->h_x_counts.reset(); ctx->x_cap = 0;
+        DevPtr<short> d_keys; DevPtr<unsigned long long> d_counts; PinnedPtr<short> h_keys; PinnedPtr<unsigned long long> h_counts;
+        LH_CUDA(ctx, cudaMalloc(d_keys.out(), cap * 2));
+        LH_CUDA(ctx, cudaMalloc(d_counts.out(), cap * 8));
+        LH_CUDA(ctx, cudaMallocHost(h_keys.out(), cap * 2));
+        LH_CUDA(ctx, cudaMallocHost(h_counts.out(), cap * 8));
+        ctx->d_x_keys = std::move(d_keys); ctx->d_x_counts = std::move(d_counts); ctx->x_cap = cap;
+        ctx->h_x_keys = std::move(h_keys); ctx->h_x_counts = std::move(h_counts);
     }
     if (total) {
-        k_export<<<ctx->H, K3_THREADS, 0, s>>>(v.buckets, v.flags, ctx->pc.win, ctx->d_offsets, ctx->d_x_keys, ctx->d_x_counts);
+        k_export<<<ctx->H, K3_THREADS, 0, s>>>(v.buckets, v.flags, ctx->pc.win, ctx->d_offsets.get(), ctx->d_x_keys.get(), ctx->d_x_counts.get());
         LH_CUDA(ctx, cudaGetLastError());
         ctx->stats.kernel_launches += 2;
-        LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_x_keys, ctx->d_x_keys, total * 2, cudaMemcpyDeviceToHost, s));
-        LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_x_counts, ctx->d_x_counts, total * 8, cudaMemcpyDeviceToHost, s));
+        LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_x_keys.get(), ctx->d_x_keys.get(), total * 2, cudaMemcpyDeviceToHost, s));
+        LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_x_counts.get(), ctx->d_x_counts.get(), total * 8, cudaMemcpyDeviceToHost, s));
         LH_CUDA(ctx, cudaStreamSynchronize(s));
     }
     ctx->stats.d2h_bytes += total * 10 + ((size_t)ctx->H + 1) * 4 + (size_t)ctx->C * 8;
-    out->offsets = ctx->h_offsets;
-    out->keys = ctx->h_x_keys;
-    out->counts = reinterpret_cast<const uint64_t *>(ctx->h_x_counts);
-    out->counter_deltas = reinterpret_cast<const uint64_t *>(ctx->h_counter_deltas);
+    out->offsets = ctx->h_offsets.get();
+    out->keys = ctx->h_x_keys.get();
+    out->counts = reinterpret_cast<const uint64_t *>(ctx->h_x_counts.get());
+    out->counter_deltas = reinterpret_cast<const uint64_t *>(ctx->h_counter_deltas.get());
     out->total_entries = total;
     return LH_OK;
 }
@@ -2177,8 +2175,8 @@ extern "C" lh_status lh_snapshot_copy_histogram(lh_ctx *ctx, uint32_t hid, uint6
     if (hid >= ctx->H) return fail(ctx, LH_ERR_RANGE, "histogram_id >= max_histograms");
     if (!h_out) return fail(ctx, LH_ERR_INVALID, "h_out is NULL");
     const View v = snapshot_view(ctx);
-    LH_CUDA(ctx, cudaMemcpyAsync(h_out, v.buckets + (size_t)hid * 65536u, 65536 * 8, cudaMemcpyDeviceToHost, ctx->snap_stream));
-    LH_CUDA(ctx, cudaStreamSynchronize(ctx->snap_stream));
+    LH_CUDA(ctx, cudaMemcpyAsync(h_out, v.buckets + (size_t)hid * 65536u, 65536 * 8, cudaMemcpyDeviceToHost, ctx->snap_stream.get()));
+    LH_CUDA(ctx, cudaStreamSynchronize(ctx->snap_stream.get()));
     ctx->stats.d2h_bytes += 65536 * 8;
     return LH_OK;
 }
@@ -2187,18 +2185,18 @@ extern "C" lh_status lh_snapshot_end(lh_ctx *ctx) {
     LH_ENTER(ctx);
     if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
     const int f = ctx->active ^ 1;
-    cudaStream_t s = ctx->snap_stream;
+    cudaStream_t s = ctx->snap_stream.get();
     // zero only what the interval touched (flags), not the whole uint64[H][65536] array
-    k_clear_touched<<<ctx->H, 256, 0, s>>>(ctx->buf[f].d_buckets, ctx->buf[f].d_flags, ctx->pc.win);
+    k_clear_touched<<<ctx->H, 256, 0, s>>>(ctx->buf[f].d_buckets.get(), ctx->buf[f].d_flags.get(), ctx->pc.win);
     LH_CUDA(ctx, cudaGetLastError());
     if (ctx->view_reduced) {
-        k_clear_touched<<<ctx->H, 256, 0, s>>>(ctx->d_red_buckets, ctx->d_red_flags, ctx->pc.win);
+        k_clear_touched<<<ctx->H, 256, 0, s>>>(ctx->d_red_buckets.get(), ctx->d_red_flags.get(), ctx->pc.win);
         LH_CUDA(ctx, cudaGetLastError());
         ctx->stats.kernel_launches++;
     }
     ctx->stats.kernel_launches++;
-    LH_CUDA(ctx, cudaMemsetAsync(ctx->buf[f].d_counters, 0, (size_t)ctx->C * 8u, s));
-    LH_CUDA(ctx, cudaEventRecord(ctx->buf[f].cleared, s));
+    LH_CUDA(ctx, cudaMemsetAsync(ctx->buf[f].d_counters.get(), 0, (size_t)ctx->C * 8u, s));
+    LH_CUDA(ctx, cudaEventRecord(ctx->buf[f].cleared.get(), s));
     ctx->frozen = false;
     ctx->pub_slot = -1;
     ctx->view_reduced = false;
@@ -2215,10 +2213,10 @@ size_t board_image_bytes(uint32_t k, uint32_t kc) {
 size_t board_table_offset(uint32_t k, uint32_t kc) { return (board_image_bytes(k, kc) + 15u) & ~(size_t)15u; }
 
 // the live board a handle names (its memory must match too), or nullptr
-const lh_board *board_of(lh_ctx *ctx, const lh_board *b) {
+Board *board_of(lh_ctx *ctx, const lh_board *b) {
     if (!b) return nullptr;
     for (auto &x : ctx->boards)
-        if (x.handle == b->handle && x.d_board == b->d_board) return &x;
+        if (x.b.handle == b->handle && x.b.d_board == b->d_board) return &x;
     return nullptr;
 }
 }  // namespace
@@ -2229,23 +2227,21 @@ extern "C" lh_status lh_board_create(lh_ctx *ctx, uint32_t k, uint32_t kc, lh_bo
     if (k == 0 && kc == 0) return fail(ctx, LH_ERR_INVALID, "a board needs a histogram or a counter row");
     if (k > ctx->H || kc > ctx->C) return fail(ctx, LH_ERR_RANGE, "more rows than max_histograms / max_counters");
     const size_t bytes = board_table_offset(k, kc) + (size_t)(k + kc) * sizeof(BoardEntry);
-    cudaStream_t s = ctx->snap_stream;
-    char *base = nullptr;
-    LH_CUDA(ctx, cudaMallocAsync((void **)&base, bytes, s));
-    cudaError_t e = cudaMemsetAsync(base, 0, bytes, s);
+    cudaStream_t s = ctx->snap_stream.get();
+    Board bd;
+    bd.mem = AsyncPtr(s);
+    LH_CUDA(ctx, cudaMallocAsync((void **)bd.mem.out(), bytes, s));
+    cudaError_t e = cudaMemsetAsync(bd.mem.get(), 0, bytes, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) {
-        cudaFreeAsync(base, s);
-        return fail(ctx, LH_ERR_CUDA, "lh_board_create", e);
-    }
-    lh_board b{};
+    if (e != cudaSuccess) return fail(ctx, LH_ERR_CUDA, "lh_board_create", e);
+    lh_board &b = bd.b;
     b.handle = graph_handle(ctx, ctx->next_board++);
-    b.d_board = base;
+    b.d_board = bd.mem.get();
     b.k = k;
     b.kc = kc;
     b.bytes = board_image_bytes(k, kc);
-    ctx->boards.push_back(b);
     *out = b;
+    ctx->boards.push_back(std::move(bd));
     return LH_OK;
 }
 
@@ -2255,41 +2251,41 @@ extern "C" lh_status lh_board_create(lh_ctx *ctx, uint32_t k, uint32_t kc, lh_bo
 extern "C" lh_status lh_snapshot_publish(lh_ctx *ctx, const lh_board *b, const uint32_t *hist_ids,
                                          const uint32_t *counter_ids, const uint64_t *counter_totals) {
     LH_ENTER(ctx);
-    const lh_board *bd = board_of(ctx, b);
+    Board *bd = board_of(ctx, b);
     if (!bd) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign board");
     if (!ctx->frozen || ctx->pub_slot < 0)
         return fail(ctx, LH_ERR_STATE, "lh_snapshot_publish needs a reduction of the open snapshot");
-    if (!ids_ok(hist_ids, bd->k, ctx->H) || !ids_ok(counter_ids, bd->kc, ctx->C))
+    if (!ids_ok(hist_ids, bd->b.k, ctx->H) || !ids_ok(counter_ids, bd->b.kc, ctx->C))
         return fail(ctx, LH_ERR_RANGE, "id >= max_histograms / max_counters");
     const int slot = ctx->pub_slot;
     const uint32_t np = ctx->res_np[slot];
     const ResLayout l = res_layout(ctx->H, np);
-    const char *d = ctx->d_res[slot];
-    cudaStream_t s = ctx->snap_stream;
+    const char *d = ctx->d_res[slot].get();
+    cudaStream_t s = ctx->snap_stream.get();
     BoardParams &p = ctx->board_prm;
-    p.board = (char *)bd->d_board;
-    p.table = reinterpret_cast<BoardEntry *>(p.board + board_table_offset(bd->k, bd->kc));
+    p.board = (char *)bd->b.d_board;
+    p.table = reinterpret_cast<BoardEntry *>(p.board + board_table_offset(bd->b.k, bd->b.kc));
     p.count = (const unsigned long long *)(d + l.count);
     p.sum = (const double *)(d + l.sum);
     p.avg = (const double *)(d + l.avg);
     p.pvals = (const double *)(d + l.pvals);
     p.pkeys = (const int *)(d + l.pkeys);
-    p.nnz = ctx->d_nnz + (size_t)slot * ctx->H;
-    p.ps = ctx->d_ps[slot];
+    p.nnz = ctx->d_nnz.get() + (size_t)slot * ctx->H;
+    p.ps = ctx->d_ps[slot].get();
     p.counters = snapshot_view(ctx).counters;
     p.np = np;
-    p.k = bd->k;
-    const uint32_t rows = bd->k + bd->kc;
+    p.k = bd->b.k;
+    const uint32_t rows = bd->b.k + bd->b.kc;
     for (uint32_t r0 = 0;; r0 += BP_MAX_ENTRIES) {
         const uint32_t n = std::min<uint32_t>(BP_MAX_ENTRIES, rows - r0);
         p.n_staged = r0;
         p.n = n;
         for (uint32_t i = 0; i < n; i++) {
             const uint32_t row = r0 + i;
-            if (row < bd->k) {
+            if (row < bd->b.k) {
                 p.e[i] = BoardEntry{row, hist_ids ? hist_ids[row] : LH_GRAPH_UNBOUND, 0ull};
             } else {
-                const uint32_t c = row - bd->k;
+                const uint32_t c = row - bd->b.k;
                 p.e[i] = BoardEntry{row, counter_ids ? counter_ids[c] : LH_GRAPH_UNBOUND,
                                     counter_totals ? (unsigned long long)counter_totals[c] : 0ull};
             }
@@ -2307,11 +2303,11 @@ extern "C" lh_status lh_snapshot_publish(lh_ctx *ctx, const lh_board *b, const u
 
 extern "C" lh_status lh_board_read(lh_ctx *ctx, const lh_board *b, void *d_out, void *stream) {
     LH_ENTER(ctx);
-    const lh_board *bd = board_of(ctx, b);
+    Board *bd = board_of(ctx, b);
     if (!bd) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign board");
     if (!d_out || ((uintptr_t)d_out & 7u)) return fail(ctx, LH_ERR_INVALID, "d_out is NULL or not 8-byte aligned");
-    k_board_read<<<1, BR_THREADS, 0, pick_stream(ctx, stream)>>>((const unsigned long long *)bd->d_board,
-                                                                 (unsigned long long *)d_out, (uint32_t)(bd->bytes / 8u));
+    k_board_read<<<1, BR_THREADS, 0, pick_stream(ctx, stream)>>>((const unsigned long long *)bd->b.d_board,
+                                                                 (unsigned long long *)d_out, (uint32_t)(bd->b.bytes / 8u));
     LH_CUDA(ctx, cudaGetLastError());
     ctx->stats.kernel_launches++;
     return LH_OK;
@@ -2319,9 +2315,9 @@ extern "C" lh_status lh_board_read(lh_ctx *ctx, const lh_board *b, void *d_out, 
 
 extern "C" lh_status lh_board_destroy(lh_ctx *ctx, const lh_board *b) {
     LH_ENTER(ctx);
-    const lh_board *bd = board_of(ctx, b);
+    Board *bd = board_of(ctx, b);
     if (!bd) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign board");
-    LH_CUDA(ctx, cudaFreeAsync(bd->d_board, ctx->snap_stream));   // after every publish issued (all on this stream)
+    LH_CUDA(ctx, bd->mem.reset());   // after every publish issued (all on this stream)
     ctx->boards.erase(ctx->boards.begin() + (bd - ctx->boards.data()));
     return LH_OK;
 }
@@ -2358,9 +2354,11 @@ lh_status raw_board_create(lh_ctx *ctx, uint32_t k, uint32_t window, lh_raw_boar
     if (window > LH_RAW_MAX_WINDOW) return fail(ctx, LH_ERR_RANGE, "window > LH_RAW_MAX_WINDOW");
     const size_t bytes = window == 1 ? raw_table_offset(k) + (size_t)k * 4u
                                      : raw_slots_offset(k, window) + (size_t)k * window * 65536u * 8u;
-    cudaStream_t s = ctx->snap_stream;
-    char *base = nullptr;
-    cudaError_t e = cudaMallocAsync((void **)&base, bytes, s);
+    cudaStream_t s = ctx->snap_stream.get();
+    RawBoard rb;
+    rb.mem = AsyncPtr(s);
+    cudaError_t e = cudaMallocAsync((void **)rb.mem.out(), bytes, s);
+    char *base = rb.mem.get();
     if (e != cudaSuccess)
         return fail(ctx, e == cudaErrorMemoryAllocation ? LH_ERR_NOMEM : LH_ERR_CUDA, "allocating a raw board", e);
     // only the headers, each an empty row (publish 0, total 0, key_lo > key_hi): a row's cells are read only inside
@@ -2372,19 +2370,15 @@ lh_status raw_board_create(lh_ctx *ctx, uint32_t k, uint32_t window, lh_raw_boar
     if (e == cudaSuccess && window > 1)
         e = cudaMemsetAsync(base + raw_window_offset(k), 0, raw_levels_offset(k) + (size_t)k * window - raw_window_offset(k), s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) {
-        cudaFreeAsync(base, s);
-        return fail(ctx, LH_ERR_CUDA, "lh_raw_board_create", e);
-    }
-    RawBoard rb;
+    if (e != cudaSuccess) return fail(ctx, LH_ERR_CUDA, "lh_raw_board_create", e);
     rb.b.handle = graph_handle(ctx, ctx->next_raw_board++);
     rb.b.d_rows = base;
-    rb.b.d_decomp = ctx->d_decomp;
+    rb.b.d_decomp = ctx->d_decomp.get();
     rb.b.k = k;
     memcpy(rb.b.prec, &ctx->pc, sizeof(Prec));
     rb.window = window;
-    ctx->raw_boards.push_back(rb);
     *out = rb.b;
+    ctx->raw_boards.push_back(std::move(rb));
     return LH_OK;
 }
 }  // namespace
@@ -2413,7 +2407,7 @@ extern "C" lh_status lh_snapshot_publish_raw(lh_ctx *ctx, const lh_raw_board *b,
     if (windowed && rb->snapshot == ctx->stats.snapshots)   // the interval would be counted twice
         return fail(ctx, LH_ERR_STATE, "a window board takes one publish per snapshot");
     const View v = snapshot_view(ctx);
-    cudaStream_t s = ctx->snap_stream;
+    cudaStream_t s = ctx->snap_stream.get();
     RawPublishParams &p = ctx->raw_prm;
     p.rows = (char *)bd->d_rows;
     p.cells = reinterpret_cast<unsigned long long *>(p.rows + LH_RAW_CELLS_OFFSET(bd->k));
@@ -2504,9 +2498,9 @@ extern "C" lh_status lh_raw_ranks_grid(lh_ctx *ctx, const lh_raw_board *b, const
 
 extern "C" lh_status lh_raw_board_destroy(lh_ctx *ctx, const lh_raw_board *b) {
     LH_ENTER(ctx);
-    const RawBoard *rb = raw_board_of(ctx, b);
+    RawBoard *rb = raw_board_of(ctx, b);
     if (!rb) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign raw board");
-    LH_CUDA(ctx, cudaFreeAsync(rb->b.d_rows, ctx->snap_stream));   // after every publish issued (all on this stream)
+    LH_CUDA(ctx, rb->mem.reset());   // after every publish issued (all on this stream)
     ctx->raw_boards.erase(ctx->raw_boards.begin() + (rb - ctx->raw_boards.data()));
     return LH_OK;
 }
@@ -2549,15 +2543,16 @@ extern "C" lh_status lh_gauges_read(lh_ctx *ctx, const lh_gauge_src *h_srcs, uin
     if (n == 0) return LH_OK;
     if (n > ctx->gauge_cap) {
         const uint32_t cap = std::max<uint32_t>(n, 4096);
-        if (ctx->h_gauges) cudaFreeHost(ctx->h_gauges);   // no read is in flight: every call waits for its launches
-        ctx->h_gauges = ctx->d_gauges = nullptr;
+        ctx->h_gauges.reset();   // no read is in flight: every call waits for its launches
+        ctx->d_gauges = nullptr;
         ctx->gauge_cap = 0;
-        LH_CUDA(ctx, cudaHostAlloc((void **)&ctx->h_gauges, (size_t)cap * 8u, cudaHostAllocMapped));
-        LH_CUDA(ctx, cudaHostGetDevicePointer((void **)&ctx->d_gauges, ctx->h_gauges, 0));
-        ctx->gauge_cap = cap;
+        PinnedPtr<double> h; double *d = nullptr;
+        LH_CUDA(ctx, cudaHostAlloc((void **)h.out(), (size_t)cap * 8u, cudaHostAllocMapped));
+        LH_CUDA(ctx, cudaHostGetDevicePointer((void **)&d, h.get(), 0));
+        ctx->h_gauges = std::move(h); ctx->d_gauges = d; ctx->gauge_cap = cap;
     }
-    if (!ctx->gauge_done) LH_CUDA(ctx, cudaEventCreateWithFlags(&ctx->gauge_done, cudaEventDisableTiming));
-    cudaStream_t s = ctx->snap_stream;
+    if (!ctx->gauge_done.get()) LH_CUDA(ctx, cudaEventCreateWithFlags(ctx->gauge_done.out(), cudaEventDisableTiming));
+    cudaStream_t s = ctx->snap_stream.get();
     GaugeParams &p = ctx->gauge_prm;
     for (uint32_t i0 = 0; i0 < n; i0 += GR_MAX_ENTRIES) {
         const uint32_t m = std::min<uint32_t>(GR_MAX_ENTRIES, n - i0);
@@ -2568,25 +2563,19 @@ extern "C" lh_status lh_gauges_read(lh_ctx *ctx, const lh_gauge_src *h_srcs, uin
         LH_CUDA(ctx, cudaGetLastError());
         ctx->stats.kernel_launches++;
     }
-    LH_CUDA(ctx, cudaEventRecord(ctx->gauge_done, s));
+    LH_CUDA(ctx, cudaEventRecord(ctx->gauge_done.get(), s));
     // wait outside the lock so ingest threads are not held up; gauge_mu keeps the buffer ours
-    cudaEvent_t ev = ctx->gauge_done;
+    cudaEvent_t ev = ctx->gauge_done.get();
     _lk.unlock();
     const cudaError_t e = cudaEventSynchronize(ev);
     _lk.lock();
     if (e != cudaSuccess) return fail(ctx, LH_ERR_CUDA, "cudaEventSynchronize(gauges)", e);
-    memcpy(h_out, ctx->h_gauges, (size_t)n * 8u);
+    memcpy(h_out, ctx->h_gauges.get(), (size_t)n * 8u);
     return LH_OK;
 }
 
 // =========================================================== reduce caller-supplied sparse histograms
 namespace {
-struct AsyncBuf {   // stream-ordered device allocation, released on every return path
-    char *p = nullptr;
-    cudaStream_t s = nullptr;
-    ~AsyncBuf() { if (p) cudaFreeAsync(p, s); }
-};
-
 // The device part of lh_reduce_sparse_host, rs_mu held: one H2D of the input, per batch of K6_BATCH segments scatter
 // + K3 + epilogue + clear into the call's own result buffer, one D2H of the packed results into h_res.
 cudaError_t reduce_sparse_device(lh_ctx *ctx, uint32_t n, const uint32_t *h_offsets, const int16_t *h_keys,
@@ -2597,18 +2586,20 @@ cudaError_t reduce_sparse_device(lh_ctx *ctx, uint32_t n, const uint32_t *h_offs
         if (_e != cudaSuccess) { *what = #call; return _e; }             \
     } while (0)
     RS_CUDA(cudaSetDevice(ctx->device));
-    if (!ctx->rs_stream) RS_CUDA(cudaStreamCreateWithFlags(&ctx->rs_stream, cudaStreamNonBlocking));
-    cudaStream_t s = ctx->rs_stream;
+    if (!ctx->rs_stream.get()) RS_CUDA(cudaStreamCreateWithFlags(ctx->rs_stream.out(), cudaStreamNonBlocking));
+    cudaStream_t s = ctx->rs_stream.get();
     const size_t row_bytes = (size_t)K6_BATCH * 65536u * 8u;
-    if (!ctx->d_rs_flags) RS_CUDA(cudaMalloc(&ctx->d_rs_flags, K6_BATCH * 4));
-    if (!ctx->d_rs_nnz) RS_CUDA(cudaMalloc(&ctx->d_rs_nnz, K6_BATCH * 4));
-    if (!ctx->d_rs_rows) {
-        RS_CUDA(cudaMalloc(&ctx->d_rs_rows, row_bytes));
+    if (!ctx->d_rs_rows.get()) {
+        DevPtr<uint32_t> flags, nnz; DevPtr<unsigned long long> rows;
+        RS_CUDA(cudaMalloc(flags.out(), K6_BATCH * 4));
+        RS_CUDA(cudaMalloc(nnz.out(), K6_BATCH * 4));
+        RS_CUDA(cudaMalloc(rows.out(), row_bytes));
+        ctx->d_rs_flags = std::move(flags); ctx->d_rs_nnz = std::move(nnz); ctx->d_rs_rows = std::move(rows);
         ctx->rs_dirty = true;
     }
     if (ctx->rs_dirty) {
-        RS_CUDA(cudaMemsetAsync(ctx->d_rs_rows, 0, row_bytes, s));
-        RS_CUDA(cudaMemsetAsync(ctx->d_rs_flags, 0, K6_BATCH * 4, s));
+        RS_CUDA(cudaMemsetAsync(ctx->d_rs_rows.get(), 0, row_bytes, s));
+        RS_CUDA(cudaMemsetAsync(ctx->d_rs_flags.get(), 0, K6_BATCH * 4, s));
     }
     ctx->rs_dirty = true;                        // until the last clear of this call has run
 
@@ -2617,10 +2608,9 @@ cudaError_t reduce_sparse_device(lh_ctx *ctx, uint32_t n, const uint32_t *h_offs
     const ResLayout l = res_layout(n, np);
     const size_t off_keys = ((size_t)n + 1) * 4, off_counts = (off_keys + ne * 2 + 7) & ~(size_t)7;
     const size_t off_ps = off_counts + ne * 8, off_res = off_ps + LH_MAX_PERCENTILES * 8;
-    AsyncBuf buf;
-    buf.s = s;
-    RS_CUDA(cudaMallocAsync((void **)&buf.p, off_res + l.total, s));
-    char *d = buf.p;
+    AsyncPtr buf(s);   // released on every return path
+    RS_CUDA(cudaMallocAsync((void **)buf.out(), off_res + l.total, s));
+    char *d = buf.get();
     RS_CUDA(cudaMemcpyAsync(d, h_offsets, off_keys, cudaMemcpyHostToDevice, s));
     if (ne) {
         RS_CUDA(cudaMemcpyAsync(d + off_keys, h_keys + base, ne * 2, cudaMemcpyHostToDevice, s));
@@ -2642,14 +2632,14 @@ cudaError_t reduce_sparse_device(lh_ctx *ctx, uint32_t n, const uint32_t *h_offs
         const size_t po = (size_t)b0 * np;
         if (m) {
             const int grid = (int)std::min<size_t>((m + 255) / 256, (size_t)ctx->sm_count * 8);
-            k_scatter_segments<<<grid, 256, 0, s>>>(d_off + b0, nb, base, d_keys, d_counts, ctx->d_rs_rows, ctx->d_rs_flags, win);
+            k_scatter_segments<<<grid, 256, 0, s>>>(d_off + b0, nb, base, d_keys, d_counts, ctx->d_rs_rows.get(), ctx->d_rs_flags.get(), win);
         }
-        k_reduce<<<nb, K3_THREADS, (size_t)smem_cells * 8, s>>>(ctx->d_rs_rows, ctx->d_rs_flags, win, ctx->d_decomp, d_ps, (int)np,
+        k_reduce<<<nb, K3_THREADS, (size_t)smem_cells * 8, s>>>(ctx->d_rs_rows.get(), ctx->d_rs_flags.get(), win, ctx->d_decomp.get(), d_ps, (int)np,
                                                                  r_count + b0, r_sum + b0, r_avg + b0, r_pkeys + po, r_pvals + po,
-                                                                 ctx->d_rs_nnz, smem_cells);
-        k_sparse_epilogue<<<nb, 256, 0, s>>>(d_off + b0, base, d_keys, ctx->d_rs_rows, ctx->d_decomp, d_ps, (int)np,
+                                                                 ctx->d_rs_nnz.get(), smem_cells);
+        k_sparse_epilogue<<<nb, 256, 0, s>>>(d_off + b0, base, d_keys, ctx->d_rs_rows.get(), ctx->d_decomp.get(), d_ps, (int)np,
                                              r_count + b0, r_sum + b0, r_avg + b0, r_pkeys + po, r_pvals + po);
-        k_clear_touched<<<nb, 256, 0, s>>>(ctx->d_rs_rows, ctx->d_rs_flags, win);
+        k_clear_touched<<<nb, 256, 0, s>>>(ctx->d_rs_rows.get(), ctx->d_rs_flags.get(), win);
         RS_CUDA(cudaGetLastError());
     }
     RS_CUDA(cudaMemcpyAsync(h_res, r, l.total, cudaMemcpyDeviceToHost, s));
@@ -2709,18 +2699,18 @@ extern "C" lh_status lh_comm_export(lh_ctx *ctx, lh_peer_handle *out) {
     w.precision = (uint32_t)ctx->pc.precision; w.device = (uint32_t)ctx->device;
     w.pid = (int64_t)getpid(); w.ctx_id = ctx->ctx_id;
     for (int b = 0; b < 2; b++) {
-        w.ptr_buckets[b] = (uint64_t)(uintptr_t)ctx->buf[b].d_buckets;
-        w.ptr_flags[b] = (uint64_t)(uintptr_t)ctx->buf[b].d_flags;
-        w.ptr_counters[b] = (uint64_t)(uintptr_t)ctx->buf[b].d_counters;
-        LH_CUDA(ctx, cudaIpcGetMemHandle(&w.ipc_buckets[b], ctx->buf[b].d_buckets));
-        LH_CUDA(ctx, cudaIpcGetMemHandle(&w.ipc_flags[b], ctx->buf[b].d_flags));
-        LH_CUDA(ctx, cudaIpcGetMemHandle(&w.ipc_counters[b], ctx->buf[b].d_counters));
+        w.ptr_buckets[b] = (uint64_t)(uintptr_t)ctx->buf[b].d_buckets.get();
+        w.ptr_flags[b] = (uint64_t)(uintptr_t)ctx->buf[b].d_flags.get();
+        w.ptr_counters[b] = (uint64_t)(uintptr_t)ctx->buf[b].d_counters.get();
+        LH_CUDA(ctx, cudaIpcGetMemHandle(&w.ipc_buckets[b], ctx->buf[b].d_buckets.get()));
+        LH_CUDA(ctx, cudaIpcGetMemHandle(&w.ipc_flags[b], ctx->buf[b].d_flags.get()));
+        LH_CUDA(ctx, cudaIpcGetMemHandle(&w.ipc_counters[b], ctx->buf[b].d_counters.get()));
     }
-    w.ptr_comm = (uint64_t)(uintptr_t)ctx->d_comm;
-    LH_CUDA(ctx, cudaIpcGetMemHandle(&w.ipc_comm, ctx->d_comm));
+    w.ptr_comm = (uint64_t)(uintptr_t)ctx->d_comm.get();
+    LH_CUDA(ctx, cudaIpcGetMemHandle(&w.ipc_comm, ctx->d_comm.get()));
     if (lh_status st = comm_alloc_reduced(ctx)) return st;
-    w.ptr_red = (uint64_t)(uintptr_t)ctx->d_red_buckets;
-    LH_CUDA(ctx, cudaIpcGetMemHandle(&w.ipc_red, ctx->d_red_buckets));
+    w.ptr_red = (uint64_t)(uintptr_t)ctx->d_red_buckets.get();
+    LH_CUDA(ctx, cudaIpcGetMemHandle(&w.ipc_red, ctx->d_red_buckets.get()));
     memset(out, 0, sizeof *out);
     memcpy(out->bytes, &w, sizeof w);
     return LH_OK;
@@ -2741,10 +2731,10 @@ extern "C" lh_status lh_comm_import(lh_ctx *ctx, uint32_t rank, uint32_t world, 
         PeerMap &pm = ctx->peers[r];
         if (r == rank) {
             if (w.ctx_id != ctx->ctx_id || w.pid != my_pid) return fail(ctx, LH_ERR_INVALID, "handles[rank] is not this context's own handle");
-            for (int b = 0; b < 2; b++) { pm.buckets[b] = ctx->buf[b].d_buckets; pm.flags[b] = ctx->buf[b].d_flags; pm.counters[b] = ctx->buf[b].d_counters; }
-            pm.comm = ctx->d_comm;
+            for (int b = 0; b < 2; b++) { pm.buckets[b] = ctx->buf[b].d_buckets.get(); pm.flags[b] = ctx->buf[b].d_flags.get(); pm.counters[b] = ctx->buf[b].d_counters.get(); }
+            pm.comm = ctx->d_comm.get();
             if (lh_status st = comm_alloc_reduced(ctx)) return st;
-            pm.red = ctx->d_red_buckets;
+            pm.red = ctx->d_red_buckets.get();
             continue;
         }
         if (w.pid == my_pid) {
@@ -2792,9 +2782,9 @@ template <typename Rows>
 lh_status launch_allreduce(lh_ctx *ctx, uint64_t seq, const uint32_t *frozen, uint32_t n_rows, uint32_t include_counters,
                            Rows rows, uint64_t *seq_out) {
     const int f = ctx->active ^ 1;
-    cudaStream_t s = ctx->snap_stream;
+    cudaStream_t s = ctx->snap_stream.get();
     // status and cells describe this all-reduce only: zeroed behind the previous one on the same stream
-    LH_CUDA(ctx, cudaMemsetAsync(ctx->d_comm_aux + 1, 0, 12, s));
+    LH_CUDA(ctx, cudaMemsetAsync(ctx->d_comm_aux.get() + 1, 0, 12, s));
     PeerParams p{};
     p.rank = ctx->comm_rank; p.world = ctx->comm_world; p.H = ctx->H; p.C = ctx->C; p.win = ctx->pc.win;
     p.do_counters = include_counters ? 1u : 0u; p.frozen = (uint32_t)f;
@@ -2808,9 +2798,9 @@ lh_status launch_allreduce(lh_ctx *ctx, uint64_t seq, const uint32_t *frozen, ui
         p.counters[r] = ctx->peers[r].counters[fr];
         p.comm[r] = ctx->peers[r].comm;
     }
-    p.out_buckets = ctx->d_red_buckets; p.out_flags = ctx->d_red_flags; p.out_counters = ctx->d_red_counters;
-    p.block_counter = ctx->d_comm_aux; p.status = ctx->d_comm_aux + 1;
-    p.cells = reinterpret_cast<unsigned long long *>(ctx->d_comm_aux + 2);
+    p.out_buckets = ctx->d_red_buckets.get(); p.out_flags = ctx->d_red_flags.get(); p.out_counters = ctx->d_red_counters.get();
+    p.block_counter = ctx->d_comm_aux.get(); p.status = ctx->d_comm_aux.get() + 1;
+    p.cells = reinterpret_cast<unsigned long long *>(ctx->d_comm_aux.get() + 2);
     for (uint32_t r = 0; r < ctx->comm_world; r++) p.out_peer[r] = ctx->peers[r].red;
     // payload = the window cells of every histogram that can be live; above 1 MiB the reduce-scatter + push form wins
     const size_t payload = (size_t)n_rows * (2u * ctx->pc.win - 1u) * 8u;
@@ -2821,7 +2811,7 @@ lh_status launch_allreduce(lh_ctx *ctx, uint64_t seq, const uint32_t *frozen, ui
     // CTAs that are not resident yet simply start later (no CTA waits for another CTA of its own grid before the end)
     const size_t items = (size_t)std::max(1u, n_rows) * (65536u / K5_CHUNK);
     int grid = (int)std::min<size_t>(items, n_rows <= 1 ? 5 : 16);
-    LH_CUDA(ctx, cudaEventRecord(ctx->comm_t0[ring], s));
+    LH_CUDA(ctx, cudaEventRecord(ctx->comm_t0[ring].get(), s));
     if (p.two_shot) {
         // An SM sustains only ~4 GB/s of NVLink loads (measured, tools/peer_probe.py: 36 MB take 9.1 / 2.3 / 0.64 / 0.21 ms
         // on 1 / 4 / 16 / 64 SMs), so the large payload cannot hide on the few SMs the ingest kernels leave free.  It goes
@@ -2837,7 +2827,7 @@ lh_status launch_allreduce(lh_ctx *ctx, uint64_t seq, const uint32_t *frozen, ui
     }
     k5_launch(grid, ctx->H, s, p, rows);
     LH_CUDA(ctx, cudaGetLastError());
-    LH_CUDA(ctx, cudaEventRecord(ctx->comm_t1[ring], s));
+    LH_CUDA(ctx, cudaEventRecord(ctx->comm_t1[ring].get(), s));
     ctx->stats.kernel_launches++;
     ctx->view_reduced = true;
     ctx->view_counters_reduced = include_counters != 0;
@@ -2860,18 +2850,20 @@ extern "C" lh_status lh_snapshot_rows(lh_ctx *ctx, uint8_t *hist_touched, uint64
     if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
     if (ctx->view_reduced) return fail(ctx, LH_ERR_STATE, "this snapshot has already been all-reduced");
     const int f = ctx->active ^ 1;
-    cudaStream_t s = ctx->snap_stream;
-    if (!ctx->h_rows_flags) {
-        LH_CUDA(ctx, cudaMallocHost(&ctx->h_rows_flags, (size_t)ctx->H * 4));
-        LH_CUDA(ctx, cudaMallocHost(&ctx->h_rows_counters, (size_t)ctx->C * 8));
+    cudaStream_t s = ctx->snap_stream.get();
+    if (!ctx->h_rows_flags.get()) {
+        PinnedPtr<uint32_t> flags; PinnedPtr<unsigned long long> counters;
+        LH_CUDA(ctx, cudaMallocHost(flags.out(), (size_t)ctx->H * 4));
+        LH_CUDA(ctx, cudaMallocHost(counters.out(), (size_t)ctx->C * 8));
+        ctx->h_rows_flags = std::move(flags); ctx->h_rows_counters = std::move(counters);
     }
     // behind the writer events, the graph drain and the hot-window fold lh_snapshot_begin ordered on this stream
-    if (hist_touched) LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_rows_flags, ctx->buf[f].d_flags, (size_t)ctx->H * 4, cudaMemcpyDeviceToHost, s));
-    if (counter_deltas) LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_rows_counters, ctx->buf[f].d_counters, (size_t)ctx->C * 8, cudaMemcpyDeviceToHost, s));
+    if (hist_touched) LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_rows_flags.get(), ctx->buf[f].d_flags.get(), (size_t)ctx->H * 4, cudaMemcpyDeviceToHost, s));
+    if (counter_deltas) LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_rows_counters.get(), ctx->buf[f].d_counters.get(), (size_t)ctx->C * 8, cudaMemcpyDeviceToHost, s));
     LH_CUDA(ctx, cudaStreamSynchronize(s));
     if (hist_touched)
-        for (uint32_t h = 0; h < ctx->H; h++) hist_touched[h] = ctx->h_rows_flags[h] != 0;
-    if (counter_deltas) memcpy(counter_deltas, ctx->h_rows_counters, (size_t)ctx->C * 8);
+        for (uint32_t h = 0; h < ctx->H; h++) hist_touched[h] = ctx->h_rows_flags.get()[h] != 0;
+    if (counter_deltas) memcpy(counter_deltas, ctx->h_rows_counters.get(), (size_t)ctx->C * 8);
     if (frozen) *frozen = (uint32_t)f;
     ctx->stats.d2h_bytes += (hist_touched ? (size_t)ctx->H * 4 : 0) + (counter_deltas ? (size_t)ctx->C * 8 : 0);
     return LH_OK;
@@ -2900,17 +2892,17 @@ extern "C" lh_status lh_snapshot_allreduce_rows(lh_ctx *ctx, uint64_t seq, const
         if (counter_map[i] != LH_ROW_ABSENT && counter_map[i] >= ctx->C) return fail(ctx, LH_ERR_RANGE, "counter map entry >= max_counters");
     if (lh_status st = comm_alloc_row_maps(ctx)) return st;
     // the staging is rewritten only after the previous upload from it has run
-    LH_CUDA(ctx, cudaEventSynchronize(ctx->row_maps_copied));
-    if (nh) memcpy(ctx->h_row_maps, hist_map, nh * 4);
-    if (nc) memcpy(ctx->h_row_maps + nh, counter_map, nc * 4);
-    cudaStream_t s = ctx->snap_stream;
+    LH_CUDA(ctx, cudaEventSynchronize(ctx->row_maps_copied.get()));
+    if (nh) memcpy(ctx->h_row_maps.get(), hist_map, nh * 4);
+    if (nc) memcpy(ctx->h_row_maps.get() + nh, counter_map, nc * 4);
+    cudaStream_t s = ctx->snap_stream.get();
     if (nh + nc) {
-        LH_CUDA(ctx, cudaMemcpyAsync(ctx->d_row_maps, ctx->h_row_maps, (nh + nc) * 4, cudaMemcpyHostToDevice, s));
+        LH_CUDA(ctx, cudaMemcpyAsync(ctx->d_row_maps.get(), ctx->h_row_maps.get(), (nh + nc) * 4, cudaMemcpyHostToDevice, s));
         ctx->stats.h2d_bytes += (nh + nc) * 4;
     }
-    LH_CUDA(ctx, cudaEventRecord(ctx->row_maps_copied, s));
+    LH_CUDA(ctx, cudaEventRecord(ctx->row_maps_copied.get(), s));
     RowMap m{};
-    m.hist = ctx->d_row_maps; m.ctr = ctx->d_row_maps + nh;
+    m.hist = ctx->d_row_maps.get(); m.ctr = ctx->d_row_maps.get() + nh;
     m.n_rows = n_rows; m.n_counter_rows = n_counter_rows;
     for (uint32_t r = 0; r < W; r++) m.frozen_mask |= frozen[r] << r;
     return launch_allreduce(ctx, seq, frozen, n_rows, 1u, m, seq_out);
@@ -2924,7 +2916,7 @@ extern "C" lh_status lh_comm_allreduce_ms(lh_ctx *ctx, uint64_t seq, float *ms) 
         if (seq == 0 || seq > ctx->comm_seq || ctx->comm_seq - seq >= (uint64_t)lh_ctx::kCommRing)
             return fail(ctx, LH_ERR_STATE, "that all-reduce is unknown or its events were recycled");
         const int ring = (int)(seq % lh_ctx::kCommRing);
-        e0 = ctx->comm_t0[ring]; e1 = ctx->comm_t1[ring];
+        e0 = ctx->comm_t0[ring].get(); e1 = ctx->comm_t1[ring].get();
     }
     cudaError_t e = cudaEventSynchronize(e1);
     if (e == cudaSuccess) e = cudaEventElapsedTime(ms, e0, e1);
@@ -2940,11 +2932,11 @@ extern "C" lh_status lh_comm_info(lh_ctx *ctx, lh_comm_stats *out) {
     out->rank = ctx->comm_rank; out->world = ctx->comm_world; out->allreduces = ctx->comm_seq;
     if (ctx->comm_world >= 2) {
         unsigned int aux[2] = {0, 0};
-        LH_CUDA(ctx, cudaMemcpy(aux, ctx->d_comm_aux, 8, cudaMemcpyDeviceToHost));
+        LH_CUDA(ctx, cudaMemcpy(aux, ctx->d_comm_aux.get(), 8, cudaMemcpyDeviceToHost));
         out->status = aux[1];
         // bytes this rank read from its peers in the last all-reduce: window (or dense) cells of every touched histogram
         unsigned long long cells = 0;
-        LH_CUDA(ctx, cudaMemcpy(&cells, ctx->d_comm_aux + 2, 8, cudaMemcpyDeviceToHost));
+        LH_CUDA(ctx, cudaMemcpy(&cells, ctx->d_comm_aux.get() + 2, 8, cudaMemcpyDeviceToHost));
         // one-shot: every cell from every peer; two-shot: this rank's 1/world of the cells from every peer (and as much pushed back)
         out->last_bytes_from_peers = ctx->comm_two_shot ? cells * 8u * (ctx->comm_world - 1) / ctx->comm_world : cells * 8u * (ctx->comm_world - 1);
     }
@@ -2967,7 +2959,7 @@ extern "C" lh_status lh_compress_f64(lh_ctx *ctx, const double *d_values, size_t
 extern "C" lh_status lh_decompress_table(lh_ctx *ctx, double *h_out) {
     LH_ENTER(ctx);
     if (!h_out) return fail(ctx, LH_ERR_INVALID, "h_out is NULL");
-    LH_CUDA(ctx, cudaMemcpy(h_out, ctx->d_decomp, 65536 * sizeof(double), cudaMemcpyDeviceToHost));
+    LH_CUDA(ctx, cudaMemcpy(h_out, ctx->d_decomp.get(), 65536 * sizeof(double), cudaMemcpyDeviceToHost));
     return LH_OK;
 }
 
@@ -2975,14 +2967,13 @@ extern "C" lh_status lh_fastpath_margin(lh_ctx *ctx, const double *d_values, siz
     LH_ENTER(ctx);
     if (n && !d_values) return fail(ctx, LH_ERR_INVALID, "NULL input");
     cudaStream_t s = pick_stream(ctx, stream);
-    unsigned long long *d = nullptr;
-    LH_CUDA(ctx, cudaMalloc(&d, 24));
-    LH_CUDA(ctx, cudaMemsetAsync(d, 0, 24, s));
-    if (n) k_fastpath_margin<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_values, n, d, ctx->pc);
+    DevPtr<unsigned long long> d;
+    LH_CUDA(ctx, cudaMalloc(d.out(), 24));
+    LH_CUDA(ctx, cudaMemsetAsync(d.get(), 0, 24, s));
+    if (n) k_fastpath_margin<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(d_values, n, d.get(), ctx->pc);
     unsigned long long h[3];
-    cudaError_t e = cudaMemcpyAsync(h, d, 24, cudaMemcpyDeviceToHost, s);
+    cudaError_t e = cudaMemcpyAsync(h, d.get(), 24, cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    cudaFree(d);
     if (e != cudaSuccess) return fail(ctx, LH_ERR_CUDA, "lh_fastpath_margin", e);
     // the larger of the two estimators' errors (positive doubles order like their bit patterns)
     const unsigned long long worst = std::max(h[0], h[2]);
@@ -3009,17 +3000,16 @@ extern "C" lh_status lh_fastpath_certify(lh_ctx *ctx, uint32_t p_lo, uint32_t p_
     const size_t rows = (size_t)(p_hi - p_lo + 1) * FC_FORMS;
     std::vector<unsigned long long> h(rows * FC_FIELDS, 0ull);
     for (size_t r = 0; r < rows; r++) h[r * FC_FIELDS + FC_MIN_MARGIN] = 0x7FF0000000000000ull;   // +Inf
-    cudaStream_t s = ctx->ingest_stream;
-    unsigned long long *d = nullptr;
-    LH_CUDA(ctx, cudaMalloc(&d, h.size() * 8));
-    cudaError_t e = cudaMemcpyAsync(d, h.data(), h.size() * 8, cudaMemcpyHostToDevice, s);
+    cudaStream_t s = ctx->ingest_stream.get();
+    DevPtr<unsigned long long> d;
+    LH_CUDA(ctx, cudaMalloc(d.out(), h.size() * 8));
+    cudaError_t e = cudaMemcpyAsync(d.get(), h.data(), h.size() * 8, cudaMemcpyHostToDevice, s);
     for (uint32_t p = p_lo; p <= p_hi && e == cudaSuccess; p++) {
-        k_fastpath_certify<<<ctx->sm_count * 8, FC_THREADS, 0, s>>>(d + (size_t)(p - p_lo) * FC_FORMS * FC_FIELDS, make_prec(p));
+        k_fastpath_certify<<<ctx->sm_count * 8, FC_THREADS, 0, s>>>(d.get() + (size_t)(p - p_lo) * FC_FORMS * FC_FIELDS, make_prec(p));
         e = cudaGetLastError();
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(h.data(), d, h.size() * 8, cudaMemcpyDeviceToHost, s);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h.data(), d.get(), h.size() * 8, cudaMemcpyDeviceToHost, s);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    cudaFree(d);
     if (e != cudaSuccess) return fail(ctx, LH_ERR_CUDA, "lh_fastpath_certify", e);
     memcpy(h_out, h.data(), h.size() * 8);
     return LH_OK;
@@ -3049,7 +3039,7 @@ extern "C" lh_status lh_get_stats(lh_ctx *ctx, lh_stats *out) {
     LH_ENTER(ctx);
     if (!out) return fail(ctx, LH_ERR_INVALID, "out is NULL");
     unsigned long long dropped = 0;
-    LH_CUDA(ctx, cudaMemcpy(&dropped, ctx->d_dropped, 8, cudaMemcpyDeviceToHost));
+    LH_CUDA(ctx, cudaMemcpy(&dropped, ctx->d_dropped.get(), 8, cudaMemcpyDeviceToHost));
     ctx->stats.dropped = dropped;
     *out = ctx->stats;
     return LH_OK;
@@ -3058,7 +3048,7 @@ extern "C" lh_status lh_sync(lh_ctx *ctx) {
     LH_ENTER(ctx);
     // this context's work only (its three streams and every caller stream that carried an ingest), not the whole
     // device: another context on the same GPU may be inside a collective that waits for THIS caller's next step
-    std::vector<cudaStream_t> streams = {ctx->ingest_stream, ctx->copy_stream, ctx->snap_stream};
+    std::vector<cudaStream_t> streams = {ctx->ingest_stream.get(), ctx->copy_stream.get(), ctx->snap_stream.get()};
     for (int b = 0; b < 2; b++)
         for (auto &w : ctx->buf[b].writers)
             if (std::find(streams.begin(), streams.end(), w.stream) == streams.end()) streams.push_back(w.stream);
@@ -3068,11 +3058,11 @@ extern "C" lh_status lh_sync(lh_ctx *ctx) {
     _lk.lock();
     if (e != cudaSuccess) return fail(ctx, LH_ERR_CUDA, "lh_sync", e);
     for (auto &sl : ctx->slots)
-        if (sl.state == SLOT_INFLIGHT && cudaEventQuery(sl.done) == cudaSuccess) sl.state = SLOT_FREE;
+        if (sl.state == SLOT_INFLIGHT && cudaEventQuery(sl.done.get()) == cudaSuccess) sl.state = SLOT_FREE;
     cudaGetLastError();
     return LH_OK;
 }
-extern "C" void *lh_ingest_stream(lh_ctx *ctx) { return ctx ? (void *)ctx->ingest_stream : nullptr; }
+extern "C" void *lh_ingest_stream(lh_ctx *ctx) { return ctx ? (void *)ctx->ingest_stream.get() : nullptr; }
 
 extern "C" lh_status lh_device_alloc(lh_ctx *ctx, size_t bytes, void **d_out) {
     LH_ENTER(ctx);
@@ -3159,7 +3149,7 @@ extern "C" lh_status lh_tune(lh_ctx *ctx, const char *key, int64_t value) {
     }
     if (!strcmp(key, "gpu_timer_slots")) {
         if (value < 1 || value > (1 << 20)) return fail(ctx, LH_ERR_RANGE, "gpu_timer_slots is 1 ... 2^20");
-        if (ctx->d_timer_marks) return fail(ctx, LH_ERR_STATE, "gpu_timer_slots is set before the first lh_gpu_timer_start");
+        if (ctx->d_timer_marks.get()) return fail(ctx, LH_ERR_STATE, "gpu_timer_slots is set before the first lh_gpu_timer_start");
         ctx->timer_slots_n = (uint32_t)value;
         return LH_OK;
     }
@@ -3190,8 +3180,8 @@ extern "C" lh_status lh_kernel_ms(lh_ctx *ctx, uint64_t seq, float *ms) {
     if (seq == 0 || seq > ctx->ingest_seq || ctx->ingest_seq - seq >= (uint64_t)lh_ctx::kTimingRing)
         return fail(ctx, LH_ERR_STATE, "that ingest launch is unknown or its events were recycled");
     const int i = (int)((seq - 1) % lh_ctx::kTimingRing);
-    LH_CUDA(ctx, cudaEventSynchronize(ctx->ev_t1s[i]));
-    LH_CUDA(ctx, cudaEventElapsedTime(ms, ctx->ev_t0s[i], ctx->ev_t1s[i]));
+    LH_CUDA(ctx, cudaEventSynchronize(ctx->ev_t1s[i].get()));
+    LH_CUDA(ctx, cudaEventElapsedTime(ms, ctx->ev_t0s[i].get(), ctx->ev_t1s[i].get()));
     return LH_OK;
 }
 
