@@ -516,6 +516,10 @@ constexpr uint32_t KS_MAX_PASSES = 4;
 // cooperative launch.
 constexpr size_t kSmemBudget = 227 * 1024;
 
+// Samples one launch of k_ingest_keyed_wc may take, both arrays of a fused pair together: its owner windows are uint32
+// cells flushed once, at the end of the launch, so no cell may receive 2^32 samples in one launch.
+constexpr size_t kWcMaxLaunch = 0xFFFFFFFFu;
+
 // What launch_keyed issues for one piece of a batch, or launch_keyed_pair for a pair (plan_keyed).
 struct KeyedPlan {
     // the kernel of the vector body (the ragged ends always go through k_ingest_keyed); APART: a pair the
@@ -534,7 +538,7 @@ struct KeyedPlan {
 // The route of keyed samples (ids, vals, n) over `nids` ids in play (ctx->H; a mapped call's k) and everything its
 // launches need; no CUDA call and no change to ctx.  No ids in play: the scalar kernel, which drops every sample.
 // A pair (float64 samples ids/vals/n, int64 samples ids2/vals2/n2) is one write-combining launch for both arrays when
-// both are vector-aligned and that kernel takes them, else APART.
+// both are vector-aligned, together at most kWcMaxLaunch samples, and that kernel takes them, else APART.
 KeyedPlan plan_keyed(const lh_ctx *ctx, uint32_t nids, size_t id_bytes, const void *ids, const void *vals, size_t n, bool pair = false,
                      const void *ids2 = nullptr, const void *vals2 = nullptr, size_t n2 = 0) {
     KeyedPlan p;
@@ -548,6 +552,7 @@ KeyedPlan plan_keyed(const lh_ctx *ctx, uint32_t nids, size_t id_bytes, const vo
         auto aligned = [&](const void *v, const void *i) { return ((uintptr_t)v & 31u) == 0 && ((uintptr_t)i & id_mask) == 0; };
         p.route = KeyedPlan::APART;
         if (!n || !n2 || ctx->keyed_mode == 1 || small || !aligned(vals, ids) || !aligned(vals2, ids2)) return p;
+        if (n + n2 > kWcMaxLaunch) return p;   // apart, each array split by launch_keyed
     } else {
         // scalar head until the values are 32-byte aligned; the vector body also needs ids aligned to 4 ids
         p.head = std::min<size_t>(n, ((32u - ((uintptr_t)vals & 31u)) & 31u) / 8u);
@@ -695,8 +700,9 @@ lh_status launch_keyed(lh_ctx *ctx, int b, const IdT *d_ids, const ValT *d_vals,
     const KeyedOut ko = keyed_out(ctx, b);
     size_t done = 0;
     while (done < n) {
-        // no uint32 cell of the hot window may wrap: drain it before 2^32 samples have gone in
-        const unsigned long long kCap = 0xFFFFFFFFull;
+        // no uint32 cell may wrap: the write-combining kernel's owner windows hold a whole launch (kWcMaxLaunch), and
+        // the hot window of the small and vector kernels everything since its last drain, which comes before 2^32
+        const unsigned long long kCap = kWcMaxLaunch;
         if (ctx->buf[b].hot_pending >= kCap - (1ull << 30)) {
             // the tally is host-side and counts what every stream has issued: the fold must come after all of it, not
             // only after this stream's kernels (each writer event follows the last bracket issued on its stream)

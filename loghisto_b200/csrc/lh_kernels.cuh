@@ -735,6 +735,8 @@ __device__ __forceinline__ void wc_spill(uint32_t rec, uint32_t owner, uint32_t 
 
 // Mapped (non-PAIR only): ids are local, owners hold ceil(k / P) windows (ids_per) and o.H's bound is k; the map is read
 // by the spills, the rare path and the final flush, which counts an unbound row's window total as dropped.
+// Bound: the owners' windows are uint32 cells, zeroed at the start and flushed once at the end of the launch, so one
+// launch takes at most 2^32 - 1 samples, n + n2 together (kWcMaxLaunch; launch_keyed and plan_keyed keep to it).
 template <typename IdT, typename ValT, int SPT, bool PAIR = false, typename Map = IdIdentity>   // PAIR: a second, int64 segment follows the float64 one
 __global__ void __launch_bounds__(WcShape<SPT>::THREADS, 1)
 k_ingest_keyed_wc(WcParams prm, Prec pc, const Map map) {

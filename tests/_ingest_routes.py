@@ -48,6 +48,10 @@ def _parse_constants() -> dict:
     c["KS_MAX_PASSES"] = _int_expr(a, r"constexpr uint32_t KS_MAX_PASSES = ([^;]+);", c)
     c["kSmemBudget"] = _int_expr(a, r"constexpr size_t kSmemBudget = ([^;]+);", c)
     c["kDefaultK1Variant"] = _int_expr(a, r"constexpr int kDefaultK1Variant = ([^;]+);", c)
+    m = re.search(r"constexpr size_t kWcMaxLaunch = 0x([0-9A-Fa-f]+)u;", a)
+    if not m:
+        raise AssertionError("dispatch constant not found in the CUDA sources: kWcMaxLaunch")
+    c["WC_MAX_LAUNCH"] = int(m.group(1), 16)
     # the owner-buffer sizes launch_keyed_wc_spt tries, largest first
     m = re.search(r"for \(uint32_t cap_try : \{([^}]*)\}\)", a)
     c["WC_ROW_CAPS"] = tuple(int(x.strip().rstrip("u")) for x in m.group(1).split(","))
@@ -208,10 +212,11 @@ def keyed_route(H: int, n: int, precision: int, sm_count: int, *, id_bytes=2, va
 
 def pair_route(H: int, n_f: int, n_ns: int, precision: int, sm_count: int, **tune) -> Route:
     """launch_keyed_pair with 32-byte aligned values and ids: one write-combining launch for both segments when it is
-    eligible, else two keyed ingests (the name is that of the last one)."""
+    eligible and they hold at most WC_MAX_LAUNCH samples together, else two keyed ingests (the route of the last one,
+    `extra["apart"]` set; an array of more than WC_MAX_LAUNCH samples that of its first piece)."""
     t = dict(DEFAULTS, **tune)
     small = small_passes(H, precision) <= 4 and t["keyed_mode"] == 0
-    if n_f and n_ns and t["keyed_mode"] != 1 and not small:
+    if n_f and n_ns and t["keyed_mode"] != 1 and not small and n_f + n_ns <= CONST["WC_MAX_LAUNCH"]:
         wc = wc_launch(H, precision, sm_count, n_f, n_ns, k1_reserve_sms=t["k1_reserve_sms"],
                        keyed_mode=t["keyed_mode"], kp_chunk=t["kp_chunk"], wc_spt=t["wc_spt"], wc_flush=t["wc_flush"])
         if wc is not None:
@@ -219,8 +224,33 @@ def pair_route(H: int, n_f: int, n_ns: int, precision: int, sm_count: int, **tun
     r = Route("")
     for m in (n_f, n_ns):
         if m:
-            r = keyed_route(H, m, precision, sm_count, previous=r.kernel, **tune)
+            r = keyed_route(H, min(m, CONST["WC_MAX_LAUNCH"]), precision, sm_count, previous=r.kernel, **tune)
+    if n_f or n_ns:
+        r.extra["apart"] = True
     return r
+
+
+def keyed_pieces(H: int, n: int, precision: int, sm_count: int, *, id_bytes=2, vals_addr=0, ids_addr=0, **tune):
+    """launch_keyed for one call whose hot window starts drained and takes nothing (every piece goes to the
+    write-combining or the scalar kernel): [(samples, Route)] of its pieces, each at most WC_MAX_LAUNCH samples and
+    routed at its own address."""
+    out, done = [], 0
+    while done < n:
+        m = min(n - done, CONST["WC_MAX_LAUNCH"])
+        r = keyed_route(H, m, precision, sm_count, id_bytes=id_bytes, vals_addr=(vals_addr + 8 * done) & 31,
+                        ids_addr=(ids_addr + id_bytes * done) & 31, **tune)
+        assert r.kernel in (WC, SCALAR), r
+        out.append((m, r))
+        done += m
+    return out
+
+
+def keyed_launches(m: int, r: Route) -> int:
+    """Kernel launches of one piece of m samples on route r (write-combining or scalar): the scalar head, the body,
+    the ragged tail past the body's whole tiles."""
+    if r.kernel == SCALAR:
+        return 1 if m else 0
+    return (1 if r.head else 0) + 1 + (1 if m - r.head - r.wc.taken else 0)
 
 
 def counter_route(C: int, n: int, *, id_bytes=2, amounts_addr=0, ids_addr=0) -> Route:

@@ -75,6 +75,25 @@ def test_pair_route():
     assert R.pair_route(1024, 1 << 21, 0, 100, SMS).kernel == R.VEC
     assert R.pair_route(44, 1 << 22, 1 << 22, 100, SMS).kernel == R.SMALL
     assert R.pair_route(1024, 1 << 22, 1 << 22, 100, SMS, keyed_mode=1).kernel == R.VEC
+    # the owner windows are uint32 for a whole launch: a fused pair takes at most 2^32 - 1 samples
+    assert R.CONST["WC_MAX_LAUNCH"] == 2 ** 32 - 1
+    fused = R.pair_route(1024, 2 ** 31, 2 ** 31 - 1, 100, SMS)
+    assert fused.kernel == R.WC and fused.wc.taken + fused.wc.taken2 > 2 ** 32 - 4096 and "apart" not in fused.extra
+    apart = R.pair_route(1024, 2 ** 31, 2 ** 31, 100, SMS)
+    assert apart.kernel == R.WC and apart.extra["apart"] and apart.wc.taken2 == 0
+    assert R.pair_route(1024, 2 ** 20, 2 ** 32, 100, SMS).extra["apart"]
+
+
+def test_keyed_pieces():
+    """A call of more than 2^32 - 1 samples on the write-combining route goes out in pieces of at most 2^32 - 1, each
+    routed at its own address: 2^32 - 1 is odd, so the pieces after the first start 24, 16 and 8 bytes past a 32-byte
+    boundary and take scalar heads of 1, 2 and 3 samples."""
+    n = 3 * (2 ** 32 - 1) + 5
+    pieces = R.keyed_pieces(32, n, 100, SMS, k1_reserve_sms=SMS - 32, keyed_mode=2)
+    assert [m for m, _ in pieces] == [2 ** 32 - 1] * 3 + [5]
+    assert [r.kernel for _, r in pieces] == [R.WC] * 3 + [R.SCALAR]
+    assert [r.head for _, r in pieces] == [0, 1, 2, 3]
+    assert [R.keyed_launches(m, r) for m, r in pieces] == [2, 3, 3, 1]
 
 
 def test_counter_routes():
