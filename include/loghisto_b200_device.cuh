@@ -25,6 +25,9 @@
 //
 // Every function here has internal or inline linkage: the header may be included by several translation units of one
 // program, with or without -rdc=true.  Needs sm_70 or later (__match_any_sync); the library itself targets sm_90a.
+// tests/test_device_api_builds_cpu.py compiles it warning-free under C++14 / 17 / 20 for compute_70 PTX, sm_80, sm_90 and
+// sm_90a and device-links two -rdc=true units; tests/test_gpu_device_api_builds.py runs one client built with the
+// library's flags, --use_fast_math, -G, -maxrregcount=32, -rdc=true and as compute_90 / compute_70 PTX against the oracle.
 //
 // Bucket arithmetic -- two evaluators of compress() (reference metrics.go:316-322; `precision` is metrics.go:40-43,
 // 100 by default and configurable through lh_config.precision):

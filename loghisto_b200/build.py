@@ -109,6 +109,78 @@ GAUGE_CLIENT_LIB = os.path.join(ROOT, "tests", "_build", "libgauge_write_client.
 RAW_CLIENT_SRC = os.path.join(ROOT, "tests", "raw_read_client.cu")
 RAW_CLIENT_LIB = os.path.join(ROOT, "tests", "_build", "libraw_read_client.so")
 
+# One client of the device API built the ways callers build it (tests/device_matrix_client.cu; tests/
+# test_gpu_device_api_builds.py runs every variant against the oracle).  Each variant adds -std=c++17 -Xcompiler -fPIC
+# -shared -I include; "rdc" compiles the client as two translation units (-DLHM_PART=1 / 2) and device-links them.
+MATRIX_SRC = os.path.join(ROOT, "tests", "device_matrix_client.cu")
+MATRIX_DIR = os.path.join(ROOT, "tests", "_build", "device_matrix")
+MATRIX_LIB_NAME = "libdevice_matrix_client.so"
+_SM90A = ["-gencode", "arch=compute_90a,code=sm_90a"]
+_MATRIX_REF = _SM90A + ["-O3", "--fmad=true"]          # the library's device flags
+DEVICE_MATRIX = {
+    "ref": _MATRIX_REF,
+    "fastmath": _MATRIX_REF + ["--use_fast_math"],
+    "debug": _SM90A + ["-G"],
+    "maxrreg": _MATRIX_REF + ["-maxrregcount=32"],
+    "rdc": _MATRIX_REF + ["-rdc=true"],
+    "ptx90": ["-gencode", "arch=compute_90,code=compute_90"],
+    "ptx70": ["-gencode", "arch=compute_70,code=compute_70", "-Wno-deprecated-gpu-targets"],
+}
+
+
+def matrix_lib(variant: str) -> str:
+    return os.path.join(MATRIX_DIR, variant, MATRIX_LIB_NAME)
+
+
+def _matrix_commands(nvcc: str, variant: str) -> list:
+    """The nvcc commands that build one variant, in order."""
+    flags = DEVICE_MATRIX[variant] + ["-std=c++17", "-Xcompiler", "-fPIC", "-I", os.path.join(ROOT, "include")]
+    out = matrix_lib(variant)
+    if variant != "rdc":
+        return [[nvcc] + flags + ["-shared", "-o", out, MATRIX_SRC]]
+    objs = [os.path.join(MATRIX_DIR, variant, "part%d.o" % k) for k in (1, 2)]
+    return ([[nvcc] + flags + ["-DLHM_PART=%d" % k, "-c", "-o", o, MATRIX_SRC] for k, o in zip((1, 2), objs)]
+            + [[nvcc] + flags + ["-shared", "-o", out] + objs])
+
+
+def _build_matrix_variant(nvcc: str, variant: str, force: bool):
+    """Builds one variant unless its library is newer than the sources and was built by the same commands (kept beside
+    it in commands.txt).  Returns None, or the failing command and its output."""
+    lib = matrix_lib(variant)
+    stamp = os.path.join(os.path.dirname(lib), "commands.txt")
+    cmds = _matrix_commands(nvcc, variant)
+    text = "\n".join(" ".join(c) for c in cmds) + "\n"
+    deps = [MATRIX_SRC, DEVICE_HEADER, os.path.join(ROOT, "include", "loghisto_b200.h")]
+    if not force and os.path.exists(lib) and os.path.exists(stamp) and _newest(deps) <= os.path.getmtime(lib):
+        with open(stamp) as f:
+            if f.read() == text:
+                return None
+    os.makedirs(os.path.dirname(lib), exist_ok=True)
+    if os.path.exists(stamp):
+        os.remove(stamp)
+    for c in cmds:
+        res = subprocess.run(c, capture_output=True, text=True)
+        if res.returncode != 0:
+            return " ".join(c) + "\n" + res.stdout + res.stderr
+    with open(stamp, "w") as f:
+        f.write(text)
+    return None
+
+
+def build_device_matrix(force: bool = False) -> dict:
+    """Every variant of DEVICE_MATRIX, built side by side; returns {variant: library path}."""
+    from concurrent.futures import ThreadPoolExecutor
+    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+    if not os.path.exists(nvcc):
+        raise RuntimeError("nvcc not found: cannot build the device-API build matrix")
+    with ThreadPoolExecutor(max_workers=len(DEVICE_MATRIX)) as pool:
+        errors = list(pool.map(lambda v: _build_matrix_variant(nvcc, v, force), DEVICE_MATRIX))
+    for e in errors:
+        if e:
+            sys.stderr.write(e)
+            raise RuntimeError("nvcc failed building the device-API build matrix")
+    return {v: matrix_lib(v) for v in DEVICE_MATRIX}
+
 
 def build_device_client(force: bool = False) -> str:
     """CUDA clients of the device API (tests/device_record_client.cu, tests/named_record_client.cu,
@@ -116,7 +188,7 @@ def build_device_client(force: bool = False) -> str:
     tests/board_read_client.cu, tests/gauge_write_client.cu, tests/raw_read_client.cu): separate shared libraries that
     record into a context from their own kernels, give the GPU timers spans to measure, read device subscriptions,
     write device gauges, or query raw device subscriptions, knowing the library only through the public headers.
-    Returns the path of the first."""
+    Then the device-API build matrix (build_device_matrix).  Returns the path of the first."""
     for src, lib in ((CLIENT_SRC, CLIENT_LIB), (NAMED_CLIENT_SRC, NAMED_CLIENT_LIB), (BLOCK_CLIENT_SRC, BLOCK_CLIENT_LIB),
                      (TIMER_CLIENT_SRC, TIMER_CLIENT_LIB), (GRAPH_CLIENT_SRC, GRAPH_CLIENT_LIB),
                      (BOARD_CLIENT_SRC, BOARD_CLIENT_LIB), (GAUGE_CLIENT_SRC, GAUGE_CLIENT_LIB),
@@ -134,6 +206,7 @@ def build_device_client(force: bool = False) -> str:
         if res.returncode != 0:
             sys.stderr.write(res.stdout + res.stderr)
             raise RuntimeError("nvcc failed building " + lib)
+    build_device_matrix(force)
     return CLIENT_LIB
 
 
