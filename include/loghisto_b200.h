@@ -141,7 +141,8 @@ typedef struct lh_batch_item {
 } lh_batch_item;
 LH_API lh_status lh_ingest_batch(lh_ctx *ctx, const lh_batch_item *h_items, uint32_t n_items, void *stream);
 
-/* Counter(name, amount), metrics.go:251-269: wrapping uint64 adds. */
+/* Counter(name, amount), metrics.go:251-269: wrapping uint64 adds.  NULL inputs with n > 0, amounts not 8-byte aligned
+ * or ids not naturally aligned give LH_ERR_INVALID, before anything is enqueued. */
 LH_API lh_status lh_counter_add_u16(lh_ctx *ctx, const uint16_t *d_ids, const uint64_t *d_amounts,
                              size_t n, void *stream);
 LH_API lh_status lh_counter_add_u32(lh_ctx *ctx, const uint32_t *d_ids, const uint64_t *d_amounts,

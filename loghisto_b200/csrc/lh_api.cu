@@ -494,15 +494,14 @@ KeyedOut keyed_out(lh_ctx *ctx, int b) {
 }
 
 // The scalar keyed kernel over a ragged piece (a head before the aligned body, a tail after it); nothing when n == 0.
-// With a map (record-scope ids), its mapped form, which copies the map into shared memory.
-template <typename IdT, typename ValT>
+// With an IdMap (record-scope ids), its mapped form, which copies the map into shared memory.
+template <typename IdT, typename ValT, typename Map>
 void launch_keyed_scalar(lh_ctx *ctx, const KeyedOut &ko, const IdT *ids, const ValT *vals, size_t n, cudaStream_t s,
-                         const IdMap *map = nullptr) {
+                         const Map &map) {
     if (!n) return;
     constexpr int T = 256;
     const int grid = grid_1d(ctx, n, T, 1, ctx->keyed_blocks_per_sm);
-    if (map) k_ingest_keyed<IdT, ValT, T, IdMap><<<grid, T, (size_t)map->k * 4, s>>>(ids, vals, n, ko, ctx->pc, *map);
-    else k_ingest_keyed<IdT, ValT, T><<<grid, T, 0, s>>>(ids, vals, n, ko, ctx->pc, IdIdentity{});
+    k_ingest_keyed<IdT, ValT, T, Map><<<grid, T, map_smem_bytes(map), s>>>(ids, vals, n, ko, ctx->pc, map);
     ctx->stats.kernel_launches++;
 }
 
@@ -519,6 +518,18 @@ constexpr size_t kSmemBudget = 227 * 1024;
 // Samples one launch of k_ingest_keyed_wc may take, both arrays of a fused pair together: its owner windows are uint32
 // cells flushed once, at the end of the launch, so no cell may receive 2^32 samples in one launch.
 constexpr size_t kWcMaxLaunch = 0xFFFFFFFFu;
+
+// The write-combining tile shape of a wc_spt value (6, 4 or 3; any other value is 8): f(std::integral_constant<int, SPT>),
+// so that f can name WcShape<SPT> and the kernels of that shape.
+template <typename F>
+auto with_wc_shape(int spt, F f) {
+    switch (spt) {
+    case 6: return f(std::integral_constant<int, 6>{});
+    case 4: return f(std::integral_constant<int, 4>{});
+    case 3: return f(std::integral_constant<int, 3>{});
+    default: return f(std::integral_constant<int, 8>{});
+    }
+}
 
 // What launch_keyed issues for one piece of a batch, or launch_keyed_pair for a pair (plan_keyed).
 struct KeyedPlan {
@@ -587,13 +598,12 @@ KeyedPlan plan_keyed(const lh_ctx *ctx, uint32_t nids, size_t id_bytes, const vo
     }
     if (!row_cap || (size_t)ids_per * ctx->pc.win > 65535) return p;           // records are 16-bit (lid*win + slot)
     if (ctx->keyed_mode != 2 && n + n2 < ((size_t)1 << 22)) return p;          // small batches: the L2-atomic kernel
-    const int spt = ctx->wc_spt == 6 || ctx->wc_spt == 4 || ctx->wc_spt == 3 ? ctx->wc_spt : 8;
-    const int tile = spt == 6 ? WcShape<6>::TILE : spt == 4 ? WcShape<4>::TILE : spt == 3 ? WcShape<3>::TILE : WcShape<8>::TILE;
+    int spt = 0, tile = 0, threads = 0;
+    with_wc_shape(ctx->wc_spt, [&](auto c) { spt = c; tile = WcShape<c>::TILE; threads = WcShape<c>::THREADS; });
     const size_t taken = n / tile * tile, taken2 = n2 / tile * tile;   // whole tiles only
     if (taken + taken2 == 0) return p;
     p.route = KeyedPlan::WC; p.name = "k_ingest_keyed_wc";
-    p.taken = taken; p.taken2 = taken2; p.grid = P; p.smem = smem; p.spt = spt;
-    p.threads = spt == 6 ? WcShape<6>::THREADS : spt == 4 ? WcShape<4>::THREADS : spt == 3 ? WcShape<3>::THREADS : WcShape<8>::THREADS;
+    p.taken = taken; p.taken2 = taken2; p.grid = P; p.smem = smem; p.spt = spt; p.threads = threads;
     WcParams &w = p.wc;
     w.n = taken; w.n2 = taken2; w.ids_per = ids_per; w.row_cap = row_cap; w.row_stride = row_cap + WC_ROW_EXTRA;
     w.inv_p = (uint32_t)(((uint64_t)1 << 32) / (uint64_t)P) + 1u;
@@ -639,10 +649,10 @@ cudaError_t wc_done_event(int device, cudaEvent_t *out) {
 }
 
 // The write-combining launch of plan p: its first p.taken samples of (ids, vals) and, in a fused pair, the first
-// p.taken2 int64 samples of (ids2, vals2).
-template <typename IdT, typename ValT>
+// p.taken2 int64 samples of (ids2, vals2).  A fused pair is never mapped.
+template <typename IdT, typename ValT, typename Map>
 lh_status launch_keyed_wc(lh_ctx *ctx, int b, const KeyedPlan &p, const IdT *ids, const ValT *vals, cudaStream_t s,
-                          const IdT *ids2 = nullptr, const long long *vals2 = nullptr, const IdMap *map = nullptr) {
+                          const Map &map, const IdT *ids2 = nullptr, const long long *vals2 = nullptr) {
     const int P = p.grid;
     if (!ctx->d_kp_queues.get() || ctx->kp_cap != p.wc.cap || ctx->kp_parts != P) {
         if (ctx->d_kp_queues.get()) {
@@ -663,12 +673,10 @@ lh_status launch_keyed_wc(lh_ctx *ctx, int b, const KeyedPlan &p, const IdT *ids
         ctx->kp_cap = p.wc.cap; ctx->kp_parts = P;
     }
     // the kernel of the planned tile shape; with an int64 second segment, its PAIR form (on the float64 instantiation)
-#define LH_WC_KERNEL(SPT) (!p.taken2 ? (const void *)k_ingest_keyed_wc<IdT, ValT, SPT, false> : (const void *)k_ingest_keyed_wc<IdT, double, SPT, true>)
-    const void *fn = p.spt == 6 ? LH_WC_KERNEL(6) : p.spt == 4 ? LH_WC_KERNEL(4) : p.spt == 3 ? LH_WC_KERNEL(3) : LH_WC_KERNEL(8);
-#undef LH_WC_KERNEL
-#define LH_WC_MAPPED(SPT) (const void *)k_ingest_keyed_wc<IdT, ValT, SPT, false, IdMap>
-    if (map) fn = p.spt == 6 ? LH_WC_MAPPED(6) : p.spt == 4 ? LH_WC_MAPPED(4) : p.spt == 3 ? LH_WC_MAPPED(3) : LH_WC_MAPPED(8);
-#undef LH_WC_MAPPED
+    const void *fn = with_wc_shape(p.spt, [&](auto c) {
+        if constexpr (kMapped<Map>) return (const void *)k_ingest_keyed_wc<IdT, ValT, c, false, Map>;
+        else return !p.taken2 ? (const void *)k_ingest_keyed_wc<IdT, ValT, c, false> : (const void *)k_ingest_keyed_wc<IdT, double, c, true>;
+    });
     // the attribute belongs to the function on the device, not to this context: one value for every context
     LH_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
     WcParams prm = p.wc;
@@ -676,8 +684,7 @@ lh_status launch_keyed_wc(lh_ctx *ctx, int b, const KeyedPlan &p, const IdT *ids
     prm.queues = ctx->d_kp_queues.get(); prm.q_cnt = ctx->d_kp_cnt.get(); prm.barrier = ctx->d_kp_cnt.get() + (size_t)2 * P * P;
     prm.rare = ctx->d_kp_rare.get(); prm.o = keyed_out(ctx, b);
     Prec pc = ctx->pc;
-    IdIdentity ident;
-    void *args[] = {&prm, &pc, map ? (void *)map : (void *)&ident};
+    void *args[] = {&prm, &pc, (void *)&map};
     {
         std::lock_guard<std::mutex> lk(g_wc_mu);
         cudaEvent_t done;
@@ -691,12 +698,12 @@ lh_status launch_keyed_wc(lh_ctx *ctx, int b, const KeyedPlan &p, const IdT *ids
     return LH_OK;
 }
 
-// With a map, ids are local to it (record-scope calls): the plan counts map->k ids and the kernels are the mapped forms.
-template <typename IdT, typename ValT>
-lh_status launch_keyed(lh_ctx *ctx, int b, const IdT *d_ids, const ValT *d_vals, size_t n, cudaStream_t s,
-                       const IdMap *map = nullptr) {
+// With an IdMap, ids are local to it (record-scope calls): the plan counts map.k ids and the kernels are the mapped forms.
+template <typename IdT, typename ValT, typename Map>
+lh_status launch_keyed(lh_ctx *ctx, int b, const IdT *d_ids, const ValT *d_vals, size_t n, cudaStream_t s, const Map &map) {
     constexpr int T = 256;
-    const uint32_t nids = map ? map->k : ctx->H;
+    uint32_t nids = ctx->H;
+    if constexpr (kMapped<Map>) nids = map.k;
     const KeyedOut ko = keyed_out(ctx, b);
     size_t done = 0;
     while (done < n) {
@@ -719,25 +726,19 @@ lh_status launch_keyed(lh_ctx *ctx, int b, const IdT *d_ids, const ValT *d_vals,
         if (p.route == KeyedPlan::SMALL) {
             // per device, not per context: a value of this context's H could be overwritten by another context's
             // between here and the launch
-            const void *fn = map ? (const void *)k_ingest_keyed_small<IdT, ValT, IdMap> : (const void *)k_ingest_keyed_small<IdT, ValT>;
+            const void *fn = (const void *)k_ingest_keyed_small<IdT, ValT, Map>;
             LH_CUDA(ctx, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
             for (uint32_t lo = 0; lo < nids; lo += p.per) {
                 const uint32_t cnt = std::min(p.per, nids - lo);
-                if (map)
-                    k_ingest_keyed_small<IdT, ValT, IdMap><<<p.grid, KS_THREADS, p.smem, s>>>(ids + p.head, vals + p.head, p.n4, lo, cnt, ko, ctx->pc, *map);
-                else
-                    k_ingest_keyed_small<IdT, ValT><<<p.grid, KS_THREADS, p.smem, s>>>(ids + p.head, vals + p.head, p.n4, lo, cnt, ko, ctx->pc, IdIdentity{});
+                k_ingest_keyed_small<IdT, ValT, Map><<<p.grid, KS_THREADS, p.smem, s>>>(ids + p.head, vals + p.head, p.n4, lo, cnt, ko, ctx->pc, map);
                 ctx->stats.kernel_launches++;
             }
         } else if (p.route == KeyedPlan::WC) {
-            lh_status st = launch_keyed_wc<IdT, ValT>(ctx, b, p, ids + p.head, vals + p.head, s, nullptr, nullptr, map);
+            lh_status st = launch_keyed_wc<IdT, ValT>(ctx, b, p, ids + p.head, vals + p.head, s, map);
             if (st != LH_OK) return st;
         } else if (p.route == KeyedPlan::VEC) {
             const int grid = grid_1d(ctx, p.n4, T, 1, ctx->keyed_blocks_per_sm);
-            if (map)
-                k_ingest_keyed_vec<IdT, ValT, T, IdMap><<<grid, T, (size_t)map->k * 4, s>>>(ids + p.head, vals + p.head, p.n4, ctx->hot_replicas, ko, ctx->pc, *map);
-            else
-                k_ingest_keyed_vec<IdT, ValT, T><<<grid, T, 0, s>>>(ids + p.head, vals + p.head, p.n4, ctx->hot_replicas, ko, ctx->pc, IdIdentity{});
+            k_ingest_keyed_vec<IdT, ValT, T, Map><<<grid, T, map_smem_bytes(map), s>>>(ids + p.head, vals + p.head, p.n4, ctx->hot_replicas, ko, ctx->pc, map);
             ctx->stats.kernel_launches++;
         }
         ctx->keyed_kernel = p.name;
@@ -760,31 +761,32 @@ lh_status launch_keyed_pair(lh_ctx *ctx, int b, const IdT *ids_f, const double *
                             const long long *vals_ns, size_t n_ns, cudaStream_t s) {
     const KeyedPlan p = plan_keyed(ctx, ctx->H, sizeof(IdT), ids_f, vals_f, n_f, true, ids_ns, vals_ns, n_ns);
     if (p.route == KeyedPlan::APART) {
-        lh_status st = launch_keyed<IdT, double>(ctx, b, ids_f, vals_f, n_f, s);
+        lh_status st = launch_keyed<IdT, double>(ctx, b, ids_f, vals_f, n_f, s, IdIdentity{});
         if (st != LH_OK) return st;
-        return launch_keyed<IdT, long long>(ctx, b, ids_ns, vals_ns, n_ns, s);
+        return launch_keyed<IdT, long long>(ctx, b, ids_ns, vals_ns, n_ns, s, IdIdentity{});
     }
-    lh_status st = launch_keyed_wc<IdT, double>(ctx, b, p, ids_f, vals_f, s, ids_ns, vals_ns);
+    lh_status st = launch_keyed_wc<IdT, double>(ctx, b, p, ids_f, vals_f, s, IdIdentity{}, ids_ns, vals_ns);
     if (st != LH_OK) return st;
     ctx->keyed_kernel = p.name;
     const KeyedOut ko = keyed_out(ctx, b);
-    launch_keyed_scalar(ctx, ko, ids_f + p.taken, vals_f + p.taken, n_f - p.taken, s);   // the ragged ends
-    launch_keyed_scalar(ctx, ko, ids_ns + p.taken2, vals_ns + p.taken2, n_ns - p.taken2, s);
+    launch_keyed_scalar(ctx, ko, ids_f + p.taken, vals_f + p.taken, n_f - p.taken, s, IdIdentity{});   // the ragged ends
+    launch_keyed_scalar(ctx, ko, ids_ns + p.taken2, vals_ns + p.taken2, n_ns - p.taken2, s, IdIdentity{});
     LH_CUDA(ctx, cudaGetLastError());
     ctx->stats.samples += n_f + n_ns;
     return LH_OK;
 }
 
 // (id, amount) pairs into `counters` (C of them, ids >= C dropped and counted); the caller counts the ops in stats.
-// With a map, ids are local: C is map->k (<= LH_MAP_MAX, so always the shared-memory kernels, whose mapped forms take
+// With an IdMap, ids are local: C is map.k (<= LH_MAP_MAX, so always the shared-memory kernels, whose mapped forms take
 // the map after the 2C halves: 12 B per id, 48 KiB at most) and an op under an unbound row is dropped and counted.
-template <typename IdT>
+static_assert(LH_MAP_MAX <= (uint32_t)K2_SMEM_COUNTERS, "k_counter_add has no mapped form");
+template <typename IdT, typename Map>
 lh_status launch_counter(lh_ctx *ctx, unsigned long long *counters, uint32_t C, const IdT *d_ids, const uint64_t *d_amounts,
-                         size_t n, cudaStream_t s, const IdMap *map = nullptr) {
+                         size_t n, cudaStream_t s, const Map &map) {
     if (n) {
         constexpr int T = 512;
         const unsigned long long *amts = reinterpret_cast<const unsigned long long *>(d_amounts);
-        if (C <= (uint32_t)K2_SMEM_COUNTERS) {
+        if (kMapped<Map> || C <= (uint32_t)K2_SMEM_COUNTERS) {
             // privatised per CTA (lo/hi halves in shared memory).  Vector body where the alignment allows: 4 ops per
             // thread and iteration; ragged head / tail through the scalar form of the same kernel.
             size_t head = std::min<size_t>(n, ((32u - ((uintptr_t)amts & 31u)) & 31u) / 8u);
@@ -792,22 +794,20 @@ lh_status launch_counter(lh_ctx *ctx, unsigned long long *counters, uint32_t C, 
             size_t n4 = vec_ok ? (n - head) / 4 : 0;
             if (n4 < 4096) { head = 0; n4 = 0; }
             const size_t tail_off = head + n4 * 4;
-            const size_t smem = (size_t)C * 8 + (map ? (size_t)C * 4 : 0);
+            const size_t smem = (size_t)C * 8 + map_smem_bytes(map);
             auto scalar = [&](int grid, size_t off, size_t cnt) {
-                if (map) k_counter_add_smem<IdT, T, IdMap><<<grid, T, smem, s>>>(d_ids + off, amts + off, cnt, counters, C, ctx->d_dropped.get(), *map);
-                else k_counter_add_smem<IdT, T><<<grid, T, smem, s>>>(d_ids + off, amts + off, cnt, counters, C, ctx->d_dropped.get(), IdIdentity{});
+                k_counter_add_smem<IdT, T, Map><<<grid, T, smem, s>>>(d_ids + off, amts + off, cnt, counters, C, ctx->d_dropped.get(), map);
                 ctx->stats.kernel_launches++;
             };
             if (head) scalar(1, 0, head);
             if (n4) {
                 // one CTA per SM (the per-CTA flush is C global atomics), fewer for small batches
                 const int grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)std::max(1, ctx->sm_count - ctx->k1_reserve_sms) * 2, n4 / (T * 4)));
-                if (map) k_counter_add_smem_vec<IdT, T, IdMap><<<grid, T, smem, s>>>(d_ids + head, amts + head, n4, counters, C, ctx->d_dropped.get(), *map);
-                else k_counter_add_smem_vec<IdT, T><<<grid, T, smem, s>>>(d_ids + head, amts + head, n4, counters, C, ctx->d_dropped.get(), IdIdentity{});
+                k_counter_add_smem_vec<IdT, T, Map><<<grid, T, smem, s>>>(d_ids + head, amts + head, n4, counters, C, ctx->d_dropped.get(), map);
                 ctx->stats.kernel_launches++;
             }
             if (tail_off < n) scalar(grid_1d(ctx, n - tail_off, T, 8, 2), tail_off, n - tail_off);
-        } else {
+        } else if constexpr (!kMapped<Map>) {
             int grid = grid_1d(ctx, n, T, 4, 4);
             k_counter_add<IdT, T><<<grid, T, 0, s>>>(d_ids, amts, n, counters, C, ctx->d_dropped.get());
             ctx->stats.kernel_launches++;
@@ -816,10 +816,11 @@ lh_status launch_counter(lh_ctx *ctx, unsigned long long *counters, uint32_t C, 
     }
     return LH_OK;
 }
-// n counter ops into buffer b, counted in stats
-template <typename IdT>
-lh_status add_counters(lh_ctx *ctx, int b, const IdT *d_ids, const uint64_t *d_amounts, size_t n, cudaStream_t s) {
-    lh_status st = launch_counter<IdT>(ctx, ctx->buf[b].d_counters.get(), ctx->C, d_ids, d_amounts, n, s);
+// n counter ops into buffer b's counters (C of them; a mapped call's kc), counted in stats
+template <typename IdT, typename Map>
+lh_status add_counters(lh_ctx *ctx, int b, uint32_t C, const IdT *d_ids, const uint64_t *d_amounts, size_t n, cudaStream_t s,
+                       const Map &map) {
+    lh_status st = launch_counter<IdT>(ctx, ctx->buf[b].d_counters.get(), C, d_ids, d_amounts, n, s, map);
     if (st == LH_OK) ctx->stats.counter_ops += n;
     return st;
 }
@@ -1273,13 +1274,25 @@ extern "C" lh_status lh_destroy(lh_ctx *ctx) {
     LH_CUDA((ctx), cudaSetDevice((ctx)->device))
 
 namespace {
+// A device (ids, values | amounts) pair of n entries: not NULL when n > 0, the 8-byte values or amounts 8-byte aligned
+// and the ids naturally aligned, so that no kernel makes a misaligned load.
+template <typename IdT>
+lh_status check_pairs(lh_ctx *ctx, const IdT *ids, const void *vals, size_t n) {
+    if (n && (!ids || !vals)) return fail(ctx, LH_ERR_INVALID, "NULL input");
+    if (((uintptr_t)vals & 7u) || ((uintptr_t)ids & (sizeof(IdT) - 1)))
+        return fail(ctx, LH_ERR_INVALID, "values / amounts not 8-byte aligned or ids not naturally aligned");
+    return LH_OK;
+}
+lh_status check_kind(lh_ctx *ctx, uint32_t kind) {
+    if (kind != LH_VALUES_F64 && kind != LH_VALUES_I64NS) return fail(ctx, LH_ERR_INVALID, "unknown values kind");
+    return LH_OK;
+}
+
 template <typename IdT, typename ValT>
 lh_status ingest_keyed(lh_ctx *ctx, const IdT *d_ids, const ValT *d_vals, size_t n, void *stream) {
-    if (n && (!d_ids || !d_vals)) return fail(ctx, LH_ERR_INVALID, "NULL input");
-    if (((uintptr_t)d_vals & 7u) || ((uintptr_t)d_ids & (sizeof(IdT) - 1)))
-        return fail(ctx, LH_ERR_INVALID, "ids / values are not naturally aligned");
+    if (lh_status st = check_pairs(ctx, d_ids, d_vals, n); st != LH_OK) return st;
     cudaStream_t s = pick_stream(ctx, stream);
-    return write_bracket(ctx, s, [&](int b) { return launch_keyed<IdT, ValT>(ctx, b, d_ids, d_vals, n, s); });
+    return write_bracket(ctx, s, [&](int b) { return launch_keyed<IdT, ValT>(ctx, b, d_ids, d_vals, n, s, IdIdentity{}); });
 }
 }  // namespace
 
@@ -1307,9 +1320,8 @@ extern "C" lh_status lh_ingest_keyed_i64ns_u16(lh_ctx *ctx, const uint16_t *d_id
 extern "C" lh_status lh_ingest_keyed_pair_u16(lh_ctx *ctx, const uint16_t *d_ids_f64, const double *d_values, size_t n_f64,
                                               const uint16_t *d_ids_ns, const int64_t *d_nanos, size_t n_ns, void *stream) {
     LH_ENTER(ctx);
-    if ((n_f64 && (!d_ids_f64 || !d_values)) || (n_ns && (!d_ids_ns || !d_nanos))) return fail(ctx, LH_ERR_INVALID, "NULL input");
-    if (((uintptr_t)d_values & 7u) || ((uintptr_t)d_nanos & 7u) || ((uintptr_t)d_ids_f64 & 1u) || ((uintptr_t)d_ids_ns & 1u))
-        return fail(ctx, LH_ERR_INVALID, "ids / values are not naturally aligned");
+    if (lh_status st = check_pairs(ctx, d_ids_f64, d_values, n_f64); st != LH_OK) return st;
+    if (lh_status st = check_pairs(ctx, d_ids_ns, d_nanos, n_ns); st != LH_OK) return st;
     if (n_f64 == 0 && n_ns == 0) return LH_OK;
     cudaStream_t s = pick_stream(ctx, stream);
     const long long *nanos = reinterpret_cast<const long long *>(d_nanos);
@@ -1319,15 +1331,15 @@ extern "C" lh_status lh_ingest_keyed_pair_u16(lh_ctx *ctx, const uint16_t *d_ids
 }
 extern "C" lh_status lh_counter_add_u16(lh_ctx *ctx, const uint16_t *d_ids, const uint64_t *d_amounts, size_t n, void *stream) {
     LH_ENTER(ctx);
-    if (n && (!d_ids || !d_amounts)) return fail(ctx, LH_ERR_INVALID, "NULL input");
+    if (lh_status st = check_pairs(ctx, d_ids, d_amounts, n); st != LH_OK) return st;
     cudaStream_t s = pick_stream(ctx, stream);
-    return write_bracket(ctx, s, [&](int b) { return add_counters<unsigned short>(ctx, b, d_ids, d_amounts, n, s); });
+    return write_bracket(ctx, s, [&](int b) { return add_counters<unsigned short>(ctx, b, ctx->C, d_ids, d_amounts, n, s, IdIdentity{}); });
 }
 extern "C" lh_status lh_counter_add_u32(lh_ctx *ctx, const uint32_t *d_ids, const uint64_t *d_amounts, size_t n, void *stream) {
     LH_ENTER(ctx);
-    if (n && (!d_ids || !d_amounts)) return fail(ctx, LH_ERR_INVALID, "NULL input");
+    if (lh_status st = check_pairs(ctx, d_ids, d_amounts, n); st != LH_OK) return st;
     cudaStream_t s = pick_stream(ctx, stream);
-    return write_bracket(ctx, s, [&](int b) { return add_counters<unsigned int>(ctx, b, d_ids, d_amounts, n, s); });
+    return write_bracket(ctx, s, [&](int b) { return add_counters<unsigned int>(ctx, b, ctx->C, d_ids, d_amounts, n, s, IdIdentity{}); });
 }
 static_assert(LH_MAP_MAX == LH_MAP_MAX_IDS, "the header and the kernels agree on the map size");
 namespace {
@@ -1346,35 +1358,27 @@ lh_status make_map(lh_ctx *ctx, const uint32_t *h_map, uint32_t k, uint32_t limi
 template <typename IdT>
 lh_status ingest_keyed_mapped(lh_ctx *ctx, const uint32_t *h_map, uint32_t k, const IdT *d_ids, const void *d_values,
                               uint32_t kind, size_t n, void *stream) {
-    if (kind != LH_VALUES_F64 && kind != LH_VALUES_I64NS) return fail(ctx, LH_ERR_INVALID, "unknown values kind");
-    if (n && (!d_ids || !d_values)) return fail(ctx, LH_ERR_INVALID, "NULL input");
-    if (((uintptr_t)d_values & 7u) || ((uintptr_t)d_ids & (sizeof(IdT) - 1)))
-        return fail(ctx, LH_ERR_INVALID, "ids / values are not naturally aligned");
+    if (lh_status st = check_kind(ctx, kind); st != LH_OK) return st;
+    if (lh_status st = check_pairs(ctx, d_ids, d_values, n); st != LH_OK) return st;
     IdMap m;
     lh_status st = make_map(ctx, h_map, k, ctx->H, m);
     if (st != LH_OK || n == 0) return st;
     cudaStream_t s = pick_stream(ctx, stream);
     return write_bracket(ctx, s, [&](int b) {
-        return kind == LH_VALUES_F64 ? launch_keyed<IdT, double>(ctx, b, d_ids, static_cast<const double *>(d_values), n, s, &m)
-                                     : launch_keyed<IdT, long long>(ctx, b, d_ids, static_cast<const long long *>(d_values), n, s, &m);
+        return kind == LH_VALUES_F64 ? launch_keyed<IdT, double>(ctx, b, d_ids, static_cast<const double *>(d_values), n, s, m)
+                                     : launch_keyed<IdT, long long>(ctx, b, d_ids, static_cast<const long long *>(d_values), n, s, m);
     });
 }
 
 template <typename IdT>
 lh_status counter_add_mapped(lh_ctx *ctx, const uint32_t *h_map, uint32_t kc, const IdT *d_ids, const uint64_t *d_amounts,
                              size_t n, void *stream) {
-    if (n && (!d_ids || !d_amounts)) return fail(ctx, LH_ERR_INVALID, "NULL input");
-    if (((uintptr_t)d_amounts & 7u) || ((uintptr_t)d_ids & (sizeof(IdT) - 1)))
-        return fail(ctx, LH_ERR_INVALID, "ids / amounts are not naturally aligned");
+    if (lh_status st = check_pairs(ctx, d_ids, d_amounts, n); st != LH_OK) return st;
     IdMap m;
     lh_status st = make_map(ctx, h_map, kc, ctx->C, m);
     if (st != LH_OK || n == 0) return st;
     cudaStream_t s = pick_stream(ctx, stream);
-    return write_bracket(ctx, s, [&](int b) {
-        lh_status r = launch_counter<IdT>(ctx, ctx->buf[b].d_counters.get(), kc, d_ids, d_amounts, n, s, &m);
-        if (r == LH_OK) ctx->stats.counter_ops += n;
-        return r;
-    });
+    return write_bracket(ctx, s, [&](int b) { return add_counters<IdT>(ctx, b, kc, d_ids, d_amounts, n, s, m); });
 }
 }  // namespace
 
@@ -1439,9 +1443,9 @@ lh_status staging_step(lh_ctx *ctx, Slot &sl, HostKind kind, uint32_t hid, const
         st = write_bracket(ctx, s, [&](int b) {
             switch (kind) {
             case HK_SINGLE: return ingest_single(ctx, b, hid, (const double *)d_a, n, s);
-            case HK_KEYED_U16: return launch_keyed<unsigned short, double>(ctx, b, d_i, (const double *)d_a, n, s);
-            case HK_KEYED_I64_U16: return launch_keyed<unsigned short, long long>(ctx, b, d_i, (const long long *)d_a, n, s);
-            default: return add_counters<unsigned short>(ctx, b, d_i, (const uint64_t *)d_a, n, s);   // HK_COUNTER_U16
+            case HK_KEYED_U16: return launch_keyed<unsigned short, double>(ctx, b, d_i, (const double *)d_a, n, s, IdIdentity{});
+            case HK_KEYED_I64_U16: return launch_keyed<unsigned short, long long>(ctx, b, d_i, (const long long *)d_a, n, s, IdIdentity{});
+            default: return add_counters<unsigned short>(ctx, b, ctx->C, d_i, (const uint64_t *)d_a, n, s, IdIdentity{});   // HK_COUNTER_U16
             }
         });
     }
@@ -1610,16 +1614,9 @@ extern "C" lh_status lh_record_begin(lh_ctx *ctx, void *stream, lh_recorder *out
     const int b = ctx->active;
     lh_status st = before_write(ctx, b, s);
     if (st != LH_OK) return st;
-    memset(out, 0, sizeof *out);
-    out->d_buckets = reinterpret_cast<uint64_t *>(ctx->buf[b].d_buckets.get());
-    out->d_flags = ctx->buf[b].d_flags.get();
-    out->d_counters = reinterpret_cast<uint64_t *>(ctx->buf[b].d_counters.get());
-    out->d_dropped = reinterpret_cast<uint64_t *>(ctx->d_dropped.get());
-    out->max_histograms = ctx->H;
-    out->max_counters = ctx->C;
+    *out = buffer_target(ctx, b);
     out->block_smem_bytes = subhist_words(ctx->pc.win) * 4u;
     out->scope = ctx->next_scope++;
-    memcpy(out->prec, &ctx->pc, sizeof ctx->pc);
     ctx->scopes.push_back(Scope{out->scope, b, s, std::this_thread::get_id()});
     return LH_OK;
 }
@@ -1734,10 +1731,8 @@ lh_status graph_keyed(lh_ctx *ctx, const lh_graph_recorder *g, const IdT *d_ids,
                       void *stream) {
     GraphRec *gr = graph_of(ctx, g);
     if (!gr) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign graph recorder");
-    if (kind != LH_VALUES_F64 && kind != LH_VALUES_I64NS) return fail(ctx, LH_ERR_INVALID, "unknown values kind");
-    if (n && (!d_ids || !d_values)) return fail(ctx, LH_ERR_INVALID, "NULL input");
-    if (((uintptr_t)d_values & 7u) || ((uintptr_t)d_ids & (sizeof(IdT) - 1)))
-        return fail(ctx, LH_ERR_INVALID, "ids / values are not naturally aligned");
+    if (lh_status st = check_kind(ctx, kind); st != LH_OK) return st;
+    if (lh_status st = check_pairs(ctx, d_ids, d_values, n); st != LH_OK) return st;
     if (n == 0) return LH_OK;
     return launch_keyed_graph<IdT>(ctx, gr->rec, d_ids, static_cast<const unsigned long long *>(d_values), n,
                                    kind == LH_VALUES_I64NS, pick_stream(ctx, stream));
@@ -1748,12 +1743,10 @@ lh_status graph_counters(lh_ctx *ctx, const lh_graph_recorder *g, const IdT *d_i
                          void *stream) {
     GraphRec *gr = graph_of(ctx, g);
     if (!gr) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign graph recorder");
-    if (n && (!d_ids || !d_amounts)) return fail(ctx, LH_ERR_INVALID, "NULL input");
-    if (((uintptr_t)d_amounts & 7u) || ((uintptr_t)d_ids & (sizeof(IdT) - 1)))
-        return fail(ctx, LH_ERR_INVALID, "ids / amounts are not naturally aligned");
+    if (lh_status st = check_pairs(ctx, d_ids, d_amounts, n); st != LH_OK) return st;
     if (n == 0) return LH_OK;
     return launch_counter<IdT>(ctx, reinterpret_cast<unsigned long long *>(gr->rec.d_counters), gr->rec.max_counters, d_ids,
-                               d_amounts, n, pick_stream(ctx, stream));
+                               d_amounts, n, pick_stream(ctx, stream), IdIdentity{});
 }
 }  // namespace
 

@@ -447,6 +447,9 @@ __device__ __forceinline__ MapRows map_to_smem(const IdMap &m, uint32_t *s) {
     __syncthreads();
     return MapRows{s, m.k, m.any_unbound != 0};
 }
+// the dynamic shared memory map_to_smem needs (host side, for the launch)
+inline size_t map_smem_bytes(const IdIdentity &) { return 0; }
+inline size_t map_smem_bytes(const IdMap &m) { return (size_t)m.k * 4; }
 
 template <typename ValT, typename V = IdIdentity>
 __device__ __forceinline__ void keyed_one(uint32_t id, ValT raw, const Prec &pc, const KeyedOut &o, unsigned int *hot, uint64_t pol,

@@ -635,6 +635,17 @@ def test_tune_and_error_paths(eng, lh):
     with pytest.raises(lh.LhError):
         eng.snapshot_reduce(list(np.linspace(0, 1, 40)))   # more than LH_MAX_PERCENTILES
     assert "histogram_id" in eng.lib.lh_last_error(eng.h).decode() or True
+    # counter adds with amounts or ids not naturally aligned are refused before any launch: nothing runs or counts
+    d_i16, d_i32 = eng.upload(np.zeros(8, np.uint16)), eng.upload(np.zeros(8, np.uint32))
+    d_a = eng.upload(np.ones(8, np.uint64))
+    eng.snapshot(PS)
+    launches = eng.stats()["kernel_launches"]
+    for add, ids, amounts in ((eng.counter_add_u16, d_i16.ptr, d_a.ptr + 4), (eng.counter_add_u32, d_i32.ptr, d_a.ptr + 4),
+                              (eng.counter_add_u32, d_i32.ptr + 2, d_a.ptr)):
+        with pytest.raises(lh.LhError):
+            add(ids, amounts, 4)
+    assert eng.stats()["kernel_launches"] == launches
+    assert not eng.snapshot(PS)[1].counter_deltas.any()
     eng.tune("k1_reserve_sms", 3)
     eng.tune("k1_reserve_sms", 0)
 
