@@ -12,11 +12,11 @@ import numpy as np
 import pytest
 
 import _ingest_routes as R
+from _op_sequences import PS, Want, check, check_reduced
 
 pytestmark = pytest.mark.gpu
 
 SEED = 0x5EA4ED
-PS = [0.0, 0.5, 0.99, 1.0]
 MS = 1_000_000                     # one millisecond of spin, in ns
 SPECIALS = np.array([np.inf, -np.inf, np.nan, 2.0 ** 63, -(2.0 ** 64), 0.0, -0.0, 5e-324, 1e300], np.float64)
 AMOUNTS = np.array([2 ** 32 - 1, 2 ** 32, 2 ** 64 - 1, 1 << 63], np.uint64)   # carry out of either half
@@ -87,72 +87,6 @@ def counter_batch(n, C, seed):
     ids16 = R.with_bad_ids(ids, np.array([65535], np.uint32), 89)
     ids32 = R.with_bad_ids(ids, R.high_ids(min(C, 65536), 5), 89)
     return ids16.astype(np.uint16), ids32, amounts
-
-
-class Want:
-    """What one interval of one context must hold: (id * 65536 + key) counts, counters and dropped samples, with the
-    keys from the oracle's compress at the context's precision."""
-
-    def __init__(self, oracle, H, C=1, precision=100):
-        self.oracle, self.H, self.C, self.precision = oracle, H, C, precision
-        self.parts = []
-        self.counters = np.zeros(C, np.uint64)
-        self.dropped = 0
-
-    def hist(self, ids, vals, times=1):
-        ids = np.asarray(ids).astype(np.int64)
-        keys = self.oracle.compress_many(np.asarray(vals, np.float64), self.precision).view(np.uint16).astype(np.int64)
-        ok = ids < self.H
-        u, c = np.unique(ids[ok] * 65536 + keys[ok], return_counts=True)
-        self.parts.append((u, c.astype(np.uint64) * np.uint64(times)))
-        self.dropped += int((~ok).sum()) * times
-
-    def single(self, hid, vals, times=1):
-        self.hist(np.full(len(vals), hid), vals, times)
-
-    def counter(self, ids, amounts):
-        ids = np.asarray(ids).astype(np.uint32)
-        ok = ids < self.C
-        self.oracle.counter_add(ids[ok], np.asarray(amounts, np.uint64)[ok], self.C, self.counters)
-        self.dropped += int((~ok).sum())
-
-    def sparse(self):
-        if not self.parts:
-            return np.zeros(0, np.int64), np.zeros(0, np.uint64)
-        u, inv = np.unique(np.concatenate([p[0] for p in self.parts]), return_inverse=True)
-        c = np.zeros(u.size, np.uint64)
-        np.add.at(c, inv, np.concatenate([p[1] for p in self.parts]))
-        return u, c
-
-
-def check_reduced(red, want, what):
-    """Counts of every histogram, and the percentile keys and values of the first and last three touched ones."""
-    u, c = want.sparse()
-    totals = np.zeros(want.H, np.uint64)
-    np.add.at(totals, u >> 16, c)
-    assert (red.counts == totals).all(), (what, np.nonzero(red.counts != totals)[0][:5])
-    hs = np.unique(u >> 16)
-    for h in np.unique(np.concatenate([hs[:3], hs[-3:]])):
-        sel = (u >> 16) == h
-        dense = np.zeros(65536, np.uint64)
-        dense[u[sel] & 0xFFFF] = c[sel]
-        ref = want.oracle.process_histogram(dense, PS, want.precision)
-        assert (red.pkeys[h] == ref["pkeys"]).all(), (what, int(h))
-        assert (red.pvals[h].view(np.uint64) == ref["pvals"].view(np.uint64)).all(), (what, int(h))
-
-
-def check(e, want, what, dropped_before=None, snap=None):
-    """The interval (a fresh snapshot, or `snap` = (Reduced, Sparse)) equals `want` bucket for bucket."""
-    red, sp = snap if snap is not None else e.snapshot(PS)
-    u, c = want.sparse()
-    flat = np.repeat(np.arange(want.H, dtype=np.int64), np.diff(sp.offsets.astype(np.int64))) * 65536 + sp.keys.view(np.uint16)
-    order = np.argsort(flat, kind="stable")
-    assert flat.size == u.size and (flat[order] == u).all(), (what, flat.size, u.size)
-    assert (sp.counts[order] == c).all(), (what, np.nonzero(sp.counts[order] != c)[0][:5])
-    check_reduced(red, want, what)
-    assert (sp.counter_deltas == want.counters).all(), (what, np.nonzero(sp.counter_deltas != want.counters)[0][:5])
-    if dropped_before is not None:
-        assert e.stats()["dropped"] - dropped_before == want.dropped, what
 
 
 def timed_since(e, seq0):
