@@ -410,6 +410,20 @@ int grid_1d(lh_ctx *ctx, size_t n, int threads, int per_thread, int blocks_per_s
     return (int)std::max<size_t>(1, std::min(need, cap));
 }
 
+// The SMs the ingest kernels may spread over: all but the k1_reserve_sms left to concurrent snapshot / collective work.
+int ingest_sms(const lh_ctx *ctx) { return std::max(1, ctx->sm_count - ctx->k1_reserve_sms); }
+// Samples one launch of `grid` CTAs may take when each CTA counts into uint32 cells of its own (K1's sub-histograms, the
+// tables of k_ingest_batch / k_ingest_keyed_graph): work is dealt round-robin, so 2^31 per CTA keeps every cell < 2^32.
+size_t launch_cap(int grid) { return std::min((size_t)1 << 36, (size_t)grid << 31); }
+// The vector body of n 8-byte samples at `vals`: `head` scalar samples (at most 3) up to the first 32-byte aligned value,
+// then n4 groups of 4; ids_ok: the ids (id_bytes each; 0: none) are aligned to 4 ids there.  Each caller decides what a
+// misaligned or short piece takes instead.
+struct VecSplit { size_t head, n4; bool ids_ok; };
+VecSplit vec_split(const void *vals, size_t n, const void *ids = nullptr, size_t id_bytes = 0) {
+    const size_t head = std::min<size_t>(n, ((32u - ((uintptr_t)vals & 31u)) & 31u) / 8u);
+    return {head, (n - head) / 4, !id_bytes || (((uintptr_t)ids + head * id_bytes) & (4 * id_bytes - 1)) == 0};
+}
+
 // The write protocol of every timed ingest (locked): order `s` after the zeroing of the active buffer, bracket
 // body(b) with the CUDA events of one sequence number, then register `s` as a writer of b, which is what
 // lh_snapshot_begin orders the snapshot after.  The body only issues kernels into buffer b and counts them in stats;
@@ -446,23 +460,16 @@ lh_recorder buffer_target(lh_ctx *ctx, int b) {
 // K1 into one row (counts, flag); the caller counts the samples in stats
 lh_status launch_single(lh_ctx *ctx, unsigned long long *counts, uint32_t *flag, const double *d_values, size_t n, cudaStream_t s) {
     const K1Variant &kv = ctx->k1[ctx->k1_variant];
-    // a CTA's uint32 sub-histogram must not overflow: tiles are dealt round-robin, so bounding a launch to
-    // 2^31 samples per CTA keeps every cell below 2^32 whatever the grid size (reserved SMs shrink it)
-    const int grid = std::max(1, ctx->sm_count - ctx->k1_reserve_sms) * kv.blocks_per_sm * ctx->k1_grid_mult;
-    const size_t kMaxPerLaunch = std::min((size_t)1 << 36, (size_t)grid << 31);
+    const int grid = ingest_sms(ctx) * kv.blocks_per_sm * ctx->k1_grid_mult;
+    const size_t cap = launch_cap(grid);
     size_t done = 0;
     while (done < n) {
-        size_t m = std::min(n - done, kMaxPerLaunch);
+        size_t m = std::min(n - done, cap);
         const double *p = d_values + done;
-        // peel up to 3 samples so the body is 32-byte aligned (4-sample load groups, 16-byte bulk copies)
-        int nhead = (int)(((32u - ((uintptr_t)p & 31u)) & 31u) / 8u);
-        if ((size_t)nhead > m) nhead = (int)m;
-        const double *head = p;
-        const double *body = p + nhead;
-        size_t nvec = (m - nhead) >> 2;
-        const double *tail = body + nvec * 4;
-        int ntail = (int)(m - nhead - nvec * 4);
-        kv.launch(grid, kv.smem, s, body, nvec, head, nhead, tail, ntail, counts, flag, ctx->pc);
+        const VecSplit v = vec_split(p, m);
+        const double *body = p + v.head;
+        const double *tail = body + v.n4 * 4;
+        kv.launch(grid, kv.smem, s, body, v.n4, p, (int)v.head, tail, (int)(m - v.head - v.n4 * 4), counts, flag, ctx->pc);
         LH_CUDA(ctx, cudaGetLastError());
         ctx->stats.kernel_launches++;
         done += m;
@@ -557,18 +564,16 @@ KeyedPlan plan_keyed(const lh_ctx *ctx, uint32_t nids, size_t id_bytes, const vo
     const uint32_t ks_per_max = std::max<uint32_t>(1, (uint32_t)(KS_SMEM_BYTES / ((size_t)ctx->pc.win * 4)));
     const uint32_t ks_passes = (nids + ks_per_max - 1) / ks_per_max;
     const bool small = ks_passes <= KS_MAX_PASSES && ctx->keyed_mode == 0;
-    const uintptr_t id_mask = 4 * id_bytes - 1;
     if (pair) {
         // few histograms: the shared-memory privatised kernel of launch_keyed is the better one, per array
-        auto aligned = [&](const void *v, const void *i) { return ((uintptr_t)v & 31u) == 0 && ((uintptr_t)i & id_mask) == 0; };
+        auto aligned = [&](const void *v, const void *i) { return ((uintptr_t)v & 31u) == 0 && ((uintptr_t)i & (4 * id_bytes - 1)) == 0; };
         p.route = KeyedPlan::APART;
         if (!n || !n2 || ctx->keyed_mode == 1 || small || !aligned(vals, ids) || !aligned(vals2, ids2)) return p;
         if (n + n2 > kWcMaxLaunch) return p;   // apart, each array split by launch_keyed
     } else {
-        // scalar head until the values are 32-byte aligned; the vector body also needs ids aligned to 4 ids
-        p.head = std::min<size_t>(n, ((32u - ((uintptr_t)vals & 31u)) & 31u) / 8u);
-        if (((uintptr_t)ids + p.head * id_bytes) & id_mask) { p.head = 0; return p; }   // misaligned: the scalar kernel only
-        p.n4 = (n - p.head) / 4;
+        const VecSplit v = vec_split(vals, n, ids, id_bytes);
+        if (!v.ids_ok) return p;                                                          // misaligned: the scalar kernel only
+        p.head = v.head; p.n4 = v.n4;
         if (!p.n4) return p;                                                              // short: the scalar kernel only
         n = p.taken = p.n4 * 4;                                  // the vector body, all the write-combining kernel is offered
         if (small && p.n4 >= 4096) {
@@ -576,15 +581,14 @@ KeyedPlan plan_keyed(const lh_ctx *ctx, uint32_t nids, size_t id_bytes, const vo
             p.per = (nids + ks_passes - 1) / ks_passes;
             p.smem = ((size_t)p.per * ctx->pc.win + 4) * 4;
             // one CTA per SM; fewer when the batch is small, so that the per-CTA flush stays negligible
-            p.grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)(ctx->sm_count - ctx->k1_reserve_sms),
-                                                               p.n4 / (KS_THREADS * 16)));
+            p.grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)ingest_sms(ctx), p.n4 / (KS_THREADS * 16)));
             return p;
         }
         p.route = KeyedPlan::VEC; p.name = "k_ingest_keyed_vec";
         if (ctx->keyed_mode == 1) return p;
     }
     // the write-combining kernel, or keep the route above when it declines
-    const int P = std::min(ctx->sm_count - ctx->k1_reserve_sms, (int)WC_MAX_PARTS);
+    const int P = std::min(ingest_sms(ctx), (int)WC_MAX_PARTS);
     if (P < 8) return p;
     const uint32_t ids_per = (nids + P - 1) / P;
     const size_t hist_bytes = (((size_t)ids_per * ctx->pc.win + 3) & ~(size_t)3) * 4;
@@ -789,10 +793,9 @@ lh_status launch_counter(lh_ctx *ctx, unsigned long long *counters, uint32_t C, 
         if (kMapped<Map> || C <= (uint32_t)K2_SMEM_COUNTERS) {
             // privatised per CTA (lo/hi halves in shared memory).  Vector body where the alignment allows: 4 ops per
             // thread and iteration; ragged head / tail through the scalar form of the same kernel.
-            size_t head = std::min<size_t>(n, ((32u - ((uintptr_t)amts & 31u)) & 31u) / 8u);
-            const bool vec_ok = (((uintptr_t)(d_ids + head)) & (4 * sizeof(IdT) - 1)) == 0 && (((uintptr_t)amts & 7u) == 0);
-            size_t n4 = vec_ok ? (n - head) / 4 : 0;
-            if (n4 < 4096) { head = 0; n4 = 0; }
+            const VecSplit v = vec_split(amts, n, d_ids, sizeof(IdT));
+            size_t head = v.head, n4 = v.n4;
+            if (!v.ids_ok || ((uintptr_t)amts & 7u) != 0 || n4 < 4096) { head = 0; n4 = 0; }
             const size_t tail_off = head + n4 * 4;
             const size_t smem = (size_t)C * 8 + map_smem_bytes(map);
             auto scalar = [&](int grid, size_t off, size_t cnt) {
@@ -802,7 +805,7 @@ lh_status launch_counter(lh_ctx *ctx, unsigned long long *counters, uint32_t C, 
             if (head) scalar(1, 0, head);
             if (n4) {
                 // one CTA per SM (the per-CTA flush is C global atomics), fewer for small batches
-                const int grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)std::max(1, ctx->sm_count - ctx->k1_reserve_sms) * 2, n4 / (T * 4)));
+                const int grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)ingest_sms(ctx) * 2, n4 / (T * 4)));
                 k_counter_add_smem_vec<IdT, T, Map><<<grid, T, smem, s>>>(d_ids + head, amts + head, n4, counters, C, ctx->d_dropped.get(), map);
                 ctx->stats.kernel_launches++;
             }
@@ -833,17 +836,14 @@ constexpr size_t kBatchK1Min = 1024 * 1024;
 // ones through launch_single, the rest through as few launches of k_ingest_batch as the parameter block and the uint32
 // table counts allow.  An item that does not fit the launch being filled is split across launches.  Kernels only (the
 // graph recorder's form is captured); the caller counts the samples in stats.
-// The grid of k_ingest_batch (and of k_ingest_keyed_graph, which has its launch bounds and table), and the samples one
-// launch of it may take: pieces are dealt round-robin, so at most 2^31 samples per CTA of the full grid keeps every
-// table count below 2^32.
-int batch_grid_max(const lh_ctx *ctx) { return std::max(1, ctx->sm_count - ctx->k1_reserve_sms) * ctx->batch_blocks_per_sm; }
-unsigned long long batch_cap(int grid_max) { return std::min<unsigned long long>(1ull << 36, (unsigned long long)grid_max << 31); }
+// The grid of k_ingest_batch (and of k_ingest_keyed_graph, which has its launch bounds and table).
+int batch_grid_max(const lh_ctx *ctx) { return ingest_sms(ctx) * ctx->batch_blocks_per_sm; }
 
 lh_status launch_batch(lh_ctx *ctx, const lh_recorder &target, const lh_batch_item *items, uint32_t n_items, cudaStream_t s) {
     BatchParams &prm = ctx->batch_prm;
     prm.rec = target;
     const int grid_max = batch_grid_max(ctx);
-    const unsigned long long cap = batch_cap(grid_max);
+    const unsigned long long cap = launch_cap(grid_max);
     uint32_t k = 0;
     unsigned long long total = 0;
     auto launch = [&]() -> lh_status {
@@ -895,15 +895,13 @@ template <typename IdT>
 lh_status launch_keyed_graph(lh_ctx *ctx, const lh_recorder &target, const IdT *ids, const unsigned long long *vals, size_t n,
                              bool ns, cudaStream_t s) {
     const int grid_max = batch_grid_max(ctx);
-    const size_t cap = (size_t)batch_cap(grid_max);
+    const size_t cap = launch_cap(grid_max);
     for (size_t done = 0; done < n;) {
         const size_t m = std::min(n - done, cap);
         const IdT *ip = ids + done;
         const unsigned long long *vp = vals + done;
-        size_t head = std::min<size_t>(m, ((32u - ((uintptr_t)vp & 31u)) & 31u) / 8u);
-        const bool vec_ok = ((uintptr_t)(ip + head) & (4 * sizeof(IdT) - 1)) == 0;
-        const size_t n4 = vec_ok ? (m - head) / 4 : 0;
-        if (!vec_ok) head = m;
+        const VecSplit v = vec_split(vp, m, ip, sizeof(IdT));
+        const size_t head = v.ids_ok ? v.head : m, n4 = v.ids_ok ? v.n4 : 0;   // misaligned ids: one sample per thread
         const int grid = (int)std::min<size_t>((size_t)grid_max, (m + BI_PIECE - 1) / BI_PIECE);
         k_ingest_keyed_graph<IdT><<<grid, BI_THREADS, BlockRecorder::smem_bytes(BI_TABLE_ENTRIES), s>>>(target, ip, vp, head, n4, m, ns);
         LH_CUDA(ctx, cudaGetLastError());

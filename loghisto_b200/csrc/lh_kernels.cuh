@@ -487,28 +487,14 @@ __device__ __noinline__ void keyed_one_slow(uint32_t id, unsigned long long raw,
     keyed_one_direct<ValT>(id, r, pc, o);
 }
 // Mapped: the row is resolved here, so that the map (in the parameter block) is only read inline.
-template <typename ValT>
-__device__ __forceinline__ void keyed_one_slow_v(uint32_t id, unsigned long long raw, const Prec &pc, const KeyedOut &o, IdIdentity) {
-    keyed_one_slow<ValT>(id, raw, pc, o);
-}
-template <typename ValT>
-__device__ __forceinline__ void keyed_one_slow_v(uint32_t id, unsigned long long raw, const Prec &pc, const KeyedOut &o, const MapRows &m) {
-    if (!m.lookup(id, o.H, id)) { atomicAdd(o.dropped, 1ull); return; }
+template <typename ValT, typename V>
+__device__ __forceinline__ void keyed_one_slow_v(uint32_t id, unsigned long long raw, const Prec &pc, const KeyedOut &o, const V &m) {
+    if constexpr (kMapped<V>) {
+        if (!m.lookup(id, o.H, id)) { atomicAdd(o.dropped, 1ull); return; }
+    }
     keyed_one_slow<ValT>(id, raw, pc, o);
 }
 
-template <typename IdT>
-__device__ __forceinline__ void load_ids4(const IdT *ids, size_t g, uint32_t (&id4)[4]) {
-    if (sizeof(IdT) == 2) {
-        unsigned int lo, hi;
-        asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0, %1}, [%2];" : "=r"(lo), "=r"(hi)
-                     : "l"(reinterpret_cast<const char *>(ids) + g * 8));
-        id4[0] = lo & 0xFFFFu; id4[1] = lo >> 16; id4[2] = hi & 0xFFFFu; id4[3] = hi >> 16;
-    } else {
-        asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(id4[0]), "=r"(id4[1]), "=r"(id4[2]), "=r"(id4[3])
-                     : "l"(reinterpret_cast<const char *>(ids) + g * 16));
-    }
-}
 __device__ __forceinline__ void load_vals4(const void *vals, size_t g, unsigned long long (&raw)[4]) {
     ldg_stream_u64x4(reinterpret_cast<const char *>(vals) + g * 32, raw);
 }
@@ -549,14 +535,14 @@ k_ingest_keyed_vec(const IdT *__restrict__ ids, const ValT *__restrict__ vals, s
     const size_t stride = (size_t)gridDim.x * THREADS;
     for (size_t g = (size_t)blockIdx.x * THREADS + threadIdx.x; g < n4; g += stride) {
         unsigned long long raw[4];
-        uint32_t id4[4];
+        IdPack<IdT> idp;
         load_vals4(vals, g, raw);
-        load_ids4<IdT>(ids, g, id4);
+        idp.load(ids, g);
 #pragma unroll
         for (int j = 0; j < 4; j++) {
             ValT r;
             memcpy(&r, &raw[j], 8);
-            keyed_one<ValT>(id4[j], r, pc, o, hot, pol, mv);
+            keyed_one<ValT>(idp.get(j), r, pc, o, hot, pol, mv);
         }
     }
 }
@@ -607,12 +593,12 @@ k_ingest_keyed_small(const IdT *__restrict__ ids, const ValT *__restrict__ vals,
     const size_t stride = (size_t)gridDim.x * KS_THREADS;
     size_t base = (size_t)blockIdx.x * KS_THREADS;
     unsigned long long cur[4] = {0, 0, 0, 0}, nxt[4] = {0, 0, 0, 0};
-    uint32_t cur_id[4] = {0, 0, 0, 0}, nxt_id[4] = {0, 0, 0, 0};
-    if (base + threadIdx.x < n4) { load_vals4(vals, base + threadIdx.x, cur); load_ids4<IdT>(ids, base + threadIdx.x, cur_id); }
+    IdPack<IdT> cur_id{}, nxt_id{};
+    if (base + threadIdx.x < n4) { load_vals4(vals, base + threadIdx.x, cur); cur_id.load(ids, base + threadIdx.x); }
     for (; base < n4; base += stride) {
         const bool valid = base + threadIdx.x < n4;
         const size_t gn = base + stride + threadIdx.x;
-        if (gn < n4) { load_vals4(vals, gn, nxt); load_ids4<IdT>(ids, gn, nxt_id); }
+        if (gn < n4) { load_vals4(vals, gn, nxt); nxt_id.load(ids, gn); }
         double v[4];
 #pragma unroll
         for (int i = 0; i < 4; i++) { ValT r; memcpy(&r, &cur[i], 8); v[i] = sample_to_f64<ValT>(r); }
@@ -622,9 +608,9 @@ k_ingest_keyed_small(const IdT *__restrict__ ids, const ValT *__restrict__ vals,
         bool any = false;
 #pragma unroll
         for (int i = 0; i < 4; i++) {
-            const uint32_t l = cur_id[i] - id_lo;                                  // local id (wraps when below id_lo)
+            const uint32_t l = cur_id.get(i) - id_lo;                              // local id (wraps when below id_lo)
             const bool mine = valid & (l < id_cnt);
-            const bool bad = valid & (cur_id[i] >= mv.bound(o.H)) & (id_lo == 0);
+            const bool bad = valid & (cur_id.get(i) >= mv.bound(o.H)) & (id_lo == 0);
             flag[i] = (mine & flag[i]) | bad;
             off[i] = mine ? off[i] + l * (row * 4u) : trash_off;
             any |= flag[i];
@@ -637,14 +623,15 @@ k_ingest_keyed_small(const IdT *__restrict__ ids, const ValT *__restrict__ vals,
                 memcpy(&rv, &cur[i], 8);
                 // uncertain samples of a valid id could stay in shared memory; the L2 route is exact too
                 // and keeps this path trivial (it handles ~0.05 % of the samples)
-                keyed_one<ValT>(cur_id[i], rv, pc, o, o.hot, pol, mv);
+                keyed_one<ValT>(cur_id.get(i), rv, pc, o, o.hot, pol, mv);
                 off[i] = trash_off;
             }
         }
 #pragma unroll
         for (int i = 0; i < 4; i++) atomicAdd(reinterpret_cast<uint32_t *>(reinterpret_cast<char *>(ks_hist) + off[i]), 1u);
 #pragma unroll
-        for (int i = 0; i < 4; i++) { cur[i] = nxt[i]; cur_id[i] = nxt_id[i]; }
+        for (int i = 0; i < 4; i++) cur[i] = nxt[i];
+        cur_id = nxt_id;
     }
     __syncthreads();
     for (uint32_t i = threadIdx.x; i < words; i += KS_THREADS) {
@@ -1055,31 +1042,43 @@ constexpr int K2_SMEM_COUNTERS = 8192;
 
 // Mapped (k_counter_add_smem{,_vec}): C is the number of local ids; the map follows the 2C halves in shared memory, an
 // op is dropped per op when its local id is >= C or unbound, and the flush adds counter i into its row.
+// The steps both kernels share: s_cnt is [C] low halves, [C] high halves, then the map.
+template <int THREADS, typename Map>
+__device__ __forceinline__ auto counter_smem_init(unsigned int *s_cnt, uint32_t C, const Map &map) {
+    for (uint32_t i = threadIdx.x; i < 2 * C; i += THREADS) s_cnt[i] = 0;
+    const auto mv = map_to_smem(map, s_cnt + 2 * C);
+    __syncthreads();
+    return mv;
+}
+template <typename MV>
+__device__ __forceinline__ void counter_smem_add(unsigned int *s_cnt, uint32_t C, uint32_t id, unsigned long long amt,
+                                                 unsigned long long *dropped, const MV &mv) {
+    if (mv.drops(id, C)) { atomicAdd(dropped, 1ull); return; }
+    unsigned int a_lo = (unsigned int)amt, a_hi = (unsigned int)(amt >> 32);
+    unsigned int old = atomicAdd(&s_cnt[id], a_lo);
+    a_hi += (old + a_lo < old) ? 1u : 0u;        // carry out of the low half
+    if (a_hi) atomicAdd(&s_cnt[C + id], a_hi);
+}
+template <int THREADS, typename MV>
+__device__ __forceinline__ void counter_smem_flush(const unsigned int *s_cnt, uint32_t C, unsigned long long *counters, const MV &mv) {
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < C; i += THREADS) {
+        unsigned long long v = ((unsigned long long)s_cnt[C + i] << 32) | s_cnt[i];
+        if (v) atomicAdd(&counters[mv.row(i)], v);            // v == 0 for an unbound row: its ops were dropped
+    }
+}
+
 template <typename IdT, int THREADS, typename Map = IdIdentity>
 __global__ void __launch_bounds__(THREADS)
 k_counter_add_smem(const IdT *__restrict__ ids, const unsigned long long *__restrict__ amounts, size_t n,
                    unsigned long long *__restrict__ counters, uint32_t C,
                    unsigned long long *__restrict__ dropped, const Map map) {
-    extern __shared__ unsigned int s_cnt[];          // [C] low halves, [C] high halves
-    unsigned int *lo = s_cnt, *hi = s_cnt + C;
-    for (uint32_t i = threadIdx.x; i < 2 * C; i += THREADS) s_cnt[i] = 0;
-    const auto mv = map_to_smem(map, s_cnt + 2 * C);
-    __syncthreads();
+    extern __shared__ unsigned int s_cnt[];
+    const auto mv = counter_smem_init<THREADS>(s_cnt, C, map);
     const size_t stride = (size_t)gridDim.x * THREADS;
-    for (size_t i = (size_t)blockIdx.x * THREADS + threadIdx.x; i < n; i += stride) {
-        uint32_t id = (uint32_t)ids[i];
-        unsigned long long amt = amounts[i];
-        if (mv.drops(id, C)) { atomicAdd(dropped, 1ull); continue; }
-        unsigned int a_lo = (unsigned int)amt, a_hi = (unsigned int)(amt >> 32);
-        unsigned int old = atomicAdd(&lo[id], a_lo);
-        a_hi += (old + a_lo < old) ? 1u : 0u;        // carry out of the low half
-        if (a_hi) atomicAdd(&hi[id], a_hi);
-    }
-    __syncthreads();
-    for (uint32_t i = threadIdx.x; i < C; i += THREADS) {
-        unsigned long long v = ((unsigned long long)hi[i] << 32) | lo[i];
-        if (v) atomicAdd(&counters[mv.row(i)], v);            // v == 0 for an unbound row: its ops were dropped
-    }
+    for (size_t i = (size_t)blockIdx.x * THREADS + threadIdx.x; i < n; i += stride)
+        counter_smem_add(s_cnt, C, (uint32_t)ids[i], amounts[i], dropped, mv);
+    counter_smem_flush<THREADS>(s_cnt, C, counters, mv);
 }
 
 // Vector body: 4 consecutive (id, amount) pairs per thread and iteration (two 128-bit amount loads, one 64/128-bit id
@@ -1089,11 +1088,8 @@ __global__ void __launch_bounds__(THREADS)
 k_counter_add_smem_vec(const IdT *__restrict__ ids, const unsigned long long *__restrict__ amounts, size_t n4,
                        unsigned long long *__restrict__ counters, uint32_t C, unsigned long long *__restrict__ dropped,
                        const Map map) {
-    extern __shared__ unsigned int s_cnt[];          // [C] low halves, [C] high halves
-    unsigned int *lo = s_cnt, *hi = s_cnt + C;
-    for (uint32_t i = threadIdx.x; i < 2 * C; i += THREADS) s_cnt[i] = 0;
-    const auto mv = map_to_smem(map, s_cnt + 2 * C);
-    __syncthreads();
+    extern __shared__ unsigned int s_cnt[];
+    const auto mv = counter_smem_init<THREADS>(s_cnt, C, map);
     const size_t stride = (size_t)gridDim.x * THREADS;
     size_t g = (size_t)blockIdx.x * THREADS + threadIdx.x;
     unsigned long long cur[4], nxt[4];
@@ -1103,25 +1099,12 @@ k_counter_add_smem_vec(const IdT *__restrict__ ids, const unsigned long long *__
         const size_t gn = g + stride;
         if (gn < n4) { load_vals4(amounts, gn, nxt); nid.load(ids, gn); }
 #pragma unroll
-        for (int j = 0; j < 4; j++) {
-            const uint32_t id = cid.get(j);
-            const unsigned long long amt = cur[j];
-            if (mv.drops(id, C)) { atomicAdd(dropped, 1ull); continue; }
-            const unsigned int a_lo = (unsigned int)amt;
-            unsigned int a_hi = (unsigned int)(amt >> 32);
-            const unsigned int old = atomicAdd(&lo[id], a_lo);
-            a_hi += (old + a_lo < old) ? 1u : 0u;        // carry out of the low half
-            if (a_hi) atomicAdd(&hi[id], a_hi);
-        }
+        for (int j = 0; j < 4; j++) counter_smem_add(s_cnt, C, cid.get(j), cur[j], dropped, mv);
 #pragma unroll
         for (int j = 0; j < 4; j++) cur[j] = nxt[j];
         cid = nid;
     }
-    __syncthreads();
-    for (uint32_t i = threadIdx.x; i < C; i += THREADS) {
-        unsigned long long v = ((unsigned long long)hi[i] << 32) | lo[i];
-        if (v) atomicAdd(&counters[mv.row(i)], v);            // v == 0 for an unbound row: its ops were dropped
-    }
+    counter_smem_flush<THREADS>(s_cnt, C, counters, mv);
 }
 
 template <typename IdT, int THREADS>
