@@ -729,6 +729,39 @@ LH_API lh_status lh_snapshot_allreduce_rows(lh_ctx *ctx, uint64_t seq, const uin
                                             const uint32_t *hist_map, uint32_t n_counter_rows,
                                             const uint32_t *counter_map, uint64_t *seq_out);
 
+/* ---- multi-GPU by rows through the caller's all-reduce ---------------------------------------------------------------
+ * The peer all-reduce needs CUDA IPC mappings, which exist only between processes of one host.  Ranks on different
+ * hosts agree on job-wide rows as above and then sum a payload through a transport the caller owns (gloo, NCCL, MPI):
+ *
+ *   lh_snapshot_row_levels  between lh_snapshot_begin and any all-reduce: levels[h] (uint8[max_histograms]) = the level
+ *                     of frozen row h: 0 no data, 1 every count inside the fast window, 3 some count beyond it.
+ *   lh_snapshot_pack_rows  between lh_snapshot_begin and any all-reduce, once per snapshot: gathers job-wide row g from
+ *                     this rank's frozen row hist_rows[g] (zeros for LH_ROW_ABSENT) at the agreed levels[g], then
+ *                     counter g from frozen counter counter_rows[g], into a payload of *n_words uint64: rows g = 0 ..
+ *                     n_rows-1 in order (level 0: nothing; 1: the 2*win-1 cells [0, win) then [65536-(win-1), 65536);
+ *                     3: all 65536 cells), then the n_counter_rows counters.  Every rank that passes the same n_rows,
+ *                     levels and n_counter_rows gets the same layout.  *d_send holds the payload and *d_recv is as
+ *                     large; both are owned by the context, grow on demand and stay valid until the next pack or
+ *                     lh_destroy.  The pack is enqueued on the snapshot stream, returned in *stream: the caller's
+ *                     all-reduce (d_recv = the element-wise wrapping uint64 sum of every rank's d_send) goes on it, or
+ *                     completes before lh_snapshot_unpack_rows.  Needs no lh_comm_import.
+ *   lh_snapshot_unpack_rows  after a pack in the same snapshot: summed = 1 writes d_recv (the job-wide sums), 0 writes
+ *                     d_send (this rank's own counts, e.g. after a failed transport) into the reduced arrays: row g
+ *                     at index g with flag levels[g], counters 0 .. n_counter_rows-1, nothing above.  Afterwards the
+ *                     snapshot's reduce, export, publish and lh_snapshot_copy_histogram read them, as after
+ *                     lh_snapshot_allreduce_rows.  A snapshot that ends after a pack without an unpack read its own
+ *                     frozen arrays throughout.
+ * Errors, before anything is launched: LH_ERR_STATE without a snapshot, after an all-reduce or unpack, for a second
+ * pack, or for an unpack without a pack; LH_ERR_INVALID for n_rows > max_histograms, n_counter_rows > max_counters, a
+ * NULL map or NULL levels with rows, a level other than 0 / 1 / 3, or a NULL output pointer; LH_ERR_RANGE for a map
+ * entry neither LH_ROW_ABSENT nor below max_histograms (max_counters).
+ */
+LH_API lh_status lh_snapshot_row_levels(lh_ctx *ctx, uint8_t *levels);
+LH_API lh_status lh_snapshot_pack_rows(lh_ctx *ctx, uint32_t n_rows, const uint32_t *hist_rows, const uint8_t *levels,
+                                       uint32_t n_counter_rows, const uint32_t *counter_rows, uint64_t **d_send,
+                                       uint64_t **d_recv, uint64_t *n_words, void **stream);
+LH_API lh_status lh_snapshot_unpack_rows(lh_ctx *ctx, uint32_t summed);
+
 /* ---- scalar helpers, evaluated ON THE DEVICE (parity probes for tests) --- */
 /* out[i] = compress(values[i]) exactly as the ingest kernels compute it
  * (mode 0: production fast path + exact fallback; mode 1: exact path only) */

@@ -236,6 +236,10 @@ SIGNATURES = {
     "lh_comm_info": (_i32, [_vp, C.POINTER(lh_comm_stats)]),
     "lh_snapshot_rows": (_i32, [_vp, _vp, _vp, C.POINTER(_u32)]),
     "lh_snapshot_allreduce_rows": (_i32, [_vp, _u64, _vp, _u32, _vp, _u32, _vp, C.POINTER(_u64)]),
+    "lh_snapshot_row_levels": (_i32, [_vp, _vp]),
+    "lh_snapshot_pack_rows": (_i32, [_vp, _u32, _vp, _vp, _u32, _vp, C.POINTER(_vp), C.POINTER(_vp), C.POINTER(_u64),
+                                     C.POINTER(_vp)]),
+    "lh_snapshot_unpack_rows": (_i32, [_vp, _u32]),
     "lh_keyed_kernel_name": (C.c_char_p, [_vp]),
     "lh_compress_f64": (_i32, [_vp, _vp, _sz, _vp, C.c_int, _vp]),
     "lh_decompress_table": (_i32, [_vp, _vp]),

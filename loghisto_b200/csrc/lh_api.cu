@@ -296,6 +296,17 @@ struct lh_ctx {
     // lh_snapshot_rows: pinned staging of the frozen flags and counters (allocated on first use)
     PinnedPtr<uint32_t> h_rows_flags;
     PinnedPtr<unsigned long long> h_rows_counters;
+    // lh_snapshot_pack_rows / lh_snapshot_unpack_rows: the row table ([H] RowsEntry, then [C] counter rows) with its
+    // pinned staging and an event behind the last upload (allocated on first use); the send and recv payloads (grown
+    // on demand, rows_cap words each); the open snapshot's pack
+    DevPtr<unsigned char> d_rows_table;
+    PinnedPtr<unsigned char> h_rows_table;
+    Event rows_table_copied;
+    DevPtr<unsigned long long> d_rows_send, d_rows_recv;
+    size_t rows_cap = 0;
+    bool rows_packed = false;
+    uint32_t rows_n = 0, rows_nc = 0;
+    uint64_t rows_words = 0;
     uint64_t ctx_id = 0;
     // lh_reduce_sparse_host: its own stream (rs_stream) and K6_BATCH scratch rows (allocated on first use), serialised
     // by rs_mu; none of the arrays above is touched by it
@@ -1066,6 +1077,16 @@ lh_status comm_alloc_row_maps(lh_ctx *ctx) {
     LH_CUDA(ctx, cudaMallocHost(h.out(), bytes));
     LH_CUDA(ctx, cudaEventCreateWithFlags(copied.out(), cudaEventDisableTiming));
     ctx->d_row_maps = std::move(d); ctx->h_row_maps = std::move(h); ctx->row_maps_copied = std::move(copied);
+    return LH_OK;
+}
+
+// pinned staging of lh_snapshot_rows and lh_snapshot_row_levels
+lh_status alloc_rows_staging(lh_ctx *ctx) {
+    if (ctx->h_rows_flags.get()) return LH_OK;
+    PinnedPtr<uint32_t> flags; PinnedPtr<unsigned long long> counters;
+    LH_CUDA(ctx, cudaMallocHost(flags.out(), (size_t)ctx->H * 4));
+    LH_CUDA(ctx, cudaMallocHost(counters.out(), (size_t)ctx->C * 8));
+    ctx->h_rows_flags = std::move(flags); ctx->h_rows_counters = std::move(counters);
     return LH_OK;
 }
 
@@ -1986,6 +2007,7 @@ extern "C" lh_status lh_snapshot_begin(lh_ctx *ctx) {
     ctx->nnz_valid = false;
     ctx->view_reduced = false;
     ctx->view_counters_reduced = false;
+    ctx->rows_packed = false;
     ctx->stats.snapshots++;
     return LH_OK;
 }
@@ -2198,6 +2220,7 @@ extern "C" lh_status lh_snapshot_end(lh_ctx *ctx) {
     ctx->pub_slot = -1;
     ctx->view_reduced = false;
     ctx->view_counters_reduced = false;
+    ctx->rows_packed = false;
     return LH_OK;
 }
 
@@ -2848,12 +2871,7 @@ extern "C" lh_status lh_snapshot_rows(lh_ctx *ctx, uint8_t *hist_touched, uint64
     if (ctx->view_reduced) return fail(ctx, LH_ERR_STATE, "this snapshot has already been all-reduced");
     const int f = ctx->active ^ 1;
     cudaStream_t s = ctx->snap_stream.get();
-    if (!ctx->h_rows_flags.get()) {
-        PinnedPtr<uint32_t> flags; PinnedPtr<unsigned long long> counters;
-        LH_CUDA(ctx, cudaMallocHost(flags.out(), (size_t)ctx->H * 4));
-        LH_CUDA(ctx, cudaMallocHost(counters.out(), (size_t)ctx->C * 8));
-        ctx->h_rows_flags = std::move(flags); ctx->h_rows_counters = std::move(counters);
-    }
+    if (lh_status st = alloc_rows_staging(ctx)) return st;
     // behind the writer events, the graph drain and the hot-window fold lh_snapshot_begin ordered on this stream
     if (hist_touched) LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_rows_flags.get(), ctx->buf[f].d_flags.get(), (size_t)ctx->H * 4, cudaMemcpyDeviceToHost, s));
     if (counter_deltas) LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_rows_counters.get(), ctx->buf[f].d_counters.get(), (size_t)ctx->C * 8, cudaMemcpyDeviceToHost, s));
@@ -2903,6 +2921,123 @@ extern "C" lh_status lh_snapshot_allreduce_rows(lh_ctx *ctx, uint64_t seq, const
     m.n_rows = n_rows; m.n_counter_rows = n_counter_rows;
     for (uint32_t r = 0; r < W; r++) m.frozen_mask |= frozen[r] << r;
     return launch_allreduce(ctx, seq, frozen, n_rows, 1u, m, seq_out);
+}
+
+// =========================================================== multi-GPU (caller's all-reduce)
+extern "C" lh_status lh_snapshot_row_levels(lh_ctx *ctx, uint8_t *levels) {
+    LH_ENTER(ctx);
+    if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
+    if (ctx->view_reduced) return fail(ctx, LH_ERR_STATE, "this snapshot has already been all-reduced");
+    if (!levels) return fail(ctx, LH_ERR_INVALID, "levels is NULL");
+    if (lh_status st = alloc_rows_staging(ctx)) return st;
+    cudaStream_t s = ctx->snap_stream.get();
+    LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_rows_flags.get(), ctx->buf[ctx->active ^ 1].d_flags.get(), (size_t)ctx->H * 4, cudaMemcpyDeviceToHost, s));
+    LH_CUDA(ctx, cudaStreamSynchronize(s));
+    for (uint32_t h = 0; h < ctx->H; h++) {
+        const uint32_t fl = ctx->h_rows_flags.get()[h];
+        levels[h] = fl == 0 ? 0 : (fl & 2u) ? 3 : 1;
+    }
+    ctx->stats.d2h_bytes += (size_t)ctx->H * 4;
+    return LH_OK;
+}
+
+extern "C" lh_status lh_snapshot_pack_rows(lh_ctx *ctx, uint32_t n_rows, const uint32_t *hist_rows, const uint8_t *levels,
+                                           uint32_t n_counter_rows, const uint32_t *counter_rows, uint64_t **d_send,
+                                           uint64_t **d_recv, uint64_t *n_words, void **stream) {
+    LH_ENTER(ctx);
+    if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
+    if (ctx->view_reduced) return fail(ctx, LH_ERR_STATE, "this snapshot has already been all-reduced");
+    if (ctx->rows_packed) return fail(ctx, LH_ERR_STATE, "this snapshot has already been packed");
+    if (n_rows > ctx->H) return fail(ctx, LH_ERR_INVALID, "n_rows > max_histograms");
+    if (n_counter_rows > ctx->C) return fail(ctx, LH_ERR_INVALID, "n_counter_rows > max_counters");
+    if ((n_rows && (!hist_rows || !levels)) || (n_counter_rows && !counter_rows))
+        return fail(ctx, LH_ERR_INVALID, "map or levels is NULL with rows");
+    if (!d_send || !d_recv || !n_words || !stream) return fail(ctx, LH_ERR_INVALID, "an output pointer is NULL");
+    for (uint32_t g = 0; g < n_rows; g++)
+        if (levels[g] != 0 && levels[g] != 1 && levels[g] != 3) return fail(ctx, LH_ERR_INVALID, "a level is not 0, 1 or 3");
+    for (uint32_t g = 0; g < n_rows; g++)
+        if (hist_rows[g] != LH_ROW_ABSENT && hist_rows[g] >= ctx->H) return fail(ctx, LH_ERR_RANGE, "histogram row >= max_histograms");
+    for (uint32_t g = 0; g < n_counter_rows; g++)
+        if (counter_rows[g] != LH_ROW_ABSENT && counter_rows[g] >= ctx->C) return fail(ctx, LH_ERR_RANGE, "counter row >= max_counters");
+    const size_t table_bytes = (size_t)ctx->H * sizeof(RowsEntry) + (size_t)ctx->C * 4;
+    if (!ctx->d_rows_table.get()) {
+        DevPtr<unsigned char> d; PinnedPtr<unsigned char> h; Event copied;
+        LH_CUDA(ctx, cudaMalloc(d.out(), table_bytes));
+        LH_CUDA(ctx, cudaMallocHost(h.out(), table_bytes));
+        LH_CUDA(ctx, cudaEventCreateWithFlags(copied.out(), cudaEventDisableTiming));
+        ctx->d_rows_table = std::move(d); ctx->h_rows_table = std::move(h); ctx->rows_table_copied = std::move(copied);
+    }
+    if (lh_status st = comm_alloc_reduced(ctx)) return st;
+    // the layout: every rank computes the same offsets from the same levels
+    const uint32_t wcells = 2u * ctx->pc.win - 1u;
+    // the staging is rewritten only after the previous upload from it has run
+    LH_CUDA(ctx, cudaEventSynchronize(ctx->rows_table_copied.get()));
+    RowsEntry *tab = reinterpret_cast<RowsEntry *>(ctx->h_rows_table.get());
+    uint64_t words = 0;
+    for (uint32_t g = 0; g < n_rows; g++) {
+        tab[g].row = hist_rows[g]; tab[g].level = levels[g]; tab[g].off = words;
+        words += levels[g] == 0 ? 0u : levels[g] == 1 ? wcells : 65536u;
+    }
+    const uint64_t ctr_off = words;
+    words += n_counter_rows;
+    uint32_t *tab_ctr = reinterpret_cast<uint32_t *>(ctx->h_rows_table.get() + (size_t)n_rows * sizeof(RowsEntry));
+    if (n_counter_rows) memcpy(tab_ctr, counter_rows, (size_t)n_counter_rows * 4);
+    if (words > ctx->rows_cap) {
+        // even, so that the 16-byte granule of the last word is inside the allocation
+        const size_t cap = (words + 1) & ~(size_t)1;
+        ctx->d_rows_send.reset(); ctx->d_rows_recv.reset(); ctx->rows_cap = 0;
+        DevPtr<unsigned long long> send, recv;
+        LH_CUDA(ctx, cudaMalloc(send.out(), cap * 8));
+        LH_CUDA(ctx, cudaMalloc(recv.out(), cap * 8));
+        ctx->d_rows_send = std::move(send); ctx->d_rows_recv = std::move(recv); ctx->rows_cap = cap;
+    }
+    cudaStream_t s = ctx->snap_stream.get();
+    const size_t up = (size_t)n_rows * sizeof(RowsEntry) + (size_t)n_counter_rows * 4;
+    if (up) {
+        LH_CUDA(ctx, cudaMemcpyAsync(ctx->d_rows_table.get(), ctx->h_rows_table.get(), up, cudaMemcpyHostToDevice, s));
+        ctx->stats.h2d_bytes += up;
+    }
+    LH_CUDA(ctx, cudaEventRecord(ctx->rows_table_copied.get(), s));
+    if (words) {
+        const int f = ctx->active ^ 1;
+        const size_t items = (size_t)n_rows * ROWS_PER_ROW + (n_counter_rows ? 1 : 0);
+        const int grid = (int)std::min<size_t>(items, (size_t)ctx->sm_count * 8);
+        const RowsEntry *dtab = reinterpret_cast<const RowsEntry *>(ctx->d_rows_table.get());
+        k_rows_pack<<<grid, ROWS_THREADS, 0, s>>>(dtab, n_rows, ctx->pc.win, ctx->buf[f].d_buckets.get(),
+                                                   reinterpret_cast<const uint32_t *>(dtab + n_rows), n_counter_rows,
+                                                   ctx->buf[f].d_counters.get(), ctr_off, ctx->d_rows_send.get());
+        LH_CUDA(ctx, cudaGetLastError());
+        ctx->stats.kernel_launches++;
+    }
+    ctx->rows_packed = true;
+    ctx->rows_n = n_rows; ctx->rows_nc = n_counter_rows; ctx->rows_words = words;
+    *d_send = reinterpret_cast<uint64_t *>(ctx->d_rows_send.get());
+    *d_recv = reinterpret_cast<uint64_t *>(ctx->d_rows_recv.get());
+    *n_words = words;
+    *stream = s;
+    return LH_OK;
+}
+
+extern "C" lh_status lh_snapshot_unpack_rows(lh_ctx *ctx, uint32_t summed) {
+    LH_ENTER(ctx);
+    if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
+    if (ctx->view_reduced) return fail(ctx, LH_ERR_STATE, "this snapshot has already been all-reduced");
+    if (!ctx->rows_packed) return fail(ctx, LH_ERR_STATE, "this snapshot has not been packed");
+    cudaStream_t s = ctx->snap_stream.get();
+    const uint32_t n_rows = ctx->rows_n;
+    const uint64_t ctr_off = ctx->rows_words - ctx->rows_nc;
+    const size_t items = std::max<size_t>((size_t)n_rows * ROWS_PER_ROW, 1);
+    const int grid = (int)std::min<size_t>(items, (size_t)ctx->sm_count * 8);
+    k_rows_unpack<<<grid, ROWS_THREADS, 0, s>>>(reinterpret_cast<const RowsEntry *>(ctx->d_rows_table.get()), n_rows,
+                                                ctx->pc.win, summed ? ctx->d_rows_recv.get() : ctx->d_rows_send.get(),
+                                                ctx->rows_nc, ctx->C, ctr_off, ctx->d_red_buckets.get(),
+                                                ctx->d_red_flags.get(), ctx->d_red_counters.get());
+    LH_CUDA(ctx, cudaGetLastError());
+    ctx->stats.kernel_launches++;
+    ctx->view_reduced = true;
+    ctx->view_counters_reduced = true;
+    ctx->nnz_valid = false;
+    return LH_OK;
 }
 
 extern "C" lh_status lh_comm_allreduce_ms(lh_ctx *ctx, uint64_t seq, float *ms) {

@@ -18,6 +18,7 @@
 //   K4   k_scan_nnz, k_export   sparse (key,count) lists (RawMetricSet.Histograms);  k_merge_sparse is the inverse
 //   K5   k_peer_allreduce       multi-GPU: sums the live window of every peer's frozen arrays over NVLink peer
 //                               mappings (SURVEY.md section 8e) -- no library collective
+//        k_rows_pack, k_rows_unpack   job-wide rows to and from a payload the caller all-reduces (any transport)
 //   K6   k_scatter_segments, k_sparse_epilogue   caller-supplied sparse histograms -> scratch rows -> K3
 //                               (lh_reduce_sparse_host)
 //   k_ingest_batch          many device arrays under many ids (lh_ingest_batch, lh_graph_recorder_ingest)
@@ -1949,6 +1950,106 @@ __global__ void __launch_bounds__(K5_THREADS, 1)
 k_peer_allreduce_rows(PeerParams p, RowMap rows) {
     extern __shared__ unsigned char s_level[];               // [n_rows]: OR over ranks of the row's flag
     k5_body(p, rows, s_level);
+}
+
+// ------------------------------------------------ job-wide rows through the caller's all-reduce (lh_snapshot_*_rows)
+// A payload every rank lays out alike, so that an element-wise uint64 sum over ranks (any transport: gloo, NCCL, MPI)
+// is the job-wide interval.  Row g of level 1 (every rank's counts inside the fast window) is its 2*win-1 window cells,
+// indices [0, win) then [65536-(win-1), 65536); level 3 is all 65536 cells in index order; level 0 is nothing.  The
+// counter rows follow.  k_rows_pack gathers this rank's frozen rows into it, k_rows_unpack writes a payload into the
+// reduced arrays at row g.  Work item = (row, chunk of ROWS_CHUNK payload words); every access is 16 bytes wide except
+// a segment's first and last word when they are unpaired.
+constexpr int ROWS_THREADS = 256;
+constexpr uint32_t ROWS_CHUNK = 8u * ROWS_THREADS;               // payload words per work item: 4 pairs per thread
+constexpr uint32_t ROWS_PER_ROW = 65536u / ROWS_CHUNK;          // work items per row (a window row uses the first few)
+
+struct RowsEntry {                  // 16 bytes per job-wide row, in the device table
+    uint32_t row;                   // this rank's frozen row (pack), or K5_ROW_ABSENT
+    uint32_t level;                 // 0, 1 or 3: the agreed level
+    unsigned long long off;         // payload word of the row's first cell
+};
+
+// dst[0, n) = src[0, n) (src NULL: zeros), one CTA.  Stores are 16-byte aligned pairs after at most one scalar head;
+// a source of the other parity is read as the aligned pairs around it (the pair before its first word and after its
+// last lie in the same 16-byte granule as a word of the segment, so they are inside the allocation).
+__device__ __forceinline__ void rows_copy(unsigned long long *dst, const unsigned long long *src, uint32_t n) {
+    const uint32_t t = threadIdx.x;
+    const uint32_t head = min(n, (uint32_t)(((uintptr_t)dst >> 3) & 1u));
+    if (t == 0 && head) dst[0] = src ? __ldg(src) : 0ull;
+    dst += head; n -= head;
+    if (src) src += head;
+    const uint32_t np = n >> 1;
+    ulonglong2 *d2 = reinterpret_cast<ulonglong2 *>(dst);
+    if (!src) {
+        for (uint32_t k = t; k < np; k += ROWS_THREADS) d2[k] = make_ulonglong2(0ull, 0ull);
+    } else if ((((uintptr_t)src >> 3) & 1u) == 0) {
+        const ulonglong2 *s2 = reinterpret_cast<const ulonglong2 *>(src);
+        for (uint32_t k = t; k < np; k += ROWS_THREADS) d2[k] = __ldg(s2 + k);
+    } else {
+        const ulonglong2 *s2 = reinterpret_cast<const ulonglong2 *>(src - 1);
+        for (uint32_t k = t; k < np; k += ROWS_THREADS) {
+            const ulonglong2 a = __ldg(s2 + k), b = __ldg(s2 + k + 1);
+            d2[k] = make_ulonglong2(a.y, b.x);
+        }
+    }
+    if (t == 0 && (n & 1u)) dst[n - 1] = src ? __ldg(src + n - 1) : 0ull;
+}
+
+// The payload words [j0, j1) of a row at level `level` and where they sit in its 65536 cells: calls
+// f(first payload word, first cell, words) for each run of consecutive cells (one or two per work item).
+template <typename F>
+__device__ __forceinline__ void rows_runs(uint32_t level, uint32_t chunk, uint32_t win, F f) {
+    const uint32_t len = (level & 2u) ? 65536u : 2u * win - 1u;
+    const uint32_t j0 = chunk * ROWS_CHUNK, j1 = min(len, j0 + ROWS_CHUNK);
+    if (j0 >= j1) return;
+    if (level & 2u) { f(j0, j0, j1 - j0); return; }
+    if (j0 < win) f(j0, j0, min(j1, win) - j0);
+    if (j1 > win) {
+        const uint32_t a = max(j0, win);
+        f(a, a + 65537u - 2u * win, j1 - a);        // payload word win is cell 65536 - (win - 1)
+    }
+}
+
+__global__ void __launch_bounds__(ROWS_THREADS)
+k_rows_pack(const RowsEntry *__restrict__ table, uint32_t n_rows, uint32_t win,
+            const unsigned long long *__restrict__ buckets, const uint32_t *__restrict__ ctr_rows, uint32_t n_counter_rows,
+            const unsigned long long *__restrict__ counters, unsigned long long ctr_off,
+            unsigned long long *__restrict__ payload) {
+    for (uint32_t i = blockIdx.x * ROWS_THREADS + threadIdx.x; i < n_counter_rows; i += gridDim.x * ROWS_THREADS) {
+        const uint32_t c = __ldg(ctr_rows + i);
+        payload[ctr_off + i] = c == K5_ROW_ABSENT ? 0ull : __ldg(counters + c);
+    }
+    const size_t items = (size_t)n_rows * ROWS_PER_ROW;
+    for (size_t item = blockIdx.x; item < items; item += gridDim.x) {
+        const RowsEntry e = table[item / ROWS_PER_ROW];
+        if (e.level == 0) continue;
+        const unsigned long long *src = e.row == K5_ROW_ABSENT ? nullptr : buckets + (size_t)e.row * 65536u;
+        rows_runs(e.level, (uint32_t)(item % ROWS_PER_ROW), win, [&](uint32_t j, uint32_t cell, uint32_t n) {
+            rows_copy(payload + e.off + j, src ? src + cell : nullptr, n);
+        });
+    }
+}
+
+// Row g < n_rows: cells from the payload, flag = level; counters below n_counter_rows from the payload, the rest 0.
+// The reduced arrays are zero outside flagged rows (lh_snapshot_end clears them by their flags), so nothing else moves.
+__global__ void __launch_bounds__(ROWS_THREADS)
+k_rows_unpack(const RowsEntry *__restrict__ table, uint32_t n_rows, uint32_t win,
+              const unsigned long long *__restrict__ payload, uint32_t n_counter_rows, uint32_t C,
+              unsigned long long ctr_off, unsigned long long *__restrict__ out_buckets, uint32_t *__restrict__ out_flags,
+              unsigned long long *__restrict__ out_counters) {
+    const uint32_t tid = blockIdx.x * ROWS_THREADS + threadIdx.x, nthreads = gridDim.x * ROWS_THREADS;
+    for (uint32_t g = tid; g < n_rows; g += nthreads) out_flags[g] = table[g].level;
+    for (uint32_t i = tid; i < C; i += nthreads) out_counters[i] = i < n_counter_rows ? __ldg(payload + ctr_off + i) : 0ull;
+    const size_t items = (size_t)n_rows * ROWS_PER_ROW;
+    for (size_t item = blockIdx.x; item < items; item += gridDim.x) {
+        const uint32_t g = (uint32_t)(item / ROWS_PER_ROW);
+        const RowsEntry e = table[g];
+        if (e.level == 0) continue;
+        unsigned long long *dst = out_buckets + (size_t)g * 65536u;
+        rows_runs(e.level, (uint32_t)(item % ROWS_PER_ROW), win, [&](uint32_t j, uint32_t cell, uint32_t n) {
+            rows_copy(dst + cell, payload + e.off + j, n);
+        });
+    }
 }
 
 // ----------------------------------------------------------- batch ingest (lh_ingest_batch)

@@ -201,3 +201,43 @@ def rank_allgather(group=None):
         return [bytes(b) for b in out]
 
     return allgather
+
+
+def rank_allreduce(group=None):
+    """The all-reduce MetricSystem.join_ranks takes beside rank_allgather(group), over a torch.distributed process group:
+    allreduce(send_ptr, recv_ptr, n_words, stream_ptr) sums the n_words int64 (the uint64 counts, wrapping alike) of
+    every rank's send buffer into recv, through zero-copy views of the two device buffers.
+
+    A gloo group (recommended: `dist.new_group(backend="gloo")` on every rank) copies send to the host on the stream,
+    sums with dist.all_reduce and copies the sums into recv on the stream, waiting for each copy.  It works across nodes and runs
+    no GPU-side collective beside the training loop's.  An NCCL group copies send into recv and runs dist.all_reduce on
+    recv under that stream.  Use a dedicated group either way: the reaper sums at every collection from its own
+    thread, and a second communicator whose kernels interleave with the training loop's in different orders on
+    different ranks can deadlock both.
+    """
+    import torch
+    import torch.distributed as dist
+
+    host = []   # gloo: one pinned buffer, grown on demand
+
+    def allreduce(send_ptr: int, recv_ptr: int, n_words: int, stream_ptr: int):
+        send = torch.as_tensor(_CudaView(send_ptr, n_words))
+        recv = torch.as_tensor(_CudaView(recv_ptr, n_words))
+        s = torch.cuda.ExternalStream(stream_ptr, device=send.device)
+        if dist.get_backend(group) == "nccl":
+            with torch.cuda.stream(s):
+                recv.copy_(send)
+                dist.all_reduce(recv, op=dist.ReduceOp.SUM, group=group)
+            return
+        if not host or host[0].numel() < n_words:
+            host[:] = [torch.empty(n_words, dtype=torch.int64, pin_memory=True)]
+        buf = host[0][:n_words]
+        # blocking copies on s: the first waits for the pack, the second is complete on return.  (An asynchronous copy
+        # would tie the pinned buffer to s, which the library destroys with its context.)
+        with torch.cuda.stream(s):
+            buf.copy_(send)
+        dist.all_reduce(buf, op=dist.ReduceOp.SUM, group=group)
+        with torch.cuda.stream(s):
+            recv.copy_(buf)
+
+    return allreduce

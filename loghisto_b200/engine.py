@@ -672,6 +672,31 @@ class Engine:
                                                         C.byref(out)))
         return int(out.value)
 
+    def snapshot_row_levels(self):
+        """lh_snapshot_row_levels: uint8[H] levels of the frozen rows (0 no data, 1 window only, 3 beyond the window)."""
+        levels = np.zeros(self.H, np.uint8)
+        self._check(self.lib.lh_snapshot_row_levels(self.h, levels.ctypes.data))
+        return levels
+
+    def snapshot_pack_rows(self, hist_rows, levels, counter_rows):
+        """lh_snapshot_pack_rows: this rank's column of the maps (LH_ROW_ABSENT for none) and the agreed levels.
+        Returns (send_ptr, recv_ptr, n_words, stream_ptr); the payload is enqueued on that stream."""
+        hr = np.ascontiguousarray(hist_rows, dtype=np.uint32)
+        lv = np.ascontiguousarray(levels, dtype=np.uint8)
+        cr = np.ascontiguousarray(counter_rows, dtype=np.uint32)
+        if lv.size != hr.size:
+            raise ValueError("levels must have one entry per histogram row")
+        send, recv, stream, n = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_uint64()
+        self._check(self.lib.lh_snapshot_pack_rows(self.h, hr.size, hr.ctypes.data if hr.size else None,
+                                                   lv.ctypes.data if lv.size else None, cr.size,
+                                                   cr.ctypes.data if cr.size else None, C.byref(send), C.byref(recv),
+                                                   C.byref(n), C.byref(stream)))
+        return int(send.value or 0), int(recv.value or 0), int(n.value), int(stream.value or 0)
+
+    def snapshot_unpack_rows(self, summed: bool):
+        """lh_snapshot_unpack_rows: the payload's sums (summed) or this rank's own counts into the reduced arrays."""
+        self._check(self.lib.lh_snapshot_unpack_rows(self.h, 1 if summed else 0))
+
     def comm_allreduce_ms(self, seq: int) -> float:
         ms = C.c_float()
         self._check(self.lib.lh_comm_allreduce_ms(self.h, seq, C.byref(ms)))

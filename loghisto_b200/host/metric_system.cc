@@ -66,6 +66,10 @@
 #pragma weak lh_snapshot_copy_histogram
 #pragma weak lh_snapshot_rows
 #pragma weak lh_snapshot_allreduce_rows
+// And for joined ranks through the caller's all-reduce: over a build without them, that JoinRanks throws.
+#pragma weak lh_snapshot_row_levels
+#pragma weak lh_snapshot_pack_rows
+#pragma weak lh_snapshot_unpack_rows
 
 namespace loghisto {
 
@@ -1213,24 +1217,40 @@ struct Reader {
     std::string str() { const uint32_t n = u32(); need(n); std::string v = b.substr(at, n); at += n; return v; }
 };
 constexpr uint32_t kJoinMagic = 0x4C48524Bu;   // first exchange: handle + shape
-constexpr uint32_t kRowsMagic = 0x4C485253u;   // per collection: sequence, frozen half, touched names
+constexpr uint32_t kRowsMagic = 0x4C485253u;   // per collection: sequence, frozen half, touched names (and levels)
 }  // namespace
 
 void MetricSystem::JoinRanks(uint32_t rank, uint32_t world, AllGather allgather) {
     if (!lh_comm_export || !lh_comm_import || !lh_comm_info || !lh_snapshot_copy_histogram || !lh_snapshot_rows ||
         !lh_snapshot_allreduce_rows)
         throw std::runtime_error("JoinRanks: this libloghisto_b200 has no row-mapped all-reduce");
+    join(rank, world, std::move(allgather), nullptr);
+}
+
+void MetricSystem::JoinRanks(uint32_t rank, uint32_t world, AllGather allgather, AllReduce allreduce) {
+    if (!lh_snapshot_copy_histogram || !lh_snapshot_rows || !lh_snapshot_row_levels || !lh_snapshot_pack_rows ||
+        !lh_snapshot_unpack_rows)
+        throw std::runtime_error("JoinRanks: this libloghisto_b200 has no lh_snapshot_pack_rows");
+    if (!allreduce) throw std::invalid_argument("JoinRanks: allreduce is empty");
+    join(rank, world, std::move(allgather), std::move(allreduce));
+}
+
+// The join of both transports: the configuration and the transport are exchanged and checked on every rank alike;
+// the peer transport (allreduce empty) then maps every rank's arrays.
+void MetricSystem::join(uint32_t rank, uint32_t world, AllGather allgather, AllReduce allreduce) {
     if (world < 2 || world > LH_MAX_RANKS || rank >= world)
         throw std::invalid_argument("JoinRanks: need 2 <= world <= LH_MAX_RANKS and rank < world");
     if (!allgather) throw std::invalid_argument("JoinRanks: allgather is empty");
     std::lock_guard<std::mutex> snap(snapshot_mu_);
     if (collected_) throw std::runtime_error("JoinRanks on a system that has collected already");
     if (allgather_) throw std::runtime_error("JoinRanks on a system that has joined already");
+    const uint32_t transport = allreduce ? 1u : 0u;   // 0 peer memory, 1 the caller's all-reduce
     lh_peer_handle mine{};
-    check(ctx_, lh_comm_export(ctx_, &mine), "lh_comm_export");
+    if (!allreduce) check(ctx_, lh_comm_export(ctx_, &mine), "lh_comm_export");
     std::string b;
     put_u32(b, kJoinMagic);
     put_u32(b, opt_.max_histograms); put_u32(b, opt_.max_counters); put_u32(b, opt_.precision);
+    put_u32(b, transport);
     b.append(reinterpret_cast<const char *>(mine.bytes), sizeof mine.bytes);
     const std::vector<std::string> all = allgather(b);
     if (all.size() != world) throw std::runtime_error("JoinRanks: allgather returned a list of the wrong size");
@@ -1239,13 +1259,16 @@ void MetricSystem::JoinRanks(uint32_t rank, uint32_t world, AllGather allgather)
         if (all[r].size() != b.size()) throw std::invalid_argument("JoinRanks: a rank's payload is malformed");
         Reader rd{all[r]};
         if (rd.u32() != kJoinMagic) throw std::invalid_argument("JoinRanks: a rank's payload is malformed");
-        const uint32_t h = rd.u32(), c = rd.u32(), p = rd.u32();
+        const uint32_t h = rd.u32(), c = rd.u32(), p = rd.u32(), t = rd.u32();
         if (h != opt_.max_histograms || c != opt_.max_counters || p != opt_.precision)
             throw std::invalid_argument("JoinRanks: the ranks differ in max_histograms, max_counters or precision");
+        if (t != transport)
+            throw std::invalid_argument("JoinRanks: the ranks differ in transport (some pass an allreduce, some not)");
         memcpy(handles[r].bytes, all[r].data() + rd.at, sizeof handles[r].bytes);
     }
-    check(ctx_, lh_comm_import(ctx_, rank, world, handles.data()), "lh_comm_import");
+    if (!allreduce) check(ctx_, lh_comm_import(ctx_, rank, world, handles.data()), "lh_comm_import");
     allgather_ = std::move(allgather);
+    allreduce_ = std::move(allreduce);
     std::lock_guard<std::mutex> lk(ranks_mu_);
     ranks_.rank = rank;
     ranks_.world = world;
@@ -1264,17 +1287,27 @@ struct MetricSystem::JobRows {
 };
 
 // Steps between lh_snapshot_begin and the reduction of a joined system's collection: lh_snapshot_rows, one exchange,
-// the unions, the maps, lh_snapshot_allreduce_rows.  False when the exchange failed (nothing was launched: the
-// collection is this rank's own).  counter_touched: the host's touched marks (Counter(name, 0) is in Rates).
+// the unions, the maps, lh_snapshot_allreduce_rows (or sum_rows through the caller's all-reduce, with each touched
+// row's level in the exchange).  False when the exchange failed (nothing was launched: the collection is this rank's
+// own).  counter_touched: the host's touched marks (Counter(name, 0) is in Rates).
 bool MetricSystem::join_collection(JobRows &j, const std::vector<uint8_t> &counter_touched) {
     const uint32_t H = opt_.max_histograms, Cn = opt_.max_counters;
     const uint32_t rank = ranks_.rank, world = ranks_.world;
+    const bool by_allreduce = static_cast<bool>(allreduce_);
     j.hist_touched.assign(H, 0);
     j.counter_deltas.assign(Cn, 0);
     uint32_t frozen = 0;
-    check(ctx_, lh_snapshot_rows(ctx_, j.hist_touched.data(), j.counter_deltas.data(), &frozen), "lh_snapshot_rows");
+    std::vector<uint8_t> my_levels;
     lh_comm_stats cs{};
-    check(ctx_, lh_comm_info(ctx_, &cs), "lh_comm_info");
+    if (by_allreduce) {
+        my_levels.assign(H, 0);
+        check(ctx_, lh_snapshot_rows(ctx_, nullptr, j.counter_deltas.data(), &frozen), "lh_snapshot_rows");
+        check(ctx_, lh_snapshot_row_levels(ctx_, my_levels.data()), "lh_snapshot_row_levels");
+        for (uint32_t h = 0; h < H; h++) j.hist_touched[h] = my_levels[h] != 0;
+    } else {
+        check(ctx_, lh_snapshot_rows(ctx_, j.hist_touched.data(), j.counter_deltas.data(), &frozen), "lh_snapshot_rows");
+        check(ctx_, lh_comm_info(ctx_, &cs), "lh_comm_info");
+    }
     std::vector<std::pair<uint32_t, std::string>> mine_h, mine_c;
     {
         std::shared_lock<std::shared_mutex> rl(histos_.mu);
@@ -1291,13 +1324,17 @@ bool MetricSystem::join_collection(JobRows &j, const std::vector<uint8_t> &count
     put_u64(b, cs.allreduces);
     put_u32(b, frozen);
     put_u32(b, (uint32_t)mine_h.size());
-    for (auto &e : mine_h) { put_u32(b, e.first); put_u32(b, (uint32_t)e.second.size()); b += e.second; }
+    for (auto &e : mine_h) {
+        put_u32(b, e.first); put_u32(b, (uint32_t)e.second.size()); b += e.second;
+        if (by_allreduce) put_u32(b, my_levels[e.first]);
+    }
     put_u32(b, (uint32_t)mine_c.size());
     for (auto &e : mine_c) { put_u32(b, e.first); put_u32(b, (uint32_t)e.second.size()); b += e.second; }
 
     std::vector<uint64_t> seqs(world);
     std::vector<uint32_t> frozens(world);
     std::vector<std::vector<std::pair<uint32_t, std::string>>> hs(world), cs_(world);
+    std::vector<std::vector<uint32_t>> hlevels(world);   // by_allreduce: the level of each entry of hs[r]
     try {
         const std::vector<std::string> all = allgather_(b);
         if (all.size() != world) throw std::runtime_error("allgather returned a list of the wrong size");
@@ -1314,6 +1351,11 @@ bool MetricSystem::join_collection(JobRows &j, const std::vector<uint8_t> &count
                     const uint32_t id = rd.u32();
                     if (id >= bound) throw std::runtime_error("a rank's payload is malformed");
                     list->emplace_back(id, rd.str());
+                    if (by_allreduce && list == &hs[r]) {
+                        const uint32_t lv = rd.u32();
+                        if (lv != 1 && lv != 3) throw std::runtime_error("a rank's payload is malformed");
+                        hlevels[r].push_back(lv);
+                    }
                 }
             }
         }
@@ -1366,6 +1408,25 @@ bool MetricSystem::join_collection(JobRows &j, const std::vector<uint8_t> &count
         for (auto &e : mine_c)
             if (!kept.count(e.second)) dropped_over_limit_.fetch_add(j.counter_deltas[e.first], std::memory_order_relaxed);
     }
+    if (by_allreduce) {
+        {
+            std::lock_guard<std::mutex> lk(ranks_mu_);
+            ranks_.names_dropped += dropped_names;
+        }
+        // the agreed level of row g: the largest any rank froze it at
+        std::unordered_map<std::string, uint32_t> row;
+        for (uint32_t g = 0; g < j.hnames.size(); g++) row.emplace(j.hnames[g], g);
+        std::vector<uint8_t> levels(j.hnames.size(), 0);
+        for (uint32_t r = 0; r < world; r++)
+            for (size_t i = 0; i < hs[r].size(); i++) {
+                auto it = row.find(hs[r][i].second);
+                if (it != row.end()) levels[it->second] = std::max<uint8_t>(levels[it->second], (uint8_t)hlevels[r][i]);
+            }
+        const size_t nh = j.hnames.size(), nc = j.cnames.size();
+        sum_rows(std::vector<uint32_t>(hmap.begin() + rank * nh, hmap.begin() + (rank + 1) * nh), levels,
+                 std::vector<uint32_t>(cmap.begin() + rank * nc, cmap.begin() + (rank + 1) * nc));
+        return true;
+    }
     const uint64_t seq = *std::max_element(seqs.begin(), seqs.end()) + 1;
     check(ctx_, lh_snapshot_allreduce_rows(ctx_, seq, frozens.data(), (uint32_t)j.hnames.size(), hmap.data(),
                                            (uint32_t)j.cnames.size(), cmap.data(), nullptr),
@@ -1373,6 +1434,34 @@ bool MetricSystem::join_collection(JobRows &j, const std::vector<uint8_t> &count
     std::lock_guard<std::mutex> lk(ranks_mu_);
     ranks_.names_dropped += dropped_names;
     return true;
+}
+
+// The job-wide rows through the caller's all-reduce: pack this rank's column of the maps at the agreed levels, sum,
+// unpack.  Every rank derives n_words from the same exchange, so every rank calls allreduce_ with the same size, or
+// none does.  An allreduce_ that throws leaves this rank's own counts under the job-wide rows (status 4).
+void MetricSystem::sum_rows(const std::vector<uint32_t> &hmap, const std::vector<uint8_t> &levels,
+                            const std::vector<uint32_t> &cmap) {
+    uint64_t *send = nullptr, *recv = nullptr, n_words = 0;
+    void *stream = nullptr;
+    check(ctx_, lh_snapshot_pack_rows(ctx_, (uint32_t)hmap.size(), hmap.data(), levels.data(), (uint32_t)cmap.size(),
+                                      cmap.data(), &send, &recv, &n_words, &stream),
+          "lh_snapshot_pack_rows");
+    uint32_t status = 0;
+    try {
+        if (n_words) allreduce_(send, recv, (size_t)n_words, stream);
+    } catch (const std::exception &e) {
+        status = 4;
+        if (!allreduce_logged_) {
+            allreduce_logged_ = true;
+            fprintf(stderr, "loghisto: rank %u: the collection's allreduce failed (%s); this rank's own counts under the "
+                    "job-wide names\n", ranks_.rank, e.what());
+        }
+    }
+    check(ctx_, lh_snapshot_unpack_rows(ctx_, status == 0 ? 1u : 0u), "lh_snapshot_unpack_rows");
+    std::lock_guard<std::mutex> lk(ranks_mu_);
+    ranks_.status = status;
+    ranks_.bytes_from_peers = status == 0 ? 8 * n_words : 0;
+    if (status == 0) ranks_.summed++;
 }
 
 // collectRawMetrics, metrics.go:420-479.
@@ -1430,7 +1519,7 @@ std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
         check(ctx_, lh_snapshot_reduce(ctx_, ps.data(), np, counts.data(), sums.data(), avgs.data(), pkeys.data(), pvals.data()),
               "lh_snapshot_reduce");
         check(ctx_, lh_snapshot_export(ctx_, &sp), "lh_snapshot_export");
-        if (joined) {
+        if (joined && !allreduce_) {
             lh_comm_stats cs{};
             check(ctx_, lh_comm_info(ctx_, &cs), "lh_comm_info");
             std::lock_guard<std::mutex> lk(ranks_mu_);
@@ -1864,22 +1953,47 @@ void gather_sink(void *sink_ctx, uint32_t rank, const void *p, uint64_t len) {
     g->parts[rank].assign(static_cast<const char *>(p), (size_t)len);
     g->seen[rank] = 1;
 }
+MetricSystem::AllGather c_allgather(lhms_ranks_allgather_fn allgather, void *user, uint32_t world) {
+    return [allgather, user, world](const std::string &mine) {
+        GatherSink g;
+        g.parts.resize(world);
+        g.seen.assign(world, 0);
+        if (allgather(user, mine.data(), mine.size(), gather_sink, &g) != 0)
+            throw std::runtime_error("the all-gather callback failed");
+        for (uint32_t r = 0; r < world; r++)
+            if (!g.seen[r]) throw std::runtime_error("the all-gather callback left a rank out");
+        return g.parts;
+    };
+}
 }  // namespace
 LHMS_API int lhms_ranks_join(void *ms, uint32_t rank, uint32_t world, lhms_ranks_allgather_fn allgather, void *user,
                              char *err, int errlen) {
     try {
         if (!ms || !allgather) throw std::invalid_argument("lhms_ranks_join: NULL system or allgather");
-        auto fn = [allgather, user, world](const std::string &mine) {
-            GatherSink g;
-            g.parts.resize(world);
-            g.seen.assign(world, 0);
-            if (allgather(user, mine.data(), mine.size(), gather_sink, &g) != 0)
-                throw std::runtime_error("the all-gather callback failed");
-            for (uint32_t r = 0; r < world; r++)
-                if (!g.seen[r]) throw std::runtime_error("the all-gather callback left a rank out");
-            return g.parts;
+        static_cast<MetricSystem *>(ms)->JoinRanks(rank, world, c_allgather(allgather, user, world));
+        return 0;
+    } catch (const std::invalid_argument &e) {
+        if (err && errlen > 0) snprintf(err, (size_t)errlen, "%s", e.what());
+        return -2;
+    } catch (const std::exception &e) {
+        if (err && errlen > 0) snprintf(err, (size_t)errlen, "%s", e.what());
+        return -1;
+    }
+}
+// MetricSystem::JoinRanks over the caller's all-reduce: allgather as for lhms_ranks_join, and allreduce(user, d_send,
+// d_recv, n_words, stream), which leaves in d_recv the wrapping uint64 sum over ranks of d_send (enqueued on stream, or
+// completed when it returns) and returns 0, or nonzero on failure.  Both are called on the collecting thread.  Returns
+// as lhms_ranks_join.
+typedef int (*lhms_ranks_allreduce_fn)(void *user, const uint64_t *d_send, uint64_t *d_recv, uint64_t n_words, void *stream);
+LHMS_API int
+lhms_ranks_join_allreduce(void *ms, uint32_t rank, uint32_t world, lhms_ranks_allgather_fn allgather,
+                          lhms_ranks_allreduce_fn allreduce, void *user, char *err, int errlen) {
+    try {
+        if (!ms || !allgather || !allreduce) throw std::invalid_argument("lhms_ranks_join_allreduce: NULL system or callback");
+        auto reduce = [allreduce, user](const uint64_t *d_send, uint64_t *d_recv, size_t n_words, void *stream) {
+            if (allreduce(user, d_send, d_recv, n_words, stream) != 0) throw std::runtime_error("the all-reduce callback failed");
         };
-        static_cast<MetricSystem *>(ms)->JoinRanks(rank, world, fn);
+        static_cast<MetricSystem *>(ms)->JoinRanks(rank, world, c_allgather(allgather, user, world), reduce);
         return 0;
     } catch (const std::invalid_argument &e) {
         if (err && errlen > 0) snprintf(err, (size_t)errlen, "%s", e.what());

@@ -457,11 +457,27 @@ class MetricSystem {
     // on it after the all-reduce's 10 s timeout and keep their own counts (status 1).
     using AllGather = std::function<std::vector<std::string>(const std::string &mine)>;
     void JoinRanks(uint32_t rank, uint32_t world, AllGather allgather);
+
+    // JoinRanks over a transport the caller owns, for ranks that cannot map each other's memory (ranks on different
+    // hosts: CUDA IPC works only within one).  The collections agree on the same job-wide rows, and the rows are summed
+    // by allreduce instead of the peer-memory all-reduce; no peer handle is exported or imported.  At each collection
+    // every rank packs its rows into a payload laid out alike on every rank (lh_snapshot_pack_rows) and calls
+    // allreduce(d_send, d_recv, n_words, stream) on the collecting thread, with the same n_words on every rank (none
+    // when nothing was touched anywhere).  It must leave in d_recv the wrapping uint64 element-wise sum over ranks of
+    // d_send, either enqueued on `stream` (the snapshot stream, behind the pack) or completed when it returns, and
+    // throw on failure.  A throw gives that rank its own counts under the job-wide rows (RanksInfo().status 4, logged
+    // once); the next collection sums again.  The join refuses, on every rank alike (std::invalid_argument), ranks
+    // that differ in transport (some with allreduce, some without) as well as in the configuration; std::runtime_error
+    // when the library lacks lh_snapshot_pack_rows.  This transport has no timeout of its own: a rank whose exchange
+    // failed while others' succeeded leaves those inside the caller's collective until its own timeout.
+    using AllReduce = std::function<void(const uint64_t *d_send, uint64_t *d_recv, size_t n_words, void *stream)>;
+    void JoinRanks(uint32_t rank, uint32_t world, AllGather allgather, AllReduce allreduce);
     struct RanksState {
         uint32_t rank = 0, world = 0;   // world 0: not joined
-        uint32_t status = 0;            // last collection: 0 summed, 1 / 2 as lh_comm_stats, 3 exchange failed
+        uint32_t status = 0;            // last collection: 0 summed, 1 / 2 as lh_comm_stats, 3 exchange failed,
+                                        // 4 the caller's allreduce threw
         uint64_t summed = 0;            // collections summed across the ranks
-        uint64_t bytes_from_peers = 0;  // of the last collection's all-reduce
+        uint64_t bytes_from_peers = 0;  // of the last collection's all-reduce (8 x n_words through allreduce)
         uint64_t names_dropped = 0;     // names left out of the job-wide union by the bounds, over all collections
     };
     RanksState RanksInfo();
@@ -575,7 +591,11 @@ class MetricSystem {
     // JoinRanks: the exchange and the job-wide rows of a collection (under snapshot_mu_)
     struct JobRows;
     bool join_collection(JobRows &j, const std::vector<uint8_t> &counter_touched);
+    void join(uint32_t rank, uint32_t world, AllGather allgather, AllReduce allreduce);
+    void sum_rows(const std::vector<uint32_t> &hmap, const std::vector<uint8_t> &levels, const std::vector<uint32_t> &cmap);
     AllGather allgather_;
+    AllReduce allreduce_;
+    bool allreduce_logged_ = false;
     bool collected_ = false;
     bool exchange_logged_ = false;
     std::mutex ranks_mu_;

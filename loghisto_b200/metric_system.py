@@ -18,6 +18,7 @@ from .engine import (_batch_array, _capture_stream, _stream, _timer_stream, boar
 _EMIT = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_char_p, C.c_int, C.c_uint64, C.c_double)
 _RANKS_SINK = C.CFUNCTYPE(None, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64)
 _RANKS_ALLGATHER = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, _RANKS_SINK, C.c_void_p)
+_RANKS_ALLREDUCE = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p)
 _lib = None
 
 
@@ -135,6 +136,9 @@ def _bind(L):
     L.lhms_ranks_join.restype = C.c_int
     L.lhms_ranks_join.argtypes = [vp, C.c_uint32, C.c_uint32, _RANKS_ALLGATHER, vp, C.c_char_p, C.c_int]
     L.lhms_ranks_info.argtypes = [vp, C.POINTER(C.c_uint64)]
+    L.lhms_ranks_join_allreduce.restype = C.c_int
+    L.lhms_ranks_join_allreduce.argtypes = [vp, C.c_uint32, C.c_uint32, _RANKS_ALLGATHER, _RANKS_ALLREDUCE, vp,
+                                            C.c_char_p, C.c_int]
     return L
 
 
@@ -756,7 +760,7 @@ class MetricSystem:
             raise RuntimeError(err.value.decode())
         return col.metrics
 
-    def join_ranks(self, rank: int, world: int, allgather):
+    def join_ranks(self, rank: int, world: int, allgather, allreduce=None):
         """Joins the systems of a multi-GPU job, so that each collection describes the whole job
         (MetricSystem::JoinRanks).  Collective: every rank calls it once, before its first collection, with
         allgather(bytes) -> list[bytes], every rank's bytes in rank order (loghisto_b200.distributed.rank_allgather builds
@@ -765,10 +769,21 @@ class MetricSystem:
 
         Afterwards Histograms, Rates, Counters, the aggregates and device subscriptions are job-wide and identical on
         every rank; gauges stay rank-local.  ValueError for a bad rank / world, or when the ranks differ in
-        max_histograms, max_counters or precision (raised on every rank alike); RuntimeError otherwise."""
+        max_histograms, max_counters or precision (raised on every rank alike); RuntimeError otherwise.
+
+        With allreduce, the rows are summed through it instead of the peer-memory all-reduce, which needs every rank
+        on one host (loghisto_b200.distributed.rank_allreduce builds one from a process group).  At each collection
+        allreduce(send_ptr, recv_ptr, n_words, stream_ptr) gets plain ints: two device buffers of n_words uint64 and
+        the CUDA stream the payload was packed on.  It must leave in recv the wrapping uint64 element-wise sum over
+        ranks of send, enqueued on that stream or complete when it returns.  Every rank calls it with the same n_words,
+        or none does.  An exception in it is logged once, and that collection gives this rank's own counts under the
+        job-wide names (ranks_info()["status"] 4); the next one sums again.  Every rank must pass an allreduce or none
+        (ValueError on every rank alike otherwise); TypeError when it is not callable."""
         rank, world = int(rank), int(world)
         if not callable(allgather):
             raise TypeError("allgather must be callable")
+        if allreduce is not None and not callable(allreduce):
+            raise TypeError("allreduce must be callable")
         if world < 2 or world > _L.LH_MAX_RANKS or not 0 <= rank < world:
             raise ValueError("join_ranks: need 2 <= world <= %d and 0 <= rank < world" % _L.LH_MAX_RANKS)
 
@@ -791,15 +806,33 @@ class MetricSystem:
 
         cb = _RANKS_ALLGATHER(gather)
         err = C.create_string_buffer(512)
-        rc = self._lib.lhms_ranks_join(self._h, rank, world, cb, None, err, 512)
+        if allreduce is None:
+            rc = self._lib.lhms_ranks_join(self._h, rank, world, cb, None, err, 512)
+        else:
+            reduce_logged = []
+
+            def reduce(_user, send, recv, n, stream):
+                try:
+                    allreduce(int(send or 0), int(recv or 0), int(n), int(stream or 0))
+                    return 0
+                except Exception as e:   # this collection keeps this rank's own counts; say why, once
+                    if not reduce_logged:
+                        reduce_logged.append(e)
+                        sys.stderr.write("loghisto: rank %d: allreduce raised %s: %s\n" % (rank, type(e).__name__, e))
+                    return 1
+            rcb = _RANKS_ALLREDUCE(reduce)
+            rc = self._lib.lhms_ranks_join_allreduce(self._h, rank, world, cb, rcb, None, err, 512)
+            if rc == 0:
+                self._ranks_reduce_cb = rcb
         if rc != 0:
             raise (ValueError if rc == -2 else RuntimeError)(err.value.decode())
         self._ranks_cb = cb   # called at every collection from now on
 
     def ranks_info(self) -> dict:
         """MetricSystem::RanksInfo: rank, world (0: not joined), status of the last collection (0 summed, 1 a peer did
-        not arrive in time, 2 peers froze different buffers, 3 the exchange failed), collections summed, bytes read
-        from peers by the last all-reduce, and names left out of the job-wide unions by the bounds."""
+        not arrive in time, 2 peers froze different buffers, 3 the exchange failed, 4 the allreduce passed to join_ranks
+        raised), collections summed, bytes read from peers by the last all-reduce (8 x n_words through an allreduce),
+        and names left out of the job-wide unions by the bounds."""
         out = (C.c_uint64 * 6)()
         self._lib.lhms_ranks_info(self._h, out)
         keys = ("rank", "world", "status", "summed", "bytes_from_peers", "names_dropped")
