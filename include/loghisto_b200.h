@@ -543,6 +543,43 @@ LH_STATIC_ASSERT(sizeof(lh_gauge_src) == 16 && offsetof(lh_gauge_src, dtype) == 
                  offsetof(lh_gauge_src, reserved) == 12, "lh_gauge_src is 16 bytes: d_value, dtype, reserved");
 LH_API lh_status lh_gauges_read(lh_ctx *ctx, const lh_gauge_src *h_srcs, uint32_t n, double *h_out);
 
+/* ---- distribution gauges: a device array's current values as one histogram, once per collection -----------------
+ * lh_snapshot_ingest_arrays records every element x of n_srcs device arrays, one per lh_array_src, as a sample
+ * float64(x) of its histogram_id, into the interval the open snapshot froze.  It is stateless: the registry of names
+ * lives in the caller (MetricSystem::RegisterDeviceDistribution), which calls it once per collection.
+ *
+ *   Values    each element is converted as lh_gauges_read converts a gauge (Go's float64(x)) and counted as one
+ *             Histogram(name, float64(x)) would count it.  The samples join every other sample of that id in the
+ *             frozen interval, and every reader of the snapshot sees them.
+ *   Loads     each element is read with one naturally aligned strong load (ld.relaxed.gpu) of its width, so an
+ *             element written by a single aligned store is never torn.
+ *   Ordering  the kernels are enqueued on the context's snapshot stream only, into the frozen rows.  They never wait for
+ *             ingest streams, record scopes, graph replays or any caller stream: they read whatever is in memory when
+ *             they run, as a Go gauge function reads the current state.  The call does not wait for them.
+ *   Checks    everything is validated before the state check and before anything is launched; on a failed check
+ *             nothing is launched: h_srcs NULL with n_srcs > 0, an unknown dtype, and, for an array with n > 0, a NULL
+ *             or not naturally aligned d_values, a d_values that is not device or managed memory of the context's
+ *             device, or a range [d_values, d_values + n * size) that does not lie inside one allocation
+ *             (cuMemGetAddressRange) return LH_ERR_INVALID; a histogram_id >= max_histograms returns LH_ERR_RANGE.  The
+ *             range check is what keeps the kernel from ever reading past an allocation.
+ *   State     then LH_ERR_STATE unless a snapshot is open (lh_snapshot_begin) and nothing has read its rows yet:
+ *             reduce (sync or async), export, copy_histogram, rows, row_levels, pack_rows, the all-reduces, publish,
+ *             publish_raw and lh_snapshot_device all read them.  Call it right after lh_snapshot_begin.
+ *   Sizes     n_srcs == 0, or every n == 0, returns LH_OK with no launch.  One launch takes up to 1 024 arrays and as
+ *             many samples as its CTAs' uint32 tables allow; longer tables and arrays are split across launches.
+ *   Counting  lh_stats.samples grows by the sum of n.  The call is not an ingest: it takes no ingest sequence number
+ *             and no kernel timing.
+ * A collection is never captured, so neither is this call. */
+typedef struct lh_array_src {
+    const void *d_values;                     /* n elements of dtype, in one allocation of the context's device */
+    uint64_t n;
+    uint32_t dtype;                           /* LH_GAUGE_* */
+    uint32_t histogram_id;
+} lh_array_src;
+LH_STATIC_ASSERT(sizeof(lh_array_src) == 24 && offsetof(lh_array_src, n) == 8 && offsetof(lh_array_src, dtype) == 16 &&
+                 offsetof(lh_array_src, histogram_id) == 20, "lh_array_src is 24 bytes: d_values, n, dtype, histogram_id");
+LH_API lh_status lh_snapshot_ingest_arrays(lh_ctx *ctx, const lh_array_src *h_srcs, uint32_t n_srcs);
+
 /* ---- GPU timers: StartTimer / Stop (metrics.go:232-246) from host code, timed on the device ------------------
  * Host StartTimer / Stop around CUDA work time the enqueue.  These calls put the two ends of the span on the GPU
  * instead: each end is a one-thread kernel on `stream` that reads %globaltimer (the clock of lh::start_timer), and

@@ -161,6 +161,12 @@ class lh_gauge_src(C.Structure):
     _fields_ = [("d_value", C.c_void_p), ("dtype", C.c_uint32), ("reserved", C.c_uint32)]
 
 
+class lh_array_src(C.Structure):
+    """One array of lh_snapshot_ingest_arrays: n elements of dtype LH_GAUGE_* at d_values, recorded under
+    histogram_id (include/loghisto_b200.h)."""
+    _fields_ = [("d_values", C.c_void_p), ("n", C.c_uint64), ("dtype", C.c_uint32), ("histogram_id", C.c_uint32)]
+
+
 _vp, _sz, _u32, _u64, _i32 = C.c_void_p, C.c_size_t, C.c_uint32, C.c_uint64, C.c_int32
 
 # name -> (restype, argtypes); every symbol include/loghisto_b200.h declares
@@ -217,6 +223,7 @@ SIGNATURES = {
     "lh_raw_ranks_grid": (_i32, [_vp, C.POINTER(lh_raw_board), _vp, _u32, _vp, _vp, _vp, _vp]),
     "lh_raw_board_destroy": (_i32, [_vp, C.POINTER(lh_raw_board)]),
     "lh_gauges_read": (_i32, [_vp, C.POINTER(lh_gauge_src), _u32, _vp]),
+    "lh_snapshot_ingest_arrays": (_i32, [_vp, C.POINTER(lh_array_src), _u32]),
     "lh_gpu_timer_start": (_i32, [_vp, _vp, C.POINTER(lh_gpu_timer)]),
     "lh_gpu_timer_stop": (_i32, [_vp, C.POINTER(lh_gpu_timer), _u32, _vp, _vp]),
     "lh_gpu_timer_release": (_i32, [_vp, C.POINTER(lh_gpu_timer)]),

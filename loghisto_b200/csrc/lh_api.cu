@@ -6,6 +6,8 @@
 #include "../../include/loghisto_b200.h"
 #include "lh_kernels.cuh"
 
+#include <cuda.h>   // driver types of cuMemGetAddressRange only: the library does not link libcuda
+
 #include <algorithm>
 #include <cmath>
 #include <condition_variable>
@@ -227,6 +229,7 @@ struct lh_ctx {
     Buffer buf[2];
     int active = 0;
     bool frozen = false;
+    bool rows_read = false;              // a reader has read the frozen rows (rows_read()): too late to add to them
     bool freezing = false;               // lh_snapshot_begin flipped the buffers and waits for record scopes to end
     bool nnz_valid = false;
     DevPtr<double> d_decomp;
@@ -353,6 +356,8 @@ struct lh_ctx {
     uint32_t gauge_cap = 0;
     Event gauge_done;
     GaugeParams gauge_prm{};
+    // distribution gauges (lh_snapshot_ingest_arrays): the parameter block of k_ingest_arrays (filled under the lock)
+    ArrayParams array_prm{};
     // stats
     lh_stats stats{};
     std::mutex mu;
@@ -390,6 +395,10 @@ struct RelaxedCapture {
         cudaError_t _e = (call);                                                \
         if (_e != cudaSuccess) return fail((ctx), LH_ERR_CUDA, #call, _e);      \
     } while (0)
+
+// Every reader of the open snapshot's rows calls this before it reads them: lh_snapshot_ingest_arrays may add to the
+// rows only until then, so that every reader of one snapshot sees the same interval.
+void mark_rows_read(lh_ctx *ctx) { ctx->rows_read = true; }
 
 // order `s` after the zeroing of buffer b, and remember `s` as a writer of b
 lh_status before_write(lh_ctx *ctx, int b, cudaStream_t s) {
@@ -1263,6 +1272,8 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
         // k_ingest_keyed_graph: the same launch bounds and table, so the same occupancy and grid (batch_grid_max)
         LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_ingest_keyed_graph<unsigned short>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
         LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_ingest_keyed_graph<unsigned int>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
+        // k_ingest_arrays (lh_snapshot_ingest_arrays): likewise
+        LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_ingest_arrays, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
     }
     LH_CREATE_CUDA(cudaStreamSynchronize(ctx->snap_stream.get()));
 #undef LH_CREATE_CUDA
@@ -2003,6 +2014,7 @@ extern "C" lh_status lh_snapshot_begin(lh_ctx *ctx) {
     }
     ctx->active = f ^ 1;
     ctx->frozen = true;
+    ctx->rows_read = false;
     ctx->pub_slot = -1;
     ctx->nnz_valid = false;
     ctx->view_reduced = false;
@@ -2016,6 +2028,7 @@ extern "C" lh_status lh_snapshot_device(lh_ctx *ctx, lh_device_view *out) {
     LH_ENTER(ctx);
     if (!out) return fail(ctx, LH_ERR_INVALID, "out is NULL");
     if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
+    mark_rows_read(ctx);   // the caller may read the rows from here on
     const int f = ctx->active ^ 1;
     out->d_buckets = reinterpret_cast<uint64_t *>(ctx->buf[f].d_buckets.get());
     out->d_counters = reinterpret_cast<uint64_t *>(ctx->buf[f].d_counters.get());
@@ -2057,6 +2070,7 @@ uint32_t k3_smem_cells(uint32_t win) {
 
 // enqueue K3 + one packed D2H for the open snapshot into result slot `slot`
 lh_status enqueue_reduce(lh_ctx *ctx, const double *ps, uint32_t np, int slot) {
+    mark_rows_read(ctx);
     cudaStream_t s = ctx->snap_stream.get();
     const ResLayout l = res_layout(ctx->H, np);
     const View v = snapshot_view(ctx);
@@ -2146,6 +2160,7 @@ extern "C" lh_status lh_snapshot_export(lh_ctx *ctx, lh_sparse *out) {
     LH_ENTER(ctx);
     if (!out) return fail(ctx, LH_ERR_INVALID, "out is NULL");
     if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
+    mark_rows_read(ctx);
     cudaStream_t s = ctx->snap_stream.get();
     const View v = snapshot_view(ctx);
     if (!ctx->nnz_valid) {
@@ -2193,6 +2208,7 @@ extern "C" lh_status lh_snapshot_copy_histogram(lh_ctx *ctx, uint32_t hid, uint6
     if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
     if (hid >= ctx->H) return fail(ctx, LH_ERR_RANGE, "histogram_id >= max_histograms");
     if (!h_out) return fail(ctx, LH_ERR_INVALID, "h_out is NULL");
+    mark_rows_read(ctx);
     const View v = snapshot_view(ctx);
     LH_CUDA(ctx, cudaMemcpyAsync(h_out, v.buckets + (size_t)hid * 65536u, 65536 * 8, cudaMemcpyDeviceToHost, ctx->snap_stream.get()));
     LH_CUDA(ctx, cudaStreamSynchronize(ctx->snap_stream.get()));
@@ -2426,6 +2442,7 @@ extern "C" lh_status lh_snapshot_publish_raw(lh_ctx *ctx, const lh_raw_board *b,
     const bool windowed = rb->window > 1;
     if (windowed && rb->snapshot == ctx->stats.snapshots)   // the interval would be counted twice
         return fail(ctx, LH_ERR_STATE, "a window board takes one publish per snapshot");
+    mark_rows_read(ctx);
     const View v = snapshot_view(ctx);
     cudaStream_t s = ctx->snap_stream.get();
     RawPublishParams &p = ctx->raw_prm;
@@ -2530,23 +2547,26 @@ namespace {
 constexpr uint32_t kGaugeBytes[] = {8, 4, 2, 2, 8, 4, 8};   // by LH_GAUGE_*
 static_assert(sizeof(GaugeEntry) == sizeof(lh_gauge_src), "one table entry per lh_gauge_src");
 
+constexpr uint32_t kGaugeKinds = sizeof kGaugeBytes / sizeof kGaugeBytes[0];
+
 // LH_OK when k_gauge_read may load the entry: a known dtype, a naturally aligned address in device or managed memory of
-// the context's device.  Anything else could fault the kernel, so it is refused before any launch.
-lh_status check_gauge(lh_ctx *ctx, uint32_t i, const lh_gauge_src &s) {
+// the context's device.  Anything else could fault the kernel, so it is refused before any launch.  `kind` and i name
+// the entry in the error ("gauge 3", "array 3").
+lh_status check_gauge(lh_ctx *ctx, const char *kind, uint32_t i, const lh_gauge_src &s) {
     char what[160];
-    if (s.dtype >= sizeof kGaugeBytes / sizeof kGaugeBytes[0] || s.reserved) {
-        snprintf(what, sizeof what, "gauge %u: unknown dtype %u or non-zero reserved", i, s.dtype);
+    if (s.dtype >= kGaugeKinds || s.reserved) {
+        snprintf(what, sizeof what, "%s %u: unknown dtype %u or non-zero reserved", kind, i, s.dtype);
         return fail(ctx, LH_ERR_INVALID, what);
     }
     if (!s.d_value || ((uintptr_t)s.d_value & (kGaugeBytes[s.dtype] - 1u))) {
-        snprintf(what, sizeof what, "gauge %u: d_value is NULL or not %u-byte aligned", i, kGaugeBytes[s.dtype]);
+        snprintf(what, sizeof what, "%s %u: address is NULL or not %u-byte aligned", kind, i, kGaugeBytes[s.dtype]);
         return fail(ctx, LH_ERR_INVALID, what);
     }
     cudaPointerAttributes a{};
     const cudaError_t e = cudaPointerGetAttributes(&a, s.d_value);
     if (e != cudaSuccess) cudaGetLastError();
     if (e != cudaSuccess || (a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != ctx->device) {
-        snprintf(what, sizeof what, "gauge %u: d_value is not device or managed memory of device %d", i, ctx->device);
+        snprintf(what, sizeof what, "%s %u: address is not device or managed memory of device %d", kind, i, ctx->device);
         return fail(ctx, LH_ERR_INVALID, what);
     }
     return LH_OK;
@@ -2559,7 +2579,7 @@ extern "C" lh_status lh_gauges_read(lh_ctx *ctx, const lh_gauge_src *h_srcs, uin
     LH_ENTER(ctx);
     if (n && (!h_srcs || !h_out)) return fail(ctx, LH_ERR_INVALID, "h_srcs / h_out is NULL");
     for (uint32_t i = 0; i < n; i++)
-        if (lh_status st = check_gauge(ctx, i, h_srcs[i]); st != LH_OK) return st;
+        if (lh_status st = check_gauge(ctx, "gauge", i, h_srcs[i]); st != LH_OK) return st;
     if (n == 0) return LH_OK;
     if (n > ctx->gauge_cap) {
         const uint32_t cap = std::max<uint32_t>(n, 4096);
@@ -2591,6 +2611,117 @@ extern "C" lh_status lh_gauges_read(lh_ctx *ctx, const lh_gauge_src *h_srcs, uin
     _lk.lock();
     if (e != cudaSuccess) return fail(ctx, LH_ERR_CUDA, "cudaEventSynchronize(gauges)", e);
     memcpy(h_out, ctx->h_gauges.get(), (size_t)n * 8u);
+    return LH_OK;
+}
+
+// =========================================================== distribution gauges
+namespace {
+static_assert(sizeof(ArraySeg) == 16, "k_ingest_arrays' table entry");
+using MemGetAddressRange = CUresult (*)(CUdeviceptr *, size_t *, CUdeviceptr);
+
+// cuMemGetAddressRange of the driver the runtime uses (the library does not link libcuda); nullptr when it has none
+MemGetAddressRange mem_get_address_range() {
+    static const MemGetAddressRange fn = [] {
+        void *p = nullptr;
+        cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+        if (cudaGetDriverEntryPoint("cuMemGetAddressRange", &p, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess) {
+            cudaGetLastError();
+            return (MemGetAddressRange) nullptr;
+        }
+        return reinterpret_cast<MemGetAddressRange>(p);
+    }();
+    return fn;
+}
+
+// LH_OK when k_ingest_arrays may load every element of the entry: a known dtype and, when it has elements, check_gauge's
+// checks on its first element, an id below max_histograms, and all n elements inside the allocation that holds the
+// first one.  A base address alone would let the kernel read past the end of its allocation.
+lh_status check_array(lh_ctx *ctx, uint32_t i, const lh_array_src &a) {
+    char what[192];
+    if (a.dtype >= kGaugeKinds) {
+        snprintf(what, sizeof what, "array %u: unknown dtype %u", i, a.dtype);
+        return fail(ctx, LH_ERR_INVALID, what);
+    }
+    if (a.n == 0) return LH_OK;
+    if (lh_status st = check_gauge(ctx, "array", i, lh_gauge_src{a.d_values, a.dtype, 0u}); st != LH_OK) return st;
+    if (a.histogram_id >= ctx->H) {
+        snprintf(what, sizeof what, "array %u: histogram_id %u >= max_histograms", i, a.histogram_id);
+        return fail(ctx, LH_ERR_RANGE, what);
+    }
+    const MemGetAddressRange range = mem_get_address_range();
+    const CUdeviceptr p = (CUdeviceptr)(uintptr_t)a.d_values;
+    CUdeviceptr base = 0;
+    size_t bytes = 0;
+    if (!range || range(&base, &bytes, p) != CUDA_SUCCESS || p < base ||
+        a.n > (uint64_t)(base + bytes - p) / kGaugeBytes[a.dtype]) {
+        snprintf(what, sizeof what, "array %u: its %llu elements of %u bytes do not lie inside one allocation", i,
+                 (unsigned long long)a.n, kGaugeBytes[a.dtype]);
+        return fail(ctx, LH_ERR_INVALID, what);
+    }
+    return LH_OK;
+}
+
+// Validated arrays into the rows of `target` on s: as few launches of k_ingest_arrays as the parameter block and the
+// uint32 table counts allow (launch_batch's packing); an array that does not fit the launch being filled is split
+// across launches.  The caller counts the samples in stats.
+lh_status launch_arrays(lh_ctx *ctx, const lh_recorder &target, const lh_array_src *srcs, uint32_t n_srcs, cudaStream_t s) {
+    ArrayParams &prm = ctx->array_prm;
+    prm.rec = target;
+    const int grid_max = batch_grid_max(ctx);
+    const unsigned long long cap = launch_cap(grid_max);
+    uint32_t k = 0;
+    unsigned long long total = 0;
+    auto launch = [&]() -> lh_status {
+        if (!k) return LH_OK;
+        prm.n_items = k;
+        const unsigned long long pieces = (total + BI_PIECE - 1) / BI_PIECE;
+        const int grid = (int)std::min<unsigned long long>((unsigned long long)grid_max, pieces);
+        k_ingest_arrays<<<grid, BI_THREADS, BlockRecorder::smem_bytes(BI_TABLE_ENTRIES), s>>>(prm);
+        LH_CUDA(ctx, cudaGetLastError());
+        ctx->stats.kernel_launches++;
+        k = 0;
+        total = 0;
+        return LH_OK;
+    };
+    for (uint32_t i = 0; i < n_srcs; i++) {
+        const lh_array_src &a = srcs[i];
+        const char *p = (const char *)a.d_values;
+        unsigned long long left = a.n;
+        while (left) {
+            if (k == (uint32_t)BI_MAX_ITEMS || total == cap) {
+                lh_status st = launch();
+                if (st != LH_OK) return st;
+            }
+            const unsigned long long m = std::min(left, cap - total);
+            prm.seg[k] = ArraySeg{p, a.histogram_id, a.dtype};
+            prm.start[k] = total;
+            total += m;
+            prm.start[k + 1] = total;
+            k++;
+            p += m * kGaugeBytes[a.dtype];
+            left -= m;
+        }
+    }
+    return launch();
+}
+}  // namespace
+
+extern "C" lh_status lh_snapshot_ingest_arrays(lh_ctx *ctx, const lh_array_src *h_srcs, uint32_t n_srcs) {
+    LH_ENTER(ctx);
+    if (n_srcs && !h_srcs) return fail(ctx, LH_ERR_INVALID, "h_srcs is NULL");
+    unsigned long long total = 0;
+    for (uint32_t i = 0; i < n_srcs; i++) {
+        if (lh_status st = check_array(ctx, i, h_srcs[i]); st != LH_OK) return st;
+        total += h_srcs[i].n;
+    }
+    if (!ctx->frozen || ctx->rows_read)
+        return fail(ctx, LH_ERR_STATE, "lh_snapshot_ingest_arrays needs an open snapshot whose rows nothing has read yet");
+    if (total == 0) return LH_OK;
+    // after lh_snapshot_begin's writer waits, graph drain and hot-window fold, all on the snapshot stream
+    lh_status st = launch_arrays(ctx, buffer_target(ctx, ctx->active ^ 1), h_srcs, n_srcs, ctx->snap_stream.get());
+    if (st != LH_OK) return st;
+    ctx->stats.samples += total;
     return LH_OK;
 }
 
@@ -2801,6 +2932,7 @@ void k5_launch(int grid, size_t smem, cudaStream_t s, const PeerParams &p, const
 template <typename Rows>
 lh_status launch_allreduce(lh_ctx *ctx, uint64_t seq, const uint32_t *frozen, uint32_t n_rows, uint32_t include_counters,
                            Rows rows, uint64_t *seq_out) {
+    mark_rows_read(ctx);
     const int f = ctx->active ^ 1;
     cudaStream_t s = ctx->snap_stream.get();
     // status and cells describe this all-reduce only: zeroed behind the previous one on the same stream
@@ -2869,6 +3001,7 @@ extern "C" lh_status lh_snapshot_rows(lh_ctx *ctx, uint8_t *hist_touched, uint64
     LH_ENTER(ctx);
     if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
     if (ctx->view_reduced) return fail(ctx, LH_ERR_STATE, "this snapshot has already been all-reduced");
+    mark_rows_read(ctx);
     const int f = ctx->active ^ 1;
     cudaStream_t s = ctx->snap_stream.get();
     if (lh_status st = alloc_rows_staging(ctx)) return st;
@@ -2929,6 +3062,7 @@ extern "C" lh_status lh_snapshot_row_levels(lh_ctx *ctx, uint8_t *levels) {
     if (!ctx->frozen) return fail(ctx, LH_ERR_STATE, "no snapshot in progress");
     if (ctx->view_reduced) return fail(ctx, LH_ERR_STATE, "this snapshot has already been all-reduced");
     if (!levels) return fail(ctx, LH_ERR_INVALID, "levels is NULL");
+    mark_rows_read(ctx);
     if (lh_status st = alloc_rows_staging(ctx)) return st;
     cudaStream_t s = ctx->snap_stream.get();
     LH_CUDA(ctx, cudaMemcpyAsync(ctx->h_rows_flags.get(), ctx->buf[ctx->active ^ 1].d_flags.get(), (size_t)ctx->H * 4, cudaMemcpyDeviceToHost, s));
@@ -2959,6 +3093,7 @@ extern "C" lh_status lh_snapshot_pack_rows(lh_ctx *ctx, uint32_t n_rows, const u
         if (hist_rows[g] != LH_ROW_ABSENT && hist_rows[g] >= ctx->H) return fail(ctx, LH_ERR_RANGE, "histogram row >= max_histograms");
     for (uint32_t g = 0; g < n_counter_rows; g++)
         if (counter_rows[g] != LH_ROW_ABSENT && counter_rows[g] >= ctx->C) return fail(ctx, LH_ERR_RANGE, "counter row >= max_counters");
+    mark_rows_read(ctx);
     const size_t table_bytes = (size_t)ctx->H * sizeof(RowsEntry) + (size_t)ctx->C * 4;
     if (!ctx->d_rows_table.get()) {
         DevPtr<unsigned char> d; PinnedPtr<unsigned char> h; Event copied;

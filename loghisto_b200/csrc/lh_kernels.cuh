@@ -22,6 +22,8 @@
 //   K6   k_scatter_segments, k_sparse_epilogue   caller-supplied sparse histograms -> scratch rows -> K3
 //                               (lh_reduce_sparse_host)
 //   k_ingest_batch          many device arrays under many ids (lh_ingest_batch, lh_graph_recorder_ingest)
+//   k_ingest_arrays         every element of device arrays of any gauge dtype -> the frozen interval (distribution
+//                           gauges, lh_snapshot_ingest_arrays)
 //   k_ingest_keyed_graph    (id,value) pairs into a graph recorder's rows (lh_graph_recorder_ingest_keyed_*)
 //   k_graph_drain           graph recorders' rows -> the interval being frozen (lh_snapshot_begin)
 //   k_raw_publish, k_raw_publish_window, k_raw_percentiles, k_raw_ranks   running bucket counts of a snapshot (or of
@@ -2410,6 +2412,28 @@ __device__ __forceinline__ double f32(float x) {   // exact, subnormals kept (no
     asm("cvt.f64.f32 %0, %1;" : "=d"(d) : "f"(x));
     return d;
 }
+// The value at p of dtype LH_GAUGE_* (checked on the host) as Go's float64(x): one strong load of its width, then the
+// conversion.  The one place both k_gauge_read and k_ingest_arrays take a value from.
+__device__ __forceinline__ double load(const void *p, uint32_t dtype) {
+    double v;
+    switch (dtype) {
+    case LH_GAUGE_F64: v = __longlong_as_double((long long)ld64(p)); break;
+    case LH_GAUGE_F32: v = f32(__uint_as_float(ld32(p))); break;
+    case LH_GAUGE_F16: {
+        float f;
+        asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(ld16(p)));
+        v = f32(f);
+        break;
+    }
+    case LH_GAUGE_BF16: v = f32(__uint_as_float((uint32_t)ld16(p) << 16)); break;
+    case LH_GAUGE_I64: asm("cvt.rn.f64.s64 %0, %1;" : "=d"(v) : "l"(ld64(p))); break;
+    case LH_GAUGE_I32: asm("cvt.rn.f64.s32 %0, %1;" : "=d"(v) : "r"(ld32(p))); break;
+    default: asm("cvt.rn.f64.u64 %0, %1;" : "=d"(v) : "l"(ld64(p))); break;   // LH_GAUGE_U64
+    }
+    return v;
+}
+// log2 of the element size of dtype LH_GAUGE_*: one nibble per dtype, F64 in the lowest (8 4 2 2 8 4 8 bytes)
+__device__ __forceinline__ uint32_t shift(uint32_t dtype) { return (0x3231123u >> (4u * dtype)) & 15u; }
 }  // namespace gauge
 
 __global__ void __launch_bounds__(GR_THREADS)
@@ -2417,22 +2441,65 @@ k_gauge_read(const __grid_constant__ GaugeParams p) {
     const uint32_t i = blockIdx.x * GR_THREADS + threadIdx.x;
     if (i >= p.n) return;
     const GaugeEntry e = p.e[i];
-    double v;
-    switch (e.dtype) {
-    case LH_GAUGE_F64: v = __longlong_as_double((long long)gauge::ld64(e.p)); break;
-    case LH_GAUGE_F32: v = gauge::f32(__uint_as_float(gauge::ld32(e.p))); break;
-    case LH_GAUGE_F16: {
-        float f;
-        asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(gauge::ld16(e.p)));
-        v = gauge::f32(f);
-        break;
+    p.out[i] = gauge::load(e.p, e.dtype);
+}
+
+// ----------------------------------------------------------- distribution gauges (lh_snapshot_ingest_arrays)
+// Every element of many device arrays, each of dtype LH_GAUGE_* under its own histogram id, into the frozen interval's
+// rows.  The work is k_ingest_batch's: the item table travels in the parameter block, the items' concatenation is cut
+// into BI_PIECE-sample pieces dealt round-robin to the CTAs, each thread walks its piece across item boundaries, and
+// every CTA counts through one lh::BlockRecorder of BI_TABLE_ENTRIES entries, flushed once.  Only the sample load
+// differs: an element is read as a device gauge is (gauge::load), so a value written by one aligned store is never
+// torn.  The host bounds a launch's samples as it bounds k_ingest_batch's (no CTA counts more than 2^31 of them).
+struct ArraySeg {
+    const void *vals;                        // dtype-aligned, the whole item inside one allocation (checked on the host)
+    uint32_t id;
+    uint32_t dtype;                          // LH_GAUGE_*
+};
+struct ArrayParams {
+    lh_recorder rec;                         // the frozen interval's rows
+    uint32_t n_items;
+    uint32_t pad;
+    unsigned long long start[BI_MAX_ITEMS + 1];   // prefix offsets of the items' lengths
+    ArraySeg seg[BI_MAX_ITEMS];
+};
+
+__global__ void __launch_bounds__(BI_THREADS, 2)
+k_ingest_arrays(const __grid_constant__ ArrayParams p) {
+    extern __shared__ __align__(16) unsigned char ia_smem[];
+    BlockRecorder br(p.rec, ia_smem, BI_TABLE_ENTRIES);
+    br.init();
+    const unsigned long long total = p.start[p.n_items];
+    const unsigned long long pieces = (total + BI_PIECE - 1) / BI_PIECE;
+    for (unsigned long long pc = blockIdx.x; pc < pieces; pc += gridDim.x) {
+        const unsigned long long lo = pc * BI_PIECE;
+        const unsigned long long hi = min(lo + BI_PIECE, total);
+        uint32_t a = 0, b = p.n_items - 1;   // the item holding sample lo (uniform over the CTA)
+        while (a < b) {
+            const uint32_t m = (a + b + 1) / 2;
+            if (p.start[m] <= lo) a = m; else b = m - 1;
+        }
+        uint32_t it = a;
+        for (unsigned long long g0 = lo + threadIdx.x; g0 < hi; g0 += 2 * BI_THREADS) {
+            double v[2];
+            uint32_t id[2];
+#pragma unroll
+            for (int k = 0; k < 2; k++) {
+                const unsigned long long g = g0 + k * BI_THREADS;
+                v[k] = 0.0; id[k] = 0u;
+                if (g < hi) {
+                    while (p.start[it + 1] <= g) ++it;
+                    const ArraySeg s = p.seg[it];
+                    id[k] = s.id;
+                    v[k] = gauge::load((const char *)s.vals + ((g - p.start[it]) << gauge::shift(s.dtype)), s.dtype);
+                }
+            }
+#pragma unroll
+            for (int k = 0; k < 2; k++)
+                if (g0 + k * BI_THREADS < hi) br.record(id[k], v[k]);
+        }
     }
-    case LH_GAUGE_BF16: v = gauge::f32(__uint_as_float((uint32_t)gauge::ld16(e.p) << 16)); break;
-    case LH_GAUGE_I64: asm("cvt.rn.f64.s64 %0, %1;" : "=d"(v) : "l"(gauge::ld64(e.p))); break;
-    case LH_GAUGE_I32: asm("cvt.rn.f64.s32 %0, %1;" : "=d"(v) : "r"(gauge::ld32(e.p))); break;
-    default: asm("cvt.rn.f64.u64 %0, %1;" : "=d"(v) : "l"(gauge::ld64(e.p))); break;   // LH_GAUGE_U64
-    }
-    p.out[i] = v;
+    br.flush();
 }
 
 // ----------------------------------------------------------- raw device subscriptions (lh_raw_*, lh_snapshot_publish_raw)

@@ -403,6 +403,21 @@ def gauge_src(t, device: int) -> tuple:
     return int(t.data_ptr()), dtype
 
 
+def array_src(t, device: int, histogram_id: int = 0) -> L.lh_array_src:
+    """lh_array_src of a distribution gauge: a contiguous CUDA tensor of any shape on `device`, of dtype float64 /
+    float32 / float16 / bfloat16 / int64 / int32 / uint64, recorded under `histogram_id`.  TypeError otherwise."""
+    if not (hasattr(t, "is_cuda") and hasattr(t, "data_ptr")):
+        raise TypeError(f"a distribution gauge is a CUDA tensor, not {type(t)!r}")
+    if not t.is_cuda or t.device.index != device:
+        raise TypeError(f"a distribution gauge must be on cuda:{device}, not {t.device}")
+    if not t.is_contiguous():
+        raise TypeError("a distribution gauge must be a contiguous tensor")
+    dtype = _GAUGE_DTYPES.get(str(t.dtype))
+    if dtype is None:
+        raise TypeError(f"a distribution gauge must be float64/32/16, bfloat16, int64/32 or uint64, not {t.dtype}")
+    return L.lh_array_src(int(t.data_ptr()), int(t.numel()), dtype, int(histogram_id))
+
+
 class Board:
     """A device subscription board of an Engine (Engine.board): `board` is the lh_board to pass by value to kernels,
     which read it with lh::read_histogram / lh::read_counter."""
@@ -898,6 +913,13 @@ class Engine:
     def snapshot_begin(self):
         self._check(self.lib.lh_snapshot_begin(self.h))
 
+    def snapshot_ingest_arrays(self, arrays):
+        """lh_snapshot_ingest_arrays: every element of each array as a sample of its id, into the open snapshot's
+        rows.  `arrays` holds (histogram_id, tensor) pairs (array_src) or lh_array_src entries passed as they are."""
+        arrays = [a if isinstance(a, L.lh_array_src) else array_src(a[1], self.device, a[0]) for a in arrays]
+        srcs = (L.lh_array_src * max(len(arrays), 1))(*arrays)
+        self._check(self.lib.lh_snapshot_ingest_arrays(self.h, srcs, len(arrays)))
+
     def snapshot_device(self) -> L.lh_device_view:
         v = L.lh_device_view()
         self._check(self.lib.lh_snapshot_device(self.h, C.byref(v)))
@@ -979,10 +1001,13 @@ class Engine:
                                                    sums.ctypes.data, avgs.ctypes.data, pkeys.ctypes.data, pvals.ctypes.data))
         return Reduced(out_counts, sums, avgs, pkeys, pvals)
 
-    def snapshot(self, percentiles, export: bool = True):
-        """begin + reduce (+ export) + end; returns (Reduced, Sparse | None)."""
+    def snapshot(self, percentiles, export: bool = True, arrays=None):
+        """begin (+ ingest arrays) + reduce (+ export) + end; returns (Reduced, Sparse | None).  `arrays`: what
+        snapshot_ingest_arrays takes, recorded into the interval this snapshot freezes."""
         self.snapshot_begin()
         try:
+            if arrays is not None:
+                self.snapshot_ingest_arrays(arrays)
             red = self.snapshot_reduce(percentiles)
             sp = self.snapshot_export() if export else None
         finally:

@@ -70,6 +70,8 @@
 #pragma weak lh_snapshot_row_levels
 #pragma weak lh_snapshot_pack_rows
 #pragma weak lh_snapshot_unpack_rows
+// And for distribution gauges: over a build without them, RegisterDeviceDistribution throws.
+#pragma weak lh_snapshot_ingest_arrays
 
 namespace loghisto {
 
@@ -761,6 +763,12 @@ RecordScope MetricSystem::BeginRecording(void *stream, const std::vector<std::st
     return s;
 }
 
+void MetricSystem::refuse_in_scope(const char *what) {
+    std::lock_guard<std::mutex> lk(scope_mu_);
+    if (scope_threads_.count(std::this_thread::get_id()))
+        throw std::runtime_error(std::string(what) + " from a thread that holds an open record scope");
+}
+
 void MetricSystem::end_scope(RecordScope &s) {
     const lh_status st = lh_record_end(ctx_, &s.rec_);
     {
@@ -1181,6 +1189,28 @@ void MetricSystem::DeregisterGaugeFunc(const std::string &name) {
     gauge_funcs_.erase(name);
     device_gauges_.erase(name);
 }
+void MetricSystem::RegisterDeviceDistribution(const std::string &name, const void *d_values, uint64_t n, uint32_t dtype) {
+    if (!lh_snapshot_ingest_arrays || !lh_gauges_read)
+        throw std::runtime_error("RegisterDeviceDistribution: this libloghisto_b200 has no distribution gauges");
+    if (dtype > LH_GAUGE_U64)
+        throw std::invalid_argument("RegisterDeviceDistribution(" + name + "): unknown dtype " + std::to_string(dtype));
+    if (n) {   // the first element, as RegisterDeviceGauge checks a gauge; the range is checked at every collection
+        const lh_gauge_src src{d_values, dtype, 0u};
+        double v = 0;
+        const lh_status st = lh_gauges_read(ctx_, &src, 1, &v);
+        if (st == LH_ERR_INVALID)
+            throw std::invalid_argument("RegisterDeviceDistribution(" + name + "): " + lh_last_error(ctx_));
+        check(ctx_, st, "lh_gauges_read");
+    }
+    refuse_in_scope("RegisterDeviceDistribution");   // before dist_mu_, which a collection holds across its scope wait
+    std::lock_guard<std::mutex> lk(dist_mu_);
+    device_dists_[name] = lh_array_src{d_values, n, dtype, 0u};
+}
+void MetricSystem::DeregisterDeviceDistribution(const std::string &name) {
+    refuse_in_scope("DeregisterDeviceDistribution");
+    std::lock_guard<std::mutex> lk(dist_mu_);
+    device_dists_.erase(name);
+}
 
 // commit whatever the shard holds and hand over (and clear) its touched-counter marks
 void MetricSystem::flush_shard(Shard &s, std::vector<uint8_t> *touched) {
@@ -1466,11 +1496,8 @@ void MetricSystem::sum_rows(const std::vector<uint32_t> &hmap, const std::vector
 
 // collectRawMetrics, metrics.go:420-479.
 std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
-    {   // lh_snapshot_begin would refuse the call after the flush below; refuse it before anything moves
-        std::lock_guard<std::mutex> lk(scope_mu_);
-        if (scope_threads_.count(std::this_thread::get_id()))
-            throw std::runtime_error("collectRawMetrics from a thread that holds an open record scope");
-    }
+    // lh_snapshot_begin would refuse the call after the flush below; refuse it before anything moves
+    refuse_in_scope("collectRawMetrics");
     std::lock_guard<std::mutex> snap(snapshot_mu_);
     collected_ = true;
     auto raw = std::make_shared<RawMetricSet>();
@@ -1497,10 +1524,27 @@ std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
         std::lock_guard<std::mutex> lk(graph_mu_);
         for (auto &g : graphs_) bind_graph(*g);
     }
+    // distribution gauges: every registered name interned (or revived) and used in this interval, so it keeps its id;
+    // a name with no free id has its samples dropped and counted.  dist_mu_ stays held until the reduction below has
+    // run after the arrays' kernels on the snapshot stream.
+    std::unique_lock<std::mutex> dists_held(dist_mu_);
+    std::vector<lh_array_src> dists;
+    if (!device_dists_.empty()) {
+        std::unique_lock<std::shared_mutex> wl(histos_.mu);
+        for (auto &d : device_dists_) {
+            const uint32_t id = intern_locked(histos_, d.first);
+            if (id == RecordScope::kUnbound) { dropped_over_limit_.fetch_add(d.second.n, std::memory_order_relaxed); continue; }
+            dists.push_back(d.second);
+            dists.back().histogram_id = id;
+        }
+    }
     if (const lh_status st = lh_snapshot_begin(ctx_); st != LH_OK) {   // the marks stay for the next collection
         carried_touched_ = std::move(touched);
         check(ctx_, st, "lh_snapshot_begin");
     }
+    // every array's current values join the interval just frozen, before anything reads it
+    if (!dists.empty() && lh_snapshot_ingest_arrays(ctx_, dists.data(), (uint32_t)dists.size()) != LH_OK)
+        fprintf(stderr, "loghisto: lh_snapshot_ingest_arrays failed: %s\n", lh_last_error(ctx_));   // the set is still delivered
     // the cache swaps of :425-428 and :460-463 happened in lh_snapshot_begin
 
     const uint32_t H = opt_.max_histograms, np = (uint32_t)raw->percentile_labels.size();
@@ -1518,6 +1562,7 @@ std::shared_ptr<RawMetricSet> MetricSystem::collectRawMetrics() {
         }
         check(ctx_, lh_snapshot_reduce(ctx_, ps.data(), np, counts.data(), sums.data(), avgs.data(), pkeys.data(), pvals.data()),
               "lh_snapshot_reduce");
+        dists_held.unlock();
         check(ctx_, lh_snapshot_export(ctx_, &sp), "lh_snapshot_export");
         if (joined && !allreduce_) {
             lh_comm_stats cs{};
@@ -1905,6 +1950,29 @@ LHMS_API int lhms_register_device_gauge(void *ms, const char *name, const void *
 // DeregisterGaugeFunc: removes a gauge function or a device gauge
 LHMS_API void lhms_deregister_gauge(void *ms, const char *name) {
     static_cast<MetricSystem *>(ms)->DeregisterGaugeFunc(name);
+}
+// RegisterDeviceDistribution: LH_OK, LH_ERR_INVALID when the dtype or the first element's address is refused,
+// LH_ERR_STATE for any other failure (a thread that holds an open record scope among them).
+LHMS_API int lhms_register_device_distribution(void *ms, const char *name, const void *d_values, uint64_t n, uint32_t dtype) {
+    if (!ms || !name) return LH_ERR_INVALID;
+    try {
+        static_cast<MetricSystem *>(ms)->RegisterDeviceDistribution(name, d_values, n, dtype);
+        return LH_OK;
+    } catch (const std::invalid_argument &) {
+        return LH_ERR_INVALID;
+    } catch (const std::exception &) {
+        return LH_ERR_STATE;
+    }
+}
+// DeregisterDeviceDistribution: LH_OK, or LH_ERR_STATE from a thread that holds an open record scope.
+LHMS_API int lhms_deregister_device_distribution(void *ms, const char *name) {
+    if (!ms || !name) return LH_ERR_INVALID;
+    try {
+        static_cast<MetricSystem *>(ms)->DeregisterDeviceDistribution(name);
+        return LH_OK;
+    } catch (const std::exception &) {
+        return LH_ERR_STATE;
+    }
 }
 // lh_get_stats of the system's context (e.g. the kernel launches a collection issues)
 LHMS_API int lhms_stats(void *ms, lh_stats *out) {

@@ -423,6 +423,21 @@ class MetricSystem {
     // libloghisto_b200 has no device gauges or the read fails otherwise.
     void RegisterDeviceGauge(const std::string &name, const void *d_value, uint32_t dtype);
     void DeregisterGaugeFunc(const std::string &name);                    // :306, device gauges too
+    // A distribution gauge: n values of type `dtype` (LH_GAUGE_*) at d_values, device or managed memory of this system's
+    // device, which must stay allocated while registered.  At every collection each element x is recorded as
+    // Histogram(name, float64(x)) into the interval that collection collects, read on the snapshot stream without
+    // waiting for any caller stream (lh_snapshot_ingest_arrays), so Histograms and the processed metrics carry the
+    // distribution of the array's current values.  A registered name keeps its id while registered; when no id is free
+    // at a collection, its n samples are dropped and counted.  Registering a name again replaces its array.  Throws
+    // std::invalid_argument when the dtype, or lh_gauges_read of the first element, is refused (the range is checked at
+    // each collection; a refused collection logs and delivers its set without the distributions), std::runtime_error
+    // when this libloghisto_b200 has no distribution gauges.
+    // Both calls wait for a collection in progress to finish reading the arrays, so an array is never read after
+    // DeregisterDeviceDistribution returns and may be freed then.  That collection may itself be waiting for the record
+    // scopes of the interval to end, so from a thread that holds an open record scope of this system both throw
+    // std::runtime_error instead of waiting, as collectRawMetrics does.
+    void RegisterDeviceDistribution(const std::string &name, const void *d_values, uint64_t n, uint32_t dtype);
+    void DeregisterDeviceDistribution(const std::string &name);
     void Start();                                                         // :644
     void Stop();                                                          // :651
 
@@ -532,6 +547,7 @@ class MetricSystem {
     void bind_names(NameTable &t, const std::vector<std::string> &names, std::vector<uint32_t> &ids, std::vector<uint32_t> &gens);
     bool pin_names(NameTable &t, const std::vector<uint32_t> &ids, const std::vector<uint32_t> &gens);
     void end_scope(RecordScope &s);
+    void refuse_in_scope(const char *what);   // std::runtime_error when the calling thread holds an open record scope
     std::mutex scope_mu_;
     std::unordered_map<std::thread::id, uint32_t> scope_threads_;   // open scopes per opening thread
     std::vector<uint8_t> carried_touched_;   // touched-counter marks of a collection that lh_snapshot_begin refused
@@ -575,6 +591,11 @@ class MetricSystem {
     std::mutex gauge_mu_;
     std::map<std::string, std::function<double()>> gauge_funcs_;
     std::map<std::string, lh_gauge_src> device_gauges_;   // no name is in both maps
+    // distribution gauges: name -> array (histogram_id unused), held from a collection's binding until its reduction
+    // has run, so an array deregistered (and then freed) is never read.  Only threads without an open record scope take
+    // it (refuse_in_scope): the collection holding it may wait for the scopes of its interval in lh_snapshot_begin.
+    std::mutex dist_mu_;
+    std::map<std::string, lh_array_src> device_dists_;
 
     std::mutex subscribers_mu_;
     std::vector<std::shared_ptr<Channel<std::shared_ptr<RawMetricSet>>>> raw_subscribers_;

@@ -11,7 +11,7 @@ import sys
 
 from . import _lib as _L
 from . import build as _build
-from .engine import (_batch_array, _capture_stream, _stream, _timer_stream, board_out, board_views, gauge_src,
+from .engine import (_batch_array, _capture_stream, _stream, _timer_stream, array_src, board_out, board_views, gauge_src,
                      graph_counter_args, graph_duration_out, graph_keyed_args, raw_percentiles, raw_ranks,
                      check_window)
 
@@ -52,6 +52,10 @@ def _bind(L):
     L.lhms_register_device_gauge.restype = C.c_int
     L.lhms_register_device_gauge.argtypes = [vp, C.c_char_p, vp, C.c_uint32]
     L.lhms_deregister_gauge.argtypes = [vp, C.c_char_p]
+    L.lhms_register_device_distribution.restype = C.c_int
+    L.lhms_register_device_distribution.argtypes = [vp, C.c_char_p, vp, C.c_uint64, C.c_uint32]
+    L.lhms_deregister_device_distribution.restype = C.c_int
+    L.lhms_deregister_device_distribution.argtypes = [vp, C.c_char_p]
     L.lhms_stats.restype = C.c_int
     L.lhms_stats.argtypes = [vp, C.POINTER(_L.lh_stats)]
     L.lhms_collect_and_process.restype = C.c_int
@@ -594,12 +598,14 @@ class MetricSystem:
             raise RuntimeError(err.value.decode())
         self._device = device
         self._device_gauges = {}   # name -> tensor: keeps the memory of every registered device gauge allocated
+        self._device_dists = {}    # name -> tensor: likewise for distribution gauges
 
     def close(self):
         if self._h:
             self._lib.lhms_free(self._h)
             self._h = None
             self._device_gauges.clear()
+            self._device_dists.clear()
 
     def __del__(self):
         try:
@@ -710,6 +716,31 @@ class MetricSystem:
         """Removes the gauge registered under `name`, a function or a device gauge (metrics.go:306)."""
         self._lib.lhms_deregister_gauge(self._h, name.encode())
         self._device_gauges.pop(name, None)
+
+    def RegisterDeviceDistribution(self, name: str, tensor):
+        """A distribution gauge: `tensor` is a contiguous CUDA tensor of any shape on this system's device, of dtype
+        float64 / float32 / float16 / bfloat16 / int64 / int32 / uint64 (TypeError otherwise).  At every collection
+        each element x is recorded as Histogram(name, float64(x)) into the interval collected, read without waiting for
+        any stream, so Histograms and the processed metrics carry the distribution of the tensor's current values.
+        Replaces the tensor registered under `name`.  The system keeps a reference to the tensor while it is
+        registered, so its memory is not reused.  Waits for a collection in progress; from a thread inside
+        `ms.recording(...)` it raises RuntimeError instead, since that collection may be waiting for the scope."""
+        src = array_src(tensor, self._device)
+        st = self._lib.lhms_register_device_distribution(self._h, name.encode(), src.d_values, src.n, src.dtype)
+        if st != 0:
+            raise (ValueError if st == _L.LH_ERR_INVALID else RuntimeError)(
+                "lhms_register_device_distribution refused %r (status %d)" % (name, st))
+        self._device_dists[name] = tensor
+
+    def DeregisterDeviceDistribution(self, name: str):
+        """Stops recording the distribution gauge registered under `name` (nothing when there is none).  Waits for a
+        collection in progress, so the tensor is not read after the call returns; from a thread inside
+        `ms.recording(...)` it raises RuntimeError instead."""
+        st = self._lib.lhms_deregister_device_distribution(self._h, name.encode())
+        if st != 0:
+            raise RuntimeError("lhms_deregister_device_distribution refused %r (status %d): the calling thread holds an "
+                               "open record scope" % (name, st))
+        self._device_dists.pop(name, None)
 
     def SubscribeToProcessedMetrics(self, capacity: int = 128) -> Subscription:
         return Subscription(self, "processed", capacity)
