@@ -580,6 +580,35 @@ LH_STATIC_ASSERT(sizeof(lh_array_src) == 24 && offsetof(lh_array_src, n) == 8 &&
                  offsetof(lh_array_src, histogram_id) == 20, "lh_array_src is 24 bytes: d_values, n, dtype, histogram_id");
 LH_API lh_status lh_snapshot_ingest_arrays(lh_ctx *ctx, const lh_array_src *h_srcs, uint32_t n_srcs);
 
+/* ---- stream-ordered ingest of device arrays of any gauge dtype -------------------------------------------------
+ * lh_ingest_arrays records every element x of n_srcs device arrays (lh_array_src above, dtype LH_GAUGE_*) as one
+ * Histogram(histogram_id, float64(x)), without widening the arrays to float64 first: a float32 or int32 sample is read
+ * as 4 bytes and a float16 or bfloat16 one as 2.  The conversion is lh_gauges_read's (Go's float64(x)): floats and int32
+ * exactly, subnormals kept; int64 and uint64 round to nearest even, so an LH_GAUGE_I64 array of nanoseconds counts
+ * exactly as LH_VALUES_I64NS does and an LH_GAUGE_F64 array as LH_VALUES_F64.
+ *
+ * In every other respect it is lh_ingest_batch: one write bracket and one ingest sequence number on `stream` (NULL =
+ * the context's ingest stream), every sample in one interval, lh_stats.samples += the sum of n; items may repeat ids,
+ * alias or overlap and come in any order; the call never waits for the device and allocates nothing.  The arrays are
+ * read in stream order with streaming loads and must stay valid until the stream's work completes.
+ *
+ * Routing: an F64 item of at least 2^20 samples goes to the single-histogram kernel (as in lh_ingest_batch), an F32 or
+ * I32 item of at least 2^20 to its 4-byte form, an F16 or BF16 item of at least 2^20 to its 16-bit form (a per-context
+ * key table from each 16-bit magnitude to its bucket, built at lh_create); every other item, and every I64 / U64 one,
+ * to the kernel of lh_snapshot_ingest_arrays with streaming loads.
+ *
+ * Every item is validated before anything is enqueued; on error nothing is launched, counted or sequenced:
+ * LH_ERR_INVALID for h_srcs NULL with n_srcs > 0 or an unknown dtype, and, for an item with n > 0, d_values NULL or not
+ * naturally aligned for its dtype; LH_ERR_RANGE for an item with n > 0 and histogram_id >= max_histograms.  The memory
+ * kind and the allocation range are not checked (the arrays are read in stream order, as lh_ingest_batch's are).
+ *
+ * lh_graph_recorder_ingest_arrays is lh_ingest_arrays into a graph recorder's rows (as lh_graph_recorder_ingest is
+ * lh_ingest_batch): kernels only, capturable, ids local (histogram_id >= the recorder's k returns LH_ERR_RANGE), no
+ * bracket, sequence number or sample tally. */
+LH_API lh_status lh_ingest_arrays(lh_ctx *ctx, const lh_array_src *h_srcs, uint32_t n_srcs, void *stream);
+LH_API lh_status lh_graph_recorder_ingest_arrays(lh_ctx *ctx, const lh_graph_recorder *g, const lh_array_src *h_srcs,
+                                                 uint32_t n_srcs, void *stream);
+
 /* ---- GPU timers: StartTimer / Stop (metrics.go:232-246) from host code, timed on the device ------------------
  * Host StartTimer / Stop around CUDA work time the enqueue.  These calls put the two ends of the span on the GPU
  * instead: each end is a one-thread kernel on `stream` that reads %globaltimer (the clock of lh::start_timer), and

@@ -224,6 +224,8 @@ SIGNATURES = {
     "lh_raw_board_destroy": (_i32, [_vp, C.POINTER(lh_raw_board)]),
     "lh_gauges_read": (_i32, [_vp, C.POINTER(lh_gauge_src), _u32, _vp]),
     "lh_snapshot_ingest_arrays": (_i32, [_vp, C.POINTER(lh_array_src), _u32]),
+    "lh_ingest_arrays": (_i32, [_vp, C.POINTER(lh_array_src), _u32, _vp]),
+    "lh_graph_recorder_ingest_arrays": (_i32, [_vp, C.POINTER(lh_graph_recorder), C.POINTER(lh_array_src), _u32, _vp]),
     "lh_gpu_timer_start": (_i32, [_vp, _vp, C.POINTER(lh_gpu_timer)]),
     "lh_gpu_timer_stop": (_i32, [_vp, C.POINTER(lh_gpu_timer), _u32, _vp, _vp]),
     "lh_gpu_timer_release": (_i32, [_vp, C.POINTER(lh_gpu_timer)]),

@@ -154,6 +154,51 @@ K1Variant g_k1_variants[] = {
     BULK_VARIANT(16, 3, 65536, 1, 0),   // 6
 };
 constexpr int kNumK1Variants = (int)(sizeof(g_k1_variants) / sizeof(g_k1_variants[0]));
+
+// The narrow forms of K1 that lh_ingest_arrays routes long float32 / int32 (4-byte form) and float16 / bfloat16
+// (16-bit form, key table) items to.  One shape each, chosen to fit kSmemBudget beside the sub-histogram at every
+// precision 1..250 (87 KB at 250): 4 x 32 KiB stages for the 4-byte form, 2 x 32 KiB plus the 64 KiB key table for
+// the 16-bit form; 16 consumer warps, negatives folded into the slot.
+constexpr int kK1nCW = 16, kK1nStage = 32768;
+constexpr int kK1nStages4 = 4, kK1nStages2 = 2;
+struct K1Narrow {
+    void (*launch)(int grid, size_t smem, cudaStream_t s, const void *v32, size_t nvec, const void *head, int nhead,
+                   const void *tail, int ntail, unsigned long long *counts, uint32_t *flag, const Prec &pc,
+                   const uint16_t *keys);
+    const void *func;
+    uint32_t bytes;      // element size
+    size_t smem_fixed;   // ring + barriers (+ key table)
+    int blocks_per_sm;   // filled at create
+    size_t smem;         // filled at create
+};
+template <typename Cv, int STAGES>
+void launch_narrow(int grid, size_t smem, cudaStream_t s, const void *v32, size_t nvec, const void *head, int nhead,
+                   const void *tail, int ntail, unsigned long long *counts, uint32_t *flag, const Prec &pc,
+                   const uint16_t *keys) {
+    using T = typename Cv::T;
+    k_ingest_single_bulk<kK1nCW, STAGES, kK1nStage, 1, true, Cv><<<grid, (kK1nCW + 1) * 32, smem, s>>>(
+        (const T *)v32, nvec, (const T *)head, nhead, (const T *)tail, ntail, counts, flag, pc, keys);
+}
+#define NARROW_FORM(CV, S, TABLE) \
+    { launch_narrow<CV, S>, (const void *)k_ingest_single_bulk<kK1nCW, S, kK1nStage, 1, true, CV>, \
+      (uint32_t)sizeof(CV::T), (size_t)S * (kK1nStage + 16) + (TABLE), 0, 0 }
+const K1Narrow g_k1_narrow[4] = {   // by k1n_index
+    NARROW_FORM(K1F32, kK1nStages4, 0),
+    NARROW_FORM(K1I32, kK1nStages4, 0),
+    NARROW_FORM(K1F16, kK1nStages2, 65536),
+    NARROW_FORM(K1BF16, kK1nStages2, 65536),
+};
+#undef NARROW_FORM
+// index into g_k1_narrow of dtype LH_GAUGE_*, -1: no narrow form (F64 takes K1 itself, I64 / U64 k_ingest_arrays)
+int k1n_index(uint32_t dtype) {
+    switch (dtype) {
+    case LH_GAUGE_F32: return 0;
+    case LH_GAUGE_I32: return 1;
+    case LH_GAUGE_F16: return 2;
+    case LH_GAUGE_BF16: return 3;
+    default: return -1;
+    }
+}
 constexpr int kDefaultK1Variant = 6;   // 3 x 64 KB stages, negatives through the fix-up: best sustained time of the bulk variants (within 2 % of each other on H100)
 
 // Everything the kernels derive from `precision` (metrics.go:40-43), see lh_device.cuh.
@@ -318,6 +363,10 @@ struct lh_ctx {
     DevPtr<uint32_t> d_rs_flags, d_rs_nnz;
     bool rs_dirty = false;                        // a call failed part-way: zero the rows before the next one
     K1Variant k1[kNumK1Variants];
+    // lh_ingest_arrays: the narrow forms of K1 (by K1Narrow index, occupancy filled at create) and the key tables of
+    // the 16-bit form ([2][32768] uint16, k_fill_key16: float16, then bfloat16)
+    K1Narrow k1n[4];
+    DevPtr<uint16_t> d_key16;
     // timing of ingest: CUDA events bracket the kernels of every write_bracket (one sequence number); a ring keeps the
     // last kTimingRing pairs
     static constexpr int kTimingRing = 16;
@@ -435,13 +484,14 @@ int ingest_sms(const lh_ctx *ctx) { return std::max(1, ctx->sm_count - ctx->k1_r
 // Samples one launch of `grid` CTAs may take when each CTA counts into uint32 cells of its own (K1's sub-histograms, the
 // tables of k_ingest_batch / k_ingest_keyed_graph): work is dealt round-robin, so 2^31 per CTA keeps every cell < 2^32.
 size_t launch_cap(int grid) { return std::min((size_t)1 << 36, (size_t)grid << 31); }
-// The vector body of n 8-byte samples at `vals`: `head` scalar samples (at most 3) up to the first 32-byte aligned value,
-// then n4 groups of 4; ids_ok: the ids (id_bytes each; 0: none) are aligned to 4 ids there.  Each caller decides what a
-// misaligned or short piece takes instead.
+// The vector body of n samples of val_bytes each (8 unless given; naturally aligned) at `vals`: `head` scalar samples
+// (at most 32 / val_bytes - 1) up to the first 32-byte aligned value, then n4 32-byte groups (of 4 samples when they are
+// 8-byte); ids_ok: the ids (id_bytes each; 0: none) are aligned to 4 ids there.  Each caller decides what a misaligned
+// or short piece takes instead.
 struct VecSplit { size_t head, n4; bool ids_ok; };
-VecSplit vec_split(const void *vals, size_t n, const void *ids = nullptr, size_t id_bytes = 0) {
-    const size_t head = std::min<size_t>(n, ((32u - ((uintptr_t)vals & 31u)) & 31u) / 8u);
-    return {head, (n - head) / 4, !id_bytes || (((uintptr_t)ids + head * id_bytes) & (4 * id_bytes - 1)) == 0};
+VecSplit vec_split(const void *vals, size_t n, const void *ids = nullptr, size_t id_bytes = 0, size_t val_bytes = 8) {
+    const size_t head = std::min<size_t>(n, ((32u - ((uintptr_t)vals & 31u)) & 31u) / val_bytes);
+    return {head, (n - head) / (32 / val_bytes), !id_bytes || (((uintptr_t)ids + head * id_bytes) & (4 * id_bytes - 1)) == 0};
 }
 
 // The write protocol of every timed ingest (locked): order `s` after the zeroing of the active buffer, bracket
@@ -496,6 +546,28 @@ lh_status launch_single(lh_ctx *ctx, unsigned long long *counts, uint32_t *flag,
     }
     return LH_OK;
 }
+// launch_single for a long array of 4-byte or 16-bit elements: the narrow form k1n of K1 (g_k1_narrow), with the grid
+// and per-launch bound of launch_single.  The caller counts the samples in stats.
+lh_status launch_narrow_single(lh_ctx *ctx, int k1n, unsigned long long *counts, uint32_t *flag, const void *d_values,
+                               size_t n, cudaStream_t s) {
+    const K1Narrow &f = ctx->k1n[k1n];
+    const int grid = ingest_sms(ctx) * f.blocks_per_sm * ctx->k1_grid_mult;
+    const size_t cap = launch_cap(grid);
+    const uint16_t *keys = ctx->d_key16.get() + (k1n == 3 ? 32768 : 0);   // the 16-bit forms' table (bfloat16 second)
+    for (size_t done = 0; done < n;) {
+        const size_t m = std::min(n - done, cap);
+        const char *p = (const char *)d_values + done * f.bytes;
+        const VecSplit v = vec_split(p, m, nullptr, 0, f.bytes);
+        const char *body = p + v.head * f.bytes;
+        const char *tail = body + v.n4 * 32;
+        f.launch(grid, f.smem, s, body, v.n4, p, (int)v.head, tail, (int)(m - v.head - v.n4 * (32 / f.bytes)), counts, flag,
+                 ctx->pc, keys);
+        LH_CUDA(ctx, cudaGetLastError());
+        ctx->stats.kernel_launches++;
+        done += m;
+    }
+    return LH_OK;
+}
 // n samples of histogram hid into buffer b, counted in stats
 lh_status ingest_single(lh_ctx *ctx, int b, uint32_t hid, const double *d_values, size_t n, cudaStream_t s) {
     lh_status st = launch_single(ctx, ctx->buf[b].d_buckets.get() + (size_t)hid * 65536u, ctx->buf[b].d_flags.get() + hid, d_values, n, s);
@@ -541,6 +613,9 @@ constexpr uint32_t KS_MAX_PASSES = 4;
 // passes but P owner CTAs (one per SM) can hold them all, and the batch is big enough to amortise the
 // cooperative launch.
 constexpr size_t kSmemBudget = 227 * 1024;
+// the narrow forms of K1 fit beside the largest sub-histogram (precision 250: win 10 918)
+static_assert(kK1nStages4 * (kK1nStage + 16) + (2 * 10918 + 8) * 4 <= kSmemBudget, "4-byte form of K1");
+static_assert(kK1nStages2 * (kK1nStage + 16) + 65536 + (2 * 10918 + 8) * 4 <= kSmemBudget, "16-bit form of K1");
 
 // Samples one launch of k_ingest_keyed_wc may take, both arrays of a fused pair together: its owner windows are uint32
 // cells flushed once, at the end of the launch, so no cell may receive 2^32 samples in one launch.
@@ -1272,8 +1347,24 @@ extern "C" lh_status lh_create(const lh_config *cfg, lh_ctx **out) {
         // k_ingest_keyed_graph: the same launch bounds and table, so the same occupancy and grid (batch_grid_max)
         LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_ingest_keyed_graph<unsigned short>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
         LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_ingest_keyed_graph<unsigned int>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
-        // k_ingest_arrays (lh_snapshot_ingest_arrays): likewise
-        LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_ingest_arrays, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
+        // k_ingest_arrays (lh_snapshot_ingest_arrays, and lh_ingest_arrays' short items): likewise
+        LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_ingest_arrays<gauge::Relaxed>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
+        LH_CREATE_CUDA(cudaFuncSetAttribute((const void *)k_ingest_arrays<gauge::Streaming>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
+    }
+    {   // lh_ingest_arrays' narrow forms of K1 and the key tables of the 16-bit one (before any capture can need them)
+        LH_CREATE_CUDA(cudaMalloc(ctx->d_key16.out(), 65536 * sizeof(uint16_t)));
+        k_fill_key16<<<65536 / 256, 256, 0, ctx->snap_stream.get()>>>(ctx->d_key16.get(), ctx->pc.precision, ctx->pc.win);
+        LH_CREATE_CUDA(cudaGetLastError());
+        const size_t hist = (size_t)subhist_words(ctx->pc.win) * 4;
+        for (int i = 0; i < 4; i++) {
+            K1Narrow &f = ctx->k1n[i];
+            f = g_k1_narrow[i];
+            f.smem = f.smem_fixed + hist;   // <= kSmemBudget at every precision (static_assert beside kSmemBudget)
+            LH_CREATE_CUDA(cudaFuncSetAttribute(f.func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBudget));
+            int nb = 0;
+            LH_CREATE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, f.func, (kK1nCW + 1) * 32, f.smem));
+            f.blocks_per_sm = std::max(nb, 1);
+        }
     }
     LH_CREATE_CUDA(cudaStreamSynchronize(ctx->snap_stream.get()));
 #undef LH_CREATE_CUDA
@@ -2662,9 +2753,24 @@ lh_status check_array(lh_ctx *ctx, uint32_t i, const lh_array_src &a) {
     return LH_OK;
 }
 
-// Validated arrays into the rows of `target` on s: as few launches of k_ingest_arrays as the parameter block and the
-// uint32 table counts allow (launch_batch's packing); an array that does not fit the launch being filled is split
-// across launches.  The caller counts the samples in stats.
+// lh_ingest_arrays routing (launch_arrays<gauge::Streaming>): an item at least this long goes to K1 in the form of its
+// dtype, float64 ones from kBatchK1Min as in lh_ingest_batch; shorter ones, and every int64 / uint64 item, go to
+// k_ingest_arrays.  Both narrow thresholds are kBatchK1Min's value, not measured for these forms: at 2^28 samples the
+// 4-byte form runs 750 G samples/s and the 16-bit form 830 G (H100 80GB HBM3, 700 W; DESIGN.md section 5.1).
+constexpr size_t kArraysK1Min4 = 1024 * 1024;   // float32, int32: the 4-byte form
+constexpr size_t kArraysK1Min2 = 1024 * 1024;   // float16, bfloat16: the 16-bit form
+size_t arrays_k1_min(uint32_t dtype) {
+    if (dtype == LH_GAUGE_F64) return kBatchK1Min;
+    const int f = k1n_index(dtype);
+    return f < 0 ? SIZE_MAX : g_k1_narrow[f].bytes == 4 ? kArraysK1Min4 : kArraysK1Min2;
+}
+
+// Validated arrays into the rows of `target` on s: as few launches of k_ingest_arrays<Ld> as the parameter block and
+// the uint32 table counts allow (launch_batch's packing); an array that does not fit the launch being filled is split
+// across launches.  With Ld = gauge::Streaming (lh_ingest_arrays, stream-ordered) long items go to K1 instead, by
+// arrays_k1_min; gauge::Relaxed (distribution gauges) takes every item through k_ingest_arrays.  Kernels only (the
+// graph recorder's form is captured); the caller counts the samples in stats.
+template <typename Ld>
 lh_status launch_arrays(lh_ctx *ctx, const lh_recorder &target, const lh_array_src *srcs, uint32_t n_srcs, cudaStream_t s) {
     ArrayParams &prm = ctx->array_prm;
     prm.rec = target;
@@ -2677,7 +2783,7 @@ lh_status launch_arrays(lh_ctx *ctx, const lh_recorder &target, const lh_array_s
         prm.n_items = k;
         const unsigned long long pieces = (total + BI_PIECE - 1) / BI_PIECE;
         const int grid = (int)std::min<unsigned long long>((unsigned long long)grid_max, pieces);
-        k_ingest_arrays<<<grid, BI_THREADS, BlockRecorder::smem_bytes(BI_TABLE_ENTRIES), s>>>(prm);
+        k_ingest_arrays<Ld><<<grid, BI_THREADS, BlockRecorder::smem_bytes(BI_TABLE_ENTRIES), s>>>(prm);
         LH_CUDA(ctx, cudaGetLastError());
         ctx->stats.kernel_launches++;
         k = 0;
@@ -2686,6 +2792,15 @@ lh_status launch_arrays(lh_ctx *ctx, const lh_recorder &target, const lh_array_s
     };
     for (uint32_t i = 0; i < n_srcs; i++) {
         const lh_array_src &a = srcs[i];
+        if (std::is_same<Ld, gauge::Streaming>::value && a.n >= arrays_k1_min(a.dtype)) {
+            unsigned long long *row = reinterpret_cast<unsigned long long *>(target.d_buckets) + (size_t)a.histogram_id * 65536u;
+            uint32_t *flag = target.d_flags + a.histogram_id;
+            const int f = k1n_index(a.dtype);
+            lh_status st = f < 0 ? launch_single(ctx, row, flag, (const double *)a.d_values, (size_t)a.n, s)
+                                 : launch_narrow_single(ctx, f, row, flag, a.d_values, (size_t)a.n, s);
+            if (st != LH_OK) return st;
+            continue;
+        }
         const char *p = (const char *)a.d_values;
         unsigned long long left = a.n;
         while (left) {
@@ -2719,10 +2834,65 @@ extern "C" lh_status lh_snapshot_ingest_arrays(lh_ctx *ctx, const lh_array_src *
         return fail(ctx, LH_ERR_STATE, "lh_snapshot_ingest_arrays needs an open snapshot whose rows nothing has read yet");
     if (total == 0) return LH_OK;
     // after lh_snapshot_begin's writer waits, graph drain and hot-window fold, all on the snapshot stream
-    lh_status st = launch_arrays(ctx, buffer_target(ctx, ctx->active ^ 1), h_srcs, n_srcs, ctx->snap_stream.get());
+    lh_status st = launch_arrays<gauge::Relaxed>(ctx, buffer_target(ctx, ctx->active ^ 1), h_srcs, n_srcs, ctx->snap_stream.get());
     if (st != LH_OK) return st;
     ctx->stats.samples += total;
     return LH_OK;
+}
+
+namespace {
+// Validation of lh_ingest_arrays / lh_graph_recorder_ingest_arrays against `limit` histogram ids (check_batch's, by
+// dtype); the samples of the call.  The arrays are read in stream order, like lh_ingest_batch's, so unlike
+// lh_snapshot_ingest_arrays the memory kind and the allocation range are the caller's to get right.
+lh_status check_stream_arrays(lh_ctx *ctx, const lh_array_src *h_srcs, uint32_t n_srcs, uint32_t limit,
+                              unsigned long long *n_out) {
+    if (n_srcs && !h_srcs) return fail(ctx, LH_ERR_INVALID, "h_srcs is NULL");
+    char what[160];
+    unsigned long long n = 0;
+    for (uint32_t i = 0; i < n_srcs; i++) {
+        const lh_array_src &a = h_srcs[i];
+        if (a.dtype >= kGaugeKinds) {
+            snprintf(what, sizeof what, "array %u: unknown dtype %u", i, a.dtype);
+            return fail(ctx, LH_ERR_INVALID, what);
+        }
+        if (a.n == 0) continue;
+        if (!a.d_values || ((uintptr_t)a.d_values & (kGaugeBytes[a.dtype] - 1u))) {
+            snprintf(what, sizeof what, "array %u: d_values is NULL or not %u-byte aligned", i, kGaugeBytes[a.dtype]);
+            return fail(ctx, LH_ERR_INVALID, what);
+        }
+        if (a.histogram_id >= limit) {
+            snprintf(what, sizeof what, "array %u: histogram_id %u >= max_histograms", i, a.histogram_id);
+            return fail(ctx, LH_ERR_RANGE, what);
+        }
+        n += a.n;
+    }
+    *n_out = n;
+    return LH_OK;
+}
+}  // namespace
+
+extern "C" lh_status lh_ingest_arrays(lh_ctx *ctx, const lh_array_src *h_srcs, uint32_t n_srcs, void *stream) {
+    LH_ENTER(ctx);
+    unsigned long long n = 0;
+    lh_status st = check_stream_arrays(ctx, h_srcs, n_srcs, ctx->H, &n);
+    if (st != LH_OK || n == 0) return st;
+    cudaStream_t s = pick_stream(ctx, stream);
+    return write_bracket(ctx, s, [&](int b) {
+        lh_status bs = launch_arrays<gauge::Streaming>(ctx, buffer_target(ctx, b), h_srcs, n_srcs, s);
+        if (bs == LH_OK) ctx->stats.samples += n;
+        return bs;
+    });
+}
+
+extern "C" lh_status lh_graph_recorder_ingest_arrays(lh_ctx *ctx, const lh_graph_recorder *g, const lh_array_src *h_srcs,
+                                                     uint32_t n_srcs, void *stream) {
+    LH_ENTER(ctx);
+    GraphRec *gr = graph_of(ctx, g);
+    if (!gr) return fail(ctx, LH_ERR_INVALID, "destroyed or foreign graph recorder");
+    unsigned long long n = 0;
+    lh_status st = check_stream_arrays(ctx, h_srcs, n_srcs, gr->rec.max_histograms, &n);
+    if (st != LH_OK || n == 0) return st;
+    return launch_arrays<gauge::Streaming>(ctx, gr->rec, h_srcs, n_srcs, pick_stream(ctx, stream));
 }
 
 // =========================================================== reduce caller-supplied sparse histograms

@@ -7,7 +7,8 @@
 //          _ldg   : 2 x 128-bit ld.global.nc loads per 4 samples, software-pipelined in registers, scalar fast_candidate() (first version;
 //                   kept as the second, independently written evaluator the parity tests run against the oracle)
 //        both privatise the histogram in shared memory (uint32 sub-histograms, ATOMS.POPC.INC) and flush once per
-//        CTA with one global 64-bit atomic per non-empty bucket.
+//        CTA with one global 64-bit atomic per non-empty bucket.  _bulk also comes in a 4-byte form (float32 / int32)
+//        and a 16-bit form (float16 / bfloat16, a key table from k_fill_key16 instead of the log) for lh_ingest_arrays.
 //   K1k  k_ingest_keyed_small   (id,value) pairs, as many ids per pass as fit privatised in shared memory (HBM-bound)
 //        k_ingest_keyed_vec     any number of ids: one L2 RED per sample into a compact, replicated uint32 window
 //        k_ingest_keyed_wc      owner-partitioned, write-combining cooperative kernel (many histograms)
@@ -23,13 +24,14 @@
 //                               (lh_reduce_sparse_host)
 //   k_ingest_batch          many device arrays under many ids (lh_ingest_batch, lh_graph_recorder_ingest)
 //   k_ingest_arrays         every element of device arrays of any gauge dtype -> the frozen interval (distribution
-//                           gauges, lh_snapshot_ingest_arrays)
+//                           gauges, lh_snapshot_ingest_arrays), or with streaming loads the short items of
+//                           lh_ingest_arrays / lh_graph_recorder_ingest_arrays
 //   k_ingest_keyed_graph    (id,value) pairs into a graph recorder's rows (lh_graph_recorder_ingest_keyed_*)
 //   k_graph_drain           graph recorders' rows -> the interval being frozen (lh_snapshot_begin)
 //   k_raw_publish, k_raw_publish_window, k_raw_percentiles, k_raw_ranks   running bucket counts of a snapshot (or of
 //                           the last `window` of them) -> raw device subscription rows, and exact percentile / rank
 //                           queries over them (lh_snapshot_publish_raw, lh_raw_*)
-//   misc k_clear_touched, k_fill_decompress, k_compress_probe, k_fastpath_margin, k_fastpath_certify, k_stream_probe,
+//   misc k_clear_touched, k_fill_decompress, k_fill_key16, k_compress_probe, k_fastpath_margin, k_fastpath_certify, k_stream_probe,
 //        k_gen_stream, k_gen_ids_u16
 //
 // Per-histogram flags (uint32[H], one array per bucket buffer): 0 = untouched since the buffer was cleared,
@@ -300,25 +302,42 @@ k_stream_probe(const double *__restrict__ vals32, size_t nvec, const double *, i
 // cp.async.bulk; CW consumer warps bucket them.  Tiles are dealt round-robin.
 // FOLD_SIGN: negative samples stay on the fast path (their slot is offset by `win`) at the price of two more integer
 // instructions per sample; without it they are flagged and re-derived in the fix-up.
-template <int CW, int STAGES, int STAGE_BYTES, int MINB, bool FOLD_SIGN>
+// Cv: the element type and its conversion to float64 (K1F64 below, the float64 kernel; K1F32 / K1I32 and K1F16 /
+// K1BF16 after the gauge conversions, lh_ingest_arrays).  The producer and the ring move bytes whatever the element;
+// vals32 is 32-byte aligned and holds nvec32 32-byte groups, head / tail the (at most 32 / sizeof(T) - 1) elements on
+// either side.  4-byte elements are converted exactly and binned with bucket_offsets_v2 like float64 ones.  16-bit
+// elements (Cv::kTable) skip the arithmetic: `keys` is the dtype's 32768-entry table of k_fill_key16, copied into
+// shared memory ahead of the sub-histogram, giving each magnitude's window slot (the sign adds `win`), or 0xFFFF for a
+// key outside the window, which goes through fixup_slot.
+struct K1F64 { using T = double; static constexpr bool kTable = false; };
+template <int CW, int STAGES, int STAGE_BYTES, int MINB, bool FOLD_SIGN, typename Cv = K1F64>
 __global__ void __launch_bounds__((CW + 1) * 32, MINB)
-k_ingest_single_bulk(const double *__restrict__ vals32, size_t nvec32, const double *head, int nhead,
-                     const double *tail, int ntail, unsigned long long *__restrict__ counts, uint32_t *flag, Prec pc) {
+k_ingest_single_bulk(const typename Cv::T *__restrict__ vals32, size_t nvec32, const typename Cv::T *head, int nhead,
+                     const typename Cv::T *tail, int ntail, unsigned long long *__restrict__ counts, uint32_t *flag, Prec pc,
+                     const uint16_t *keys = nullptr) {
+    using T = typename Cv::T;
+    constexpr bool F64 = std::is_same<T, double>::value;
+    constexpr int SPV = 16 / (int)sizeof(T);          // samples per 16-byte vector
     const double2 *vals16 = reinterpret_cast<const double2 *>(vals32);
     const size_t nvec = nvec32 * 2;   // 16-byte vectors
     constexpr int CT = CW * 32;                       // consumer threads
     constexpr int STAGE_VEC = STAGE_BYTES / 16;
-    constexpr int PER_THREAD = STAGE_VEC / CT;        // double2 per consumer thread per stage
+    constexpr int PER_THREAD = STAGE_VEC / CT;        // 16-byte vectors per consumer thread per stage
     static_assert(STAGE_VEC % CT == 0, "stage must divide evenly over consumer threads");
     extern __shared__ __align__(128) unsigned char s_raw[];
     double2 *s_data = reinterpret_cast<double2 *>(s_raw);
     uint64_t *full = reinterpret_cast<uint64_t *>(s_raw + (size_t)STAGES * STAGE_BYTES);
     uint64_t *empty = full + STAGES;
-    uint32_t *s_hist = reinterpret_cast<uint32_t *>(empty + STAGES);
+    uint16_t *s_keys = reinterpret_cast<uint16_t *>(empty + STAGES);   // Cv::kTable only
+    uint32_t *s_hist = reinterpret_cast<uint32_t *>(empty + STAGES) + (Cv::kTable ? 16384 : 0);
 
     const int tid = threadIdx.x;
     const int warp = tid >> 5;
     for (uint32_t i = tid; i < subhist_words(pc.win); i += (CW + 1) * 32) s_hist[i] = 0;
+    if constexpr (Cv::kTable) {
+        for (uint32_t i = tid; i < 4096u; i += (CW + 1) * 32)
+            reinterpret_cast<uint4 *>(s_keys)[i] = __ldg(reinterpret_cast<const uint4 *>(keys) + i);
+    }
     if (tid == 0) {
         for (int s = 0; s < STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], CW); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -353,30 +372,72 @@ k_ingest_single_bulk(const double *__restrict__ vals32, size_t nvec32, const dou
             size_t first = tile * (size_t)STAGE_VEC;
             size_t rem = nvec - first;
             if (rem >= (size_t)STAGE_VEC) {
-                double v[2 * PER_THREAD];
+                if constexpr (F64) {
+                    double v[2 * PER_THREAD];
 #pragma unroll
-                for (int u = 0; u < PER_THREAD; u++) {
-                    double2 d = st[u * CT + tid];
-                    v[2 * u] = d.x; v[2 * u + 1] = d.y;
-                }
-                __syncwarp();
-                if ((tid & 31) == 0) mbar_arrive(&empty[s]);   // registers hold the data: release early
+                    for (int u = 0; u < PER_THREAD; u++) {
+                        double2 d = st[u * CT + tid];
+                        v[2 * u] = d.x; v[2 * u + 1] = d.y;
+                    }
+                    __syncwarp();
+                    if ((tid & 31) == 0) mbar_arrive(&empty[s]);   // registers hold the data: release early
 #pragma unroll
-                for (int q = 0; q < 2 * PER_THREAD; q += 4) {
-                    const double v4[4] = {v[q], v[q + 1], v[q + 2], v[q + 3]};
-                    bucket_samples_v2<4, FOLD_SIGN>(v4, s_hist, pc, one_bits, counts, flag);
+                    for (int q = 0; q < 2 * PER_THREAD; q += 4) {
+                        const double v4[4] = {v[q], v[q + 1], v[q + 2], v[q + 3]};
+                        bucket_samples_v2<4, FOLD_SIGN>(v4, s_hist, pc, one_bits, counts, flag);
+                    }
+                } else {
+                    uint32_t w[4 * PER_THREAD];
+#pragma unroll
+                    for (int u = 0; u < PER_THREAD; u++) {
+                        const uint4 d = reinterpret_cast<const uint4 *>(st)[u * CT + tid];
+                        w[4 * u] = d.x; w[4 * u + 1] = d.y; w[4 * u + 2] = d.z; w[4 * u + 3] = d.w;
+                    }
+                    __syncwarp();
+                    if ((tid & 31) == 0) mbar_arrive(&empty[s]);
+                    if constexpr (Cv::kTable) {
+#pragma unroll
+                        for (int q = 0; q < 4 * PER_THREAD; q++) {
+#pragma unroll
+                            for (int h = 0; h < 2; h++) {
+                                const uint32_t x = h ? w[q] >> 16 : w[q] & 0xFFFFu;
+                                uint32_t slot = s_keys[x & 0x7FFFu];
+                                if (slot == 0xFFFFu) slot = fixup_slot(Cv::f64((unsigned short)x), pc, counts, flag);
+                                else slot += (x >> 15) * pc.win;
+                                atomicAdd(&s_hist[slot], 1u);
+                            }
+                        }
+                    } else {
+#pragma unroll
+                        for (int q = 0; q < 4 * PER_THREAD; q += 4) {
+                            const double v4[4] = {Cv::f64(w[q]), Cv::f64(w[q + 1]), Cv::f64(w[q + 2]), Cv::f64(w[q + 3])};
+                            bucket_samples_v2<4, FOLD_SIGN>(v4, s_hist, pc, one_bits, counts, flag);
+                        }
+                    }
                 }
             } else {
-                for (int j = tid; j < (int)rem; j += CT) {
-                    double2 d = st[j];
-                    atomicAdd(&s_hist[fixup_slot(d.x, pc, counts, flag)], 1u);
-                    atomicAdd(&s_hist[fixup_slot(d.y, pc, counts, flag)], 1u);
+                if constexpr (F64) {
+                    for (int j = tid; j < (int)rem; j += CT) {
+                        double2 d = st[j];
+                        atomicAdd(&s_hist[fixup_slot(d.x, pc, counts, flag)], 1u);
+                        atomicAdd(&s_hist[fixup_slot(d.y, pc, counts, flag)], 1u);
+                    }
+                } else {
+                    const T *e = reinterpret_cast<const T *>(st);
+                    for (int j = tid; j < (int)rem * SPV; j += CT) atomicAdd(&s_hist[fixup_slot(Cv::f64(e[j]), pc, counts, flag)], 1u);
                 }
                 __syncwarp();
                 if ((tid & 31) == 0) mbar_arrive(&empty[s]);
             }
         }
-        if (blockIdx.x == 0 && tid == 0) { bucket_stragglers(head, nhead, pc, counts, flag); bucket_stragglers(tail, ntail, pc, counts, flag); }
+        if (blockIdx.x == 0 && tid == 0) {
+            if constexpr (F64) {
+                bucket_stragglers(head, nhead, pc, counts, flag); bucket_stragglers(tail, ntail, pc, counts, flag);
+            } else {
+                for (int i = 0; i < nhead; i++) add_bucket_global(counts, flag, key16_of(Cv::f64(head[i]), pc), 1ull, pc.win);
+                for (int i = 0; i < ntail; i++) add_bucket_global(counts, flag, key16_of(Cv::f64(tail[i]), pc), 1ull, pc.win);
+            }
+        }
     }
     __syncthreads();
     flush_subhist(s_hist, tid, (CW + 1) * 32, counts, flag, pc.win);
@@ -2412,23 +2473,57 @@ __device__ __forceinline__ double f32(float x) {   // exact, subnormals kept (no
     asm("cvt.f64.f32 %0, %1;" : "=d"(d) : "f"(x));
     return d;
 }
-// The value at p of dtype LH_GAUGE_* (checked on the host) as Go's float64(x): one strong load of its width, then the
-// conversion.  The one place both k_gauge_read and k_ingest_arrays take a value from.
+// Go's float64(x) of the raw bits of one element: exact widening for f32 (and f16 / bf16 through f32) and s32, cvt.rn
+// (round to nearest even) for s64 / u64.  The one definition of the conversion: every kernel that takes LH_GAUGE_*
+// elements (k_gauge_read, k_ingest_arrays, the narrow forms of K1 and the key table of k_fill_key16) converts here.
+__device__ __forceinline__ double from_f32(uint32_t b) { return f32(__uint_as_float(b)); }
+__device__ __forceinline__ double from_f16(unsigned short b) {
+    float f;
+    asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(b));
+    return f32(f);
+}
+__device__ __forceinline__ double from_bf16(unsigned short b) { return f32(__uint_as_float((uint32_t)b << 16)); }
+__device__ __forceinline__ double from_i64(unsigned long long b) {
+    double v;
+    asm("cvt.rn.f64.s64 %0, %1;" : "=d"(v) : "l"(b));
+    return v;
+}
+__device__ __forceinline__ double from_i32(uint32_t b) {
+    double v;
+    asm("cvt.rn.f64.s32 %0, %1;" : "=d"(v) : "r"(b));
+    return v;
+}
+__device__ __forceinline__ double from_u64(unsigned long long b) {
+    double v;
+    asm("cvt.rn.f64.u64 %0, %1;" : "=d"(v) : "l"(b));
+    return v;
+}
+// Load policies of load(): Relaxed, one strong load (a device gauge or a distribution read outside stream order, never
+// torn against an aligned store); Streaming, read-once stream-ordered data (lh_ingest_arrays), ld.global.cs as
+// k_ingest_batch loads its samples.
+struct Relaxed {
+    static __device__ __forceinline__ unsigned long long ld64(const void *p) { return gauge::ld64(p); }
+    static __device__ __forceinline__ uint32_t ld32(const void *p) { return gauge::ld32(p); }
+    static __device__ __forceinline__ unsigned short ld16(const void *p) { return gauge::ld16(p); }
+};
+struct Streaming {
+    static __device__ __forceinline__ unsigned long long ld64(const void *p) { return __ldcs((const unsigned long long *)p); }
+    static __device__ __forceinline__ uint32_t ld32(const void *p) { return __ldcs((const unsigned int *)p); }
+    static __device__ __forceinline__ unsigned short ld16(const void *p) { return __ldcs((const unsigned short *)p); }
+};
+// The value at p of dtype LH_GAUGE_* (checked on the host) as Go's float64(x): one load of its width under policy Ld,
+// then the conversion.
+template <typename Ld = Relaxed>
 __device__ __forceinline__ double load(const void *p, uint32_t dtype) {
     double v;
     switch (dtype) {
-    case LH_GAUGE_F64: v = __longlong_as_double((long long)ld64(p)); break;
-    case LH_GAUGE_F32: v = f32(__uint_as_float(ld32(p))); break;
-    case LH_GAUGE_F16: {
-        float f;
-        asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"(ld16(p)));
-        v = f32(f);
-        break;
-    }
-    case LH_GAUGE_BF16: v = f32(__uint_as_float((uint32_t)ld16(p) << 16)); break;
-    case LH_GAUGE_I64: asm("cvt.rn.f64.s64 %0, %1;" : "=d"(v) : "l"(ld64(p))); break;
-    case LH_GAUGE_I32: asm("cvt.rn.f64.s32 %0, %1;" : "=d"(v) : "r"(ld32(p))); break;
-    default: asm("cvt.rn.f64.u64 %0, %1;" : "=d"(v) : "l"(ld64(p))); break;   // LH_GAUGE_U64
+    case LH_GAUGE_F64: v = __longlong_as_double((long long)Ld::ld64(p)); break;
+    case LH_GAUGE_F32: v = from_f32(Ld::ld32(p)); break;
+    case LH_GAUGE_F16: v = from_f16(Ld::ld16(p)); break;
+    case LH_GAUGE_BF16: v = from_bf16(Ld::ld16(p)); break;
+    case LH_GAUGE_I64: v = from_i64(Ld::ld64(p)); break;
+    case LH_GAUGE_I32: v = from_i32(Ld::ld32(p)); break;
+    default: v = from_u64(Ld::ld64(p)); break;   // LH_GAUGE_U64
     }
     return v;
 }
@@ -2444,6 +2539,31 @@ k_gauge_read(const __grid_constant__ GaugeParams p) {
     p.out[i] = gauge::load(e.p, e.dtype);
 }
 
+// ----------------------------------------------------------- narrow forms of K1 (lh_ingest_arrays)
+// The element converters of k_ingest_single_bulk for long arrays of 4-byte and 16-bit samples: T is the raw element,
+// f64 the gauge conversion of its bits.
+struct K1F32 { using T = uint32_t; static constexpr bool kTable = false;
+               static __device__ __forceinline__ double f64(uint32_t b) { return gauge::from_f32(b); } };
+struct K1I32 { using T = uint32_t; static constexpr bool kTable = false;
+               static __device__ __forceinline__ double f64(uint32_t b) { return gauge::from_i32(b); } };
+struct K1F16 { using T = unsigned short; static constexpr bool kTable = true;
+               static __device__ __forceinline__ double f64(unsigned short b) { return gauge::from_f16(b); } };
+struct K1BF16 { using T = unsigned short; static constexpr bool kTable = true;
+                static __device__ __forceinline__ double f64(unsigned short b) { return gauge::from_bf16(b); } };
+
+// The key tables of the 16-bit form, built once per context: table[0] for float16, table[1] for bfloat16, entry m
+// (magnitude bits, x & 0x7FFF) the window slot of exact_key16(float64(m)), 0xFFFF when that key has no slot below win.
+// compress(-v) = -compress(v) and key16_to_slot puts key -k at slot win + k, so a sample with the sign bit set takes
+// the entry plus win (slot win is key 0, as is slot 0).  Inf and NaN take the entry of whatever key exact_key16 gives.
+__global__ void k_fill_key16(uint16_t *__restrict__ table, double precision, uint32_t win) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 65536u) return;
+    const unsigned short m = (unsigned short)(i & 0x7FFFu);
+    const double v = (i >> 15) ? gauge::from_bf16(m) : gauge::from_f16(m);
+    const uint32_t slot = key16_to_slot(exact_key16(v, precision), win);
+    table[i] = slot < win ? (uint16_t)slot : (uint16_t)0xFFFFu;
+}
+
 // ----------------------------------------------------------- distribution gauges (lh_snapshot_ingest_arrays)
 // Every element of many device arrays, each of dtype LH_GAUGE_* under its own histogram id, into the frozen interval's
 // rows.  The work is k_ingest_batch's: the item table travels in the parameter block, the items' concatenation is cut
@@ -2451,6 +2571,8 @@ k_gauge_read(const __grid_constant__ GaugeParams p) {
 // every CTA counts through one lh::BlockRecorder of BI_TABLE_ENTRIES entries, flushed once.  Only the sample load
 // differs: an element is read as a device gauge is (gauge::load), so a value written by one aligned store is never
 // torn.  The host bounds a launch's samples as it bounds k_ingest_batch's (no CTA counts more than 2^31 of them).
+// Ld = gauge::Streaming is the short-item route of lh_ingest_arrays / lh_graph_recorder_ingest_arrays: the same walk
+// over stream-ordered arrays with streaming loads, into the active interval's or a graph recorder's rows.
 struct ArraySeg {
     const void *vals;                        // dtype-aligned, the whole item inside one allocation (checked on the host)
     uint32_t id;
@@ -2464,6 +2586,7 @@ struct ArrayParams {
     ArraySeg seg[BI_MAX_ITEMS];
 };
 
+template <typename Ld>
 __global__ void __launch_bounds__(BI_THREADS, 2)
 k_ingest_arrays(const __grid_constant__ ArrayParams p) {
     extern __shared__ __align__(16) unsigned char ia_smem[];
@@ -2491,7 +2614,7 @@ k_ingest_arrays(const __grid_constant__ ArrayParams p) {
                     while (p.start[it + 1] <= g) ++it;
                     const ArraySeg s = p.seg[it];
                     id[k] = s.id;
-                    v[k] = gauge::load((const char *)s.vals + ((g - p.start[it]) << gauge::shift(s.dtype)), s.dtype);
+                    v[k] = gauge::load<Ld>((const char *)s.vals + ((g - p.start[it]) << gauge::shift(s.dtype)), s.dtype);
                 }
             }
 #pragma unroll

@@ -287,6 +287,13 @@ class GraphRecorder:
         arr, n = _batch_items(items, "local histogram id")
         self._eng._check(self._eng.lib.lh_graph_recorder_ingest(self._eng.h, C.byref(self.g), arr, n, _capture_stream(stream)))
 
+    def ingest_arrays(self, items, stream=None):
+        """lh_graph_recorder_ingest_arrays of (local id, tensor) pairs, tensors as Engine.ingest_arrays takes them, on
+        `stream` (None = torch's current stream, so that it is captured inside torch.cuda.graph)."""
+        arr, n = array_items(items, self._eng.device, "local histogram id")
+        self._eng._check(self._eng.lib.lh_graph_recorder_ingest_arrays(self._eng.h, C.byref(self.g), arr, n,
+                                                                       _capture_stream(stream)))
+
     def keyed(self, ids, values, stream=None):
         """lh_graph_recorder_ingest_keyed_u16 / _u32: values[i] into local histogram ids[i], on `stream` (None =
         torch's current stream).  ids uint16 (_u16), int32 or uint32 (_u32); values float64 or int64 nanoseconds."""
@@ -403,19 +410,32 @@ def gauge_src(t, device: int) -> tuple:
     return int(t.data_ptr()), dtype
 
 
-def array_src(t, device: int, histogram_id: int = 0) -> L.lh_array_src:
-    """lh_array_src of a distribution gauge: a contiguous CUDA tensor of any shape on `device`, of dtype float64 /
-    float32 / float16 / bfloat16 / int64 / int32 / uint64, recorded under `histogram_id`.  TypeError otherwise."""
+def array_src(t, device: int, histogram_id: int = 0, what: str = "a distribution gauge") -> L.lh_array_src:
+    """lh_array_src of a distribution gauge (or of an lh_ingest_arrays item; `what` names it in messages): a contiguous
+    CUDA tensor of any shape on `device`, of dtype float64 / float32 / float16 / bfloat16 / int64 / int32 / uint64,
+    recorded under `histogram_id`.  TypeError otherwise."""
     if not (hasattr(t, "is_cuda") and hasattr(t, "data_ptr")):
-        raise TypeError(f"a distribution gauge is a CUDA tensor, not {type(t)!r}")
+        raise TypeError(f"{what} is a CUDA tensor, not {type(t)!r}")
     if not t.is_cuda or t.device.index != device:
-        raise TypeError(f"a distribution gauge must be on cuda:{device}, not {t.device}")
+        raise TypeError(f"{what} must be on cuda:{device}, not {t.device}")
     if not t.is_contiguous():
-        raise TypeError("a distribution gauge must be a contiguous tensor")
+        raise TypeError(f"{what} must be a contiguous tensor")
     dtype = _GAUGE_DTYPES.get(str(t.dtype))
     if dtype is None:
-        raise TypeError(f"a distribution gauge must be float64/32/16, bfloat16, int64/32 or uint64, not {t.dtype}")
+        raise TypeError(f"{what} must be float64/32/16, bfloat16, int64/32 or uint64, not {t.dtype}")
     return L.lh_array_src(int(t.data_ptr()), int(t.numel()), dtype, int(histogram_id))
+
+
+def array_items(items, device: int, limit_name: str):
+    """lh_array_src array of (id, tensor) pairs for lh_ingest_arrays / lh_graph_recorder_ingest_arrays, each tensor as
+    array_src takes it; TypeError / ValueError before any call."""
+    items = list(items)
+    arr = (L.lh_array_src * max(len(items), 1))()
+    for i, (hid, t) in enumerate(items):
+        if not 0 <= int(hid) < 1 << 32:
+            raise ValueError(f"{limit_name} {hid} is not a uint32")
+        arr[i] = array_src(t, device, int(hid), "an ingested array")
+    return arr, len(items)
 
 
 class Board:
@@ -768,6 +788,14 @@ class Engine:
         anything else."""
         arr, n = _batch_items(items, "histogram id")
         self._check(self.lib.lh_ingest_batch(self.h, arr, n, _stream(stream)))
+
+    def ingest_arrays(self, items, stream=None):
+        """Many device arrays of any gauge dtype, each under its own histogram id, in one call (lh_ingest_arrays):
+        `items` is a list of (histogram id, tensor) pairs, each tensor contiguous, on this engine's device, float64 /
+        float32 / float16 / bfloat16 / int64 / int32 / uint64, every element x recorded as float64(x).  TypeError or
+        ValueError before the call for anything else."""
+        arr, n = array_items(items, self.device, "histogram id")
+        self._check(self.lib.lh_ingest_arrays(self.h, arr, n, _stream(stream)))
 
     def counter_add_u16(self, d_ids, d_amounts, n: int, stream=None):
         self._check(self.lib.lh_counter_add_u16(self.h, _ptr(d_ids), _ptr(d_amounts), n, _stream(stream)))

@@ -40,6 +40,9 @@
 #pragma weak lh_graph_recorder_counter_add_u32
 #pragma weak lh_graph_recorder_timer_start
 #pragma weak lh_graph_recorder_timer_stop
+// Arrays of any gauge dtype: over a build without them, RecordScope::Arrays / GraphRecorder::Arrays throw.
+#pragma weak lh_ingest_arrays
+#pragma weak lh_graph_recorder_ingest_arrays
 
 #pragma weak lh_ingest_keyed_mapped_u16
 #pragma weak lh_ingest_keyed_mapped_u32
@@ -816,6 +819,21 @@ void RecordScope::Histograms(const std::vector<Item> &items) {
     check(ms_->ctx_, lh_ingest_batch(ms_->ctx_, batch.data(), (uint32_t)batch.size(), stream_), "lh_ingest_batch");
     ms_->dropped_over_limit_.fetch_add(unbound, std::memory_order_relaxed);
 }
+void RecordScope::Arrays(const std::vector<ArrayItem> &items) {
+    if (!ms_) throw std::runtime_error("RecordScope::Arrays after End()");
+    for (const ArrayItem &it : items) (void)hids_.at(it.name);   // std::out_of_range before anything is issued
+    if (!lh_ingest_arrays) throw std::runtime_error("lh_ingest_arrays: not in this build of the library");
+    std::vector<lh_array_src> srcs;
+    srcs.reserve(items.size());
+    uint64_t unbound = 0;
+    for (const ArrayItem &it : items) {
+        const uint32_t id = hids_[it.name];
+        if (id == kUnbound) { unbound += it.n; continue; }
+        srcs.push_back(lh_array_src{it.d_values, (uint64_t)it.n, it.dtype, id});
+    }
+    check(ms_->ctx_, lh_ingest_arrays(ms_->ctx_, srcs.data(), (uint32_t)srcs.size(), stream_), "lh_ingest_arrays");
+    ms_->dropped_over_limit_.fetch_add(unbound, std::memory_order_relaxed);
+}
 void RecordScope::Keyed(const void *d_ids, size_t id_bytes, const void *d_values, uint32_t kind, size_t n) {
     if (!ms_) throw std::runtime_error("RecordScope::Keyed after End()");
     if (id_bytes != 2 && id_bytes != 4) throw std::invalid_argument("RecordScope::Keyed: id_bytes must be 2 or 4");
@@ -893,6 +911,20 @@ void GraphRecorder::Histograms(const std::vector<Item> &items, void *stream) {
     MetricSystem *ms = st_->ms;
     check(ms->ctx_, lh_graph_recorder_ingest(ms->ctx_, &st_->g, batch.data(), (uint32_t)batch.size(), stream),
           "lh_graph_recorder_ingest");
+}
+
+void GraphRecorder::Arrays(const std::vector<ArrayItem> &items, void *stream) {
+    if (!st_ || !st_->ms) throw std::runtime_error("GraphRecorder::Arrays of a closed recorder");
+    std::vector<lh_array_src> srcs;
+    srcs.reserve(items.size());
+    for (const ArrayItem &it : items) {
+        if (it.name >= st_->hnames.size()) throw std::out_of_range("GraphRecorder::Arrays: no such histogram name");
+        srcs.push_back(lh_array_src{it.d_values, (uint64_t)it.n, it.dtype, (uint32_t)it.name});
+    }
+    if (!lh_graph_recorder_ingest_arrays) throw std::runtime_error("lh_graph_recorder_ingest_arrays: not in this build of the library");
+    MetricSystem *ms = st_->ms;
+    check(ms->ctx_, lh_graph_recorder_ingest_arrays(ms->ctx_, &st_->g, srcs.data(), (uint32_t)srcs.size(), stream),
+          "lh_graph_recorder_ingest_arrays");
 }
 
 void GraphRecorder::Keyed(const void *d_ids, size_t id_bytes, const void *d_values, uint32_t kind, size_t n, void *stream) {
@@ -2241,6 +2273,35 @@ LHMS_API int lhms_graph_recorder_histograms(void *g, const uint32_t *name_index,
         std::vector<GraphRecorder::Item> items(n_items);
         for (uint32_t i = 0; i < n_items; i++) items[i] = GraphRecorder::Item{name_index[i], d_values[i], (size_t)n[i], kinds[i]};
         static_cast<GraphRecorder *>(g)->Histograms(items, stream);
+        return LH_OK;
+    } catch (const std::exception &e) {
+        return scope_status(e);
+    }
+}
+// RecordScope::Arrays of the open scope `rec` and GraphRecorder::Arrays, items as lhms_scope_histograms' with dtypes
+// (LH_GAUGE_*) for kinds; statuses as theirs.
+LHMS_API int lhms_arrays_scope(void *ms, const lh_recorder *rec, const uint32_t *name_index, const void *const *d_values,
+                               const uint64_t *n, const uint32_t *dtypes, uint32_t n_items) {
+    if (!ms || !rec || (n_items && (!name_index || !d_values || !n || !dtypes))) return LH_ERR_INVALID;
+    std::lock_guard<std::mutex> lk(g_scopes_mu);
+    auto it = g_scopes.find(std::make_pair(ms, rec->scope));
+    if (it == g_scopes.end()) return LH_ERR_INVALID;
+    try {
+        std::vector<RecordScope::ArrayItem> items(n_items);
+        for (uint32_t i = 0; i < n_items; i++) items[i] = RecordScope::ArrayItem{name_index[i], d_values[i], (size_t)n[i], dtypes[i]};
+        it->second.Arrays(items);
+        return LH_OK;
+    } catch (const std::exception &e) {
+        return scope_status(e);
+    }
+}
+LHMS_API int lhms_arrays_graph_recorder(void *g, const uint32_t *name_index, const void *const *d_values, const uint64_t *n,
+                                        const uint32_t *dtypes, uint32_t n_items, void *stream) {
+    if (!g || (n_items && (!name_index || !d_values || !n || !dtypes))) return LH_ERR_INVALID;
+    try {
+        std::vector<GraphRecorder::ArrayItem> items(n_items);
+        for (uint32_t i = 0; i < n_items; i++) items[i] = GraphRecorder::ArrayItem{name_index[i], d_values[i], (size_t)n[i], dtypes[i]};
+        static_cast<GraphRecorder *>(g)->Arrays(items, stream);
         return LH_OK;
     } catch (const std::exception &e) {
         return scope_status(e);

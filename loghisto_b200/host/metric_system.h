@@ -152,6 +152,17 @@ class RecordScope {
         uint32_t kind;
     };
     void Histograms(const std::vector<Item> &items);
+    // Many device arrays of any gauge dtype in one lh_ingest_arrays on the scope's stream: n elements at d_values
+    // (device memory, naturally aligned) of dtype LH_GAUGE_* under histogram name `name`, each element x recorded as
+    // Histogram(name, float64(x)) without a float64 copy.  Names may repeat.  Unbound names, exceptions and a library
+    // without the call as in Histograms.
+    struct ArrayItem {
+        size_t name;
+        const void *d_values;
+        size_t n;
+        uint32_t dtype;
+    };
+    void Arrays(const std::vector<ArrayItem> &items);
     // (local id, value) pairs in device memory on the scope's stream, local id i being histogram name i
     // (lh_ingest_keyed_mapped_u16 for id_bytes 2, _u32 for 4): values of `kind` as in Histograms.  An id >= the number
     // of names, or under an unbound name, is dropped and counted in dropped_samples().  Names may repeat.
@@ -247,6 +258,10 @@ class GraphRecorder {
         uint32_t kind;
     };
     void Histograms(const std::vector<Item> &items, void *stream);
+    // lh_graph_recorder_ingest_arrays on `stream`: Histograms for arrays of dtype LH_GAUGE_* (RecordScope::Arrays),
+    // throwing as Histograms does, and std::runtime_error when the library lacks the call.
+    using ArrayItem = RecordScope::ArrayItem;
+    void Arrays(const std::vector<ArrayItem> &items, void *stream);
     // Kernels only, like Histograms, so each may be captured; each throws before anything is issued (std::out_of_range
     // for a bad name index, std::invalid_argument for id_bytes other than 2 or 4, std::runtime_error when the library
     // lacks the call or refuses it, or the recorder is closed).

@@ -101,6 +101,10 @@ def _bind(L):
     L.lhms_graph_recorder_new.argtypes = [vp, C.c_uint32, names, C.c_uint32, names, rec, C.POINTER(C.c_int)]
     L.lhms_graph_recorder_histograms.restype = C.c_int
     L.lhms_graph_recorder_histograms.argtypes = [vp, u32p, C.POINTER(vp), C.POINTER(C.c_uint64), u32p, C.c_uint32, vp]
+    L.lhms_arrays_scope.restype = C.c_int
+    L.lhms_arrays_scope.argtypes = [vp, rec, u32p, C.POINTER(vp), C.POINTER(C.c_uint64), u32p, C.c_uint32]
+    L.lhms_arrays_graph_recorder.restype = C.c_int
+    L.lhms_arrays_graph_recorder.argtypes = [vp, u32p, C.POINTER(vp), C.POINTER(C.c_uint64), u32p, C.c_uint32, vp]
     L.lhms_graph_recorder_close.restype = C.c_int
     L.lhms_graph_recorder_close.argtypes = [vp, vp]
     L.lhms_graph_recorder_free.argtypes = [vp]
@@ -274,6 +278,18 @@ class RecordScope:
         if st != 0:
             raise RuntimeError("lhms_scope_histograms failed (status %d)" % st)
 
+    def arrays(self, arrays):
+        """Histogram(name, float64(x)) for every element x of several device tensors in one call (lh_ingest_arrays),
+        on the scope's stream, without a float64 copy: `arrays` as histograms() takes them, each tensor contiguous, on
+        the system's device, of any shape, float64 / float32 / float16 / bfloat16 / int64 / int32 / uint64.  TypeError
+        for any other array and KeyError for a name the scope was not opened with, before anything is issued."""
+        pairs = list(arrays.items()) if isinstance(arrays, dict) else list(arrays)
+        idx, ptrs, ns, dts = _array_table(pairs, lambda name: self._hnames.index(name) if name in self._hnames else None,
+                                          "scope", self._ms._device)
+        st = self._ms._lib.lhms_arrays_scope(self._ms._h, C.byref(self.recorder), idx, ptrs, ns, dts, len(pairs))
+        if st != 0:
+            raise RuntimeError("lhms_arrays_scope failed (status %d)" % st)
+
     def keyed(self, ids, values):
         """Histogram(name, values[i]) with name the scope's histogram at position ids[i], for every i, in one call on
         the scope's stream (lh_ingest_keyed_mapped_*).  ids and values as GraphRecorder.keyed takes them (uint16, int32
@@ -298,6 +314,20 @@ class RecordScope:
             st = self._ms._lib.lhms_record_end(self._ms._h, C.byref(self.recorder))
             if st != 0:
                 raise RuntimeError("lhms_record_end failed (status %d)" % st)
+
+
+def _array_table(pairs, index_of, owner, device):
+    """(name indices, addresses, lengths, LH_GAUGE_* dtypes) of (name, tensor) pairs for lhms_arrays_scope /
+    lhms_arrays_graph_recorder; KeyError for a name index_of does not know, TypeError for a tensor array_src refuses."""
+    k = max(len(pairs), 1)
+    idx, ptrs, ns, dts = (C.c_uint32 * k)(), (C.c_void_p * k)(), (C.c_uint64 * k)(), (C.c_uint32 * k)()
+    for i, (name, t) in enumerate(pairs):
+        j = index_of(name)
+        if j is None:
+            raise KeyError("%r is not a histogram of this %s" % (name, owner))
+        src = array_src(t, device, 0, "an ingested array")
+        idx[i], ptrs[i], ns[i], dts[i] = j, src.d_values, src.n, src.dtype
+    return idx, ptrs, ns, dts
 
 
 class GraphRecorder:
@@ -337,6 +367,18 @@ class GraphRecorder:
         st = self._ms._lib.lhms_graph_recorder_histograms(self._h, idx, ptrs, ns, kinds, len(pairs), _capture_stream(stream))
         if st != 0:
             raise RuntimeError("lhms_graph_recorder_histograms failed (status %d)" % st)
+
+    def arrays(self, arrays, stream=None):
+        """Histogram(name, float64(x)) for every element x of several device tensors (lh_graph_recorder_ingest_arrays):
+        `arrays` as RecordScope.arrays takes them.  Kernels only, on `stream` (None = torch's current stream), so inside
+        torch.cuda.graph the call is captured and every replay records the tensors' contents at that time."""
+        pairs = list(arrays.items()) if isinstance(arrays, dict) else list(arrays)
+        idx, ptrs, ns, dts = _array_table(pairs, self.histogram_ids.get, "recorder", self._ms._device)
+        if self._h is None:
+            raise RuntimeError("the graph recorder is closed")
+        st = self._ms._lib.lhms_arrays_graph_recorder(self._h, idx, ptrs, ns, dts, len(pairs), _capture_stream(stream))
+        if st != 0:
+            raise RuntimeError("lhms_arrays_graph_recorder failed (status %d)" % st)
 
     def _call(self, what, *args):
         if self._h is None:
